@@ -1,4 +1,4 @@
-"""whenet_b200 - B200-native WHENet per-crop forward (hand-written sm_100a CUDA behind a C ABI).
+"""whenet_b200 - H100-native WHENet per-crop forward (hand-written sm_90a CUDA behind a C ABI).
 
 The directory is named ``headposeestimation-whenet_b200`` (not importable as
 is); import it as ``whenet_b200`` through the shim package at the repo root.

@@ -1,4 +1,4 @@
-"""Build ``libwhenet_b200.so`` in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build ``libwhenet_b200.so`` in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -24,7 +24,7 @@ SOURCES = list(UNITS)
 HEADERS = sorted({h for hs in UNITS.values() for h in hs})
 
 # no --use_fast_math: precise expf / division are required by the fp32 parity mode
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC"]
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
 def _obj(src: str) -> str:
@@ -71,7 +71,7 @@ def build_lib(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError("nvcc failed on %s:\n%s\n%s" % (src, r.stdout, r.stderr))
         if verbose:
             print(r.stderr, file=sys.stderr)
-    r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + [_obj(s) for s in SOURCES],
+    r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + [_obj(s) for s in SOURCES],
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -5,7 +5,7 @@
 // blocks do not have (their expanded tensors - 29..135 MB per 256..512 crops - live in the 126 MB L2), and pays for it with
 // a chain of CTA-wide phases (MMA wait -> TMEM epilogue -> barrier -> depthwise -> barrier -> reduce) at one CTA per SM;
 // measured 13.9 k cycles per channel chunk at 7x7 for ~6.5 k warp instructions (profiles/README.md, round 2).  Here the
-// expand conv runs as a plain tcgen05 GEMM whose epilogue writes E as fp16 (pw_tc2, OUT_H) and this kernel does the rest
+// expand conv runs as a plain tensor-core GEMM whose epilogue writes E as fp16 (pw_tc2, OUT_H) and this kernel does the rest
 // with every thread busy on identical work:
 //
 //   CTA = one crop; for each chunk of CC channels (two buffers; thread 0 issues the TMA copies of chunk i+2 as soon as every

@@ -1,6 +1,6 @@
 // kernels_fused.cuh - K1: the fused front half of an MBConv block.
 //
-//   expand 1x1 (tcgen05, accumulators in TMEM, BN shift folded in as two extra K columns)
+//   expand 1x1 (warpgroup MMA, fp32 accumulators in registers, BN shift folded in as two extra K columns)
 //   -> swish -> shared memory (never HBM)
 //   -> depthwise KSxKS stride S, TF-SAME (CUDA-core FMA on the smem tile) -> BN shift + swish
 //   -> D (global, 16-bit) + deterministic SE squeeze partial sums
@@ -13,8 +13,8 @@
 // consumed CC at a time:
 //
 //   for each chunk of CC expanded channels (W chunk + depthwise constants of chunk i+1 prefetched with cp.async):
-//       tcgen05.mma  D[mt][128 x CC] = [A | 1 1] (128 x (Cin+8)) * [Wc | shift_hi shift_lo]^T   for every 128-row tile mt
-//       TMEM -> registers -> swish -> 16-bit -> E[halo pixel][CC] in smem
+//       wgmma  D[u][64 x CC] = [A | 1 1] (64 x (Cin+8)) * [Wc | shift_hi shift_lo]^T   for every 64-row half u (the warp
+//       groups of the CTA take the halves in turn) -> swish -> 16-bit -> E[halo pixel][CC] in smem
 //       depthwise strips straight out of E (ld.shared.v2), the KS weights of one kernel row from smem
 //       -> store D, accumulate the squeeze sums
 //
@@ -63,7 +63,7 @@ struct K1Params {
     int TH, TW, IH, IW;    // output tile, input halo tile
     int tiles_x, tiles_y;
     int CC, n_chunks;      // expanded channels per chunk (multiple of 16), number of chunks
-    int mtiles;            // most 128-row GEMM tiles any CTA needs (<= 3); sizes TMEM
+    int mtiles;            // most 128-row GEMM tiles any CTA needs (<= 3)
     int rows_alloc;        // A rows per K block in smem: most GEMM rows any CTA has, rounded up to 8 (the last M tile's
                            // UMMA reads on past them into whatever follows - those accumulator rows are never used)
     int NB;                // crops per CTA (> 1 only when one tile is the whole image)
@@ -72,11 +72,9 @@ struct K1Params {
     int PYc;               // strip lanes per crop = PY / NB
     int cpr;               // 16-byte chunks per operand row incl. the ones/shift chunk, rounded up to even
     int nkb;               // ceil(cpr / 8)
-    int tmem_cols;         // power of two >= mtiles*CC
     int pitchE;            // bytes per E row = CC*2 + 16
     int PY;                // strip lanes in the depthwise phase = threads / (CC/4), rounded down to a multiple of NB
     int spr_log2;          // log2(strips per output row)
-    uint32_t idesc;
     int smem_A, smem_W, smem_C, smem_E;   // region sizes in bytes (W and C are per buffer; both double-buffered)
     int* tflag;            // the context's mbarrier-timeout flag (mapped pinned host memory)
     int chunks_per_cta;    // grid.z CTAs share one tile, each takes this many consecutive chunks (small batches: more CTAs per crop)
@@ -97,11 +95,10 @@ __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
     return v;
 }
-// two IEEE fp32 FMAs in one instruction (FFMA2): d.x = a.x*b.x + d.x, d.y = a.y*b.y + d.y
+// two IEEE fp32 FMAs on a channel pair: d.x = a.x*b.x + d.x, d.y = a.y*b.y + d.y
 __device__ __forceinline__ void ffma2(float2& d, const float2& a, const float2& b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;"
-        : "+l"(reinterpret_cast<unsigned long long&>(d))
-        : "l"(reinterpret_cast<const unsigned long long&>(a)), "l"(reinterpret_cast<const unsigned long long&>(b)));
+    d.x = fmaf(a.x, b.x, d.x);
+    d.y = fmaf(a.y, b.y, d.y);
 }
 template <typename T> __device__ __forceinline__ void unpack2(uint32_t u, float& lo, float& hi);
 template <> __device__ __forceinline__ void unpack2<__nv_bfloat16>(uint32_t u, float& lo, float& hi) {
@@ -134,22 +131,6 @@ __device__ __forceinline__ uint32_t sw128(int r, int c) {
 // (x + 0.5) / d is at least 0.5 / d away from every integer, far more than the float rounding error
 __device__ __forceinline__ int div_small(int x, float inv) { return __float2int_rz(((float)x + 0.5f) * inv); }
 
-// tcgen05.ld without the wait, and a wait that carries the destination registers as in/out operands so that no consumer
-// can be scheduled above it: lets the load of the next 16 columns fly while the current ones are being processed
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_wait(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :: "memory");
-}
-
 // NOEXP: the block has no expand conv (block 1): the halo tile of the block INPUT is copied straight into E and only the
 // depthwise half of the kernel runs (single chunk, no tensor-core work).
 // CCT != 0 bakes the chunk width (and with it the E row pitch and every constant-table offset) into the code: the
@@ -162,11 +143,8 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
     const int pitchE = CCT ? CCT * 2 + 16 : p.pitchE;
     // depthwise on HFMA2 (fp16 running sums over the fp16 E tile, fp16 weights): bf16 storage with an expand conv
     constexpr bool HDW = !NOEXP && std::is_same<T, __nv_bfloat16>::value;
-    constexpr int NG = NT / 128;                                // warp groups of four (one warp per TMEM lane quadrant)
+    constexpr int NG = NT / 128;                                // warp groups (each issues the MMAs of its 64-row halves)
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t s_tmem_base;
-    __shared__ int s_abort;
     __shared__ int s_last;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -194,22 +172,12 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
     const int IHin = min(p.IH, p.Hin - iy0) - ty_lo, IWin = min(p.IW, p.Hin - ix0) - tx_lo;
     const int npix_in = IHin * IWin;
     const int rows_gemm = nb_here * npix_in;
-    const int mtc = (rows_gemm + BM - 1) / BM;          // M tiles of this CTA (<= p.mtiles)
     const float inv_IWin = 1.0f / (float)IWin, inv_npix = 1.0f / (float)npix_in;
     const int kchunks = p.Cin >> 3;                     // data chunks per row; chunk `kchunks` holds the ones / the shift
     const int Kaug = p.Cin + 8;
     const uint32_t a_kb_stride = (uint32_t)p.rows_alloc * 128u;
     const float inv_cpr = 1.0f / (float)p.cpr, inv_q = 4.0f / (float)CC;
 
-    if (tid == 0) {
-        tc::mbar_init(&mbar, 1);
-        s_abort = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (!NOEXP && warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&s_tmem_base)), "r"((uint32_t)p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (NOEXP) {
         // ---- E <- the input halo tile itself (Cin == Cexp == CC), zero outside the image (depthwise SAME padding)
         const T* in_n = in + (long long)n0 * p.Hin * p.Hin * p.Cin;
@@ -295,20 +263,13 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
     asm volatile("cp.async.commit_group;" ::: "memory");
 
     // ---- per-thread constants of the two compute phases
-    // epilogue 1: warp w reads TMEM lane quadrant (w & 3); the NG warp groups share the 16-column units of every M tile
-    const int q4 = warp & 3, grp = warp >> 2;
-    uint32_t e_row[3];
-    bool e_valid[3];
-#pragma unroll
-    for (int mt = 0; mt < 3; ++mt) {
-        const int r = mt * BM + q4 * 32 + lane;
-        e_valid[mt] = !NOEXP && r < rows_gemm;
-        const int rc = e_valid[mt] ? r : 0;
-        const int j = div_small(rc, inv_npix), q = rc - j * npix_in;
+    // epilogue 1: fragment row of thread (warp w of its group, lane l) -> E row of that GEMM row (halo pixel)
+    const int grp = warp >> 2, wq = warp & 3;
+    auto e_row_of = [&](int r) -> uint32_t {
+        const int j = div_small(r, inv_npix), q = r - j * npix_in;
         const int ty = div_small(q, inv_IWin), tx = q - ty * IWin;
-        e_row[mt] = sE + (uint32_t)(j * p.e_rows + (ty_lo + ty) * p.IW + tx_lo + tx) * pitchE;
-    }
-    const int units = CC >> 4;
+        return sE + (uint32_t)(j * p.e_rows + (ty_lo + ty) * p.IW + tx_lo + tx) * pitchE;
+    };
     // depthwise: thread = (4-channel vector cv, strip lane py); with NB crops per CTA the lanes split evenly between them
     const int CVc = CC >> 2;
     const int py = tid / CVc, cv = tid - py * CVc;
@@ -319,86 +280,59 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
     constexpr int NCOL = (R - 1) * S + KS;
     T* const out_n = out + (long long)(n0 + jc) * p.Ho * p.Ho * p.Cexp;
 
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = NOEXP ? 0u : s_tmem_base;
-
-    // tensor-core work runs one chunk AHEAD of the CUDA-core work: MMA(ch+1) is issued as soon as epilogue 1 has
-    // drained TMEM(ch) and executes while the whole CTA is busy with the depthwise of chunk ch.
-    auto issue_mma = [&](int buf) {
-        const int ksteps_total = p.cpr >> 1;
-        for (int mt = 0; mt < mtc; ++mt) {
-            for (int ks = 0; ks < ksteps_total; ++ks) {
-                const int kb = ks >> 2, k = ks & 3;
-                const uint64_t ad = tc::make_desc(sA + (uint32_t)kb * a_kb_stride + (uint32_t)mt * BM * 128);
-                const uint64_t bd = tc::make_desc(sW + buf * p.smem_W + (uint32_t)kb * CC * 128);
-                tc::umma_f16(tmem_d + (uint32_t)(mt * CC), ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), p.idesc, ks ? 1u : 0u);
-            }
-        }
-        tc::umma_commit(&mbar);
-    };
-    // chunk 0: operands (A, W0, constants 0) have to land first (W1 may still be in flight)
-    asm volatile("cp.async.wait_group 1;" ::: "memory");
+    // A, W(ch_begin), constants(ch_begin) and W(ch_begin + 1) have landed
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (!NOEXP && tid == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        issue_mma(ch_begin & 1);
-    }
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+    const int nch16 = CC >> 4;
 
     for (int ch = ch_begin; ch < ch_end; ++ch) {
         const int buf = ch & 1;
         const int cbase = ch * CC;
+        // ---- expand MMA + epilogue 1: swish -> E (fp16).  The BN shift is already in the accumulator.  The 64-row halves of
+        //      the GEMM rows go round-robin over the warp groups; halves past the last GEMM row are skipped.
         if (!NOEXP) {
-            if (!tc::mbar_wait(&mbar, (ch - ch_begin) & 1, p.tflag)) s_abort = 1;      // MMA(ch): issued one phase ago, normally long done
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        // constants of chunk ch+1 (group 1), then W of chunk ch+2 into the buffer MMA(ch) has just released (group 2)
-        if (ch + 1 < ch_end) prefetch_c(ch + 1, buf ^ 1);
-        asm volatile("cp.async.commit_group;" ::: "memory");
-        if (ch + 2 < ch_end) prefetch_w(ch + 2, buf);
-        asm volatile("cp.async.commit_group;" ::: "memory");
-        const bool ok = !s_abort;
-
-        // ---- epilogue 1: TMEM -> swish -> E (16-bit).  The BN shift is already in the accumulator.
-        //      (M tile, 16-column unit) pairs go round-robin over the warp groups so all carry the same load;
-        //      a warp whose 32 rows of an M tile are all past the last GEMM row skips the tile.
-        if (ok && !NOEXP) {
+            for (int u = grp; u * 64 < rows_gemm; u += NG) {
+                float d[8][8];
+                tc::wg_fence();
+                tc::wg_mma_m64<BF16, 8>(d, sA + (uint32_t)u * 64 * 128, a_kb_stride, sW + buf * p.smem_W, (uint32_t)CC * 128, p.cpr >> 1, nch16);
+                tc::wg_commit();
+                tc::wg_wait<0>();
+                const int r_lo = u * 64 + 16 * wq + (lane >> 2), cq = 2 * (lane & 3);
 #pragma unroll
-            for (int mt = 0; mt < 3; ++mt) {
-                if (mt * BM + q4 * 32 < rows_gemm) {
-                    for (int u = (grp + NG * 8 - mt * units) % NG; u < units; u += NG) {
-                        float v[16];
-                        tc::tmem_ld16(tmem_d + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(mt * CC + u * 16), v);
-                        if (e_valid[mt]) {
+                for (int hr = 0; hr < 2; ++hr) {
+                    const int r = r_lo + 8 * hr;
+                    if (r < rows_gemm) {
+                        const uint32_t er = e_row_of(r);
 #pragma unroll
-                            for (int j = 0; j < 16; ++j) v[j] = swish_from_half(v[j]);
-                            // E is fp16 whatever the storage type: 3 more mantissa bits than bf16 and HFMA2-ready
-                            const uint4 lo = make_uint4(pack2<__half>(v[0], v[1]), pack2<__half>(v[2], v[3]), pack2<__half>(v[4], v[5]), pack2<__half>(v[6], v[7]));
-                            const uint4 hi = make_uint4(pack2<__half>(v[8], v[9]), pack2<__half>(v[10], v[11]), pack2<__half>(v[12], v[13]), pack2<__half>(v[14], v[15]));
-                            sts128(e_row[mt] + u * 32, lo);
-                            sts128(e_row[mt] + u * 32 + 16, hi);
+                        for (int jj = 0; jj < 8; ++jj) {
+                            if (jj < nch16) {
+#pragma unroll
+                                for (int i = 0; i < 2; ++i) {
+                                    // E is fp16 whatever the storage type: 3 more mantissa bits than bf16 and HFMA2-ready
+                                    const uint32_t v = pack2<__half>(swish_from_half(d[jj][4 * i + 2 * hr]), swish_from_half(d[jj][4 * i + 2 * hr + 1]));
+                                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(er + (uint32_t)(16 * jj + 8 * i + cq) * 2u), "r"(v) : "memory");
+                                }
+                            }
                         }
                     }
                 }
             }
         }
-        // TMEM(ch) is drained and E(ch) is complete; W(ch+1) and constants(ch+1) have landed (only the newest group,
-        // W(ch+2), may still be in flight) -> hand the tensor core its next chunk
-        asm volatile("cp.async.wait_group 1;" ::: "memory");
+        // constants of chunk ch+1 into the buffer the depthwise of chunk ch-1 has finished with
+        if (ch + 1 < ch_end) prefetch_c(ch + 1, buf ^ 1);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        // E(ch) is complete, every MMA of chunk ch is done with W[buf], W(ch+1) and constants(ch+1) have landed
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (!NOEXP && tid == 0 && ch + 1 < ch_end && !s_abort) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            issue_mma(buf ^ 1);
-        }
+        if (ch + 2 < ch_end) prefetch_w(ch + 2, buf);
+        asm volatile("cp.async.commit_group;" ::: "memory");
 
         // ---- depthwise on E: 8-byte ld.shared, fp32 FMA, weights of one kernel row from smem
         float sum[4] = {0.f, 0.f, 0.f, 0.f};
-        if (ok && dw_active) {
+        if (dw_active) {
             const int c0 = cbase + cv * 4;
             const uint32_t cst = sC + buf * p.smem_C + (uint32_t)cv * 16;         // this thread's column of the constants
             const float4 bq = lds_f4(cst);
@@ -505,7 +439,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
                          "f"(sum[0]), "f"(sum[1]), "f"(sum[2]), "f"(sum[3]) : "memory");
         }
         __syncthreads();
-        if (ok && tid < p.NB * CC) {
+        if (tid < p.NB * CC) {
             const int jj = tid >= CC ? 1 : 0, cc = tid - jj * CC;          // NB <= 2
             if (jj < nb_here) {
                 // four independent chains (lane mod 4) keep this short: the two warps doing it are the ones every other warp
@@ -531,17 +465,15 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
                 if (p.se_tail) sM[jj * p.Cexp + cbase + cc] = tot * p.inv_hw;      // == the mean se_gate_crop forms from one tile
             }
         }
-        // E, the squeeze scratch and TMEM are reused only after the barrier at the top of the next chunk
+        // E and the squeeze scratch are reused only after this barrier
+        __syncthreads();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     if (p.se_counter) __threadfence();     // fused SE only: this CTA's squeeze partials are visible device-wide before the ticket
                                            // (unconditional, the MEMBAR made every CTA wait out its own output stores)
     __syncthreads();
-    if (!NOEXP && warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((uint32_t)p.tmem_cols) : "memory");
 
     // ---- SE excite for the crops of this CTA when it holds all of their pixels and channels
-    if (p.se_tail && !s_abort) {
+    if (p.se_tail) {
         for (int jj = 0; jj < nb_here; ++jj) {
             float* const g_sm = sM + jj * p.Cexp;           // means in, gate out
             se_gate_fc<NT>(g_sm, sM + p.NB * p.Cexp, p.w_se1t, p.b_se1, p.w_se2, p.b_se2,
@@ -568,7 +500,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
             if (s_last) p.se_counter[n0] = 0;
         }
         __syncthreads();
-        if (s_last && !s_abort) {
+        if (s_last) {
             __threadfence();
             float* sm = reinterpret_cast<float*>(smem_raw + (sE - tc::smem_u32(smem_raw)));    // E is free now
             se_gate_crop<true, NT>(p.partial + (long long)n0 * gridDim.x * p.Cexp, (int)gridDim.x, 1.0f / (float)(p.Ho * p.Ho),
@@ -578,7 +510,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
 }
 
 // One tile plan: TH x TW output tile, R outputs per depthwise strip, CC expanded channels per chunk, NT threads per CTA,
-// NB crops per CTA.  Returns false when K1 cannot run it (shape does not divide, TMEM / shared memory exceeded).
+// NB crops per CTA.  Returns false when K1 cannot run it (shape does not divide, shared memory exceeded).
 inline bool plan_k1_candidate(int Hin, int Ho, int Cin, int Cexp, int k, int s, int pad, bool is_bf16, int TH, int TW, int R, int CC,
                               int NT, int NB, K1Params* p, size_t* smem_out) {
     if (Ho % TH || Ho % TW || Cexp % CC || (NT != 256 && NT != 512) || NB < 1) return false;
@@ -588,7 +520,7 @@ inline bool plan_k1_candidate(int Hin, int Ho, int Cin, int Cexp, int k, int s, 
     p->tiles_x = Ho / TW; p->tiles_y = Ho / TH;
     if (NB > 1 && p->tiles_x * p->tiles_y != 1) return false;
     p->NB = NB;
-    // GEMM rows of a CTA = halo pixels inside the image; the largest count over all tiles sizes TMEM and the A buffer
+    // GEMM rows of a CTA = halo pixels inside the image; the largest count over all tiles sizes the A buffer
     int max_in = 0;
     for (int ty = 0; ty < p->tiles_y; ++ty)
         for (int tx = 0; tx < p->tiles_x; ++tx) {
@@ -597,15 +529,12 @@ inline bool plan_k1_candidate(int Hin, int Ho, int Cin, int Cexp, int k, int s, 
             max_in = std::max(max_in, ih * iw);
         }
     p->mtiles = (NB * max_in + BM - 1) / BM;
-    if (p->mtiles > 3 || p->mtiles * CC > 512) return false;
+    if (p->mtiles > 3 || CC > 128) return false;
     p->rows_alloc = (NB * max_in + 7) & ~7;
     p->cpr = ((Cin >> 3) + 1 + 1) & ~1;
     p->nkb = (p->cpr + 7) / 8;
     p->CC = CC; p->n_chunks = Cexp / CC;
     p->chunks_per_cta = p->n_chunks;
-    int cols = 32;
-    while (cols < p->mtiles * CC) cols <<= 1;
-    p->tmem_cols = cols;
     p->pitchE = CC * 2 + 16;
     p->PYc = NT / (CC / 4) / NB;
     p->PY = p->PYc * NB;
@@ -613,7 +542,6 @@ inline bool plan_k1_candidate(int Hin, int Ho, int Cin, int Cexp, int k, int s, 
     const int spr = (TW + R - 1) / R;         // a ragged last strip computes (and discards) up to R-1 extra outputs
     p->spr_log2 = spr == 1 ? 0 : spr == 2 ? 1 : spr == 4 ? 2 : -1;
     if (p->spr_log2 < 0) return false;
-    p->idesc = tc::make_idesc(is_bf16, CC);
     p->smem_A = p->nkb * p->rows_alloc * 128;           // multiple of 1024 (rows_alloc % 8 == 0)
     p->smem_W = p->nkb * CC * 128;                      // multiple of 2048 (CC % 16 == 0)
     p->smem_C = (k * k + 1) * CC * 4;
@@ -622,17 +550,17 @@ inline bool plan_k1_candidate(int Hin, int Ho, int Cin, int Cexp, int k, int s, 
     p->smem_E = NB * p->e_rows * p->pitchE;
     const size_t se_tail_bytes = p->tiles_x * p->tiles_y == 1 ? (size_t)(NB * Cexp + 64) * 4 : 0;     // means + hidden layer
     *smem_out = (size_t)p->smem_A + 2 * p->smem_W + 2 * p->smem_C + p->smem_E + (size_t)p->PY * CC * 4 + se_tail_bytes + 1024;
-    // the UMMA of the last M tile reads 128 rows even when fewer are staged: that read must stay inside the CTA's window
-    if ((size_t)(p->nkb - 1) * p->rows_alloc * 128 + (size_t)p->mtiles * BM * 128 + 1024 > *smem_out) return false;
+    // the MMA of the last 64-row half reads 64 rows even when fewer are staged: that read must stay inside the CTA's window
+    if ((size_t)(p->nkb - 1) * p->rows_alloc * 128 + (size_t)((p->rows_alloc + 63) / 64) * 64 * 128 + 1024 > *smem_out) return false;
     return *smem_out <= K1_MAX_SMEM;
 }
 
-// can two CTAs of this plan share an SM?  (228 KB per SM, 1 KB reserved per CTA, 512 TMEM columns)
-inline bool k1_two_per_sm(const K1Params& p, size_t smem, int NT) { return NT == 256 && smem <= 115000 && p.tmem_cols <= 256; }
+// can two CTAs of this plan share an SM?  (228 KB per SM, 1 KB reserved per CTA)
+inline bool k1_two_per_sm(const K1Params& p, size_t smem, int NT) { (void)p; return NT == 256 && smem <= 115000; }
 
 struct K1Choice { int th, tw, r, cc, nt, nb; };
 
-// Per-block plan.  The table holds the plans measured fastest on B200 by tools/tune_k1.py; blocks without an entry
+// Per-block plan.  The table holds the plans tools/tune_k1.py measured fastest; blocks without an entry
 // (or whose entry does not fit) fall back to a small search ranked by a thread-instruction model.
 inline bool plan_k1(int Hin, int Ho, int Cin, int Cexp, int k, int s, int pad, bool is_bf16, bool allow_nb, K1Params* p, K1Choice* choice,
                     size_t* smem_out) {
@@ -701,7 +629,7 @@ inline bool plan_dw_only(int Hin, int C, int k, int s, int pad, K1Params* p, siz
     p->Hin = Hin; p->Ho = Hin; p->Cin = C; p->Cexp = C; p->pad = pad;
     p->TH = 14; p->TW = 14; p->IH = 16; p->IW = 16;
     p->tiles_x = Hin / 14; p->tiles_y = Hin / 14;
-    p->mtiles = 2; p->rows_alloc = 256; p->cpr = 2; p->nkb = 1; p->CC = C; p->n_chunks = 1; p->tmem_cols = 32;
+    p->mtiles = 2; p->rows_alloc = 256; p->cpr = 2; p->nkb = 1; p->CC = C; p->n_chunks = 1;
     p->NB = 1;
     p->pitchE = C * 2 + 16;
     p->PY = 256 / (C / 4);

@@ -1,30 +1,29 @@
 // kernels_k1w.cuh - K1W: weight-stationary, persistent, warp-specialised front half of an MBConv block.
 //
-//   expand 1x1 (tcgen05, fp32 accumulators in TMEM) -> + BN shift -> swish -> 16-bit E tile in shared memory (never HBM)
-//   -> depthwise KSxKS stride S, TF-SAME (fp32 FFMA2 on the E tile) -> + BN shift -> swish
+//   expand 1x1 (warpgroup MMA, fp32 accumulators in registers) -> + BN shift -> swish -> 16-bit E tile in shared memory
+//   -> depthwise KSxKS stride S, TF-SAME (HFMA2 on the E tile) -> + BN shift -> swish
 //   -> D (global, 16-bit) + deterministic SE squeeze partial sums
 //
 // Same arithmetic as K1 (kernels_fused.cuh), different machine mapping.  K1 gives one CTA one tile and walks its phases
-// behind CTA-wide barriers; on B200 that leaves the SM at ~50 % issue utilisation in the early blocks and latency-bound
-// (one 512-thread CTA per SM, 6-18 serial chunks per crop) in the late ones.  K1W instead:
+// behind CTA-wide barriers, which leaves the late blocks latency-bound (one 512-thread CTA per SM, 6-18 serial chunks per
+// crop).  K1W instead:
 //
 //   * a CTA owns ONE chunk of CC expanded channels for the whole launch: its slice of the expand weights (TMA, once), its
 //     BN shifts and its depthwise constants stay in shared memory ("weight stationary"), and it loops over ITEMS
 //     = (crop [pair], output tile); grid = n_chunks x groups <= #SMs, items are dealt round-robin to the groups;
 //   * the halo tile of the block INPUT of an item arrives by ONE TMA box per 64-channel K block
-//     (cp.async.bulk.tensor.4d over the NHWC tensor, SWIZZLE_128B = the UMMA K-major operand layout, rows = halo
+//     (cp.async.bulk.tensor.4d over the NHWC tensor, SWIZZLE_128B = the wgmma K-major operand layout, rows = halo
 //     pixels in raster order).  Out-of-image halo pixels and channels past Cin are zero-filled by the TMA unit, so
 //     TF-SAME padding and K padding cost no instructions;
 //   * warp roles, connected by mbarriers (no CTA-wide barrier in the item loop):
 //       warp 0            TMA producer   A ring (NA stages)
-//       warp 1            MMA issuer     tcgen05.mma into a 2-deep TMEM accumulator ring, tcgen05.commit -> mbarrier
 //       warps 2-3         reducer        fixed-order column sums of the depthwise lanes' squeeze partials -> global
-//       warps 4..4+E-1    epilogue       TMEM -> +shift -> swish -> 16-bit -> E ring (2 deep); rows outside the image -> 0
-//       remaining warps   depthwise      E -> k x k FFMA2 -> +shift, swish -> D; per-lane squeeze sums -> smem ring
+//       last E warps      MMA + epilogue wgmma of (64-row half, 16 columns) pieces, round-robin over the epilogue warpgroups
+//                                        -> +shift -> swish -> 16-bit -> E ring (2 deep); rows outside the image -> 0
+//       remaining warps   depthwise      E -> k x k HFMA2 -> +shift, swish -> D; per-lane squeeze sums -> smem ring
 //     Registers follow the roles (setmaxnreg): 48 for the control group, 72-80 for the epilogue, 88-96 for the depthwise
 //     warps, which lets 12-16 of them run beside 4-8 epilogue warps in one 768-thread CTA.
-//     so the SFU-bound epilogue of item i+1, the FMA-bound depthwise of item i, the tensor core and the TMA unit all run
-//     at the same time.
+//     so the MMA + SFU-bound epilogue of item i+1, the FMA-bound depthwise of item i and the TMA unit all run at the same time.
 //
 // E row index == GEMM row index == raster index of the halo pixel, so neither the epilogue nor the depthwise needs
 // a division to find its data.  Every mbarrier wait is bounded (flag in mapped host memory + fast exit).
@@ -56,12 +55,10 @@ struct alignas(64) K1WParams {
     int mtiles;            // 128-row GEMM tiles of one item
     int rows;              // GEMM rows of one item = NB * IH * IW
     int rows_alloc;        // A rows per K block in shared memory (rows rounded up to 8)
-    int tbuf_cols, tmem_cols;
-    uint32_t idesc;
     int pitchE;            // bytes per E row = CC * 2 + 16
     int e_rows;            // E rows per crop (IH * IW + slack for ragged strips)
     int NA;                // A ring depth (1 or 2)
-    int n_epi;             // epilogue warps: 4 (one per TMEM lane quadrant) or 8
+    int n_epi;             // epilogue warps: 4 or 8 (one or two warpgroups)
     int n_dw;              // depthwise threads
     int PY, PYc;           // strip lanes (all crops of the item / per crop)
     int spr_log2;          // log2(strips per output row)
@@ -118,9 +115,6 @@ __device__ __forceinline__ void arrive_warp(uint32_t bar_addr) {
 __device__ __forceinline__ void arrive_expect_tx(uint32_t bar_addr, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void commit(uint32_t bar_addr) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_addr) : "memory");
-}
 __device__ __forceinline__ void tma_4d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, uint32_t bar_addr) {
     asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
                  ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar_addr) : "memory");
@@ -129,14 +123,8 @@ __device__ __forceinline__ void tma_2d(uint32_t dst, const CUtensorMap* tm, int 
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(bar_addr) : "memory");
 }
-// two fp32 adds in one instruction
-__device__ __forceinline__ float2 fadd2(const float2& a, const float2& b) {
-    float2 d;
-    asm("add.rn.f32x2 %0, %1, %2;"
-        : "=l"(reinterpret_cast<unsigned long long&>(d))
-        : "l"(reinterpret_cast<const unsigned long long&>(a)), "l"(reinterpret_cast<const unsigned long long&>(b)));
-    return d;
-}
+// two fp32 adds on a channel pair
+__device__ __forceinline__ float2 fadd2(const float2& a, const float2& b) { return make_float2(a.x + b.x, a.y + b.y); }
 // swish of two values that are already x/2: h + h * tanh(h)
 __device__ __forceinline__ float2 swish2_from_half(const float2& h) {
     float2 t;
@@ -170,9 +158,8 @@ constexpr int kK1WThreads = 768;       // six warpgroups: control | EPI_WG x epi
 template <typename T, int KS, int S, int R, int EPI_WG>
 __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) {
     extern __shared__ uint8_t smem_raw[];
-    // [0,1] a_full  [2,3] a_empty  [4,5] t_full  [6,7] t_empty  [8,9] e_full  [10,11] e_empty  [12] w  [13,14] r_full  [15,16] r_empty
+    // [0,1] a_full  [2,3] a_empty  [8,9] e_full  [10,11] e_empty  [12] w  [13,14] r_full  [15,16] r_empty
     __shared__ __align__(8) uint64_t bars[17];
-    __shared__ uint32_t s_tmem_base;
     __shared__ int s_abort_mem;
     volatile int* s_abort = &s_abort_mem;
 
@@ -180,7 +167,7 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
     const uint32_t smem0 = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sA = smem0, sW = smem0 + p.off_w, sC = smem0 + p.off_c, sE = smem0 + p.off_e, sR = smem0 + p.off_r;
     const uint32_t bar0 = tc::smem_u32(&bars[0]);
-    const uint32_t b_a_full = bar0, b_a_empty = bar0 + 16, b_t_full = bar0 + 32, b_t_empty = bar0 + 48, b_e_full = bar0 + 64,
+    const uint32_t b_a_full = bar0, b_a_empty = bar0 + 16, b_e_full = bar0 + 64,
                    b_e_empty = bar0 + 80, b_w = bar0 + 96, b_r_full = bar0 + 104, b_r_empty = bar0 + 120;
     const int CC = p.CC, pitchE = p.pitchE;
     const int chunk = blockIdx.x % p.n_chunks, group = blockIdx.x / p.n_chunks;
@@ -194,9 +181,7 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
         for (int i = 0; i < 2; ++i) {
             tc::mbar_init(&bars[0 + i], 1);
             tc::mbar_init(&bars[2 + i], 1);
-            tc::mbar_init(&bars[4 + i], 1);
-            tc::mbar_init(&bars[6 + i], p.n_epi);          // counts are WARPS (arrive_warp)
-            tc::mbar_init(&bars[8 + i], p.n_epi);
+            tc::mbar_init(&bars[8 + i], p.n_epi);          // counts are WARPS (arrive_warp)
             tc::mbar_init(&bars[10 + i], p.n_dw >> 5);
             tc::mbar_init(&bars[13 + i], p.n_dw >> 5);
             tc::mbar_init(&bars[15 + i], 2);
@@ -205,14 +190,7 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
         s_abort_mem = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&s_tmem_base)), "r"((uint32_t)p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem_base;
 
     // registers follow the roles: the launch gives every thread 80; control and epilogue groups hand theirs back, the
     // depthwise groups (the only code with 28-56 accumulators + a kernel row of weights live) take them
@@ -244,30 +222,7 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
             }
         }
       } else if (warp == 1) {
-        // =========================================================================== MMA issuer
-        k1w::wait(b_w, 0, s_abort, p.tflag);
-        for (int k = 0; it.item < p.items; it.next(), ++k) {
-            const int st = p.NA == 2 ? (k & 1) : 0;
-            const uint32_t par = p.NA == 2 ? ((k >> 1) & 1) : (k & 1);
-            const int tb = k & 1;
-            k1w::wait_t(b_a_full + 8 * st, par, s_abort, p.tflag, tr, tw0);
-            k1w::wait_t(b_t_empty + 8 * tb, ((k >> 1) & 1) ^ 1, s_abort, p.tflag, tr, tw1);  // the epilogue has drained this accumulator
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (lane == 0 && !*s_abort) {
-                const uint32_t a0 = sA + (uint32_t)st * p.a_stage;
-                for (int mt = 0; mt < p.mtiles; ++mt)
-                    for (int ks = 0; ks < p.ksteps; ++ks) {
-                        const int kb = ks >> 2, kk = ks & 3;
-                        const uint64_t ad = tc::make_desc(a0 + (uint32_t)kb * p.rows_alloc * 128 + (uint32_t)mt * BM * 128);
-                        const uint64_t bd = tc::make_desc(sW + (uint32_t)kb * CC * 128);
-                        tc::umma_f16(tmem_base + (uint32_t)(tb * p.tbuf_cols + mt * CC), ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2),
-                                     p.idesc, ks ? 1u : 0u);
-                    }
-                k1w::commit(b_t_full + 8 * tb);
-                k1w::commit(b_a_empty + 8 * st);
-            }
-            __syncwarp();
-        }
+        // idle: the epilogue warpgroups issue their own MMAs
       } else {
         // =========================================================================== reducer: squeeze partial sums of an item
         // The depthwise lanes leave their per-lane sums in a 2-slot ring; these two warps add them up in a FIXED order
@@ -306,116 +261,71 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
         // register budget of the CTA: 768 x 80 = 61440 = 128 x 48 (control) + 128 x 80 + 512 x 88   (one epilogue group)
         //                                               = 128 x 48 (control) + 256 x 72 + 384 x 96   (two epilogue groups)
         if (EPI_WG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");          // one group: keeps its 80
-        // =========================================================================== epilogue: TMEM -> +shift -> swish -> E
-        const int q4 = warp & 3;                       // TMEM lane quadrant of this warp
+        // =========================================================================== MMA + epilogue: wgmma -> +shift -> swish -> E
+        constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+        const int wq = warp & 3;
         const int e_first = kK1WThreads - n_epi_threads;     // first epilogue thread
         const int grp = (warp - (e_first >> 5)) >> 2, NG = p.n_epi >> 2;
         const int units = CC >> 4;
         const int npix = p.IH * p.IW;
-        const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+        const float inv_IW = 1.0f / (float)p.IW, inv_npix = 1.0f / (float)npix;
         // BN shifts of this CTA's channels -> shared memory (read by this group only; published by a group barrier)
         {
             float* sh = reinterpret_cast<float*>(smem_raw + (sC - tc::smem_u32(smem_raw)));
             for (int c = tid - e_first; c < CC; c += n_epi_threads) sh[c] = p.shift[cbase + c];
             asm volatile("bar.sync 2, %0;" ::"r"(n_epi_threads) : "memory");
         }
-        // rows of this thread: r = mt * 128 + q4 * 32 + lane.  Their crop / position inside the halo tile and their E row
-        // do not depend on the item; only the tile origin does.
-        int r_ty[3], r_tx[3], r_j[3];
-        uint32_t r_e[3];
-        bool in_box[3];
-        {
-            const float inv_IW = 1.0f / (float)p.IW, inv_npix = 1.0f / (float)npix;
-#pragma unroll
-            for (int mt = 0; mt < 3; ++mt) {
-                const int r = mt * BM + q4 * 32 + lane;
-                in_box[mt] = mt < p.mtiles && r < p.rows;
-                const int rc = in_box[mt] ? r : 0;
-                r_j[mt] = p.NB == 1 ? 0 : div_small(rc, inv_npix);
-                const int q = rc - r_j[mt] * npix;
-                r_ty[mt] = div_small(q, inv_IW);
-                r_tx[mt] = q - r_ty[mt] * p.IW;
-                r_e[mt] = (uint32_t)(r_j[mt] * p.e_rows + q) * pitchE;
-            }
-        }
-        int mt_count = 0;
-#pragma unroll
-        for (int mt = 0; mt < 3; ++mt) mt_count += (mt < p.mtiles && mt * BM + q4 * 32 < p.rows) ? 1 : 0;   // a prefix of the tiles
-        const uint32_t t_q = tmem_base + ((uint32_t)(q4 * 32) << 16);
+        k1w::wait(b_w, 0, s_abort, p.tflag);
+        const int halves = (p.rows + 63) >> 6;
         for (int k = 0; it.item < p.items; it.next(), ++k) {
             const int tyi = div_small(it.t, inv_tx);
             const int iy0 = tyi * p.TH * S - p.pad, ix0 = (it.t - tyi * p.tiles_x) * p.TW * S - p.pad, n0 = it.q * p.NB;
             const int buf = k & 1;
-            bool in_img[3];
-#pragma unroll
-            for (int mt = 0; mt < 3; ++mt)
-                in_img[mt] = in_box[mt] && (unsigned)(iy0 + r_ty[mt]) < (unsigned)p.Hin && (unsigned)(ix0 + r_tx[mt]) < (unsigned)p.Hin && n0 + r_j[mt] < p.N;
-            k1w::wait_t(b_t_full + 8 * buf, (k >> 1) & 1, s_abort, p.tflag, tr, tw0);
+            const int st = p.NA == 2 ? (k & 1) : 0;
+            const uint32_t par = p.NA == 2 ? ((k >> 1) & 1) : (k & 1);
+            k1w::wait_t(b_a_full + 8 * st, par, s_abort, p.tflag, tr, tw0);
             k1w::wait_t(b_e_empty + 8 * buf, ((k >> 1) & 1) ^ 1, s_abort, p.tflag, tr, tw1);     // the depthwise of item k-2 is done with this E
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
             if (!*s_abort) {
                 const uint32_t e0 = sE + (uint32_t)buf * p.e_buf;
-                const uint32_t t0 = t_q + (uint32_t)(buf * p.tbuf_cols);
-                // (M tile, 16-column unit) pairs of this warp: f = grp, grp + NG, ... ; f -> (mt, u) advances without a division.
-                // Two units are loaded and processed TOGETHER: with one or two epilogue warps per scheduler nothing hides the
-                // LDS -> FADD2 -> MUFU -> FFMA2 -> F2FP -> STS chain of one value but the other values of the same warp, and one
-                // unit gave ptxas four independent groups only (role trace: ~700 cycles per unit for ~70 instructions).
-                auto stage = [&](const uint32_t (&r)[16], int mt, int u, int j, float2 (&h)[2], bool& img, uint32_t& dst) {
-                    img = mt == 0 ? in_img[0] : (mt == 1 ? in_img[1] : in_img[2]);
-                    dst = e0 + (mt == 0 ? r_e[0] : (mt == 1 ? r_e[1] : r_e[2])) + u * 32;
-                    const float4 sh = lds_f4(sC + (uint32_t)(u * 16 + j * 4) * 4);
-                    h[0] = k1w::fadd2(make_float2(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1])), make_float2(sh.x, sh.y));
-                    h[1] = k1w::fadd2(make_float2(__uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])), make_float2(sh.z, sh.w));
-                };
-                auto process2 = [&](const uint32_t (&ra)[16], int mta, int ua, const uint32_t (&rb)[16], int mtb, int ub, bool have_b) {
-                    uint32_t oa[8], ob[8];
-                    bool ia = false, ib = false;
-                    uint32_t da = 0, db = 0;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        float2 ha[2], hb[2];
-                        stage(ra, mta, ua, j, ha, ia, da);
-                        stage(rb, mtb, ub, j, hb, ib, db);
-                        const float2 a0 = k1w::swish2_from_half(ha[0]), b0 = k1w::swish2_from_half(hb[0]);
-                        const float2 a1 = k1w::swish2_from_half(ha[1]), b1 = k1w::swish2_from_half(hb[1]);
-                        oa[2 * j] = pack2<__half>(a0.x, a0.y); oa[2 * j + 1] = pack2<__half>(a1.x, a1.y);
-                        ob[2 * j] = pack2<__half>(b0.x, b0.y); ob[2 * j + 1] = pack2<__half>(b1.x, b1.y);
-                    }
-                    const bool boxa = mta == 0 ? in_box[0] : (mta == 1 ? in_box[1] : in_box[2]);
-                    const bool boxb = have_b && (mtb == 0 ? in_box[0] : (mtb == 1 ? in_box[1] : in_box[2]));
-                    // halo pixels outside the image (or crops past the batch): the depthwise pads the EXPANDED tensor with zeros
-                    if (boxa) {
-                        sts128(da, ia ? make_uint4(oa[0], oa[1], oa[2], oa[3]) : zero);
-                        sts128(da + 16, ia ? make_uint4(oa[4], oa[5], oa[6], oa[7]) : zero);
-                    }
-                    if (boxb) {
-                        sts128(db, ib ? make_uint4(ob[0], ob[1], ob[2], ob[3]) : zero);
-                        sts128(db + 16, ib ? make_uint4(ob[4], ob[5], ob[6], ob[7]) : zero);
-                    }
-                };
-                uint32_t ra[16], rb[16];
-                int mt = 0, u = grp;
-                if (u >= units) { u -= units; ++mt; }                  // NG <= 2: at most one wrap
-                auto advance = [&](int& m, int& uu) { uu += NG; if (uu >= units) { uu -= units; ++m; } };
-                while (mt < mt_count) {
-                    int mt2 = mt, u2 = u;
-                    advance(mt2, u2);
-                    const bool have_b = mt2 < mt_count;
-                    tmem_ld16_issue(t0 + (uint32_t)(mt * CC + u * 16), ra);
-                    tmem_ld16_issue(t0 + (uint32_t)((have_b ? mt2 : mt) * CC + (have_b ? u2 : u) * 16), rb);
+                const uint32_t a0 = sA + (uint32_t)st * p.a_stage;
+                // (64-row half, 16-column unit) pieces f = grp, grp + NG, ...
+                for (int f = grp; f < halves * units; f += NG) {
+                    const int hh = f / units, u = f - hh * units;
+                    float d[1][8];
                     long long tq = tr ? clock64() : 0;
-                    tmem_ld16_wait(ra);
-                    tmem_ld16_wait(rb);
+                    tc::wg_fence();
+                    tc::wg_mma_m64<BF16, 1>(d, a0 + (uint32_t)hh * 64 * 128, (uint32_t)p.rows_alloc * 128, sW + (uint32_t)u * 2048, (uint32_t)CC * 128, p.ksteps, 1);
+                    tc::wg_commit();
+                    tc::wg_wait<0>();
                     if (tr) tw2 += clock64() - tq;
                     tq = tr ? clock64() : 0;
-                    process2(ra, mt, u, rb, have_b ? mt2 : mt, have_b ? u2 : u, have_b);
-                    if (tr) { tw3 += clock64() - tq; tn += have_b ? 2 : 1; }
-                    mt = mt2; u = u2;
-                    advance(mt, u);
+                    // fragment: register 4i + e -> row 16 wq + lane/4 (+8 for e >= 2), column 8 i + 2 (lane % 4) + (e & 1)
+#pragma unroll
+                    for (int e2 = 0; e2 < 2; ++e2) {
+                        const int r = hh * 64 + 16 * wq + (lane >> 2) + 8 * e2;
+                        if (r >= p.rows) continue;
+                        const int j = p.NB == 1 ? 0 : div_small(r, inv_npix);
+                        const int q = r - j * npix;
+                        const int ty = div_small(q, inv_IW), tx = q - ty * p.IW;
+                        // halo pixels outside the image (or crops past the batch): the depthwise pads the EXPANDED tensor with zeros
+                        const bool img = (unsigned)(iy0 + ty) < (unsigned)p.Hin && (unsigned)(ix0 + tx) < (unsigned)p.Hin && n0 + j < p.N;
+                        const uint32_t dst = e0 + (uint32_t)(j * p.e_rows + q) * pitchE;
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const int c = u * 16 + 8 * i + 2 * (lane & 3);
+                            float2 sh;
+                            asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(sh.x), "=f"(sh.y) : "r"(sC + (uint32_t)c * 4u));
+                            const float2 h = k1w::swish2_from_half(k1w::fadd2(make_float2(d[0][4 * i + 2 * e2], d[0][4 * i + 2 * e2 + 1]), sh));
+                            const uint32_t v = img ? pack2<__half>(h.x, h.y) : 0u;
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst + (uint32_t)c * 2u), "r"(v) : "memory");
+                        }
+                    }
+                    if (tr) { tw3 += clock64() - tq; ++tn; }
                 }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            k1w::arrive_warp(b_t_empty + 8 * buf);
+            // every epilogue warpgroup's MMAs are done with the A stage
+            asm volatile("bar.sync 2, %0;" ::"r"(n_epi_threads) : "memory");
+            if (tid == e_first) k1w::arrive(b_a_empty + 8 * st);
             k1w::arrive_warp(b_e_full + 8 * buf);
         }
     } else {
@@ -524,17 +434,13 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
         }
     }
     if (tr && (warp == 0 || warp == 1 || warp == 4 || warp == 24 - 4 * EPI_WG)) {
-        // trace row of this CTA: [0] total cycles, then per role (producer, MMA, epilogue warp 0, depthwise warp 0): its waits
+        // trace row of this CTA: [0] total cycles, then per role (producer, idle warp 1, epilogue warp 0, depthwise warp 0): its waits
         long long* row = p.trace + (long long)blockIdx.x * 16;
         const int slot = warp == 0 ? 1 : (warp == 1 ? 4 : (warp == 4 ? 10 : 7));
         row[slot] = tw0; row[slot + 1] = tw1; row[slot + 2] = clock64() - t_begin;
-        if (warp == 24 - 4 * EPI_WG) { row[13] = tw2; row[14] = tw3; row[15] = tn; }      // epilogue: in tcgen05.wait::ld, in process(), units
+        if (warp == 24 - 4 * EPI_WG) { row[13] = tw2; row[14] = tw3; row[15] = tn; }      // epilogue: in the MMAs, in the epilogue, pieces
         if (warp == 0) row[0] = clock64() - t_begin;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
 }
 
 // ----------------------------------------------------------------------------- planning (host)
@@ -557,12 +463,7 @@ inline bool plan_k1w_candidate(int Hin, int Ho, int Cin, int Cexp, int k, int s,
     p->mtiles = (p->rows + BM - 1) / BM;
     if (p->mtiles > 3) return false;
     p->rows_alloc = (p->rows + 7) & ~7;
-    p->tbuf_cols = p->mtiles * CC;
-    int cols = 32;
-    while (cols < 2 * p->tbuf_cols) cols <<= 1;
-    if (cols > 512) return false;
-    p->tmem_cols = cols;
-    p->idesc = tc::make_idesc(is_bf16, CC);
+    (void)is_bf16;
     p->pitchE = CC * 2 + 16;
     p->e_rows = p->IH * p->IW + R * s + 16;          // a ragged strip still LOADS the columns of its discarded outputs
     p->n_epi = n_epi;

@@ -3,19 +3,19 @@
 //   out[m, n] = act( bias[n] + sum_k (A[m,k] * gate[m/hw, k]) * Wt[n,k] ) (+ resid[m,n])
 //
 // Same contract as pw_tc2_kernel (kernels_tc.cuh); different machine mapping.  pw_tc2 gives one 128-thread CTA one
-// 128-row tile: every tile pays TMEM allocation, barrier set-up, a cold cp.async ring and a serial fill -> MMA -> epilogue
-// sequence, which leaves the early projects at 35-60 % of the HBM roof and the late ones (K = 1152: 18 serial K blocks per
-// tile, one issuing thread) latency-bound.  K2 keeps ONE CTA per SM for the whole launch:
+// 128-row tile: every tile pays barrier set-up, a cold cp.async ring and a serial fill -> MMA -> epilogue sequence.
+// K2 keeps ONE CTA per SM for the whole launch:
 //
 //   warp 0            TMA producer   A[128 x 64] (+ W[n_tile x 64] when the weights are streamed) per K block -> ring
-//   warp 1            MMA issuer     tcgen05.mma into a 2-deep TMEM accumulator ring; tcgen05.commit frees ring stages
-//   warps 4-7, 8-11   epilogue       two groups, one per TMEM accumulator (group 0: this CTA's even tiles, group 1: the odd ones):
-//                                    TMEM -> +bias (-> swish) (+residual) -> 16-bit -> global.  The bias row sits in shared memory
-//                                    (pre-halved for the swish form h = acc/2 + b/2: one FFMA, then MUFU.TANH + FFMA) - the first
-//                                    version loaded it with LDG inside the loop and ncu showed the epilogue warps parked on those
-//                                    loads (long_scoreboard, 12 % issue-active, profiles/README.md round 2)
+//   warps 4-7, 8-11   MMA + epilogue two warpgroups (group 0: this CTA's even tiles, group 1: the odd ones): wgmma over the ring
+//                                    stages of the tile (each stage handed back to the producer once its MMAs are complete;
+//                                    the groups take the ring in turns, tile by tile, so that no group waits on a ring slot
+//                                    more than one phase ahead of the producer - parity waits cannot tell phases two apart),
+//                                    then registers -> +bias (-> swish) (+residual) -> 16-bit -> global, while the other group
+//                                    runs the MMAs of its tile.  The bias row sits in shared memory (pre-halved for the swish
+//                                    form h = acc/2 + b/2: one FFMA, then MUFU.TANH + FFMA)
 //   warps 12-15       gate           (gated convs) rescale the freshly landed A stage in shared memory by the SE gate of
-//                                    each row's crop, fence.proxy.async, hand the stage to the MMA warp
+//                                    each row's crop, fence.proxy.async, hand the stage to the MMA warpgroup
 //
 // Tiles (128 rows x n_tile columns) are dealt round-robin; weights that fit (<= 64 KB: every project up to block 9) are
 // loaded once per CTA and stay resident.  The producer runs several K blocks ahead, across tile boundaries.
@@ -36,14 +36,12 @@ struct alignas(64) K2Params {
     void* out;             // T [M][N]
     int* tflag;
     int M, K, N, hw;
-    int n_tile, n_tiles;   // columns per tile (multiple of 16, <= 256), tiles along N
+    int n_tile, n_tiles;   // columns per tile (multiple of 16, <= kK2MaxN), tiles along N
     int m_tiles, tiles;    // tiles = m_tiles * n_tiles
     int nkb;               // 64-channel K blocks
     int ksteps_last;       // K = 16 MMA steps of the last K block
     int stages;            // ring depth
     int w_resident;        // 1: the whole [n_tile x K] weight slice of this CTA's n tile stays in shared memory
-    int tmem_cols;
-    uint32_t idesc;
     uint32_t a_stage, w_stage;        // bytes per ring stage (w_stage = 0 when resident)
     uint32_t off_w, off_ring, off_g;  // shared-memory offsets from the 1024-aligned base: resident W | ring | gate rows
     uint32_t off_b;                   // ... | bias row [N] fp32
@@ -51,14 +49,14 @@ struct alignas(64) K2Params {
 };
 
 constexpr int kK2Threads = 512;
+constexpr int kK2MaxN = 64;       // accumulator registers per MMA thread = n_tile (128 rows x n_tile over one warpgroup)
 
 template <typename T, bool SWISH, bool GATE, bool RESID, bool OUT_H = false>     // OUT_H: fp16 result whatever T is (expand conv feeding KD)
 __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant__ K2Params p) {
     using namespace whenet::fused;
     extern __shared__ uint8_t smem_raw[];
-    // [0..7] full  [8..15] ready  [16..23] empty  [24,25] t_full  [26,27] t_empty  [28] w
-    __shared__ __align__(8) uint64_t bars[29];
-    __shared__ uint32_t s_tmem_base;
+    // [0..7] full  [8..15] ready  [16..23] empty  [24] w  [25, 26] turn of MMA group 0 / 1
+    __shared__ __align__(8) uint64_t bars[27];
     __shared__ int s_abort_mem;
     volatile int* s_abort = &s_abort_mem;
 
@@ -66,7 +64,7 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sW = smem0 + p.off_w, sRing = smem0 + p.off_ring, sG = smem0 + p.off_g, sB = smem0 + p.off_b;
     const uint32_t bar0 = smem_u32(&bars[0]);
-    const uint32_t b_full = bar0, b_ready = bar0 + 64, b_empty = bar0 + 128, b_t_full = bar0 + 192, b_t_empty = bar0 + 208, b_w = bar0 + 224;
+    const uint32_t b_full = bar0, b_ready = bar0 + 64, b_empty = bar0 + 128, b_w = bar0 + 192, b_turn = bar0 + 200;
     const uint32_t stage_bytes = p.a_stage + p.w_stage;
     constexpr int kGateThreads = 128;
 
@@ -76,26 +74,17 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
             mbar_init(&bars[8 + i], kGateThreads / 32);     // counts are WARPS (arrive_warp)
             mbar_init(&bars[16 + i], 1);
         }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&bars[24 + i], 1);
-            mbar_init(&bars[26 + i], 4);
-        }
-        mbar_init(&bars[28], 1);
+        mbar_init(&bars[24], 1);
+        mbar_init(&bars[25], 1);
+        mbar_init(&bars[26], 1);
         s_abort_mem = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"((uint32_t)p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     for (int i = tid; i < p.N; i += kK2Threads) {
         const float b = __ldg(p.bias + i);
         asm volatile("st.shared.f32 [%0], %1;" ::"r"(sB + (uint32_t)i * 4u), "f"(SWISH ? 0.5f * b : b) : "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = s_tmem_base;
 
     // tile -> (m tile, n tile): the n tiles of one m tile are adjacent (A re-read from L2); with resident weights every
     // CTA keeps ONE n tile (n_tiles == 1 in that mode)
@@ -123,102 +112,66 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
                 }
             }
         }
-    } else if (warp == 1) {
-        // =========================================================================== MMA issuer
+    } else if (warp >= 4 && warp < 12) {
+        // =========================================================================== MMA + epilogue (group grp: tiles k = grp, grp + 2, ...)
+        constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+        const int wq = warp & 3, grp = (warp - 4) >> 2;
+        const int wt = tid & 127;
+        const T* resid = reinterpret_cast<const T*>(p.resid);
+        T* out = reinterpret_cast<T*>(p.out);
+        const int nch16 = p.n_tile >> 4;
         if (p.w_resident) k1w::wait(b_w, 0, s_abort, p.tflag);
-        int g = 0, k = 0;
-        for (int tile = first; tile < p.tiles; tile += step, ++k) {
-            const int tb = k & 1;
-            k1w::wait(b_t_empty + 8 * tb, ((k >> 1) & 1) ^ 1, s_abort, p.tflag);    // the epilogue has drained this accumulator
-            for (int kb = 0; kb < p.nkb; ++kb, ++g) {
+        for (int tile = first + grp * step, k = grp; tile < p.tiles; tile += 2 * step, k += 2) {
+            const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
+            WgAcc<kK2MaxN / 16> acc;
+            if (k > 0) k1w::wait(b_turn + 8 * grp, (uint32_t)((k - 1) >> 1) & 1u, s_abort, p.tflag);    // the other group is done with tile k-1
+            for (int kb = 0; kb < p.nkb; ++kb) {
+                const int g = k * p.nkb + kb;                    // ring slots are filled in tile order
                 const int s = g % p.stages;
                 const uint32_t par = (uint32_t)(g / p.stages) & 1u;
                 k1w::wait((GATE ? b_ready : b_full) + 8 * s, par, s_abort, p.tflag);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0 && !*s_abort) {
-                    const uint32_t a_st = sRing + (uint32_t)s * stage_bytes;
-                    const uint32_t w_st = p.w_resident ? sW + (uint32_t)kb * p.n_tile * 128 : a_st + p.a_stage;
-                    const uint64_t ad = make_desc(a_st), bd = make_desc(w_st);
-                    const int ksteps = kb == p.nkb - 1 ? p.ksteps_last : 4;
-                    for (int kk = 0; kk < ksteps; ++kk)
-                        umma_f16(tmem_base + (uint32_t)(tb * p.n_tile), ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2), p.idesc, (kb | kk) ? 1u : 0u);
-                    k1w::commit(b_empty + 8 * s);
-                    if (kb == p.nkb - 1) k1w::commit(b_t_full + 8 * tb);
-                }
-                __syncwarp();
+                const uint32_t a_st = sRing + (uint32_t)s * stage_bytes;
+                const uint32_t w_st = p.w_resident ? sW + (uint32_t)kb * p.n_tile * 128 : a_st + p.a_stage;
+                wg_fence();
+                wg_mma_tile<BF16, kK2MaxN / 16>(acc, a_st, w_st, kb == p.nkb - 1 ? p.ksteps_last : 4, nch16, kb ? 1u : 0u);
+                wg_commit();
+                wg_wait<0>();
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");      // the whole warpgroup's MMAs are done with the stage
+                if (wt == 0) k1w::arrive(b_empty + 8 * s);
             }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // =========================================================================== epilogue (group g owns accumulator g)
-        const int q4 = warp & 3, grp = (warp - 4) >> 2;
-        const int row = q4 * 32 + lane;                          // row of the tile == TMEM lane
-        const T* resid = reinterpret_cast<const T*>(p.resid);
-        T* out = reinterpret_cast<T*>(p.out);
-        for (int tile = first + grp * step, k = grp; tile < p.tiles; tile += 2 * step, k += 2) {
-            const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
-            const int tb = grp;
-            const long long m = (long long)mt * BM + row;
+            if (wt == 0) k1w::arrive(b_turn + 8 * (grp ^ 1));
+            if (*s_abort) continue;
+            // fragment -> output: register 4i + e of piece j = row 16 wq + lane/4 (+8 for e >= 2) of row half h,
+            // columns 16 j + 8 i + 2 (lane % 4) + {0, 1}
             const int n0 = nt * p.n_tile;
             const int n_valid = min(p.n_tile, p.N - n0);
-            const bool row_ok = m < p.M;
-            const bool wide = (p.N & 15) == 0;                   // rows start on 32-byte boundaries
-            k1w::wait(b_t_full + 8 * tb, (k >> 1) & 1, s_abort, p.tflag);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (!*s_abort) {
-                const uint32_t t0 = tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(tb * p.n_tile);
-                uint32_t ra[16], rb[16];
-                tmem_ld16_issue(t0, ra);
-                for (int c0 = 0; c0 < n_valid; c0 += 32) {
-                    tmem_ld16_wait(ra);
-                    if (c0 + 16 < n_valid) tmem_ld16_issue(t0 + (uint32_t)(c0 + 16), rb);
-                    // one 16-column unit of this thread's row: 32 contiguous bytes of the output -> ONE 256-bit store (a full
-                    // 32-byte sector; the first version issued two 16-byte stores per unit and the scattered half-sector
-                    // writes of the 32 rows of a warp were the limit of the epilogue)
-                    auto emit = [&](const uint32_t (&r)[16], int c) {
-                        uint32_t pk[8];
 #pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const int n = n0 + c + h * 8;
-                            if (c + h * 8 >= n_valid) break;
-                            const float4 b0 = lds_f4(sB + (uint32_t)n * 4u), b1 = lds_f4(sB + (uint32_t)n * 4u + 16u);
-                            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                            float o[8];
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                // swish: bb holds b/2 -> h = acc/2 + b/2 == (acc + b)/2 bit for bit (the halving is exact)
-                                const float a = __uint_as_float(r[h * 8 + j]);
-                                o[j] = SWISH ? swish_from_half(fmaf(a, 0.5f, bb[j])) : a + bb[j];
+                for (int e2 = 0; e2 < 2; ++e2) {
+                    const long long m = (long long)mt * BM + 64 * h + 16 * wq + (lane >> 2) + 8 * e2;
+                    if (m >= p.M) continue;
+#pragma unroll
+                    for (int j = 0; j < kK2MaxN / 16; ++j)
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const int c = 16 * j + 8 * i + 2 * (lane & 3);
+                            if (c >= n_valid) continue;
+                            const int n = n0 + c;
+                            float2 b;
+                            asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(b.x), "=f"(b.y) : "r"(sB + (uint32_t)n * 4u));
+                            const float a0 = acc.d[h][j][4 * i + 2 * e2], a1 = acc.d[h][j][4 * i + 2 * e2 + 1];
+                            // swish: b holds b/2 -> h = acc/2 + b/2 == (acc + b)/2 bit for bit (the halving is exact)
+                            float o0 = SWISH ? swish_from_half(fmaf(a0, 0.5f, b.x)) : a0 + b.x;
+                            float o1 = SWISH ? swish_from_half(fmaf(a1, 0.5f, b.y)) : a1 + b.y;
+                            if (RESID) {
+                                float lo, hi;
+                                unpack2<T>(*reinterpret_cast<const uint32_t*>(resid + m * p.N + n), lo, hi);
+                                o0 += lo; o1 += hi;
                             }
-                            if (RESID && row_ok) {
-                                float rr[8];
-                                ld8<T>(resid + m * p.N + n, rr);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) o[j] += rr[j];
-                            }
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                pk[h * 4 + j] = OUT_H ? pack2<__half>(o[2 * j], o[2 * j + 1]) : pack2<T>(o[2 * j], o[2 * j + 1]);
+                            *reinterpret_cast<uint32_t*>(out + m * p.N + n) = OUT_H ? pack2<__half>(o0, o1) : pack2<T>(o0, o1);
                         }
-                        if (row_ok) {
-                            T* dst = out + m * p.N + n0 + c;
-                            if (wide && c + 16 <= n_valid)
-                                asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]),
-                                             "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7]) : "memory");
-                            else {
-                                *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                                if (c + 8 < n_valid) *reinterpret_cast<uint4*>(dst + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                            }
-                        }
-                    };
-                    emit(ra, c0);
-                    if (c0 + 16 >= n_valid) break;
-                    tmem_ld16_wait(rb);
-                    if (c0 + 32 < n_valid) tmem_ld16_issue(t0 + (uint32_t)(c0 + 32), ra);
-                    emit(rb, c0 + 16);
                 }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            k1w::arrive_warp(b_t_empty + 8 * tb);
         }
     } else if (GATE && warp >= 12) {
         // =========================================================================== gate: A stage <- A stage * gate[crop(row)]
@@ -275,10 +228,6 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
 }
 
 // Fills every field of K2Params except the tensor maps and the pointers.  false: shape not supported (caller falls back).
@@ -286,11 +235,11 @@ inline bool plan_k2(long long M, int K, int N, int hw, bool has_gate, bool is_bf
     if ((K & 7) || (N & 7) || M < 1 || M > 0x7fffffffLL || K < 16) return false;
     p->M = (int)M; p->K = K; p->N = N; p->hw = hw;
     int n_tile = N;
-    if (N > 256) {
-        int parts = (N + 255) / 256;
+    if (N > kK2MaxN) {
+        int parts = (N + kK2MaxN - 1) / kK2MaxN;
         while (true) {
             n_tile = ((N + parts - 1) / parts + 15) & ~15;
-            if (n_tile <= 256) break;
+            if (n_tile <= kK2MaxN) break;
             ++parts;
         }
     }
@@ -301,11 +250,7 @@ inline bool plan_k2(long long M, int K, int N, int hw, bool has_gate, bool is_bf
     p->tiles = p->m_tiles * p->n_tiles;
     p->nkb = (K + 63) / 64;
     p->ksteps_last = ((K - (p->nkb - 1) * 64) + 15) / 16;
-    int cols = 32;
-    while (cols < 2 * n_tile) cols <<= 1;
-    if (cols > 512) return false;
-    p->tmem_cols = cols;
-    p->idesc = make_idesc(is_bf16, n_tile);
+    (void)is_bf16;
     p->a_stage = BM * 128;
     const size_t w_all = (size_t)p->nkb * n_tile * 128;
     p->g_rows = has_gate ? (uint32_t)std::min(4, (BM - 1) / hw + 2) : 0;

@@ -231,8 +231,7 @@ __global__ void __launch_bounds__(224) stem_tile_kernel(const void* __restrict__
     if (tid < 15) s_in[(tid / 3) * ROWF + 672 + tid % 3] = 0.f;   // pad pixel (column 224) of the 5 rows
     __syncthreads();
     const int oyl = tid / 112, ox = tid - oyl * 112;
-    // 32 output channels as 16 pairs: one FFMA2 (fma.rn.f32x2) per pair and tap - the same IEEE FMAs in half the issue
-    // slots; ptxas feeds the weight pair from the constant bank through a uniform register and broadcasts the scalar input
+    // 32 output channels as 16 pairs, weights from the constant bank, the scalar input broadcast
     float2 acc2[16];
 #pragma unroll
     for (int c = 0; c < 16; ++c) acc2[c] = make_float2(sp.b[2 * c], sp.b[2 * c + 1]);
@@ -246,9 +245,8 @@ __global__ void __launch_bounds__(224) stem_tile_kernel(const void* __restrict__
 #pragma unroll
             for (int c = 0; c < 16; ++c) {
                 const float2 w2 = make_float2(sp.w[(ky * 9 + t) * 32 + 2 * c], sp.w[(ky * 9 + t) * 32 + 2 * c + 1]);
-                asm("fma.rn.f32x2 %0, %1, %2, %0;"
-                    : "+l"(reinterpret_cast<unsigned long long&>(acc2[c]))
-                    : "l"(reinterpret_cast<const unsigned long long&>(xx)), "l"(reinterpret_cast<const unsigned long long&>(w2)));
+                acc2[c].x = fmaf(xx.x, w2.x, acc2[c].x);
+                acc2[c].y = fmaf(xx.y, w2.y, acc2[c].y);
             }
         }
     }

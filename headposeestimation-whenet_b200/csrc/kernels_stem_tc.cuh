@@ -9,11 +9,12 @@
 //   channel that holds float32(((v/255) - mean)/std) (reference whenet.py:25-26, evaluated in float64 like numpy) already split
 //   into a bf16 high part and a bf16 low part (hi + lo carries 16 mantissa bits: the bf16 rounding of the INPUT alone would cost
 //   0.24 deg, SURVEY.md 8c) -> K = 64: [hi(27) 0(5) | lo(27) 0(5)] against W = [w | 0 | w | 0] (bf16 weights).
-//   One tcgen05.mma block (128 pixels x 32 channels x K 64, four K steps) per output row; accumulators in TMEM.
+//   One warpgroup MMA block (128 pixels x 32 channels x K 64, four K steps) per output row; fp32 accumulators in registers.
 //
 // CTA = 128 threads = one output row at a time (112 pixels + 16 idle rows of the M = 128 tile), ROWS rows per CTA.  Thread p
 // builds A row p for output row r+1 (27 byte loads, 27 table loads, 28 PRMT, 8 swizzled 16-byte stores) while the MMA of row r
-// runs, then drains row r from TMEM: h = acc/2 + b/2 -> MUFU.TANH -> FMA -> 16-bit -> two 256-bit stores (32 channels).
+// runs, then drains row r through the shared accumulator tile: h = acc/2 + b/2 -> MUFU.TANH -> FMA -> 16-bit -> four 16-byte
+// stores (32 channels).
 #pragma once
 #include "kernels_fused.cuh"
 
@@ -28,31 +29,20 @@ struct StemTcGeom {
 
 template <typename TOUT>
 __global__ void __launch_bounds__(128) stem_tc_kernel(const uint8_t* __restrict__ in, TOUT* __restrict__ out,
-                                                      const __grid_constant__ StemParams sp, const float* __restrict__ lut, int* tflag) {
+                                                      const __grid_constant__ StemParams sp, const float* __restrict__ lut) {
     using G = StemTcGeom;
     constexpr int A_BYTES = 128 * 128;              // one A tile: 128 rows x 64 bf16, SWIZZLE_128B
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t mbar[2];
-    __shared__ uint32_t s_tmem_base;
-    __shared__ int s_abort;
     const uint32_t smem0 = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sA = smem0;                                  // 2 x A tile
     const uint32_t sW = sA + 2 * A_BYTES;                       // [32 rows n][128 B]  (4 KB)
     const uint32_t sL = sW + 32 * 128;                          // table [3][256] u32 = hi | lo << 16
     const uint32_t sI = sL + 3 * 256 * 4;                       // staged input rows [IN_ROWS][ROW_PITCH] bytes
     const uint32_t sB = sI + G::IN_ROWS * G::ROW_PITCH;         // 32 floats: b/2
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const uint32_t sAcc = sB + 128;                             // shared accumulator tile, 32 columns
+    const int tid = threadIdx.x;
     const int n = blockIdx.y, oy0 = blockIdx.x * G::ROWS;
 
-    if (tid == 0) {
-        tc::mbar_init(&mbar[0], 1); tc::mbar_init(&mbar[1], 1);
-        s_abort = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&s_tmem_base)), "r"(64u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     // ---- table: float -> bf16 hi | bf16 lo
     for (int i = tid; i < 768; i += 128) {
         const float f = lut[i];
@@ -84,13 +74,9 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const uint8_t* __restrict_
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = s_tmem_base;
-    const uint32_t idesc = tc::make_idesc(true, 32);
 
-    const int ox = tid;                                         // pixel of the row = A row = TMEM lane
+    const int ox = tid;                                         // pixel of the row = A row = accumulator row
     const bool px_ok = ox < 112;
     // one A row: 27 taps -> table -> hi chunks 0..3, lo chunks 4..7
     auto build = [&](int rl, int buf) {                          // rl = output row inside the CTA
@@ -124,65 +110,54 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const uint8_t* __restrict_
             fused::sts128(a0 + (uint32_t)(((c + 4) ^ (ox & 7)) << 4), make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]));
         }
     };
-    auto issue = [&](int buf) {                                  // thread 0, after the barrier that follows build()
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t ad = tc::make_desc(sA + buf * A_BYTES), bd = tc::make_desc(sW);
+    auto drain = [&](int rl) {
+        TOUT* dst = out + (((long long)n * 112 + oy0 + rl) * 112 + ox) * 32;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_f16(tmem_d + (uint32_t)(buf * 32), ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, k ? 1u : 0u);
-        tc::umma_commit(&mbar[buf]);
-    };
-    auto drain = [&](int rl, int buf, int use) {                 // use = how many times mbar[buf] completed before
-        if (!tc::mbar_wait(&mbar[buf], (uint32_t)use & 1u, tflag)) s_abort = 1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (!s_abort) {
-            const uint32_t t0 = tmem_d + ((uint32_t)(warp * 32) << 16) + (uint32_t)(buf * 32);
-            TOUT* dst = out + (((long long)n * 112 + oy0 + rl) * 112 + ox) * 32;
+        for (int u = 0; u < 2; ++u) {
+            float v[16];
+            tc::acc_ld16(sAcc, ox, u * 16, v);
+            uint32_t pk[8];
 #pragma unroll
-            for (int u = 0; u < 2; ++u) {
-                float v[16];
-                tc::tmem_ld16(t0 + (uint32_t)(u * 16), v);
-                uint32_t pk[8];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float4 bq = fused::lds_f4(sB + (uint32_t)(u * 16 + j * 4) * 4u);
-                    const float h0 = swish_from_half(fmaf(v[4 * j], 0.5f, bq.x)), h1 = swish_from_half(fmaf(v[4 * j + 1], 0.5f, bq.y));
-                    const float h2 = swish_from_half(fmaf(v[4 * j + 2], 0.5f, bq.z)), h3 = swish_from_half(fmaf(v[4 * j + 3], 0.5f, bq.w));
-                    pk[2 * j] = fused::pack2<TOUT>(h0, h1);
-                    pk[2 * j + 1] = fused::pack2<TOUT>(h2, h3);
-                }
-                if (px_ok)
-                    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + u * 16), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]),
-                                 "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7]) : "memory");
+            for (int j = 0; j < 4; ++j) {
+                const float4 bq = fused::lds_f4(sB + (uint32_t)(u * 16 + j * 4) * 4u);
+                const float h0 = swish_from_half(fmaf(v[4 * j], 0.5f, bq.x)), h1 = swish_from_half(fmaf(v[4 * j + 1], 0.5f, bq.y));
+                const float h2 = swish_from_half(fmaf(v[4 * j + 2], 0.5f, bq.z)), h3 = swish_from_half(fmaf(v[4 * j + 3], 0.5f, bq.w));
+                pk[2 * j] = fused::pack2<TOUT>(h0, h1);
+                pk[2 * j + 1] = fused::pack2<TOUT>(h2, h3);
+            }
+            if (px_ok) {
+                *reinterpret_cast<uint4*>(dst + u * 16) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                *reinterpret_cast<uint4*>(dst + u * 16 + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
             }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     };
 
+    tc::WgAcc<2> acc;
     build(0, 0);
     for (int rl = 0; rl < G::ROWS; ++rl) {
         const int buf = rl & 1;
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();                            // A(rl) complete; TMEM[buf] drained (row rl-2), A[buf^1] free (MMA rl-1 waited below)
-        if (tid == 0 && !s_abort) issue(buf);
-        if (rl >= 1) drain(rl - 1, buf ^ 1, (rl - 1) >> 1);      // also proves MMA(rl-1) done with A[buf^1]
-        if (rl + 1 < G::ROWS) build(rl + 1, buf ^ 1);
+        __syncthreads();                            // A(rl) complete; row rl-1 drained out of the accumulator tile
+        tc::wg_fence();
+        tc::wg_mma_tile<true, 2>(acc, sA + buf * A_BYTES, sW, 4, 2, 0u);
+        tc::wg_commit();
+        if (rl + 1 < G::ROWS) build(rl + 1, buf ^ 1);           // A[buf^1]: its MMA (row rl-1) completed last iteration
+        tc::wg_wait<0>();
+        tc::wg_acc_store<2>(acc, sAcc, 2, tid);
+        __syncthreads();
+        drain(rl);
     }
-    drain(G::ROWS - 1, (G::ROWS - 1) & 1, (G::ROWS - 1) >> 1);
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(64u) : "memory");
 }
 
 constexpr size_t stem_tc_smem() {
-    return (size_t)2 * 128 * 128 + 32 * 128 + 3 * 256 * 4 + (size_t)StemTcGeom::IN_ROWS * StemTcGeom::ROW_PITCH + 128 + 1024;
+    return (size_t)2 * 128 * 128 + 32 * 128 + 3 * 256 * 4 + (size_t)StemTcGeom::IN_ROWS * StemTcGeom::ROW_PITCH + 128 + tc::acc_tile_bytes(32) + 1024;
 }
 
 template <typename TOUT>
-int launch_stem_tc(cudaStream_t stream, const uint8_t* in, TOUT* out, const StemParams& sp, const float* lut, int* tflag, int n_crops) {
+int launch_stem_tc(cudaStream_t stream, const uint8_t* in, TOUT* out, const StemParams& sp, const float* lut, int n_crops) {
     auto kfn = stem_tc_kernel<TOUT>;
     if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stem_tc_smem()) != cudaSuccess) return -1;
-    kfn<<<dim3(112 / StemTcGeom::ROWS, n_crops), 128, stem_tc_smem(), stream>>>(in, out, sp, lut, tflag);
+    kfn<<<dim3(112 / StemTcGeom::ROWS, n_crops), 128, stem_tc_smem(), stream>>>(in, out, sp, lut);
     return 0;
 }
 

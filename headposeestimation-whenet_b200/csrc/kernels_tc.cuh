@@ -1,15 +1,15 @@
-// kernels_tc.cuh - tcgen05 (5th-gen tensor core) kernels for the 1x1 convolutions + the helpers every tcgen05 kernel shares.
+// kernels_tc.cuh - Hopper warpgroup-MMA (wgmma) kernels for the 1x1 convolutions + the helpers every tensor-core kernel shares.
 //
 //   out[m, n] = act( bias[n] + sum_k (A[m,k] * gate[m/hw, k]) * Wt[n,k] ) (+ resid[m,n])
 //
 // A  : activations, NHWC == row-major [M = crops*H*W][K = Cin], 16-bit (bf16 / fp16)   -> "K-major"
 // Wt : BN-folded weights transposed to [N = Cout][K], 16-bit                           -> "K-major"
-// D  : fp32 accumulator in tensor memory (TMEM), 128 lanes (pixels) x n_tile columns
+// D  : fp32 accumulators in the registers of the issuing warpgroup (128 threads)
 //
-// Operands sit in shared memory in the canonical K-major SWIZZLE_128B UMMA layout (16-byte chunk c of row r lands at
-// chunk c ^ (r & 7) of its 128-byte row; 8-row atoms of 1024 B); one elected thread issues
-// tcgen05.mma.cta_group::1.kind::f16 (M=128, N=n_tile, K=16), tcgen05.commit -> mbarrier hands stages back, and the
-// epilogue reads TMEM lanes with tcgen05.ld (thread == pixel row).
+// Operands sit in shared memory in the canonical K-major SWIZZLE_128B layout (16-byte chunk c of row r lands at chunk
+// c ^ (r & 7) of its 128-byte row; 8-row atoms of 1024 B).  A 128-row tile is two wgmma.m64nNk16 row halves; N is walked in
+// 16-column pieces so one code path serves every channel count.  After the last K step the warpgroup writes its fragments
+// to a shared-memory accumulator tile ([column][kAccPitch] fp32), where the epilogues read one pixel row per thread.
 //
 // Every mbarrier wait is bounded: a wait that exceeds its budget raises the context's timeout flag (mapped pinned host
 // memory) and the CTA bails out instead of hanging the GPU.
@@ -24,13 +24,15 @@
 namespace whenet {
 namespace tc {
 
-// Timeout flag: ONE int per context in mapped pinned host memory (whenet_api.cu); every tcgen05 kernel gets its device
-// address as a parameter and raises it when a bounded mbarrier wait expires.  The host reads it straight from the pinned
-// page after any stream synchronisation - no per-translation-unit device symbols, no extra copies.
+// Timeout flag: ONE int per context in mapped pinned host memory (whenet_api.cu); every pipelined tensor-core kernel gets its
+// device address as a parameter and raises it when a bounded mbarrier wait expires.  The host reads it straight from the
+// pinned page after any stream synchronisation - no per-translation-unit device symbols, no extra copies.
 
-constexpr int BM = 128;          // pixels per CTA == TMEM lanes == UMMA M
+constexpr int BM = 128;          // pixels per tile (two wgmma row halves of 64)
 constexpr int BK = 64;           // channels per stage (one 128-byte swizzle row of 16-bit elements)
 constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KB
+constexpr int kAccPitch = 132;   // floats per column of the shared-memory accumulator tile (128 rows + 4: conflict-free both ways)
+__host__ __device__ constexpr uint32_t acc_tile_bytes(int cols) { return (uint32_t)cols * kAccPitch * 4u; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -53,50 +55,102 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* t
     return false;
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 = 1 | [32,46) SBO >> 4 = 64 (8 rows x 128 B)
-//   [46,48) version = 1 (Blackwell) | [61,64) layout type = 2 (SWIZZLE_128B)
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA descriptor):
+//   [0,14) start address >> 4 | [16,30) LBO >> 4 = 1 | [32,46) SBO >> 4 = 64 (8 rows x 128 B) | [62,64) layout = 1 (SWIZZLE_128B)
+// A K step of 16 elements (32 bytes inside the swizzle row) advances the start address field by 2.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)64 << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): D=f32, A/B = bf16 or f16, both K-major.
-__host__ __device__ inline uint32_t make_idesc(bool is_bf16, int umma_n, int b_fmt = -1) {
-    uint32_t d = 0;
-    d |= 1u << 4;                           // c_format = F32
-    d |= (is_bf16 ? 1u : 0u) << 7;          // a_format
-    d |= ((b_fmt < 0 ? is_bf16 : b_fmt != 0) ? 1u : 0u) << 10;         // b_format (b_fmt: -1 = as A, 0 = f16, 1 = bf16)
-    d |= (uint32_t)(umma_n >> 3) << 17;     // n_dim
-    d |= (uint32_t)(BM >> 4) << 24;         // m_dim
-    return d;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D(64 x 16) (+)= A(64 x 16) * B(16 x 16)^T, both operands K-major in shared memory; fp32 accumulators
+template <bool BF16>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t ad, uint64_t bd, uint32_t accumulate) {
+    if constexpr (BF16)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(ad), "l"(bd), "r"(accumulate));
+    else
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(ad), "l"(bd), "r"(accumulate));
 }
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// Accumulators of one warpgroup: row half h (rows 64h..64h+63) x NCH 16-column pieces
+template <int NCH> struct WgAcc { float d[2][NCH][8]; };
+
+// Issue the K steps [k0, k0 + ksteps) of a 128-row tile: a_st / b_st are the K block's operand bases (8-row atoms of
+// 1024 B), `nch` 16-column pieces of B (rows 16j.. of the weight tile).  Called by all 128 threads of a warpgroup.
+// `accumulate` == 0 starts the sums at zero with the first step.  The caller commits / waits.
+template <bool BF16, int NCH>
+__device__ __forceinline__ void wg_mma_tile(WgAcc<NCH>& acc, uint32_t a_st, uint32_t b_st, int ksteps, int nch, uint32_t accumulate) {
+    const uint64_t a0 = make_desc(a_st), a1 = make_desc(a_st + 64 * 128);
+    for (int k = 0; k < ksteps; ++k) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+        for (int j = 0; j < NCH; ++j) {
+            if (j < nch) {
+                const uint64_t bd = make_desc(b_st + (uint32_t)j * 2048u) + (uint64_t)(k * 2);
+                wgmma_n16<BF16>(acc.d[0][j], a0 + (uint64_t)(k * 2), bd, (accumulate | (uint32_t)k) ? 1u : 0u);
+                wgmma_n16<BF16>(acc.d[1][j], a1 + (uint64_t)(k * 2), bd, (accumulate | (uint32_t)k) ? 1u : 0u);
+            }
+        }
+    }
+}
+
+// One 64-row half on its own (kernels whose warpgroups split the M tiles of a CTA between them): D(64 x 16 nch) (+)= A * B^T
+// over `ksteps` K steps; a_kb / b_kb = byte distance between consecutive 64-channel K blocks of A / B.
+template <bool BF16, int NCH>
+__device__ __forceinline__ void wg_mma_m64(float (&d)[NCH][8], uint32_t a_st, uint32_t a_kb, uint32_t b_st, uint32_t b_kb, int ksteps, int nch) {
+    for (int ks = 0; ks < ksteps; ++ks) {
+        const int kb = ks >> 2, k = ks & 3;
+        const uint64_t ad = make_desc(a_st + (uint32_t)kb * a_kb) + (uint64_t)(k * 2);
+#pragma unroll
+        for (int j = 0; j < NCH; ++j)
+            if (j < nch) wgmma_n16<BF16>(d[j], ad, make_desc(b_st + (uint32_t)kb * b_kb + (uint32_t)j * 2048u) + (uint64_t)(k * 2), ks ? 1u : 0u);
+    }
+}
+
+// Fragments -> shared accumulator tile [column][kAccPitch] (fp32).  `wt` = thread index inside the warpgroup.
+// m64n16 fragment: register 4i + {0,1} -> row 16 w + l/4, columns 8 i + 2 (l%4) + {0,1}; 4i + {2,3} -> row + 8
+template <int NCH>
+__device__ __forceinline__ void wg_acc_store(const WgAcc<NCH>& acc, uint32_t dst, int nch, int wt) {
+    const int w = wt >> 5, l = wt & 31;
+    const int r = 16 * w + (l >> 2), cq = 2 * (l & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < NCH; ++j) {
+            if (j < nch) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int row = 64 * h + r + (e >> 1) * 8, col = 16 * j + 8 * i + cq + (e & 1);
+                        asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (uint32_t)(col * kAccPitch + row) * 4u), "f"(acc.d[h][j][4 * i + e]) : "memory");
+                    }
+            }
+        }
+}
+
+// 16 consecutive columns of one accumulator row from the shared accumulator tile
+__device__ __forceinline__ void acc_ld16(uint32_t base, int row, int c0, float (&v)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[i]) : "r"(base + (uint32_t)((c0 + i) * kAccPitch + row) * 4u));
 }
 
 template <typename T> __device__ __forceinline__ uint4 scale8(uint4 raw, const float* g);
@@ -130,7 +184,7 @@ template <> __device__ __forceinline__ uint4 scale8<__half>(uint4 raw, const flo
 //   * the SE gate is applied IN shared memory by the thread that copied the chunk (so no extra barrier):
 //       GATE == 1: on the A rows (tiles may span up to four crops; their gate rows sit in smem)
 //       GATE == 2: on the W rows (per-crop tiling: a tile never leaves its crop, used while H*W >= 784)
-//   * stage reuse is gated by the mbarrier of the previous block's tcgen05.commit.
+//   * stage reuse waits for the wgmma group of the block that last read the stage.
 // exact floor(x / d) for small non-negative ints (x < 2^17, d < 2^8) with inv = 1.0f / d: (x + 0.5) / d is at least 0.5 / d
 // away from every integer, far more than the float rounding error - replaces the ~20-instruction integer division
 __device__ __forceinline__ int fdiv_small(int x, float inv) { return __float2int_rz(((float)x + 0.5f) * inv); }
@@ -180,15 +234,12 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
                                                      const float* __restrict__ bias, const float* __restrict__ gate,
                                                      const T* __restrict__ resid, T* __restrict__ out,
                                                      int M, int K, int N, int hw,
-                                                     int n_tile, int umma_n, int tmem_cols, int n_stages,
-                                                     int tiles_per_crop,     // GATE == 2 only
-                                                     uint32_t idesc, int* tflag) {
+                                                     int n_tile, int umma_n, int n_stages,
+                                                     int tiles_per_crop) {    // GATE == 2 only
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t mbar[4];
-    __shared__ uint32_t s_tmem_base;
-    __shared__ int s_abort;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const int w_stage_bytes = umma_n * BK * 2;
     const uint32_t stage_bytes = A_STAGE_BYTES + w_stage_bytes;
@@ -211,15 +262,6 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
     const int nkb = (K + BK - 1) / BK;
     const int kchunks = K >> 3;
 
-    if (tid == 0) {
-        for (int i = 0; i < 4; ++i) mbar_init(&mbar[i], 1);
-        s_abort = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"((uint32_t)tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     // gate rows of the crops this tile touches -> smem (joins the first cp.async group)
     if (GATE) {
         const int ncrops = GATE == 2 ? 1 : ((m0 + rows_valid - 1) / hw - crop0 + 1);
@@ -269,10 +311,8 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
         if (j < nkb) fill(j);
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = s_tmem_base;
+    WgAcc<8> acc;
+    const int nch16 = umma_n >> 4;
 
     // GATE == 1: byte offset of the gate row (crop) of each of the 8 rows this thread rescales, fixed for the whole K loop
     uint32_t g_row[8];
@@ -337,45 +377,40 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (tid == 0 && !s_abort) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        {
             const int krem = min(BK, K - kb * BK);
-            const int ksteps = (krem + 15) >> 4;
-            const uint64_t ad = make_desc(a_st), bd = make_desc(w_st);
-            for (int k = 0; k < ksteps; ++k)
-                umma_f16(tmem_d, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-            umma_commit(&mbar[s]);
+            wg_fence();
+            wg_mma_tile<BF16, 8>(acc, a_st, w_st, (krem + 15) >> 4, nch16, kb ? 1u : 0u);
+            wg_commit();
         }
-        // refill the stage block kb-1 used (its MMAs are done or about to be) with block kb-1+n_stages
+        // refill the stage block kb-1 used with block kb-1+n_stages once its MMAs have completed (every thread's group)
         if (kb >= 1 && kb - 1 + n_stages < nkb) {
-            const int pb = kb - 1;
-            if (!mbar_wait(&mbar[pb % n_stages], (pb / n_stages) & 1, tflag)) s_abort = 1;
-            fill(pb + n_stages);
+            wg_wait<1>();
+            __syncthreads();
+            fill(kb - 1 + n_stages);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
-    {
-        const int last = nkb - 1;
-        if (!mbar_wait(&mbar[last % n_stages], (last / n_stages) & 1, tflag)) s_abort = 1;
-    }
+    wg_wait<0>();
     asm volatile("cp.async.wait_group 0;" ::: "memory");
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    __syncthreads();
+    // the operand ring is free: accumulators -> shared accumulator tile at smem0, the 16-bit output stage after it
+    const uint32_t sAcc = smem0;
+    wg_acc_store<8>(acc, sAcc, nch16, tid);
     __syncthreads();
 
     // ---- epilogue: TMEM -> +shift, swish, +residual -> 16-bit -> stage -> coalesced stores
     const int nch = n_valid >> 3;
     const float inv_nch = 1.0f / (float)(nch > 0 ? nch : 1);
     const int pitch16 = nch | 1;
-    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (smem0 - smem_u32(smem_raw)));
+    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (smem0 + acc_tile_bytes(umma_n) - smem_u32(smem_raw)));
     const bool row_ok = tid < rows_valid;
     const long long m = (long long)m0 + tid;
-    if (!s_abort) {
-        const uint32_t lane_base = tmem_d + ((uint32_t)(warp * 32) << 16);
+    {
         for (int c0 = 0; c0 < n_valid; c0 += 16) {
             float v[16];
-            tmem_ld16(lane_base + (uint32_t)c0, v);
+            acc_ld16(sAcc, tid, c0, v);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int n = n0 + c0 + h * 8;
@@ -400,33 +435,28 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
         }
     }
     __syncthreads();
-    if (!s_abort) {
-        for (int idx = tid; idx < rows_valid * nch; idx += 128) {
-            const int r = fdiv_small(idx, inv_nch), j = idx - r * nch;
-            *reinterpret_cast<uint4*>(out + ((long long)m0 + r) * N + n0 + j * 8) = stage[r * pitch16 + j];
-        }
+    for (int idx = tid; idx < rows_valid * nch; idx += 128) {
+        const int r = fdiv_small(idx, inv_nch), j = idx - r * nch;
+        *reinterpret_cast<uint4*>(out + ((long long)m0 + r) * N + n0 + j * 8) = stage[r * pitch16 + j];
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((uint32_t)tmem_cols) : "memory");
 }
 
 template <typename T>
-int launch_pw_tc2(cudaStream_t stream, int* tflag, const T* A, const void* Wt16, const float* bias, const float* gate, const T* resid,
-                  T* out, long long M, int K, int N, int hw, bool swish, int stage_cap = 0, int smem_budget_kb = 54, int min_ctas = 296,
-                  bool out_half = false, int b_fmt = -1) {
+int launch_pw_tc2(cudaStream_t stream, const T* A, const void* Wt16, const float* bias, const float* gate, const T* resid,
+                  T* out, long long M, int K, int N, int hw, bool swish, int stage_cap = 0, int smem_budget_kb = 54, int min_ctas = 264,
+                  bool out_half = false) {
     if (sizeof(T) != 2) return 1;
     if ((K & 7) || (N & 7) || M > 0x7fffffffLL) return 1;
     const bool per_crop = gate && hw >= 784;                 // gate on W, tiles stay inside a crop
     const int tpc = (hw + BM - 1) / BM;
     const long long m_tiles = per_crop ? (M / hw) * tpc : (M + BM - 1) / BM;
+    // at most 128 columns per tile: the warpgroup holds the whole 128 x n_tile accumulator in registers (n_tile per thread)
     int n_tile = N;
-    if (N > 256) {
-        int parts = (N + 255) / 256;
+    if (N > 128) {
+        int parts = (N + 127) / 128;
         while (true) {
             n_tile = ((N + parts - 1) / parts + 15) & ~15;
-            if (n_tile <= 256) break;
+            if (n_tile <= 128) break;
             ++parts;
         }
     }
@@ -437,18 +467,15 @@ int launch_pw_tc2(cudaStream_t stream, int* tflag, const T* A, const void* Wt16,
         n_tile = nt;
     }
     const int umma_n = (n_tile + 15) & ~15;
-    int tmem_cols = 32;
-    while (tmem_cols < umma_n) tmem_cols <<= 1;
-    const uint32_t idesc = make_idesc(std::is_same<T, __nv_bfloat16>::value, umma_n, b_fmt);
     const int nkb = (K + BK - 1) / BK;
     const size_t stage_bytes = A_STAGE_BYTES + (size_t)umma_n * BK * 2;
     const int gate_crops = per_crop ? 1 : std::min(4, (BM - 1) / hw + 2);      // crops one 128-row tile can touch
     const size_t gate_bytes = gate ? (size_t)gate_crops * K * 4 : 0;
-    const size_t out_bytes = (size_t)BM * ((size_t)(n_tile >> 3) | 1) * 16;
+    const size_t out_bytes = acc_tile_bytes(umma_n) + (size_t)BM * ((size_t)(n_tile >> 3) | 1) * 16;     // accumulator tile + output stage
     int n_stages = nkb < 4 ? nkb : 4;
     if (stage_cap > 0 && n_stages > stage_cap) n_stages = stage_cap;
     // a grid that does not even fill the SMs once (single-crop latency path) gains nothing from co-residency: deepest ring
-    if (m_tiles * ((N + n_tile - 1) / n_tile) < 148) smem_budget_kb = 180;
+    if (m_tiles * ((N + n_tile - 1) / n_tile) < 132) smem_budget_kb = 180;
     // ring depth vs co-residency: a shallower ring lets more CTAs share the SM (budget = smem per CTA)
     while (n_stages > 2 && n_stages * stage_bytes + gate_bytes > (size_t)smem_budget_kb * 1024) --n_stages;
     size_t smem = n_stages * stage_bytes + gate_bytes;
@@ -461,7 +488,7 @@ int launch_pw_tc2(cudaStream_t stream, int* tflag, const T* A, const void* Wt16,
     do {                                                                                                             \
         auto kfn = pw_tc2_kernel<T, SW, GA, RE, OH>;                                                       \
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) != cudaSuccess) return -1; \
-        kfn<<<grid, 128, smem, stream>>>(A, W, bias, gate, resid, out, (int)M, K, N, hw, n_tile, umma_n, tmem_cols, n_stages, tpc, idesc, tflag); \
+        kfn<<<grid, 128, smem, stream>>>(A, W, bias, gate, resid, out, (int)M, K, N, hw, n_tile, umma_n, n_stages, tpc); \
     } while (0)
     if (out_half && !(swish && !gate && !resid)) return 1;
     if (swish && !gate && !resid) { if (out_half) TC2(true, 0, false, true); else TC2(true, 0, false, false); }
@@ -477,42 +504,30 @@ int launch_pw_tc2(cudaStream_t stream, int* tflag, const T* A, const void* Wt16,
 
 // ----------------------------------------------------------------------------- pw_tc3: gated projects of the large maps
 // The gated project convs of blocks 1-5 are streams of tiny GEMMs (K = 32..144, N = 16..40, millions of rows): with one 128-row
-// tile per CTA (pw_tc2) every tile pays TMEM allocation, the gate row, the W copy + its rescale and a cold load -> MMA ->
-// epilogue chain - block 1 ran at 2.2 TB/s.  Here a CTA walks `tpc` consecutive tiles of ONE crop: gate row and W' = bf16(W * g)
-// once per CTA (the same scale8s as pw_tc2's per-crop route, so the results are bit-identical), then a two-deep software
-// pipeline over the tiles: cp.async of tile t+1 and the MMA of tile t (second TMEM accumulator) run under the epilogue of
-// tile t-1.
+// tile per CTA (pw_tc2) every tile pays the gate row, the W copy + its rescale and a cold load -> MMA -> epilogue chain.
+// Here a CTA walks `tpc` consecutive tiles of ONE crop: gate row and W' = bf16(W * g) once per CTA (the same scale8s and the
+// same wgmma sequence as pw_tc2's per-crop route, so the results are bit-identical); the cp.async of tile t+1 runs under the
+// MMA and the epilogue of tile t.
 template <typename T, bool RESID>
 __global__ void __launch_bounds__(128) pw_tc3_kernel(const T* __restrict__ A, const T* __restrict__ Wt, const float* __restrict__ bias,
                                                      const float* __restrict__ gate, const T* __restrict__ resid, T* __restrict__ out,
-                                                     int K, int N, int hw, int umma_n, int tmem_cols, int tiles_per_crop, int tpc, int groups,
-                                                     uint32_t idesc, int* tflag) {
+                                                     int K, int N, int hw, int umma_n, int tiles_per_crop, int tpc, int groups) {
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t mbar[2];
-    __shared__ uint32_t s_tmem_base;
-    __shared__ int s_abort;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int nkb = (K + BK - 1) / BK, kchunks = K >> 3;
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t w_bytes = (uint32_t)nkb * umma_n * 128, a_bytes = (uint32_t)nkb * A_STAGE_BYTES;
     const uint32_t sW = smem0, sA = sW + ((w_bytes + 1023u) & ~1023u), sG = sA + 2 * a_bytes;
+    const uint32_t sAcc = sG + (((uint32_t)K * 4 + 15u) & ~15u);
     const int nch = N >> 3, pitch16 = nch | 1;
-    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (sG + (((uint32_t)K * 4 + 15u) & ~15u) - smem_u32(smem_raw)));
+    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (sAcc + acc_tile_bytes(umma_n) - smem_u32(smem_raw)));
     const float inv_nch = 1.0f / (float)nch;
 
     const int crop = blockIdx.x / groups, g = blockIdx.x - crop * groups;
     const int t_begin = g * tpc, t_end = min(tiles_per_crop, t_begin + tpc);
     if (t_begin >= t_end) return;
 
-    if (tid == 0) {
-        mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1);
-        s_abort = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"((uint32_t)tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     // one K block of an operand: 16-byte chunk c of rows r0, r0+16, ... (the mapping pw_tc2 uses; ragged last block: zero fill)
     auto fill_rows = [&](uint32_t dst, const T* src0, int rows, int kb) {
         const int kc0 = kb * 8;
@@ -567,90 +582,66 @@ __global__ void __launch_bounds__(128) pw_tc3_kernel(const T* __restrict__ A, co
                 }
         }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = s_tmem_base;
-
-    auto epilogue = [&](int t, int buf, int it) {
-        if (!mbar_wait(&mbar[buf], (uint32_t)(it >> 1) & 1u, tflag)) s_abort = 1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    const int nch16 = umma_n >> 4;
+    auto epilogue = [&](int t) {
         const int rows_valid = min(BM, hw - t * BM);
         const long long m0 = (long long)crop * hw + (long long)t * BM;
         const bool row_ok = tid < rows_valid;
-        if (!s_abort) {
-            const uint32_t lane_base = tmem_d + ((uint32_t)(warp * 32) << 16) + (uint32_t)(buf * umma_n);
-            for (int c0 = 0; c0 < N; c0 += 16) {
-                float v[16];
-                tmem_ld16(lane_base + (uint32_t)c0, v);
+        for (int c0 = 0; c0 < N; c0 += 16) {
+            float v[16];
+            acc_ld16(sAcc, tid, c0, v);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int n = c0 + h * 8;
-                    if (n >= N) break;
-                    float o[8];
-                    const float4 b0 = *reinterpret_cast<const float4*>(bias + n), b1 = *reinterpret_cast<const float4*>(bias + n + 4);
-                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+            for (int h = 0; h < 2; ++h) {
+                const int n = c0 + h * 8;
+                if (n >= N) break;
+                float o[8];
+                const float4 b0 = *reinterpret_cast<const float4*>(bias + n), b1 = *reinterpret_cast<const float4*>(bias + n + 4);
+                const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) o[j] = v[h * 8 + j] + bb[j];
-                    if (RESID && row_ok) {
-                        float r[8];
-                        ld8<T>(resid + (m0 + tid) * N + n, r);
+                for (int j = 0; j < 8; ++j) o[j] = v[h * 8 + j] + bb[j];
+                if (RESID && row_ok) {
+                    float r[8];
+                    ld8<T>(resid + (m0 + tid) * N + n, r);
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] += r[j];
-                    }
-                    st8<T>(reinterpret_cast<T*>(stage + tid * pitch16 + ((c0 >> 3) + h)), o);
+                    for (int j = 0; j < 8; ++j) o[j] += r[j];
                 }
+                st8<T>(reinterpret_cast<T*>(stage + tid * pitch16 + ((c0 >> 3) + h)), o);
             }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (!s_abort)
-            for (int idx = tid; idx < rows_valid * nch; idx += 128) {
-                const int r = fdiv_small(idx, inv_nch), j = idx - r * nch;
-                *reinterpret_cast<uint4*>(out + (m0 + r) * N + j * 8) = stage[r * pitch16 + j];
-            }
+        for (int idx = tid; idx < rows_valid * nch; idx += 128) {
+            const int r = fdiv_small(idx, inv_nch), j = idx - r * nch;
+            *reinterpret_cast<uint4*>(out + (m0 + r) * N + j * 8) = stage[r * pitch16 + j];
+        }
     };
 
     const int ntiles = t_end - t_begin;
+    WgAcc<4> acc;
     for (int it = 0; it < ntiles; ++it) {
         const int t = t_begin + it, buf = it & 1;
         asm volatile("cp.async.wait_group 0;" ::: "memory");            // A(t) has landed (this thread's part)
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();                                                // ... everyone's; the store loop of tile t-2 is done with `stage`
-        if (tid == 0 && !s_abort) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int krem = min(BK, K - kb * BK);
-                const int ksteps = (krem + 15) >> 4;
-                const uint64_t ad = make_desc(sA + buf * a_bytes + kb * A_STAGE_BYTES), bd = make_desc(sW + (uint32_t)kb * umma_n * 128);
-                for (int k = 0; k < ksteps; ++k)
-                    umma_f16(tmem_d + (uint32_t)(buf * umma_n), ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-            }
-            umma_commit(&mbar[buf]);
+        __syncthreads();                                                // ... everyone's; the store loop of tile t-1 is done with `stage`
+        wg_fence();
+        for (int kb = 0; kb < nkb; ++kb) {
+            const int krem = min(BK, K - kb * BK);
+            wg_mma_tile<BF16, 4>(acc, sA + buf * a_bytes + kb * A_STAGE_BYTES, sW + (uint32_t)kb * umma_n * 128, (krem + 15) >> 4, nch16, kb ? 1u : 0u);
         }
-        if (it >= 1) {
-            // tile t-1: its MMA has finished (mbar) -> its A buffer is free for tile t+1, its accumulator is ready
-            if (!mbar_wait(&mbar[buf ^ 1], (uint32_t)((it - 1) >> 1) & 1u, tflag)) s_abort = 1;
-        }
+        wg_commit();
+        // A buffer buf ^ 1 was read by the MMA of tile t-1, which has completed
         if (it + 1 < ntiles) fill_a(t + 1, buf ^ 1);
         asm volatile("cp.async.commit_group;" ::: "memory");
-        if (it >= 1) epilogue(t - 1, buf ^ 1, it - 1);
+        wg_wait<0>();
+        wg_acc_store<4>(acc, sAcc, nch16, tid);
+        __syncthreads();
+        epilogue(t);
     }
-    __syncthreads();            // the store loop of tile n-2 is done with `stage` (inside the loop the barrier at the top does this)
-    epilogue(t_end - 1, (ntiles - 1) & 1, ntiles - 1);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((uint32_t)tmem_cols) : "memory");
 }
 
 // Which gated projects pw_tc3 takes and how it walks them (host-side, tested without a GPU by tests/test_route_plans.py).
-struct Pw3Plan { int tiles_per_crop, tpc, groups, umma_n, tmem_cols; size_t smem; };
+struct Pw3Plan { int tiles_per_crop, tpc, groups, umma_n; size_t smem; };
 inline bool plan_pw_tc3(long long M, int K, int N, int hw, bool has_gate, Pw3Plan* pl) {
-    // K <= 64 (one K block): measured b01 (K = 32) 0.275 -> 0.170 ms, b02 (K = 96) unchanged, b03 / b04 (K = 144: three blocks,
-    // 96 KB of A buffers, two CTAs per SM) 1.7x SLOWER than pw_tc2
+    // K <= 64 (one K block): the larger K of blocks 2-4 need two or three A blocks per buffer and lose co-residency
     if (!has_gate || hw < 784 || (K & 7) || (N & 7) || K > 64 || N > 64 || M < 1 || M % hw) return false;
     const int crops = (int)(M / hw);
     pl->tiles_per_crop = (hw + BM - 1) / BM;
@@ -661,33 +652,30 @@ inline bool plan_pw_tc3(long long M, int K, int N, int hw, bool has_gate, Pw3Pla
     pl->groups = (pl->tiles_per_crop + pl->tpc - 1) / pl->tpc;
     if (pl->tpc < 3) return false;                                // nothing to pipeline
     pl->umma_n = (N + 15) & ~15;
-    pl->tmem_cols = 32;
-    while (pl->tmem_cols < 2 * pl->umma_n) pl->tmem_cols <<= 1;
     const int nkb = (K + BK - 1) / BK;
     const size_t w_bytes = ((size_t)nkb * pl->umma_n * 128 + 1023) & ~(size_t)1023;
-    pl->smem = w_bytes + 2 * (size_t)nkb * A_STAGE_BYTES + (((size_t)K * 4 + 15) & ~(size_t)15) + (size_t)BM * ((size_t)(N >> 3) | 1) * 16 + 1024;
+    pl->smem = w_bytes + 2 * (size_t)nkb * A_STAGE_BYTES + (((size_t)K * 4 + 15) & ~(size_t)15) + acc_tile_bytes(pl->umma_n) + (size_t)BM * ((size_t)(N >> 3) | 1) * 16 + 1024;
     return pl->smem <= 200 * 1024;
 }
 
 // 0 = launched; 1 = shape not covered (caller falls back to pw_tc2)
 template <typename T>
-int launch_pw_tc3(cudaStream_t stream, int* tflag, const T* A, const void* Wt16, const float* bias, const float* gate, const T* resid, T* out,
+int launch_pw_tc3(cudaStream_t stream, const T* A, const void* Wt16, const float* bias, const float* gate, const T* resid, T* out,
                   long long M, int K, int N, int hw) {
     Pw3Plan pl{};
     if (sizeof(T) != 2 || !plan_pw_tc3(M, K, N, hw, gate != nullptr, &pl)) return 1;
     const int crops = (int)(M / hw);
-    const int tiles_per_crop = pl.tiles_per_crop, tpc = pl.tpc, groups = pl.groups, umma_n = pl.umma_n, tmem_cols = pl.tmem_cols;
+    const int tiles_per_crop = pl.tiles_per_crop, tpc = pl.tpc, groups = pl.groups, umma_n = pl.umma_n;
     const size_t smem = pl.smem;
-    const uint32_t idesc = make_idesc(std::is_same<T, __nv_bfloat16>::value, umma_n);
     const T* W = reinterpret_cast<const T*>(Wt16);
     if (resid) {
         auto kfn = pw_tc3_kernel<T, true>;
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;
-        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, umma_n, tmem_cols, tiles_per_crop, tpc, groups, idesc, tflag);
+        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, umma_n, tiles_per_crop, tpc, groups);
     } else {
         auto kfn = pw_tc3_kernel<T, false>;
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;
-        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, umma_n, tmem_cols, tiles_per_crop, tpc, groups, idesc, tflag);
+        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, umma_n, tiles_per_crop, tpc, groups);
     }
     return 0;
 }

@@ -2,16 +2,16 @@
 //
 //   out[m, n] = act( bias[n] + sum_k (A[m,k] * gate[m/hw, k]) * W[k,n] ) (+ resid[m,n])      A, out, resid: fp32 in HBM
 //
-// tcgen05 has no fp32 x fp32 MMA; kind::tf32 keeps 10 mantissa bits (0.034 deg on the Sample crops, SURVEY.md 8c - over the
+// The tensor core has no fp32 x fp32 MMA; tf32 keeps 10 mantissa bits (0.034 deg on the Sample crops, SURVEY.md 8c - over the
 // 0.01 deg target).  Here every fp32 operand is split into two bf16 terms, x = hi + lo with hi = bf16(x), lo = bf16(x - hi)
-// (|x - hi - lo| <= 2^-18 |x|), and the product is three bf16 MMAs accumulated in fp32 in TMEM:
+// (|x - hi - lo| <= 2^-18 |x|), and the product is three bf16 MMAs accumulated in fp32 registers:
 //
 //   A*W ~= Ahi*Whi + Ahi*Wlo + Alo*Whi          (the dropped Alo*Wlo term and the split residuals are ~2^-17 relative)
 //
 // The weights are split once at load time (two K-major [N][K] bf16 arrays); activations are split on the fly by the threads
 // that stage them: global fp32 -> registers -> (x SE gate, in fp32) -> hi / lo -> two SWIZZLE_128B tiles in shared memory.
 // One 128-thread CTA owns a 128-pixel x n_tile tile; K runs in blocks of 64 channels through a 2-stage ring whose stages are
-// recycled by tcgen05.commit -> mbarrier; the epilogue is fp32 throughout (precise expf swish, as the CUDA-core parity kernels).
+// recycled once wgmma.wait_group reports the block that read them complete; the epilogue is fp32 throughout (precise expf swish, as the CUDA-core parity kernels).
 #pragma once
 #include "kernels_tc.cuh"
 
@@ -37,13 +37,10 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
                                                       const __nv_bfloat16* __restrict__ Wlo, const float* __restrict__ bias,
                                                       const float* __restrict__ gate, const float* __restrict__ resid,
                                                       float* __restrict__ out, int M, int K, int N, int hw,
-                                                      int n_tile, int umma_n, int tmem_cols, uint32_t idesc, int* tflag) {
+                                                      int n_tile, int umma_n) {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t mbar[2];
-    __shared__ uint32_t s_tmem_base;
-    __shared__ int s_abort;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t w_bytes = (uint32_t)umma_n * 128;
     const uint32_t stage_bytes = 2 * A_STAGE_BYTES + 2 * w_bytes;      // A hi | A lo | W hi | W lo
@@ -52,20 +49,8 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
     const int rows_valid = min(BM, M - m0), n_valid = min(n_tile, N - n0);
     const int nkb = (K + BK - 1) / BK, kchunks = K >> 3;
 
-    if (tid == 0) {
-        mbar_init(&mbar[0], 1);
-        mbar_init(&mbar[1], 1);
-        s_abort = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"((uint32_t)tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = s_tmem_base;
+    WgAcc<8> acc;
+    const int nch16 = umma_n >> 4;
 
     // this thread stages chunk c (8 channels) of rows r0 + 16 i: its gate row index per row is fixed for the whole K loop
     const int c = tid & 7, r0 = tid >> 3;
@@ -73,7 +58,10 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
 
     for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb & 1;
-        if (kb >= 2 && !mbar_wait(&mbar[s], ((kb >> 1) - 1) & 1, tflag)) s_abort = 1;      // the MMAs of block kb-2 are done with this stage
+        if (kb >= 2) {              // the MMAs of block kb-2 are done with this stage (in every thread)
+            wg_wait<1>();
+            __syncthreads();
+        }
         const uint32_t a_hi = smem0 + s * stage_bytes, a_lo = a_hi + A_STAGE_BYTES, w_hi = a_lo + A_STAGE_BYTES, w_lo = w_hi + w_bytes;
         const int kc = kb * 8 + c;                        // global 16-byte (8-channel) chunk of this thread
         const bool cvalid = kc < kchunks;
@@ -105,35 +93,28 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
             sts128_(w_lo + swz + i * 2048, lo);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (tid == 0 && !s_abort) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int krem = min(BK, K - kb * BK), ksteps = (krem + 15) >> 4;
-            const uint64_t ah = make_desc(a_hi), al = make_desc(a_lo), wh = make_desc(w_hi), wl = make_desc(w_lo);
-            for (int k = 0; k < ksteps; ++k) {
-                umma_f16(tmem_d, ah + (uint64_t)(k * 2), wh + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-                umma_f16(tmem_d, ah + (uint64_t)(k * 2), wl + (uint64_t)(k * 2), idesc, 1u);
-                umma_f16(tmem_d, al + (uint64_t)(k * 2), wh + (uint64_t)(k * 2), idesc, 1u);
-            }
-            umma_commit(&mbar[s]);
-        }
+        const int ksteps = (min(BK, K - kb * BK) + 15) >> 4;
+        wg_fence();
+        wg_mma_tile<true, 8>(acc, a_hi, w_hi, ksteps, nch16, kb ? 1u : 0u);
+        wg_mma_tile<true, 8>(acc, a_hi, w_lo, ksteps, nch16, 1u);
+        wg_mma_tile<true, 8>(acc, a_lo, w_hi, ksteps, nch16, 1u);
+        wg_commit();
     }
-    {
-        const int last = nkb - 1;
-        if (!mbar_wait(&mbar[last & 1], (last >> 1) & 1, tflag)) s_abort = 1;
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    wg_wait<0>();
+    __syncthreads();
+    // the operand stages are free: accumulators -> shared accumulator tile
+    const uint32_t sAcc = smem0;
+    wg_acc_store<8>(acc, sAcc, nch16, tid);
     __syncthreads();
 
     // ---- epilogue, fp32: thread == pixel row; + shift, swish (precise), + residual; 16-byte stores
     const bool row_ok = tid < rows_valid;
     const long long m = (long long)m0 + tid;
-    if (!s_abort) {
-        const uint32_t lane_base = tmem_d + ((uint32_t)(warp * 32) << 16);
+    {
         for (int c0 = 0; c0 < n_valid; c0 += 16) {
             float v[16];
-            tmem_ld16(lane_base + (uint32_t)c0, v);
+            acc_ld16(sAcc, tid, c0, v);
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int n = n0 + c0 + q * 4;
@@ -154,14 +135,10 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((uint32_t)tmem_cols) : "memory");
 }
 
 // 0 = launched, > 0 = shape unsupported (caller falls back to the CUDA-core kernel), < 0 = error
-inline int launch_pw_tc32(cudaStream_t stream, int* tflag, const float* A, const void* Whi, const void* Wlo, const float* bias, const float* gate,
+inline int launch_pw_tc32(cudaStream_t stream, const float* A, const void* Whi, const void* Wlo, const float* bias, const float* gate,
                           const float* resid, float* out, long long M, int K, int N, int hw, bool swish) {
     if ((K & 7) || (N & 7) || M > 0x7fffffffLL || !Whi || !Wlo) return 1;
     int n_tile = N;
@@ -174,17 +151,14 @@ inline int launch_pw_tc32(cudaStream_t stream, int* tflag, const float* A, const
         }
     }
     const int umma_n = (n_tile + 15) & ~15;
-    int tmem_cols = 32;
-    while (tmem_cols < umma_n) tmem_cols <<= 1;
-    const uint32_t idesc = make_idesc(true, umma_n);
-    const size_t smem = 2 * (2 * (size_t)A_STAGE_BYTES + 2 * (size_t)umma_n * 128) + 1024;
+    const size_t smem = std::max((size_t)2 * (2 * A_STAGE_BYTES + 2 * (size_t)umma_n * 128), (size_t)acc_tile_bytes(umma_n)) + 1024;
     dim3 grid((unsigned)((N + n_tile - 1) / n_tile), (unsigned)((M + BM - 1) / BM));
     const __nv_bfloat16 *wh = reinterpret_cast<const __nv_bfloat16*>(Whi), *wl = reinterpret_cast<const __nv_bfloat16*>(Wlo);
 #define TC32(SW, GA, RE)                                                                                                   \
     do {                                                                                                                   \
         auto kfn = pw_tc32_kernel<SW, GA, RE>;                                                                             \
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;  \
-        kfn<<<grid, 128, smem, stream>>>(A, wh, wl, bias, gate, resid, out, (int)M, K, N, hw, n_tile, umma_n, tmem_cols, idesc, tflag); \
+        kfn<<<grid, 128, smem, stream>>>(A, wh, wl, bias, gate, resid, out, (int)M, K, N, hw, n_tile, umma_n); \
         return 0;                                                                                                          \
     } while (0)
     if (swish && !gate && !resid) TC32(true, false, false);

@@ -44,10 +44,10 @@ extern template int launch_dwse_spatial<__nv_bfloat16>(cudaStream_t, DwSeParams,
 }  // namespace fused
 namespace tc {
 #define WHENET_EXTERN_PW(T)                                                                                                         \
-    extern template int launch_pw_tc2<T>(cudaStream_t, int*, const T*, const void*, const float*, const float*, const T*, T*, long long, \
-                                         int, int, int, bool, int, int, int, bool, int);                                                 \
+    extern template int launch_pw_tc2<T>(cudaStream_t, const T*, const void*, const float*, const float*, const T*, T*, long long, \
+                                         int, int, int, bool, int, int, int, bool);                                                 \
     extern template int launch_k2<T>(cudaStream_t, const K2Params&, size_t, bool, bool, bool, int, bool);          \
-    extern template int launch_pw_tc3<T>(cudaStream_t, int*, const T*, const void*, const float*, const float*, const T*, T*, long long, int, int, int);
+    extern template int launch_pw_tc3<T>(cudaStream_t, const T*, const void*, const float*, const float*, const T*, T*, long long, int, int, int);
 WHENET_EXTERN_PW(__nv_bfloat16)
 WHENET_EXTERN_PW(__half)
 #undef WHENET_EXTERN_PW
@@ -146,13 +146,13 @@ struct whenet_ctx {
     int device = 0, max_batch = 0, precision = 0;
     int chunk = 0;          // crops per pass through the net
     int use_tc = 0;         // tensor-core kernels for the 1x1 convs
-    int* h_tflag = nullptr; // mbarrier-timeout flag: mapped pinned host memory, raised by any tcgen05 kernel of this context
+    int* h_tflag = nullptr; // mbarrier-timeout flag: mapped pinned host memory, raised by any pipelined tensor-core kernel of this context
     int* d_tflag = nullptr; // ... its device address (kernel parameter)
     int dw_variant = 1;     // 0 = one output per thread, 1 = register-blocked strips
     int pw_variant = 4;     // tensor-core 1x1 kernel: 2 = pw_tc2 (one tile per CTA, cp.async ring), 3 = K2 (persistent, TMA, warp-specialised),
                             // 4 = per layer (launch_pw)
     std::map<TmapKey, CUtensorMap> tmaps2;  // K2 tensor maps: activations by (K, M, pointer), weights by (-N, K, pointer)
-    int pw_stage_cap = 0, pw_smem_kb = 54, pw_min_ctas = 148;    // pw_tc2 ring: max stages (0 = up to 4) and per-CTA smem budget that trades depth for co-residency
+    int pw_stage_cap = 0, pw_smem_kb = 54, pw_min_ctas = 132;    // pw_tc2 ring: max stages (0 = up to 4) and per-CTA smem budget that trades depth for co-residency
     int stem_variant = 1;   // 0 = 4 threads / pixel straight from global, 1 = smem-tiled, weights in the constant bank
     whenet::StemParams stem_params{};
     bool async_host = false;    // set by whenet_forward_u8_async for the duration of the call
@@ -160,7 +160,7 @@ struct whenet_ctx {
     float* d_angles_slot[2] = {nullptr, nullptr};
     float* d_logits_slot[2] = {nullptr, nullptr};
     int host_chunk = 1 << 30;   // host inputs can run in passes of at most this many crops so the H2D of pass i+1 hides behind
-                                // pass i; measured on B200 (round 1): whole-batch passes win (45.3k vs 42.1k crops/s at 256)
+                                // pass i; default: whole-batch passes
     int cfg_epoch = 0;      // bumped by every set_option / plan change: part of the graph cache key
     int use_graph = 0;      // replay device-resident forwards from a captured CUDA graph (small-batch latency)
     std::vector<GraphEntry> graphs;
@@ -180,7 +180,7 @@ struct whenet_ctx {
     std::map<TmapKey, CUtensorMap> tmaps;   // input tensor maps of K1W by (block, crops, buffer)
     std::vector<CUtensorMap> tmap_w;        // weight tensor maps of K1W by block
   // k1_variant 3: persistent warp-specialised K1 for the blocks with several tiles per crop
-    int sm_count = 148;
+    int sm_count = 132;
     int k1w_trace_block = 0;   // debug: the K1W launch of this block records where its roles wait (whenet_debug_read_trace)
     long long* d_trace = nullptr;
     K1Plan dw1;                // block 1 (no expand): depthwise-only instance of K1
@@ -202,7 +202,7 @@ struct whenet_ctx {
     size_t ws_io = 0, ws_ex = 0, ws_dw = 0, ws_part = 0;   // per-crop element counts of the workspace buffers
     cudaStream_t aux_stream[4] = {nullptr, nullptr, nullptr, nullptr};   // multi-stream mode: batch parts run concurrently
     cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr}, ev_half[4] = {nullptr, nullptr, nullptr, nullptr};
-    int n_streams = 2;   // measured on B200: 67.1k vs 62.6k crops/s at 512 crops (late one-CTA-per-SM kernels share SMs with the other half)
+    int n_streams = 2;   // two half-batch streams: the late one-CTA-per-SM kernels share SMs with the other half
     void *bufA = nullptr, *bufB = nullptr, *bufE = nullptr, *bufD = nullptr;
     float *d_partial = nullptr, *d_gate = nullptr, *d_angles = nullptr, *d_logits = nullptr, *d_pooled = nullptr;
     int* d_se_counter = nullptr;   // per-crop tickets of the fused SE excite (zero between kernels)
@@ -211,9 +211,8 @@ struct whenet_ctx {
     int k1_split_ctas = 120;       // small batches: split a crop's chunks over CTAs until the K1 grid has this many (measured: at 256
                                    // crops per stream the late blocks run faster unsplit, with the SE tail, than split to 296)
     int se_tail = 1;               // K1 CTAs that hold whole crops (blocks 7-16 at large batch) compute the SE gate themselves
-    int se_fused = 0;              // K1's/K0's last CTA per crop computes the SE gate (no se_gate launch).  Measured on
-                                   // B200 (round 1): the fence + ticket tail costs more (+0.7 ms / 512 crops) than the 15
-                                   // small se_gate launches it saves (0.37 ms), so it is off by default.
+    int se_fused = 0;              // K1's/K0's last CTA per crop computes the SE gate (no se_gate launch); off by default: the
+                                   // fence + ticket tail serialises the last CTA of every crop
     void* d_in[2] = {nullptr, nullptr};
     void* h_stage = nullptr;            // pinned staging for PAGEABLE host inputs (upload_input)
     size_t h_stage_bytes = 0;
@@ -239,12 +238,12 @@ namespace {
 
 size_t esize(int precision) { return precision == WHENET_PRECISION_FP32 ? 4 : 2; }
 
-// The stream has been synchronised: did any tcgen05 kernel of this context give up on an mbarrier?  (plain host read of
+// The stream has been synchronised: did any pipelined tensor-core kernel of this context give up on an mbarrier?  (plain host read of
 // the mapped pinned flag; the flag is cleared so the context stays usable)
 int check_timeout(whenet_ctx* c) {
     if (c->h_tflag && *reinterpret_cast<volatile int*>(c->h_tflag)) {
         *reinterpret_cast<volatile int*>(c->h_tflag) = 0;
-        return fail(WHENET_ECUDA, "a tcgen05 kernel timed out waiting on an mbarrier (results invalid)");
+        return fail(WHENET_ECUDA, "a tensor-core kernel timed out waiting on an mbarrier (results invalid)");
     }
     return 0;
 }
@@ -476,12 +475,12 @@ int launch_pw(whenet_ctx* c, const char* name, const T* A, const float* W, const
         }
         if (c->use_tc && Wt16 && gate && hw >= 784 && c->pw3 && !out_half && !swish) {
             // gated projects of the large maps: several tiles of one crop per CTA (pw_tc3; same bits as pw_tc2's per-crop route)
-            int rc = whenet::tc::launch_pw_tc3<T>(c->stream, c->d_tflag, A, Wt16, bias, gate, resid, out, M, K, N, hw);
+            int rc = whenet::tc::launch_pw_tc3<T>(c->stream, A, Wt16, bias, gate, resid, out, M, K, N, hw);
             if (rc == 0) { CK(cudaGetLastError()); return 0; }
             if (rc < 0) return fail(WHENET_ECUDA, "pw_tc3 launch failed for %s (rc=%d)", name, rc);
         }
         if (c->use_tc && Wt16) {
-            int rc = whenet::tc::launch_pw_tc2<T>(c->stream, c->d_tflag, A, Wt16, bias, gate, resid, out, M, K, N, hw, swish, c->pw_stage_cap, c->pw_smem_kb, c->pw_min_ctas, out_half);
+            int rc = whenet::tc::launch_pw_tc2<T>(c->stream, A, Wt16, bias, gate, resid, out, M, K, N, hw, swish, c->pw_stage_cap, c->pw_smem_kb, c->pw_min_ctas, out_half);
             if (rc == 0) { CK(cudaGetLastError()); return 0; }
             if (rc < 0) return fail(WHENET_ECUDA, "tensor-core 1x1 launch failed for %s (rc=%d)", name, rc);
             // rc > 0: shape not supported by the tensor-core kernel -> CUDA-core kernel below
@@ -489,7 +488,7 @@ int launch_pw(whenet_ctx* c, const char* name, const T* A, const float* W, const
     }
     if constexpr (sizeof(T) == 4) {
         if (c->use_tc && Wt16 && c->split_lo_bytes) {
-            int rc = whenet::tc::launch_pw_tc32(c->stream, c->d_tflag, A, Wt16, (const char*)Wt16 + c->split_lo_bytes, bias, gate, resid, out, M, K, N, hw, swish);
+            int rc = whenet::tc::launch_pw_tc32(c->stream, A, Wt16, (const char*)Wt16 + c->split_lo_bytes, bias, gate, resid, out, M, K, N, hw, swish);
             if (rc == 0) { CK(cudaGetLastError()); return 0; }
             if (rc < 0) return fail(WHENET_ECUDA, "split-bf16 tensor-core 1x1 launch failed for %s (rc=%d)", name, rc);
         }
@@ -558,8 +557,8 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
         if constexpr (IN_U8 && std::is_same<T, __nv_bfloat16>::value) {
             if (c->stem_tc && c->use_tc && c->use_fused) {
                 // bf16 throughput mode, uint8 input: the stem as an im2col GEMM on the tensor core (kernels_stem_tc.cuh)
-                const int rc = stem_half ? whenet::launch_stem_tc<__half>(c->stream, (const uint8_t*)d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut, c->d_tflag, nb)
-                                         : whenet::launch_stem_tc<T>(c->stream, (const uint8_t*)d_in, cur, c->stem_params, c->lut, c->d_tflag, nb);
+                const int rc = stem_half ? whenet::launch_stem_tc<__half>(c->stream, (const uint8_t*)d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut, nb)
+                                         : whenet::launch_stem_tc<T>(c->stream, (const uint8_t*)d_in, cur, c->stem_params, c->lut, nb);
                 if (rc != 0) return fail(WHENET_ECUDA, "tensor-core stem launch failed (rc=%d)", rc);
                 stem_done = true;
             }
@@ -643,7 +642,7 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                 did_k1 = true;
             } else if (use_kd) {
               if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-                // late blocks: expand as a plain tcgen05 GEMM (fp16 E, L2-resident) + KD (depthwise + SE + gating)
+                // late blocks: expand as a plain tensor-core GEMM (fp16 E, L2-resident) + KD (depthwise + SE + gating)
                 snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
                 int rc = launch_pw<T>(c, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, E,
                                       (long long)nb * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, true, true);
@@ -1139,7 +1138,7 @@ int bind_packed(whenet_ctx* c, const float* arena, size_t n_f32, const uint16_t*
 extern "C" {
 
 const char* whenet_last_error(void) { return g_err; }
-const char* whenet_version(void) { return "whenet_b200 0.1 (sm_100a)"; }
+const char* whenet_version(void) { return "whenet_b200 0.1 (sm_90a)"; }
 
 int whenet_create(whenet_ctx** out, int device, int max_batch, int precision) {
     if (!out) return fail(WHENET_EINVAL, "out is NULL");
@@ -1152,8 +1151,8 @@ int whenet_create(whenet_ctx** out, int device, int max_batch, int precision) {
     CK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return fail(WHENET_ECUDA, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(WHENET_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     whenet_ctx* c = new whenet_ctx();
     c->device = device;
     c->max_batch = max_batch;
@@ -1558,9 +1557,9 @@ int debug_conv_impl(whenet_ctx* c, int use_tc, const float* A, const float* W, c
                 c->pw_variant = saved_v;
                 c->tmaps2.clear();
             } else if (use_tc == 5) {
-                rc = whenet::tc::launch_pw_tc3<T>(c->stream, c->d_tflag, dA, dWt, dB, dG, dR, dO, M, K, N, hw);
+                rc = whenet::tc::launch_pw_tc3<T>(c->stream, dA, dWt, dB, dG, dR, dO, M, K, N, hw);
             } else
-            rc = whenet::tc::launch_pw_tc2<T>(c->stream, c->d_tflag, dA, dWt, dB, dG, dR, dO, M, K, N, hw, swish != 0);
+            rc = whenet::tc::launch_pw_tc2<T>(c->stream, dA, dWt, dB, dG, dR, dO, M, K, N, hw, swish != 0);
         uint16_t* dS = nullptr;
         if constexpr (sizeof(T) == 4) {
             // fp32 parity mode on the tensor core: bf16 hi | lo split of the K-major weights, as whenet_load_weights builds it
@@ -1574,7 +1573,7 @@ int debug_conv_impl(whenet_ctx* c, int use_tc, const float* A, const float* W, c
             if (cudaMalloc(&dS, hs.size() * 2 + 256) == cudaSuccess) {
                 cudaMemcpyAsync(dS, hs.data(), hs.size() * 2, cudaMemcpyHostToDevice, c->stream);
                 cudaStreamSynchronize(c->stream);
-                rc = whenet::tc::launch_pw_tc32(c->stream, c->d_tflag, (const float*)dA, dS, dS + (size_t)N * K, dB, dG, (const float*)dR, (float*)dO, M, K, N, hw, swish != 0);
+                rc = whenet::tc::launch_pw_tc32(c->stream, (const float*)dA, dS, dS + (size_t)N * K, dB, dG, (const float*)dR, (float*)dO, M, K, N, hw, swish != 0);
                 cudaStreamSynchronize(c->stream);
                 cudaFree(dS);
             } else rc = -1;

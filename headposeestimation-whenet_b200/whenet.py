@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's ``whenet.py``: same class, same methods,
 same argument meaning and error behaviour - the arithmetic runs in
-``libwhenet_b200.so`` (hand-written sm_100a CUDA) instead of Keras/TensorFlow.
+``libwhenet_b200.so`` (hand-written sm_90a CUDA) instead of Keras/TensorFlow.
 
 Reference surface kept (SURVEY.md section 8b):
   ``WHENet(snapshot=None)``                      reference whenet.py:7-20
@@ -9,7 +9,7 @@ Reference surface kept (SURVEY.md section 8b):
   ``.idx_tensor`` / ``.idx_tensor_yaw``          reference whenet.py:17-20
   ``.get_angle(img)``                            reference whenet.py:22-34  -> (yaw, pitch, roll) float32 (N,)
 
-There is no CPU fallback: without the shared library or a B200 the constructor raises.
+There is no CPU fallback: without the shared library or an H100 the constructor raises.
 """
 from __future__ import annotations
 
@@ -65,7 +65,7 @@ class WHENetModel:
         return [logits[:, :120].copy(), logits[:, 120:186].copy(), logits[:, 186:].copy()]
 
     def summary(self, print_fn=print):
-        lines = ["WHENet (EfficientNet-B0 backbone, B200-native CUDA path, precision=%s)" % self._o.precision,
+        lines = ["WHENet (EfficientNet-B0 backbone, H100-native CUDA path, precision=%s)" % self._o.precision,
                  "%-22s %-18s %-10s" % ("Layer", "Output shape", "Params"), "=" * 54]
         total = 0
         def row(name, shape, params):
@@ -188,7 +188,7 @@ class WHENet:
         angles, _ = self._forward(x)
         return angles[:, 0].copy(), angles[:, 1].copy(), angles[:, 2].copy()
 
-    # ------------------------------------------------------------------ B200 extras (device-resident, async)
+    # ------------------------------------------------------------------ GPU extras (device-resident, async)
     def forward_device(self, crops_u8, angles_out, logits_out=None, n: Optional[int] = None):
         """Device-resident forward: ``crops_u8`` (n,224,224,3) uint8 CUDA tensor, ``angles_out`` (n,3)
         float32 CUDA tensor; asynchronous on the context's stream."""

@@ -1,5 +1,5 @@
 /*
- * whenet_b200.h - C ABI of the B200-native WHENet per-crop forward.
+ * whenet_b200.h - C ABI of the H100-native WHENet per-crop forward.
  *
  * The reference has no FFI of its own: its whole hot path is the Python class
  * in reference whenet.py (WHENet.__init__ :7-20, WHENet.get_angle :22-34,
@@ -135,7 +135,7 @@ int whenet_debug_enable_taps(whenet_ctx* ctx, int enable);
 /* Copy a tap to host; *n_elems receives its element count (call with out=NULL to query). */
 int whenet_debug_tap(whenet_ctx* ctx, const char* name, float* out, size_t cap_elems, size_t* n_elems);
 
-/* Run ONE 1x1 convolution through the kernel family chosen by use_tc (0 CUDA-core, 1 tcgen05):
+/* Run ONE 1x1 convolution through the kernel family chosen by use_tc (0 CUDA-core, 1 tensor core):
  * out[m,n] = act(bias[n] + sum_k A[m,k]*gate[m/hw,k]*W[k,n]) (+ resid[m,n]).  All arrays are host
  * float32 (converted to the context's storage type on the way in and back on the way out);
  * gate / resid may be NULL.  Returns WHENET_EINVAL when the family cannot run the shape. */
@@ -152,7 +152,7 @@ int whenet_debug_set_k1_plan(whenet_ctx* ctx, int block, int th, int tw, int r, 
  * (softmax of reference utils.py:7-11, expectation of whenet.py:31-33).  Synchronous. */
 int whenet_debug_decode(whenet_ctx* ctx, const float* logits_host, int n, float* angles_host);
 
-/* A device kernel raises the context's mbarrier-timeout flag (what a tcgen05 kernel does when a bounded wait expires):
+/* A device kernel raises the context's mbarrier-timeout flag (what a tensor-core kernel does when a bounded wait expires):
  * the next synchronising call (host-output forward, whenet_synchronize) must return WHENET_ECUDA. */
 int whenet_debug_raise_timeout(whenet_ctx* ctx);
 
@@ -178,8 +178,8 @@ int64_t whenet_launch_count(whenet_ctx* ctx);
  *   "chunk"          crops per pass through the network (default max_batch: one pass)
  *   "streams"        1..4 batch parts running concurrently on internal streams (default 2)
  *   "graph"          1: replay device-resident forwards from a captured CUDA graph (default 0)
- *   "tensor_cores"   16-bit modes: 0 = CUDA-core kernels for every 1x1 conv, 1 = tcgen05 (default 1).
- *                    fp32 mode: 0 = fp32 FMA kernels (default), 1 = the 1x1 convs on tcgen05 through the bf16 hi/lo split
+ *   "tensor_cores"   16-bit modes: 0 = CUDA-core kernels for every 1x1 conv, 1 = tensor core, wgmma (default 1).
+ *                    fp32 mode: 0 = fp32 FMA kernels (default), 1 = the 1x1 convs on the tensor core through the bf16 hi/lo split
  *                    (three MMAs per product, fp32 accumulation: 6e-4 deg from the float64 oracle on the golden crops)
  *   "fused"          1: K1 (expand + depthwise fused, expanded tensor in shared memory) for blocks 2..fused_max_block
  *   "k1_variant"     1 = K1 (one tile per CTA), 4 = K1W (weight-stationary persistent CTAs, TMA input tiles, warp roles)

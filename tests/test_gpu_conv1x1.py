@@ -120,10 +120,10 @@ def test_conv1x1_residual_without_gate(net, use_tc, K, N):
 @pytest.mark.parametrize("K,N,hw,res", [(96, 24, 3136, False), (240, 40, 784, True), (480, 80, 196, True), (1152, 192, 49, True),
                                         (1152, 320, 49, False), (320, 1280, 49, None)])
 def test_k2_persistent_many_tiles(net, K, N, hw, res):
-    """K2 with more tiles than CTAs (every CTA loops over several tiles: ring wrap-around, both TMEM accumulators, gate rows
+    """K2 with more tiles than CTAs (every CTA loops over several tiles: ring wrap-around, both MMA warpgroups, gate rows
     reloaded when a tile changes crop), resident and streamed weights, two n tiles (N = 320) and the swish head conv (N = 1280)."""
     rng = np.random.default_rng(K + N)
-    M = 2 * 148 * 128 + 3 * 128 + 77
+    M = 2 * 132 * 128 + 3 * 128 + 77
     A = _bf16_round(rng.standard_normal((M, K)))
     W = _bf16_round(rng.standard_normal((K, N)) / np.sqrt(K))
     bias = rng.standard_normal(N).astype(np.float32)

@@ -199,7 +199,7 @@ def test_fused_k1_plan_variants(prec, plan_set, oracle32, sample_crops, jitter_c
 
 
 def test_kd_route(oracle32, sample_crops, jitter_crops):
-    """Late blocks (7-16) in bf16: expand as a tcgen05 GEMM writing fp16 E + KD (depthwise + squeeze-excite + gating in one
+    """Late blocks (7-16) in bf16: expand as a tensor-core GEMM writing fp16 E + KD (depthwise + squeeze-excite + gating in one
     kernel, kernels_dwse.cuh).  Depthwise outputs, gates and block outputs against the oracle; agreement with the K1 route
     (same arithmetic up to the rounding of the expand accumulators); bitwise equality of the chunk-split route (small
     batches: several CTAs per crop, gate from se_gate_kernel, gated project conv) and the one-CTA-per-crop route (gate and
@@ -270,7 +270,7 @@ def test_pageable_input_staging(sample_crops, jitter_crops):
 
 
 def test_stem_on_tensor_core_option(oracle32, sample_crops, jitter_crops):
-    """Option stem_tc=1 (bf16, uint8 input): the stem as an im2col GEMM on tcgen05 - table lookups build the [hi | lo] bf16
+    """Option stem_tc=1 (bf16, uint8 input): the stem as an im2col GEMM on the tensor core - table lookups build the [hi | lo] bf16
     operand rows in shared memory, TF-SAME padding by masking the taps of the missing row / column 224.  The stem output must
     stay within the rounding of its bf16 weights of the oracle and the angles within the bf16 bound."""
     import whenet_b200

@@ -35,7 +35,7 @@ def bench_ref(port, bench_crops):
 
 @pytest.mark.parametrize("prec,tol", [("fp32", 0.01), ("bf16", 0.6), ("fp16", 0.08)])
 def test_batch512_random_uint8_vs_cpu_port(prec, tol, bench_crops, bench_ref):
-    """configs[2]: one 512-crop call in the default configuration (two half-batch streams, fused tcgen05 kernels)."""
+    """configs[2]: one 512-crop call in the default configuration (two half-batch streams, fused tensor-core kernels)."""
     import whenet_b200
     m = whenet_b200.WHENet(SNAP, device=0, precision=prec, max_batch=512)
     got = np.stack(m.get_angle(bench_crops), axis=1)
@@ -211,7 +211,7 @@ def test_packed_artefact_round_trip(prec, tmp_path, sample_crops, jitter_crops):
 
 
 def test_fp32_tensor_core_parity_mode(oracle64, oracle32, sample_crops, jitter_crops, golden):
-    """fp32 storage, 1x1 convolutions on tcgen05 through the bf16 hi/lo split (3 MMAs per product): the north_star tolerance
+    """fp32 storage, 1x1 convolutions on the tensor core through the bf16 hi/lo split (3 MMAs per product): the north_star tolerance
     (0.01 deg vs the float64 oracle) on tensor cores, every block boundary within 2e-4 relative of the float32 oracle,
     and agreement with the CUDA-core fp32 kernels far below that."""
     import whenet_b200

@@ -8,15 +8,15 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXE = os.path.join(ROOT, "build_tmp", "k1_plan_dump")
 LINE = re.compile(r"b(\d+)\s+(\d+)->\s*(\d+) k(\d) s(\d) cin\s*(\d+) cexp\s*(\d+) :\s*(\d+)x(\d+)\s+r(\d) cc(\d+)\s+nt(\d+) nb(\d)\s+mtiles (\d) "
-                  r"rows_alloc\s+(\d+) tmem\s+(\d+) chunks\s+(\d+) PY\s+(\d+) PYc\s+(\d+) smem\s+(\d+) \(A\s+(\d+) W\s+(\d+) C\s+(\d+) E\s+(\d+)\) (\d)/SM")
-KEYS = "idx hin ho k s cin cexp th tw r cc nt nb mtiles rows_alloc tmem chunks PY PYc smem A W C E per_sm".split()
+                  r"rows_alloc\s+(\d+) chunks\s+(\d+) PY\s+(\d+) PYc\s+(\d+) smem\s+(\d+) \(A\s+(\d+) W\s+(\d+) C\s+(\d+) E\s+(\d+)\) (\d)/SM")
+KEYS = "idx hin ho k s cin cexp th tw r cc nt nb mtiles rows_alloc chunks PY PYc smem A W C E per_sm".split()
 
 
 @pytest.fixture(scope="module")
 def dump():
     os.makedirs(os.path.dirname(EXE), exist_ok=True)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    r = subprocess.run([nvcc, "-std=c++17", "-arch=sm_100a", "-o", EXE, os.path.join(ROOT, "tools", "k1_plan_dump.cu")],
+    r = subprocess.run([nvcc, "-std=c++17", "-arch=sm_90a", "-o", EXE, os.path.join(ROOT, "tools", "k1_plan_dump.cu")],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
 
@@ -39,11 +39,11 @@ def test_every_block_has_a_plan_that_fits(dump):
     for r in rows:
         assert r["smem"] <= 227 * 1024 - 256
         assert r["cexp"] % r["cc"] == 0 and r["cc"] % 16 == 0
-        assert r["mtiles"] * r["cc"] <= r["tmem"] <= 512 and r["tmem"] & (r["tmem"] - 1) == 0
+        assert r["mtiles"] <= 3 and r["cc"] <= 128                  # a 64 x cc accumulator half lives in one warpgroup's registers
         assert r["rows_alloc"] % 8 == 0 and r["rows_alloc"] <= r["mtiles"] * 128
         assert r["PY"] == r["PYc"] * r["nb"] and r["PY"] * (r["cc"] // 4) <= r["nt"]
         assert r["nb"] * r["cc"] <= r["nt"]                         # one thread per (crop, channel) in the squeeze reduction
-        two = r["nt"] == 256 and r["smem"] <= 115000 and r["tmem"] <= 256
+        two = r["nt"] == 256 and r["smem"] <= 115000
         assert r["per_sm"] == (2 if two else 1)
     by = {r["idx"]: r for r in rows}
     # the GEMM rows are the halo pixels inside the image: 14x14 inputs with a 5x5 window need 196 rows, not 18*18

@@ -4,9 +4,7 @@ import os
 import numpy as np
 import pytest
 
-from conftest import SNAP
-
-REF_H5 = "/root/reference/WHENet.h5"
+from conftest import GOLD, SNAP
 
 
 def test_npz_inventory():
@@ -73,16 +71,28 @@ def test_random_weights_cover_everything():
     assert len(w) == 315
 
 
-@pytest.mark.skipif(not os.path.exists(REF_H5), reason="reference artefact only exists in the build container")
-def test_h5_reader_matches_npz_bit_for_bit():
+def test_h5_reader_matches_npz_bit_for_bit(tmp_path):
+    """h5lite on the reference's WHENet.h5 layout: tests/golden/whenet_h5_shrunk.h5.gz is that file with every metadata byte
+    kept and large tensors thinned to their first and last 128 values (tools/make_h5_fixture.py).  Layer order, file
+    attributes, every tensor's name / shape / dtype and every kept value must match the committed npz bit for bit."""
+    import gzip
     from whenet_b200 import h5lite
-    names, w, meta = h5lite.read_keras_weights(REF_H5)
+    path = os.path.join(tmp_path, "WHENet.h5")
+    with gzip.open(os.path.join(GOLD, "whenet_h5_shrunk.h5.gz"), "rb") as src, open(path, "wb") as dst:
+        dst.write(src.read())
+    names, w, meta = h5lite.read_keras_weights(path)
     z = np.load(SNAP)
     assert names == [str(s) for s in z["__layer_names__"]]
     assert meta == {"backend": "tensorflow", "keras_version": "2.1.6"}
-    assert len(w) == 315
+    assert len(w) == 315 and sorted(w) == sorted(k for k in z.files if not k.startswith("__"))
     for k, v in w.items():
-        assert v.dtype == np.float32 and np.array_equal(v, z[k]), k
+        ref = z[k]
+        assert v.dtype == np.float32 and v.shape == ref.shape, k
+        a, b = v.reshape(-1).view(np.uint32), ref.reshape(-1).view(np.uint32)
+        if a.size <= 512:
+            assert np.array_equal(a, b), k
+        else:
+            assert np.array_equal(a[:128], b[:128]) and np.array_equal(a[-128:], b[-128:]), k
 
 
 def test_h5_reader_rejects_garbage(tmp_path):

@@ -1,6 +1,6 @@
 // Host-only dump of the round-2 route planners (no GPU): K2 (persistent 1x1 conv) plans of the late expands / projects / head conv,
 // KD chunk widths, thread counts and shared memory, pw_tc3's tile walk of the early gated projects.
-//   nvcc -std=c++17 -arch=sm_100a -o build_tmp/route_plan_dump tools/route_plan_dump.cu && build_tmp/route_plan_dump [crops]
+//   nvcc -std=c++17 -arch=sm_90a -o build_tmp/route_plan_dump tools/route_plan_dump.cu && build_tmp/route_plan_dump [crops]
 #include <cstdio>
 #include <cstdlib>
 #include "../headposeestimation-whenet_b200/csrc/kernels_simt.cuh"
@@ -21,8 +21,8 @@ static void k2_line(const char* what, int idx, long long M, int K, int N, int hw
     tc::K2Params p{};
     size_t smem = 0;
     if (!tc::plan_k2(M, K, N, hw, gate, true, &p, &smem)) { printf("  k2 %s b%02d: no plan\n", what, idx); return; }
-    printf("  k2 %s b%02d M %lld K %d N %d gate %d : n_tile %d n_tiles %d tiles %d nkb %d stages %d resident %d tmem %d smem %zu\n", what, idx, M, K, N,
-           (int)gate, p.n_tile, p.n_tiles, p.tiles, p.nkb, p.stages, p.w_resident, p.tmem_cols, smem);
+    printf("  k2 %s b%02d M %lld K %d N %d gate %d : n_tile %d n_tiles %d tiles %d nkb %d stages %d resident %d smem %zu\n", what, idx, M, K, N,
+           (int)gate, p.n_tile, p.n_tiles, p.tiles, p.nkb, p.stages, p.w_resident, smem);
 }
 int main(int argc, char** argv) {
     const int crops = argc > 1 ? atoi(argv[1]) : 256;
@@ -41,7 +41,7 @@ int main(int argc, char** argv) {
             if (b.idx == 1) kd_line<3, 1, 14, 32>(b);
             tc::Pw3Plan pl{};
             const bool ok = tc::plan_pw_tc3((long long)crops * b.ho * b.ho, b.cexp, b.cout, b.ho * b.ho, true, &pl);
-            if (ok) printf("  pw3 b%02d tiles_per_crop %d tpc %d groups %d umma_n %d tmem %d smem %zu\n", b.idx, pl.tiles_per_crop, pl.tpc, pl.groups, pl.umma_n, pl.tmem_cols, pl.smem);
+            if (ok) printf("  pw3 b%02d tiles_per_crop %d tpc %d groups %d umma_n %d smem %zu\n", b.idx, pl.tiles_per_crop, pl.tpc, pl.groups, pl.umma_n, pl.smem);
             else printf("  pw3 b%02d: not taken\n", b.idx);
         }
     }
