@@ -286,6 +286,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
     __syncthreads();
     constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     const int nch16 = CC >> 4;
+    constexpr int kMaxPieces = CCT ? CCT / 16 : 8;        // 16-column pieces of the expand tile (at most 128 columns)
 
     for (int ch = ch_begin; ch < ch_end; ++ch) {
         const int buf = ch & 1;
@@ -294,10 +295,18 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
         //      the GEMM rows go round-robin over the warp groups; halves past the last GEMM row are skipped.
         if (!NOEXP) {
             for (int u = grp; u * 64 < rows_gemm; u += NG) {
-                float d[8][8];
-                tc::wg_fence();
-                tc::wg_mma_m64<BF16, 8>(d, sA + (uint32_t)u * 64 * 128, a_kb_stride, sW + buf * p.smem_W, (uint32_t)CC * 128, p.cpr >> 1, nch16);
-                tc::wg_commit();
+                // fragment register 8 jj + 4 i + e: piece jj of the m64nCC fragment
+                float d[8 * kMaxPieces];
+                if constexpr (CCT != 0) {
+                    tc::wg_mma_m64<BF16, CCT>(d, sA + (uint32_t)u * 64 * 128, a_kb_stride, sW + buf * p.smem_W, (uint32_t)CC * 128, p.cpr >> 1);
+                } else {
+                    // chunk width chosen at run time: one m64n16 sequence per 16-column piece
+#pragma unroll
+                    for (int jj = 0; jj < kMaxPieces; ++jj)
+                        if (jj < nch16)
+                            tc::wg_mma_m64<BF16, 16>(*reinterpret_cast<float(*)[8]>(d + 8 * jj), sA + (uint32_t)u * 64 * 128, a_kb_stride,
+                                                     sW + buf * p.smem_W + (uint32_t)jj * 2048u, (uint32_t)CC * 128, p.cpr >> 1);
+                }
                 tc::wg_wait<0>();
                 const int r_lo = u * 64 + 16 * wq + (lane >> 2), cq = 2 * (lane & 3);
 #pragma unroll
@@ -306,12 +315,12 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
                     if (r < rows_gemm) {
                         const uint32_t er = e_row_of(r);
 #pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) {
+                        for (int jj = 0; jj < kMaxPieces; ++jj) {
                             if (jj < nch16) {
 #pragma unroll
                                 for (int i = 0; i < 2; ++i) {
                                     // E is fp16 whatever the storage type: 3 more mantissa bits than bf16 and HFMA2-ready
-                                    const uint32_t v = pack2<__half>(swish_from_half(d[jj][4 * i + 2 * hr]), swish_from_half(d[jj][4 * i + 2 * hr + 1]));
+                                    const uint32_t v = pack2<__half>(swish_from_half(d[8 * jj + 4 * i + 2 * hr]), swish_from_half(d[8 * jj + 4 * i + 2 * hr + 1]));
                                     asm volatile("st.shared.b32 [%0], %1;" ::"r"(er + (uint32_t)(16 * jj + 8 * i + cq) * 2u), "r"(v) : "memory");
                                 }
                             }

@@ -291,11 +291,9 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
                 // (64-row half, 16-column unit) pieces f = grp, grp + NG, ...
                 for (int f = grp; f < halves * units; f += NG) {
                     const int hh = f / units, u = f - hh * units;
-                    float d[1][8];
+                    float d[8];
                     long long tq = tr ? clock64() : 0;
-                    tc::wg_fence();
-                    tc::wg_mma_m64<BF16, 1>(d, a0 + (uint32_t)hh * 64 * 128, (uint32_t)p.rows_alloc * 128, sW + (uint32_t)u * 2048, (uint32_t)CC * 128, p.ksteps, 1);
-                    tc::wg_commit();
+                    tc::wg_mma_m64<BF16, 16>(d, a0 + (uint32_t)hh * 64 * 128, (uint32_t)p.rows_alloc * 128, sW + (uint32_t)u * 2048, (uint32_t)CC * 128, p.ksteps);
                     tc::wg_wait<0>();
                     if (tr) tw2 += clock64() - tq;
                     tq = tr ? clock64() : 0;
@@ -315,7 +313,7 @@ __global__ void __maxnreg__(80) k1w_kernel(const __grid_constant__ K1WParams p) 
                             const int c = u * 16 + 8 * i + 2 * (lane & 3);
                             float2 sh;
                             asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(sh.x), "=f"(sh.y) : "r"(sC + (uint32_t)c * 4u));
-                            const float2 h = k1w::swish2_from_half(k1w::fadd2(make_float2(d[0][4 * i + 2 * e2], d[0][4 * i + 2 * e2 + 1]), sh));
+                            const float2 h = k1w::swish2_from_half(k1w::fadd2(make_float2(d[4 * i + 2 * e2], d[4 * i + 2 * e2 + 1]), sh));
                             const uint32_t v = img ? pack2<__half>(h.x, h.y) : 0u;
                             asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst + (uint32_t)c * 2u), "r"(v) : "memory");
                         }

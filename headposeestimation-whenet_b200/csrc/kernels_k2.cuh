@@ -8,7 +8,8 @@
 //
 //   warp 0            TMA producer   A[128 x 64] (+ W[n_tile x 64] when the weights are streamed) per K block -> ring
 //   warps 4-7, 8-11   MMA + epilogue two warpgroups (group 0: this CTA's even tiles, group 1: the odd ones): wgmma over the ring
-//                                    stages of the tile (each stage handed back to the producer once its MMAs are complete;
+//                                    stages of the tile (full-width m64nNk16, one commit group per K block, two blocks in
+//                                    flight; each stage handed back to the producer once its MMAs are complete;
 //                                    the groups take the ring in turns, tile by tile, so that no group waits on a ring slot
 //                                    more than one phase ahead of the producer - parity waits cannot tell phases two apart),
 //                                    then registers -> +bias (-> swish) (+residual) -> 16-bit -> global, while the other group
@@ -51,7 +52,8 @@ struct alignas(64) K2Params {
 constexpr int kK2Threads = 512;
 constexpr int kK2MaxN = 64;       // accumulator registers per MMA thread = n_tile (128 rows x n_tile over one warpgroup)
 
-template <typename T, bool SWISH, bool GATE, bool RESID, bool OUT_H = false>     // OUT_H: fp16 result whatever T is (expand conv feeding KD)
+// OUT_H: fp16 result whatever T is (expand conv feeding KD); NT = p.n_tile (16, 32, 48 or 64): the MMA width
+template <typename T, bool SWISH, bool GATE, bool RESID, bool OUT_H, int NT>
 __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant__ K2Params p) {
     using namespace whenet::fused;
     extern __shared__ uint8_t smem_raw[];
@@ -119,32 +121,39 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
         const int wt = tid & 127;
         const T* resid = reinterpret_cast<const T*>(p.resid);
         T* out = reinterpret_cast<T*>(p.out);
-        const int nch16 = p.n_tile >> 4;
         if (p.w_resident) k1w::wait(b_w, 0, s_abort, p.tflag);
         for (int tile = first + grp * step, k = grp; tile < p.tiles; tile += 2 * step, k += 2) {
             const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
-            WgAcc<kK2MaxN / 16> acc;
+            WgAcc<NT> acc;
             if (k > 0) k1w::wait(b_turn + 8 * grp, (uint32_t)((k - 1) >> 1) & 1u, s_abort, p.tflag);    // the other group is done with tile k-1
+            // one wgmma group per K block, up to two in flight: once block kb is issued, wait for block kb-1's group and hand
+            // ITS slot back to the producer, so the MMAs of block kb-1 are still running while block kb is issued
+            const int g0 = k * p.nkb;                            // ring slots are filled in tile order
             for (int kb = 0; kb < p.nkb; ++kb) {
-                const int g = k * p.nkb + kb;                    // ring slots are filled in tile order
+                const int g = g0 + kb;
                 const int s = g % p.stages;
                 const uint32_t par = (uint32_t)(g / p.stages) & 1u;
                 k1w::wait((GATE ? b_ready : b_full) + 8 * s, par, s_abort, p.tflag);
                 const uint32_t a_st = sRing + (uint32_t)s * stage_bytes;
-                const uint32_t w_st = p.w_resident ? sW + (uint32_t)kb * p.n_tile * 128 : a_st + p.a_stage;
-                wg_fence();
-                wg_mma_tile<BF16, kK2MaxN / 16>(acc, a_st, w_st, kb == p.nkb - 1 ? p.ksteps_last : 4, nch16, kb ? 1u : 0u);
-                wg_commit();
-                wg_wait<0>();
-                asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");      // the whole warpgroup's MMAs are done with the stage
-                if (wt == 0) k1w::arrive(b_empty + 8 * s);
+                const uint32_t w_st = p.w_resident ? sW + (uint32_t)kb * NT * 128 : a_st + p.a_stage;
+                wg_mma_tile<BF16, NT>(acc, a_st, w_st, kb == p.nkb - 1 ? p.ksteps_last : 4, kb ? 1u : 0u);     // one commit group
+                if (kb > 0) {
+                    wg_wait<1>();
+                    asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");  // the whole warpgroup's MMAs are done with slot g-1
+                    if (wt == 0) k1w::arrive(b_empty + 8 * ((g - 1) % p.stages));
+                }
             }
-            if (wt == 0) k1w::arrive(b_turn + 8 * (grp ^ 1));
+            wg_wait<0>();
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");
+            if (wt == 0) {
+                k1w::arrive(b_empty + 8 * ((g0 + p.nkb - 1) % p.stages));
+                k1w::arrive(b_turn + 8 * (grp ^ 1));
+            }
             if (*s_abort) continue;
-            // fragment -> output: register 4i + e of piece j = row 16 wq + lane/4 (+8 for e >= 2) of row half h,
-            // columns 16 j + 8 i + 2 (lane % 4) + {0, 1}
-            const int n0 = nt * p.n_tile;
-            const int n_valid = min(p.n_tile, p.N - n0);
+            // fragment -> output: register 4i + e = row 16 wq + lane/4 (+8 for e >= 2) of row half h,
+            // columns 8 i + 2 (lane % 4) + {0, 1}
+            const int n0 = nt * NT;
+            const int n_valid = min(NT, p.N - n0);
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -152,25 +161,23 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
                     const long long m = (long long)mt * BM + 64 * h + 16 * wq + (lane >> 2) + 8 * e2;
                     if (m >= p.M) continue;
 #pragma unroll
-                    for (int j = 0; j < kK2MaxN / 16; ++j)
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            const int c = 16 * j + 8 * i + 2 * (lane & 3);
-                            if (c >= n_valid) continue;
-                            const int n = n0 + c;
-                            float2 b;
-                            asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(b.x), "=f"(b.y) : "r"(sB + (uint32_t)n * 4u));
-                            const float a0 = acc.d[h][j][4 * i + 2 * e2], a1 = acc.d[h][j][4 * i + 2 * e2 + 1];
-                            // swish: b holds b/2 -> h = acc/2 + b/2 == (acc + b)/2 bit for bit (the halving is exact)
-                            float o0 = SWISH ? swish_from_half(fmaf(a0, 0.5f, b.x)) : a0 + b.x;
-                            float o1 = SWISH ? swish_from_half(fmaf(a1, 0.5f, b.y)) : a1 + b.y;
-                            if (RESID) {
-                                float lo, hi;
-                                unpack2<T>(*reinterpret_cast<const uint32_t*>(resid + m * p.N + n), lo, hi);
-                                o0 += lo; o1 += hi;
-                            }
-                            *reinterpret_cast<uint32_t*>(out + m * p.N + n) = OUT_H ? pack2<__half>(o0, o1) : pack2<T>(o0, o1);
+                    for (int i = 0; i < NT / 8; ++i) {
+                        const int c = 8 * i + 2 * (lane & 3);
+                        if (c >= n_valid) continue;
+                        const int n = n0 + c;
+                        float2 b;
+                        asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(b.x), "=f"(b.y) : "r"(sB + (uint32_t)n * 4u));
+                        const float a0 = acc.d[h][4 * i + 2 * e2], a1 = acc.d[h][4 * i + 2 * e2 + 1];
+                        // swish: b holds b/2 -> h = acc/2 + b/2 == (acc + b)/2 bit for bit (the halving is exact)
+                        float o0 = SWISH ? swish_from_half(fmaf(a0, 0.5f, b.x)) : a0 + b.x;
+                        float o1 = SWISH ? swish_from_half(fmaf(a1, 0.5f, b.y)) : a1 + b.y;
+                        if (RESID) {
+                            float lo, hi;
+                            unpack2<T>(*reinterpret_cast<const uint32_t*>(resid + m * p.N + n), lo, hi);
+                            o0 += lo; o1 += hi;
                         }
+                        *reinterpret_cast<uint32_t*>(out + m * p.N + n) = OUT_H ? pack2<__half>(o0, o1) : pack2<T>(o0, o1);
+                    }
                 }
         }
     } else if (GATE && warp >= 12) {
@@ -277,12 +284,12 @@ int launch_k2(cudaStream_t stream, const K2Params& p, size_t smem, bool swish, b
     const int ctas = p.tiles < sm_count ? p.tiles : sm_count;
     if (ctas < 1) return 0;
 #define K2_GO(SW, GA, RE, OH)                                                                                                 \
-    do {                                                                                                                    \
-        auto kfn = k2_kernel<T, SW, GA, RE, OH>;                                                                            \
+    return with_mma_width<kK2MaxN>(p.n_tile, [&](auto nt) {                                                                 \
+        auto kfn = k2_kernel<T, SW, GA, RE, OH, decltype(nt)::value>;                                                       \
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) != cudaSuccess) return -1;   \
         kfn<<<ctas, kK2Threads, smem, stream>>>(p);                                                                         \
         return 0;                                                                                                           \
-    } while (0)
+    })
     if (out_half && !(swish && !gate && !resid)) return 1;
     if (swish && !gate && !resid && out_half) K2_GO(true, false, false, true);
     if (swish && !gate && !resid) K2_GO(true, false, false, false);

@@ -132,18 +132,16 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const uint8_t* __restrict_
         }
     };
 
-    tc::WgAcc<2> acc;
+    tc::WgAcc<32> acc;
     build(0, 0);
     for (int rl = 0; rl < G::ROWS; ++rl) {
         const int buf = rl & 1;
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();                            // A(rl) complete; row rl-1 drained out of the accumulator tile
-        tc::wg_fence();
-        tc::wg_mma_tile<true, 2>(acc, sA + buf * A_BYTES, sW, 4, 2, 0u);
-        tc::wg_commit();
+        tc::wg_mma_tile<true, 32>(acc, sA + buf * A_BYTES, sW, 4, 0u);
         if (rl + 1 < G::ROWS) build(rl + 1, buf ^ 1);           // A[buf^1]: its MMA (row rl-1) completed last iteration
         tc::wg_wait<0>();
-        tc::wg_acc_store<2>(acc, sAcc, 2, tid);
+        tc::wg_acc_store<32>(acc, sAcc, tid);
         __syncthreads();
         drain(rl);
     }

@@ -7,9 +7,10 @@
 // D  : fp32 accumulators in the registers of the issuing warpgroup (128 threads)
 //
 // Operands sit in shared memory in the canonical K-major SWIZZLE_128B layout (16-byte chunk c of row r lands at chunk
-// c ^ (r & 7) of its 128-byte row; 8-row atoms of 1024 B).  A 128-row tile is two wgmma.m64nNk16 row halves; N is walked in
-// 16-column pieces so one code path serves every channel count.  After the last K step the warpgroup writes its fragments
-// to a shared-memory accumulator tile ([column][kAccPitch] fp32), where the epilogues read one pixel row per thread.
+// c ^ (r & 7) of its 128-byte row; 8-row atoms of 1024 B).  A 128-row tile is two wgmma.m64nNk16 row halves, one
+// instruction per half and K step for the full tile width N (a template parameter of the kernels).  After the last K step
+// the warpgroup writes its fragments to a shared-memory accumulator tile ([column][kAccPitch] fp32), where the epilogues
+// read one pixel row per thread.
 //
 // Every mbarrier wait is bounded: a wait that exceeds its budget raises the context's timeout flag (mapped pinned host
 // memory) and the CTA bails out instead of hanging the GPU.
@@ -71,79 +72,140 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D(64 x 16) (+)= A(64 x 16) * B(16 x 16)^T, both operands K-major in shared memory; fp32 accumulators
-template <bool BF16>
-__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t ad, uint64_t bd, uint32_t accumulate) {
-    if constexpr (BF16)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %10, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-            : "l"(ad), "l"(bd), "r"(accumulate));
-    else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %10, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-            : "l"(ad), "l"(bd), "r"(accumulate));
-}
-
-// Accumulators of one warpgroup: row half h (rows 64h..64h+63) x NCH 16-column pieces
-template <int NCH> struct WgAcc { float d[2][NCH][8]; };
-
-// Issue the K steps [k0, k0 + ksteps) of a 128-row tile: a_st / b_st are the K block's operand bases (8-row atoms of
-// 1024 B), `nch` 16-column pieces of B (rows 16j.. of the weight tile).  Called by all 128 threads of a warpgroup.
-// `accumulate` == 0 starts the sums at zero with the first step.  The caller commits / waits.
-template <bool BF16, int NCH>
-__device__ __forceinline__ void wg_mma_tile(WgAcc<NCH>& acc, uint32_t a_st, uint32_t b_st, int ksteps, int nch, uint32_t accumulate) {
-    const uint64_t a0 = make_desc(a_st), a1 = make_desc(a_st + 64 * 128);
-    for (int k = 0; k < ksteps; ++k) {
-#pragma unroll
-        for (int j = 0; j < NCH; ++j) {
-            if (j < nch) {
-                const uint64_t bd = make_desc(b_st + (uint32_t)j * 2048u) + (uint64_t)(k * 2);
-                wgmma_n16<BF16>(acc.d[0][j], a0 + (uint64_t)(k * 2), bd, (accumulate | (uint32_t)k) ? 1u : 0u);
-                wgmma_n16<BF16>(acc.d[1][j], a1 + (uint64_t)(k * 2), bd, (accumulate | (uint32_t)k) ? 1u : 0u);
-            }
-        }
+// Operand lists of wgmma.mma_async.m64nNk16 for N = 16 k (k = 1..8): the N / 2 fp32 accumulators are operands %0 .. %(8k - 1),
+// the A and B descriptors and the scale-d flag follow them.  WG_REGS_k extends WG_REGS_(k-1) by one group of eight.
+#define WG_D8(g) "+f"(d[8 * g]), "+f"(d[8 * g + 1]), "+f"(d[8 * g + 2]), "+f"(d[8 * g + 3]), \
+                 "+f"(d[8 * g + 4]), "+f"(d[8 * g + 5]), "+f"(d[8 * g + 6]), "+f"(d[8 * g + 7])
+#define WG_OPS_1 WG_D8(0)
+#define WG_OPS_2 WG_OPS_1, WG_D8(1)
+#define WG_OPS_3 WG_OPS_2, WG_D8(2)
+#define WG_OPS_4 WG_OPS_3, WG_D8(3)
+#define WG_OPS_5 WG_OPS_4, WG_D8(4)
+#define WG_OPS_6 WG_OPS_5, WG_D8(5)
+#define WG_OPS_7 WG_OPS_6, WG_D8(6)
+#define WG_OPS_8 WG_OPS_7, WG_D8(7)
+#define WG_REGS_1 "%0,%1,%2,%3,%4,%5,%6,%7"
+#define WG_REGS_2 WG_REGS_1 ",%8,%9,%10,%11,%12,%13,%14,%15"
+#define WG_REGS_3 WG_REGS_2 ",%16,%17,%18,%19,%20,%21,%22,%23"
+#define WG_REGS_4 WG_REGS_3 ",%24,%25,%26,%27,%28,%29,%30,%31"
+#define WG_REGS_5 WG_REGS_4 ",%32,%33,%34,%35,%36,%37,%38,%39"
+#define WG_REGS_6 WG_REGS_5 ",%40,%41,%42,%43,%44,%45,%46,%47"
+#define WG_REGS_7 WG_REGS_6 ",%48,%49,%50,%51,%52,%53,%54,%55"
+#define WG_REGS_8 WG_REGS_7 ",%56,%57,%58,%59,%60,%61,%62,%63"
+// N, then the operand numbers of (A descriptor, B descriptor) and of the scale-d flag
+#define WG_TAIL_1 "16", "%8, %9", "%10"
+#define WG_TAIL_2 "32", "%16, %17", "%18"
+#define WG_TAIL_3 "48", "%24, %25", "%26"
+#define WG_TAIL_4 "64", "%32, %33", "%34"
+#define WG_TAIL_5 "80", "%40, %41", "%42"
+#define WG_TAIL_6 "96", "%48, %49", "%50"
+#define WG_TAIL_7 "112", "%56, %57", "%58"
+#define WG_TAIL_8 "128", "%64, %65", "%66"
+#define WG_ASM_(TY, REGS, NS, AB, SC, ...)                                                                              \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " SC ", 0;\n\t"                                                    \
+                 "wgmma.mma_async.sync.aligned.m64n" NS "k16.f32." TY "." TY " {" REGS "}, " AB ", p, 1, 1, 0, 0;\n\t}" \
+                 : __VA_ARGS__ : "l"(ad), "l"(bd), "r"(accumulate))
+#define WG_ASM(TY, REGS, TAIL, OPS) WG_ASM_(TY, REGS, TAIL, OPS)     // (one more expansion: TAIL and OPS split into their commas)
+#define WG_CASE(k)                                                                                                 \
+    if constexpr (N == 16 * k) {                                                                                   \
+        if constexpr (BF16) WG_ASM("bf16", WG_REGS_##k, WG_TAIL_##k, WG_OPS_##k);                                  \
+        else WG_ASM("f16", WG_REGS_##k, WG_TAIL_##k, WG_OPS_##k);                                                  \
     }
-}
 
-// One 64-row half on its own (kernels whose warpgroups split the M tiles of a CTA between them): D(64 x 16 nch) (+)= A * B^T
-// over `ksteps` K steps; a_kb / b_kb = byte distance between consecutive 64-channel K blocks of A / B.
-template <bool BF16, int NCH>
-__device__ __forceinline__ void wg_mma_m64(float (&d)[NCH][8], uint32_t a_st, uint32_t a_kb, uint32_t b_st, uint32_t b_kb, int ksteps, int nch) {
-    for (int ks = 0; ks < ksteps; ++ks) {
-        const int kb = ks >> 2, k = ks & 3;
-        const uint64_t ad = make_desc(a_st + (uint32_t)kb * a_kb) + (uint64_t)(k * 2);
+// D(64 x N) (+)= A(64 x 16) * B(N x 16)^T, both operands K-major in shared memory; fp32 accumulators.  ONE instruction for
+// the whole width: B's N rows are 8-row atoms of 1024 B from `bd` on.  The m64nN fragment is the m64n16 fragments laid end
+// to end: register 8j + 4i + e holds what register 4i + e of 16-column piece j would.
+template <bool BF16, int N>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t ad, uint64_t bd, uint32_t accumulate) {
+    static_assert(N % 16 == 0 && N >= 16 && N <= 128, "wgmma: N = 16, 32, ..., 128");
+    WG_CASE(1) WG_CASE(2) WG_CASE(3) WG_CASE(4) WG_CASE(5) WG_CASE(6) WG_CASE(7) WG_CASE(8)
+}
+#undef WG_CASE
+#undef WG_ASM
+#undef WG_ASM_
+
+// Accumulators of one warpgroup for an N-column tile: row half h (rows 64h..64h+63), fragment register r
+template <int N> struct WgAcc { float d[2][N / 2]; };
+
+// KS K steps of one 64-channel K block for H row halves (A descriptors a0, a1), issued as ONE straight run between its own
+// wgmma.fence and commit_group: with no branch and no other register traffic inside the run, ptxas has no reason to inject
+// warpgroup arrives or to serialise the MMAs.  `accumulate` == 0 starts the sums at zero with the first step.
+template <bool BF16, int N, int H, int KS>
+__device__ __forceinline__ void wg_mma_run(float (&d)[H][N / 2], uint64_t a0, uint64_t a1, uint64_t b0, uint32_t accumulate) {
+    wg_fence();
 #pragma unroll
-        for (int j = 0; j < NCH; ++j)
-            if (j < nch) wgmma_n16<BF16>(d[j], ad, make_desc(b_st + (uint32_t)kb * b_kb + (uint32_t)j * 2048u) + (uint64_t)(k * 2), ks ? 1u : 0u);
+    for (int k = 0; k < KS; ++k) {
+        const uint32_t sc = (accumulate | (uint32_t)k) ? 1u : 0u;
+        wgmma<BF16, N>(d[0], a0 + (uint64_t)(k * 2), b0 + (uint64_t)(k * 2), sc);
+        if constexpr (H == 2) wgmma<BF16, N>(d[1], a1 + (uint64_t)(k * 2), b0 + (uint64_t)(k * 2), sc);
     }
+    wg_commit();
+}
+// the run for the block's K step count (1..4; a ragged last block has fewer than 4)
+template <bool BF16, int N, int H>
+__device__ __forceinline__ void wg_mma_block(float (&d)[H][N / 2], uint64_t a0, uint64_t a1, uint64_t b0, int ksteps, uint32_t accumulate) {
+    if (ksteps >= 4) wg_mma_run<BF16, N, H, 4>(d, a0, a1, b0, accumulate);
+    else if (ksteps == 3) wg_mma_run<BF16, N, H, 3>(d, a0, a1, b0, accumulate);
+    else if (ksteps == 2) wg_mma_run<BF16, N, H, 2>(d, a0, a1, b0, accumulate);
+    else wg_mma_run<BF16, N, H, 1>(d, a0, a1, b0, accumulate);
 }
 
-// Fragments -> shared accumulator tile [column][kAccPitch] (fp32).  `wt` = thread index inside the warpgroup.
-// m64n16 fragment: register 4i + {0,1} -> row 16 w + l/4, columns 8 i + 2 (l%4) + {0,1}; 4i + {2,3} -> row + 8
-template <int NCH>
-__device__ __forceinline__ void wg_acc_store(const WgAcc<NCH>& acc, uint32_t dst, int nch, int wt) {
+// One K block (ksteps = 1..4 K steps) of a 128 x N tile: a_st / b_st are the block's operand bases (8-row atoms of 1024 B),
+// B = rows 0..N-1 of the weight tile (rows past the valid columns zero-filled; their columns are never stored).  Called by
+// all 128 threads of a warpgroup: one wgmma per row half and K step, fenced and committed (one group) here; the caller waits.
+template <bool BF16, int N>
+__device__ __forceinline__ void wg_mma_tile(WgAcc<N>& acc, uint32_t a_st, uint32_t b_st, int ksteps, uint32_t accumulate) {
+    wg_mma_block<BF16, N, 2>(acc.d, make_desc(a_st), make_desc(a_st + 64 * 128), make_desc(b_st), ksteps, accumulate);
+}
+
+// One 64-row half on its own (kernels whose warpgroups split the M tiles of a CTA between them): D(64 x N) = A * B^T over
+// `ksteps` K steps, 4 per 64-channel K block (one commit group each); a_kb / b_kb = byte distance between consecutive K
+// blocks of A / B.  The caller waits.
+template <bool BF16, int N>
+__device__ __forceinline__ void wg_mma_m64(float (&d)[N / 2], uint32_t a_st, uint32_t a_kb, uint32_t b_st, uint32_t b_kb, int ksteps) {
+    float (&d1)[1][N / 2] = *reinterpret_cast<float(*)[1][N / 2]>(&d);
+    for (int kb = 0; kb * 4 < ksteps; ++kb)
+        wg_mma_block<BF16, N, 1>(d1, make_desc(a_st + (uint32_t)kb * a_kb), 0, make_desc(b_st + (uint32_t)kb * b_kb), ksteps - 4 * kb, kb ? 1u : 0u);
+}
+
+// Fragments -> shared accumulator tile [column][kAccPitch] (fp32), all N columns.  `wt` = thread index inside the warpgroup.
+// m64nN fragment: register 4i + {0,1} -> row 16 w + l/4, columns 8 i + 2 (l%4) + {0,1}; 4i + {2,3} -> row + 8
+template <int N>
+__device__ __forceinline__ void wg_acc_store(const WgAcc<N>& acc, uint32_t dst, int wt) {
     const int w = wt >> 5, l = wt & 31;
     const int r = 16 * w + (l >> 2), cq = 2 * (l & 3);
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int j = 0; j < NCH; ++j) {
-            if (j < nch) {
+        for (int i = 0; i < N / 8; ++i)
 #pragma unroll
-                for (int i = 0; i < 2; ++i)
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int row = 64 * h + r + (e >> 1) * 8, col = 16 * j + 8 * i + cq + (e & 1);
-                        asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (uint32_t)(col * kAccPitch + row) * 4u), "f"(acc.d[h][j][4 * i + e]) : "memory");
-                    }
+            for (int e = 0; e < 4; ++e) {
+                const int row = 64 * h + r + (e >> 1) * 8, col = 8 * i + cq + (e & 1);
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (uint32_t)(col * kAccPitch + row) * 4u), "f"(acc.d[h][4 * i + e]) : "memory");
             }
-        }
+}
+
+// MMA widths the 1x1 kernels are instantiated for; a tile of n columns runs at the smallest one >= n (the extra B rows are
+// zero-filled, the extra columns never stored)
+__host__ __device__ constexpr int pw_mma_width(int n) { return n <= 64 ? (n + 15) & ~15 : n <= 96 ? 96 : 128; }
+
+// Host: f(std::integral_constant<int, w>{}) when w is one of those widths and <= MAXW (only those are instantiated); else 1
+template <int W, int MAXW, typename F>
+int call_with_width(F& f) {
+    if constexpr (W <= MAXW) return f(std::integral_constant<int, W>{});
+    else return 1;
+}
+template <int MAXW, typename F>
+int with_mma_width(int w, F&& f) {
+    switch (w) {
+        case 16: return call_with_width<16, MAXW>(f);
+        case 32: return call_with_width<32, MAXW>(f);
+        case 48: return call_with_width<48, MAXW>(f);
+        case 64: return call_with_width<64, MAXW>(f);
+        case 96: return call_with_width<96, MAXW>(f);
+        case 128: return call_with_width<128, MAXW>(f);
+    }
+    return 1;
 }
 
 // 16 consecutive columns of one accumulator row from the shared accumulator tile
@@ -229,19 +291,20 @@ template <> __device__ __forceinline__ uint4 scale8s<__half>(uint4 raw, uint32_t
 }
 
 // OUT_H: the result is written as fp16 whatever T is (the expand conv feeding the HFMA2 depthwise kernel KD)
-template <typename T, bool SWISH, int GATE, bool RESID, bool OUT_H = false>
+// UN: MMA width (pw_mma_width(n_tile)): rows of the W stage, columns of the accumulator tile
+template <typename T, bool SWISH, int GATE, bool RESID, bool OUT_H, int UN>
 __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, const T* __restrict__ Wt,
                                                      const float* __restrict__ bias, const float* __restrict__ gate,
                                                      const T* __restrict__ resid, T* __restrict__ out,
                                                      int M, int K, int N, int hw,
-                                                     int n_tile, int umma_n, int n_stages,
+                                                     int n_tile, int n_stages,
                                                      int tiles_per_crop) {    // GATE == 2 only
     constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     extern __shared__ uint8_t smem_raw[];
 
     const int tid = threadIdx.x;
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const int w_stage_bytes = umma_n * BK * 2;
+    constexpr int w_stage_bytes = UN * BK * 2;
     const uint32_t stage_bytes = A_STAGE_BYTES + w_stage_bytes;
     const uint32_t sG = smem0 + n_stages * stage_bytes;          // gate rows: [<=4 crops][K] fp32 (GATE only)
 
@@ -288,7 +351,9 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
                 cp_async16_z(a_st + swz + i * 2048, valid ? asrc + (long long)i * 16 * K : A, valid);
             }
             const T* wsrc = Wt + (long long)(n0 + r0) * K + (kc0 + c) * 8;
-            for (int r = r0, i = 0; r < umma_n; r += 16, ++i) {
+#pragma unroll
+            for (int i = 0; i < UN / 16; ++i) {
+                const int r = r0 + 16 * i;
                 const bool valid = cvalid && r < n_valid;
                 cp_async16_z(w_st + swz + i * 2048, valid ? wsrc + (long long)i * 16 * K : Wt, valid);
             }
@@ -300,7 +365,7 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
             cp_async16_z(a_st + (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4),
                          valid ? A + (long long)(m0 + r) * K + (kc0 + c) * 8 : A, valid);
         }
-        for (int idx = tid; idx < umma_n * cbp; idx += 128) {
+        for (int idx = tid; idx < UN * cbp; idx += 128) {
             const int r = fdiv_small(idx, 1.0f / (float)cbp), c = idx - r * cbp;
             const bool valid = r < n_valid && c < cb;
             cp_async16_z(w_st + (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4),
@@ -311,8 +376,7 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
         if (j < nkb) fill(j);
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
-    WgAcc<8> acc;
-    const int nch16 = umma_n >> 4;
+    WgAcc<UN> acc;
 
     // GATE == 1: byte offset of the gate row (crop) of each of the 8 rows this thread rescales, fixed for the whole K loop
     uint32_t g_row[8];
@@ -366,7 +430,7 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
                             sts128_(addr, scale8s<T>(lds128(addr), sG + (uint32_t)((kc0 + c) * 8) * 4));
                         }
                 } else {
-                    for (int idx = tid; idx < umma_n * cbp; idx += 128) {
+                    for (int idx = tid; idx < UN * cbp; idx += 128) {
                         const int r = fdiv_small(idx, 1.0f / (float)cbp), c = idx - r * cbp;
                         if (r < n_valid && c < cb) {
                             const uint32_t addr = w_st + (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4);
@@ -380,9 +444,7 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
         __syncthreads();
         {
             const int krem = min(BK, K - kb * BK);
-            wg_fence();
-            wg_mma_tile<BF16, 8>(acc, a_st, w_st, (krem + 15) >> 4, nch16, kb ? 1u : 0u);
-            wg_commit();
+            wg_mma_tile<BF16, UN>(acc, a_st, w_st, (krem + 15) >> 4, kb ? 1u : 0u);     // one commit group per K block
         }
         // refill the stage block kb-1 used with block kb-1+n_stages once its MMAs have completed (every thread's group)
         if (kb >= 1 && kb - 1 + n_stages < nkb) {
@@ -397,14 +459,14 @@ __global__ void __launch_bounds__(128) pw_tc2_kernel(const T* __restrict__ A, co
     __syncthreads();
     // the operand ring is free: accumulators -> shared accumulator tile at smem0, the 16-bit output stage after it
     const uint32_t sAcc = smem0;
-    wg_acc_store<8>(acc, sAcc, nch16, tid);
+    wg_acc_store<UN>(acc, sAcc, tid);
     __syncthreads();
 
     // ---- epilogue: TMEM -> +shift, swish, +residual -> 16-bit -> stage -> coalesced stores
     const int nch = n_valid >> 3;
     const float inv_nch = 1.0f / (float)(nch > 0 ? nch : 1);
     const int pitch16 = nch | 1;
-    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (smem0 + acc_tile_bytes(umma_n) - smem_u32(smem_raw)));
+    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (smem0 + acc_tile_bytes(UN) - smem_u32(smem_raw)));
     const bool row_ok = tid < rows_valid;
     const long long m = (long long)m0 + tid;
     {
@@ -466,7 +528,7 @@ int launch_pw_tc2(cudaStream_t stream, const T* A, const void* Wt16, const float
         if (nt >= n_tile) break;
         n_tile = nt;
     }
-    const int umma_n = (n_tile + 15) & ~15;
+    const int umma_n = pw_mma_width(n_tile);
     const int nkb = (K + BK - 1) / BK;
     const size_t stage_bytes = A_STAGE_BYTES + (size_t)umma_n * BK * 2;
     const int gate_crops = per_crop ? 1 : std::min(4, (BM - 1) / hw + 2);      // crops one 128-row tile can touch
@@ -484,21 +546,21 @@ int launch_pw_tc2(cudaStream_t stream, const T* A, const void* Wt16, const float
     if (smem > 225 * 1024) return 1;
     dim3 grid((unsigned)((N + n_tile - 1) / n_tile), (unsigned)m_tiles);
     const T* W = reinterpret_cast<const T*>(Wt16);
-#define TC2(SW, GA, RE, OH)                                                                                          \
-    do {                                                                                                             \
-        auto kfn = pw_tc2_kernel<T, SW, GA, RE, OH>;                                                       \
+#define TC2(SW, GA, RE, OH)                                                                                              \
+    return with_mma_width<128>(umma_n, [&](auto un) {                                                                         \
+        auto kfn = pw_tc2_kernel<T, SW, GA, RE, OH, decltype(un)::value>;                                                \
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) != cudaSuccess) return -1; \
-        kfn<<<grid, 128, smem, stream>>>(A, W, bias, gate, resid, out, (int)M, K, N, hw, n_tile, umma_n, n_stages, tpc); \
-    } while (0)
+        kfn<<<grid, 128, smem, stream>>>(A, W, bias, gate, resid, out, (int)M, K, N, hw, n_tile, n_stages, tpc);         \
+        return 0;                                                                                                        \
+    })
     if (out_half && !(swish && !gate && !resid)) return 1;
     if (swish && !gate && !resid) { if (out_half) TC2(true, 0, false, true); else TC2(true, 0, false, false); }
     else if (!swish && !gate && !resid) TC2(false, 0, false, false);
     else if (!swish && !gate && resid) TC2(false, 0, true, false);           // project conv whose input K1 has already gated
     else if (!swish && gate && !resid) { if (per_crop) TC2(false, 2, false, false); else TC2(false, 1, false, false); }
     else if (!swish && gate && resid) { if (per_crop) TC2(false, 2, true, false); else TC2(false, 1, true, false); }
-    else return 1;
 #undef TC2
-    return 0;
+    return 1;
 }
 
 
@@ -508,11 +570,13 @@ int launch_pw_tc2(cudaStream_t stream, const T* A, const void* Wt16, const float
 // Here a CTA walks `tpc` consecutive tiles of ONE crop: gate row and W' = bf16(W * g) once per CTA (the same scale8s and the
 // same wgmma sequence as pw_tc2's per-crop route, so the results are bit-identical); the cp.async of tile t+1 runs under the
 // MMA and the epilogue of tile t.
-template <typename T, bool RESID>
+// UN = the plan's umma_n (N rounded up to 16): rows of the resident W, MMA width
+template <typename T, bool RESID, int UN>
 __global__ void __launch_bounds__(128) pw_tc3_kernel(const T* __restrict__ A, const T* __restrict__ Wt, const float* __restrict__ bias,
                                                      const float* __restrict__ gate, const T* __restrict__ resid, T* __restrict__ out,
-                                                     int K, int N, int hw, int umma_n, int tiles_per_crop, int tpc, int groups) {
+                                                     int K, int N, int hw, int tiles_per_crop, int tpc, int groups) {
     constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+    constexpr int umma_n = UN;
     extern __shared__ uint8_t smem_raw[];
     const int tid = threadIdx.x;
     const int nkb = (K + BK - 1) / BK, kchunks = K >> 3;
@@ -582,7 +646,6 @@ __global__ void __launch_bounds__(128) pw_tc3_kernel(const T* __restrict__ A, co
                 }
         }
     }
-    const int nch16 = umma_n >> 4;
     auto epilogue = [&](int t) {
         const int rows_valid = min(BM, hw - t * BM);
         const long long m0 = (long long)crop * hw + (long long)t * BM;
@@ -616,23 +679,21 @@ __global__ void __launch_bounds__(128) pw_tc3_kernel(const T* __restrict__ A, co
     };
 
     const int ntiles = t_end - t_begin;
-    WgAcc<4> acc;
+    WgAcc<UN> acc;
     for (int it = 0; it < ntiles; ++it) {
         const int t = t_begin + it, buf = it & 1;
         asm volatile("cp.async.wait_group 0;" ::: "memory");            // A(t) has landed (this thread's part)
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();                                                // ... everyone's; the store loop of tile t-1 is done with `stage`
-        wg_fence();
         for (int kb = 0; kb < nkb; ++kb) {
             const int krem = min(BK, K - kb * BK);
-            wg_mma_tile<BF16, 4>(acc, sA + buf * a_bytes + kb * A_STAGE_BYTES, sW + (uint32_t)kb * umma_n * 128, (krem + 15) >> 4, nch16, kb ? 1u : 0u);
+            wg_mma_tile<BF16, UN>(acc, sA + buf * a_bytes + kb * A_STAGE_BYTES, sW + (uint32_t)kb * umma_n * 128, (krem + 15) >> 4, kb ? 1u : 0u);
         }
-        wg_commit();
         // A buffer buf ^ 1 was read by the MMA of tile t-1, which has completed
         if (it + 1 < ntiles) fill_a(t + 1, buf ^ 1);
         asm volatile("cp.async.commit_group;" ::: "memory");
         wg_wait<0>();
-        wg_acc_store<4>(acc, sAcc, nch16, tid);
+        wg_acc_store<UN>(acc, sAcc, tid);
         __syncthreads();
         epilogue(t);
     }
@@ -665,19 +726,16 @@ int launch_pw_tc3(cudaStream_t stream, const T* A, const void* Wt16, const float
     Pw3Plan pl{};
     if (sizeof(T) != 2 || !plan_pw_tc3(M, K, N, hw, gate != nullptr, &pl)) return 1;
     const int crops = (int)(M / hw);
-    const int tiles_per_crop = pl.tiles_per_crop, tpc = pl.tpc, groups = pl.groups, umma_n = pl.umma_n;
+    const int tiles_per_crop = pl.tiles_per_crop, tpc = pl.tpc, groups = pl.groups;
     const size_t smem = pl.smem;
     const T* W = reinterpret_cast<const T*>(Wt16);
-    if (resid) {
-        auto kfn = pw_tc3_kernel<T, true>;
+    // umma_n <= 64: a multiple of 16, so pw_mma_width(umma_n) == umma_n
+    return with_mma_width<64>(pl.umma_n, [&](auto un) {
+        auto kfn = resid ? pw_tc3_kernel<T, true, decltype(un)::value> : pw_tc3_kernel<T, false, decltype(un)::value>;
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;
-        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, umma_n, tiles_per_crop, tpc, groups);
-    } else {
-        auto kfn = pw_tc3_kernel<T, false>;
-        if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;
-        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, umma_n, tiles_per_crop, tpc, groups);
-    }
-    return 0;
+        kfn<<<crops * groups, 128, smem, stream>>>(A, W, bias, gate, resid, out, K, N, hw, tiles_per_crop, tpc, groups);
+        return 0;
+    });
 }
 
 }  // namespace tc

@@ -32,25 +32,25 @@ __device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo
     lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-template <bool SWISH, bool GATE, bool RESID>
+// UN = pw_mma_width(n_tile): rows of the W stages, MMA width
+template <bool SWISH, bool GATE, bool RESID, int UN>
 __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ A, const __nv_bfloat16* __restrict__ Whi,
                                                       const __nv_bfloat16* __restrict__ Wlo, const float* __restrict__ bias,
                                                       const float* __restrict__ gate, const float* __restrict__ resid,
                                                       float* __restrict__ out, int M, int K, int N, int hw,
-                                                      int n_tile, int umma_n) {
+                                                      int n_tile) {
     extern __shared__ uint8_t smem_raw[];
 
     const int tid = threadIdx.x;
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t w_bytes = (uint32_t)umma_n * 128;
+    constexpr uint32_t w_bytes = (uint32_t)UN * 128;
     const uint32_t stage_bytes = 2 * A_STAGE_BYTES + 2 * w_bytes;      // A hi | A lo | W hi | W lo
 
     const int m0 = blockIdx.y * BM, n0 = blockIdx.x * n_tile;
     const int rows_valid = min(BM, M - m0), n_valid = min(n_tile, N - n0);
     const int nkb = (K + BK - 1) / BK, kchunks = K >> 3;
 
-    WgAcc<8> acc;
-    const int nch16 = umma_n >> 4;
+    WgAcc<UN> acc;
 
     // this thread stages chunk c (8 channels) of rows r0 + 16 i: its gate row index per row is fixed for the whole K loop
     const int c = tid & 7, r0 = tid >> 3;
@@ -58,8 +58,8 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
 
     for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb & 1;
-        if (kb >= 2) {              // the MMAs of block kb-2 are done with this stage (in every thread)
-            wg_wait<1>();
+        if (kb >= 2) {              // the MMAs of block kb-2 are done with this stage (in every thread): block kb-1's three groups may be pending
+            wg_wait<3>();
             __syncthreads();
         }
         const uint32_t a_hi = smem0 + s * stage_bytes, a_lo = a_hi + A_STAGE_BYTES, w_hi = a_lo + A_STAGE_BYTES, w_lo = w_hi + w_bytes;
@@ -83,7 +83,9 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
             sts128_(a_hi + swz + i * 2048, hi);
             sts128_(a_lo + swz + i * 2048, lo);
         }
-        for (int r = r0, i = 0; r < umma_n; r += 16, ++i) {
+#pragma unroll
+        for (int i = 0; i < UN / 16; ++i) {
+            const int r = r0 + 16 * i;
             uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
             if (cvalid && r < n_valid) {
                 hi = __ldg(reinterpret_cast<const uint4*>(Whi + (long long)(n0 + r) * K + kc * 8));
@@ -95,17 +97,15 @@ __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ 
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
         const int ksteps = (min(BK, K - kb * BK) + 15) >> 4;
-        wg_fence();
-        wg_mma_tile<true, 8>(acc, a_hi, w_hi, ksteps, nch16, kb ? 1u : 0u);
-        wg_mma_tile<true, 8>(acc, a_hi, w_lo, ksteps, nch16, 1u);
-        wg_mma_tile<true, 8>(acc, a_lo, w_hi, ksteps, nch16, 1u);
-        wg_commit();
+        wg_mma_tile<true, UN>(acc, a_hi, w_hi, ksteps, kb ? 1u : 0u);      // one commit group each
+        wg_mma_tile<true, UN>(acc, a_hi, w_lo, ksteps, 1u);
+        wg_mma_tile<true, UN>(acc, a_lo, w_hi, ksteps, 1u);
     }
     wg_wait<0>();
     __syncthreads();
     // the operand stages are free: accumulators -> shared accumulator tile
     const uint32_t sAcc = smem0;
-    wg_acc_store<8>(acc, sAcc, nch16, tid);
+    wg_acc_store<UN>(acc, sAcc, tid);
     __syncthreads();
 
     // ---- epilogue, fp32: thread == pixel row; + shift, swish (precise), + residual; 16-byte stores
@@ -150,17 +150,17 @@ inline int launch_pw_tc32(cudaStream_t stream, const float* A, const void* Whi, 
             ++parts;
         }
     }
-    const int umma_n = (n_tile + 15) & ~15;
+    const int umma_n = pw_mma_width(n_tile);
     const size_t smem = std::max((size_t)2 * (2 * A_STAGE_BYTES + 2 * (size_t)umma_n * 128), (size_t)acc_tile_bytes(umma_n)) + 1024;
     dim3 grid((unsigned)((N + n_tile - 1) / n_tile), (unsigned)((M + BM - 1) / BM));
     const __nv_bfloat16 *wh = reinterpret_cast<const __nv_bfloat16*>(Whi), *wl = reinterpret_cast<const __nv_bfloat16*>(Wlo);
 #define TC32(SW, GA, RE)                                                                                                   \
-    do {                                                                                                                   \
-        auto kfn = pw_tc32_kernel<SW, GA, RE>;                                                                             \
+    return with_mma_width<128>(umma_n, [&](auto un) {                                                                      \
+        auto kfn = pw_tc32_kernel<SW, GA, RE, decltype(un)::value>;                                                        \
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;  \
-        kfn<<<grid, 128, smem, stream>>>(A, wh, wl, bias, gate, resid, out, (int)M, K, N, hw, n_tile, umma_n); \
+        kfn<<<grid, 128, smem, stream>>>(A, wh, wl, bias, gate, resid, out, (int)M, K, N, hw, n_tile);                     \
         return 0;                                                                                                          \
-    } while (0)
+    })
     if (swish && !gate && !resid) TC32(true, false, false);
     if (!swish && gate && !resid) TC32(false, true, false);
     if (!swish && gate && resid) TC32(false, true, true);
