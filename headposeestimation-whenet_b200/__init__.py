@@ -4,7 +4,9 @@ The directory is named ``headposeestimation-whenet_b200`` (not importable as
 is); import it as ``whenet_b200`` through the shim package at the repo root.
 """
 from .whenet import WHENet, WHENetModel  # noqa: F401
-from . import arch, build, crops, dp, overlay, weights  # noqa: F401
+from .yolo import YOLO  # noqa: F401
+from . import arch, build, crops, dp, overlay, pipeline, weights, yolo_arch  # noqa: F401
 from ._lib import WhenetError, lib_path  # noqa: F401
 
-__all__ = ["WHENet", "WHENetModel", "WhenetError", "arch", "build", "crops", "dp", "overlay", "weights", "lib_path"]
+__all__ = ["WHENet", "WHENetModel", "YOLO", "WhenetError", "arch", "build", "crops", "dp", "overlay", "pipeline", "weights", "yolo_arch",
+           "lib_path"]

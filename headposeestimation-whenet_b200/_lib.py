@@ -14,6 +14,8 @@ EXPORTS = [
     "whenet_crop_resize_u8", "whenet_synchronize", "whenet_host_alloc", "whenet_host_free", "whenet_debug_enable_taps", "whenet_debug_tap",
     "whenet_debug_conv1x1", "whenet_debug_decode", "whenet_debug_raise_timeout", "whenet_debug_read_trace", "whenet_debug_set_k1_plan", "whenet_debug_set_k1w_plan", "whenet_profile_enable", "whenet_profile_read", "whenet_launch_count", "whenet_set_option",
     "whenet_last_error", "whenet_version", "whenet_destroy",
+    "whenet_det_create", "whenet_det_load_weights", "whenet_det_num_classes", "whenet_det_set_stream", "whenet_det_detect_u8",
+    "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_decode",
 ]
 
 
@@ -89,6 +91,18 @@ def load():
     L.whenet_version.restype = C.c_char_p
     L.whenet_destroy.argtypes = [P]
     L.whenet_destroy.restype = None
+    I = C.c_int
+    L.whenet_det_create.argtypes = [C.POINTER(P), I, I, I, I]
+    L.whenet_det_load_weights.argtypes = [P, C.POINTER(Tensor), I, P, I]
+    L.whenet_det_num_classes.argtypes = [P]
+    L.whenet_det_set_stream.argtypes = [P, P]
+    L.whenet_det_detect_u8.argtypes = [P, P, I, I, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
+    L.whenet_det_synchronize.argtypes = [P]
+    L.whenet_det_destroy.argtypes = [P]
+    L.whenet_det_destroy.restype = None
+    L.whenet_det_debug_tap.argtypes = [P, I, P, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.whenet_det_debug_conv.argtypes = [P, P, P, I, I, I, I, I, P, P, I, I, I, I, P, P]
+    L.whenet_det_debug_decode.argtypes = [P, P, P, P, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
     _lib = L
     return L
 

@@ -1,0 +1,60 @@
+// The YOLOv3 detector's kernels (kernels_yolo.cuh) and their launchers, in a unit of their own.
+#include "kernels_yolo.cuh"
+
+namespace whenet {
+namespace yolo {
+
+int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb) {
+    const long long hx = (long long)lp.rows * lp.nw;
+    letterbox_h_kernel<<<dim3((unsigned)((hx + 255) / 256), n), 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx, swap_rb);
+    letterbox_v_kernel<<<dim3((unsigned)((S_h * S_w + 255) / 256), n), 256, 0, s>>>(tmp, out, lp.nw, lp.nh, lp.rows, S_h, S_w, lp.ox, lp.oy,
+                                                                                   lp.yb, lp.ky, lp.ksy);
+    return (int)cudaGetLastError();
+}
+
+constexpr size_t kConv0Smem = 128 * 128 + 32 * 128 + 256 * 4 + tc::acc_tile_bytes(32) + 1024;
+
+int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w) {
+    cudaError_t e = cudaFuncSetAttribute(yolo_conv0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kConv0Smem);
+    if (e != cudaSuccess) return (int)e;
+    const long long tiles = (long long)n * S_h * S_w / 128;           // S_h * S_w is a multiple of 1024
+    yolo_conv0_kernel<<<(unsigned)tiles, 128, kConv0Smem, s>>>(img, w0, bias, out, S_h, S_w);
+    return (int)cudaGetLastError();
+}
+
+template <int MODE, int UN>
+int launch_igemm_t(cudaStream_t s, const IgemmParams& p, size_t smem, int grid_n, int grid_m) {
+    auto kfn = conv_igemm_kernel<MODE, UN>;
+    cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    kfn<<<dim3(grid_n, grid_m), 128, smem, s>>>(p);
+    return (int)cudaGetLastError();
+}
+
+template <int MODE>
+int launch_igemm_m(cudaStream_t s, const IgemmParams& p, int un, size_t smem, int grid_n, int grid_m) {
+    switch (un) {
+        case 32: return launch_igemm_t<MODE, 32>(s, p, smem, grid_n, grid_m);
+        case 64: return launch_igemm_t<MODE, 64>(s, p, smem, grid_n, grid_m);
+        case 128: return launch_igemm_t<MODE, 128>(s, p, smem, grid_n, grid_m);
+    }
+    return (int)cudaErrorInvalidValue;
+}
+
+int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
+    switch (mode) {
+        case kLeaky: return launch_igemm_m<kLeaky>(s, p, un, smem, grid_n, grid_m);
+        case kLeakyRes: return launch_igemm_m<kLeakyRes>(s, p, un, smem, grid_n, grid_m);
+        case kLeakyCat: return launch_igemm_m<kLeakyCat>(s, p, un, smem, grid_n, grid_m);
+        case kLinearF32: return launch_igemm_m<kLinearF32>(s, p, un, smem, grid_n, grid_m);
+    }
+    return (int)cudaErrorInvalidValue;
+}
+
+int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n) {
+    yolo_decode_nms_kernel<<<n, kNmsThreads, 0, s>>>(p);
+    return (int)cudaGetLastError();
+}
+
+}  // namespace yolo
+}  // namespace whenet

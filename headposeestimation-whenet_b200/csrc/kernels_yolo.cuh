@@ -1,0 +1,500 @@
+// kernels_yolo.cuh - the YOLOv3 head detector (reference yolo_v3/): letterbox, Darknet-53 + three heads on wgmma, decode + NMS.
+//
+//   letterbox_h_kernel / letterbox_v_kernel   Pillow's uint8 BICUBIC resample (two integer passes, 22-bit coefficients computed on
+//                                             the host exactly as ImagingResample does) + the (128,128,128) canvas and the paste
+//                                             (reference utils.py:23-34)
+//   yolo_conv0_kernel                          first conv (3 -> 32, 3x3): im2col row built in shared memory from the uint8 canvas
+//                                             through a v/255 table split into bf16 hi + lo parts, one K = 64 wgmma block per row
+//   conv_igemm_kernel<MODE, UN>                every other conv as an implicit GEMM (M = pixels, N = Cout, K = taps x Cin): the A
+//                                             operand is gathered per (tap, 64-channel chunk) with cp.async, out-of-image taps are
+//                                             zero-filled (= the padding); concat convs read [upsample(up), skip] virtually
+//   yolo_decode_nms_kernel                     one CTA per frame: decode every candidate, per-class score mask, greedy NMS
+//
+// Storage bf16 NHWC, fp32 accumulation; the three output convs write fp32.
+#pragma once
+#include "kernels_tc.cuh"
+
+namespace whenet {
+namespace yolo {
+
+using tc::BK;
+using tc::BM;
+using tc::cp_async16_z;
+using tc::smem_u32;
+
+// ----------------------------------------------------------------------------- host-visible parameters and plans
+enum { kLeaky = 0, kLeakyRes = 1, kLeakyCat = 2, kLinearF32 = 3 };
+
+struct IgemmParams {
+    const __nv_bfloat16* in;     // [n][Hi][Wi][Cin - c_up]  (concat: the skip tensor)
+    const __nv_bfloat16* up;     // concat: [n][Hi/2][Wi/2][c_up], read at (y >> 1, x >> 1)
+    const __nv_bfloat16* wt;     // [N][K], K = k*k*Cin, k index = (ky*k + kx)*Cin + ci
+    const float* bias;           // [N]
+    const __nv_bfloat16* resid;  // [M][N]
+    void* out;                   // [M][N] bf16, fp32 for kLinearF32
+    int M, Hi, Wi, Ho, Wo, Cin, c_up, N, k, stride, n_tile, n_stages;
+};
+
+// Tile plan of one conv.  It depends on the per-frame shape only, never on the batch size, so a frame's results are the same bits
+// whatever batch it runs in: the widest tile (<= 128 columns, what one warpgroup holds in registers) that still gives one frame
+// at least one CTA per SM, down to 32 columns.  The ring is as deep as fits two CTAs per SM.
+struct IgemmPlan { int n_tile, un, n_stages; size_t smem; };
+inline IgemmPlan plan_igemm(int Ho, int Wo, int N, int Cin, int k, int sm_count) {
+    IgemmPlan pl{};
+    const long long m_tiles = ((long long)Ho * Wo + BM - 1) / BM;
+    int n_tile = (N + 15) & ~15;
+    if (n_tile > 128) {
+        int parts = (N + 127) / 128;
+        n_tile = (((N + parts - 1) / parts) + 15) & ~15;
+    }
+    while (n_tile > 32 && m_tiles * ((N + n_tile - 1) / n_tile) < sm_count) n_tile = ((n_tile / 2) + 15) & ~15;
+    pl.n_tile = n_tile;
+    pl.un = n_tile <= 32 ? 32 : n_tile <= 64 ? 64 : 128;
+    const int nkb = k * k * ((Cin + BK - 1) / BK);
+    const size_t stage_bytes = tc::A_STAGE_BYTES + (size_t)pl.un * BK * 2;
+    int st = 4;
+    while (st > 2 && st * stage_bytes > 100 * 1024) --st;
+    pl.n_stages = nkb < st ? (nkb < 2 ? 2 : nkb) : st;
+    const size_t out_bytes = tc::acc_tile_bytes(pl.un) + (size_t)BM * ((size_t)(n_tile >> 3) | 1) * 16;
+    pl.smem = std::max((size_t)pl.n_stages * stage_bytes, out_bytes) + 1024;
+    return pl;
+}
+
+constexpr int kNmsThreads = 1024;
+constexpr int kNmsPer = 24;             // candidates per thread: 24 x 1024 >= 22,743 (608 x 608)
+constexpr int kMaxBoxes = 256;
+
+struct DecodeParams {
+    const float* head[3];               // [n][gh_l][gw_l][3 * (5 + C)] fp32 logits, l = 0, 1, 2 (13x13, 26x26, 52x52 at 416)
+    float4* cand;                       // workspace [n][NC] boxes (y_min, x_min, y_max, x_max)
+    float* cand_score;                  // workspace [n][C][NC]
+    float* out_boxes;                   // [n][C * max_boxes][4]
+    float* out_scores;                  // [n][C * max_boxes]
+    int* out_classes;                   // [n][C * max_boxes]
+    int* out_count;                     // [n]
+    float anchors[18];                  // (w, h) x 9
+    int gh0, gw0, C, NC, max_boxes;
+    float in_h, in_w;                   // model input size
+    float img_h, img_w;                 // original image size
+    float off_y, off_x, scale_y, scale_x;   // yolo_correct_boxes (model.py:159-161), float32 on the host
+    float score, iou;
+};
+
+// launchers (inst_yolo.cu); each returns 0 or the CUDA error of the launch
+struct LetterboxPlan {
+    int H, W;                // source frame
+    int nw, nh, ox, oy;      // resized size and paste offset on the S_h x S_w canvas
+    int y0, rows;            // source rows the vertical pass reads (Pillow's ybox)
+    int ksx, ksy;            // coefficients per output column / row
+    const int2* xb;          // [nw] (xmin, count)
+    const int* kx;           // [nw][ksx]
+    const int2* yb;          // [nh] (first row relative to y0, count)
+    const int* ky;           // [nh][ksy]
+};
+int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb);
+int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w);
+int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m);
+int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n);
+
+#ifndef WHENET_YOLO_HOST_ONLY
+// ----------------------------------------------------------------------------- letterbox
+constexpr int kPrecisionBits = 22;          // Pillow Resample.c PRECISION_BITS (32 - 8 - 2)
+
+__device__ __forceinline__ uint8_t clip8(int v) {
+    if (v >= (1 << kPrecisionBits << 8)) return 255;
+    if (v <= 0) return 0;
+    return (uint8_t)(v >> kPrecisionBits);
+}
+
+// Horizontal pass: rows [y0, y0 + rows) of every frame, W -> nw columns.  in: n x H x W x 3 (BGR when swap_rb), tmp: n x rows x nw x 3.
+// xb = (xmin, count) per output column, kx = ksize int32 coefficients per output column.
+__global__ void letterbox_h_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ tmp, int H, int W, int nw, int y0, int rows,
+                                   const int2* __restrict__ xb, const int* __restrict__ kx, int ksize, int swap_rb) {
+    const int f = blockIdx.y;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)rows * nw) return;
+    const int r = (int)(i / nw), x = (int)(i - (long long)r * nw);
+    const int2 b = xb[x];
+    const int* k = kx + (long long)x * ksize;
+    const uint8_t* src = in + (((long long)f * H + y0 + r) * W + b.x) * 3;
+    int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+    for (int j = 0; j < b.y; ++j) {
+        const int w = k[j];
+        s0 += src[3 * j] * w;
+        s1 += src[3 * j + 1] * w;
+        s2 += src[3 * j + 2] * w;
+    }
+    uint8_t* dst = tmp + (((long long)f * rows + r) * nw + x) * 3;
+    dst[0] = clip8(swap_rb ? s2 : s0);
+    dst[1] = clip8(s1);
+    dst[2] = clip8(swap_rb ? s0 : s2);
+}
+
+// Vertical pass + canvas: every pixel of the S_h x S_w canvas; inside the pasted nw x nh image at (ox, oy) the vertical sum over tmp
+// rows yb = (first row relative to tmp, count), elsewhere 128.
+__global__ void letterbox_v_kernel(const uint8_t* __restrict__ tmp, uint8_t* __restrict__ out, int nw, int nh, int rows, int S_h, int S_w,
+                                   int ox, int oy, const int2* __restrict__ yb, const int* __restrict__ ky, int ksize) {
+    const int f = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= S_h * S_w) return;
+    const int y = i / S_w, x = i - y * S_w;
+    uint8_t* dst = out + ((long long)f * S_h * S_w + i) * 3;
+    const int yy = y - oy, xx = x - ox;
+    if (yy < 0 || yy >= nh || xx < 0 || xx >= nw) {
+        dst[0] = dst[1] = dst[2] = 128;
+        return;
+    }
+    const int2 b = yb[yy];
+    const int* k = ky + (long long)yy * ksize;
+    const uint8_t* src = tmp + (((long long)f * rows + b.x) * nw + xx) * 3;
+    int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+    for (int j = 0; j < b.y; ++j) {
+        const int w = k[j];
+        const uint8_t* p = src + (long long)j * nw * 3;
+        s0 += p[0] * w;
+        s1 += p[1] * w;
+        s2 += p[2] * w;
+    }
+    dst[0] = clip8(s0);
+    dst[1] = clip8(s1);
+    dst[2] = clip8(s2);
+}
+
+// ----------------------------------------------------------------------------- shared epilogue pieces
+__device__ __forceinline__ float leaky(float x) { return x > 0.f ? x : 0.1f * x; }
+
+// ----------------------------------------------------------------------------- first conv
+// 128 consecutive output pixels per CTA (S_h * S_w is a multiple of 1024: a tile never straddles frames).  A row = 27 taps
+// (ky, kx, ci) of v/255 as bf16 hi (K 0..26) and bf16 lo (K 32..58); B row n = [w | 0 | w | 0] (w0: 32 x 64 bf16, packed by the host).
+__global__ void __launch_bounds__(128) yolo_conv0_kernel(const uint8_t* __restrict__ img, const __nv_bfloat16* __restrict__ w0,
+                                                         const float* __restrict__ bias, __nv_bfloat16* __restrict__ out, int S_h, int S_w) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    const uint32_t sA = smem0;                      // 128 rows x 128 B
+    const uint32_t sW = sA + 128 * 128;             // 32 rows x 128 B
+    const uint32_t sL = sW + 32 * 128;              // 256 x u32 (hi | lo << 16)
+    const uint32_t sAcc = sL + 256 * 4;             // accumulator tile, 32 columns
+    const int tid = threadIdx.x;
+    for (int i = tid; i < 256; i += 128) {
+        const float f = (float)i / 255.0f;          // float32(v / 255.), as np.array(.., 'float32') / 255. (yolo_postprocess.py:191-195)
+        const __nv_bfloat16 hi = __float2bfloat16_rn(f), lo = __float2bfloat16_rn(f - __bfloat162float(hi));
+        const uint32_t w = (uint32_t)__bfloat16_as_ushort(hi) | ((uint32_t)__bfloat16_as_ushort(lo) << 16);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sL + (uint32_t)i * 4u), "r"(w) : "memory");
+    }
+    for (int i = tid; i < 32 * 8; i += 128) {
+        const int r = i >> 3, c = i & 7;
+        tc::sts128_(sW + (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4)),
+                    *reinterpret_cast<const uint4*>(w0 + r * 64 + c * 8));
+    }
+    __syncthreads();
+    const long long m = (long long)blockIdx.x * 128 + tid;
+    const int hw = S_h * S_w;
+    const int f = (int)(m / hw), p = (int)(m - (long long)f * hw);
+    const int y = p / S_w, x = p - y * S_w;
+    uint32_t hi[16], lo[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) { hi[j] = 0u; lo[j] = 0u; }
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) {
+            const int iy = y + ky - 1, ix = x + kx - 1;
+            const bool ok = iy >= 0 && iy < S_h && ix >= 0 && ix < S_w;
+            const uint8_t* src = img + (((long long)f * S_h + (ok ? iy : 0)) * S_w + (ok ? ix : 0)) * 3;
+#pragma unroll
+            for (int ci = 0; ci < 3; ++ci) {
+                const int k = (ky * 3 + kx) * 3 + ci;
+                uint32_t w;
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(sL + (uint32_t)src[ci] * 4u));
+                w = ok ? w : 0u;
+                if ((k & 1) == 0) { hi[k >> 1] = w & 0xffffu; lo[k >> 1] = w >> 16; }
+                else { hi[k >> 1] |= w << 16; lo[k >> 1] |= w & 0xffff0000u; }
+            }
+        }
+    const uint32_t a0 = sA + (uint32_t)((tid >> 3) * 1024 + (tid & 7) * 128);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        tc::sts128_(a0 + (uint32_t)((c ^ (tid & 7)) << 4), make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]));
+        tc::sts128_(a0 + (uint32_t)(((c + 4) ^ (tid & 7)) << 4), make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]));
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    tc::WgAcc<32> acc;
+    tc::wg_mma_tile<true, 32>(acc, sA, sW, 4, 0u);
+    tc::wg_wait<0>();
+    tc::wg_acc_store<32>(acc, sAcc, tid);
+    __syncthreads();
+    __nv_bfloat16* dst = out + m * 32;
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+        float v[16];
+        tc::acc_ld16(sAcc, tid, u * 16, v);
+        float o[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) o[j] = leaky(v[j] + bias[u * 16 + j]);
+        float a[8], b[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { a[j] = o[j]; b[j] = o[8 + j]; }
+        st8<__nv_bfloat16>(dst + u * 16, a);
+        st8<__nv_bfloat16>(dst + u * 16 + 8, b);
+    }
+}
+
+// ----------------------------------------------------------------------------- implicit-GEMM conv
+// one 128-pixel x UN-column output tile per CTA; K blocks = (tap, 64-channel chunk) through an n_stages cp.async ring, one wgmma
+// commit group per block (the pw_tc2 pipeline)
+template <int MODE, int UN>
+__global__ void __launch_bounds__(128) conv_igemm_kernel(const __grid_constant__ IgemmParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    const int tid = threadIdx.x;
+    const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    constexpr uint32_t w_stage_bytes = UN * BK * 2;
+    constexpr uint32_t stage_bytes = tc::A_STAGE_BYTES + w_stage_bytes;
+    const int m0 = blockIdx.y * BM;
+    const int n0 = blockIdx.x * p.n_tile;
+    const int n_valid = min(p.n_tile, p.N - n0);
+    const int cchunks = (p.Cin + BK - 1) / BK;
+    const int nkb = p.k * p.k * cchunks;
+    const int K = p.k * p.k * p.Cin;
+    const int pad = p.k >> 1;
+    const int hw = p.Ho * p.Wo;
+
+    // this thread's 8 A rows (r0 + 16 i) and its 16-byte chunk c: frame row base and top-left input coordinate
+    const int c = tid & 7, r0 = tid >> 3;
+    int rbase[8], iy0[8], ix0[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int m = m0 + r0 + 16 * i;
+        if (m < p.M) {
+            const int f = m / hw, q = m - f * hw;
+            const int oy = q / p.Wo, ox = q - oy * p.Wo;
+            rbase[i] = f * p.Hi;
+            iy0[i] = oy * p.stride - pad;
+            ix0[i] = ox * p.stride - pad;
+        } else {
+            rbase[i] = 0;
+            iy0[i] = -(1 << 20);
+            ix0[i] = 0;
+        }
+    }
+    const uint32_t swz = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + ((c ^ (r0 & 7)) << 4));
+
+    auto fill = [&](int kb) {
+        const int s = kb % p.n_stages;
+        const uint32_t a_st = smem0 + s * stage_bytes, w_st = a_st + tc::A_STAGE_BYTES;
+        const int tap = kb / cchunks, cc = kb - tap * cchunks;
+        const int ky = tap / p.k, kx = tap - ky * p.k;
+        const int c0 = cc * BK;
+        const bool cvalid = c0 + c * 8 < p.Cin;
+        // source of this chunk: the skip tensor, or (concat, c0 < c_up) the low-resolution tensor at half the coordinates
+        const bool from_up = MODE == kLeakyCat && c0 < p.c_up;
+        const __nv_bfloat16* src = from_up ? p.up : p.in;
+        const int cs = from_up ? p.c_up : p.Cin - p.c_up;
+        const int sh = from_up ? 1 : 0;
+        const int Ws = p.Wi >> sh;
+        const int ch = (from_up ? c0 : c0 - p.c_up) + c * 8;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int iy = iy0[i] + ky, ix = ix0[i] + kx;
+            const bool valid = cvalid && iy >= 0 && iy < p.Hi && ix >= 0 && ix < p.Wi;
+            const __nv_bfloat16* a = src + ((long long)((rbase[i] + iy) >> sh) * Ws + (ix >> sh)) * cs + ch;
+            cp_async16_z(a_st + swz + i * 2048, valid ? a : p.in, valid);
+        }
+        const __nv_bfloat16* wsrc = p.wt + (long long)(n0 + r0) * K + tap * p.Cin + c0 + c * 8;
+#pragma unroll
+        for (int i = 0; i < UN / 16; ++i) {
+            const bool valid = cvalid && r0 + 16 * i < n_valid;
+            cp_async16_z(w_st + swz + i * 2048, valid ? wsrc + (long long)i * 16 * K : p.wt, valid);
+        }
+    };
+    for (int j = 0; j < p.n_stages; ++j) {
+        if (j < nkb) fill(j);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    }
+    tc::WgAcc<UN> acc;
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % p.n_stages;
+        const uint32_t a_st = smem0 + s * stage_bytes, w_st = a_st + tc::A_STAGE_BYTES;
+        if (p.n_stages >= 4) asm volatile("cp.async.wait_group 2;" ::: "memory");
+        else if (p.n_stages == 3) asm volatile("cp.async.wait_group 1;" ::: "memory");
+        else asm volatile("cp.async.wait_group 0;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();
+        {
+            const int cc = kb % cchunks;
+            const int krem = min(BK, p.Cin - cc * BK);
+            tc::wg_mma_tile<true, UN>(acc, a_st, w_st, (krem + 15) >> 4, kb ? 1u : 0u);
+        }
+        // refill the stage block kb-1 used once its MMAs have completed
+        if (kb >= 1 && kb - 1 + p.n_stages < nkb) {
+            tc::wg_wait<1>();
+            __syncthreads();
+            fill(kb - 1 + p.n_stages);
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    }
+    tc::wg_wait<0>();
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    __syncthreads();
+    const uint32_t sAcc = smem0;
+    tc::wg_acc_store<UN>(acc, sAcc, tid);
+    __syncthreads();
+
+    const int rows_valid = min(BM, p.M - m0);
+    const bool row_ok = tid < rows_valid;
+    const long long m = (long long)m0 + tid;
+    if (MODE == kLinearF32) {      // output convs: bias, no activation, fp32 (any N)
+        float* out = reinterpret_cast<float*>(p.out);
+        if (row_ok)
+            for (int j = 0; j < n_valid; ++j) {
+                float v;
+                asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(sAcc + (uint32_t)(j * tc::kAccPitch + tid) * 4u));
+                out[m * p.N + n0 + j] = v + p.bias[n0 + j];
+            }
+        return;
+    }
+    const int nch = n_valid >> 3;
+    const float inv_nch = 1.0f / (float)(nch > 0 ? nch : 1);
+    const int pitch16 = nch | 1;
+    uint4* stage = reinterpret_cast<uint4*>(smem_raw + (smem0 + tc::acc_tile_bytes(UN) - smem_u32(smem_raw)));
+    for (int c0 = 0; c0 < n_valid; c0 += 16) {
+        float v[16];
+        tc::acc_ld16(sAcc, tid, c0, v);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int n = n0 + c0 + h * 8;
+            if (c0 + h * 8 >= n_valid) break;
+            float o[8];
+            const float4 b0 = *reinterpret_cast<const float4*>(p.bias + n), b1 = *reinterpret_cast<const float4*>(p.bias + n + 4);
+            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+            for (int j = 0; j < 8; ++j) o[j] = leaky(v[h * 8 + j] + bb[j]);
+            if (MODE == kLeakyRes && row_ok) {
+                float r[8];
+                ld8<__nv_bfloat16>(p.resid + m * p.N + n, r);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) o[j] += r[j];
+            }
+            st8<__nv_bfloat16>(reinterpret_cast<__nv_bfloat16*>(stage + tid * pitch16 + ((c0 >> 3) + h)), o);
+        }
+    }
+    __syncthreads();
+    __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
+    for (int idx = tid; idx < rows_valid * nch; idx += 128) {
+        const int r = tc::fdiv_small(idx, inv_nch), j = idx - r * nch;
+        *reinterpret_cast<uint4*>(out + ((long long)m0 + r) * p.N + n0 + j * 8) = stage[r * pitch16 + j];
+    }
+}
+
+// ----------------------------------------------------------------------------- decode + NMS
+__device__ __forceinline__ float sigmoidf_(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
+
+// TF's IoU (non_max_suppression_op.cc): corners via min/max, 0 when either area <= 0
+__device__ __forceinline__ float iou_tf(float4 a, float4 b) {
+    const float aymin = fminf(a.x, a.z), aymax = fmaxf(a.x, a.z), axmin = fminf(a.y, a.w), axmax = fmaxf(a.y, a.w);
+    const float bymin = fminf(b.x, b.z), bymax = fmaxf(b.x, b.z), bxmin = fminf(b.y, b.w), bxmax = fmaxf(b.y, b.w);
+    const float area_a = __fmul_rn(__fsub_rn(aymax, aymin), __fsub_rn(axmax, axmin));
+    const float area_b = __fmul_rn(__fsub_rn(bymax, bymin), __fsub_rn(bxmax, bxmin));
+    if (area_a <= 0.f || area_b <= 0.f) return 0.f;
+    const float iymin = fmaxf(aymin, bymin), ixmin = fmaxf(axmin, bxmin), iymax = fminf(aymax, bymax), ixmax = fminf(axmax, bxmax);
+    const float inter = __fmul_rn(fmaxf(__fsub_rn(iymax, iymin), 0.f), fmaxf(__fsub_rn(ixmax, ixmin), 0.f));
+    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
+}
+
+__global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __grid_constant__ DecodeParams p) {
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int CH = 5 + p.C;
+    float4* cand = p.cand + (long long)f * p.NC;
+    float* cscore = p.cand_score + (long long)f * p.C * p.NC;
+    // ---- decode (model.py:125-187): candidates ordered layer 0, 1, 2, then (y, x, anchor)
+    for (int i = tid; i < p.NC; i += kNmsThreads) {
+        int l = 0, rem = i;
+        int gh = p.gh0, gw = p.gw0;
+        while (rem >= 3 * gh * gw) { rem -= 3 * gh * gw; ++l; gh *= 2; gw *= 2; }
+        const int cell = rem / 3, a = rem - cell * 3;
+        const int y = cell / gw, x = cell - y * gw;
+        const float* t = p.head[l] + (((long long)f * gh + y) * gw + x) * 3 * CH + a * CH;
+        const int an = 3 * (2 - l) + a;                                     // anchor_mask[l] = [[6,7,8],[3,4,5],[0,1,2]][l]
+        const float bx = __fdiv_rn(__fadd_rn(sigmoidf_(t[0]), (float)x), (float)gw);
+        const float by = __fdiv_rn(__fadd_rn(sigmoidf_(t[1]), (float)y), (float)gh);
+        const float bw = __fdiv_rn(__fmul_rn(expf(t[2]), p.anchors[2 * an]), p.in_w);
+        const float bh = __fdiv_rn(__fmul_rn(expf(t[3]), p.anchors[2 * an + 1]), p.in_h);
+        // yolo_correct_boxes (model.py:153-176)
+        const float yc = __fmul_rn(__fsub_rn(by, p.off_y), p.scale_y), xc = __fmul_rn(__fsub_rn(bx, p.off_x), p.scale_x);
+        const float hh = __fmul_rn(bh, p.scale_y), ww = __fmul_rn(bw, p.scale_x);
+        const float hh2 = __fdiv_rn(hh, 2.0f), ww2 = __fdiv_rn(ww, 2.0f);
+        cand[i] = make_float4(__fmul_rn(__fsub_rn(yc, hh2), p.img_h), __fmul_rn(__fsub_rn(xc, ww2), p.img_w),
+                              __fmul_rn(__fadd_rn(yc, hh2), p.img_h), __fmul_rn(__fadd_rn(xc, ww2), p.img_w));
+        const float conf = sigmoidf_(t[4]);
+        for (int c = 0; c < p.C; ++c) cscore[(long long)c * p.NC + i] = __fmul_rn(conf, sigmoidf_(t[5 + c]));
+    }
+    __syncthreads();
+    __shared__ unsigned long long s_red[kNmsThreads / 32];
+    __shared__ unsigned long long s_best;
+    int kept_total = 0;
+    for (int c = 0; c < p.C; ++c) {
+        const float* sc = cscore + (long long)c * p.NC;
+        // alive bit j: candidate tid + j * 1024 passes the class mask (model.py:211: score >= threshold) and is not suppressed yet
+        uint32_t alive = 0u;
+#pragma unroll
+        for (int j = 0; j < kNmsPer; ++j) {
+            const int i = tid + j * kNmsThreads;
+            if (i < p.NC && sc[i] >= p.score) alive |= 1u << j;
+        }
+        // greedy NMS (tf.image.non_max_suppression): the highest remaining score is never suppressed by an already kept box (those
+        // were removed when each was kept), so it is the next box kept; equal scores: lower candidate index first
+        int kept = 0;
+        while (kept < p.max_boxes) {
+            unsigned long long best = 0ull;
+#pragma unroll
+            for (int j = 0; j < kNmsPer; ++j)
+                if (alive & (1u << j)) {
+                    const int i = tid + j * kNmsThreads;
+                    // scores are >= 0: their float bits order like the floats; ~i makes the lower index win a tie
+                    const unsigned long long key = ((unsigned long long)__float_as_uint(sc[i]) << 32) | (unsigned)(~i);
+                    best = key > best ? key : best;
+                }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long v = __shfl_xor_sync(0xffffffffu, best, o);
+                best = v > best ? v : best;
+            }
+            if ((tid & 31) == 0) s_red[tid >> 5] = best;
+            __syncthreads();
+            if (tid < 32) {
+                unsigned long long v = s_red[tid];
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    const unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
+                    v = u > v ? u : v;
+                }
+                if (tid == 0) s_best = v;
+            }
+            __syncthreads();
+            best = s_best;
+            __syncthreads();                                        // s_red / s_best are rewritten by the next round
+            if (best == 0ull) break;
+            const int bi = (int)(~(unsigned)(best & 0xffffffffu));
+            const float4 bb = cand[bi];
+            if (tid == 0) {
+                const long long o = (long long)f * p.C * p.max_boxes + kept_total + kept;
+                reinterpret_cast<float4*>(p.out_boxes)[o] = bb;
+                p.out_scores[o] = __uint_as_float((unsigned)(best >> 32));
+                p.out_classes[o] = c;
+            }
+#pragma unroll
+            for (int j = 0; j < kNmsPer; ++j)
+                if (alive & (1u << j)) {
+                    const int i = tid + j * kNmsThreads;
+                    if (i == bi || iou_tf(cand[i], bb) > p.iou) alive &= ~(1u << j);
+                }
+            ++kept;
+        }
+        kept_total += kept;
+    }
+    if (tid == 0) p.out_count[f] = kept_total;
+}
+
+#endif  // WHENET_YOLO_HOST_ONLY
+}  // namespace yolo
+}  // namespace whenet

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/whenet_b200.h"
+#include "api_error.h"
 #include "kernels_simt.cuh"
 #include "kernels_tc.cuh"
 #include "kernels_fused.cuh"
@@ -56,15 +57,8 @@ WHENET_EXTERN_PW(__half)
 
 namespace {
 
-thread_local char g_err[512] = "";
-
-int fail(int code, const char* fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
+using whenet::api::fail;
+using whenet::api::g_err;
 
 #define CK(call)                                                                                   \
     do {                                                                                           \

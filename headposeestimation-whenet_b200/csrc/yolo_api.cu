@@ -1,0 +1,553 @@
+// yolo_api.cu - C ABI of the YOLOv3 head detector (whenet_det_*): weights, workspaces, the captured forward, decode + NMS.
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <initializer_list>
+#include <map>
+#include <string>
+#include <tuple>
+#include <vector>
+
+#include "../../include/whenet_b200.h"
+#include "api_error.h"
+#define WHENET_YOLO_HOST_ONLY
+#include "kernels_yolo.cuh"
+
+using whenet::api::fail;
+namespace Y = whenet::yolo;
+
+#define CKD(call)                                                                                  \
+    do {                                                                                           \
+        cudaError_t e__ = (call);                                                                  \
+        if (e__ != cudaSuccess)                                                                    \
+            return fail(WHENET_ECUDA, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,         \
+                        cudaGetErrorString(e__));                                                  \
+    } while (0)
+
+namespace {
+
+constexpr double kBnEps = 1e-3;     // keras BatchNormalization default (reference yolo_v3/model.py:34)
+
+// The 75 convolutions in Keras weight order; the python twin (and the documentation of every field) is yolo_arch.py.
+struct ConvCfg { int k, stride, cin, cout, src, res, up; bool bn; int head; };
+
+std::vector<ConvCfg> make_table() {
+    std::vector<ConvCfg> v;
+    auto add = [&](int k, int s, int cin, int cout, int src, bool bn = true, int res = -1, int up = -1, int head = -1) {
+        v.push_back(ConvCfg{k, s, cin, cout, src, res, up, bn, head});
+        return (int)v.size() - 1;
+    };
+    int x = add(3, 1, 3, 32, -1), c = 32;
+    int skip256 = -1, skip512 = -1;
+    const int nfs[5] = {64, 128, 256, 512, 1024}, nbs[5] = {1, 2, 8, 8, 4};
+    for (int b = 0; b < 5; ++b) {
+        x = add(3, 2, c, nfs[b], x);
+        for (int i = 0; i < nbs[b]; ++i) {
+            const int y = add(1, 1, nfs[b], nfs[b] / 2, x);
+            x = add(3, 1, nfs[b] / 2, nfs[b], y, true, x);
+        }
+        c = nfs[b];
+        if (c == 256) skip256 = x;
+        if (c == 512) skip512 = x;
+    }
+    int last5[3];
+    auto five = [&](int x, int cin, int nf, int up, int h) {
+        x = add(1, 1, cin, nf, x, true, -1, up);
+        for (int i = 0; i < 2; ++i) {
+            x = add(3, 1, nf, 2 * nf, x);
+            x = add(1, 1, 2 * nf, nf, x);
+        }
+        last5[h] = x;
+        return x;
+    };
+    x = five(x, 1024, 512, -1, 0);
+    int u = add(1, 1, 512, 256, x);
+    x = five(skip512, 256 + 512, 256, u, 1);
+    u = add(1, 1, 256, 128, x);
+    five(skip256, 128 + 256, 128, u, 2);
+    int y3[3];
+    const int nf3[3] = {512, 256, 128};
+    for (int h = 0; h < 3; ++h) y3[h] = add(3, 1, nf3[h], 2 * nf3[h], last5[h]);
+    for (int h = 0; h < 3; ++h) add(1, 1, 2 * nf3[h], 0, y3[h], false, -1, -1, h);
+    return v;
+}
+
+uint16_t bf16_bits(float f) {      // round to nearest even (finite inputs)
+    uint32_t u;
+    std::memcpy(&u, &f, 4);
+    u += 0x7FFFu + ((u >> 16) & 1u);
+    return (uint16_t)(u >> 16);
+}
+
+struct LayerDev { int Hi, Wi, Ho, Wo, N; Y::IgemmPlan plan; void* out = nullptr; };
+
+struct GraphEntry {
+    cudaGraphExec_t exec = nullptr;
+    void* coef = nullptr;           // letterbox tables (xb, kx, yb, ky) in one allocation
+    uint8_t* tmp = nullptr;         // horizontal-pass output
+};
+
+// Pillow ImagingResample (libImaging/Resample.c) coefficient tables for BICUBIC: support 2 scaled by the downscale factor,
+// weights normalised in double and quantised to 22 bits (normalize_coeffs_8bpc).
+double bicubic(double x) {
+    const double a = -0.5;
+    if (x < 0.0) x = -x;
+    if (x < 1.0) return ((a + 2.0) * x - (a + 3.0)) * x * x + 1;
+    if (x < 2.0) return (((x - 5) * x + 8) * x - 4) * a;
+    return 0.0;
+}
+int precompute_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<int>& kk) {
+    const double scale = (double)(float)in_size / out_size;
+    const double filterscale = scale < 1.0 ? 1.0 : scale;
+    const double support = 2.0 * filterscale;
+    const int ksize = (int)std::ceil(support) * 2 + 1;
+    bounds.assign(2 * out_size, 0);
+    kk.assign((size_t)out_size * ksize, 0);
+    std::vector<double> k(ksize);
+    for (int xx = 0; xx < out_size; ++xx) {
+        const double center = (xx + 0.5) * scale;
+        double ww = 0.0;
+        const double ss = 1.0 / filterscale;
+        int xmin = (int)(center - support + 0.5);
+        if (xmin < 0) xmin = 0;
+        int xmax = (int)(center + support + 0.5);
+        if (xmax > in_size) xmax = in_size;
+        xmax -= xmin;
+        for (int x = 0; x < xmax; ++x) {
+            const double w = bicubic((x + xmin - center + 0.5) * ss);
+            k[x] = w;
+            ww += w;
+        }
+        for (int x = 0; x < xmax; ++x)
+            if (ww != 0.0) k[x] /= ww;
+        for (int x = 0; x < ksize; ++x) {
+            const double v = x < xmax ? k[x] : 0.0;
+            kk[(size_t)xx * ksize + x] = v < 0 ? (int)(-0.5 + v * (1 << 22)) : (int)(0.5 + v * (1 << 22));
+        }
+        bounds[2 * xx] = xmin;
+        bounds[2 * xx + 1] = xmax;
+    }
+    return ksize;
+}
+
+}  // namespace
+
+struct whenet_det {
+    int device = 0, in_h = 0, in_w = 0, max_frames = 0, sm_count = 132;
+    int num_classes = 0;
+    bool loaded = false;
+    cudaStream_t own_stream = nullptr, stream = nullptr, cap_stream = nullptr;
+    std::vector<ConvCfg> table;
+    std::vector<LayerDev> L;
+    void* warena = nullptr;             // bf16 kernels, [N][K] each, 256-byte aligned
+    float* barena = nullptr;            // fp32 biases
+    std::vector<size_t> w_off, b_off;
+    float anchors[18] = {};
+    uint8_t* d_frames = nullptr; size_t frames_cap = 0;
+    uint8_t* d_canvas = nullptr;
+    float4* d_cand = nullptr; float* d_cand_score = nullptr;
+    float* d_boxes = nullptr; float* d_scores = nullptr; int* d_classes = nullptr; int* d_count = nullptr;
+    std::map<std::tuple<int, int, int>, GraphEntry> graphs;
+    int last_n = 0;
+};
+
+namespace {
+
+int ncand(const whenet_det* d) { return 3 * (d->in_h / 32) * (d->in_w / 32) * 21; }    // 1 + 4 + 16 cells per 32x32 block
+
+void free_graphs(whenet_det* d) {
+    for (auto& kv : d->graphs) {
+        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+        cudaFree(kv.second.coef);
+        cudaFree(kv.second.tmp);
+    }
+    d->graphs.clear();
+}
+
+const __nv_bfloat16* bf(const whenet_det* d, size_t off) { return reinterpret_cast<const __nv_bfloat16*>((const char*)d->warena + off); }
+
+// enqueue one conv (layers 1..74) on stream s, n frames
+int enqueue_conv(whenet_det* d, cudaStream_t s, int i, int n) {
+    const ConvCfg& c = d->table[i];
+    const LayerDev& l = d->L[i];
+    Y::IgemmParams p{};
+    const int N = l.N;
+    p.in = reinterpret_cast<const __nv_bfloat16*>(d->L[c.src].out);
+    p.up = c.up >= 0 ? reinterpret_cast<const __nv_bfloat16*>(d->L[c.up].out) : nullptr;
+    p.wt = bf(d, d->w_off[i]);
+    p.bias = d->barena + d->b_off[i];
+    p.resid = c.res >= 0 ? reinterpret_cast<const __nv_bfloat16*>(d->L[c.res].out) : nullptr;
+    p.out = l.out;
+    p.M = n * l.Ho * l.Wo; p.Hi = l.Hi; p.Wi = l.Wi; p.Ho = l.Ho; p.Wo = l.Wo;
+    p.Cin = c.cin; p.c_up = c.up >= 0 ? d->table[c.up].cout : 0; p.N = N; p.k = c.k; p.stride = c.stride;
+    p.n_tile = l.plan.n_tile; p.n_stages = l.plan.n_stages;
+    const int mode = c.head >= 0 ? Y::kLinearF32 : c.up >= 0 ? Y::kLeakyCat : c.res >= 0 ? Y::kLeakyRes : Y::kLeaky;
+    const int rc = Y::launch_igemm(s, p, mode, l.plan.un, l.plan.smem, (N + l.plan.n_tile - 1) / l.plan.n_tile, (p.M + Y::BM - 1) / Y::BM);
+    if (rc) return fail(WHENET_ECUDA, "conv %d launch failed: %s", i, cudaGetErrorString((cudaError_t)rc));
+    return 0;
+}
+
+int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
+    // letterbox geometry (reference utils.py:25-33): scale in float64, int() truncation, paste at the floor-halved offsets
+    const double scale = std::min((double)d->in_w / W, (double)d->in_h / H);
+    const int nw = (int)(W * scale), nh = (int)(H * scale);
+    if (nw < 1 || nh < 1) return fail(WHENET_EINVAL, "a %dx%d frame letterboxes to an empty %dx%d image", W, H, nw, nh);
+    std::vector<int> xb, kx, yb, ky;
+    const int ksx = precompute_coeffs(W, nw, xb, kx), ksy = precompute_coeffs(H, nh, yb, ky);
+    const int y0 = yb[0], rows = yb[2 * (nh - 1)] + yb[2 * nh - 1] - y0;      // Pillow's ybox_first / ybox_last
+    for (int y = 0; y < nh; ++y) yb[2 * y] -= y0;
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };      // each table 256-byte aligned (int2 loads)
+    const size_t b_xb = al(xb.size() * 4), b_kx = al(kx.size() * 4), b_yb = al(yb.size() * 4), b_ky = al(ky.size() * 4);
+    CKD(cudaMalloc(&e->coef, b_xb + b_kx + b_yb + b_ky));
+    char* base = (char*)e->coef;
+    CKD(cudaMemcpy(base, xb.data(), xb.size() * 4, cudaMemcpyHostToDevice));
+    CKD(cudaMemcpy(base + b_xb, kx.data(), kx.size() * 4, cudaMemcpyHostToDevice));
+    CKD(cudaMemcpy(base + b_xb + b_kx, yb.data(), yb.size() * 4, cudaMemcpyHostToDevice));
+    CKD(cudaMemcpy(base + b_xb + b_kx + b_yb, ky.data(), ky.size() * 4, cudaMemcpyHostToDevice));
+    CKD(cudaMalloc(&e->tmp, (size_t)n * rows * nw * 3));
+    Y::LetterboxPlan lp{H, W, nw, nh, (d->in_w - nw) / 2, (d->in_h - nh) / 2, y0, rows, ksx, ksy,
+                        (const int2*)base, (const int*)(base + b_xb), (const int2*)(base + b_xb + b_kx), (const int*)(base + b_xb + b_kx + b_yb)};
+    // the whole body as one graph, captured on the context's private stream
+    cudaStream_t s = d->cap_stream;
+    CKD(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
+    int rc = Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb);
+    if (!rc) rc = Y::launch_conv0(s, d->d_canvas, bf(d, d->w_off[0]), d->barena + d->b_off[0], (__nv_bfloat16*)d->L[0].out, n, d->in_h, d->in_w);
+    int rc2 = rc ? fail(WHENET_ECUDA, "letterbox / first conv launch failed: %s", cudaGetErrorString((cudaError_t)rc)) : 0;
+    for (size_t i = 1; i < d->table.size() && !rc2; ++i) rc2 = enqueue_conv(d, s, (int)i, n);
+    cudaGraph_t g = nullptr;
+    const cudaError_t ee = cudaStreamEndCapture(s, &g);
+    if (rc2) { if (g) cudaGraphDestroy(g); return rc2; }
+    CKD(ee);
+    const cudaError_t ie = cudaGraphInstantiate(&e->exec, g, 0);
+    cudaGraphDestroy(g);
+    CKD(ie);
+    return 0;
+}
+
+int check_frames(const whenet_det* d, int n, int H, int W) {
+    if (n < 1 || n > d->max_frames) return fail(WHENET_EINVAL, "n=%d outside [1, max_frames=%d]", n, d->max_frames);
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    return 0;
+}
+
+// DecodeParams of one call: yolo_correct_boxes' float32 arithmetic (model.py:157-161) on the host
+Y::DecodeParams decode_params(const whenet_det* d, int img_h, int img_w, float score, float iou, int max_boxes) {
+    Y::DecodeParams p{};
+    p.cand = d->d_cand; p.cand_score = d->d_cand_score;
+    p.out_boxes = d->d_boxes; p.out_scores = d->d_scores; p.out_classes = d->d_classes; p.out_count = d->d_count;
+    std::memcpy(p.anchors, d->anchors, sizeof(p.anchors));
+    p.gh0 = d->in_h / 32; p.gw0 = d->in_w / 32; p.C = d->num_classes; p.NC = ncand(d); p.max_boxes = max_boxes;
+    p.in_h = (float)d->in_h; p.in_w = (float)d->in_w; p.img_h = (float)img_h; p.img_w = (float)img_w;
+    const float m = std::min(p.in_h / p.img_h, p.in_w / p.img_w);
+    const float nh = std::nearbyint(p.img_h * m), nw = std::nearbyint(p.img_w * m);       // K.round: half to even
+    p.off_y = (p.in_h - nh) / 2.0f / p.in_h; p.off_x = (p.in_w - nw) / 2.0f / p.in_w;
+    p.scale_y = p.in_h / nh; p.scale_x = p.in_w / nw;
+    p.score = score; p.iou = iou;
+    for (int l = 0; l < 3; ++l) p.head[l] = (const float*)d->L[d->table.size() - 3 + l].out;
+    return p;
+}
+
+int run_decode(whenet_det* d, const Y::DecodeParams& p, int n, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    const int rc = Y::launch_decode_nms(d->stream, p, n);
+    if (rc) return fail(WHENET_ECUDA, "decode/NMS launch failed: %s", cudaGetErrorString((cudaError_t)rc));
+    const size_t slots = (size_t)n * p.C * p.max_boxes;
+    CKD(cudaMemcpyAsync(boxes, d->d_boxes, slots * 16, cudaMemcpyDeviceToHost, d->stream));
+    CKD(cudaMemcpyAsync(scores, d->d_scores, slots * 4, cudaMemcpyDeviceToHost, d->stream));
+    CKD(cudaMemcpyAsync(classes, d->d_classes, slots * 4, cudaMemcpyDeviceToHost, d->stream));
+    CKD(cudaMemcpyAsync(counts, d->d_count, (size_t)n * 4, cudaMemcpyDeviceToHost, d->stream));
+    CKD(cudaStreamSynchronize(d->stream));
+    return 0;
+}
+
+int check_decode_args(const whenet_det* d, float score, float iou, int max_boxes, const void* boxes, const void* scores, const void* classes,
+                      const void* counts) {
+    if (!d->loaded) return fail(WHENET_ENOWEIGHTS, "whenet_det_load_weights has not been called");
+    if (!boxes || !scores || !classes || !counts) return fail(WHENET_EINVAL, "null output pointer");
+    if (max_boxes < 1 || max_boxes > Y::kMaxBoxes) return fail(WHENET_EINVAL, "max_boxes=%d outside [1, %d]", max_boxes, Y::kMaxBoxes);
+    if (!(score >= 0.f && score <= 1.f) || !(iou >= 0.f && iou <= 1.f)) return fail(WHENET_EINVAL, "score / iou thresholds must be in [0, 1]");
+    return 0;
+}
+
+int to_f32_tap(const void* src, bool is_f32, size_t n, float* out) {
+    if (is_f32) { CKD(cudaMemcpy(out, src, n * 4, cudaMemcpyDeviceToHost)); return 0; }
+    std::vector<uint16_t> h(n);
+    CKD(cudaMemcpy(h.data(), src, n * 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; ++i) { const uint32_t u = (uint32_t)h[i] << 16; std::memcpy(out + i, &u, 4); }
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, int max_frames) {
+    if (!out) return fail(WHENET_EINVAL, "out is NULL");
+    *out = nullptr;
+    for (int v : {input_h, input_w})
+        if (v < 32 || v > 608 || v % 32) return fail(WHENET_EINVAL, "input size %dx%d: both must be multiples of 32 in [32, 608]", input_w, input_h);
+    if (max_frames < 1 || max_frames > 64) return fail(WHENET_EINVAL, "max_frames=%d outside [1, 64]", max_frames);
+    int ndev = 0;
+    CKD(cudaGetDeviceCount(&ndev));
+    if (device < 0 || device >= ndev) return fail(WHENET_EINVAL, "device %d not in [0,%d)", device, ndev);
+    CKD(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    CKD(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(WHENET_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
+    whenet_det* d = new whenet_det();
+    d->device = device; d->in_h = input_h; d->in_w = input_w; d->max_frames = max_frames; d->sm_count = prop.multiProcessorCount;
+    d->table = make_table();
+    d->L.resize(d->table.size());
+    auto bail = [&](int rc) { whenet_det_destroy(d); return rc; };
+    if (cudaStreamCreateWithFlags(&d->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&d->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
+        return bail(fail(WHENET_ECUDA, "stream creation failed"));
+    d->stream = d->own_stream;
+    if (cudaMalloc(&d->d_canvas, (size_t)max_frames * input_h * input_w * 3) != cudaSuccess)
+        return bail(fail(WHENET_ECUDA, "out of device memory (canvas)"));
+    *out = d;
+    return 0;
+}
+
+int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors, const float* anchors, int n_anchors) {
+    if (!d || !t || !anchors) return fail(WHENET_EINVAL, "bad arguments");
+    if (n_anchors != 9) return fail(WHENET_EINVAL, "YOLOv3 needs 9 anchors, got %d", n_anchors);
+    const std::vector<ConvCfg>& T = d->table;
+    // tensors in table order: kernel [k,k,cin,cout], then gamma, beta, moving_mean, moving_variance (BN convs) or bias (output convs)
+    size_t need = 0;
+    for (const ConvCfg& c : T) need += c.bn ? 5 : 2;
+    if ((size_t)n_tensors != need) return fail(WHENET_ESHAPE, "expected %zu tensors (75 convs + BatchNorms), got %d", need, n_tensors);
+    const whenet_tensor& h0 = t[need - 2];      // output conv of head 2 (its kernel), all heads have the same width
+    if (h0.ndim != 4 || h0.dims[3] < 18 || h0.dims[3] % 3) return fail(WHENET_ESHAPE, "%s: output conv width is not 3 * (5 + classes)", h0.name ? h0.name : "?");
+    const int C = (int)h0.dims[3] / 3 - 5;
+    std::vector<uint16_t> hw;
+    std::vector<float> hb;
+    std::vector<size_t> w_off, b_off;
+    size_t ti = 0;
+    for (size_t i = 0; i < T.size(); ++i) {
+        const ConvCfg& c = T[i];
+        const int co = c.head >= 0 ? 3 * (5 + C) : c.cout;
+        const whenet_tensor& k = t[ti++];
+        const char* kn = k.name ? k.name : "?";
+        if (k.ndim != 4 || k.dims[0] != c.k || k.dims[1] != c.k || k.dims[2] != c.cin || k.dims[3] != co)
+            return fail(WHENET_ESHAPE, "%s (conv %zu): kernel must be [%d,%d,%d,%d]", kn, i, c.k, c.k, c.cin, co);
+        std::vector<double> scale(co, 1.0), shift(co, 0.0);
+        if (c.bn) {
+            const whenet_tensor* bn[4] = {&t[ti], &t[ti + 1], &t[ti + 2], &t[ti + 3]};
+            ti += 4;
+            for (auto* b : bn)
+                if (b->ndim != 1 || b->dims[0] != co) return fail(WHENET_ESHAPE, "%s (BatchNorm of conv %zu): must be [%d]", b->name ? b->name : "?", i, co);
+            for (int o = 0; o < co; ++o) {
+                scale[o] = (double)bn[0]->data[o] / std::sqrt((double)bn[3]->data[o] + kBnEps);
+                shift[o] = (double)bn[1]->data[o] - (double)bn[2]->data[o] * scale[o];
+            }
+        } else {
+            const whenet_tensor& b = t[ti++];
+            if (b.ndim != 1 || b.dims[0] != co) return fail(WHENET_ESHAPE, "%s (output conv %zu): bias must be [%d]", b.name ? b.name : "?", i, co);
+            for (int o = 0; o < co; ++o) shift[o] = b.data[o];
+        }
+        // kernel -> [N][K] bf16 (K = (ky*k + kx)*cin + ci); conv 0 -> [32][64] = [w(27) 0(5) w(27) 0(5)] for the hi/lo input split
+        const int taps = c.k * c.k;
+        const int N = co, K = i == 0 ? 64 : taps * c.cin;
+        const int rows = (N + 127) / 128 * 128;     // every weight tile the kernels may touch exists (zero rows past N)
+        w_off.push_back(hw.size() * 2);
+        hw.resize(hw.size() + (size_t)rows * K + 128, 0);
+        uint16_t* dst = hw.data() + w_off.back() / 2;
+        for (int o = 0; o < N; ++o)
+            for (int tp = 0; tp < taps; ++tp)
+                for (int ci = 0; ci < c.cin; ++ci) {
+                    const uint16_t v = bf16_bits((float)((double)k.data[((size_t)tp * c.cin + ci) * co + o] * scale[o]));
+                    if (i == 0) { dst[(size_t)o * K + tp * 3 + ci] = v; dst[(size_t)o * K + 32 + tp * 3 + ci] = v; }
+                    else dst[(size_t)o * K + (size_t)tp * c.cin + ci] = v;
+                }
+        b_off.push_back(hb.size());
+        hb.resize(hb.size() + (size_t)(N + 127) / 128 * 128, 0.f);
+        for (int o = 0; o < N; ++o) hb[b_off.back() + o] = (float)shift[o];
+    }
+    CKD(cudaSetDevice(d->device));
+    CKD(cudaStreamSynchronize(d->stream));
+    free_graphs(d);
+    cudaFree(d->warena); cudaFree(d->barena);
+    d->warena = nullptr; d->barena = nullptr; d->loaded = false;
+    CKD(cudaMalloc(&d->warena, hw.size() * 2));
+    CKD(cudaMalloc(&d->barena, hb.size() * 4));
+    CKD(cudaMemcpy(d->warena, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice));
+    CKD(cudaMemcpy(d->barena, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
+    d->w_off = w_off; d->b_off = b_off;
+    std::memcpy(d->anchors, anchors, sizeof(d->anchors));
+    // activations: one buffer per conv output (the concat and residual sources and the taps stay addressable), workspaces
+    if (C != d->num_classes || !d->L[0].out) {
+        for (auto& l : d->L) { cudaFree(l.out); l.out = nullptr; }
+        cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
+        d->num_classes = C;
+        for (size_t i = 0; i < T.size(); ++i) {
+            const ConvCfg& c = T[i];
+            LayerDev& l = d->L[i];
+            l.Hi = c.src < 0 ? d->in_h : d->L[c.src].Ho;
+            l.Wi = c.src < 0 ? d->in_w : d->L[c.src].Wo;
+            l.Ho = l.Hi / c.stride; l.Wo = l.Wi / c.stride;
+            l.N = c.head >= 0 ? 3 * (5 + C) : c.cout;
+            l.plan = Y::plan_igemm(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
+            CKD(cudaMalloc(&l.out, (size_t)d->max_frames * l.Ho * l.Wo * l.N * (c.head >= 0 ? 4 : 2)));
+        }
+        const size_t nc = (size_t)ncand(d), slots = (size_t)d->max_frames * C * Y::kMaxBoxes;
+        CKD(cudaMalloc(&d->d_cand, (size_t)d->max_frames * nc * 16));
+        CKD(cudaMalloc(&d->d_cand_score, (size_t)d->max_frames * C * nc * 4));
+        CKD(cudaMalloc(&d->d_boxes, slots * 16));
+        CKD(cudaMalloc(&d->d_scores, slots * 4));
+        CKD(cudaMalloc(&d->d_classes, slots * 4));
+        CKD(cudaMalloc(&d->d_count, (size_t)d->max_frames * 4));
+    }
+    d->loaded = true;
+    return 0;
+}
+
+int whenet_det_num_classes(whenet_det* d) { return d ? d->num_classes : 0; }
+
+int whenet_det_set_stream(whenet_det* d, void* s) {
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    d->stream = s ? (cudaStream_t)s : d->own_stream;
+    return 0;
+}
+
+int whenet_det_detect_u8(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb, float score, float iou,
+                         int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    if (!d || !frames) return fail(WHENET_EINVAL, "null detector or frames");
+    if (int rc = check_frames(d, n, H, W)) return rc;
+    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+    CKD(cudaSetDevice(d->device));
+    // frames -> the context's input buffer (the captured graph reads a fixed address); RGB order there
+    const size_t bytes = (size_t)n * H * W * 3;
+    if (d->frames_cap < bytes) {
+        CKD(cudaStreamSynchronize(d->stream));
+        cudaFree(d->d_frames);
+        d->d_frames = nullptr; d->frames_cap = 0;
+        free_graphs(d);                         // they captured the old buffer
+        CKD(cudaMalloc(&d->d_frames, bytes));
+        d->frames_cap = bytes;
+    }
+    CKD(cudaMemcpyAsync(d->d_frames, frames, bytes, frames_are_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, d->stream));
+    const auto key = std::make_tuple(n, H, swap_rb ? W : -W);      // graphs keyed on (n, H, W) and the channel order
+    auto it = d->graphs.find(key);
+    if (it == d->graphs.end()) {
+        if (d->graphs.size() >= 16) { CKD(cudaStreamSynchronize(d->stream)); free_graphs(d); }
+        GraphEntry e{};
+        int rc = make_entry(d, n, H, W, swap_rb ? 1 : 0, &e);
+        if (rc) { if (e.exec) cudaGraphExecDestroy(e.exec); cudaFree(e.coef); cudaFree(e.tmp); return rc; }
+        it = d->graphs.emplace(key, e).first;
+    }
+    CKD(cudaGraphLaunch(it->second.exec, d->stream));
+    d->last_n = n;
+    return run_decode(d, decode_params(d, H, W, score, iou, max_boxes), n, boxes, scores, classes, counts);
+}
+
+int whenet_det_synchronize(whenet_det* d) {
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    CKD(cudaSetDevice(d->device));
+    CKD(cudaStreamSynchronize(d->stream));
+    return 0;
+}
+
+void whenet_det_destroy(whenet_det* d) {
+    if (!d) return;
+    cudaSetDevice(d->device);
+    if (d->stream) cudaStreamSynchronize(d->stream);
+    free_graphs(d);
+    for (auto& l : d->L) cudaFree(l.out);
+    cudaFree(d->warena); cudaFree(d->barena); cudaFree(d->d_frames); cudaFree(d->d_canvas);
+    cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
+    if (d->own_stream) cudaStreamDestroy(d->own_stream);
+    if (d->cap_stream) cudaStreamDestroy(d->cap_stream);
+    delete d;
+}
+
+int whenet_det_debug_tap(whenet_det* d, int layer, float* out, size_t cap, size_t* n_elems) {
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    if (!d->loaded || d->last_n < 1) return fail(WHENET_ENOTFOUND, "no detection has run yet");
+    if (layer < -1 || layer >= (int)d->table.size()) return fail(WHENET_ENOTFOUND, "no conv layer %d (0..74, -1 = letterboxed canvas)", layer);
+    const size_t n = layer < 0 ? (size_t)d->last_n * d->in_h * d->in_w * 3 : (size_t)d->last_n * d->L[layer].Ho * d->L[layer].Wo * d->L[layer].N;
+    if (n_elems) *n_elems = n;
+    if (!out) return 0;
+    if (cap < n) return fail(WHENET_EINVAL, "tap %d needs %zu elements, buffer holds %zu", layer, n, cap);
+    CKD(cudaSetDevice(d->device));
+    CKD(cudaStreamSynchronize(d->stream));
+    if (layer < 0) {
+        std::vector<uint8_t> h(n);
+        CKD(cudaMemcpy(h.data(), d->d_canvas, n, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < n; ++i) out[i] = h[i];
+        return 0;
+    }
+    return to_f32_tap(d->L[layer].out, d->table[layer].head >= 0, n, out);
+}
+
+int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n, int H, int W, int cin, int c_up, const float* w, const float* bias,
+                          int k, int stride, int cout, int leaky, const float* resid, float* out) {
+    if (!d || !x || !w || !bias || !out) return fail(WHENET_EINVAL, "null argument");
+    if (n < 1 || H < 1 || W < 1 || cin < 8 || cout < 1 || cin % 8) return fail(WHENET_EINVAL, "bad shape (n=%d H=%d W=%d cin=%d cout=%d)", n, H, W, cin, cout);
+    if (!((k == 1 && stride == 1) || (k == 3 && (stride == 1 || (stride == 2 && H >= 2 && W >= 2)))))
+        return fail(WHENET_EINVAL, "unsupported conv k=%d stride=%d", k, stride);
+    if (leaky && cout % 8) return fail(WHENET_EINVAL, "bf16 outputs need cout %% 8 == 0");
+    if (!leaky && (resid || up)) return fail(WHENET_EINVAL, "the linear fp32 conv has no residual or concat source");
+    if (resid && up) return fail(WHENET_EINVAL, "residual and concat source together are not a YOLOv3 layer");
+    if (up && (k != 1 || c_up < 64 || c_up % 64 || c_up >= cin || H % 2 || W % 2)) return fail(WHENET_EINVAL, "bad concat shape");
+    if (!up) c_up = 0;
+    CKD(cudaSetDevice(d->device));
+    const int Ho = H / stride, Wo = W / stride;
+    const size_t nx = (size_t)n * H * W * (cin - c_up), nu = (size_t)n * (H / 2) * (W / 2) * c_up, no = (size_t)n * Ho * Wo * cout;
+    const int K = k * k * cin, rows = (cout + 127) / 128 * 128;
+    std::vector<uint16_t> hx(nx), hu(nu), hw((size_t)rows * K, 0), hr(resid ? no : 0);
+    for (size_t i = 0; i < nx; ++i) hx[i] = bf16_bits(x[i]);
+    for (size_t i = 0; i < nu; ++i) hu[i] = bf16_bits(up[i]);
+    for (int o = 0; o < cout; ++o)
+        for (int i = 0; i < K; ++i) hw[(size_t)o * K + i] = bf16_bits(w[(size_t)i * cout + o]);
+    for (size_t i = 0; i < hr.size(); ++i) hr[i] = bf16_bits(resid[i]);
+    std::vector<float> hb((size_t)rows, 0.f);
+    std::copy(bias, bias + cout, hb.begin());
+    void *dx = nullptr, *du = nullptr, *dw = nullptr, *db = nullptr, *dr = nullptr, *dout = nullptr;
+    auto cleanup = [&]() { cudaFree(dx); cudaFree(du); cudaFree(dw); cudaFree(db); cudaFree(dr); cudaFree(dout); };
+    const size_t osz = no * (leaky ? 2 : 4);
+    if (cudaMalloc(&dx, nx * 2) || (nu && cudaMalloc(&du, nu * 2)) || cudaMalloc(&dw, hw.size() * 2) || cudaMalloc(&db, hb.size() * 4) ||
+        (resid && cudaMalloc(&dr, no * 2)) || cudaMalloc(&dout, osz)) {
+        cleanup();
+        return fail(WHENET_ECUDA, "out of device memory");
+    }
+    cudaMemcpy(dx, hx.data(), nx * 2, cudaMemcpyHostToDevice);
+    if (nu) cudaMemcpy(du, hu.data(), nu * 2, cudaMemcpyHostToDevice);
+    cudaMemcpy(dw, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice);
+    cudaMemcpy(db, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice);
+    if (resid) cudaMemcpy(dr, hr.data(), no * 2, cudaMemcpyHostToDevice);
+    Y::IgemmParams p{};
+    p.in = (const __nv_bfloat16*)dx; p.up = (const __nv_bfloat16*)du; p.wt = (const __nv_bfloat16*)dw; p.bias = (const float*)db;
+    p.resid = (const __nv_bfloat16*)dr; p.out = dout;
+    p.M = n * Ho * Wo; p.Hi = H; p.Wi = W; p.Ho = Ho; p.Wo = Wo; p.Cin = cin; p.c_up = c_up; p.N = cout; p.k = k; p.stride = stride;
+    const Y::IgemmPlan pl = Y::plan_igemm(Ho, Wo, cout, cin, k, d->sm_count);
+    p.n_tile = pl.n_tile; p.n_stages = pl.n_stages;
+    const int mode = !leaky ? Y::kLinearF32 : up ? Y::kLeakyCat : resid ? Y::kLeakyRes : Y::kLeaky;
+    int rc = Y::launch_igemm(d->stream, p, mode, pl.un, pl.smem, (cout + pl.n_tile - 1) / pl.n_tile, (p.M + Y::BM - 1) / Y::BM);
+    if (!rc) rc = (int)cudaStreamSynchronize(d->stream);
+    if (!rc) rc = to_f32_tap(dout, !leaky, no, out) ? -1 : 0;
+    cleanup();
+    if (rc > 0) return fail(WHENET_ECUDA, "debug conv failed: %s", cudaGetErrorString((cudaError_t)rc));
+    return rc ? WHENET_ECUDA : 0;
+}
+
+int whenet_det_debug_decode(whenet_det* d, const float* head0, const float* head1, const float* head2, int n, int img_h, int img_w, float score,
+                            float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    if (!d || !head0 || !head1 || !head2) return fail(WHENET_EINVAL, "null argument");
+    if (int rc = check_frames(d, n, img_h, img_w)) return rc;
+    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+    CKD(cudaSetDevice(d->device));
+    const float* hs[3] = {head0, head1, head2};
+    Y::DecodeParams p = decode_params(d, img_h, img_w, score, iou, max_boxes);
+    for (int l = 0; l < 3; ++l) {
+        const LayerDev& L = d->L[d->table.size() - 3 + l];
+        const size_t bytes = (size_t)n * L.Ho * L.Wo * L.N * 4;
+        CKD(cudaMemcpyAsync(L.out, hs[l], bytes, cudaMemcpyHostToDevice, d->stream));
+    }
+    return run_decode(d, p, n, boxes, scores, classes, counts);
+}
+
+}  // extern "C"

@@ -259,8 +259,16 @@ def read_keras_weights(path):
     """
     f = H5File(path)
     root_attrs = f.attrs(f.root_addr)
+    wroot = f.root_addr
+    if "layer_names" not in root_attrs:
+        # a full ``model.save`` file (what YOLO's load_model reads first, reference yolo_v3/yolo_postprocess.py:75): the
+        # layer list and the layer groups sit under "model_weights"
+        top = dict(f.children(f.root_addr))
+        if "model_weights" in top:
+            wroot = top["model_weights"]
+            root_attrs = f.attrs(wroot)
     layer_names = list(root_attrs.get("layer_names", []))
-    groups = dict(f.children(f.root_addr))
+    groups = dict(f.children(wroot))
     weights = OrderedDict()
     for lname in layer_names:
         gaddr = groups[lname]

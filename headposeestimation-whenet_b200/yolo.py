@@ -1,0 +1,169 @@
+"""Host-side mirror of the reference's ``yolo_v3/yolo_postprocess.py`` ``YOLO`` class: same constructor keywords, same
+``detect`` result - letterbox, Darknet-53, decode and NMS run in ``libwhenet_b200.so`` (hand-written sm_90a CUDA).
+
+``YOLO(**vars(args))`` from reference ``demo_video.py:41`` works: unknown keywords are kept as attributes, as the
+reference's ``self.__dict__.update(kwargs)`` does.  ``model_path=None`` means seeded random weights (``yolo_arch.random_weights``),
+flagged by ``self.random_weights``; the reference's trained ``head_detect.h5`` is not shipped.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+from typing import List, Optional, Tuple
+
+import numpy as np
+
+from . import _lib, h5lite, yolo_arch
+from ._lib import check
+from .whenet import _is_device, _ptr
+
+
+def _tensor_list(layers):
+    """Mapped layers -> the ABI's tensor list (kernel, then BN gamma/beta/mean/var or bias, in table order)."""
+    arrs, names = [], []
+    for d in layers:
+        keys = ["kernel"] + (["gamma", "beta", "moving_mean", "moving_variance"] if "gamma" in d else ["bias"])
+        for k in keys:
+            arrs.append(np.ascontiguousarray(d[k], np.float32))
+            names.append(("%s/%s:0" % (d["name"], k)).encode())
+    t = (_lib.Tensor * len(arrs))()
+    for i, (a, nm) in enumerate(zip(arrs, names)):
+        t[i].name = nm
+        t[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
+        t[i].ndim = a.ndim
+        for j in range(a.ndim):
+            t[i].dims[j] = a.shape[j]
+    return t, (arrs, names)
+
+
+class YOLO:
+    def __init__(self, model_path=None, anchors_path=None, classes_path=None, score=0.3, iou=0.45, model_image_size=(416, 416),
+                 gpu_num=1, *, device: Optional[int] = None, max_frames: int = 8, seed: int = 0, **kwargs):
+        self.__dict__.update(kwargs)
+        self.model_path, self.anchors_path, self.classes_path = model_path, anchors_path, classes_path
+        self.score, self.iou, self.gpu_num = float(score), float(iou), gpu_num
+        size = tuple(model_image_size)
+        if len(size) != 2 or None in size:
+            raise ValueError("model_image_size (None, None) (image-sized input) is not supported; use multiples of 32")
+        yolo_arch.check_size(*size)
+        self.model_image_size = size
+        self.anchors = yolo_arch.read_anchors(os.path.expanduser(anchors_path)) if anchors_path else yolo_arch.DEFAULT_ANCHORS.copy()
+        if self.anchors.shape != (9, 2):
+            raise ValueError("YOLOv3 needs 9 anchors, %s has %d" % (anchors_path, len(self.anchors)))
+        self.class_names = yolo_arch.read_classes(os.path.expanduser(classes_path)) if classes_path else list(yolo_arch.DEFAULT_CLASSES)
+        self.random_weights = model_path is None
+        if model_path is None:
+            names, w = yolo_arch.random_weights(seed, len(self.class_names))
+        else:
+            mp = os.path.expanduser(os.fspath(model_path))
+            if not mp.endswith(".h5"):
+                raise ValueError("Keras model or weights must be a .h5 file.")     # yolo_postprocess.py:68
+            names, w, _meta = h5lite.read_keras_weights(mp)
+        layers, num_classes = yolo_arch.map_weights(names, w)
+        if num_classes != len(self.class_names):
+            raise ValueError("Mismatch between model and given anchor and class sizes: the model has %d classes, %d class names"
+                             % (num_classes, len(self.class_names)))
+        self.num_classes = num_classes
+        self.device = int(os.environ.get("LOCAL_RANK", "0")) if device is None else int(device)
+        self.max_frames = int(max_frames)
+        self._L = _lib.load()
+        self._h = C.c_void_p()
+        check(self._L.whenet_det_create(C.byref(self._h), self.device, size[0], size[1], self.max_frames))
+        self.load_layers(layers)
+
+    def load_layers(self, layers):
+        """Mapped layers (``yolo_arch.map_weights``) -> device."""
+        t, keep = _tensor_list(layers)
+        anchors = np.ascontiguousarray(self.anchors, np.float32)
+        check(self._L.whenet_det_load_weights(self._h, t, len(t), _ptr(anchors), len(anchors)))
+        del keep
+
+    # ------------------------------------------------------------------ reference surface
+    def detect(self, image) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """reference yolo_postprocess.py:180-205: PIL RGB image or (H, W, 3) RGB uint8 array -> (boxes (k,4) float32
+        (y_min, x_min, y_max, x_max), scores (k,) float32, classes (k,) int32)."""
+        a = np.asarray(image.convert("RGB") if hasattr(image, "convert") else image)
+        return self._detect(a[None], swap_rb=False)[0]
+
+    def detect_frames(self, frames_bgr) -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
+        """A batch of BGR frames of one size (n, H, W, 3) uint8, numpy or a CUDA tensor -> one detect() tuple per frame."""
+        return self._detect(frames_bgr, swap_rb=True)
+
+    def _detect(self, frames, swap_rb: bool, max_boxes: int = 20):
+        dev = _is_device(frames)
+        if not dev:
+            frames = np.ascontiguousarray(frames, dtype=np.uint8)
+        elif not frames.is_contiguous() or str(frames.dtype) != "torch.uint8":
+            raise ValueError("device frames must be a contiguous uint8 CUDA tensor")
+        if len(frames.shape) != 4 or frames.shape[3] != 3:
+            raise ValueError("frames must be (n, H, W, 3) uint8")
+        n, H, W = (int(v) for v in frames.shape[:3])
+        out = []
+        for off in range(0, n, self.max_frames):
+            nb = min(self.max_frames, n - off)
+            slots = self.num_classes * max_boxes
+            boxes = np.empty((nb, slots, 4), np.float32)
+            scores = np.empty((nb, slots), np.float32)
+            classes = np.empty((nb, slots), np.int32)
+            counts = np.empty((nb,), np.int32)
+            check(self._L.whenet_det_detect_u8(self._h, _ptr(frames[off:off + nb]), nb, H, W, int(dev), int(swap_rb), self.score, self.iou,
+                                               max_boxes, _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
+            for i in range(nb):
+                k = int(counts[i])
+                out.append((boxes[i, :k].copy(), scores[i, :k].copy(), classes[i, :k].copy()))
+        return out
+
+    # ------------------------------------------------------------------ test hooks
+    def tap(self, layer: int) -> np.ndarray:
+        """float32 output of conv ``layer`` (0..74) of the last call, or (-1) its letterboxed canvas, flat."""
+        n = C.c_size_t(0)
+        check(self._L.whenet_det_debug_tap(self._h, int(layer), None, 0, C.byref(n)))
+        out = np.empty((n.value,), np.float32)
+        check(self._L.whenet_det_debug_tap(self._h, int(layer), _ptr(out), n.value, C.byref(n)))
+        return out
+
+    def debug_conv(self, x, w, bias, k: int, stride: int, leaky: bool = True, resid=None, up=None):
+        """One conv through the implicit-GEMM kernel (see whenet_det_debug_conv).  x (n,H,W,C), up (n,H/2,W/2,Cu) or None."""
+        x = np.ascontiguousarray(x, np.float32)
+        w = np.ascontiguousarray(w, np.float32)
+        bias = np.ascontiguousarray(bias, np.float32)
+        n, H, W, cx = x.shape
+        c_up = 0 if up is None else up.shape[3]
+        up = None if up is None else np.ascontiguousarray(up, np.float32)
+        resid = None if resid is None else np.ascontiguousarray(resid, np.float32)
+        cout = w.shape[3]
+        out = np.empty((n, H // stride, W // stride, cout), np.float32)
+        check(self._L.whenet_det_debug_conv(self._h, _ptr(x), _ptr(up), n, H, W, cx + c_up, c_up, _ptr(w), _ptr(bias), k, stride, cout,
+                                            int(leaky), _ptr(resid), _ptr(out)))
+        return out
+
+    def debug_decode(self, heads, img_h: int, img_w: int, max_boxes: int = 20):
+        """Raw fp32 head tensors [(n,gh,gw,3(5+C)) x 3] -> per-frame (boxes, scores, classes) through the device decode + NMS."""
+        hs = [np.ascontiguousarray(h, np.float32) for h in heads]
+        n = hs[0].shape[0]
+        slots = self.num_classes * max_boxes
+        boxes = np.empty((n, slots, 4), np.float32)
+        scores = np.empty((n, slots), np.float32)
+        classes = np.empty((n, slots), np.int32)
+        counts = np.empty((n,), np.int32)
+        check(self._L.whenet_det_debug_decode(self._h, _ptr(hs[0]), _ptr(hs[1]), _ptr(hs[2]), n, img_h, img_w, self.score, self.iou, max_boxes,
+                                              _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
+        return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(n)]
+
+    def synchronize(self):
+        check(self._L.whenet_det_synchronize(self._h))
+
+    def close_session(self):
+        """reference yolo_postprocess.py:177-178"""
+        self.close()
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._L.whenet_det_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -204,6 +204,58 @@ const char* whenet_last_error(void);
 const char* whenet_version(void);
 void whenet_destroy(whenet_ctx* ctx);
 
+/* ==== YOLOv3 head detector (reference yolo_v3/yolo_postprocess.py:26-205, yolo_v3/model.py) ====
+ * A detector handle is bound to one device, one stream and one model input size (multiples of 32 in [32, 608]; the
+ * reference's model_image_size, default 416 x 416) and is NOT thread-safe.  Errors use the WHENET_E* codes and
+ * whenet_last_error().  Storage is bf16, accumulation fp32; the head logits stay fp32. */
+typedef struct whenet_det whenet_det;
+
+/* replaces: YOLO.__init__ graph construction (yolo_postprocess.py:44-50, 77-78 yolo_body).  `max_frames` bounds n of one
+ * detect call (1..64). */
+int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, int max_frames);
+
+/* replaces: load_model / yolo_model.load_weights(model_path) (yolo_postprocess.py:74-79) and _get_anchors (:59-64).
+ * `tensors`: the 75 convs in Keras weight order (whenet_b200/yolo_arch.py), each its kernel [k,k,cin,cout] followed by
+ * BatchNorm gamma, beta, moving_mean, moving_variance (bias-free convs) or by its bias (the three output convs); BatchNorm
+ * (eps 1e-3) is folded in double and the kernels rounded once to bf16.  The class count follows from the output convs'
+ * width 3 * (5 + classes).  `anchors`: 9 (w, h) pairs in input pixels. */
+int whenet_det_load_weights(whenet_det* det, const whenet_tensor* tensors, int n_tensors, const float* anchors, int n_anchors);
+
+/* Number of classes of the loaded weights (0 before whenet_det_load_weights). */
+int whenet_det_num_classes(whenet_det* det);
+
+/* Run on an existing CUDA stream; NULL restores the internal one. */
+int whenet_det_set_stream(whenet_det* det, void* cuda_stream);
+
+/* replaces: YOLO.detect (yolo_postprocess.py:180-205) for n frames of one size at once: letterbox_image (utils.py:23-34,
+ * bit-exact with Pillow's BICUBIC), /255, the body, yolo_eval (model.py:190-232: decode, yolo_correct_boxes, per-class
+ * score >= `score`, greedy NMS with IoU > `iou` suppressing, at most `max_boxes` (1..256) per class; equal scores keep
+ * the lower candidate index first).  `frames`: n x H x W x 3 uint8, host or device memory; swap_rb != 0 reads BGR.
+ * Outputs (host): per frame num_classes * max_boxes slots of boxes (y_min, x_min, y_max, x_max, original pixels,
+ * unclipped), scores and classes, filled class by class; counts[i] = slots used by frame i.  The forward is a CUDA graph
+ * captured on the first call for each (n, H, W) and replayed after.  Synchronous. */
+int whenet_det_detect_u8(whenet_det* det, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb,
+                         float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
+
+/* Block until everything queued by this detector has finished. */
+int whenet_det_synchronize(whenet_det* det);
+void whenet_det_destroy(whenet_det* det);
+
+/* ---- detector test hooks (no reference counterpart) ---- */
+/* float32 copy of the output of conv `layer` (0..74, table order) of the last detect call (n x Ho x Wo x Cout), or with
+ * layer = -1 of its letterboxed uint8 canvas (n x input_h x input_w x 3). out=NULL queries the element count. */
+int whenet_det_debug_tap(whenet_det* det, int layer, float* out, size_t cap_elems, size_t* n_elems);
+/* One conv through the detector's implicit-GEMM kernel on host float32 arrays (rounded to bf16 on the way in):
+ * x n x H x W x (cin - c_up); `up` NULL or the concat source n x H/2 x W/2 x c_up (put first, read upsampled x2);
+ * w [k][k][cin][cout]; k = 1 or 3, stride 1 or 2 (3x3 only; padding 1 top/left); leaky != 0: bias + LeakyReLU(0.1)
+ * (+ resid n x Ho x Wo x cout) rounded to bf16, leaky = 0: bias only, fp32 output (the output convs). */
+int whenet_det_debug_conv(whenet_det* det, const float* x, const float* up, int n, int H, int W, int cin, int c_up,
+                          const float* w, const float* bias, int k, int stride, int cout, int leaky, const float* resid, float* out);
+/* Decode + NMS alone: host fp32 head logits (n x gh_l x gw_l x 3(5+C) for the detector's input size) of frames of
+ * img_h x img_w pixels -> the outputs of whenet_det_detect_u8. */
+int whenet_det_debug_decode(whenet_det* det, const float* head0, const float* head1, const float* head2, int n, int img_h, int img_w,
+                            float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
+
 #ifdef __cplusplus
 }
 #endif
