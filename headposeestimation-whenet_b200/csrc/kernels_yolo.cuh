@@ -12,6 +12,8 @@
 //
 // Storage bf16 NHWC, fp32 accumulation; the three output convs write fp32.
 #pragma once
+#include <vector>
+
 #include "kernels_tc.cuh"
 
 namespace whenet {
@@ -59,6 +61,53 @@ inline IgemmPlan plan_igemm(int Ho, int Wo, int N, int Cin, int k, int sm_count)
     pl.smem = std::max((size_t)pl.n_stages * stage_bytes, out_bytes) + 1024;
     return pl;
 }
+
+// The 75 convolutions in Keras weight order; the python twin (and the documentation of every field) is yolo_arch.py.
+struct ConvCfg { int k, stride, cin, cout, src, res, up; bool bn; int head; };
+
+inline std::vector<ConvCfg> make_table() {
+    std::vector<ConvCfg> v;
+    auto add = [&](int k, int s, int cin, int cout, int src, bool bn = true, int res = -1, int up = -1, int head = -1) {
+        v.push_back(ConvCfg{k, s, cin, cout, src, res, up, bn, head});
+        return (int)v.size() - 1;
+    };
+    int x = add(3, 1, 3, 32, -1), c = 32;
+    int skip256 = -1, skip512 = -1;
+    const int nfs[5] = {64, 128, 256, 512, 1024}, nbs[5] = {1, 2, 8, 8, 4};
+    for (int b = 0; b < 5; ++b) {
+        x = add(3, 2, c, nfs[b], x);
+        for (int i = 0; i < nbs[b]; ++i) {
+            const int y = add(1, 1, nfs[b], nfs[b] / 2, x);
+            x = add(3, 1, nfs[b] / 2, nfs[b], y, true, x);
+        }
+        c = nfs[b];
+        if (c == 256) skip256 = x;
+        if (c == 512) skip512 = x;
+    }
+    int last5[3];
+    auto five = [&](int x, int cin, int nf, int up, int h) {
+        x = add(1, 1, cin, nf, x, true, -1, up);
+        for (int i = 0; i < 2; ++i) {
+            x = add(3, 1, nf, 2 * nf, x);
+            x = add(1, 1, 2 * nf, nf, x);
+        }
+        last5[h] = x;
+        return x;
+    };
+    x = five(x, 1024, 512, -1, 0);
+    int u = add(1, 1, 512, 256, x);
+    x = five(skip512, 256 + 512, 256, u, 1);
+    u = add(1, 1, 256, 128, x);
+    five(skip256, 128 + 256, 128, u, 2);
+    int y3[3];
+    const int nf3[3] = {512, 256, 128};
+    for (int h = 0; h < 3; ++h) y3[h] = add(3, 1, nf3[h], 2 * nf3[h], last5[h]);
+    for (int h = 0; h < 3; ++h) add(1, 1, 2 * nf3[h], 0, y3[h], false, -1, -1, h);
+    return v;
+}
+
+// conv_igemm_kernel's epilogue mode for a table conv
+inline int igemm_mode(const ConvCfg& c) { return c.head >= 0 ? kLinearF32 : c.up >= 0 ? kLeakyCat : c.res >= 0 ? kLeakyRes : kLeaky; }
 
 constexpr int kNmsThreads = 1024;
 constexpr int kNmsPer = 24;             // candidates per thread: 24 x 1024 >= 22,743 (608 x 608)

@@ -31,49 +31,8 @@ namespace {
 
 constexpr double kBnEps = 1e-3;     // keras BatchNormalization default (reference yolo_v3/model.py:34)
 
-// The 75 convolutions in Keras weight order; the python twin (and the documentation of every field) is yolo_arch.py.
-struct ConvCfg { int k, stride, cin, cout, src, res, up; bool bn; int head; };
-
-std::vector<ConvCfg> make_table() {
-    std::vector<ConvCfg> v;
-    auto add = [&](int k, int s, int cin, int cout, int src, bool bn = true, int res = -1, int up = -1, int head = -1) {
-        v.push_back(ConvCfg{k, s, cin, cout, src, res, up, bn, head});
-        return (int)v.size() - 1;
-    };
-    int x = add(3, 1, 3, 32, -1), c = 32;
-    int skip256 = -1, skip512 = -1;
-    const int nfs[5] = {64, 128, 256, 512, 1024}, nbs[5] = {1, 2, 8, 8, 4};
-    for (int b = 0; b < 5; ++b) {
-        x = add(3, 2, c, nfs[b], x);
-        for (int i = 0; i < nbs[b]; ++i) {
-            const int y = add(1, 1, nfs[b], nfs[b] / 2, x);
-            x = add(3, 1, nfs[b] / 2, nfs[b], y, true, x);
-        }
-        c = nfs[b];
-        if (c == 256) skip256 = x;
-        if (c == 512) skip512 = x;
-    }
-    int last5[3];
-    auto five = [&](int x, int cin, int nf, int up, int h) {
-        x = add(1, 1, cin, nf, x, true, -1, up);
-        for (int i = 0; i < 2; ++i) {
-            x = add(3, 1, nf, 2 * nf, x);
-            x = add(1, 1, 2 * nf, nf, x);
-        }
-        last5[h] = x;
-        return x;
-    };
-    x = five(x, 1024, 512, -1, 0);
-    int u = add(1, 1, 512, 256, x);
-    x = five(skip512, 256 + 512, 256, u, 1);
-    u = add(1, 1, 256, 128, x);
-    five(skip256, 128 + 256, 128, u, 2);
-    int y3[3];
-    const int nf3[3] = {512, 256, 128};
-    for (int h = 0; h < 3; ++h) y3[h] = add(3, 1, nf3[h], 2 * nf3[h], last5[h]);
-    for (int h = 0; h < 3; ++h) add(1, 1, 2 * nf3[h], 0, y3[h], false, -1, -1, h);
-    return v;
-}
+using Y::ConvCfg;
+using Y::make_table;
 
 uint16_t bf16_bits(float f) {      // round to nearest even (finite inputs)
     uint32_t u;
@@ -184,8 +143,7 @@ int enqueue_conv(whenet_det* d, cudaStream_t s, int i, int n) {
     p.M = n * l.Ho * l.Wo; p.Hi = l.Hi; p.Wi = l.Wi; p.Ho = l.Ho; p.Wo = l.Wo;
     p.Cin = c.cin; p.c_up = c.up >= 0 ? d->table[c.up].cout : 0; p.N = N; p.k = c.k; p.stride = c.stride;
     p.n_tile = l.plan.n_tile; p.n_stages = l.plan.n_stages;
-    const int mode = c.head >= 0 ? Y::kLinearF32 : c.up >= 0 ? Y::kLeakyCat : c.res >= 0 ? Y::kLeakyRes : Y::kLeaky;
-    const int rc = Y::launch_igemm(s, p, mode, l.plan.un, l.plan.smem, (N + l.plan.n_tile - 1) / l.plan.n_tile, (p.M + Y::BM - 1) / Y::BM);
+    const int rc = Y::launch_igemm(s, p, Y::igemm_mode(c), l.plan.un, l.plan.smem, (N + l.plan.n_tile - 1) / l.plan.n_tile, (p.M + Y::BM - 1) / Y::BM);
     if (rc) return fail(WHENET_ECUDA, "conv %d launch failed: %s", i, cudaGetErrorString((cudaError_t)rc));
     return 0;
 }

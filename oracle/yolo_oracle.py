@@ -254,13 +254,14 @@ def iou_tf(a, b):
 
 def nms_tf(boxes, scores, max_output_size, iou_threshold):
     """tf.image.non_max_suppression: greedy in descending score (equal scores: lower index first), a box is suppressed when
-    its IoU with a kept box is > the threshold.  Returns kept indices."""
+    its IoU with a kept box is > the threshold (so a NaN IoU, of two boxes with infinite corners, suppresses nothing).
+    Returns kept indices."""
     order = sorted(range(len(scores)), key=lambda i: (-float(scores[i]), i))
     keep = []
     for i in order:
         if len(keep) >= max_output_size:
             break
-        if all(iou_tf(boxes[i], boxes[j]) <= f32(iou_threshold) for j in keep):
+        if not any(iou_tf(boxes[i], boxes[j]) > f32(iou_threshold) for j in keep):
             keep.append(i)
     return keep
 

@@ -8,36 +8,8 @@ import pytest
 
 from conftest import GOLD
 import yolo_oracle as O
+from yolo_cases import SIZES, int_round_differ as _int_round_differ, pil_letterbox as _pil_letterbox, nan_iou_heads
 from whenet_b200 import yolo_arch as Y
-
-
-def _pil_letterbox(img, size):
-    """The reference's letterbox_image (utils.py:23-34) on Pillow itself."""
-    from PIL import Image
-    im = Image.fromarray(img)
-    iw, ih = im.size
-    w, h = size
-    scale = min(w / iw, h / ih)
-    nw, nh = int(iw * scale), int(ih * scale)
-    im = im.resize((nw, nh), Image.BICUBIC)
-    new = Image.new("RGB", size, (128, 128, 128))
-    new.paste(im, ((w - nw) // 2, (h - nh) // 2))
-    return np.asarray(new)
-
-
-def _int_round_differ():
-    """A frame size whose letterbox extent differs between int() (utils.py:28) and round() (model.py:159) at 416."""
-    for W in range(300, 2000):
-        H = 333
-        s = min(416 / W, 416 / H)
-        if int(W * s) != round(W * s) or int(H * s) != round(H * s):
-            return W, H
-    raise AssertionError("no such size")
-
-
-SIZES = [(1, 1), (2, 3), (3, 2), (7, 5), (13, 13), (31, 17), (64, 48), (99, 101), (100, 300), (300, 100), (415, 415), (416, 416),
-         (417, 417), (416, 234), (234, 416), (640, 480), (480, 640), (500, 499), (800, 600), (1280, 720), (1920, 1080), (1080, 1920),
-         (1000, 5), (123, 457), (333, 222), (208, 208), (832, 832), (200, 100), (57, 911), _int_round_differ()]
 
 
 @pytest.mark.parametrize("wh", SIZES)
@@ -167,6 +139,16 @@ def test_two_classes_and_threshold_inclusive():
 def test_equal_scores_keep_lower_index_first():
     boxes = np.stack([_box(0, 0, 10, 10), _box(0, 0, 10, 10)])
     assert O.nms_tf(boxes, np.array([0.5, 0.5], np.float32), 20, 0.45) == [0]
+
+
+def test_nan_iou_suppresses_nothing():
+    heads = nan_iou_heads()
+    with np.errstate(over="ignore", invalid="ignore"):
+        boxes, scores = O.decode([h[0] for h in heads], Y.DEFAULT_ANCHORS, 1, 480, 640)
+        i, j = np.nonzero(scores[:, 0] == 1)[0]
+        assert np.isnan(O.iou_tf(boxes[i], boxes[j]))
+        _b, s, _c, idx = O.yolo_eval(boxes, scores, 0.3, 0.45)
+    assert idx.tolist() == [i, j] and s.tolist() == [1.0, 1.0]         # TF suppresses only when IoU > threshold
 
 
 def test_correct_boxes_reproduce_round_and_int():
