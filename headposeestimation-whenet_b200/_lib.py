@@ -15,7 +15,8 @@ EXPORTS = [
     "whenet_debug_conv1x1", "whenet_debug_decode", "whenet_debug_raise_timeout", "whenet_debug_read_trace", "whenet_debug_set_k1_plan", "whenet_debug_set_k1w_plan", "whenet_profile_enable", "whenet_profile_read", "whenet_launch_count", "whenet_set_option",
     "whenet_last_error", "whenet_version", "whenet_destroy",
     "whenet_det_create", "whenet_det_load_weights", "whenet_det_num_classes", "whenet_det_set_stream", "whenet_det_detect_u8",
-    "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_decode",
+    "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_maxpool",
+    "whenet_det_debug_decode",
 ]
 
 
@@ -102,6 +103,7 @@ def load():
     L.whenet_det_destroy.restype = None
     L.whenet_det_debug_tap.argtypes = [P, I, P, C.c_size_t, C.POINTER(C.c_size_t)]
     L.whenet_det_debug_conv.argtypes = [P, P, P, I, I, I, I, I, P, P, I, I, I, I, P, P]
+    L.whenet_det_debug_maxpool.argtypes = [P, P, I, I, I, I, I, P]
     L.whenet_det_debug_decode.argtypes = [P, P, P, P, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
     _lib = L
     return L

@@ -12,13 +12,28 @@ int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in,
     return (int)cudaGetLastError();
 }
 
-constexpr size_t kConv0Smem = 128 * 128 + 32 * 128 + 256 * 4 + tc::acc_tile_bytes(32) + 1024;
-
-int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w) {
-    cudaError_t e = cudaFuncSetAttribute(yolo_conv0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kConv0Smem);
+template <int N>
+int launch_conv0_t(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w) {
+    constexpr size_t smem = 128 * 128 + N * 128 + 256 * 4 + tc::acc_tile_bytes(N) + 1024;
+    cudaError_t e = cudaFuncSetAttribute(yolo_conv0_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     const long long tiles = (long long)n * S_h * S_w / 128;           // S_h * S_w is a multiple of 1024
-    yolo_conv0_kernel<<<(unsigned)tiles, 128, kConv0Smem, s>>>(img, w0, bias, out, S_h, S_w);
+    yolo_conv0_kernel<N><<<(unsigned)tiles, 128, smem, s>>>(img, w0, bias, out, S_h, S_w);
+    return (int)cudaGetLastError();
+}
+
+int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w,
+                 int cout) {
+    switch (cout) {
+        case 16: return launch_conv0_t<16>(s, img, w0, bias, out, n, S_h, S_w);
+        case 32: return launch_conv0_t<32>(s, img, w0, bias, out, n, S_h, S_w);
+    }
+    return (int)cudaErrorInvalidValue;
+}
+
+int launch_maxpool(cudaStream_t s, const __nv_bfloat16* in, __nv_bfloat16* out, int n, int H, int W, int C, int stride) {
+    const long long threads = (long long)n * ((H + stride - 1) / stride) * ((W + stride - 1) / stride) * (C / 8);
+    yolo_maxpool_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(in, out, n, H, W, C, stride);
     return (int)cudaGetLastError();
 }
 

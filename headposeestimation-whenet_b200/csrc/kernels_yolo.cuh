@@ -1,16 +1,19 @@
-// kernels_yolo.cuh - the YOLOv3 head detector (reference yolo_v3/): letterbox, Darknet-53 + three heads on wgmma, decode + NMS.
+// kernels_yolo.cuh - the YOLOv3 head detector (reference yolo_v3/): letterbox, Darknet-53 + three heads (or tiny YOLOv3's
+// 13 convs, six max-pools and two heads) on wgmma, decode + NMS.
 //
 //   letterbox_h_kernel / letterbox_v_kernel   Pillow's uint8 BICUBIC resample (two integer passes, 22-bit coefficients computed on
 //                                             the host exactly as ImagingResample does) + the (128,128,128) canvas and the paste
 //                                             (reference utils.py:23-34)
-//   yolo_conv0_kernel                          first conv (3 -> 32, 3x3): im2col row built in shared memory from the uint8 canvas
-//                                             through a v/255 table split into bf16 hi + lo parts, one K = 64 wgmma block per row
+//   yolo_conv0_kernel<N>                       first conv (3 -> N = 32, tiny: 16, 3x3): im2col row built in shared memory from the
+//                                             uint8 canvas through a v/255 table split into bf16 hi + lo parts, one K = 64 wgmma
+//                                             block per row
 //   conv_igemm_kernel<MODE, UN>                every other conv as an implicit GEMM (M = pixels, N = Cout, K = taps x Cin): the A
 //                                             operand is gathered per (tap, 64-channel chunk) with cp.async, out-of-image taps are
 //                                             zero-filled (= the padding); concat convs read [upsample(up), skip] virtually
+//   yolo_maxpool_kernel                        tiny YOLOv3's 2x2 max-pools (stride 2, or stride 1 with TF SAME padding)
 //   yolo_decode_nms_kernel                     one CTA per frame: decode every candidate, per-class score mask, greedy NMS
 //
-// Storage bf16 NHWC, fp32 accumulation; the three output convs write fp32.
+// Storage bf16 NHWC, fp32 accumulation; the output convs write fp32.
 #pragma once
 #include <vector>
 
@@ -62,8 +65,9 @@ inline IgemmPlan plan_igemm(int Ho, int Wo, int N, int Cin, int k, int sm_count)
     return pl;
 }
 
-// The 75 convolutions in Keras weight order; the python twin (and the documentation of every field) is yolo_arch.py.
-struct ConvCfg { int k, stride, cin, cout, src, res, up; bool bn; int head; };
+// The 75 convolutions (tiny YOLOv3: 13) in Keras weight order; the python twin (and the documentation of every field) is
+// yolo_arch.py.  pool: the conv's input is out[src] max-pooled 2x2 with this stride (0: no pool).
+struct ConvCfg { int k, stride, cin, cout, src, res, up; bool bn; int head; int pool = 0; };
 
 inline std::vector<ConvCfg> make_table() {
     std::vector<ConvCfg> v;
@@ -106,6 +110,34 @@ inline std::vector<ConvCfg> make_table() {
     return v;
 }
 
+// The 13 convolutions of tiny YOLOv3 (reference model.py:92-122) in Keras weight order (yolo_arch.TINY_LAYERS)
+inline std::vector<ConvCfg> make_tiny_table() {
+    std::vector<ConvCfg> v;
+    auto add = [&](int k, int cin, int cout, int src, int pool = 0, int up = -1, int head = -1) {
+        ConvCfg c{k, 1, cin, cout, src, -1, up, head < 0, head};
+        c.pool = pool;
+        v.push_back(c);
+    };
+    add(3, 3, 16, -1);
+    for (int i = 1; i <= 5; ++i) add(3, 8 << i, 16 << i, i - 1, 2);    // 16 -> 32 ... 256 -> 512, each after a stride-2 pool
+    add(3, 512, 1024, 5, 1);                                          // after the stride-1 pool
+    add(1, 1024, 256, 6);
+    add(1, 256, 128, 7);                                              // upsampled into conv 10
+    add(3, 256, 512, 7);
+    add(3, 128 + 256, 256, 4, 0, 8);                                  // 3x3 concat conv: [upsample(out[8]), out[4]]
+    add(1, 512, 0, 9, 0, -1, 0);
+    add(1, 256, 0, 10, 0, -1, 1);
+    return v;
+}
+
+// anchor_mask (model.py:199): the anchors of head l, anchor-in-layer a.  The host writes the anchors into (l, a) slots in
+// this order, so the decode reads slot 3 * l + a for either network.
+constexpr int kAnchorMask[3][3] = {{6, 7, 8}, {3, 4, 5}, {0, 1, 2}};
+constexpr int kTinyAnchorMask[2][3] = {{3, 4, 5}, {1, 2, 3}};
+
+// input size of a table conv from its source's output size (the pool of a tiny conv: TF SAME, ceil(h / stride))
+inline int pooled(int h, int pool) { return pool ? (h + pool - 1) / pool : h; }
+
 // conv_igemm_kernel's epilogue mode for a table conv
 inline int igemm_mode(const ConvCfg& c) { return c.head >= 0 ? kLinearF32 : c.up >= 0 ? kLeakyCat : c.res >= 0 ? kLeakyRes : kLeaky; }
 
@@ -114,15 +146,15 @@ constexpr int kNmsPer = 24;             // candidates per thread: 24 x 1024 >= 2
 constexpr int kMaxBoxes = 256;
 
 struct DecodeParams {
-    const float* head[3];               // [n][gh_l][gw_l][3 * (5 + C)] fp32 logits, l = 0, 1, 2 (13x13, 26x26, 52x52 at 416)
+    const float* head[3];               // [n][gh_l][gw_l][3 * (5 + C)] fp32 logits, l = 0, 1, 2 (13x13, 26x26, 52x52 at 416; tiny: 2 heads)
     float4* cand;                       // workspace [n][NC] boxes (y_min, x_min, y_max, x_max)
     float* cand_score;                  // workspace [n][C][NC]
     float* out_boxes;                   // [n][C * max_boxes][4]
     float* out_scores;                  // [n][C * max_boxes]
     int* out_classes;                   // [n][C * max_boxes]
     int* out_count;                     // [n]
-    float anchors[18];                  // (w, h) x 9
-    int gh0, gw0, C, NC, max_boxes;
+    float anchors[18];                  // (w, h) of head l, anchor-in-layer a at slot 3 * l + a (kAnchorMask / kTinyAnchorMask)
+    int gh0, gw0, C, NC, max_boxes;     // NC: candidates of all heads (the walk over the heads ends there)
     float in_h, in_w;                   // model input size
     float img_h, img_w;                 // original image size
     float off_y, off_x, scale_y, scale_x;   // yolo_correct_boxes (model.py:159-161), float32 on the host
@@ -141,8 +173,10 @@ struct LetterboxPlan {
     const int* ky;           // [nh][ksy]
 };
 int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb);
-int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w);
+int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w,
+                 int cout);
 int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m);
+int launch_maxpool(cudaStream_t s, const __nv_bfloat16* in, __nv_bfloat16* out, int n, int H, int W, int C, int stride);
 int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n);
 
 #ifndef WHENET_YOLO_HOST_ONLY
@@ -214,15 +248,18 @@ __device__ __forceinline__ float leaky(float x) { return x > 0.f ? x : 0.1f * x;
 
 // ----------------------------------------------------------------------------- first conv
 // 128 consecutive output pixels per CTA (S_h * S_w is a multiple of 1024: a tile never straddles frames).  A row = 27 taps
-// (ky, kx, ci) of v/255 as bf16 hi (K 0..26) and bf16 lo (K 32..58); B row n = [w | 0 | w | 0] (w0: 32 x 64 bf16, packed by the host).
+// (ky, kx, ci) of v/255 as bf16 hi (K 0..26) and bf16 lo (K 32..58); B row n = [w | 0 | w | 0] (w0: N x 64 bf16, packed by the host).
+// N = 32 output channels (YOLOv3) or 16 (tiny YOLOv3).
+template <int N>
 __global__ void __launch_bounds__(128) yolo_conv0_kernel(const uint8_t* __restrict__ img, const __nv_bfloat16* __restrict__ w0,
                                                          const float* __restrict__ bias, __nv_bfloat16* __restrict__ out, int S_h, int S_w) {
+    static_assert(N == 16 || N == 32, "first conv: 16 or 32 outputs");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sA = smem0;                      // 128 rows x 128 B
-    const uint32_t sW = sA + 128 * 128;             // 32 rows x 128 B
-    const uint32_t sL = sW + 32 * 128;              // 256 x u32 (hi | lo << 16)
-    const uint32_t sAcc = sL + 256 * 4;             // accumulator tile, 32 columns
+    const uint32_t sW = sA + 128 * 128;             // N rows x 128 B
+    const uint32_t sL = sW + N * 128;               // 256 x u32 (hi | lo << 16)
+    const uint32_t sAcc = sL + 256 * 4;             // accumulator tile, N columns
     const int tid = threadIdx.x;
     for (int i = tid; i < 256; i += 128) {
         const float f = (float)i / 255.0f;          // float32(v / 255.), as np.array(.., 'float32') / 255. (yolo_postprocess.py:191-195)
@@ -230,7 +267,7 @@ __global__ void __launch_bounds__(128) yolo_conv0_kernel(const uint8_t* __restri
         const uint32_t w = (uint32_t)__bfloat16_as_ushort(hi) | ((uint32_t)__bfloat16_as_ushort(lo) << 16);
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(sL + (uint32_t)i * 4u), "r"(w) : "memory");
     }
-    for (int i = tid; i < 32 * 8; i += 128) {
+    for (int i = tid; i < N * 8; i += 128) {
         const int r = i >> 3, c = i & 7;
         tc::sts128_(sW + (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4)),
                     *reinterpret_cast<const uint4*>(w0 + r * 64 + c * 8));
@@ -268,14 +305,14 @@ __global__ void __launch_bounds__(128) yolo_conv0_kernel(const uint8_t* __restri
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    tc::WgAcc<32> acc;
-    tc::wg_mma_tile<true, 32>(acc, sA, sW, 4, 0u);
+    tc::WgAcc<N> acc;
+    tc::wg_mma_tile<true, N>(acc, sA, sW, 4, 0u);
     tc::wg_wait<0>();
-    tc::wg_acc_store<32>(acc, sAcc, tid);
+    tc::wg_acc_store<N>(acc, sAcc, tid);
     __syncthreads();
-    __nv_bfloat16* dst = out + m * 32;
+    __nv_bfloat16* dst = out + m * N;
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
+    for (int u = 0; u < N / 16; ++u) {
         float v[16];
         tc::acc_ld16(sAcc, tid, u * 16, v);
         float o[16];
@@ -435,6 +472,37 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const __grid_constant__
     }
 }
 
+// ----------------------------------------------------------------------------- max-pool (tiny YOLOv3)
+// MaxPooling2D(pool_size 2, padding 'same') with TF's SAME rule: Ho = ceil(H / stride), the window of output y is input rows
+// y * stride and y * stride + 1, padding only at the bottom / right, and a padded cell never wins (it is left out).  bf16
+// rounding is monotone, so the max of the bf16 inputs is exact.  One thread per 8-channel chunk of an output pixel; C % 8 == 0.
+__global__ void __launch_bounds__(256) yolo_maxpool_kernel(const __nv_bfloat16* __restrict__ in, __nv_bfloat16* __restrict__ out, int n,
+                                                           int H, int W, int C, int stride) {
+    const int Ho = (H + stride - 1) / stride, Wo = (W + stride - 1) / stride, cc = C >> 3;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n * Ho * Wo * cc) return;
+    const int c = (int)(i % cc);
+    const long long px = i / cc;
+    const int ox = (int)(px % Wo);
+    const long long fy = px / Wo;
+    const int oy = (int)(fy % Ho), f = (int)(fy / Ho);
+    const int y0 = oy * stride, x0 = ox * stride;
+    const bool y1 = y0 + 1 < H, x1 = x0 + 1 < W;
+    const uint4* src = reinterpret_cast<const uint4*>(in + (((long long)f * H + y0) * W + x0) * C) + c;
+    const long long row = (long long)W * cc;            // uint4s per input row
+    uint4 v = src[0];
+    auto mx = [](uint4& a, uint4 b) {
+        __nv_bfloat162* pa = reinterpret_cast<__nv_bfloat162*>(&a);
+        const __nv_bfloat162* pb = reinterpret_cast<const __nv_bfloat162*>(&b);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) pa[j] = __hmax2(pa[j], pb[j]);
+    };
+    if (x1) mx(v, src[cc]);
+    if (y1) mx(v, src[row]);
+    if (x1 && y1) mx(v, src[row + cc]);
+    reinterpret_cast<uint4*>(out)[i] = v;
+}
+
 // ----------------------------------------------------------------------------- decode + NMS
 __device__ __forceinline__ float sigmoidf_(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
 
@@ -455,7 +523,7 @@ __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __gr
     const int CH = 5 + p.C;
     float4* cand = p.cand + (long long)f * p.NC;
     float* cscore = p.cand_score + (long long)f * p.C * p.NC;
-    // ---- decode (model.py:125-187): candidates ordered layer 0, 1, 2, then (y, x, anchor)
+    // ---- decode (model.py:125-187): candidates ordered layer 0, 1 (, 2), then (y, x, anchor)
     for (int i = tid; i < p.NC; i += kNmsThreads) {
         int l = 0, rem = i;
         int gh = p.gh0, gw = p.gw0;
@@ -463,7 +531,7 @@ __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __gr
         const int cell = rem / 3, a = rem - cell * 3;
         const int y = cell / gw, x = cell - y * gw;
         const float* t = p.head[l] + (((long long)f * gh + y) * gw + x) * 3 * CH + a * CH;
-        const int an = 3 * (2 - l) + a;                                     // anchor_mask[l] = [[6,7,8],[3,4,5],[0,1,2]][l]
+        const int an = 3 * l + a;                                           // the host put anchor_mask[l][a] in this slot
         const float bx = __fdiv_rn(__fadd_rn(sigmoidf_(t[0]), (float)x), (float)gw);
         const float by = __fdiv_rn(__fadd_rn(sigmoidf_(t[1]), (float)y), (float)gh);
         const float bw = __fdiv_rn(__fmul_rn(expf(t[2]), p.anchors[2 * an]), p.in_w);

@@ -30,6 +30,7 @@ namespace Y = whenet::yolo;
 namespace {
 
 constexpr double kBnEps = 1e-3;     // keras BatchNormalization default (reference yolo_v3/model.py:34)
+constexpr int kPoolTap = 100;       // whenet_det_debug_tap: kPoolTap + i = the max-pooled input of tiny conv i
 
 using Y::ConvCfg;
 using Y::make_table;
@@ -41,7 +42,8 @@ uint16_t bf16_bits(float f) {      // round to nearest even (finite inputs)
     return (uint16_t)(u >> 16);
 }
 
-struct LayerDev { int Hi, Wi, Ho, Wo, N; Y::IgemmPlan plan; void* out = nullptr; };
+// Hi, Wi: the conv's input size (after the pool of a tiny conv); pooled: that pool's output, a buffer of its own
+struct LayerDev { int Hi, Wi, Ho, Wo, N; Y::IgemmPlan plan; void* out = nullptr; void* pooled = nullptr; };
 
 struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
@@ -97,6 +99,7 @@ int precompute_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::
 struct whenet_det {
     int device = 0, in_h = 0, in_w = 0, max_frames = 0, sm_count = 132;
     int num_classes = 0;
+    bool tiny = false;                  // tiny YOLOv3 (6 anchors, 13 convs, two heads) instead of YOLOv3 (9 anchors, 75 convs)
     bool loaded = false;
     cudaStream_t own_stream = nullptr, stream = nullptr, cap_stream = nullptr;
     std::vector<ConvCfg> table;
@@ -104,7 +107,7 @@ struct whenet_det {
     void* warena = nullptr;             // bf16 kernels, [N][K] each, 256-byte aligned
     float* barena = nullptr;            // fp32 biases
     std::vector<size_t> w_off, b_off;
-    float anchors[18] = {};
+    float anchors[18] = {};             // in (head, anchor-in-layer) slots, see DecodeParams
     uint8_t* d_frames = nullptr; size_t frames_cap = 0;
     uint8_t* d_canvas = nullptr;
     float4* d_cand = nullptr; float* d_cand_score = nullptr;
@@ -115,7 +118,13 @@ struct whenet_det {
 
 namespace {
 
-int ncand(const whenet_det* d) { return 3 * (d->in_h / 32) * (d->in_w / 32) * 21; }    // 1 + 4 + 16 cells per 32x32 block
+// candidates per frame: 1 + 4 + 16 cells per 32x32 block (tiny: 1 + 4)
+int ncand(const whenet_det* d) { return 3 * (d->in_h / 32) * (d->in_w / 32) * (d->tiny ? 5 : 21); }
+int num_heads(const whenet_det* d) { return d->tiny ? 2 : 3; }
+
+void free_layers(whenet_det* d) {
+    for (auto& l : d->L) { cudaFree(l.out); cudaFree(l.pooled); l.out = l.pooled = nullptr; }
+}
 
 void free_graphs(whenet_det* d) {
     for (auto& kv : d->graphs) {
@@ -128,13 +137,18 @@ void free_graphs(whenet_det* d) {
 
 const __nv_bfloat16* bf(const whenet_det* d, size_t off) { return reinterpret_cast<const __nv_bfloat16*>((const char*)d->warena + off); }
 
-// enqueue one conv (layers 1..74) on stream s, n frames
+// enqueue one conv (every table conv but the first), with the max-pool of its input for a tiny conv, on stream s, n frames
 int enqueue_conv(whenet_det* d, cudaStream_t s, int i, int n) {
     const ConvCfg& c = d->table[i];
     const LayerDev& l = d->L[i];
+    if (c.pool) {
+        const LayerDev& src = d->L[c.src];
+        const int rc = Y::launch_maxpool(s, (const __nv_bfloat16*)src.out, (__nv_bfloat16*)l.pooled, n, src.Ho, src.Wo, src.N, c.pool);
+        if (rc) return fail(WHENET_ECUDA, "max-pool before conv %d launch failed: %s", i, cudaGetErrorString((cudaError_t)rc));
+    }
     Y::IgemmParams p{};
     const int N = l.N;
-    p.in = reinterpret_cast<const __nv_bfloat16*>(d->L[c.src].out);
+    p.in = reinterpret_cast<const __nv_bfloat16*>(c.pool ? l.pooled : d->L[c.src].out);
     p.up = c.up >= 0 ? reinterpret_cast<const __nv_bfloat16*>(d->L[c.up].out) : nullptr;
     p.wt = bf(d, d->w_off[i]);
     p.bias = d->barena + d->b_off[i];
@@ -172,7 +186,8 @@ int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
     cudaStream_t s = d->cap_stream;
     CKD(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
     int rc = Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb);
-    if (!rc) rc = Y::launch_conv0(s, d->d_canvas, bf(d, d->w_off[0]), d->barena + d->b_off[0], (__nv_bfloat16*)d->L[0].out, n, d->in_h, d->in_w);
+    if (!rc) rc = Y::launch_conv0(s, d->d_canvas, bf(d, d->w_off[0]), d->barena + d->b_off[0], (__nv_bfloat16*)d->L[0].out, n, d->in_h, d->in_w,
+                                 d->table[0].cout);
     int rc2 = rc ? fail(WHENET_ECUDA, "letterbox / first conv launch failed: %s", cudaGetErrorString((cudaError_t)rc)) : 0;
     for (size_t i = 1; i < d->table.size() && !rc2; ++i) rc2 = enqueue_conv(d, s, (int)i, n);
     cudaGraph_t g = nullptr;
@@ -204,7 +219,8 @@ Y::DecodeParams decode_params(const whenet_det* d, int img_h, int img_w, float s
     p.off_y = (p.in_h - nh) / 2.0f / p.in_h; p.off_x = (p.in_w - nw) / 2.0f / p.in_w;
     p.scale_y = p.in_h / nh; p.scale_x = p.in_w / nw;
     p.score = score; p.iou = iou;
-    for (int l = 0; l < 3; ++l) p.head[l] = (const float*)d->L[d->table.size() - 3 + l].out;
+    const int heads = num_heads(d);
+    for (int l = 0; l < heads; ++l) p.head[l] = (const float*)d->L[d->table.size() - heads + l].out;
     return p;
 }
 
@@ -271,13 +287,16 @@ int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, in
 }
 
 int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors, const float* anchors, int n_anchors) {
+    // the anchor count picks the network, as the reference does (yolo_postprocess.py:73)
+    if (n_anchors != 6 && n_anchors != 9) return fail(WHENET_EINVAL, "YOLOv3 needs 9 anchors and tiny YOLOv3 6, got %d", n_anchors);
     if (!d || !t || !anchors) return fail(WHENET_EINVAL, "bad arguments");
-    if (n_anchors != 9) return fail(WHENET_EINVAL, "YOLOv3 needs 9 anchors, got %d", n_anchors);
-    const std::vector<ConvCfg>& T = d->table;
+    const bool tiny = n_anchors == 6;
+    const std::vector<ConvCfg> T = tiny ? Y::make_tiny_table() : make_table();
     // tensors in table order: kernel [k,k,cin,cout], then gamma, beta, moving_mean, moving_variance (BN convs) or bias (output convs)
     size_t need = 0;
     for (const ConvCfg& c : T) need += c.bn ? 5 : 2;
-    if ((size_t)n_tensors != need) return fail(WHENET_ESHAPE, "expected %zu tensors (75 convs + BatchNorms), got %d", need, n_tensors);
+    if ((size_t)n_tensors != need)
+        return fail(WHENET_ESHAPE, "expected %zu tensors (%s: %zu convs + BatchNorms), got %d", need, tiny ? "tiny YOLOv3" : "YOLOv3", T.size(), n_tensors);
     const whenet_tensor& h0 = t[need - 2];      // output conv of head 2 (its kernel), all heads have the same width
     if (h0.ndim != 4 || h0.dims[3] < 18 || h0.dims[3] % 3) return fail(WHENET_ESHAPE, "%s: output conv width is not 3 * (5 + classes)", h0.name ? h0.name : "?");
     const int C = (int)h0.dims[3] / 3 - 5;
@@ -307,7 +326,7 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
             if (b.ndim != 1 || b.dims[0] != co) return fail(WHENET_ESHAPE, "%s (output conv %zu): bias must be [%d]", b.name ? b.name : "?", i, co);
             for (int o = 0; o < co; ++o) shift[o] = b.data[o];
         }
-        // kernel -> [N][K] bf16 (K = (ky*k + kx)*cin + ci); conv 0 -> [32][64] = [w(27) 0(5) w(27) 0(5)] for the hi/lo input split
+        // kernel -> [N][K] bf16 (K = (ky*k + kx)*cin + ci); conv 0 -> [N][64] = [w(27) 0(5) w(27) 0(5)] for the hi/lo input split
         const int taps = c.k * c.k;
         const int N = co, K = i == 0 ? 64 : taps * c.cin;
         const int rows = (N + 127) / 128 * 128;     // every weight tile the kernels may touch exists (zero rows past N)
@@ -335,21 +354,33 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
     CKD(cudaMemcpy(d->warena, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice));
     CKD(cudaMemcpy(d->barena, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
     d->w_off = w_off; d->b_off = b_off;
-    std::memcpy(d->anchors, anchors, sizeof(d->anchors));
-    // activations: one buffer per conv output (the concat and residual sources and the taps stay addressable), workspaces
-    if (C != d->num_classes || !d->L[0].out) {
-        for (auto& l : d->L) { cudaFree(l.out); l.out = nullptr; }
+    // anchors in (head, anchor-in-layer) slots: the decode reads slot 3 * l + a for either network
+    for (int l = 0; l < (tiny ? 2 : 3); ++l)
+        for (int a = 0; a < 3; ++a) {
+            const int an = tiny ? Y::kTinyAnchorMask[l][a] : Y::kAnchorMask[l][a];
+            d->anchors[2 * (3 * l + a)] = anchors[2 * an];
+            d->anchors[2 * (3 * l + a) + 1] = anchors[2 * an + 1];
+        }
+    // activations: one buffer per conv output and per pooled conv input (the concat and residual sources and the taps stay
+    // addressable), workspaces; rebuilt when the network or the class count changes
+    if (C != d->num_classes || tiny != d->tiny || !d->L[0].out) {
+        free_layers(d);
         cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
+        d->d_cand = nullptr; d->d_cand_score = nullptr; d->d_boxes = nullptr; d->d_scores = nullptr; d->d_classes = nullptr; d->d_count = nullptr;
         d->num_classes = C;
+        d->tiny = tiny;
+        d->table = T;
+        d->L.assign(T.size(), LayerDev{});
         for (size_t i = 0; i < T.size(); ++i) {
             const ConvCfg& c = T[i];
             LayerDev& l = d->L[i];
-            l.Hi = c.src < 0 ? d->in_h : d->L[c.src].Ho;
-            l.Wi = c.src < 0 ? d->in_w : d->L[c.src].Wo;
+            l.Hi = Y::pooled(c.src < 0 ? d->in_h : d->L[c.src].Ho, c.pool);
+            l.Wi = Y::pooled(c.src < 0 ? d->in_w : d->L[c.src].Wo, c.pool);
             l.Ho = l.Hi / c.stride; l.Wo = l.Wi / c.stride;
             l.N = c.head >= 0 ? 3 * (5 + C) : c.cout;
             l.plan = Y::plan_igemm(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
             CKD(cudaMalloc(&l.out, (size_t)d->max_frames * l.Ho * l.Wo * l.N * (c.head >= 0 ? 4 : 2)));
+            if (c.pool) CKD(cudaMalloc(&l.pooled, (size_t)d->max_frames * l.Hi * l.Wi * c.cin * 2));
         }
         const size_t nc = (size_t)ncand(d), slots = (size_t)d->max_frames * C * Y::kMaxBoxes;
         CKD(cudaMalloc(&d->d_cand, (size_t)d->max_frames * nc * 16));
@@ -414,7 +445,7 @@ void whenet_det_destroy(whenet_det* d) {
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_graphs(d);
-    for (auto& l : d->L) cudaFree(l.out);
+    free_layers(d);
     cudaFree(d->warena); cudaFree(d->barena); cudaFree(d->d_frames); cudaFree(d->d_canvas);
     cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
     if (d->own_stream) cudaStreamDestroy(d->own_stream);
@@ -425,20 +456,27 @@ void whenet_det_destroy(whenet_det* d) {
 int whenet_det_debug_tap(whenet_det* d, int layer, float* out, size_t cap, size_t* n_elems) {
     if (!d) return fail(WHENET_EINVAL, "null detector");
     if (!d->loaded || d->last_n < 1) return fail(WHENET_ENOTFOUND, "no detection has run yet");
-    if (layer < -1 || layer >= (int)d->table.size()) return fail(WHENET_ENOTFOUND, "no conv layer %d (0..74, -1 = letterboxed canvas)", layer);
-    const size_t n = layer < 0 ? (size_t)d->last_n * d->in_h * d->in_w * 3 : (size_t)d->last_n * d->L[layer].Ho * d->L[layer].Wo * d->L[layer].N;
+    const int nl = (int)d->table.size();
+    const bool pool_tap = layer >= kPoolTap && layer < kPoolTap + nl && d->table[layer - kPoolTap].pool;
+    if (!pool_tap && (layer < -1 || layer >= nl))
+        return fail(WHENET_ENOTFOUND, "no tap %d (conv outputs 0..%d, -1 = letterboxed canvas, %d + i = the max-pooled input of tiny conv i)", layer,
+                    nl - 1, kPoolTap);
+    const LayerDev* l = pool_tap ? &d->L[layer - kPoolTap] : layer >= 0 ? &d->L[layer] : nullptr;
+    const size_t n = !l ? (size_t)d->last_n * d->in_h * d->in_w * 3
+                        : pool_tap ? (size_t)d->last_n * l->Hi * l->Wi * d->table[layer - kPoolTap].cin : (size_t)d->last_n * l->Ho * l->Wo * l->N;
     if (n_elems) *n_elems = n;
     if (!out) return 0;
     if (cap < n) return fail(WHENET_EINVAL, "tap %d needs %zu elements, buffer holds %zu", layer, n, cap);
     CKD(cudaSetDevice(d->device));
     CKD(cudaStreamSynchronize(d->stream));
-    if (layer < 0) {
+    if (!l) {
         std::vector<uint8_t> h(n);
         CKD(cudaMemcpy(h.data(), d->d_canvas, n, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < n; ++i) out[i] = h[i];
         return 0;
     }
-    return to_f32_tap(d->L[layer].out, d->table[layer].head >= 0, n, out);
+    if (pool_tap) return to_f32_tap(l->pooled, false, n, out);
+    return to_f32_tap(l->out, d->table[layer].head >= 0, n, out);
 }
 
 int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n, int H, int W, int cin, int c_up, const float* w, const float* bias,
@@ -450,7 +488,7 @@ int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n,
     if (leaky && cout % 8) return fail(WHENET_EINVAL, "bf16 outputs need cout %% 8 == 0");
     if (!leaky && (resid || up)) return fail(WHENET_EINVAL, "the linear fp32 conv has no residual or concat source");
     if (resid && up) return fail(WHENET_EINVAL, "residual and concat source together are not a YOLOv3 layer");
-    if (up && (k != 1 || c_up < 64 || c_up % 64 || c_up >= cin || H % 2 || W % 2)) return fail(WHENET_EINVAL, "bad concat shape");
+    if (up && (stride != 1 || c_up < 64 || c_up % 64 || c_up >= cin || H % 2 || W % 2)) return fail(WHENET_EINVAL, "bad concat shape");
     if (!up) c_up = 0;
     CKD(cudaSetDevice(d->device));
     const int Ho = H / stride, Wo = W / stride;
@@ -492,16 +530,39 @@ int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n,
     return rc ? WHENET_ECUDA : 0;
 }
 
+int whenet_det_debug_maxpool(whenet_det* d, const float* x, int n, int H, int W, int C, int stride, float* out) {
+    if (!d || !x || !out) return fail(WHENET_EINVAL, "null argument");
+    if (n < 1 || H < 1 || W < 1 || C < 8 || C % 8 || (stride != 1 && stride != 2))
+        return fail(WHENET_EINVAL, "bad max-pool shape (n=%d H=%d W=%d C=%d stride=%d)", n, H, W, C, stride);
+    CKD(cudaSetDevice(d->device));
+    const size_t ni = (size_t)n * H * W * C, no = (size_t)n * Y::pooled(H, stride) * Y::pooled(W, stride) * C;
+    std::vector<uint16_t> hx(ni);
+    for (size_t i = 0; i < ni; ++i) hx[i] = bf16_bits(x[i]);
+    void *dx = nullptr, *dout = nullptr;
+    if (cudaMalloc(&dx, ni * 2) || cudaMalloc(&dout, no * 2)) {
+        cudaFree(dx); cudaFree(dout);
+        return fail(WHENET_ECUDA, "out of device memory");
+    }
+    int rc = (int)cudaMemcpy(dx, hx.data(), ni * 2, cudaMemcpyHostToDevice);
+    if (!rc) rc = Y::launch_maxpool(d->stream, (const __nv_bfloat16*)dx, (__nv_bfloat16*)dout, n, H, W, C, stride);
+    if (!rc) rc = (int)cudaStreamSynchronize(d->stream);
+    if (!rc) rc = to_f32_tap(dout, false, no, out) ? -1 : 0;
+    cudaFree(dx); cudaFree(dout);
+    if (rc > 0) return fail(WHENET_ECUDA, "debug max-pool failed: %s", cudaGetErrorString((cudaError_t)rc));
+    return rc ? WHENET_ECUDA : 0;
+}
+
 int whenet_det_debug_decode(whenet_det* d, const float* head0, const float* head1, const float* head2, int n, int img_h, int img_w, float score,
                             float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
-    if (!d || !head0 || !head1 || !head2) return fail(WHENET_EINVAL, "null argument");
+    if (!d || !head0 || !head1 || (!head2 && !d->tiny)) return fail(WHENET_EINVAL, "null argument");
     if (int rc = check_frames(d, n, img_h, img_w)) return rc;
     if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
     CKD(cudaSetDevice(d->device));
     const float* hs[3] = {head0, head1, head2};
     Y::DecodeParams p = decode_params(d, img_h, img_w, score, iou, max_boxes);
-    for (int l = 0; l < 3; ++l) {
-        const LayerDev& L = d->L[d->table.size() - 3 + l];
+    const int nh = num_heads(d);
+    for (int l = 0; l < nh; ++l) {
+        const LayerDev& L = d->L[d->table.size() - nh + l];
         const size_t bytes = (size_t)n * L.Ho * L.Wo * L.N * 4;
         CKD(cudaMemcpyAsync(L.out, hs[l], bytes, cudaMemcpyHostToDevice, d->stream));
     }

@@ -4,6 +4,9 @@
 ``YOLO(**vars(args))`` from reference ``demo_video.py:41`` works: unknown keywords are kept as attributes, as the
 reference's ``self.__dict__.update(kwargs)`` does.  ``model_path=None`` means seeded random weights (``yolo_arch.random_weights``),
 flagged by ``self.random_weights``; the reference's trained ``head_detect.h5`` is not shipped.
+
+As in the reference (yolo_postprocess.py:71-79), the anchors pick the network: 9 anchors mean YOLOv3 (``yolo_body``), 6 mean
+tiny YOLOv3 (``tiny_yolo_body``, ``self.tiny``).
 """
 from __future__ import annotations
 
@@ -48,18 +51,19 @@ class YOLO:
         yolo_arch.check_size(*size)
         self.model_image_size = size
         self.anchors = yolo_arch.read_anchors(os.path.expanduser(anchors_path)) if anchors_path else yolo_arch.DEFAULT_ANCHORS.copy()
-        if self.anchors.shape != (9, 2):
-            raise ValueError("YOLOv3 needs 9 anchors, %s has %d" % (anchors_path, len(self.anchors)))
+        if self.anchors.shape not in ((9, 2), (6, 2)):
+            raise ValueError("YOLOv3 needs 9 anchors and tiny YOLOv3 6, %s has %d" % (anchors_path, len(self.anchors)))
+        self.tiny = len(self.anchors) == 6
         self.class_names = yolo_arch.read_classes(os.path.expanduser(classes_path)) if classes_path else list(yolo_arch.DEFAULT_CLASSES)
         self.random_weights = model_path is None
         if model_path is None:
-            names, w = yolo_arch.random_weights(seed, len(self.class_names))
+            names, w = yolo_arch.random_weights(seed, len(self.class_names), tiny=self.tiny)
         else:
             mp = os.path.expanduser(os.fspath(model_path))
             if not mp.endswith(".h5"):
                 raise ValueError("Keras model or weights must be a .h5 file.")     # yolo_postprocess.py:68
             names, w, _meta = h5lite.read_keras_weights(mp)
-        layers, num_classes = yolo_arch.map_weights(names, w)
+        layers, num_classes = yolo_arch.map_weights(names, w, tiny=self.tiny)
         if num_classes != len(self.class_names):
             raise ValueError("Mismatch between model and given anchor and class sizes: the model has %d classes, %d class names"
                              % (num_classes, len(self.class_names)))
@@ -71,12 +75,16 @@ class YOLO:
         check(self._L.whenet_det_create(C.byref(self._h), self.device, size[0], size[1], self.max_frames))
         self.load_layers(layers)
 
-    def load_layers(self, layers):
-        """Mapped layers (``yolo_arch.map_weights``) -> device."""
+    def load_layers(self, layers, anchors=None):
+        """Mapped layers (``yolo_arch.map_weights``) -> device.  ``anchors`` ((w, h) pairs, 9 or 6) replace the detector's
+        and with their count the network: pass them to load the layers of the other network into a live detector."""
+        a = self.anchors if anchors is None else np.asarray(anchors, np.float64).reshape(-1, 2)
         t, keep = _tensor_list(layers)
-        anchors = np.ascontiguousarray(self.anchors, np.float32)
-        check(self._L.whenet_det_load_weights(self._h, t, len(t), _ptr(anchors), len(anchors)))
+        a32 = np.ascontiguousarray(a, np.float32)
+        check(self._L.whenet_det_load_weights(self._h, t, len(t), _ptr(a32), len(a32)))
         del keep
+        self.anchors, self.tiny = a, len(a) == 6
+        self.num_classes = self._L.whenet_det_num_classes(self._h)
 
     # ------------------------------------------------------------------ reference surface
     def detect(self, image) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
@@ -115,7 +123,8 @@ class YOLO:
 
     # ------------------------------------------------------------------ test hooks
     def tap(self, layer: int) -> np.ndarray:
-        """float32 output of conv ``layer`` (0..74) of the last call, or (-1) its letterboxed canvas, flat."""
+        """float32 output of conv ``layer`` (0..74, tiny: 0..12) of the last call, (-1) its letterboxed canvas, or (100 + i)
+        the max-pooled input of tiny conv i, flat."""
         n = C.c_size_t(0)
         check(self._L.whenet_det_debug_tap(self._h, int(layer), None, 0, C.byref(n)))
         out = np.empty((n.value,), np.float32)
@@ -137,16 +146,27 @@ class YOLO:
                                             int(leaky), _ptr(resid), _ptr(out)))
         return out
 
+    def debug_maxpool(self, x, stride: int):
+        """The device 2x2 max-pool (TF SAME) of x (n,H,W,C), rounded to bf16 on the way in -> (n, ceil(H/s), ceil(W/s), C)."""
+        x = np.ascontiguousarray(x, np.float32)
+        n, H, W, c = x.shape
+        out = np.empty((n, -(-H // stride), -(-W // stride), c), np.float32)
+        check(self._L.whenet_det_debug_maxpool(self._h, _ptr(x), n, H, W, c, int(stride), _ptr(out)))
+        return out
+
     def debug_decode(self, heads, img_h: int, img_w: int, max_boxes: int = 20):
-        """Raw fp32 head tensors [(n,gh,gw,3(5+C)) x 3] -> per-frame (boxes, scores, classes) through the device decode + NMS."""
+        """Raw fp32 head tensors [(n,gh,gw,3(5+C)) x 3 (tiny: 2)] -> per-frame (boxes, scores, classes) through the device
+        decode + NMS."""
         hs = [np.ascontiguousarray(h, np.float32) for h in heads]
+        if len(hs) != len(yolo_arch.heads(self.tiny)):
+            raise ValueError("%d head tensors for a detector with %d heads" % (len(hs), len(yolo_arch.heads(self.tiny))))
         n = hs[0].shape[0]
         slots = self.num_classes * max_boxes
         boxes = np.empty((n, slots, 4), np.float32)
         scores = np.empty((n, slots), np.float32)
         classes = np.empty((n, slots), np.int32)
         counts = np.empty((n,), np.int32)
-        check(self._L.whenet_det_debug_decode(self._h, _ptr(hs[0]), _ptr(hs[1]), _ptr(hs[2]), n, img_h, img_w, self.score, self.iou, max_boxes,
+        check(self._L.whenet_det_debug_decode(self._h, _ptr(hs[0]), _ptr(hs[1]), _ptr(hs[2]) if len(hs) > 2 else None, n, img_h, img_w, self.score, self.iou, max_boxes,
                                               _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
         return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(n)]
 

@@ -7,6 +7,26 @@ and three output convs of the heads last.  A conv reads the output of conv ``src
 conv reads ``[upsample2x(out[up]), out[src]]`` (upsampled tensor first, model.py:81,87); ``res`` adds ``out[res]`` after
 the LeakyReLU (resblock ``x + y``, model.py:46).  Stride-2 convs are ZeroPadding2D(((1,0),(1,0))) + VALID, every other
 conv SAME: both are "pad 1 top/left" for a 3x3 kernel.
+
+Tiny YOLOv3 (``tiny_yolo_body``, model.py:92-122; the reference builds it when the anchors file holds 6 anchors,
+yolo_postprocess.py:71-79) is ``TINY_LAYERS``: 13 convs, all stride 1, six of them reading their source through a 2x2
+max-pool (``pool``: 2 = stride 2, 1 = stride 1; MaxPooling2D padding 'same', so the stride-1 pool pads one row and column
+at the bottom/right that never win the max).  Two heads, 13x13 and 26x26 at 416, decoded with ``TINY_ANCHOR_MASK``
+(model.py:199; anchor 0 is never used).
+
+Weight order of the tiny model.  Keras 2.1.6 ``load_weights`` walks ``model.layers``, which sorts the layers by decreasing
+depth, the depth of a layer being its longest path to an output counting every layer (BatchNorm, LeakyReLU, pooling,
+upsampling and concatenation included); layers at the same depth keep the order in which the walk back from
+``outputs[0]``, then ``outputs[1]``, first met them.  The chain conv2d_1 .. conv2d_8 comes first.  Of the layers after
+conv2d_8 (the 1x1 to 256), the 1x1 to 128 before the upsample is depth 8 (to ``y2``: BN, LeakyReLU, UpSampling2D,
+Concatenate, conv, BN, LeakyReLU, output conv), the 3x3 to 512 of ``y1`` and the 3x3 concat conv of ``y2`` are both depth
+3 (``y1``'s first), and the two output convs depth 0 (``y1``'s first).  Conv and BatchNorm names number in creation order
+(the order tiny_yolo_body builds them): the 3x3 to 512 is conv2d_9, ``y1``'s output conv conv2d_10, the 1x1 to 128
+conv2d_11, the concat conv conv2d_12 and ``y2``'s output conv conv2d_13, so the weight order is conv2d_1 .. conv2d_8,
+conv2d_11, conv2d_9, conv2d_12, conv2d_10, conv2d_13 and batch_normalization_1 .. 8, 10, 9, 11.  This order is derived,
+not checked against a file Keras wrote.  Within each tie (conv2d_9 / conv2d_12, conv2d_10 / conv2d_13, and their
+BatchNorms) the shapes differ, so a file in the other order is refused with a "kernel shape" or BatchNorm-shape
+ValueError, never loaded wrongly.
 """
 from __future__ import annotations
 
@@ -19,6 +39,7 @@ import numpy as np
 BN_EPS = 1e-3           # keras BatchNormalization default epsilon
 LEAKY = 0.1             # model.py:35
 ANCHOR_MASK = [[6, 7, 8], [3, 4, 5], [0, 1, 2]]     # model.py:199
+TINY_ANCHOR_MASK = [[3, 4, 5], [1, 2, 3]]          # model.py:199, two heads
 # the nine YOLOv3 COCO anchor clusters (w, h) of the YOLOv3 paper (Redmon & Farhadi 2018, section 2.3)
 DEFAULT_ANCHORS = np.array([[10, 13], [16, 30], [33, 23], [30, 61], [62, 45], [59, 119], [116, 90], [156, 198], [373, 326]],
                            dtype=np.float64)
@@ -39,10 +60,12 @@ class Conv:
     up: Optional[int] = None      # concat: conv whose output is upsampled x2 and put first
     keras_id: int = 0     # creation number: conv2d_<keras_id> in a freshly built model
     head: Optional[int] = None    # output conv of head l (0: 13x13 at 416, 1: 26x26, 2: 52x52)
+    pool: int = 0         # tiny: the input is out[src] max-pooled 2x2 with this stride (0: no pool)
+    tiny: bool = False    # a TINY_LAYERS row
 
     @property
     def c_up(self) -> int:
-        return 0 if self.up is None else LAYERS[self.up].cout
+        return 0 if self.up is None else table(self.tiny)[self.up].cout
 
 
 def _build() -> List[Conv]:
@@ -95,10 +118,41 @@ def _build() -> List[Conv]:
     return [Conv(keras_id=keras_id[r["idx"]], **r) for r in rows]
 
 
+def _build_tiny() -> List[Conv]:
+    rows = []
+    # (k, cin, cout, src, pool, up, head, keras_id)
+    for k, cin, cout_, src, pool, up, head, kid in (
+            (3, 3, 16, -1, 0, None, None, 1), (3, 16, 32, 0, 2, None, None, 2), (3, 32, 64, 1, 2, None, None, 3),
+            (3, 64, 128, 2, 2, None, None, 4), (3, 128, 256, 3, 2, None, None, 5), (3, 256, 512, 4, 2, None, None, 6),
+            (3, 512, 1024, 5, 1, None, None, 7), (1, 1024, 256, 6, 0, None, None, 8), (1, 256, 128, 7, 0, None, None, 11),
+            (3, 256, 512, 7, 0, None, None, 9), (3, 128 + 256, 256, 4, 0, 8, None, 12), (1, 512, 0, 9, 0, None, 0, 10),
+            (1, 256, 0, 10, 0, None, 1, 13)):
+        rows.append(Conv(idx=len(rows), k=k, stride=1, cin=cin, cout=cout_, bn=head is None, src=src, up=up, keras_id=kid, head=head,
+                         pool=pool, tiny=True))
+    return rows
+
+
 LAYERS: List[Conv] = _build()
 N_CONV = len(LAYERS)                 # 75
 HEADS = [L.idx for L in LAYERS if L.head is not None]          # the three output convs, head 0..2
 SKIP_LAYERS = sorted({L.src for L in LAYERS if L.up is not None})
+
+TINY_LAYERS: List[Conv] = _build_tiny()
+TINY_N_CONV = len(TINY_LAYERS)       # 13
+TINY_HEADS = [L.idx for L in TINY_LAYERS if L.head is not None]    # the two output convs, head 0, 1
+TINY_POOLED = [L.idx for L in TINY_LAYERS if L.pool]               # convs whose input is max-pooled
+
+
+def table(tiny: bool = False) -> List[Conv]:
+    return TINY_LAYERS if tiny else LAYERS
+
+
+def heads(tiny: bool = False) -> List[int]:
+    return TINY_HEADS if tiny else HEADS
+
+
+def anchor_mask(tiny: bool = False) -> List[List[int]]:
+    return TINY_ANCHOR_MASK if tiny else ANCHOR_MASK
 
 
 def head_channels(num_classes: int) -> int:
@@ -109,16 +163,21 @@ def cout(L: Conv, num_classes: int) -> int:
     return head_channels(num_classes) if L.head is not None else L.cout
 
 
-def out_hw(h: int, w: int) -> List[Tuple[int, int]]:
+def in_hw(h: int, w: int, tiny: bool = False) -> List[Tuple[int, int]]:
+    """Input (height, width) of every conv for a (h, w) model input, after the max-pool of a tiny conv (TF SAME: ceil)."""
+    ins, outs = [], []
+    for L in table(tiny):
+        ih, iw = (h, w) if L.src < 0 else outs[L.src]
+        if L.pool:
+            ih, iw = -(-ih // L.pool), -(-iw // L.pool)
+        ins.append((ih, iw))
+        outs.append((ih // L.stride, iw // L.stride))
+    return ins
+
+
+def out_hw(h: int, w: int, tiny: bool = False) -> List[Tuple[int, int]]:
     """Output (height, width) of every conv for a (h, w) input."""
-    hw = []
-    for L in LAYERS:
-        if L.src < 0:
-            ih, iw = h, w
-        else:
-            ih, iw = hw[L.src]
-        hw.append((ih // L.stride, iw // L.stride))
-    return hw
+    return [(ih // L.stride, iw // L.stride) for L, (ih, iw) in zip(table(tiny), in_hw(h, w, tiny))]
 
 
 def check_size(h: int, w: int) -> None:
@@ -129,14 +188,15 @@ def check_size(h: int, w: int) -> None:
             raise ValueError("model_image_size must be multiples of 32 in [%d, %d], got (%r, %r)" % (MIN_SIZE, MAX_SIZE, h, w))
 
 
-def macs_per_frame(h: int, w: int, num_classes: int = 1) -> int:
-    """Multiply-accumulates of the 75 convs for one (h, w) frame (the algorithmic count: no padding, no tile rounding)."""
-    hw = out_hw(h, w)
-    return sum(hw[i][0] * hw[i][1] * L.k * L.k * L.cin * cout(L, num_classes) for i, L in enumerate(LAYERS))
+def macs_per_frame(h: int, w: int, num_classes: int = 1, tiny: bool = False) -> int:
+    """Multiply-accumulates of the 75 (tiny: 13) convs for one (h, w) frame (the algorithmic count: no padding, no tile
+    rounding, no pools)."""
+    hw = out_hw(h, w, tiny)
+    return sum(hw[i][0] * hw[i][1] * L.k * L.k * L.cin * cout(L, num_classes) for i, L in enumerate(table(tiny)))
 
 
-def num_candidates(h: int, w: int) -> int:
-    return sum(3 * (h // 32 << l) * (w // 32 << l) for l in range(3))
+def num_candidates(h: int, w: int, tiny: bool = False) -> int:
+    return sum(3 * (h // 32 << l) * (w // 32 << l) for l in range(2 if tiny else 3))
 
 
 def keras_names(L: Conv, bn_id: int) -> List[str]:
@@ -147,18 +207,18 @@ def keras_names(L: Conv, bn_id: int) -> List[str]:
                                                  for s in ("gamma", "beta", "moving_mean", "moving_variance")]
 
 
-def random_weights(seed: int = 0, num_classes: int = 1) -> Tuple[List[str], "OrderedDict[str, np.ndarray]"]:
+def random_weights(seed: int = 0, num_classes: int = 1, tiny: bool = False) -> Tuple[List[str], "OrderedDict[str, np.ndarray]"]:
     """Seeded weights with keras-yolo3 names and shapes, in file order (layer_names, {name: float32}).
 
     Kernels are N(0, 1/fan_in) and BatchNorm statistics are randomised (gamma, beta, mean, var all away from the identity) so
     that BN folding is exercised; with the 0.5 kernel gain of the residual branches the activations stay O(1) through all 75
     layers.  Output-conv kernels are small and their biases zero: head logits near 0, scores sigmoid * sigmoid near 0.25."""
     rng = np.random.default_rng(seed)
-    bn_ids = _bn_ids()
+    bn_ids = _bn_ids(tiny)
     names: List[str] = []
     w: "OrderedDict[str, np.ndarray]" = OrderedDict()
     convs, bns = [], []
-    for L in LAYERS:
+    for L in table(tiny):
         co = cout(L, num_classes)
         fan_in = L.k * L.k * L.cin
         gain = 0.5 if (L.res is not None) else 1.0
@@ -176,7 +236,7 @@ def random_weights(seed: int = 0, num_classes: int = 1) -> Tuple[List[str], "Ord
             convs[-1][1][rest[0]] = np.zeros((co,), np.float32)
     # file order: every conv directly followed by its BatchNorm (the relative order of each kind is what matters, see _classify)
     bn_iter = iter(bns)
-    for L, (cn, cw) in zip(LAYERS, convs):
+    for L, (cn, cw) in zip(table(tiny), convs):
         names.append(cn)
         w.update(cw)
         if L.bn:
@@ -186,9 +246,9 @@ def random_weights(seed: int = 0, num_classes: int = 1) -> Tuple[List[str], "Ord
     return names, w
 
 
-def _bn_ids() -> Dict[int, int]:
+def _bn_ids(tiny: bool = False) -> Dict[int, int]:
     """batch_normalization_<id> of every BN conv: BN layers are numbered in creation order like the convs."""
-    by_creation = sorted((L for L in LAYERS if L.bn), key=lambda L: L.keras_id)
+    by_creation = sorted((L for L in table(tiny) if L.bn), key=lambda L: L.keras_id)
     return {L.idx: i + 1 for i, L in enumerate(by_creation)}
 
 
@@ -216,25 +276,29 @@ def _classify(layer_names: List[str], weights: Dict[str, np.ndarray]):
     return convs, bns
 
 
-def map_weights(layer_names: List[str], weights: Dict[str, np.ndarray]):
+def map_weights(layer_names: List[str], weights: Dict[str, np.ndarray], tiny: bool = False):
     """File tensors -> per-table-layer dicts {kernel, bias | gamma, beta, moving_mean, moving_variance, name}.
 
     Layers are matched by ORDER among the layers that carry weights (what Keras ``load_weights`` does), convs and
     BatchNorms each in their own sequence, never by name: the conv2d_<N> numbering depends on the session that built the
-    model.  Returns (layers, num_classes).  Anything that does not fit the table raises ValueError naming the layer."""
+    model.  ``tiny``: the file is a tiny YOLOv3 (TINY_LAYERS).  Returns (layers, num_classes).  Anything that does not fit
+    the table raises ValueError naming the layer or the count."""
+    T = table(tiny)
+    net = "tiny YOLOv3 (6 anchors)" if tiny else "YOLOv3 (9 anchors)"
     convs, bns = _classify(layer_names, weights)
-    if len(convs) != N_CONV:
-        raise ValueError("expected %d conv layers for YOLOv3, the file has %d" % (N_CONV, len(convs)))
-    n_bn = sum(L.bn for L in LAYERS)
+    if len(convs) != len(T):
+        raise ValueError("expected %d conv layers for %s, the file has %d" % (len(T), net, len(convs)))
+    n_bn = sum(L.bn for L in T)
     if len(bns) != n_bn:
-        raise ValueError("expected %d BatchNormalization layers for YOLOv3, the file has %d" % (n_bn, len(bns)))
-    hc = convs[HEADS[0]][1]["kernel"].shape[-1] if convs[HEADS[0]][1]["kernel"].ndim == 4 else -1
+        raise ValueError("expected %d BatchNormalization layers for %s, the file has %d" % (n_bn, net, len(bns)))
+    h0 = heads(tiny)[0]
+    hc = convs[h0][1]["kernel"].shape[-1] if convs[h0][1]["kernel"].ndim == 4 else -1
     if hc < 18 or hc % 3 or (hc // 3 - 5) < 1:
-        raise ValueError("layer %s: output conv has %d channels, not 3 * (5 + classes)" % (convs[HEADS[0]][0], hc))
+        raise ValueError("layer %s: output conv has %d channels, not 3 * (5 + classes)" % (convs[h0][0], hc))
     num_classes = hc // 3 - 5
     out = []
     bn_iter = iter(bns)
-    for L, (cname, g) in zip(LAYERS, convs):
+    for L, (cname, g) in zip(T, convs):
         co = cout(L, num_classes)
         want = (L.k, L.k, L.cin, co)
         if tuple(g["kernel"].shape) != want:

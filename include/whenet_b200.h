@@ -215,10 +215,12 @@ typedef struct whenet_det whenet_det;
 int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, int max_frames);
 
 /* replaces: load_model / yolo_model.load_weights(model_path) (yolo_postprocess.py:74-79) and _get_anchors (:59-64).
- * `tensors`: the 75 convs in Keras weight order (whenet_b200/yolo_arch.py), each its kernel [k,k,cin,cout] followed by
- * BatchNorm gamma, beta, moving_mean, moving_variance (bias-free convs) or by its bias (the three output convs); BatchNorm
- * (eps 1e-3) is folded in double and the kernels rounded once to bf16.  The class count follows from the output convs'
- * width 3 * (5 + classes).  `anchors`: 9 (w, h) pairs in input pixels. */
+ * `anchors`: 9 (w, h) pairs in input pixels for YOLOv3 (yolo_body), 6 for tiny YOLOv3 (tiny_yolo_body, model.py:92-122);
+ * any other count is WHENET_EINVAL.  `tensors`: the network's 75 (tiny: 13) convs in Keras weight order
+ * (whenet_b200/yolo_arch.py), each its kernel [k,k,cin,cout] followed by BatchNorm gamma, beta, moving_mean,
+ * moving_variance (bias-free convs) or by its bias (the output convs); BatchNorm (eps 1e-3) is folded in double and the
+ * kernels rounded once to bf16.  The class count follows from the output convs' width 3 * (5 + classes).  Loading the
+ * other network or another class count into a live detector rebuilds its buffers and captured graphs. */
 int whenet_det_load_weights(whenet_det* det, const whenet_tensor* tensors, int n_tensors, const float* anchors, int n_anchors);
 
 /* Number of classes of the loaded weights (0 before whenet_det_load_weights). */
@@ -242,17 +244,23 @@ int whenet_det_synchronize(whenet_det* det);
 void whenet_det_destroy(whenet_det* det);
 
 /* ---- detector test hooks (no reference counterpart) ---- */
-/* float32 copy of the output of conv `layer` (0..74, table order) of the last detect call (n x Ho x Wo x Cout), or with
- * layer = -1 of its letterboxed uint8 canvas (n x input_h x input_w x 3). out=NULL queries the element count. */
+/* float32 copy of the output of conv `layer` (0..74, tiny: 0..12, table order) of the last detect call (n x Ho x Wo x Cout),
+ * with layer = -1 of its letterboxed uint8 canvas (n x input_h x input_w x 3), or with layer = 100 + i of the max-pooled
+ * input of tiny conv i (i = 1..6; n x Hi x Wi x Cin). out=NULL queries the element count. */
 int whenet_det_debug_tap(whenet_det* det, int layer, float* out, size_t cap_elems, size_t* n_elems);
 /* One conv through the detector's implicit-GEMM kernel on host float32 arrays (rounded to bf16 on the way in):
  * x n x H x W x (cin - c_up); `up` NULL or the concat source n x H/2 x W/2 x c_up (put first, read upsampled x2);
- * w [k][k][cin][cout]; k = 1 or 3, stride 1 or 2 (3x3 only; padding 1 top/left); leaky != 0: bias + LeakyReLU(0.1)
- * (+ resid n x Ho x Wo x cout) rounded to bf16, leaky = 0: bias only, fp32 output (the output convs). */
+ * w [k][k][cin][cout]; k = 1 or 3, stride 1 or 2 (3x3 only; padding 1 top/left; a concat conv has stride 1);
+ * leaky != 0: bias + LeakyReLU(0.1) (+ resid n x Ho x Wo x cout) rounded to bf16, leaky = 0: bias only, fp32 output
+ * (the output convs). */
 int whenet_det_debug_conv(whenet_det* det, const float* x, const float* up, int n, int H, int W, int cin, int c_up,
                           const float* w, const float* bias, int k, int stride, int cout, int leaky, const float* resid, float* out);
+/* The detector's 2x2 max-pool (tiny YOLOv3's MaxPooling2D, padding 'same': n x ceil(H/stride) x ceil(W/stride) x C, padded
+ * cells never win) on host float32 arrays rounded to bf16 on the way in; x n x H x W x C, C a multiple of 8, stride 1 or 2. */
+int whenet_det_debug_maxpool(whenet_det* det, const float* x, int n, int H, int W, int C, int stride, float* out);
 /* Decode + NMS alone: host fp32 head logits (n x gh_l x gw_l x 3(5+C) for the detector's input size) of frames of
- * img_h x img_w pixels -> the outputs of whenet_det_detect_u8. */
+ * img_h x img_w pixels -> the outputs of whenet_det_detect_u8.  A tiny YOLOv3 detector has two heads: head2 is ignored and
+ * may be NULL. */
 int whenet_det_debug_decode(whenet_det* det, const float* head0, const float* head1, const float* head2, int n, int img_h, int img_w,
                             float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
 

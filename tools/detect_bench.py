@@ -1,8 +1,9 @@
 """Detector throughput on one GPU: frames/s and TFLOP/s of whenet_b200.YOLO at 416^2 and 608^2 for n = 1 and 8 frames per
 call, a per-kernel breakdown from CUDA events (torch.profiler), and the full detect_and_estimate frames/s with the head
-biases set so that each frame yields about 20 boxes.  Prints the card's name and power limit of the same run.
+biases set so that each frame yields about 20 boxes.  Prints the card's name, power limit and max SM clock of the same run.
+``--tiny`` measures tiny YOLOv3 (the 6 anchors of tests/golden/tiny_yolo_anchors.txt) instead of YOLOv3.
 
-    python tools/detect_bench.py [--iters 50] [--out detect_bench.json]
+    python tools/detect_bench.py [--tiny] [--iters 50] [--out detect_bench.json]
 """
 import argparse
 import json
@@ -17,6 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 PEAK_BF16_DENSE = 989e12        # H100 SXM data sheet, dense BF16 (700 W part)
+TINY_ANCHORS = os.path.join(ROOT, "tests", "golden", "tiny_yolo_anchors.txt")
 
 
 def card():
@@ -58,6 +60,8 @@ def kernel_table(fn):
     for e in prof.events():
         if e.device_type == torch.autograd.DeviceType.CUDA:
             name = e.name.split("(")[0].replace("void ", "")
+            if "yolo_conv0_kernel" in e.name:
+                name = "yolo_conv0_kernel"
             for key in ("conv_igemm_kernel<0", "conv_igemm_kernel<1", "conv_igemm_kernel<2", "conv_igemm_kernel<3"):
                 if key in e.name:
                     name = "conv_igemm[%s]" % {"0": "leaky", "1": "leaky+res", "2": "concat", "3": "head fp32"}[key[-1]]
@@ -71,18 +75,20 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--tiny", action="store_true", help="tiny YOLOv3 (6 anchors) instead of YOLOv3")
     a = ap.parse_args()
     import torch
     import whenet_b200
     from whenet_b200 import yolo_arch as Y
     if not torch.cuda.is_available():
         raise SystemExit("no GPU: nothing to measure")
-    res = {"card": card(), "device": torch.cuda.get_device_name(0), "runs": []}
-    print("card:", res["card"])
+    anchors = TINY_ANCHORS if a.tiny else None
+    res = {"card": card(), "device": torch.cuda.get_device_name(0), "network": "tiny YOLOv3" if a.tiny else "YOLOv3", "runs": []}
+    print("card:", res["card"], " network:", res["network"])
     f = frame1080()
     for size in (416, 608):
-        m = whenet_b200.YOLO(None, model_image_size=(size, size), max_frames=8)
-        flops = 2.0 * Y.macs_per_frame(size, size)
+        m = whenet_b200.YOLO(None, anchors_path=anchors, model_image_size=(size, size), max_frames=8)
+        flops = 2.0 * Y.macs_per_frame(size, size, tiny=a.tiny)
         for n in (1, 8):
             frames = np.stack([f] * n)[:, :, :, ::-1].copy()
             d_frames = torch.from_numpy(frames).cuda()
@@ -100,13 +106,13 @@ def main():
                 print("    %-40s %8.4f ms  x%d" % tuple(k))
         m.close()
     # full pipeline: head objectness biases raised so that about 20 boxes survive NMS per frame
-    m = whenet_b200.YOLO(None, max_frames=1)
-    names, w = Y.random_weights(0)
-    layers, _ = Y.map_weights(names, w)
+    m = whenet_b200.YOLO(None, anchors_path=anchors, max_frames=1)
+    names, w = Y.random_weights(0, tiny=a.tiny)
+    layers, _ = Y.map_weights(names, w, tiny=a.tiny)
     wn = whenet_b200.WHENet(whenet_b200.weights.DEFAULT_NPZ, device=0, precision="bf16", max_batch=64)
     best = None
     for bias in np.arange(-1.0, 3.01, 0.25):
-        for i in Y.HEADS:
+        for i in Y.heads(a.tiny):
             b = np.zeros_like(layers[i]["bias"])
             b[4::6] = bias
             layers[i]["bias"] = b
@@ -114,7 +120,7 @@ def main():
         k = len(m.detect(f[:, :, ::-1].copy())[0])
         if best is None or abs(k - 20) < abs(best[1] - 20):
             best = (bias, k)
-    for i in Y.HEADS:
+    for i in Y.heads(a.tiny):
         b = np.zeros_like(layers[i]["bias"])
         b[4::6] = best[0]
         layers[i]["bias"] = b

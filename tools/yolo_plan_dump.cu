@@ -1,7 +1,9 @@
 // Host-only dump of the YOLOv3 detector's implicit-GEMM tile plans (no GPU): plan_igemm of convs 1-74 of the library's own table
-// for a model input size, class count and SM count, or of single debug-conv shapes, plus the decode/NMS capacity constants.
+// (tiny YOLOv3: convs 1-12) for a model input size, class count and SM count, or of single debug-conv shapes, plus the
+// decode/NMS capacity constants.
 //   nvcc -std=c++17 -arch=sm_90a -o build_tmp/yolo_plan_dump tools/yolo_plan_dump.cu
 //   build_tmp/yolo_plan_dump net C SM [H W]         every legal input size (32..608 step 32 per side), or one
+//   build_tmp/yolo_plan_dump tiny C SM [H W]        the same for tiny YOLOv3 (lines start with "tiny" instead of "net")
 //   build_tmp/yolo_plan_dump conv SM Ho Wo N Cin k [Ho Wo N Cin k ...]
 #include <cstdio>
 #include <cstdlib>
@@ -21,27 +23,28 @@ static void plan_line(int Ho, int Wo, int N, int Cin, int k, int sm) {
 }
 
 // the per-layer shapes whenet_det_load_weights derives from the table
-static void net(int h, int w, int C, int sm) {
-    const std::vector<ConvCfg> T = make_table();
+static void net(int h, int w, int C, int sm, bool tiny) {
+    const std::vector<ConvCfg> T = tiny ? make_tiny_table() : make_table();
     std::vector<int> Ho(T.size()), Wo(T.size());
     for (size_t i = 0; i < T.size(); ++i) {
         const ConvCfg& c = T[i];
-        Ho[i] = (c.src < 0 ? h : Ho[c.src]) / c.stride;
-        Wo[i] = (c.src < 0 ? w : Wo[c.src]) / c.stride;
+        Ho[i] = pooled(c.src < 0 ? h : Ho[c.src], c.pool) / c.stride;
+        Wo[i] = pooled(c.src < 0 ? w : Wo[c.src], c.pool) / c.stride;
         if (i == 0) continue;                       // conv 0 is yolo_conv0_kernel
-        printf("net %d %d conv %zu mode %s stride %d ", h, w, i, mode_name(igemm_mode(c)), c.stride);
+        printf("%s %d %d conv %zu mode %s stride %d ", tiny ? "tiny" : "net", h, w, i, mode_name(igemm_mode(c)), c.stride);
         plan_line(Ho[i], Wo[i], c.head >= 0 ? 3 * (5 + C) : c.cout, c.cin, c.k, sm);
     }
 }
 
 int main(int argc, char** argv) {
     printf("nms per %d threads %d max_boxes %d\n", kNmsPer, kNmsThreads, kMaxBoxes);
-    if (argc >= 4 && std::string(argv[1]) == "net") {
+    if (argc >= 4 && (std::string(argv[1]) == "net" || std::string(argv[1]) == "tiny")) {
+        const bool tiny = std::string(argv[1]) == "tiny";
         const int C = atoi(argv[2]), sm = atoi(argv[3]);
-        if (argc >= 6) net(atoi(argv[4]), atoi(argv[5]), C, sm);
+        if (argc >= 6) net(atoi(argv[4]), atoi(argv[5]), C, sm, tiny);
         else
             for (int h = 32; h <= 608; h += 32)
-                for (int w = 32; w <= 608; w += 32) net(h, w, C, sm);
+                for (int w = 32; w <= 608; w += 32) net(h, w, C, sm, tiny);
         return 0;
     }
     if (argc >= 3 && std::string(argv[1]) == "conv" && (argc - 3) % 5 == 0) {
@@ -52,6 +55,6 @@ int main(int argc, char** argv) {
         }
         return 0;
     }
-    fprintf(stderr, "usage: %s net C SM [H W] | conv SM Ho Wo N Cin k [...]\n", argv[0]);
+    fprintf(stderr, "usage: %s net C SM [H W] | tiny C SM [H W] | conv SM Ho Wo N Cin k [...]\n", argv[0]);
     return 2;
 }
