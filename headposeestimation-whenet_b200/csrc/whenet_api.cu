@@ -215,7 +215,7 @@ struct whenet_ctx {
     cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr};
     // crop front-end staging
     uint8_t* d_frame = nullptr; size_t frame_cap = 0;
-    int4* d_rects = nullptr; int rects_cap = 0;
+    int4* d_rects = nullptr; int* d_frame_of = nullptr; int rects_cap = 0;
     // taps
     bool taps_on = false;
     std::map<std::string, std::pair<float*, size_t>> taps;
@@ -1126,6 +1126,76 @@ int bind_packed(whenet_ctx* c, const float* arena, size_t n_f32, const uint16_t*
     return 0;
 }
 
+// ----------------------------------------------------------------------------- crop front-end
+// Python's builtin max(0, t) / min(lim, u) on the numpy float32 scalars of demo_video.py:15-18: the second argument wins
+// only when it compares greater / smaller, so a NaN gives the bound (np.maximum / np.minimum would propagate it).
+inline float py_max0(float t) { return t > 0.f ? t : 0.f; }
+inline float py_min(float lim, float u) { return u < lim ? u : lim; }
+
+// int(v) (truncation toward zero) when it lies in [lo, hi]; false for NaN, +-inf and anything outside - decided in double
+// before the conversion, so no out-of-range float is ever cast to int.
+inline bool trunc_within(float v, int lo, int hi, int* out) {
+    const double t = std::trunc((double)v);
+    if (!(t >= lo && t <= hi)) return false;
+    *out = (int)t;
+    return true;
+}
+
+// The margin arithmetic of reference demo_video.py:13-21 (whenet_b200/crops.py enlarge_box) bit for bit: float32 throughout
+// (numpy 2 scalar rules), correctly rounded divisions by 10 and 5, and the far side grown from the ALREADY updated near side
+// as the reference does.  Returns whether the slice is non-empty and inside the frame (0 <= y0 < y1 <= H, 0 <= x0 < x1 <= W,
+// the predicate whenet_crop_resize_u8 enforces); r = (y0, y1, x0, x1) then, zeros otherwise.
+bool enlarge_box(const float* b, int H, int W, int32_t r[4]) {
+    float y_min = b[0], x_min = b[1], y_max = b[2], x_max = b[3];
+    y_min = py_max0(y_min - std::fabs(y_min - y_max) / 10.f);
+    y_max = py_min((float)H, y_max + std::fabs(y_min - y_max) / 10.f);
+    x_min = py_max0(x_min - std::fabs(x_min - x_max) / 5.f);
+    x_max = py_min((float)W, x_max + std::fabs(x_min - x_max) / 5.f);
+    int y0, y1, x0, x1;
+    const bool ok = trunc_within(y_min, 0, H, &y0) && trunc_within(y_max, 0, H, &y1) && trunc_within(x_min, 0, W, &x0) &&
+                    trunc_within(x_max, 0, W, &x1) && y0 < y1 && x0 < x1;
+    r[0] = ok ? y0 : 0; r[1] = ok ? y1 : 0; r[2] = ok ? x0 : 0; r[3] = ok ? x1 : 0;
+    return ok;
+}
+
+// Frames (uploaded into the context's staging buffer when on the host) and the crop table -> crop_resize_kernel, one launch
+// per 65535 crops (the grid's y limit).  rects: m x (y0, y1, x0, x1) host int32, an empty one marks a zero crop; frame_of:
+// m host frame indices or NULL (all frame 0).
+int launch_crops(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const int32_t* rects,
+                 const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
+    CK(cudaSetDevice(c->device));
+    const uint8_t* d_frames = frames;
+    if (!frames_are_device) {
+        const size_t bytes = (size_t)n * H * W * 3;
+        if (c->frame_cap < bytes) {
+            if (c->d_frame) cudaFree(c->d_frame);
+            c->d_frame = nullptr; c->frame_cap = 0;
+            CK(cudaMalloc(&c->d_frame, bytes));
+            c->frame_cap = bytes;
+        }
+        CK(cudaMemcpyAsync(c->d_frame, frames, bytes, cudaMemcpyHostToDevice, c->stream));
+        d_frames = c->d_frame;
+    }
+    if (c->rects_cap < m) {
+        if (c->d_rects) cudaFree(c->d_rects);
+        if (c->d_frame_of) cudaFree(c->d_frame_of);
+        c->d_rects = nullptr; c->d_frame_of = nullptr; c->rects_cap = 0;
+        CK(cudaMalloc(&c->d_rects, (size_t)m * sizeof(int4)));
+        CK(cudaMalloc(&c->d_frame_of, (size_t)m * sizeof(int)));
+        c->rects_cap = m;
+    }
+    CK(cudaMemcpyAsync(c->d_rects, rects, (size_t)m * sizeof(int4), cudaMemcpyHostToDevice, c->stream));
+    if (frame_of) CK(cudaMemcpyAsync(c->d_frame_of, frame_of, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    Scope sc(c, "crop_resize", (double)m * 224 * 224 * 3 * 2, 0.0);
+    for (int m0 = 0; m0 < m; m0 += 65535) {
+        const int mb = std::min(65535, m - m0);
+        whenet::crop_resize_kernel<<<dim3((224 * 224 + 255) / 256, mb), 256, 0, c->stream>>>(
+            d_frames, H, W, c->d_rects + m0, frame_of ? c->d_frame_of + m0 : nullptr, crops_out + (size_t)m0 * 224 * 224 * 3, swap_rb);
+        CK(cudaGetLastError());
+    }
+    return 0;
+}
+
 }  // namespace
 
 // ============================================================================= C ABI
@@ -1444,30 +1514,35 @@ int whenet_crop_resize_u8(whenet_ctx* c, const uint8_t* frame, int H, int W, int
             return fail(WHENET_EINVAL, "box %d: slice [%d:%d, %d:%d] is empty or outside the %dx%d frame (cv2.resize would raise)",
                         i, r[0], r[1], r[2], r[3], H, W);
     }
-    CK(cudaSetDevice(c->device));
-    const uint8_t* d_frame = frame;
-    if (!frame_is_device) {
-        const size_t bytes = (size_t)H * W * 3;
-        if (c->frame_cap < bytes) {
-            if (c->d_frame) cudaFree(c->d_frame);
-            c->d_frame = nullptr; c->frame_cap = 0;
-            CK(cudaMalloc(&c->d_frame, bytes));
-            c->frame_cap = bytes;
-        }
-        CK(cudaMemcpyAsync(c->d_frame, frame, bytes, cudaMemcpyHostToDevice, c->stream));
-        d_frame = c->d_frame;
+    return launch_crops(c, frame, 1, H, W, frame_is_device, rects, nullptr, m, swap_rb, crops_out);
+}
+
+int whenet_crop_boxes_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes,
+                         const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+    // the context is checked last so that every other argument can be validated without a GPU
+    if (!frames || !boxes || !frame_of || !crops_out) return fail(WHENET_EINVAL, "null frames, boxes, frame_of or crops_out");
+    if (n < 1 || n > 64) return fail(WHENET_EINVAL, "n=%d frames outside [1, 64]", n);
+    if (H < 1 || W < 1) return fail(WHENET_EINVAL, "bad frame size %dx%d", H, W);
+    if (m < 1) return fail(WHENET_EINVAL, "m=%d boxes", m);
+    for (int i = 0; i < m; ++i)
+        if (frame_of[i] < 0 || frame_of[i] >= n) return fail(WHENET_EINVAL, "box %d: frame_of=%d outside [0, %d)", i, frame_of[i], n);
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    std::vector<int32_t> rects((size_t)m * 4);
+    for (int i = 0; i < m; ++i) {
+        const bool ok = enlarge_box(boxes + 4 * i, H, W, &rects[(size_t)4 * i]);
+        if (valid_out) valid_out[i] = ok;
     }
-    if (c->rects_cap < m) {
-        if (c->d_rects) cudaFree(c->d_rects);
-        c->d_rects = nullptr; c->rects_cap = 0;
-        CK(cudaMalloc(&c->d_rects, (size_t)m * sizeof(int4)));
-        c->rects_cap = m;
-    }
-    CK(cudaMemcpyAsync(c->d_rects, rects, (size_t)m * sizeof(int4), cudaMemcpyHostToDevice, c->stream));
-    {
-        Scope sc(c, "crop_resize", (double)m * 224 * 224 * 3 * 2, 0.0);
-        whenet::crop_resize_kernel<<<dim3((224 * 224 + 255) / 256, m), 256, 0, c->stream>>>(d_frame, H, W, c->d_rects, crops_out, swap_rb);
-        CK(cudaGetLastError());
+    if (rects_out) memcpy(rects_out, rects.data(), rects.size() * sizeof(int32_t));
+    return launch_crops(c, frames, n, H, W, frames_are_device, rects.data(), frame_of, m, swap_rb, crops_out);
+}
+
+int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out) {
+    if (!boxes || m < 1 || H < 1 || W < 1) return fail(WHENET_EINVAL, "bad arguments");
+    for (int i = 0; i < m; ++i) {
+        int32_t r[4];
+        const bool ok = enlarge_box(boxes + 4 * i, H, W, r);
+        if (rects_out) memcpy(rects_out + 4 * i, r, sizeof(r));
+        if (valid_out) valid_out[i] = ok;
     }
     return 0;
 }
@@ -1759,6 +1834,7 @@ void whenet_destroy(whenet_ctx* c) {
     free_ws(c);
     if (c->d_frame) cudaFree(c->d_frame);
     if (c->d_rects) cudaFree(c->d_rects);
+    if (c->d_frame_of) cudaFree(c->d_frame_of);
     for (auto& kv : c->taps) cudaFree(kv.second.first);
     for (auto& p : c->ev_used) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }
     for (auto e : c->ev_pool) cudaEventDestroy(e);

@@ -1,38 +1,144 @@
-"""Frame -> head poses on the GPU (reference demo_video.py:54-58 steps 1-3 for every head of a frame at once)."""
+"""Frames -> head poses on the GPU: reference demo_video.py:49-63 (detect, then margin, crop, resize and get_angle for every
+head, demo_video.py:13-23 and 54-58) for the heads of many frames at once."""
 from __future__ import annotations
 
 import numpy as np
 
 from . import crops as _crops
-from ._lib import check
-from .whenet import _ptr
+from ._lib import WhenetError, check
+from .whenet import _is_device, _ptr
 
 
 def detect_and_estimate(yolo, whenet, frame_bgr):
-    """``frame_bgr``: H x W x 3 uint8 as cv2 delivers it.  The frame is uploaded once; the detector reads it on the device
-    (yolo.detect on its RGB view), only the small box arrays visit the host for the margin arithmetic
-    (crops.rects_from_boxes, demo_video.py:13-21), and the crops are cut, resized and fed to WHENet without leaving the device.
-
-    Returns (boxes (k,4) float32, scores (k,) float32, angles (k,3) float32 yaw/pitch/roll in degrees)."""
-    import torch
+    """``frame_bgr``: H x W x 3 uint8 as cv2 delivers it -> (boxes (k,4) float32, scores (k,) float32, angles (k,3) float32
+    yaw/pitch/roll in degrees).  The one-frame case of ``detect_and_estimate_frames``, except that a head whose slice is
+    empty or outside the frame raises ``WhenetError`` (code -1, naming the box and its slice) as cv2.resize raises in the
+    reference, instead of getting NaN angles."""
     frame = np.ascontiguousarray(frame_bgr, dtype=np.uint8)
     if frame.ndim != 3 or frame.shape[2] != 3:
         raise ValueError("frame must be H x W x 3 uint8")
-    H, W = frame.shape[:2]
+    return _run(yolo, whenet, frame[None], strict=True)[0]
+
+
+def detect_and_estimate_frames(yolo, whenet, frames_bgr):
+    """``frames_bgr``: (n, H, W, 3) uint8 BGR frames of one size, a numpy array or a contiguous CUDA uint8 tensor on
+    ``whenet.device`` -> n tuples (boxes (k,4) float32, scores (k,) float32, angles (k,3) float32), per frame bit-identical
+    to ``detect_and_estimate`` on that frame alone.
+
+    Frames go through the detector ``yolo.max_frames`` at a time (host frames are uploaded chunk by chunk into two reused
+    device buffers); each chunk's boxes are enlarged, cut out of that chunk's device frames, resized and fed to WHENet in
+    sub-batches of ``whenet.max_batch`` through one reused crop buffer, queued on WHENet's stream while the detector runs the
+    next chunk on its own.  One synchronisation at the end.
+
+    A head whose enlarged slice is empty or leaves the frame (where the reference's cv2.resize raises and ends the video
+    loop) gets NaN angles; its box and score are returned as the detector gave them."""
+    return _run(yolo, whenet, frames_bgr, strict=False)
+
+
+def _checked_frames(yolo, whenet, frames):
+    if yolo.device != whenet.device:
+        raise ValueError("the detector runs on device %d and WHENet on device %d" % (yolo.device, whenet.device))
+    if _is_device(frames):
+        if str(frames.dtype) != "torch.uint8" or not frames.is_contiguous():
+            raise ValueError("device frames must be a contiguous uint8 CUDA tensor")
+        if frames.device.index != whenet.device:
+            raise ValueError("frames are on cuda:%s, WHENet on cuda:%d" % (frames.device.index, whenet.device))
+    else:
+        frames = np.asarray(frames)
+        if frames.dtype != np.uint8:
+            raise ValueError("frames must be uint8, not %s" % frames.dtype)
+    if len(frames.shape) != 4 or frames.shape[3] != 3:
+        raise ValueError("frames must be (n, H, W, 3) uint8, not %s" % (tuple(frames.shape),))
+    return frames
+
+
+def _raise_first_invalid(L, boxes, H, W):
+    """detect_and_estimate's error: the first box whose slice cv2.resize would refuse, as whenet_crop_resize_u8 names it."""
+    valid = np.empty(len(boxes), np.int32)
+    check(L.whenet_debug_enlarge_boxes(_ptr(boxes), len(boxes), H, W, None, _ptr(valid)))
+    if valid.all():
+        return
+    i = int(np.flatnonzero(valid == 0)[0])
+    y0, y1, x0, x1 = _crops.enlarge_box(boxes[i], H, W)
+    raise WhenetError(-1, "box %d: slice [%d:%d, %d:%d] is empty or outside the %dx%d frame (cv2.resize would raise)"
+                      % (i, y0, y1, x0, x1, H, W))
+
+
+def _run(yolo, whenet, frames, strict):
+    frames = _checked_frames(yolo, whenet, frames)
+    n, H, W = (int(v) for v in frames.shape[:3])
+    if n == 0:
+        return []
+    import torch
+    L = whenet._L
+    dev = _is_device(frames)
+    step = yolo.max_frames
+    n_chunks = -(-n // step)
+    results = []            # per chunk: (detections, device angles or None, validity or None)
+    keep = []               # device buffers WHENet's stream may still read or write: alive until the final synchronisation
+    stage = [None, None]    # host frames: chunk k goes to stage[k % 2]
+    crop_buf = None
+
+    def chunk(k):
+        lo, hi = k * step, min(n, (k + 1) * step)
+        if dev:
+            return frames[lo:hi]
+        buf = stage[k % 2]
+        if buf is None:
+            buf = stage[k % 2] = torch.empty((min(step, n), H, W, 3), dtype=torch.uint8, device="cuda")
+        buf[:hi - lo].copy_(torch.from_numpy(np.ascontiguousarray(frames[lo:hi])))
+        torch.cuda.current_stream().synchronize()       # the detector reads it on its own stream
+        return buf[:hi - lo]
+
     with torch.cuda.device(whenet.device):
-        d_frame = torch.from_numpy(frame).to("cuda")
-        torch.cuda.current_stream().synchronize()
-        boxes, scores, _classes = yolo.detect_frames(d_frame[None])[0]
-        m = len(boxes)
-        if m == 0:
-            return boxes, scores, np.zeros((0, 3), np.float32)
-        rects = _crops.rects_from_boxes(boxes, H, W, True)
-        d_crops = torch.empty((m, 224, 224, 3), dtype=torch.uint8, device="cuda")
-        d_ang = torch.empty((m, 3), dtype=torch.float32, device="cuda")
-        L = whenet._L
-        check(L.whenet_crop_resize_u8(whenet._h, _ptr(d_frame), H, W, 1, _ptr(rects), m, 1, _ptr(d_crops)))
-        for off in range(0, m, whenet.max_batch):
-            nb = min(whenet.max_batch, m - off)
-            check(L.whenet_forward_u8(whenet._h, _ptr(d_crops[off:off + nb]), nb, 1, _ptr(d_ang[off:off + nb]), None, 1))
+        if dev:
+            torch.cuda.current_stream().synchronize()   # frames the caller wrote on torch's stream are complete
+        try:
+            cur = chunk(0)
+            for k in range(n_chunks):
+                nb = int(cur.shape[0])
+                dets = yolo.detect_frames(cur)          # synchronous, on the detector's stream
+                if k + 1 < n_chunks:
+                    if not dev:
+                        whenet.synchronize()            # chunk k-1's crops have read the buffer chunk k+1 goes to
+                    nxt = chunk(k + 1)
+                counts = [len(d[0]) for d in dets]
+                m = sum(counts)
+                if m == 0:
+                    results.append((dets, None, None))
+                else:
+                    boxes = np.ascontiguousarray(np.concatenate([d[0] for d in dets]), np.float32)
+                    frame_of = np.repeat(np.arange(nb, dtype=np.int32), counts)
+                    if strict:
+                        _raise_first_invalid(L, boxes, H, W)
+                    valid = np.empty(m, np.int32)
+                    d_ang = torch.empty((m, 3), dtype=torch.float32, device="cuda")
+                    keep.append(d_ang)
+                    for s in range(0, m, whenet.max_batch):
+                        mb = min(whenet.max_batch, m - s)
+                        if crop_buf is None or crop_buf.shape[0] < mb:
+                            crop_buf = torch.empty((mb, 224, 224, 3), dtype=torch.uint8, device="cuda")
+                            keep.append(crop_buf)
+                        check(L.whenet_crop_boxes_u8(whenet._h, _ptr(cur), nb, H, W, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, 1,
+                                                     _ptr(crop_buf), None, _ptr(valid[s:])))
+                        check(L.whenet_forward_u8(whenet._h, _ptr(crop_buf), mb, 1, _ptr(d_ang[s:s + mb]), None, 1))
+                    results.append((dets, d_ang, valid))
+                if k + 1 < n_chunks:
+                    keep.append(cur)
+                    cur = nxt
+        except BaseException:
+            L.whenet_synchronize(whenet._h)             # unchecked: the buffers must outlive the queued work on the way out
+            raise
         whenet.synchronize()
-        return boxes, scores, d_ang.cpu().numpy()
+        out = []
+        for dets, d_ang, valid in results:
+            if d_ang is None:
+                out.extend((b, s, np.zeros((0, 3), np.float32)) for b, s, _c in dets)
+                continue
+            ang = d_ang.cpu().numpy()
+            ang[valid == 0] = np.nan
+            off = 0
+            for b, s, _c in dets:
+                out.append((b, s, ang[off:off + len(b)].copy()))
+                off += len(b)
+        return out

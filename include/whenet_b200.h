@@ -119,6 +119,19 @@ int whenet_forward_f32(whenet_ctx* ctx, const float* nhwc_normalised, int n, int
 int whenet_crop_resize_u8(whenet_ctx* ctx, const uint8_t* frame, int H, int W, int frame_is_device,
                           const int32_t* rects, int m, int swap_rb, uint8_t* crops_out);
 
+/* replaces, for the heads of n frames at once, reference demo_video.py:13-23: the margin arithmetic (:13-19), the slice,
+ * cv2.cvtColor(BGR2RGB) and cv2.resize(.., (224,224)).  `frames`: n (1..64) x H x W x 3 uint8 (host, or device when
+ * frames_are_device); `boxes`: m x 4 float32 host array in the detector's order (y_min, x_min, y_max, x_max), unclipped,
+ * original pixels; `frame_of`: m int32 host frame indices in [0, n).  The margin arithmetic runs on the host in float32,
+ * bit for bit what whenet_b200/crops.py enlarge_box computes with numpy; a box whose slice is empty or leaves the frame
+ * (where cv2.resize would raise) gets valid_out 0 and an all-zero crop.  `crops_out`: m x 224 x 224 x 3 uint8 in DEVICE
+ * memory; `rects_out` (m x 4 slice bounds (y0, y1, x0, x1), zeros for an invalid box) and `valid_out` (m int32) are host
+ * arrays, each may be NULL, filled before the call returns.  The crops are asynchronous on the context's stream: feed them to
+ * whenet_forward_u8 with in_is_device=1.  One launch serves every crop; host frames are uploaded once per call. */
+int whenet_crop_boxes_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, int W, int frames_are_device,
+                         const float* boxes, const int32_t* frame_of, int m, int swap_rb,
+                         uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+
 /* Block until everything queued by this context has finished. */
 int whenet_synchronize(whenet_ctx* ctx);
 
@@ -165,6 +178,10 @@ int whenet_debug_read_trace(whenet_ctx* ctx, int64_t* out, int n_rows);
 /* Same for K1W (option "k1_variant" = 4, every block with an expand conv): output tile, strip length, channels per CTA,
  * crops per item (2 only where one tile is the whole image), epilogue warps (4 or 8), threads per CTA (768). */
 int whenet_debug_set_k1w_plan(whenet_ctx* ctx, int block, int th, int tw, int r, int cc, int nb, int n_epi, int nt);
+
+/* The margin arithmetic of whenet_crop_boxes_u8 alone, on the host (no context, no GPU): m boxes of an H x W frame ->
+ * rects_out / valid_out as that call fills them (each may be NULL). */
+int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out);
 
 /* Time every kernel of the NEXT forwards with CUDA events. */
 int whenet_profile_enable(whenet_ctx* ctx, int enable);
