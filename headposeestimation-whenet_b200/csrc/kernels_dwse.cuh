@@ -24,7 +24,7 @@
 #pragma once
 #include <cuda.h>
 
-#include "kernels_k1w.cuh"
+#include "kernels_fused.cuh"
 
 namespace whenet {
 namespace fused {
@@ -116,13 +116,13 @@ __global__ void __launch_bounds__((DwSeThreads<KS, S, HIN, CC>::value)) dwse_ker
     auto issue = [&](int ch, int buf) {
         const int cbase = SPATIAL ? 0 : ch * CC;
         const uint32_t bar = b_full + 8 * buf;
-        k1w::arrive_expect_tx(bar, (uint32_t)(TILE_TX + CST_TX));
+        tc::mbar::arrive_expect_tx(bar, (uint32_t)(TILE_TX + CST_TX));
         if (SPATIAL) {
             const int ty = ch / p.tiles_x, tx = ch - ty * p.tiles_x;
-            k1w::tma_4d(sT + buf * TILE_BYTES, &p.tmE, 0, tx * G::HO * S - p.pad, ty * G::HO * S - p.pad, n, bar);
+            tc::mbar::tma_4d(sT + buf * TILE_BYTES, &p.tmE, 0, tx * G::HO * S - p.pad, ty * G::HO * S - p.pad, n, bar);
         } else
-            k1w::tma_4d(sT + buf * TILE_BYTES, &p.tmE, cbase, -p.pad, -p.pad, n, bar);
-        k1w::tma_2d(sC + buf * CST_BYTES + CC * 4, &p.tmW, cbase, 0, bar);
+            tc::mbar::tma_4d(sT + buf * TILE_BYTES, &p.tmE, cbase, -p.pad, -p.pad, n, bar);
+        tc::mbar::tma_2d(sC + buf * CST_BYTES + CC * 4, &p.tmW, cbase, 0, bar);
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(sC + buf * CST_BYTES), "l"(p.b_dw + cbase), "r"((uint32_t)(CC * 4)), "r"(bar) : "memory");
     };
@@ -159,7 +159,7 @@ __global__ void __launch_bounds__((DwSeThreads<KS, S, HIN, CC>::value)) dwse_ker
     for (int ch = ch_begin; ch < ch_end; ++ch) {
         const int it = ch - ch_begin, buf = it & 1;
         const uint32_t par = (uint32_t)(it >> 1) & 1u;
-        k1w::wait(b_full + 8 * buf, par, s_abort, p.tflag);        // tile + constants of chunk ch have landed
+        tc::mbar::wait(b_full + 8 * buf, par, s_abort, p.tflag);        // tile + constants of chunk ch have landed
         if (active && !*s_abort) {
             const uint32_t cst = sC + buf * CST_BYTES;
             const float4 bq = lds_f4(cst + (uint32_t)cv * 16);
@@ -218,11 +218,11 @@ __global__ void __launch_bounds__((DwSeThreads<KS, S, HIN, CC>::value)) dwse_ker
                          "f"(sum[0]), "f"(sum[1]), "f"(sum[2]), "f"(sum[3]) : "memory");
         }
         // this warp is done with tile / constants / (its part of) the squeeze scratch of buffer `buf`
-        k1w::arrive_warp(b_empty + 8 * buf);
+        tc::mbar::arrive_warp(b_empty + 8 * buf);
         if (warp == 0) {
             // warp 0 closes the chunk: once EVERY warp has released the buffer it reduces the squeeze scratch and only then
             // refills the buffer with chunk ch+2 - no warp can reach chunk ch+2 (and overwrite the scratch) before that copy lands
-            k1w::wait(b_empty + 8 * buf, par, s_abort, p.tflag);
+            tc::mbar::wait(b_empty + 8 * buf, par, s_abort, p.tflag);
             finish_sums(ch, buf);
             __syncwarp();
             if (lane == 0 && ch + 2 < ch_end) issue(ch + 2, buf);

@@ -23,7 +23,7 @@
 #pragma once
 #include <cuda.h>
 
-#include "kernels_k1w.cuh"
+#include "kernels_fused.cuh"
 
 namespace whenet {
 namespace tc {
@@ -98,8 +98,8 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
             asm volatile("prefetch.tensormap [%0];" ::"l"(&p.tmA) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&p.tmW) : "memory");
             if (p.w_resident) {
-                k1w::arrive_expect_tx(b_w, (uint32_t)p.nkb * p.n_tile * 128);
-                for (int kb = 0; kb < p.nkb; ++kb) k1w::tma_2d(sW + (uint32_t)kb * p.n_tile * 128, &p.tmW, kb * 64, 0, b_w);
+                mbar::arrive_expect_tx(b_w, (uint32_t)p.nkb * p.n_tile * 128);
+                for (int kb = 0; kb < p.nkb; ++kb) mbar::tma_2d(sW + (uint32_t)kb * p.n_tile * 128, &p.tmW, kb * 64, 0, b_w);
             }
             int g = 0;                                  // global K-block counter of this CTA: ring slot = g % stages
             for (int tile = first; tile < p.tiles; tile += step) {
@@ -107,10 +107,10 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
                 for (int kb = 0; kb < p.nkb; ++kb, ++g) {
                     const int s = g % p.stages;
                     const uint32_t par = (uint32_t)(g / p.stages) & 1u;
-                    k1w::wait(b_empty + 8 * s, par ^ 1, s_abort, p.tflag);          // the MMAs that read this slot have completed
-                    k1w::arrive_expect_tx(b_full + 8 * s, stage_bytes);
-                    k1w::tma_2d(sRing + (uint32_t)s * stage_bytes, &p.tmA, kb * 64, mt * BM, b_full + 8 * s);
-                    if (!p.w_resident) k1w::tma_2d(sRing + (uint32_t)s * stage_bytes + p.a_stage, &p.tmW, kb * 64, nt * p.n_tile, b_full + 8 * s);
+                    mbar::wait(b_empty + 8 * s, par ^ 1, s_abort, p.tflag);          // the MMAs that read this slot have completed
+                    mbar::arrive_expect_tx(b_full + 8 * s, stage_bytes);
+                    mbar::tma_2d(sRing + (uint32_t)s * stage_bytes, &p.tmA, kb * 64, mt * BM, b_full + 8 * s);
+                    if (!p.w_resident) mbar::tma_2d(sRing + (uint32_t)s * stage_bytes + p.a_stage, &p.tmW, kb * 64, nt * p.n_tile, b_full + 8 * s);
                 }
             }
         }
@@ -121,11 +121,11 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
         const int wt = tid & 127;
         const T* resid = reinterpret_cast<const T*>(p.resid);
         T* out = reinterpret_cast<T*>(p.out);
-        if (p.w_resident) k1w::wait(b_w, 0, s_abort, p.tflag);
+        if (p.w_resident) mbar::wait(b_w, 0, s_abort, p.tflag);
         for (int tile = first + grp * step, k = grp; tile < p.tiles; tile += 2 * step, k += 2) {
             const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
             WgAcc<NT> acc;
-            if (k > 0) k1w::wait(b_turn + 8 * grp, (uint32_t)((k - 1) >> 1) & 1u, s_abort, p.tflag);    // the other group is done with tile k-1
+            if (k > 0) mbar::wait(b_turn + 8 * grp, (uint32_t)((k - 1) >> 1) & 1u, s_abort, p.tflag);    // the other group is done with tile k-1
             // one wgmma group per K block, up to two in flight: once block kb is issued, wait for block kb-1's group and hand
             // ITS slot back to the producer, so the MMAs of block kb-1 are still running while block kb is issued
             const int g0 = k * p.nkb;                            // ring slots are filled in tile order
@@ -133,21 +133,21 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
                 const int g = g0 + kb;
                 const int s = g % p.stages;
                 const uint32_t par = (uint32_t)(g / p.stages) & 1u;
-                k1w::wait((GATE ? b_ready : b_full) + 8 * s, par, s_abort, p.tflag);
+                mbar::wait((GATE ? b_ready : b_full) + 8 * s, par, s_abort, p.tflag);
                 const uint32_t a_st = sRing + (uint32_t)s * stage_bytes;
                 const uint32_t w_st = p.w_resident ? sW + (uint32_t)kb * NT * 128 : a_st + p.a_stage;
                 wg_mma_tile<BF16, NT>(acc, a_st, w_st, kb == p.nkb - 1 ? p.ksteps_last : 4, kb ? 1u : 0u);     // one commit group
                 if (kb > 0) {
                     wg_wait<1>();
                     asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");  // the whole warpgroup's MMAs are done with slot g-1
-                    if (wt == 0) k1w::arrive(b_empty + 8 * ((g - 1) % p.stages));
+                    if (wt == 0) mbar::arrive(b_empty + 8 * ((g - 1) % p.stages));
                 }
             }
             wg_wait<0>();
             asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");
             if (wt == 0) {
-                k1w::arrive(b_empty + 8 * ((g0 + p.nkb - 1) % p.stages));
-                k1w::arrive(b_turn + 8 * (grp ^ 1));
+                mbar::arrive(b_empty + 8 * ((g0 + p.nkb - 1) % p.stages));
+                mbar::arrive(b_turn + 8 * (grp ^ 1));
             }
             if (*s_abort) continue;
             // fragment -> output: register 4i + e = row 16 wq + lane/4 (+8 for e >= 2) of row half h,
@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
             for (int kb = 0; kb < p.nkb; ++kb, ++g) {
                 const int s = g % p.stages;
                 const uint32_t par = (uint32_t)(g / p.stages) & 1u;
-                k1w::wait(b_full + 8 * s, par, s_abort, p.tflag);
+                mbar::wait(b_full + 8 * s, par, s_abort, p.tflag);
                 const uint32_t a0 = sRing + (uint32_t)s * stage_bytes + swz;
                 if (kb * 8 + c < kchunks) {
 #pragma unroll
@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
                             sts128_(a0 + i * 2048, scale8s<T>(lds128(a0 + i * 2048), sG + g_row[i] + (uint32_t)((kb * 8 + c) * 8) * 4));
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                k1w::arrive_warp(b_ready + 8 * s);
+                mbar::arrive_warp(b_ready + 8 * s);
             }
         }
     }

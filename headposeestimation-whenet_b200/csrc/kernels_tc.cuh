@@ -15,6 +15,7 @@
 // Every mbarrier wait is bounded: a wait that exceeds its budget raises the context's timeout flag (mapped pinned host
 // memory) and the CTA bails out instead of hanging the GPU.
 #pragma once
+#include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -55,6 +56,61 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* t
     *reinterpret_cast<volatile int*>(tflag) = 1;
     return false;
 }
+
+// Barriers by shared-memory address and the TMA copies that complete on them, for the warp-specialised kernels (K2, KD),
+// whose roles share one abort flag per CTA.
+namespace mbar {
+
+// Bounded wait on a barrier given by its shared-memory address.  The loop body is try_wait + branch (ncu showed the
+// re-poll loop of the first version at 16-22 % of all issued instructions, taken from the warps that had work); the abort
+// flag is looked at every 64 polls only.  A protocol bug ends in the timeout flag instead of a hung GPU.
+// No suspend-time hint: with one, ptxas emits NANOSLEEP.SYNCS and the wake-up after the arrive was measured to cost the
+// waiting role far more than the polls it saves (K2: 1.9 us per 128-row tile of a K = 32 layer).
+__device__ __forceinline__ void wait(uint32_t bar_addr, uint32_t parity, volatile int* abort_flag, int* tflag) {
+    for (uint32_t outer = 0; outer < (1u << 18); ++outer) {
+        uint32_t done;
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\t"
+            "mov.u32 n, 64;\n"
+            "MBAR_POLL_%=:\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "@p bra MBAR_DONE_%=;\n\t"
+            "sub.u32 n, n, 1;\n\t"
+            "setp.ne.u32 p, n, 0;\n\t"
+            "@p bra MBAR_POLL_%=;\n\t"
+            "setp.eq.u32 p, n, 1;\n"          // false: n == 0 here
+            "MBAR_DONE_%=:\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done) : "r"(bar_addr), "r"(parity) : "memory");
+        if (done) return;
+        if (*abort_flag) return;
+    }
+    *abort_flag = 1;
+    *reinterpret_cast<volatile int*>(tflag) = 1;
+}
+__device__ __forceinline__ void arrive(uint32_t bar_addr) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_addr) : "memory");
+}
+// One arrival per WARP: __syncwarp orders the lanes' shared-memory accesses before lane 0's (releasing) arrive.  Per-thread
+// arrives are 32 serialised shared-memory atomics per warp on one word; with 20+ warps signalling 4-5 barriers per item they
+// kept the LSU busy for more than a thousand cycles per item.
+__device__ __forceinline__ void arrive_warp(uint32_t bar_addr) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) arrive(bar_addr);
+}
+__device__ __forceinline__ void arrive_expect_tx(uint32_t bar_addr, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_4d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, uint32_t bar_addr) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+                 ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar_addr) : "memory");
+}
+__device__ __forceinline__ void tma_2d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar_addr) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(bar_addr) : "memory");
+}
+
+}  // namespace mbar
 
 // K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA descriptor):
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 = 1 | [32,46) SBO >> 4 = 64 (8 rows x 128 B) | [62,64) layout = 1 (SWIZZLE_128B)

@@ -23,11 +23,9 @@
 #include "kernels_tc.cuh"
 #include "kernels_fused.cuh"
 #include "kernels_crop.cuh"
-#include "kernels_k1w.cuh"
 #include "kernels_k2.cuh"
 #include "kernels_tc32.cuh"
 #include "kernels_dwse.cuh"
-#include "kernels_stem_tc.cuh"
 #include <cudaTypedefs.h>
 
 // The fused-kernel launchers are instantiated in their own translation units (inst_k1_bf16.cu, inst_k1_f16.cu, inst_k1x.cu)
@@ -35,8 +33,7 @@ namespace whenet {
 namespace fused {
 #define WHENET_EXTERN_FUSED(T)                                                                            \
     extern template int launch_k1<T>(cudaStream_t, K1Params, int, int, int, int, size_t, int);            \
-    extern template int launch_dw_only<T>(cudaStream_t, K1Params, size_t, int);                           \
-    extern template int launch_k1w<T>(cudaStream_t, K1WParams, int, int, int, int, size_t, int, int);
+    extern template int launch_dw_only<T>(cudaStream_t, K1Params, size_t, int);
 WHENET_EXTERN_FUSED(__nv_bfloat16)
 WHENET_EXTERN_FUSED(__half)
 #undef WHENET_EXTERN_FUSED
@@ -111,15 +108,12 @@ struct BlockW {   // device pointers into the fp32 arena
     float *w_se2 = nullptr, *b_se2 = nullptr;     // [cse][cexp], [cexp]
     float *w_proj = nullptr, *b_proj = nullptr;   // [cexp][cout], [cout]
     void *wt_exp = nullptr, *wt_proj = nullptr;   // 16-bit [N][K] copies for the tensor-core path
-    void* wt_exp_h = nullptr;                     // 16-bit [cexp][cin]: 0.5 * weights (K1W; its shift is b_exp_h)
-    float* b_exp_h = nullptr;                     // 0.5 * BN shift of the expand conv (K1W)
     void* wt_exp_aug = nullptr;                   // 16-bit [cexp][cin+8]: 0.5*(weights | shift_hi | shift_lo) | 0... (K1)
     float *w_dw_h = nullptr, *b_dw_h = nullptr;   // 0.5 * depthwise weights / shift (K1)
-    void* w_dw16 = nullptr;                       // fp16 [k*k][cexp]: 0.5 * depthwise weights / kDwScale (HFMA2 depthwise of K1 / K1W)
+    void* w_dw16 = nullptr;                       // fp16 [k*k][cexp]: 0.5 * depthwise weights / kDwScale (HFMA2 depthwise of K1 / KD)
 };
 
 struct K1Plan { bool valid = false; whenet::fused::K1Params p{}; int R = 0; int NT = 256; size_t smem = 0; };
-struct K1WPlan { bool valid = false; whenet::fused::K1WParams p{}; int R = 0, NT = 0; size_t smem = 0; };
 struct TmapKey {
     int block, n; const void* ptr;
     bool operator<(const TmapKey& o) const { return block != o.block ? block < o.block : (n != o.n ? n < o.n : ptr < o.ptr); }
@@ -163,23 +157,15 @@ struct whenet_ctx {
     int kd_expand_k2 = 1;      // the expand GEMM of the KD route: 1 = persistent K2 kernel, 0 = pw_tc2
     int kd_tail = 0;           // KD computes the SE gate and gates its output itself (1) or leaves both to se_gate + the project conv (0)
     int se_batch = 1;          // batches >= 64: se_gate_batch_kernel (four crops per CTA)
-    int stem_tc = 0;           // bf16, uint8 input: 1 = the stem as an im2col GEMM on the tensor core (kernels_stem_tc.cuh) instead of 27 x 32 FFMAs
-                               // per pixel.  Correct (stem tap 2e-3 rms-relative: bf16 weights) but not faster: 0.346 vs 0.338 ms per 512 crops
     int pw3 = 1;               // gated projects with H*W >= 784: pw_tc3 (a CTA walks several tiles of one crop) instead of pw_tc2
     int dw1_kd = 1;            // bf16: the stem writes fp16 and block 1's depthwise runs on KD (spatial tiles, TMA, HFMA2) instead of K1's depthwise half
     int head_batch = 1;        // batches >= 64: GAP kernel + Dense/decode for four crops per CTA
     int kd_from = 7;           // bf16: blocks >= kd_from whose map fits one CTA run expand GEMM (fp16 E through L2) + KD; 0 = off
     std::vector<K1Plan> k1;
-    std::vector<K1WPlan> k1w;  // k1_variant 4: weight-stationary persistent K1 (TMA-staged input tiles)
-    std::map<TmapKey, CUtensorMap> tmaps;   // input tensor maps of K1W by (block, crops, buffer)
-    std::vector<CUtensorMap> tmap_w;        // weight tensor maps of K1W by block
-  // k1_variant 3: persistent warp-specialised K1 for the blocks with several tiles per crop
+    std::map<TmapKey, CUtensorMap> tmaps;   // KD tensor maps: E tiles by (100 + block, crops, buffer), depthwise weights by (200 + block, 0, pointer)
     int sm_count = 132;
-    int k1w_trace_block = 0;   // debug: the K1W launch of this block records where its roles wait (whenet_debug_read_trace)
-    long long* d_trace = nullptr;
     K1Plan dw1;                // block 1 (no expand): depthwise-only instance of K1
     int dw1_fused = 1;
-    int k1_variant = 1;        // 1 = K1, 4 = K1W (weight-stationary persistent CTAs, TMA input tiles) for every block with an expand conv
     cudaStream_t own_stream = nullptr, stream = nullptr, copy_stream = nullptr;
     bool weights_loaded = false;
     std::vector<BlockCfg> blocks;
@@ -341,8 +327,9 @@ int ensure_ws(whenet_ctx* c) {
     }
     for (const K1Plan& pl : c->k1)
         if (pl.valid) part = std::max(part, (size_t)pl.p.tiles_x * pl.p.tiles_y * pl.p.Cexp);
-    for (const K1WPlan& pl : c->k1w)
-        if (pl.valid) part = std::max(part, (size_t)pl.p.tiles * pl.p.Cexp);
+    // block 1 on KD (bf16): squeeze partials per 14x14 output tile
+    const BlockCfg& b1 = c->blocks[0];
+    if (c->precision == WHENET_PRECISION_BF16) part = std::max(part, (size_t)(b1.hin / 14) * (b1.hin / 14) * b1.cexp);
     if (c->dw1.valid) part = std::max(part, (size_t)c->dw1.p.tiles_x * c->dw1.p.tiles_y * c->dw1.p.Cexp);
     c->ws_io = io; c->ws_ex = ex; c->ws_dw = dw; c->ws_part = part;
     CK(cudaMalloc(&c->bufA, ch * io * es));
@@ -359,7 +346,7 @@ int ensure_ws(whenet_ctx* c) {
     return 0;
 }
 
-// ----------------------------------------------------------------------------- TMA tensor maps (K1W)
+// ----------------------------------------------------------------------------- TMA tensor maps (K2, KD)
 PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
     static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
     if (!fn) {
@@ -369,20 +356,6 @@ PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
             fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
     }
     return fn;
-}
-// NHWC activation tensor [n][H][H][C] (16-bit): box = {64 channels, box_w, box_h, box_n}, SWIZZLE_128B, zero fill outside
-int make_tmap_act(CUtensorMap* tm, const void* base, int n, int H, int C, int box_w, int box_h, int box_n, bool is_bf16) {
-    auto fn = tmap_encode_fn();
-    if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)H, (cuuint64_t)H, (cuuint64_t)n};
-    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * C * 2, (cuuint64_t)H * H * C * 2};
-    const cuuint32_t box[4] = {64, (cuuint32_t)box_w, (cuuint32_t)box_h, (cuuint32_t)box_n};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = fn(tm, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides,
-                          box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(activation %dx%dx%dx%d, box %dx%dx%d) failed: %d", n, H, H, C, box_n, box_h, box_w, (int)r);
-    return 0;
 }
 // K-major weight matrix [rows][K] (16-bit): box = {64, box_rows}
 int make_tmap_w(CUtensorMap* tm, const void* base, int rows, int K, int box_rows, bool is_bf16) {
@@ -547,18 +520,7 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
     {
         Scope sc(c, "stem", (double)nb * (kImgElems * (IN_U8 ? 1.0 : 4.0) + 112.0 * 112 * 32 * sizeof(T)),
                  2.0 * nb * 112.0 * 112 * 27 * 32);
-        bool stem_done = false;
-        if constexpr (IN_U8 && std::is_same<T, __nv_bfloat16>::value) {
-            if (c->stem_tc && c->use_tc && c->use_fused) {
-                // bf16 throughput mode, uint8 input: the stem as an im2col GEMM on the tensor core (kernels_stem_tc.cuh)
-                const int rc = stem_half ? whenet::launch_stem_tc<__half>(c->stream, (const uint8_t*)d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut, nb)
-                                         : whenet::launch_stem_tc<T>(c->stream, (const uint8_t*)d_in, cur, c->stem_params, c->lut, nb);
-                if (rc != 0) return fail(WHENET_ECUDA, "tensor-core stem launch failed (rc=%d)", rc);
-                stem_done = true;
-            }
-        }
-        if (stem_done) {
-        } else if (stem_half) {
+        if (stem_half) {
             // block 1's depthwise is KD (HFMA2 over an fp16 tile): the stem output, read by nothing else, is written as fp16
             whenet::stem_tile_kernel<__half, IN_U8, true><<<dim3(56, nb), 224, 0, c->stream>>>(d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut);
         } else if (c->stem_variant == 0) {
@@ -685,34 +647,6 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                 tiles = 1;
                 did_k1 = true;
               }
-            } else if (c->use_fused && c->k1_variant == 4 && c->k1w[i].valid && b.idx <= c->fused_max_block) {
-                const K1WPlan& pl = c->k1w[i];
-                whenet::fused::K1WParams p = pl.p;
-                const TmapKey key{b.idx, nb, (const void*)cur};
-                auto it = c->tmaps.find(key);
-                if (it == c->tmaps.end()) {
-                    if (c->tmaps.size() > 512) c->tmaps.clear();
-                    CUtensorMap tm;
-                    int rc = make_tmap_act(&tm, cur, nb, b.hin, b.cin, p.IW, p.IH, p.NB, c->precision == WHENET_PRECISION_BF16);
-                    if (rc) return rc;
-                    it = c->tmaps.emplace(key, tm).first;
-                }
-                p.tmA = it->second; p.tmW = c->tmap_w[i];
-                p.shift = w.b_exp_h; p.w_dw16 = w.w_dw16; p.b_dw = w.b_dw_h; p.out = D; p.partial = c->d_partial; p.tflag = c->d_tflag;
-                p.trace = nullptr;
-                if (c->k1w_trace_block == b.idx) {
-                    if (!c->d_trace) CK(cudaMalloc(&c->d_trace, 256 * 16 * sizeof(long long)));
-                    CK(cudaMemsetAsync(c->d_trace, 0, 256 * 16 * sizeof(long long), c->stream));
-                    p.trace = c->d_trace;
-                }
-                snprintf(nm, sizeof nm, "b%02d.k1", b.idx);
-                Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
-                         2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
-                int rc = whenet::fused::launch_k1w<T>(c->stream, p, b.k, b.s, pl.R, pl.NT, pl.smem, nb, c->sm_count);
-                if (rc != 0) return fail(WHENET_ECUDA, "K1W launch failed for block %d (rc=%d)", b.idx, rc);
-                CK(cudaGetLastError());
-                tiles = p.tiles;
-                did_k1 = true;
             } else if (c->use_fused && c->k1[i].valid && b.idx <= c->fused_max_block) {
                 whenet::fused::K1Params p = c->k1[i].p;
                 p.in = cur; p.wt_aug = w.wt_exp_aug; p.w_dw = w.w_dw_h; p.w_dw16 = w.w_dw16; p.b_dw = w.b_dw_h; p.out = D; p.partial = c->d_partial; p.tflag = c->d_tflag;
@@ -1063,8 +997,8 @@ template <> __nv_bfloat16 to16<__nv_bfloat16>(float v) { return __float2bfloat16
 template <> __half to16<__half>(float v) { return __float2half_rn(v); }
 
 constexpr int64_t kPackMagic = 0x57484e3242323030LL;   // "WHN2B200"
-constexpr int64_t kPackVersion = 3;
-constexpr int kPackHeader = 14, kPackPerBlock = 18;
+constexpr int64_t kPackVersion = 4;
+constexpr int kPackHeader = 14, kPackPerBlock = 16;
 
 // Upload a packed weight image (fp32 arena + 16-bit arena + index) and point the context at it.  Shared by
 // whenet_load_weights (which has just built the image from the raw Keras tensors) and whenet_import_packed (which read it
@@ -1104,19 +1038,13 @@ int bind_packed(whenet_ctx* c, const float* arena, size_t n_f32, const uint16_t*
             w.w_exp = A + o[0]; w.b_exp = A + o[1];
             w.wt_exp = base16 ? base16 + o[10] * 2 : nullptr;
             w.wt_exp_aug = base16 ? base16 + o[12] * 2 : nullptr;
-            w.wt_exp_h = base16 ? base16 + o[15] * 2 : nullptr;
-            w.b_exp_h = A + o[16];
-            if (base16 && c->k1w[i].valid) {
-                int rc = make_tmap_w(&c->tmap_w[i], w.wt_exp_h, c->blocks[i].cexp, c->blocks[i].cin, c->k1w[i].p.CC, c->precision == WHENET_PRECISION_BF16);
-                if (rc) return rc;
-            }
         }
         w.w_dw = A + o[2]; w.b_dw = A + o[3];
         w.w_se1t = A + o[4]; w.b_se1 = A + o[5]; w.w_se2 = A + o[6]; w.b_se2 = A + o[7];
         w.w_proj = A + o[8]; w.b_proj = A + o[9];
         w.wt_proj = base16 ? base16 + o[11] * 2 : nullptr;
         w.w_dw_h = A + o[13]; w.b_dw_h = A + o[14];
-        w.w_dw16 = base16 ? base16 + o[17] * 2 : nullptr;
+        w.w_dw16 = base16 ? base16 + o[15] * 2 : nullptr;
     }
     c->layout = L;
     c->weights_loaded = true;
@@ -1231,8 +1159,6 @@ int whenet_create(whenet_ctx** out, int device, int max_batch, int precision) {
     c->blocks = make_blocks();
     c->bw.resize(c->blocks.size());
     c->k1.resize(c->blocks.size());
-    c->k1w.resize(c->blocks.size());
-    c->tmap_w.resize(c->blocks.size());
     if (precision != WHENET_PRECISION_FP32) {
         const BlockCfg& b1 = c->blocks[0];
         c->dw1.valid = !b1.has_expand && whenet::fused::plan_dw_only(b1.hin, b1.cexp, b1.k, b1.s, b1.pad, &c->dw1.p, &c->dw1.smem);
@@ -1248,12 +1174,6 @@ int whenet_create(whenet_ctx** out, int device, int max_batch, int precision) {
                                               &pl.p, &ch, &pl.smem);
             pl.R = ch.r;
             pl.NT = ch.nt;
-            {
-                K1WPlan& pw = c->k1w[i];
-                whenet::fused::K1WChoice wc{};
-                pw.valid = whenet::fused::plan_k1w(b.hin, b.hout, b.cin, b.cexp, b.k, b.s, b.pad, precision == WHENET_PRECISION_BF16, &pw.p, &wc, &pw.smem);
-                pw.R = wc.r; pw.NT = wc.nt;
-            }
         }
     c->use_fused = precision != WHENET_PRECISION_FP32;
     if (const char* e3 = getenv("WHENET_FUSED")) c->use_fused = atoi(e3) && precision != WHENET_PRECISION_FP32;
@@ -1296,7 +1216,7 @@ int whenet_load_weights(whenet_ctx* c, const whenet_tensor* tensors, int n_tenso
                                                   while (arena.size() % 4) arena.push_back(0.f); return off; };
     auto put16 = [&](const std::vector<float>& v) { size_t off = arena16src.size(); arena16src.insert(arena16src.end(), v.begin(), v.end());
                                                     while (arena16src.size() % 8) arena16src.push_back(0.f); return off; };
-    struct Off { size_t w_exp, b_exp, w_dw, b_dw, w_se1t, b_se1, w_se2, b_se2, w_proj, b_proj, t_exp, t_proj, t_aug, w_dw_h, b_dw_h, t_exp_h, b_exp_h, w_dw16; };
+    struct Off { size_t w_exp, b_exp, w_dw, b_dw, w_se1t, b_se1, w_se2, b_se2, w_proj, b_proj, t_exp, t_proj, t_aug, w_dw_h, b_dw_h, w_dw16; };
     std::vector<std::pair<size_t, size_t>> force_f16;     // ranges of the 16-bit arena that are fp16 whatever the storage type
     // values of the augmented expand weights; shift columns are filled after 16-bit rounding of the high part
     std::vector<std::pair<size_t, float>> shift_lo_fix;   // (index in arena16src of the hi column, full-precision shift)
@@ -1356,14 +1276,6 @@ int whenet_load_weights(whenet_ctx* c, const whenet_tensor* tensors, int n_tenso
                 aug[(size_t)n * ka + b.cin] = 0.5f * arena[o.b_exp + n];
             }
             o.t_aug = put16(aug);
-            // K1W: 0.5 * weights [cexp][cin] (exact halving) and 0.5 * shift in fp32
-            {
-                std::vector<float> wh((size_t)b.cexp * b.cin), bh(b.cexp);
-                for (size_t j = 0; j < wh.size(); ++j) wh[j] = 0.5f * arena16src[o.t_exp + j];
-                for (int n = 0; n < b.cexp; ++n) bh[n] = 0.5f * arena[o.b_exp + n];
-                o.t_exp_h = put16(wh);
-                o.b_exp_h = put(bh);
-            }
             for (int n = 0; n < b.cexp; ++n) shift_lo_fix.push_back({o.t_aug + (size_t)n * ka + b.cin, 0.5f * arena[o.b_exp + n]});
         }
         {
@@ -1458,7 +1370,7 @@ int whenet_load_weights(whenet_ctx* c, const whenet_tensor* tensors, int n_tenso
         const Off& o = offs[i];
         const bool e = c->blocks[i].has_expand;
         for (size_t v : {e ? o.w_exp : 0, e ? o.b_exp : 0, o.w_dw, o.b_dw, o.w_se1t, o.b_se1, o.w_se2, o.b_se2, o.w_proj, o.b_proj, e ? o.t_exp : 0, o.t_proj,
-                         e ? o.t_aug : 0, o.w_dw_h, o.b_dw_h, e ? o.t_exp_h : 0, e ? o.b_exp_h : 0, o.w_dw16})
+                         e ? o.t_aug : 0, o.w_dw_h, o.b_dw_h, o.w_dw16})
             layout.push_back((int64_t)v);
     }
     return bind_packed(c, arena.data(), arena.size(), h16.data(), h16.size(), layout);
@@ -1695,15 +1607,6 @@ int whenet_debug_decode(whenet_ctx* c, const float* logits_host, int n, float* a
     return 0;
 }
 
-int whenet_debug_read_trace(whenet_ctx* c, int64_t* out, int n_rows) {
-    if (!c || !out || n_rows < 1 || n_rows > 256) return fail(WHENET_EINVAL, "bad arguments");
-    if (!c->d_trace) return fail(WHENET_ENOTFOUND, "no trace recorded (set option k1w_trace to a block index and run a forward)");
-    CK(cudaSetDevice(c->device));
-    CK(cudaStreamSynchronize(c->stream));
-    CK(cudaMemcpy(out, c->d_trace, (size_t)n_rows * 16 * sizeof(long long), cudaMemcpyDeviceToHost));
-    return 0;
-}
-
 int whenet_debug_raise_timeout(whenet_ctx* c) {
     if (!c) return fail(WHENET_EINVAL, "null context");
     CK(cudaSetDevice(c->device));
@@ -1727,27 +1630,6 @@ int whenet_debug_set_k1_plan(whenet_ctx* c, int block, int th, int tw, int r, in
     pl.R = r;
     pl.NT = nt;
     c->k1[block - 1] = pl;
-    c->cfg_epoch++;
-    free_ws(c);      // the squeeze-partials buffer depends on the tile count
-    return 0;
-}
-
-int whenet_debug_set_k1w_plan(whenet_ctx* c, int block, int th, int tw, int r, int cc, int nb, int n_epi, int nt) {
-    if (!c || block < 2 || block > (int)c->blocks.size()) return fail(WHENET_EINVAL, "bad block index");
-    if (c->precision == WHENET_PRECISION_FP32) return fail(WHENET_EINVAL, "K1W needs a 16-bit storage mode");
-    const BlockCfg& b = c->blocks[block - 1];
-    if (!whenet::fused::k1w_has_instance(b.k, b.s, r, nt)) return fail(WHENET_EINVAL, "no K1W instantiation for k=%d s=%d r=%d nt=%d", b.k, b.s, r, nt);
-    K1WPlan pw;
-    pw.valid = whenet::fused::plan_k1w_candidate(b.hin, b.hout, b.cin, b.cexp, b.k, b.s, b.pad, c->precision == WHENET_PRECISION_BF16, th, tw, r, cc, nb,
-                                                 n_epi, nt, &pw.p, &pw.smem);
-    if (!pw.valid) return fail(WHENET_EINVAL, "K1W plan %dx%d r%d cc%d nb%d epi%d nt%d does not fit block %d", th, tw, r, cc, nb, n_epi, nt, block);
-    pw.R = r; pw.NT = nt;
-    if (c->weights_loaded) {
-        int rc = make_tmap_w(&c->tmap_w[block - 1], c->bw[block - 1].wt_exp_h, b.cexp, b.cin, cc, c->precision == WHENET_PRECISION_BF16);
-        if (rc) return rc;
-    }
-    c->k1w[block - 1] = pw;
-    c->tmaps.clear();
     c->cfg_epoch++;
     free_ws(c);      // the squeeze-partials buffer depends on the tile count
     return 0;
@@ -1795,13 +1677,11 @@ int whenet_set_option(whenet_ctx* c, const char* key, int value) {
     if (!strcmp(key, "se_tail")) { c->se_tail = value; return 0; }
     if (!strcmp(key, "se_scale_out")) { c->se_scale_out = value; return 0; }
     if (!strcmp(key, "k1_split_ctas")) { c->k1_split_ctas = value; return 0; }
-    if (!strcmp(key, "k1w_trace")) { c->k1w_trace_block = value; return 0; }
     if (!strcmp(key, "se_wide")) { c->se_wide = value; return 0; }
     if (!strcmp(key, "host_chunk")) { if (value < 1) return fail(WHENET_EINVAL, "host_chunk must be >= 1"); c->host_chunk = value; return 0; }
     if (!strcmp(key, "graph")) { c->use_graph = value; if (!value) drop_graphs(c); return 0; }
     if (!strcmp(key, "dw_variant")) { c->dw_variant = value; return 0; }
     if (!strcmp(key, "stem_variant")) { c->stem_variant = value; return 0; }
-    if (!strcmp(key, "k1_variant")) { c->k1_variant = value; return 0; }
     if (!strcmp(key, "dw1_fused")) { c->dw1_fused = value; return 0; }
     if (!strcmp(key, "pw_variant")) { c->pw_variant = value; return 0; }
     if (!strcmp(key, "pw_stage_cap")) { c->pw_stage_cap = value; return 0; }
@@ -1816,7 +1696,6 @@ int whenet_set_option(whenet_ctx* c, const char* key, int value) {
     if (!strcmp(key, "head_batch")) { c->head_batch = value; return 0; }
     if (!strcmp(key, "dw1_kd")) { c->dw1_kd = value; return 0; }
     if (!strcmp(key, "pw3")) { c->pw3 = value; return 0; }
-    if (!strcmp(key, "stem_tc")) { c->stem_tc = value; return 0; }
     if (!strcmp(key, "stage_threads")) { c->stage_threads = value < 0 ? 0 : (value > 32 ? 32 : value); return 0; }
     if (!strcmp(key, "chunk")) {
         if (value < 1) return fail(WHENET_EINVAL, "chunk must be >= 1");
@@ -1843,7 +1722,6 @@ void whenet_destroy(whenet_ctx* c) {
     if (c->d_angles) cudaFree(c->d_angles);
     if (c->d_logits) cudaFree(c->d_logits);
     if (c->h_tflag) cudaFreeHost(c->h_tflag);
-    if (c->d_trace) cudaFree(c->d_trace);
     for (int i = 0; i < 2; ++i) {
         if (c->ev_ready[i]) cudaEventDestroy(c->ev_ready[i]);
         if (c->ev_free[i]) cudaEventDestroy(c->ev_free[i]);

@@ -510,11 +510,13 @@ int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n,
         cleanup();
         return fail(WHENET_ECUDA, "out of device memory");
     }
-    cudaMemcpy(dx, hx.data(), nx * 2, cudaMemcpyHostToDevice);
-    if (nu) cudaMemcpy(du, hu.data(), nu * 2, cudaMemcpyHostToDevice);
-    cudaMemcpy(dw, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice);
-    cudaMemcpy(db, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice);
-    if (resid) cudaMemcpy(dr, hr.data(), no * 2, cudaMemcpyHostToDevice);
+    // on the detector's stream: a cudaMemcpy from pageable memory can return before its DMA has landed, and the
+    // non-blocking stream would not wait for it
+    cudaMemcpyAsync(dx, hx.data(), nx * 2, cudaMemcpyHostToDevice, d->stream);
+    if (nu) cudaMemcpyAsync(du, hu.data(), nu * 2, cudaMemcpyHostToDevice, d->stream);
+    cudaMemcpyAsync(dw, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice, d->stream);
+    cudaMemcpyAsync(db, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice, d->stream);
+    if (resid) cudaMemcpyAsync(dr, hr.data(), no * 2, cudaMemcpyHostToDevice, d->stream);
     Y::IgemmParams p{};
     p.in = (const __nv_bfloat16*)dx; p.up = (const __nv_bfloat16*)du; p.wt = (const __nv_bfloat16*)dw; p.bias = (const float*)db;
     p.resid = (const __nv_bfloat16*)dr; p.out = dout;
@@ -543,7 +545,7 @@ int whenet_det_debug_maxpool(whenet_det* d, const float* x, int n, int H, int W,
         cudaFree(dx); cudaFree(dout);
         return fail(WHENET_ECUDA, "out of device memory");
     }
-    int rc = (int)cudaMemcpy(dx, hx.data(), ni * 2, cudaMemcpyHostToDevice);
+    int rc = (int)cudaMemcpyAsync(dx, hx.data(), ni * 2, cudaMemcpyHostToDevice, d->stream);     // ordered before the kernel (see above)
     if (!rc) rc = Y::launch_maxpool(d->stream, (const __nv_bfloat16*)dx, (__nv_bfloat16*)dout, n, H, W, C, stride);
     if (!rc) rc = (int)cudaStreamSynchronize(d->stream);
     if (!rc) rc = to_f32_tap(dout, false, no, out) ? -1 : 0;

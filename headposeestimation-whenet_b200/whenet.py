@@ -106,7 +106,7 @@ class WHENet:
         self.idx_tensor_yaw = np.array([idx for idx in range(120)], dtype=np.float32)
 
     # ------------------------------------------------------------------ plumbing
-    PACKED_FORMAT = "whenet-b200-packed-v2"
+    PACKED_FORMAT = "whenet-b200-packed-v3"
 
     def _load(self, snapshot):
         if snapshot is not None and os.fspath(snapshot).endswith(".safetensors"):
@@ -282,12 +282,6 @@ class WHENet:
         check(self._L.whenet_debug_decode(self._h, _ptr(logits), logits.shape[0], _ptr(out)))
         return out
 
-    def read_trace(self, n_rows: int = 148) -> np.ndarray:
-        """Rows of 16 cycle counters, one per CTA of the K1W launch selected by option ``k1w_trace`` (see kernels_k1w.cuh)."""
-        out = np.zeros((n_rows, 16), np.int64)
-        check(self._L.whenet_debug_read_trace(self._h, _ptr(out), n_rows))
-        return out
-
     def debug_raise_timeout(self):
         """Test hook: a device kernel raises the mbarrier-timeout flag; the next synchronising call must fail."""
         check(self._L.whenet_debug_raise_timeout(self._h))
@@ -295,10 +289,6 @@ class WHENet:
     def set_k1_plan(self, block: int, th: int, tw: int, r: int, cc: int, nt: int = 256, nb: int = 1) -> bool:
         """Tuning hook (see whenet_debug_set_k1_plan); returns False when the plan cannot run."""
         return self._L.whenet_debug_set_k1_plan(self._h, block, th, tw, r, cc, nt, nb) == 0
-
-    def set_k1w_plan(self, block: int, th: int, tw: int, r: int, cc: int, nb: int = 1, n_epi: int = 4, nt: int = 768) -> bool:
-        """Tuning hook for the weight-stationary variant (see whenet_debug_set_k1w_plan); False when the plan cannot run."""
-        return self._L.whenet_debug_set_k1w_plan(self._h, block, th, tw, r, cc, nb, n_epi, nt) == 0
 
     def enable_profile(self, on: bool = True):
         check(self._L.whenet_profile_enable(self._h, int(on)))

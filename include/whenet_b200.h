@@ -169,16 +169,6 @@ int whenet_debug_decode(whenet_ctx* ctx, const float* logits_host, int n, float*
  * the next synchronising call (host-output forward, whenet_synchronize) must return WHENET_ECUDA. */
 int whenet_debug_raise_timeout(whenet_ctx* ctx);
 
-/* Where the warp roles of the K1W kernel waited: set option "k1w_trace" to a block index (2..16), run a forward, then read
- * n_rows x 16 int64 cycle counters (one row per CTA): [0] CTA cycles; producer [1] wait a_empty [3] busy span; MMA [4] wait
- * a_full [5] wait t_empty; epilogue warp 0 [7] wait t_full [8] wait e_empty [9] span; depthwise warp 0 [10] wait e_full
- * [11] group barrier [12] span. */
-int whenet_debug_read_trace(whenet_ctx* ctx, int64_t* out, int n_rows);
-
-/* Same for K1W (option "k1_variant" = 4, every block with an expand conv): output tile, strip length, channels per CTA,
- * crops per item (2 only where one tile is the whole image), epilogue warps (4 or 8), threads per CTA (768). */
-int whenet_debug_set_k1w_plan(whenet_ctx* ctx, int block, int th, int tw, int r, int cc, int nb, int n_epi, int nt);
-
 /* The margin arithmetic of whenet_crop_boxes_u8 alone, on the host (no context, no GPU): m boxes of an H x W frame ->
  * rects_out / valid_out as that call fills them (each may be NULL). */
 int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out);
@@ -199,7 +189,6 @@ int64_t whenet_launch_count(whenet_ctx* ctx);
  *                    fp32 mode: 0 = fp32 FMA kernels (default), 1 = the 1x1 convs on the tensor core through the bf16 hi/lo split
  *                    (three MMAs per product, fp32 accumulation: 6e-4 deg from the float64 oracle on the golden crops)
  *   "fused"          1: K1 (expand + depthwise fused, expanded tensor in shared memory) for blocks 2..fused_max_block
- *   "k1_variant"     1 = K1 (one tile per CTA), 4 = K1W (weight-stationary persistent CTAs, TMA input tiles, warp roles)
  *   "pw_variant"     2 = pw_tc2 (one tile per CTA, cp.async ring), 3 = K2 (persistent, TMA, warp-specialised), 4 = per layer (default):
  *                    K2 for the ungated / small-map convs that have at least 2 x 148 tiles, pw_tc2 otherwise
  *   "kd_from"        bf16: blocks >= this (default 7) run expand GEMM (fp16 E) + KD (depthwise + squeeze over TMA tiles) instead of K1;
@@ -207,10 +196,9 @@ int64_t whenet_launch_count(whenet_ctx* ctx);
  *                    gated project); "kd_expand_k2" 0: that expand GEMM on pw_tc2; "dw1_kd" 0: block 1's depthwise on K1's depthwise
  *                    half over a bf16 stem output (default 1: KD over an fp16 stem output); "pw3" 0: block-1 project on pw_tc2
  *   "se_batch", "head_batch"   batches >= 64: four crops per CTA in the SE gate / in the Dense + decode head (default 1; same bits)
- *   "stem_tc"        bf16, uint8 input: 1 = the stem as an im2col GEMM on the tensor core (default 0: not faster)
  *   "stage_threads"  host threads that stage PAGEABLE inputs of 8 MB and more into the context's pinned buffer (default 8; 0 = plain
  *                    cudaMemcpyAsync from the caller's buffer)
- *   "fused_max_block", "dw1_fused", "k1_split_ctas", "k1w_trace" (block whose K1W launch records its role waits),
+ *   "fused_max_block", "dw1_fused", "k1_split_ctas",
  *   "se_fused", "se_tail" (K1 CTAs that hold whole crops compute the SE gate themselves, default 1), "se_scale_out", "se_wide",
  *   "pw_stage_cap", "pw_smem_kb", "pw_min_ctas" (split N until the grid has this many CTAs),
  *   "dw_variant", "stem_variant", "host_chunk".

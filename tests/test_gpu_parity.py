@@ -269,30 +269,6 @@ def test_pageable_input_staging(sample_crops, jitter_crops):
     m32.close()
 
 
-def test_stem_on_tensor_core_option(oracle32, sample_crops, jitter_crops):
-    """Option stem_tc=1 (bf16, uint8 input): the stem as an im2col GEMM on the tensor core - table lookups build the [hi | lo] bf16
-    operand rows in shared memory, TF-SAME padding by masking the taps of the missing row / column 224.  The stem output must
-    stay within the rounding of its bf16 weights of the oracle and the angles within the bf16 bound."""
-    import whenet_b200
-    crops = np.concatenate([sample_crops, jitter_crops[:3]])
-    m = whenet_b200.WHENet(SNAP, device=0, precision="bf16", max_batch=8)
-    m.set_option("stem_tc", 1)
-    taps = {}
-    ref_ang = np.stack(oracle32.get_angle(crops, taps), axis=1)
-    m.enable_taps(True)
-    got = np.stack(m.get_angle(crops), axis=1)
-    for nm, lim in (("stem", 6e-3), ("dw1", 1e-2), ("block1", 5e-2), ("block16", 5e-2)):
-        r = taps[nm].astype(np.float64).reshape(-1)
-        g = m.tap(nm).astype(np.float64)
-        e = float(np.sqrt(((g - r) ** 2).mean()) / (np.sqrt((r ** 2).mean()) + 1e-30))
-        assert e < lim, (nm, e)
-    assert np.abs(got - ref_ang).max() < 0.8
-    m.enable_taps(False)
-    one = np.stack(m.get_angle(crops[4:5]), axis=1)
-    assert np.array_equal(one[0], got[4])
-    m.close()
-
-
 @pytest.mark.parametrize("prec", ["bf16", "fp16"])
 def test_se_batch_and_k2_routes_bitwise(prec, sample_crops, jitter_crops):
     """Throughput-sized batches switch three kernels: the SE gates come from se_gate_batch_kernel (four crops per CTA share
