@@ -4,6 +4,7 @@
 namespace whenet {
 namespace fused {
 template int launch_dwse<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int);
+template int launch_dwse_x<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int);
 template int launch_dwse_spatial<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int);
 }  // namespace fused
 }  // namespace whenet

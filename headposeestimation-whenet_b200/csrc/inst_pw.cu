@@ -9,7 +9,7 @@ namespace tc {
 #define WHENET_INST_PW(T)                                                                                                    \
     template int launch_pw_tc2<T>(cudaStream_t, const T*, const void*, const float*, const float*, const T*, T*, long long, \
                                   int, int, int, bool, int, int, int, bool);                                                 \
-    template int launch_k2<T>(cudaStream_t, const K2Params&, size_t, bool, bool, bool, int, bool);          \
+    template int launch_k2<T>(cudaStream_t, const K2Params&, size_t, bool, bool, bool, int);                \
     template int launch_pw_tc3<T>(cudaStream_t, const T*, const void*, const float*, const float*, const T*, T*, long long, int, int, int);
 WHENET_INST_PW(__nv_bfloat16)
 WHENET_INST_PW(__half)

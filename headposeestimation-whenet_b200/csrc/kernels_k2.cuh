@@ -52,8 +52,8 @@ struct alignas(64) K2Params {
 constexpr int kK2Threads = 512;
 constexpr int kK2MaxN = 64;       // accumulator registers per MMA thread = n_tile (128 rows x n_tile over one warpgroup)
 
-// OUT_H: fp16 result whatever T is (expand conv feeding KD); NT = p.n_tile (16, 32, 48 or 64): the MMA width
-template <typename T, bool SWISH, bool GATE, bool RESID, bool OUT_H, int NT>
+// NT = p.n_tile (16, 32, 48 or 64): the MMA width
+template <typename T, bool SWISH, bool GATE, bool RESID, int NT>
 __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant__ K2Params p) {
     using namespace whenet::fused;
     extern __shared__ uint8_t smem_raw[];
@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(kK2Threads, 1) k2_kernel(const __grid_constant
                             unpack2<T>(*reinterpret_cast<const uint32_t*>(resid + m * p.N + n), lo, hi);
                             o0 += lo; o1 += hi;
                         }
-                        *reinterpret_cast<uint32_t*>(out + m * p.N + n) = OUT_H ? pack2<__half>(o0, o1) : pack2<T>(o0, o1);
+                        *reinterpret_cast<uint32_t*>(out + m * p.N + n) = pack2<T>(o0, o1);
                     }
                 }
         }
@@ -280,23 +280,21 @@ inline bool plan_k2(long long M, int K, int N, int hw, bool has_gate, bool is_bf
 }
 
 template <typename T>
-int launch_k2(cudaStream_t stream, const K2Params& p, size_t smem, bool swish, bool gate, bool resid, int sm_count, bool out_half = false) {
+int launch_k2(cudaStream_t stream, const K2Params& p, size_t smem, bool swish, bool gate, bool resid, int sm_count) {
     const int ctas = p.tiles < sm_count ? p.tiles : sm_count;
     if (ctas < 1) return 0;
-#define K2_GO(SW, GA, RE, OH)                                                                                                 \
+#define K2_GO(SW, GA, RE)                                                                                                     \
     return with_mma_width<kK2MaxN>(p.n_tile, [&](auto nt) {                                                                 \
-        auto kfn = k2_kernel<T, SW, GA, RE, OH, decltype(nt)::value>;                                                       \
+        auto kfn = k2_kernel<T, SW, GA, RE, decltype(nt)::value>;                                                           \
         if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) != cudaSuccess) return -1;   \
         kfn<<<ctas, kK2Threads, smem, stream>>>(p);                                                                         \
         return 0;                                                                                                           \
     })
-    if (out_half && !(swish && !gate && !resid)) return 1;
-    if (swish && !gate && !resid && out_half) K2_GO(true, false, false, true);
-    if (swish && !gate && !resid) K2_GO(true, false, false, false);
-    if (!swish && !gate && !resid) K2_GO(false, false, false, false);
-    if (!swish && !gate && resid) K2_GO(false, false, true, false);
-    if (!swish && gate && !resid) K2_GO(false, true, false, false);
-    if (!swish && gate && resid) K2_GO(false, true, true, false);
+    if (swish && !gate && !resid) K2_GO(true, false, false);
+    if (!swish && !gate && !resid) K2_GO(false, false, false);
+    if (!swish && !gate && resid) K2_GO(false, false, true);
+    if (!swish && gate && !resid) K2_GO(false, true, false);
+    if (!swish && gate && resid) K2_GO(false, true, true);
 #undef K2_GO
     return 1;
 }

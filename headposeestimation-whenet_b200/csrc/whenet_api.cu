@@ -38,13 +38,14 @@ WHENET_EXTERN_FUSED(__nv_bfloat16)
 WHENET_EXTERN_FUSED(__half)
 #undef WHENET_EXTERN_FUSED
 extern template int launch_dwse<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int);
+extern template int launch_dwse_x<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int);
 extern template int launch_dwse_spatial<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int);
 }  // namespace fused
 namespace tc {
 #define WHENET_EXTERN_PW(T)                                                                                                         \
     extern template int launch_pw_tc2<T>(cudaStream_t, const T*, const void*, const float*, const float*, const T*, T*, long long, \
                                          int, int, int, bool, int, int, int, bool);                                                 \
-    extern template int launch_k2<T>(cudaStream_t, const K2Params&, size_t, bool, bool, bool, int, bool);          \
+    extern template int launch_k2<T>(cudaStream_t, const K2Params&, size_t, bool, bool, bool, int);          \
     extern template int launch_pw_tc3<T>(cudaStream_t, const T*, const void*, const float*, const float*, const T*, T*, long long, int, int, int);
 WHENET_EXTERN_PW(__nv_bfloat16)
 WHENET_EXTERN_PW(__half)
@@ -154,7 +155,6 @@ struct whenet_ctx {
     std::vector<GraphEntry> graphs;
     int use_fused = 0;      // K1: expand + depthwise in one kernel (16-bit storage only; default on for bf16/fp16)
     int fused_max_block = 16;  // blocks 2..fused_max_block use K1
-    int kd_expand_k2 = 1;      // the expand GEMM of the KD route: 1 = persistent K2 kernel, 0 = pw_tc2
     int kd_tail = 0;           // KD computes the SE gate and gates its output itself (1) or leaves both to se_gate + the project conv (0)
     int se_batch = 1;          // batches >= 64: se_gate_batch_kernel (four crops per CTA)
     int pw3 = 1;               // gated projects with H*W >= 784: pw_tc3 (a CTA walks several tiles of one crop) instead of pw_tc2
@@ -408,9 +408,10 @@ int launch_pw(whenet_ctx* c, const char* name, const T* A, const float* W, const
     Scope sc(c, name, bytes, flops);
     if constexpr (sizeof(T) == 2) {
         // pw_variant 4 (default): K2 for the ungated convs (expands, head, projects whose input is already gated) and for the gated
-        // projects of the small maps; pw_tc2 (per-crop gate on W) for the gated projects of blocks 1-6
-        const bool want_k2 = c->pw_variant == 3 || (c->pw_variant == 4 && (gate == nullptr || hw <= 196) && (!out_half || c->kd_expand_k2));
-        if (c->use_tc && Wt16 && want_k2) {
+        // projects of the small maps; pw_tc2 (per-crop gate on W) for the gated projects of blocks 1-6 and for the fp16-output
+        // expands that feed KD at small batches
+        const bool want_k2 = c->pw_variant == 3 || (c->pw_variant == 4 && (gate == nullptr || hw <= 196));
+        if (c->use_tc && Wt16 && want_k2 && !out_half) {
             whenet::tc::K2Params kp{};
             size_t smem = 0;
             // (the persistent kernel needs enough tiles to keep every SM busy for a while; below that pw_tc2's N split wins)
@@ -434,7 +435,7 @@ int launch_pw(whenet_ctx* c, const char* name, const T* A, const float* W, const
                 }
                 kp.tmA = ia->second; kp.tmW = iw->second;
                 kp.bias = bias; kp.gate = gate; kp.resid = resid; kp.out = out; kp.tflag = c->d_tflag;
-                int rc = whenet::tc::launch_k2<T>(c->stream, kp, smem, swish, gate != nullptr, resid != nullptr, c->sm_count, out_half);
+                int rc = whenet::tc::launch_k2<T>(c->stream, kp, smem, swish, gate != nullptr, resid != nullptr, c->sm_count);
                 if (rc == 0) { CK(cudaGetLastError()); return 0; }
                 if (rc < 0) return fail(WHENET_ECUDA, "K2 launch failed for %s (rc=%d)", name, rc);
             }
@@ -598,52 +599,83 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                 did_k1 = true;
             } else if (use_kd) {
               if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-                // late blocks: expand as a plain tensor-core GEMM (fp16 E, L2-resident) + KD (depthwise + SE + gating)
-                snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
-                int rc = launch_pw<T>(c, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, E,
+                // late blocks: KD (depthwise + SE + gating, one CTA per crop).  Small batches spread one crop's channel chunks
+                // over several CTAs (the gate then comes from se_gate_kernel) and read E from an expand GEMM; otherwise each
+                // CTA computes its crop's expand conv on chip and E never leaves the SM.
+                const int cc = whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp);
+                int split = 1;
+                while (split < b.cexp / cc && (long long)nb * split < c->k1_split_ctas) ++split;
+                int rc = 0;
+                if (split > 1) {
+                    snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
+                    rc = launch_pw<T>(c, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, E,
                                       (long long)nb * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, true, true);
-                if (rc) return rc;
+                    if (rc) return rc;
+                }
                 whenet::fused::DwSeParams p{};
                 {
-                    const int cc = whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp), pw = (b.hout - 1) * b.s + b.k;
+                    const int pw = (b.hout - 1) * b.s + b.k;
                     if (c->tmaps.size() > 512) c->tmaps.clear();
-                    const TmapKey ke{100 + b.idx, nb, (const void*)E}, kw{200 + b.idx, 0, (const void*)w.w_dw16};
-                    auto ie = c->tmaps.find(ke);
-                    if (ie == c->tmaps.end()) {
-                        CUtensorMap tm;
-                        if ((rc = make_tmap_kd_e(&tm, E, nb, b.hin, b.cexp, cc, pw))) return rc;
-                        ie = c->tmaps.emplace(ke, tm).first;
-                    }
+                    const TmapKey kw{200 + b.idx, 0, (const void*)w.w_dw16};
                     auto iw = c->tmaps.find(kw);
                     if (iw == c->tmaps.end()) {
                         CUtensorMap tm;
                         if ((rc = make_tmap_kd_w(&tm, w.w_dw16, b.k * b.k, b.cexp, cc))) return rc;
                         iw = c->tmaps.emplace(kw, tm).first;
                     }
-                    p.tmE = ie->second; p.tmW = iw->second;
+                    p.tmW = iw->second;
+                    if (split > 1) {
+                        const TmapKey ke{100 + b.idx, nb, (const void*)E};
+                        auto ie = c->tmaps.find(ke);
+                        if (ie == c->tmaps.end()) {
+                            CUtensorMap tm;
+                            if ((rc = make_tmap_kd_e(&tm, E, nb, b.hin, b.cexp, cc, pw))) return rc;
+                            ie = c->tmaps.emplace(ke, tm).first;
+                        }
+                        p.tmE = ie->second;
+                    } else {
+                        // block input [nb*H*W][Cin]: box rows = one crop's pixels rounded up to a swizzle atom; expand weights [Cexp][Cin]
+                        const TmapKey kx{300 + b.idx, nb, (const void*)cur}, kwx{400 + b.idx, 0, (const void*)w.wt_exp};
+                        auto ix = c->tmaps.find(kx);
+                        if (ix == c->tmaps.end()) {
+                            CUtensorMap tm;
+                            if ((rc = make_tmap_w(&tm, cur, nb * b.hin * b.hin, b.cin, (b.hin * b.hin + 7) / 8 * 8, true))) return rc;
+                            ix = c->tmaps.emplace(kx, tm).first;
+                        }
+                        auto iwx = c->tmaps.find(kwx);
+                        if (iwx == c->tmaps.end()) {
+                            CUtensorMap tm;
+                            if ((rc = make_tmap_w(&tm, w.wt_exp, b.cexp, b.cin, cc, true))) return rc;
+                            iwx = c->tmaps.emplace(kwx, tm).first;
+                        }
+                        p.tmX = ix->second; p.tmWx = iwx->second;
+                        p.b_exp = w.b_exp;
+                    }
                 }
                 p.b_dw = w.b_dw_h; p.tflag = c->d_tflag;
                 p.out = D; p.partial = c->d_partial;
                 p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = c->d_gate; p.Cse = b.cse;
                 p.inv_hw = 1.0f / (float)(b.hout * b.hout);
                 p.C = b.cexp; p.pad = b.pad;
-                // small batches: spread one crop's channel chunks over several CTAs (the gate then comes from se_gate_kernel)
-                int split = 1;
-                {
-                    const int n_chunks = b.cexp / whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp);
-                    while (split < n_chunks && (long long)nb * split < c->k1_split_ctas) ++split;
-                }
                 if (split == 1 && c->se_tail && c->kd_tail) {
                     p.se_tail = 1;
                     se_in_k1 = true;
                     if (c->se_scale_out && !taps) { p.scale_out = 1; d_gated = true; }
                 }
                 snprintf(nm, sizeof nm, "b%02d.kd", b.idx);
-                Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin + (double)b.hout * b.hout) * b.cexp * sizeof(T),
-                         2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
-                rc = whenet::fused::launch_dwse<T>(c->stream, p, b.k, b.s, b.hin, nb, split);
-                if (rc != 0) return fail(WHENET_ECUDA, "KD launch failed for block %d (rc=%d)", b.idx, rc);
-                CK(cudaGetLastError());
+                if (split == 1) {
+                    Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
+                             2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
+                    rc = whenet::fused::launch_dwse_x<T>(c->stream, p, b.k, b.s, b.hin, b.cin, nb);
+                    if (rc != 0) return fail(WHENET_ECUDA, "KD (on-chip expand) launch failed for block %d (rc=%d)", b.idx, rc);
+                    CK(cudaGetLastError());
+                } else {
+                    Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin + (double)b.hout * b.hout) * b.cexp * sizeof(T),
+                             2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
+                    rc = whenet::fused::launch_dwse<T>(c->stream, p, b.k, b.s, b.hin, nb, split);
+                    if (rc != 0) return fail(WHENET_ECUDA, "KD launch failed for block %d (rc=%d)", b.idx, rc);
+                    CK(cudaGetLastError());
+                }
                 tiles = 1;
                 did_k1 = true;
               }
@@ -1690,7 +1722,6 @@ int whenet_set_option(whenet_ctx* c, const char* key, int value) {
     if (!strcmp(key, "fused")) { c->use_fused = value && c->precision != WHENET_PRECISION_FP32; return 0; }
     if (!strcmp(key, "fused_max_block")) { c->fused_max_block = value; return 0; }
     if (!strcmp(key, "kd_from")) { c->kd_from = value; return 0; }
-    if (!strcmp(key, "kd_expand_k2")) { c->kd_expand_k2 = value; return 0; }
     if (!strcmp(key, "kd_tail")) { c->kd_tail = value; return 0; }
     if (!strcmp(key, "se_batch")) { c->se_batch = value; return 0; }
     if (!strcmp(key, "head_batch")) { c->head_batch = value; return 0; }

@@ -191,9 +191,9 @@ int64_t whenet_launch_count(whenet_ctx* ctx);
  *   "fused"          1: K1 (expand + depthwise fused, expanded tensor in shared memory) for blocks 2..fused_max_block
  *   "pw_variant"     2 = pw_tc2 (one tile per CTA, cp.async ring), 3 = K2 (persistent, TMA, warp-specialised), 4 = per layer (default):
  *                    K2 for the ungated / small-map convs that have at least 2 x 148 tiles, pw_tc2 otherwise
- *   "kd_from"        bf16: blocks >= this (default 7) run expand GEMM (fp16 E) + KD (depthwise + squeeze over TMA tiles) instead of K1;
- *                    0 = K1 on every block.  "kd_tail" 1: KD computes the SE gate and gates its output itself (default 0: se_gate +
- *                    gated project); "kd_expand_k2" 0: that expand GEMM on pw_tc2; "dw1_kd" 0: block 1's depthwise on K1's depthwise
+ *   "kd_from"        bf16: blocks >= this (default 7) run KD (expand conv on chip + depthwise + squeeze; at small batches expand
+ *                    GEMM (fp16 E) + KD over TMA tiles) instead of K1; 0 = K1 on every block.  "kd_tail" 1: KD computes the SE gate
+ *                    and gates its output itself (default 0: se_gate + gated project); "dw1_kd" 0: block 1's depthwise on K1's depthwise
  *                    half over a bf16 stem output (default 1: KD over an fp16 stem output); "pw3" 0: block-1 project on pw_tc2
  *   "se_batch", "head_batch"   batches >= 64: four crops per CTA in the SE gate / in the Dense + decode head (default 1; same bits)
  *   "stage_threads"  host threads that stage PAGEABLE inputs of 8 MB and more into the context's pinned buffer (default 8; 0 = plain

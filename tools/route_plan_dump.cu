@@ -1,5 +1,5 @@
 // Host-only dump of the round-2 route planners (no GPU): K2 (persistent 1x1 conv) plans of the late expands / projects / head conv,
-// KD chunk widths, thread counts and shared memory, pw_tc3's tile walk of the early gated projects.
+// KD chunk widths, thread counts and shared memory (both KD kernels), pw_tc3's tile walk of the early gated projects.
 //   nvcc -std=c++17 -arch=sm_90a -o build_tmp/route_plan_dump tools/route_plan_dump.cu && build_tmp/route_plan_dump [crops]
 #include <cstdio>
 #include <cstdlib>
@@ -16,6 +16,12 @@ static const Blk blocks[] = {
 template <int KS, int S, int HIN, int CC> static void kd_line(const Blk& b) {
     printf("  kd b%02d cc %d threads %d strips %d pw %d smem %zu chunks %d\n", b.idx, CC, fused::DwSeThreads<KS, S, HIN, CC>::value,
            fused::DwSeGeom<KS, S, HIN>::NSTRIPS, fused::DwSeGeom<KS, S, HIN>::PW, fused::dwse_smem<KS, S, HIN, CC>(b.cexp, b.cse), b.cexp / CC);
+}
+// KD with the on-chip expand (one CTA per crop): CIN input channels
+template <int KS, int S, int HIN, int CC, int CIN> static void kdx_line(const Blk& b) {
+    using X = fused::DwSeX<KS, S, HIN, CC, CIN>;
+    printf("  kdx b%02d cc %d cin %d threads %d halves %d nwg %d smem %zu chunks %d ctas_per_sm %d\n", b.idx, CC, CIN, X::NT, X::HALVES,
+           X::NWG, X::smem(b.cexp, b.cse), b.cexp / CC, X::CTAS_PER_SM);
 }
 static void k2_line(const char* what, int idx, long long M, int K, int N, int hw, bool gate) {
     tc::K2Params p{};
@@ -35,6 +41,12 @@ int main(int argc, char** argv) {
             if (b.hin == 14 && b.s == 2 && b.k == 5) kd_line<5, 2, 14, 96>(b);
             if (b.hin == 7 && b.k == 5) kd_line<5, 1, 7, 128>(b);
             if (b.hin == 7 && b.k == 3) kd_line<3, 1, 7, 128>(b);
+            if (b.hin == 14 && b.s == 1 && b.k == 3) kdx_line<3, 1, 14, 32, 80>(b);
+            if (b.hin == 14 && b.s == 1 && b.k == 5 && b.cin == 80) kdx_line<5, 1, 14, 32, 80>(b);
+            if (b.hin == 14 && b.s == 1 && b.k == 5 && b.cin == 112) kdx_line<5, 1, 14, 32, 112>(b);
+            if (b.hin == 14 && b.s == 2 && b.k == 5) kdx_line<5, 2, 14, 96, 112>(b);
+            if (b.hin == 7 && b.k == 5) kdx_line<5, 1, 7, 128, 192>(b);
+            if (b.hin == 7 && b.k == 3) kdx_line<3, 1, 7, 128, 192>(b);
             k2_line("expand ", b.idx, (long long)crops * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, false);
             k2_line("project", b.idx, (long long)crops * b.ho * b.ho, b.cexp, b.cout, b.ho * b.ho, true);
         } else {
