@@ -131,6 +131,93 @@ __device__ __forceinline__ uint32_t sw128(int r, int c) {
 // (x + 0.5) / d is at least 0.5 / d away from every integer, far more than the float rounding error
 __device__ __forceinline__ int div_small(int x, float inv) { return __float2int_rz(((float)x + 0.5f) * inv); }
 
+// The arithmetic of one 16-bit-storage K1 tile that k1x_kernel (kernels_k1x.cuh) shares, so that the two kernels cannot drift
+// apart by a bit.
+//
+// Expand epilogue of one fragment row: the NP 16-column pieces of accumulator row `hr` (0: row lane/4, 1: that + 8) of a
+// m64nN fragment -> swish -> fp16 -> E row at `er` (cq = 2 (lane % 4)).  The BN shift is already in the accumulator.
+// E is fp16 whatever the storage type: 3 more mantissa bits than bf16 and HFMA2-ready.
+template <int NP>
+__device__ __forceinline__ void expand_row_to_e(const float (&d)[8 * NP], int nch16, int hr, uint32_t er, int cq) {
+#pragma unroll
+    for (int jj = 0; jj < NP; ++jj) {
+        if (jj < nch16) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const uint32_t v = pack2<__half>(swish_from_half(d[8 * jj + 4 * i + 2 * hr]), swish_from_half(d[8 * jj + 4 * i + 2 * hr + 1]));
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(er + (uint32_t)(16 * jj + 8 * i + cq) * 2u), "r"(v) : "memory");
+            }
+        }
+    }
+}
+
+// HFMA2 depthwise of one strip (R outputs of one row, 4 channels): fp16 E, fp16 weights, fp16 running sums - the loaded
+// words ARE the operands (no unpack instructions), one HFMA2 per channel pair and tap - then sum * kDwScale + shift in fp32.
+// Measured against the float64 oracle this is MORE accurate than the bf16-E / fp32-FMA form it replaced (0.12 vs 0.19 deg
+// on the golden crops): E keeps 11 mantissa bits.  `erow` = top-left of the strip's input window (rows e_rowstride, pixels
+// pitchE bytes apart), `wts` = this thread's 4 channels of tap 0 (taps w_pitch bytes apart), bq = their BN shifts.
+template <int KS, int S, int R>
+__device__ __forceinline__ void dw_strip_hfma2(uint32_t erow, uint32_t e_rowstride, uint32_t pitchE, uint32_t wts, uint32_t w_pitch,
+                                               const float4& bq, float2 (&acc)[R][2]) {
+    constexpr int NCOL = (R - 1) * S + KS;
+    __half2 hacc[R][2];
+#pragma unroll
+    for (int r = 0; r < R; ++r) { hacc[r][0] = __float2half2_rn(0.f); hacc[r][1] = __float2half2_rn(0.f); }
+#pragma unroll
+    for (int ky = 0; ky < KS; ++ky) {
+        __half2 wr[KS][2];
+#pragma unroll
+        for (int kx = 0; kx < KS; ++kx) {
+            uint32_t w0, w1;
+            lds64(wts + (uint32_t)(ky * KS + kx) * w_pitch, w0, w1);
+            wr[kx][0] = *reinterpret_cast<__half2*>(&w0); wr[kx][1] = *reinterpret_cast<__half2*>(&w1);
+        }
+        uint32_t ea = erow;
+#pragma unroll
+        for (int col = 0; col < NCOL; ++col) {
+            uint32_t a, b;
+            lds64(ea, a, b);
+            ea += pitchE;
+            const __half2 x01 = *reinterpret_cast<__half2*>(&a), x23 = *reinterpret_cast<__half2*>(&b);
+#pragma unroll
+            for (int r = 0; r < R; ++r) {
+                const int kx = col - r * S;          // compile-time after unrolling
+                if (kx >= 0 && kx < KS) {
+                    hacc[r][0] = __hfma2(x01, wr[kx][0], hacc[r][0]);
+                    hacc[r][1] = __hfma2(x23, wr[kx][1], hacc[r][1]);
+                }
+            }
+        }
+        erow += e_rowstride;
+    }
+    const float2 sc = make_float2(kDwScale, kDwScale);
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        acc[r][0] = make_float2(bq.x, bq.y); acc[r][1] = make_float2(bq.z, bq.w);
+        ffma2(acc[r][0], __half22float2(hacc[r][0]), sc);          // sum * kDwScale + shift, in fp32
+        ffma2(acc[r][1], __half22float2(hacc[r][1]), sc);
+    }
+}
+
+// The strip's first `nvalid` outputs: swish, squeeze sums (in strip order), 16-bit store to dst (pixels Cexp apart).
+template <typename T, int R>
+__device__ __forceinline__ void dw_strip_finish(float2 (&acc)[R][2], int nvalid, T* dst, int Cexp, float (&sum)[4]) {
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        if (r < nvalid) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                acc[r][i].x = swish_from_half(acc[r][i].x); acc[r][i].y = swish_from_half(acc[r][i].y);
+                sum[2 * i] += acc[r][i].x; sum[2 * i + 1] += acc[r][i].y;
+            }
+            uint2 o;
+            o.x = pack2<T>(acc[r][0].x, acc[r][0].y);
+            o.y = pack2<T>(acc[r][1].x, acc[r][1].y);
+            *reinterpret_cast<uint2*>(dst + (long long)r * Cexp) = o;
+        }
+    }
+}
+
 // NOEXP: the block has no expand conv (block 1): the halo tile of the block INPUT is copied straight into E and only the
 // depthwise half of the kernel runs (single chunk, no tensor-core work).
 // CCT != 0 bakes the chunk width (and with it the E row pitch and every constant-table offset) into the code: the
@@ -313,18 +400,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
                 for (int hr = 0; hr < 2; ++hr) {
                     const int r = r_lo + 8 * hr;
                     if (r < rows_gemm) {
-                        const uint32_t er = e_row_of(r);
-#pragma unroll
-                        for (int jj = 0; jj < kMaxPieces; ++jj) {
-                            if (jj < nch16) {
-#pragma unroll
-                                for (int i = 0; i < 2; ++i) {
-                                    // E is fp16 whatever the storage type: 3 more mantissa bits than bf16 and HFMA2-ready
-                                    const uint32_t v = pack2<__half>(swish_from_half(d[8 * jj + 4 * i + 2 * hr]), swish_from_half(d[8 * jj + 4 * i + 2 * hr + 1]));
-                                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(er + (uint32_t)(16 * jj + 8 * i + cq) * 2u), "r"(v) : "memory");
-                                }
-                            }
-                        }
+                        expand_row_to_e<kMaxPieces>(d, nch16, hr, e_row_of(r), cq);
                     }
                 }
             }
@@ -385,64 +461,12 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k1_expand_dw_kernel(con
                         erow += e_rowstride;
                     }
                 } else {
-                    // fp16 E, fp16 weights, HFMA2 running sums: the loaded words ARE the operands (no unpack instructions),
-                    // one HFMA2 per channel pair and tap.  Measured against the float64 oracle this is MORE accurate than the
-                    // bf16-E / fp32-FMA form it replaces (0.12 vs 0.19 deg on the golden crops): E keeps 11 mantissa bits.
-                    __half2 hacc[R][2];
-#pragma unroll
-                    for (int r = 0; r < R; ++r) { hacc[r][0] = __float2half2_rn(0.f); hacc[r][1] = __float2half2_rn(0.f); }
-                    const uint32_t cst_h = cst - (uint32_t)cv * 16 + (uint32_t)CC * 4 + (uint32_t)cv * 8;
-#pragma unroll
-                    for (int ky = 0; ky < KS; ++ky) {
-                        __half2 wr[KS][2];
-#pragma unroll
-                        for (int kx = 0; kx < KS; ++kx) {
-                            uint32_t w0, w1;
-                            lds64(cst_h + (uint32_t)((ky * KS + kx) * CC) * 2, w0, w1);
-                            wr[kx][0] = *reinterpret_cast<__half2*>(&w0); wr[kx][1] = *reinterpret_cast<__half2*>(&w1);
-                        }
-                        uint32_t ea = erow;
-#pragma unroll
-                        for (int col = 0; col < NCOL; ++col) {
-                            uint32_t a, b;
-                            lds64(ea, a, b);
-                            ea += pitchE;
-                            const __half2 x01 = *reinterpret_cast<__half2*>(&a), x23 = *reinterpret_cast<__half2*>(&b);
-#pragma unroll
-                            for (int r = 0; r < R; ++r) {
-                                const int kx = col - r * S;          // compile-time after unrolling
-                                if (kx >= 0 && kx < KS) {
-                                    hacc[r][0] = __hfma2(x01, wr[kx][0], hacc[r][0]);
-                                    hacc[r][1] = __hfma2(x23, wr[kx][1], hacc[r][1]);
-                                }
-                            }
-                        }
-                        erow += e_rowstride;
-                    }
-                    const float2 sc = make_float2(kDwScale, kDwScale);
-#pragma unroll
-                    for (int r = 0; r < R; ++r) {
-                        acc[r][0] = make_float2(bq.x, bq.y); acc[r][1] = make_float2(bq.z, bq.w);
-                        ffma2(acc[r][0], __half22float2(hacc[r][0]), sc);          // sum * kDwScale + shift, in fp32
-                        ffma2(acc[r][1], __half22float2(hacc[r][1]), sc);
-                    }
+                    dw_strip_hfma2<KS, S, R>(erow, e_rowstride, (uint32_t)pitchE, cst - (uint32_t)cv * 16 + (uint32_t)CC * 4 + (uint32_t)cv * 8,
+                                             (uint32_t)CC * 2, bq, acc);
                 }
                 const int oy = ty0 + oyl;
                 T* dst = out_n + ((long long)oy * p.Ho + tx0 + oxl0) * p.Cexp + c0;
-#pragma unroll
-                for (int r = 0; r < R; ++r) {
-                    if (oxl0 + r < p.TW && oy < p.Ho && tx0 + oxl0 + r < p.Ho) {
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            acc[r][i].x = swish_from_half(acc[r][i].x); acc[r][i].y = swish_from_half(acc[r][i].y);
-                            sum[2 * i] += acc[r][i].x; sum[2 * i + 1] += acc[r][i].y;
-                        }
-                        uint2 o;
-                        o.x = pack2<T>(acc[r][0].x, acc[r][0].y);
-                        o.y = pack2<T>(acc[r][1].x, acc[r][1].y);
-                        *reinterpret_cast<uint2*>(dst + (long long)r * p.Cexp) = o;
-                    }
-                }
+                dw_strip_finish<T, R>(acc, oy < p.Ho ? min(p.TW - oxl0, p.Ho - tx0 - oxl0) : 0, dst, p.Cexp, sum);
             }
             asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(sR + (uint32_t)(py * CC + cv * 4) * 4),
                          "f"(sum[0]), "f"(sum[1]), "f"(sum[2]), "f"(sum[3]) : "memory");

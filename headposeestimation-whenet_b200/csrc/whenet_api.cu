@@ -26,9 +26,10 @@
 #include "kernels_k2.cuh"
 #include "kernels_tc32.cuh"
 #include "kernels_dwse.cuh"
+#include "kernels_k1x.cuh"
 #include <cudaTypedefs.h>
 
-// The fused-kernel launchers are instantiated in their own translation units (inst_k1_bf16.cu, inst_k1_f16.cu, inst_k1x.cu)
+// The fused-kernel launchers are instantiated in their own translation units (inst_k1_bf16.cu, inst_k1_f16.cu, inst_dwse.cu)
 namespace whenet {
 namespace fused {
 #define WHENET_EXTERN_FUSED(T)                                                                            \
@@ -40,6 +41,7 @@ WHENET_EXTERN_FUSED(__half)
 extern template int launch_dwse<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int);
 extern template int launch_dwse_x<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int);
 extern template int launch_dwse_spatial<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int);
+extern template int launch_k1x<__nv_bfloat16>(cudaStream_t, DwSeParams, int, int, int, int, int, int, int, int);
 }  // namespace fused
 namespace tc {
 #define WHENET_EXTERN_PW(T)                                                                                                         \
@@ -160,6 +162,7 @@ struct whenet_ctx {
     int pw3 = 1;               // gated projects with H*W >= 784: pw_tc3 (a CTA walks several tiles of one crop) instead of pw_tc2
     int dw1_kd = 1;            // bf16: the stem writes fp16 and block 1's depthwise runs on KD (spatial tiles, TMA, HFMA2) instead of K1's depthwise half
     int head_batch = 1;        // batches >= 64: GAP kernel + Dense/decode for four crops per CTA
+    int k1x = 0;               // bf16: the blocks with a K1X instance (K1 fed by TMA, same bits) run it where a CTA holds all chunks of its tile; 0 = K1
     int kd_from = 7;           // bf16: blocks >= kd_from whose map fits one CTA run expand GEMM (fp16 E through L2) + KD; 0 = off
     std::vector<K1Plan> k1;
     std::map<TmapKey, CUtensorMap> tmaps;   // KD tensor maps: E tiles by (100 + block, crops, buffer), depthwise weights by (200 + block, 0, pointer)
@@ -384,6 +387,20 @@ int make_tmap_kd_e(CUtensorMap* tm, const void* base, int n, int H, int C, int c
     const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(KD tile %dx%dx%dx%d, box %dx%dx%d) failed: %d", n, H, H, C, pw, pw, cc, (int)r);
+    return 0;
+}
+// K1X's block input (bf16) [n][H][H][C]: box {64, iw, iw, 1}, SWIZZLE_128B - a halo tile lands as the K-major A operand, one
+// 128-byte row per pixel; channels >= C and pixels outside the image are zero-filled
+int make_tmap_k1x_in(CUtensorMap* tm, const void* base, int n, int H, int C, int iw) {
+    auto fn = tmap_encode_fn();
+    if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)H, (cuuint64_t)H, (cuuint64_t)n};
+    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * C * 2, (cuuint64_t)H * H * C * 2};
+    const cuuint32_t box[4] = {64, (cuuint32_t)iw, (cuuint32_t)iw, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(K1X input %dx%dx%dx%d, box %dx%d) failed: %d", n, H, H, C, iw, iw, (int)r);
     return 0;
 }
 int make_tmap_kd_w(CUtensorMap* tm, const void* base, int kk, int C, int cc) {
@@ -704,9 +721,46 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                 snprintf(nm, sizeof nm, "b%02d.k1", b.idx);
                 Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
                          2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
-                int rc = whenet::fused::launch_k1<T>(c->stream, p, b.k, b.s, c->k1[i].R, c->k1[i].NT, c->k1[i].smem, nb);
-                if (rc != 0) return fail(WHENET_ECUDA, "K1 launch failed for block %d (rc=%d)", b.idx, rc);
-                CK(cudaGetLastError());
+                bool did_k1x = false;
+                if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+                    // throughput batches (a CTA holds every chunk of its tile): K1X, the same tiles and bits fed by TMA
+                    if (c->k1x && c->use_tc && p.chunks_per_cta == p.n_chunks && !se_in_k1 &&
+                        whenet::fused::k1x_has_instance(b.k, b.s, b.hin, b.cin, b.pad, p, c->k1[i].R)) {
+                        whenet::fused::DwSeParams q{};
+                        int rc = 0;
+                        if (c->tmaps.size() > 512) c->tmaps.clear();
+                        const TmapKey kx{600 + b.idx, nb, (const void*)cur}, kwx{700 + b.idx, 0, (const void*)w.wt_exp_aug}, kw{500 + b.idx, 0, (const void*)w.w_dw16};
+                        auto ix = c->tmaps.find(kx);
+                        if (ix == c->tmaps.end()) {
+                            CUtensorMap tm;
+                            if ((rc = make_tmap_k1x_in(&tm, cur, nb, b.hin, b.cin, p.IW))) return rc;
+                            ix = c->tmaps.emplace(kx, tm).first;
+                        }
+                        auto iwx = c->tmaps.find(kwx);
+                        if (iwx == c->tmaps.end()) {
+                            CUtensorMap tm;
+                            if ((rc = make_tmap_w(&tm, w.wt_exp_aug, b.cexp, b.cin + 8, p.CC, true))) return rc;
+                            iwx = c->tmaps.emplace(kwx, tm).first;
+                        }
+                        auto iw = c->tmaps.find(kw);
+                        if (iw == c->tmaps.end()) {
+                            CUtensorMap tm;
+                            if ((rc = make_tmap_kd_w(&tm, w.w_dw16, b.k * b.k, b.cexp, p.CC))) return rc;
+                            iw = c->tmaps.emplace(kw, tm).first;
+                        }
+                        q.tmX = ix->second; q.tmWx = iwx->second; q.tmW = iw->second;
+                        q.b_dw = w.b_dw_h; q.tflag = c->d_tflag; q.out = D; q.partial = c->d_partial; q.C = b.cexp; q.pad = b.pad;
+                        rc = whenet::fused::launch_k1x<T>(c->stream, q, b.k, b.s, b.hin, b.cin, p.TH, c->k1[i].R, p.CC, nb);
+                        if (rc != 0) return fail(WHENET_ECUDA, "K1X launch failed for block %d (rc=%d)", b.idx, rc);
+                        CK(cudaGetLastError());
+                        did_k1x = true;
+                    }
+                }
+                if (!did_k1x) {
+                    int rc = whenet::fused::launch_k1<T>(c->stream, p, b.k, b.s, c->k1[i].R, c->k1[i].NT, c->k1[i].smem, nb);
+                    if (rc != 0) return fail(WHENET_ECUDA, "K1 launch failed for block %d (rc=%d)", b.idx, rc);
+                    CK(cudaGetLastError());
+                }
                 tiles = p.tiles_x * p.tiles_y;
                 did_k1 = true;
             }
@@ -1208,6 +1262,7 @@ int whenet_create(whenet_ctx** out, int device, int max_batch, int precision) {
             pl.NT = ch.nt;
         }
     c->use_fused = precision != WHENET_PRECISION_FP32;
+    c->k1x = precision == WHENET_PRECISION_BF16;
     if (const char* e3 = getenv("WHENET_FUSED")) c->use_fused = atoi(e3) && precision != WHENET_PRECISION_FP32;
     CK(cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
@@ -1722,6 +1777,7 @@ int whenet_set_option(whenet_ctx* c, const char* key, int value) {
     if (!strcmp(key, "fused")) { c->use_fused = value && c->precision != WHENET_PRECISION_FP32; return 0; }
     if (!strcmp(key, "fused_max_block")) { c->fused_max_block = value; return 0; }
     if (!strcmp(key, "kd_from")) { c->kd_from = value; return 0; }
+    if (!strcmp(key, "k1x")) { c->k1x = value && c->precision == WHENET_PRECISION_BF16; return 0; }
     if (!strcmp(key, "kd_tail")) { c->kd_tail = value; return 0; }
     if (!strcmp(key, "se_batch")) { c->se_batch = value; return 0; }
     if (!strcmp(key, "head_batch")) { c->head_batch = value; return 0; }

@@ -1,5 +1,6 @@
 // Host-only dump of the round-2 route planners (no GPU): K2 (persistent 1x1 conv) plans of the late expands / projects / head conv,
-// KD chunk widths, thread counts and shared memory (both KD kernels), pw_tc3's tile walk of the early gated projects.
+// KD chunk widths, thread counts and shared memory (both KD kernels), the K1X instances, pw_tc3's tile walk of the
+// early gated projects.
 //   nvcc -std=c++17 -arch=sm_90a -o build_tmp/route_plan_dump tools/route_plan_dump.cu && build_tmp/route_plan_dump [crops]
 #include <cstdio>
 #include <cstdlib>
@@ -7,6 +8,7 @@
 #include "../headposeestimation-whenet_b200/csrc/kernels_tc.cuh"
 #include "../headposeestimation-whenet_b200/csrc/kernels_k2.cuh"
 #include "../headposeestimation-whenet_b200/csrc/kernels_dwse.cuh"
+#include "../headposeestimation-whenet_b200/csrc/kernels_k1x.cuh"
 using namespace whenet;
 struct Blk { int idx, hin, ho, cin, cexp, cout, k, s, cse; };
 static const Blk blocks[] = {
@@ -22,6 +24,13 @@ template <int KS, int S, int HIN, int CC, int CIN> static void kdx_line(const Bl
     using X = fused::DwSeX<KS, S, HIN, CC, CIN>;
     printf("  kdx b%02d cc %d cin %d threads %d halves %d nwg %d smem %zu chunks %d ctas_per_sm %d\n", b.idx, CC, CIN, X::NT, X::HALVES,
            X::NWG, X::smem(b.cexp, b.cse), b.cexp / CC, X::CTAS_PER_SM);
+}
+// K1X (K1 fed by TMA): geometry and shared memory of the instance
+template <int KS, int S, int HIN, int TH, int R, int CC, int CIN> static void k1x_line(const Blk& b) {
+    using X = fused::K1X<KS, S, HIN, TH, R, CC, CIN>;
+    if (b.k == KS && b.s == S && b.hin == HIN && b.cin == CIN)
+        printf("  k1x b%02d th %d r %d cc %d cin %d tiles %d pix %d halves %d ksteps %d lanes %d smem %zu chunks %d\n", b.idx, TH, R, CC, CIN, X::TILES,
+               X::NPIX, X::HALVES, X::KSTEPS, X::PY, X::SMEM, b.cexp / CC);
 }
 static void k2_line(const char* what, int idx, long long M, int K, int N, int hw, bool gate) {
     tc::K2Params p{};
@@ -51,6 +60,9 @@ int main(int argc, char** argv) {
             k2_line("project", b.idx, (long long)crops * b.ho * b.ho, b.cexp, b.cout, b.ho * b.ho, true);
         } else {
             if (b.idx == 1) kd_line<3, 1, 14, 32>(b);
+#define K1X_LINE(KS, S, HIN, TH, R, CC, CIN) k1x_line<KS, S, HIN, TH, R, CC, CIN>(b);
+            WHENET_K1X_INSTANCES(K1X_LINE)
+#undef K1X_LINE
             tc::Pw3Plan pl{};
             const bool ok = tc::plan_pw_tc3((long long)crops * b.ho * b.ho, b.cexp, b.cout, b.ho * b.ho, true, &pl);
             if (ok) printf("  pw3 b%02d tiles_per_crop %d tpc %d groups %d umma_n %d smem %zu\n", b.idx, pl.tiles_per_crop, pl.tpc, pl.groups, pl.umma_n, pl.smem);
