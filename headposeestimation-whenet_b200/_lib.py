@@ -16,7 +16,7 @@ EXPORTS = [
     "whenet_last_error", "whenet_version", "whenet_destroy",
     "whenet_det_create", "whenet_det_load_weights", "whenet_det_num_classes", "whenet_det_set_stream", "whenet_det_detect_u8",
     "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_maxpool",
-    "whenet_det_debug_decode",
+    "whenet_det_debug_decode", "whenet_det_create_ex", "whenet_det_precision",
 ]
 
 
@@ -94,6 +94,8 @@ def load():
     L.whenet_destroy.restype = None
     I = C.c_int
     L.whenet_det_create.argtypes = [C.POINTER(P), I, I, I, I]
+    L.whenet_det_create_ex.argtypes = [C.POINTER(P), I, I, I, I, I]
+    L.whenet_det_precision.argtypes = [P]
     L.whenet_det_load_weights.argtypes = [P, C.POINTER(Tensor), I, P, I]
     L.whenet_det_num_classes.argtypes = [P]
     L.whenet_det_set_stream.argtypes = [P, P]

@@ -19,7 +19,8 @@ UNITS = {
     "inst_dwse.cu": _SIMT_TC + ["kernels_fused.cuh", "kernels_dwse.cuh"],
     "inst_pw.cu": _SIMT_TC + ["kernels_fused.cuh", "kernels_k2.cuh"],
     "inst_yolo.cu": _SIMT_TC + ["kernels_yolo.cuh"],
-    "yolo_api.cu": _SIMT_TC + ["kernels_yolo.cuh", "api_error.h", _ABI],
+    "inst_yolo32.cu": _SIMT_TC + ["kernels_yolo.cuh", "kernels_yolo32.cuh"],
+    "yolo_api.cu": _SIMT_TC + ["kernels_yolo.cuh", "kernels_yolo32.cuh", "api_error.h", _ABI],
 }
 SOURCES = list(UNITS)
 HEADERS = sorted({h for hs in UNITS.values() for h in hs})

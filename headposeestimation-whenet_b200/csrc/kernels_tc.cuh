@@ -241,6 +241,22 @@ __device__ __forceinline__ void wg_acc_store(const WgAcc<N>& acc, uint32_t dst, 
             }
 }
 
+// fp32 -> bf16 hi + lo, x = hi + lo with hi = bf16(x), lo = bf16(x - hi) (|x - hi - lo| <= 2^-18 |x|), for the MMAs of the fp32
+// parity kernels (pw_tc32_kernel, conv_igemm32_kernel)
+__device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo) {
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const __nv_bfloat162 hh = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+        const float2 hf = __bfloat1622float2(hh);
+        const __nv_bfloat162 ll = __floats2bfloat162_rn(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
+        h[i] = *reinterpret_cast<const uint32_t*>(&hh);
+        l[i] = *reinterpret_cast<const uint32_t*>(&ll);
+    }
+    hi = make_uint4(h[0], h[1], h[2], h[3]);
+    lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
 // MMA widths the 1x1 kernels are instantiated for; a tile of n columns runs at the smallest one >= n (the extra B rows are
 // zero-filled, the extra columns never stored)
 __host__ __device__ constexpr int pw_mma_width(int n) { return n <= 64 ? (n + 15) & ~15 : n <= 96 ? 96 : 128; }

@@ -18,20 +18,6 @@
 namespace whenet {
 namespace tc {
 
-__device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const __nv_bfloat162 hh = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
-        const float2 hf = __bfloat1622float2(hh);
-        const __nv_bfloat162 ll = __floats2bfloat162_rn(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
-        h[i] = *reinterpret_cast<const uint32_t*>(&hh);
-        l[i] = *reinterpret_cast<const uint32_t*>(&ll);
-    }
-    hi = make_uint4(h[0], h[1], h[2], h[3]);
-    lo = make_uint4(l[0], l[1], l[2], l[3]);
-}
-
 // UN = pw_mma_width(n_tile): rows of the W stages, MMA width
 template <bool SWISH, bool GATE, bool RESID, int UN>
 __global__ void __launch_bounds__(128) pw_tc32_kernel(const float* __restrict__ A, const __nv_bfloat16* __restrict__ Whi,

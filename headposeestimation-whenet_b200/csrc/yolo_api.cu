@@ -14,7 +14,9 @@
 #include "../../include/whenet_b200.h"
 #include "api_error.h"
 #define WHENET_YOLO_HOST_ONLY
+#define WHENET_YOLO32_HOST_ONLY
 #include "kernels_yolo.cuh"
+#include "kernels_yolo32.cuh"
 
 using whenet::api::fail;
 namespace Y = whenet::yolo;
@@ -42,8 +44,18 @@ uint16_t bf16_bits(float f) {      // round to nearest even (finite inputs)
     return (uint16_t)(u >> 16);
 }
 
+// the fp32 mode's weight split: hi = bf16(v), lo = bf16(v - hi) (v - hi is exact in float)
+void split_bits(float v, uint16_t& hi, uint16_t& lo) {
+    hi = bf16_bits(v);
+    const uint32_t u = (uint32_t)hi << 16;
+    float h;
+    std::memcpy(&h, &u, 4);
+    lo = bf16_bits(v - h);
+}
+
 // Hi, Wi: the conv's input size (after the pool of a tiny conv); pooled: that pool's output, a buffer of its own
-struct LayerDev { int Hi, Wi, Ho, Wo, N; Y::IgemmPlan plan; void* out = nullptr; void* pooled = nullptr; };
+// plan / plan32: the tile plan of the bf16 / fp32 kernels (the one of the detector's precision is set)
+struct LayerDev { int Hi, Wi, Ho, Wo, N; Y::IgemmPlan plan; Y::Igemm32Plan plan32; void* out = nullptr; void* pooled = nullptr; };
 
 struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
@@ -99,12 +111,14 @@ int precompute_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::
 struct whenet_det {
     int device = 0, in_h = 0, in_w = 0, max_frames = 0, sm_count = 132;
     int num_classes = 0;
+    int precision = WHENET_PRECISION_BF16;      // or WHENET_PRECISION_FP32: fp32 activations, split-bf16 MMAs (kernels_yolo32.cuh)
     bool tiny = false;                  // tiny YOLOv3 (6 anchors, 13 convs, two heads) instead of YOLOv3 (9 anchors, 75 convs)
     bool loaded = false;
     cudaStream_t own_stream = nullptr, stream = nullptr, cap_stream = nullptr;
     std::vector<ConvCfg> table;
     std::vector<LayerDev> L;
-    void* warena = nullptr;             // bf16 kernels, [N][K] each, 256-byte aligned
+    void* warena = nullptr;             // bf16 kernels, [N][K] each, 256-byte aligned (fp32 mode: their hi parts)
+    void* warena_lo = nullptr;          // fp32 mode: the lo parts, at the same offsets
     float* barena = nullptr;            // fp32 biases
     std::vector<size_t> w_off, b_off;
     float anchors[18] = {};             // in (head, anchor-in-layer) slots, see DecodeParams
@@ -121,6 +135,7 @@ namespace {
 // candidates per frame: 1 + 4 + 16 cells per 32x32 block (tiny: 1 + 4)
 int ncand(const whenet_det* d) { return 3 * (d->in_h / 32) * (d->in_w / 32) * (d->tiny ? 5 : 21); }
 int num_heads(const whenet_det* d) { return d->tiny ? 2 : 3; }
+bool is_fp32(const whenet_det* d) { return d->precision == WHENET_PRECISION_FP32; }
 
 void free_layers(whenet_det* d) {
     for (auto& l : d->L) { cudaFree(l.out); cudaFree(l.pooled); l.out = l.pooled = nullptr; }
@@ -136,9 +151,38 @@ void free_graphs(whenet_det* d) {
 }
 
 const __nv_bfloat16* bf(const whenet_det* d, size_t off) { return reinterpret_cast<const __nv_bfloat16*>((const char*)d->warena + off); }
+const __nv_bfloat16* bf_lo(const whenet_det* d, size_t off) { return reinterpret_cast<const __nv_bfloat16*>((const char*)d->warena_lo + off); }
+
+// enqueue_conv of an fp32 detector
+int enqueue_conv32(whenet_det* d, cudaStream_t s, int i, int n) {
+    const ConvCfg& c = d->table[i];
+    const LayerDev& l = d->L[i];
+    if (c.pool) {
+        const LayerDev& src = d->L[c.src];
+        const int rc = Y::launch_maxpool32(s, (const float*)src.out, (float*)l.pooled, n, src.Ho, src.Wo, src.N, c.pool);
+        if (rc) return fail(WHENET_ECUDA, "max-pool before conv %d launch failed: %s", i, cudaGetErrorString((cudaError_t)rc));
+    }
+    Y::Igemm32Params p{};
+    const int N = l.N;
+    p.in = (const float*)(c.pool ? l.pooled : d->L[c.src].out);
+    p.up = c.up >= 0 ? (const float*)d->L[c.up].out : nullptr;
+    p.w_hi = bf(d, d->w_off[i]);
+    p.w_lo = bf_lo(d, d->w_off[i]);
+    p.bias = d->barena + d->b_off[i];
+    p.resid = c.res >= 0 ? (const float*)d->L[c.res].out : nullptr;
+    p.out = (float*)l.out;
+    p.M = n * l.Ho * l.Wo; p.Hi = l.Hi; p.Wi = l.Wi; p.Ho = l.Ho; p.Wo = l.Wo;
+    p.Cin = c.cin; p.c_up = c.up >= 0 ? d->table[c.up].cout : 0; p.N = N; p.k = c.k; p.stride = c.stride;
+    p.n_tile = l.plan32.n_tile; p.n_stages = l.plan32.n_stages;
+    const int rc = Y::launch_igemm32(s, p, Y::igemm_mode(c), l.plan32.un, l.plan32.smem, (N + l.plan32.n_tile - 1) / l.plan32.n_tile,
+                                     (p.M + Y::BM - 1) / Y::BM);
+    if (rc) return fail(WHENET_ECUDA, "conv %d launch failed: %s", i, cudaGetErrorString((cudaError_t)rc));
+    return 0;
+}
 
 // enqueue one conv (every table conv but the first), with the max-pool of its input for a tiny conv, on stream s, n frames
 int enqueue_conv(whenet_det* d, cudaStream_t s, int i, int n) {
+    if (is_fp32(d)) return enqueue_conv32(d, s, i, n);
     const ConvCfg& c = d->table[i];
     const LayerDev& l = d->L[i];
     if (c.pool) {
@@ -186,8 +230,12 @@ int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
     cudaStream_t s = d->cap_stream;
     CKD(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
     int rc = Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb);
-    if (!rc) rc = Y::launch_conv0(s, d->d_canvas, bf(d, d->w_off[0]), d->barena + d->b_off[0], (__nv_bfloat16*)d->L[0].out, n, d->in_h, d->in_w,
-                                 d->table[0].cout);
+    if (!rc && is_fp32(d))
+        rc = Y::launch_conv0_32(s, d->d_canvas, bf(d, d->w_off[0]), bf_lo(d, d->w_off[0]), d->barena + d->b_off[0], (float*)d->L[0].out, n,
+                                d->in_h, d->in_w, d->table[0].cout);
+    else if (!rc)
+        rc = Y::launch_conv0(s, d->d_canvas, bf(d, d->w_off[0]), d->barena + d->b_off[0], (__nv_bfloat16*)d->L[0].out, n, d->in_h, d->in_w,
+                             d->table[0].cout);
     int rc2 = rc ? fail(WHENET_ECUDA, "letterbox / first conv launch failed: %s", cudaGetErrorString((cudaError_t)rc)) : 0;
     for (size_t i = 1; i < d->table.size() && !rc2; ++i) rc2 = enqueue_conv(d, s, (int)i, n);
     cudaGraph_t g = nullptr;
@@ -253,16 +301,64 @@ int to_f32_tap(const void* src, bool is_f32, size_t n, float* out) {
     return 0;
 }
 
+// whenet_det_debug_conv on an fp32 detector (arguments checked): the host float32 values as given, the weights split into hi
+// and lo as whenet_det_load_weights splits them, conv_igemm32_kernel, fp32 output
+int debug_conv32(whenet_det* d, const float* x, const float* up, int n, int H, int W, int cin, int c_up, const float* w, const float* bias,
+                 int k, int stride, int cout, int leaky, const float* resid, float* out) {
+    const int Ho = H / stride, Wo = W / stride;
+    const size_t nx = (size_t)n * H * W * (cin - c_up), nu = (size_t)n * (H / 2) * (W / 2) * c_up, no = (size_t)n * Ho * Wo * cout;
+    const int K = k * k * cin, rows = (cout + 127) / 128 * 128;
+    std::vector<uint16_t> hw((size_t)rows * K, 0), hl((size_t)rows * K, 0);
+    for (int o = 0; o < cout; ++o)
+        for (int i = 0; i < K; ++i) split_bits(w[(size_t)i * cout + o], hw[(size_t)o * K + i], hl[(size_t)o * K + i]);
+    std::vector<float> hb((size_t)rows, 0.f);
+    std::copy(bias, bias + cout, hb.begin());
+    void *dx = nullptr, *du = nullptr, *dw = nullptr, *dl = nullptr, *db = nullptr, *dr = nullptr, *dout = nullptr;
+    auto cleanup = [&]() { cudaFree(dx); cudaFree(du); cudaFree(dw); cudaFree(dl); cudaFree(db); cudaFree(dr); cudaFree(dout); };
+    if (cudaMalloc(&dx, nx * 4) || (nu && cudaMalloc(&du, nu * 4)) || cudaMalloc(&dw, hw.size() * 2) || cudaMalloc(&dl, hl.size() * 2) ||
+        cudaMalloc(&db, hb.size() * 4) || (resid && cudaMalloc(&dr, no * 4)) || cudaMalloc(&dout, no * 4)) {
+        cleanup();
+        return fail(WHENET_ECUDA, "out of device memory");
+    }
+    // on the detector's stream, as whenet_det_debug_conv does (pageable copies may return before their DMA has landed)
+    cudaMemcpyAsync(dx, x, nx * 4, cudaMemcpyHostToDevice, d->stream);
+    if (nu) cudaMemcpyAsync(du, up, nu * 4, cudaMemcpyHostToDevice, d->stream);
+    cudaMemcpyAsync(dw, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice, d->stream);
+    cudaMemcpyAsync(dl, hl.data(), hl.size() * 2, cudaMemcpyHostToDevice, d->stream);
+    cudaMemcpyAsync(db, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice, d->stream);
+    if (resid) cudaMemcpyAsync(dr, resid, no * 4, cudaMemcpyHostToDevice, d->stream);
+    Y::Igemm32Params p{};
+    p.in = (const float*)dx; p.up = (const float*)du; p.w_hi = (const __nv_bfloat16*)dw; p.w_lo = (const __nv_bfloat16*)dl;
+    p.bias = (const float*)db; p.resid = (const float*)dr; p.out = (float*)dout;
+    p.M = n * Ho * Wo; p.Hi = H; p.Wi = W; p.Ho = Ho; p.Wo = Wo; p.Cin = cin; p.c_up = c_up; p.N = cout; p.k = k; p.stride = stride;
+    const Y::Igemm32Plan pl = Y::plan_igemm32(Ho, Wo, cout, cin, k, d->sm_count);
+    p.n_tile = pl.n_tile; p.n_stages = pl.n_stages;
+    const int mode = !leaky ? Y::kLinearF32 : up ? Y::kLeakyCat : resid ? Y::kLeakyRes : Y::kLeaky;
+    int rc = Y::launch_igemm32(d->stream, p, mode, pl.un, pl.smem, (cout + pl.n_tile - 1) / pl.n_tile, (p.M + Y::BM - 1) / Y::BM);
+    if (!rc) rc = (int)cudaStreamSynchronize(d->stream);
+    if (!rc) rc = to_f32_tap(dout, true, no, out) ? -1 : 0;
+    cleanup();
+    if (rc > 0) return fail(WHENET_ECUDA, "debug conv failed: %s", cudaGetErrorString((cudaError_t)rc));
+    return rc ? WHENET_ECUDA : 0;
+}
+
 }  // namespace
 
 extern "C" {
 
 int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, int max_frames) {
+    return whenet_det_create_ex(out, device, input_h, input_w, max_frames, WHENET_PRECISION_BF16);
+}
+
+int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision) {
     if (!out) return fail(WHENET_EINVAL, "out is NULL");
     *out = nullptr;
     for (int v : {input_h, input_w})
         if (v < 32 || v > 608 || v % 32) return fail(WHENET_EINVAL, "input size %dx%d: both must be multiples of 32 in [32, 608]", input_w, input_h);
     if (max_frames < 1 || max_frames > 64) return fail(WHENET_EINVAL, "max_frames=%d outside [1, 64]", max_frames);
+    if (precision != WHENET_PRECISION_BF16 && precision != WHENET_PRECISION_FP32)
+        return fail(WHENET_EINVAL, "precision %d: the detector runs in WHENET_PRECISION_BF16 (%d) or WHENET_PRECISION_FP32 (%d)", precision,
+                    WHENET_PRECISION_BF16, WHENET_PRECISION_FP32);
     int ndev = 0;
     CKD(cudaGetDeviceCount(&ndev));
     if (device < 0 || device >= ndev) return fail(WHENET_EINVAL, "device %d not in [0,%d)", device, ndev);
@@ -273,6 +369,7 @@ int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, in
         return fail(WHENET_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     whenet_det* d = new whenet_det();
     d->device = device; d->in_h = input_h; d->in_w = input_w; d->max_frames = max_frames; d->sm_count = prop.multiProcessorCount;
+    d->precision = precision;
     d->table = make_table();
     d->L.resize(d->table.size());
     auto bail = [&](int rc) { whenet_det_destroy(d); return rc; };
@@ -300,7 +397,8 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
     const whenet_tensor& h0 = t[need - 2];      // output conv of head 2 (its kernel), all heads have the same width
     if (h0.ndim != 4 || h0.dims[3] < 18 || h0.dims[3] % 3) return fail(WHENET_ESHAPE, "%s: output conv width is not 3 * (5 + classes)", h0.name ? h0.name : "?");
     const int C = (int)h0.dims[3] / 3 - 5;
-    std::vector<uint16_t> hw;
+    const bool f32 = is_fp32(d);
+    std::vector<uint16_t> hw, hw_lo;       // hw_lo: fp32 mode, the lo parts
     std::vector<float> hb;
     std::vector<size_t> w_off, b_off;
     size_t ti = 0;
@@ -326,19 +424,27 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
             if (b.ndim != 1 || b.dims[0] != co) return fail(WHENET_ESHAPE, "%s (output conv %zu): bias must be [%d]", b.name ? b.name : "?", i, co);
             for (int o = 0; o < co; ++o) shift[o] = b.data[o];
         }
-        // kernel -> [N][K] bf16 (K = (ky*k + kx)*cin + ci); conv 0 -> [N][64] = [w(27) 0(5) w(27) 0(5)] for the hi/lo input split
+        // kernel -> [N][K] bf16 (K = (ky*k + kx)*cin + ci); conv 0 -> [N][64] = [w(27) 0(5) w(27) 0(5)] for the hi/lo input split.
+        // fp32 mode: hw holds the hi parts in that layout, hw_lo the lo parts ([N][K]; conv 0: [N][64] = [w_lo(27) 0(37)])
         const int taps = c.k * c.k;
         const int N = co, K = i == 0 ? 64 : taps * c.cin;
         const int rows = (N + 127) / 128 * 128;     // every weight tile the kernels may touch exists (zero rows past N)
         w_off.push_back(hw.size() * 2);
         hw.resize(hw.size() + (size_t)rows * K + 128, 0);
+        if (f32) hw_lo.resize(hw.size(), 0);
         uint16_t* dst = hw.data() + w_off.back() / 2;
+        uint16_t* dst_lo = f32 ? hw_lo.data() + w_off.back() / 2 : nullptr;
         for (int o = 0; o < N; ++o)
             for (int tp = 0; tp < taps; ++tp)
                 for (int ci = 0; ci < c.cin; ++ci) {
-                    const uint16_t v = bf16_bits((float)((double)k.data[((size_t)tp * c.cin + ci) * co + o] * scale[o]));
-                    if (i == 0) { dst[(size_t)o * K + tp * 3 + ci] = v; dst[(size_t)o * K + 32 + tp * 3 + ci] = v; }
-                    else dst[(size_t)o * K + (size_t)tp * c.cin + ci] = v;
+                    const float wf = (float)((double)k.data[((size_t)tp * c.cin + ci) * co + o] * scale[o]);
+                    uint16_t v, lo = 0;
+                    if (f32) split_bits(wf, v, lo);
+                    else v = bf16_bits(wf);
+                    const size_t j = (size_t)o * K + (i == 0 ? (size_t)tp * 3 + ci : (size_t)tp * c.cin + ci);
+                    dst[j] = v;
+                    if (i == 0) dst[j + 32] = v;
+                    if (f32) dst_lo[j] = lo;
                 }
         b_off.push_back(hb.size());
         hb.resize(hb.size() + (size_t)(N + 127) / 128 * 128, 0.f);
@@ -347,11 +453,15 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
     CKD(cudaSetDevice(d->device));
     CKD(cudaStreamSynchronize(d->stream));
     free_graphs(d);
-    cudaFree(d->warena); cudaFree(d->barena);
-    d->warena = nullptr; d->barena = nullptr; d->loaded = false;
+    cudaFree(d->warena); cudaFree(d->warena_lo); cudaFree(d->barena);
+    d->warena = nullptr; d->warena_lo = nullptr; d->barena = nullptr; d->loaded = false;
     CKD(cudaMalloc(&d->warena, hw.size() * 2));
     CKD(cudaMalloc(&d->barena, hb.size() * 4));
     CKD(cudaMemcpy(d->warena, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice));
+    if (f32) {
+        CKD(cudaMalloc(&d->warena_lo, hw_lo.size() * 2));
+        CKD(cudaMemcpy(d->warena_lo, hw_lo.data(), hw_lo.size() * 2, cudaMemcpyHostToDevice));
+    }
     CKD(cudaMemcpy(d->barena, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
     d->w_off = w_off; d->b_off = b_off;
     // anchors in (head, anchor-in-layer) slots: the decode reads slot 3 * l + a for either network
@@ -378,9 +488,10 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
             l.Wi = Y::pooled(c.src < 0 ? d->in_w : d->L[c.src].Wo, c.pool);
             l.Ho = l.Hi / c.stride; l.Wo = l.Wi / c.stride;
             l.N = c.head >= 0 ? 3 * (5 + C) : c.cout;
-            l.plan = Y::plan_igemm(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
-            CKD(cudaMalloc(&l.out, (size_t)d->max_frames * l.Ho * l.Wo * l.N * (c.head >= 0 ? 4 : 2)));
-            if (c.pool) CKD(cudaMalloc(&l.pooled, (size_t)d->max_frames * l.Hi * l.Wi * c.cin * 2));
+            if (f32) l.plan32 = Y::plan_igemm32(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
+            else l.plan = Y::plan_igemm(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
+            CKD(cudaMalloc(&l.out, (size_t)d->max_frames * l.Ho * l.Wo * l.N * (c.head >= 0 || f32 ? 4 : 2)));
+            if (c.pool) CKD(cudaMalloc(&l.pooled, (size_t)d->max_frames * l.Hi * l.Wi * c.cin * (f32 ? 4 : 2)));
         }
         const size_t nc = (size_t)ncand(d), slots = (size_t)d->max_frames * C * Y::kMaxBoxes;
         CKD(cudaMalloc(&d->d_cand, (size_t)d->max_frames * nc * 16));
@@ -395,6 +506,11 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
 }
 
 int whenet_det_num_classes(whenet_det* d) { return d ? d->num_classes : 0; }
+
+int whenet_det_precision(whenet_det* d) {
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    return d->precision;
+}
 
 int whenet_det_set_stream(whenet_det* d, void* s) {
     if (!d) return fail(WHENET_EINVAL, "null detector");
@@ -446,7 +562,7 @@ void whenet_det_destroy(whenet_det* d) {
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_graphs(d);
     free_layers(d);
-    cudaFree(d->warena); cudaFree(d->barena); cudaFree(d->d_frames); cudaFree(d->d_canvas);
+    cudaFree(d->warena); cudaFree(d->warena_lo); cudaFree(d->barena); cudaFree(d->d_frames); cudaFree(d->d_canvas);
     cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
     if (d->own_stream) cudaStreamDestroy(d->own_stream);
     if (d->cap_stream) cudaStreamDestroy(d->cap_stream);
@@ -475,8 +591,8 @@ int whenet_det_debug_tap(whenet_det* d, int layer, float* out, size_t cap, size_
         for (size_t i = 0; i < n; ++i) out[i] = h[i];
         return 0;
     }
-    if (pool_tap) return to_f32_tap(l->pooled, false, n, out);
-    return to_f32_tap(l->out, d->table[layer].head >= 0, n, out);
+    if (pool_tap) return to_f32_tap(l->pooled, is_fp32(d), n, out);
+    return to_f32_tap(l->out, d->table[layer].head >= 0 || is_fp32(d), n, out);
 }
 
 int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n, int H, int W, int cin, int c_up, const float* w, const float* bias,
@@ -491,6 +607,7 @@ int whenet_det_debug_conv(whenet_det* d, const float* x, const float* up, int n,
     if (up && (stride != 1 || c_up < 64 || c_up % 64 || c_up >= cin || H % 2 || W % 2)) return fail(WHENET_EINVAL, "bad concat shape");
     if (!up) c_up = 0;
     CKD(cudaSetDevice(d->device));
+    if (is_fp32(d)) return debug_conv32(d, x, up, n, H, W, cin, c_up, w, bias, k, stride, cout, leaky, resid, out);
     const int Ho = H / stride, Wo = W / stride;
     const size_t nx = (size_t)n * H * W * (cin - c_up), nu = (size_t)n * (H / 2) * (W / 2) * c_up, no = (size_t)n * Ho * Wo * cout;
     const int K = k * k * cin, rows = (cout + 127) / 128 * 128;
@@ -538,6 +655,20 @@ int whenet_det_debug_maxpool(whenet_det* d, const float* x, int n, int H, int W,
         return fail(WHENET_EINVAL, "bad max-pool shape (n=%d H=%d W=%d C=%d stride=%d)", n, H, W, C, stride);
     CKD(cudaSetDevice(d->device));
     const size_t ni = (size_t)n * H * W * C, no = (size_t)n * Y::pooled(H, stride) * Y::pooled(W, stride) * C;
+    if (is_fp32(d)) {                   // the host values as given, the fp32 kernel
+        void *dx = nullptr, *dout = nullptr;
+        if (cudaMalloc(&dx, ni * 4) || cudaMalloc(&dout, no * 4)) {
+            cudaFree(dx); cudaFree(dout);
+            return fail(WHENET_ECUDA, "out of device memory");
+        }
+        int rc = (int)cudaMemcpyAsync(dx, x, ni * 4, cudaMemcpyHostToDevice, d->stream);
+        if (!rc) rc = Y::launch_maxpool32(d->stream, (const float*)dx, (float*)dout, n, H, W, C, stride);
+        if (!rc) rc = (int)cudaStreamSynchronize(d->stream);
+        if (!rc) rc = (int)cudaMemcpy(out, dout, no * 4, cudaMemcpyDeviceToHost);
+        cudaFree(dx); cudaFree(dout);
+        if (rc) return fail(WHENET_ECUDA, "debug max-pool failed: %s", cudaGetErrorString((cudaError_t)rc));
+        return 0;
+    }
     std::vector<uint16_t> hx(ni);
     for (size_t i = 0; i < ni; ++i) hx[i] = bf16_bits(x[i]);
     void *dx = nullptr, *dout = nullptr;

@@ -7,6 +7,10 @@ flagged by ``self.random_weights``; the reference's trained ``head_detect.h5`` i
 
 As in the reference (yolo_postprocess.py:71-79), the anchors pick the network: 9 anchors mean YOLOv3 (``yolo_body``), 6 mean
 tiny YOLOv3 (``tiny_yolo_body``, ``self.tiny``).
+
+``precision`` (keyword only) is ``"bf16"`` (the default: bf16 activations, fp32 accumulation) or ``"fp32"``, the parity mode:
+fp32 activations and every conv as three bf16 MMAs on the hi / lo split of activations and weights (DESIGN.md 8.3).  The
+reference runs its detector in float32.
 """
 from __future__ import annotations
 
@@ -19,6 +23,8 @@ import numpy as np
 from . import _lib, h5lite, yolo_arch
 from ._lib import check
 from .whenet import _is_device, _ptr
+
+_PRECISIONS = {"bf16": _lib.PRECISIONS["bf16"], "fp32": _lib.PRECISIONS["fp32"]}
 
 
 def _tensor_list(layers):
@@ -41,8 +47,11 @@ def _tensor_list(layers):
 
 class YOLO:
     def __init__(self, model_path=None, anchors_path=None, classes_path=None, score=0.3, iou=0.45, model_image_size=(416, 416),
-                 gpu_num=1, *, device: Optional[int] = None, max_frames: int = 8, seed: int = 0, **kwargs):
+                 gpu_num=1, *, device: Optional[int] = None, max_frames: int = 8, seed: int = 0, precision: str = "bf16", **kwargs):
+        if precision not in _PRECISIONS:
+            raise ValueError("precision must be one of %s, not %r" % (sorted(_PRECISIONS), precision))
         self.__dict__.update(kwargs)
+        self.precision = precision
         self.model_path, self.anchors_path, self.classes_path = model_path, anchors_path, classes_path
         self.score, self.iou, self.gpu_num = float(score), float(iou), gpu_num
         size = tuple(model_image_size)
@@ -72,7 +81,7 @@ class YOLO:
         self.max_frames = int(max_frames)
         self._L = _lib.load()
         self._h = C.c_void_p()
-        check(self._L.whenet_det_create(C.byref(self._h), self.device, size[0], size[1], self.max_frames))
+        check(self._L.whenet_det_create_ex(C.byref(self._h), self.device, size[0], size[1], self.max_frames, _PRECISIONS[precision]))
         self.load_layers(layers)
 
     def load_layers(self, layers, anchors=None):
@@ -147,7 +156,8 @@ class YOLO:
         return out
 
     def debug_maxpool(self, x, stride: int):
-        """The device 2x2 max-pool (TF SAME) of x (n,H,W,C), rounded to bf16 on the way in -> (n, ceil(H/s), ceil(W/s), C)."""
+        """The device 2x2 max-pool (TF SAME) of x (n,H,W,C), rounded to bf16 on the way in (fp32 detector: as given)
+        -> (n, ceil(H/s), ceil(W/s), C)."""
         x = np.ascontiguousarray(x, np.float32)
         n, H, W, c = x.shape
         out = np.empty((n, -(-H // stride), -(-W // stride), c), np.float32)

@@ -212,19 +212,29 @@ void whenet_destroy(whenet_ctx* ctx);
 /* ==== YOLOv3 head detector (reference yolo_v3/yolo_postprocess.py:26-205, yolo_v3/model.py) ====
  * A detector handle is bound to one device, one stream and one model input size (multiples of 32 in [32, 608]; the
  * reference's model_image_size, default 416 x 416) and is NOT thread-safe.  Errors use the WHENET_E* codes and
- * whenet_last_error().  Storage is bf16, accumulation fp32; the head logits stay fp32. */
+ * whenet_last_error().  Storage is bf16, accumulation fp32; the head logits stay fp32 (whenet_det_create).  The fp32
+ * parity mode (whenet_det_create_ex with WHENET_PRECISION_FP32) keeps every activation in fp32 and runs each conv as three
+ * bf16 MMAs on the hi / lo split of activations and weights, with fp32 accumulation (DESIGN.md 8.3). */
 typedef struct whenet_det whenet_det;
 
 /* replaces: YOLO.__init__ graph construction (yolo_postprocess.py:44-50, 77-78 yolo_body).  `max_frames` bounds n of one
  * detect call (1..64). */
 int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, int max_frames);
+/* whenet_det_create with a precision: WHENET_PRECISION_BF16 (what whenet_det_create makes) or WHENET_PRECISION_FP32 (the
+ * parity mode); any other value is WHENET_EINVAL.  The activation buffers of one frame take, for one class, 77 MB at 416 x 416
+ * and 164 MB at 608 x 608 in bf16 (tiny YOLOv3: 15 and 32 MB), and twice that in fp32: 153 and 328 MB (tiny: 30 and 63 MB);
+ * they are allocated for `max_frames` frames. */
+int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision);
+
+/* The detector's precision (WHENET_PRECISION_BF16 or WHENET_PRECISION_FP32). */
+int whenet_det_precision(whenet_det* det);
 
 /* replaces: load_model / yolo_model.load_weights(model_path) (yolo_postprocess.py:74-79) and _get_anchors (:59-64).
  * `anchors`: 9 (w, h) pairs in input pixels for YOLOv3 (yolo_body), 6 for tiny YOLOv3 (tiny_yolo_body, model.py:92-122);
  * any other count is WHENET_EINVAL.  `tensors`: the network's 75 (tiny: 13) convs in Keras weight order
  * (whenet_b200/yolo_arch.py), each its kernel [k,k,cin,cout] followed by BatchNorm gamma, beta, moving_mean,
  * moving_variance (bias-free convs) or by its bias (the output convs); BatchNorm (eps 1e-3) is folded in double and the
- * kernels rounded once to bf16.  The class count follows from the output convs' width 3 * (5 + classes).  Loading the
+ * kernels rounded once to bf16 (fp32 detector: to fp32, then split into bf16 hi = bf16(w) and lo = bf16(w - hi)).  The class count follows from the output convs' width 3 * (5 + classes).  Loading the
  * other network or another class count into a live detector rebuilds its buffers and captured graphs. */
 int whenet_det_load_weights(whenet_det* det, const whenet_tensor* tensors, int n_tensors, const float* anchors, int n_anchors);
 
@@ -249,6 +259,8 @@ int whenet_det_synchronize(whenet_det* det);
 void whenet_det_destroy(whenet_det* det);
 
 /* ---- detector test hooks (no reference counterpart) ---- */
+/* On an fp32 detector the hooks below take and return its fp32 values: taps are the fp32 activations, and debug_conv /
+ * debug_maxpool use the host float32 inputs as given (no bf16 rounding) and run the fp32 kernels. */
 /* float32 copy of the output of conv `layer` (0..74, tiny: 0..12, table order) of the last detect call (n x Ho x Wo x Cout),
  * with layer = -1 of its letterboxed uint8 canvas (n x input_h x input_w x 3), or with layer = 100 + i of the max-pooled
  * input of tiny conv i (i = 1..6; n x Hi x Wi x Cin). out=NULL queries the element count. */

@@ -1,9 +1,10 @@
 """Detector throughput on one GPU: frames/s and TFLOP/s of whenet_b200.YOLO at 416^2 and 608^2 for n = 1 and 8 frames per
 call, a per-kernel breakdown from CUDA events (torch.profiler), and the full detect_and_estimate frames/s with the head
 biases set so that each frame yields about 20 boxes.  Prints the card's name, power limit and max SM clock of the same run.
-``--tiny`` measures tiny YOLOv3 (the 6 anchors of tests/golden/tiny_yolo_anchors.txt) instead of YOLOv3.
+``--tiny`` measures tiny YOLOv3 (the 6 anchors of tests/golden/tiny_yolo_anchors.txt) instead of YOLOv3; ``--precision fp32``
+the detector's fp32 parity mode (and WHENet's fp32 mode in the detect_and_estimate row) instead of bf16.
 
-    python tools/detect_bench.py [--tiny] [--iters 50] [--out detect_bench.json]
+    python tools/detect_bench.py [--tiny] [--precision {bf16,fp32}] [--iters 50] [--out detect_bench.json]
 """
 import argparse
 import json
@@ -84,11 +85,13 @@ def kernel_table(fn):
     for e in prof.events():
         if e.device_type == torch.autograd.DeviceType.CUDA:
             name = e.name.split("(")[0].replace("void ", "")
-            if "yolo_conv0_kernel" in e.name:
-                name = "yolo_conv0_kernel"
-            for key in ("conv_igemm_kernel<0", "conv_igemm_kernel<1", "conv_igemm_kernel<2", "conv_igemm_kernel<3"):
-                if key in e.name:
-                    name = "conv_igemm[%s]" % {"0": "leaky", "1": "leaky+res", "2": "concat", "3": "head fp32"}[key[-1]]
+            for k0 in ("yolo_conv0_kernel", "yolo_conv0_32_kernel"):
+                if k0 + "<" in e.name:
+                    name = k0
+            for kern in ("conv_igemm_kernel", "conv_igemm32_kernel"):
+                for mode in "0123":
+                    if "%s<%s" % (kern, mode) in e.name:
+                        name = "%s[%s]" % (kern.replace("_kernel", ""), {"0": "leaky", "1": "leaky+res", "2": "concat", "3": "head fp32"}[mode])
             r = rows.setdefault(name, [0.0, 0])
             r[0] += e.device_time_total / 1e3
             r[1] += 1
@@ -100,6 +103,7 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--out", default=None)
     ap.add_argument("--tiny", action="store_true", help="tiny YOLOv3 (6 anchors) instead of YOLOv3")
+    ap.add_argument("--precision", choices=("bf16", "fp32"), default="bf16", help="the detector's precision (default bf16)")
     a = ap.parse_args()
     import torch
     import whenet_b200
@@ -107,11 +111,12 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("no GPU: nothing to measure")
     anchors = TINY_ANCHORS if a.tiny else None
-    res = {"card": card(), "device": torch.cuda.get_device_name(0), "network": "tiny YOLOv3" if a.tiny else "YOLOv3", "runs": []}
-    print("card:", res["card"], " network:", res["network"])
+    res = {"card": card(), "device": torch.cuda.get_device_name(0), "network": "tiny YOLOv3" if a.tiny else "YOLOv3",
+           "precision": a.precision, "runs": []}
+    print("card:", res["card"], " network:", res["network"], " precision:", a.precision)
     f = frame1080()
     for size in (416, 608):
-        m = whenet_b200.YOLO(None, anchors_path=anchors, model_image_size=(size, size), max_frames=8)
+        m = whenet_b200.YOLO(None, anchors_path=anchors, model_image_size=(size, size), max_frames=8, precision=a.precision)
         flops = 2.0 * Y.macs_per_frame(size, size, tiny=a.tiny)
         for n in (1, 8):
             frames = np.stack([f] * n)[:, :, :, ::-1].copy()
@@ -130,8 +135,8 @@ def main():
                 print("    %-40s %8.4f ms  x%d" % tuple(k))
         m.close()
     # full pipeline: head objectness biases raised so that about 20 boxes survive NMS per frame
-    m = whenet_b200.YOLO(None, anchors_path=anchors, max_frames=1)
-    wn = whenet_b200.WHENet(whenet_b200.weights.DEFAULT_NPZ, device=0, precision="bf16", max_batch=64)
+    m = whenet_b200.YOLO(None, anchors_path=anchors, max_frames=1, precision=a.precision)
+    wn = whenet_b200.WHENet(whenet_b200.weights.DEFAULT_NPZ, device=0, precision=a.precision, max_batch=64)
     best = set_objectness_for_boxes(m, f, a.tiny)
     sec = time_calls(lambda: whenet_b200.pipeline.detect_and_estimate(m, wn, f), a.iters)
     res["pipeline"] = {"boxes_per_frame": best[1], "objectness_bias": float(best[0]), "ms_per_frame": sec * 1e3, "frames_per_s": 1 / sec}
