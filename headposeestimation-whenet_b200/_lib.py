@@ -16,7 +16,7 @@ EXPORTS = [
     "whenet_last_error", "whenet_version", "whenet_destroy",
     "whenet_det_create", "whenet_det_load_weights", "whenet_det_num_classes", "whenet_det_set_stream", "whenet_det_detect_u8",
     "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_maxpool",
-    "whenet_det_debug_decode", "whenet_det_create_ex", "whenet_det_precision",
+    "whenet_det_debug_decode", "whenet_det_create_ex", "whenet_det_precision", "whenet_det_detect_ragged_u8", "whenet_crop_boxes_ragged_u8",
 ]
 
 
@@ -71,6 +71,7 @@ def load():
     L.whenet_forward_u8_async.argtypes = [P, P, C.c_int, P, P]
     L.whenet_crop_resize_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, C.c_int, C.c_int, P]
     L.whenet_crop_boxes_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P]
+    L.whenet_crop_boxes_ragged_u8.argtypes = [P, P, P, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P]
     L.whenet_debug_enlarge_boxes.argtypes = [P, C.c_int, C.c_int, C.c_int, P, P]
     L.whenet_synchronize.argtypes = [P]
     L.whenet_host_alloc.argtypes = [C.c_size_t]
@@ -100,6 +101,7 @@ def load():
     L.whenet_det_num_classes.argtypes = [P]
     L.whenet_det_set_stream.argtypes = [P, P]
     L.whenet_det_detect_u8.argtypes = [P, P, I, I, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
+    L.whenet_det_detect_ragged_u8.argtypes = [P, P, P, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
     L.whenet_det_synchronize.argtypes = [P]
     L.whenet_det_destroy.argtypes = [P]
     L.whenet_det_destroy.restype = None

@@ -12,6 +12,13 @@ int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in,
     return (int)cudaGetLastError();
 }
 
+int launch_letterbox_ragged(cudaStream_t s, const LetterboxFrame* plans, const char* coef, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n,
+                            long long max_hx, int S_h, int S_w, int swap_rb) {
+    letterbox_h_ragged_kernel<<<dim3((unsigned)((max_hx + 255) / 256), n), 256, 0, s>>>(plans, coef, in, tmp, swap_rb);
+    letterbox_v_ragged_kernel<<<dim3((unsigned)((S_h * S_w + 255) / 256), n), 256, 0, s>>>(plans, coef, tmp, out, S_h, S_w);
+    return (int)cudaGetLastError();
+}
+
 template <int N>
 int launch_conv0_t(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w) {
     constexpr size_t smem = 128 * 128 + N * 128 + 256 * 4 + tc::acc_tile_bytes(N) + 1024;

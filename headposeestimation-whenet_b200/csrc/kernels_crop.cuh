@@ -4,12 +4,14 @@
 // 224x224 exactly as cv2.resize's 8-bit INTER_LINEAR kernel does (reference demo_video.py:21-23,
 // demo.py:10-11): half-pixel centres, 11-bit weights rounded to nearest-even, int32 horizontal pass,
 // ((b0*(r0>>4))>>16) + ((b1*(r1>>4))>>16) + 2 >> 2 vertical pass, 2x2 box for exact 2x down-scaling.
-// All heads of one frame or of n frames of one size come out as ONE uint8 NHWC batch that feeds the
+// All heads of one frame, of n frames of one size or of n frames of their own sizes come out as ONE uint8 NHWC batch that feeds the
 // stem kernel directly - the reference crops, resizes and runs the network one head at a time
 // (demo_video.py:13-23, 57-58).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace whenet {
 
@@ -37,10 +39,23 @@ __device__ __forceinline__ AxisTap axis_tap(int d, int src, bool clamp_weights) 
     return t;
 }
 
-// grid = (ceil(224*224/256), M).  frames: n frames of H x W x 3 back to back; rects[m] = (y0, y1, x0, x1) slice
-// bounds inside frame frame_of[m] (frame 0 for every crop when frame_of is NULL).  An empty rect (y1 <= y0 or
-// x1 <= x0) marks an invalid crop: it reads nothing and is written as zeros.
-__global__ void __launch_bounds__(256) crop_resize_kernel(const uint8_t* __restrict__ frames, int H, int W,
+constexpr int kMaxCropFrames = 64;
+
+// n frames of one size H x W x 3, back to back
+struct OneSizeFrames {
+    const uint8_t* frames;
+    int H, W;
+};
+// n <= kMaxCropFrames frames of their own sizes, each H x W x 3 at its own base (the host checked every rect against its H)
+struct PerFrameSources {
+    struct Frame { const uint8_t* base; int W; } f[kMaxCropFrames];
+};
+
+// grid = (ceil(224*224/256), M).  src: the frames; rects[m] = (y0, y1, x0, x1) slice bounds inside frame frame_of[m]
+// (frame 0 for every crop when frame_of is NULL, OneSizeFrames only).  An empty rect (y1 <= y0 or x1 <= x0) marks an
+// invalid crop: it reads nothing and is written as zeros.
+template <class Frames>
+__global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant__ Frames src_frames,
                                                           const int4* __restrict__ rects, const int* __restrict__ frame_of,
                                                           uint8_t* __restrict__ out, int swap_rb) {
     const int m = blockIdx.y;
@@ -51,9 +66,19 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const uint8_t* __restr
     const int y0 = r.x, h = r.y - r.x, x0 = r.z, w = r.w - r.z;
     uint8_t* dst = out + ((long long)m * 224 * 224 + pix) * 3;
     if (h <= 0 || w <= 0) { dst[0] = 0; dst[1] = 0; dst[2] = 0; return; }
+    const uint8_t* frame;
+    int W;
+    if constexpr (std::is_same<Frames, OneSizeFrames>::value) {
+        W = src_frames.W;
+        const long long f = frame_of ? frame_of[m] : 0;
+        frame = src_frames.frames + f * src_frames.H * ((long long)W * 3);
+    } else {
+        const auto& fr = src_frames.f[frame_of[m]];
+        W = fr.W;
+        frame = fr.base;
+    }
     const long long pitch = (long long)W * 3;
-    const long long f = frame_of ? frame_of[m] : 0;
-    const uint8_t* src = frames + f * H * pitch + ((long long)y0 * W + x0) * 3;
+    const uint8_t* src = frame + ((long long)y0 * W + x0) * 3;
     int v[3];
     if (h == 448 && w == 448) {                     // resize(): INTER_LINEAR with exact 2x down-scale -> 2x2 box
         const uint8_t* p = src + (long long)(2 * dy) * pitch + (2 * dx) * 3;

@@ -4,6 +4,7 @@
 //   letterbox_h_kernel / letterbox_v_kernel   Pillow's uint8 BICUBIC resample (two integer passes, 22-bit coefficients computed on
 //                                             the host exactly as ImagingResample does) + the (128,128,128) canvas and the paste
 //                                             (reference utils.py:23-34)
+//   letterbox_{h,v}_ragged_kernel              the same two passes over frames of different sizes, one LetterboxFrame each
 //   yolo_conv0_kernel<N>                       first conv (3 -> N = 32, tiny: 16, 3x3): im2col row built in shared memory from the
 //                                             uint8 canvas through a v/255 table split into bf16 hi + lo parts, one K = 64 wgmma
 //                                             block per row
@@ -145,6 +146,14 @@ constexpr int kNmsThreads = 1024;
 constexpr int kNmsPer = 24;             // candidates per thread: 24 x 1024 >= 22,743 (608 x 608)
 constexpr int kMaxBoxes = 256;
 
+constexpr int kMaxFrames = 64;          // frames per detector call (whenet_det_create's max_frames)
+
+// yolo_correct_boxes (model.py:159-161) of one frame, float32 on the host
+struct FrameGeo {
+    float img_h, img_w;                 // original image size
+    float off_y, off_x, scale_y, scale_x;
+};
+
 struct DecodeParams {
     const float* head[3];               // [n][gh_l][gw_l][3 * (5 + C)] fp32 logits, l = 0, 1, 2 (13x13, 26x26, 52x52 at 416; tiny: 2 heads)
     float4* cand;                       // workspace [n][NC] boxes (y_min, x_min, y_max, x_max)
@@ -156,9 +165,8 @@ struct DecodeParams {
     float anchors[18];                  // (w, h) of head l, anchor-in-layer a at slot 3 * l + a (kAnchorMask / kTinyAnchorMask)
     int gh0, gw0, C, NC, max_boxes;     // NC: candidates of all heads (the walk over the heads ends there)
     float in_h, in_w;                   // model input size
-    float img_h, img_w;                 // original image size
-    float off_y, off_x, scale_y, scale_x;   // yolo_correct_boxes (model.py:159-161), float32 on the host
     float score, iou;
+    FrameGeo geo[kMaxFrames];           // row f: frame f (a one-size batch repeats one row)
 };
 
 // launchers (inst_yolo.cu); each returns 0 or the CUDA error of the launch
@@ -172,7 +180,17 @@ struct LetterboxPlan {
     const int2* yb;          // [nh] (first row relative to y0, count)
     const int* ky;           // [nh][ksy]
 };
+// One frame of a batch of differently sized frames: LetterboxPlan's geometry, where its tables sit in the batch's coefficient
+// allocation and where its pixels and its horizontal-pass rows sit in the input and tmp buffers (byte offsets).
+struct LetterboxFrame {
+    long long src, tmp;
+    int H, W, nw, nh, ox, oy, y0, rows, ksx, ksy;
+    int xb, kx, yb, ky;
+};
 int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb);
+// plans: n device LetterboxFrame; max_hx: the largest rows * nw among them
+int launch_letterbox_ragged(cudaStream_t s, const LetterboxFrame* plans, const char* coef, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n,
+                            long long max_hx, int S_h, int S_w, int swap_rb);
 int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w,
                  int cout);
 int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m);
@@ -230,6 +248,60 @@ __global__ void letterbox_v_kernel(const uint8_t* __restrict__ tmp, uint8_t* __r
     const int2 b = yb[yy];
     const int* k = ky + (long long)yy * ksize;
     const uint8_t* src = tmp + (((long long)f * rows + b.x) * nw + xx) * 3;
+    int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+    for (int j = 0; j < b.y; ++j) {
+        const int w = k[j];
+        const uint8_t* p = src + (long long)j * nw * 3;
+        s0 += p[0] * w;
+        s1 += p[1] * w;
+        s2 += p[2] * w;
+    }
+    dst[0] = clip8(s0);
+    dst[1] = clip8(s1);
+    dst[2] = clip8(s2);
+}
+
+// The two passes over n frames that each have their own size: frame blockIdx.y follows plans[blockIdx.y], with the arithmetic of
+// letterbox_h_kernel / letterbox_v_kernel, so its canvas is the one those give it alone.  The x grid covers the largest frame.
+__global__ void letterbox_h_ragged_kernel(const LetterboxFrame* __restrict__ plans, const char* __restrict__ coef, const uint8_t* __restrict__ in,
+                                          uint8_t* __restrict__ tmp, int swap_rb) {
+    const LetterboxFrame& P = plans[blockIdx.y];
+    const int nw = P.nw, ksize = P.ksx;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)P.rows * nw) return;
+    const int r = (int)(i / nw), x = (int)(i - (long long)r * nw);
+    const int2 b = reinterpret_cast<const int2*>(coef + P.xb)[x];
+    const int* k = reinterpret_cast<const int*>(coef + P.kx) + (long long)x * ksize;
+    const uint8_t* src = in + P.src + ((long long)(P.y0 + r) * P.W + b.x) * 3;
+    int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+    for (int j = 0; j < b.y; ++j) {
+        const int w = k[j];
+        s0 += src[3 * j] * w;
+        s1 += src[3 * j + 1] * w;
+        s2 += src[3 * j + 2] * w;
+    }
+    uint8_t* dst = tmp + P.tmp + ((long long)r * nw + x) * 3;
+    dst[0] = clip8(swap_rb ? s2 : s0);
+    dst[1] = clip8(s1);
+    dst[2] = clip8(swap_rb ? s0 : s2);
+}
+
+__global__ void letterbox_v_ragged_kernel(const LetterboxFrame* __restrict__ plans, const char* __restrict__ coef, const uint8_t* __restrict__ tmp,
+                                          uint8_t* __restrict__ out, int S_h, int S_w) {
+    const int f = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= S_h * S_w) return;
+    const LetterboxFrame& P = plans[f];
+    const int y = i / S_w, x = i - y * S_w;
+    uint8_t* dst = out + ((long long)f * S_h * S_w + i) * 3;
+    const int nw = P.nw, yy = y - P.oy, xx = x - P.ox;
+    if (yy < 0 || yy >= P.nh || xx < 0 || xx >= nw) {
+        dst[0] = dst[1] = dst[2] = 128;
+        return;
+    }
+    const int2 b = reinterpret_cast<const int2*>(coef + P.yb)[yy];
+    const int* k = reinterpret_cast<const int*>(coef + P.ky) + (long long)yy * P.ksy;
+    const uint8_t* src = tmp + P.tmp + ((long long)b.x * nw + xx) * 3;
     int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
     for (int j = 0; j < b.y; ++j) {
         const int w = k[j];
@@ -521,6 +593,11 @@ __device__ __forceinline__ float iou_tf(float4 a, float4 b) {
 __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __grid_constant__ DecodeParams p) {
     const int f = blockIdx.x, tid = threadIdx.x;
     const int CH = 5 + p.C;
+    // the frame's row through shared memory: read from the parameter bank by a register index, it costs the decode loop a
+    // register it does not have at 32 per thread, and spills
+    __shared__ FrameGeo g;
+    if (tid == 0) g = p.geo[f];
+    __syncthreads();
     float4* cand = p.cand + (long long)f * p.NC;
     float* cscore = p.cand_score + (long long)f * p.C * p.NC;
     // ---- decode (model.py:125-187): candidates ordered layer 0, 1 (, 2), then (y, x, anchor)
@@ -537,11 +614,11 @@ __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __gr
         const float bw = __fdiv_rn(__fmul_rn(expf(t[2]), p.anchors[2 * an]), p.in_w);
         const float bh = __fdiv_rn(__fmul_rn(expf(t[3]), p.anchors[2 * an + 1]), p.in_h);
         // yolo_correct_boxes (model.py:153-176)
-        const float yc = __fmul_rn(__fsub_rn(by, p.off_y), p.scale_y), xc = __fmul_rn(__fsub_rn(bx, p.off_x), p.scale_x);
-        const float hh = __fmul_rn(bh, p.scale_y), ww = __fmul_rn(bw, p.scale_x);
+        const float yc = __fmul_rn(__fsub_rn(by, g.off_y), g.scale_y), xc = __fmul_rn(__fsub_rn(bx, g.off_x), g.scale_x);
+        const float hh = __fmul_rn(bh, g.scale_y), ww = __fmul_rn(bw, g.scale_x);
         const float hh2 = __fdiv_rn(hh, 2.0f), ww2 = __fdiv_rn(ww, 2.0f);
-        cand[i] = make_float4(__fmul_rn(__fsub_rn(yc, hh2), p.img_h), __fmul_rn(__fsub_rn(xc, ww2), p.img_w),
-                              __fmul_rn(__fadd_rn(yc, hh2), p.img_h), __fmul_rn(__fadd_rn(xc, ww2), p.img_w));
+        cand[i] = make_float4(__fmul_rn(__fsub_rn(yc, hh2), g.img_h), __fmul_rn(__fsub_rn(xc, ww2), g.img_w),
+                              __fmul_rn(__fadd_rn(yc, hh2), g.img_h), __fmul_rn(__fadd_rn(xc, ww2), g.img_w));
         const float conf = sigmoidf_(t[4]);
         for (int c = 0; c < p.C; ++c) cscore[(long long)c * p.NC + i] = __fmul_rn(conf, sigmoidf_(t[5 + c]));
     }

@@ -1172,24 +1172,21 @@ bool enlarge_box(const float* b, int H, int W, int32_t r[4]) {
     return ok;
 }
 
-// Frames (uploaded into the context's staging buffer when on the host) and the crop table -> crop_resize_kernel, one launch
-// per 65535 crops (the grid's y limit).  rects: m x (y0, y1, x0, x1) host int32, an empty one marks a zero crop; frame_of:
-// m host frame indices or NULL (all frame 0).
-int launch_crops(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const int32_t* rects,
-                 const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
-    CK(cudaSetDevice(c->device));
-    const uint8_t* d_frames = frames;
-    if (!frames_are_device) {
-        const size_t bytes = (size_t)n * H * W * 3;
-        if (c->frame_cap < bytes) {
-            if (c->d_frame) cudaFree(c->d_frame);
-            c->d_frame = nullptr; c->frame_cap = 0;
-            CK(cudaMalloc(&c->d_frame, bytes));
-            c->frame_cap = bytes;
-        }
-        CK(cudaMemcpyAsync(c->d_frame, frames, bytes, cudaMemcpyHostToDevice, c->stream));
-        d_frames = c->d_frame;
+// The context's frame staging buffer, grown to at least `bytes`
+int frame_staging(whenet_ctx* c, size_t bytes) {
+    if (c->frame_cap < bytes) {
+        if (c->d_frame) cudaFree(c->d_frame);
+        c->d_frame = nullptr; c->frame_cap = 0;
+        CK(cudaMalloc(&c->d_frame, bytes));
+        c->frame_cap = bytes;
     }
+    return 0;
+}
+
+// The crop table -> crop_resize_kernel<Frames>, one launch per 65535 crops (the grid's y limit).  rects: m x (y0, y1, x0, x1)
+// host int32, an empty one marks a zero crop; frame_of: m host frame indices or NULL (all frame 0, OneSizeFrames only).
+template <class Frames>
+int launch_crop_kernel(whenet_ctx* c, const Frames& src, const int32_t* rects, const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
     if (c->rects_cap < m) {
         if (c->d_rects) cudaFree(c->d_rects);
         if (c->d_frame_of) cudaFree(c->d_frame_of);
@@ -1203,11 +1200,46 @@ int launch_crops(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int 
     Scope sc(c, "crop_resize", (double)m * 224 * 224 * 3 * 2, 0.0);
     for (int m0 = 0; m0 < m; m0 += 65535) {
         const int mb = std::min(65535, m - m0);
-        whenet::crop_resize_kernel<<<dim3((224 * 224 + 255) / 256, mb), 256, 0, c->stream>>>(
-            d_frames, H, W, c->d_rects + m0, frame_of ? c->d_frame_of + m0 : nullptr, crops_out + (size_t)m0 * 224 * 224 * 3, swap_rb);
+        whenet::crop_resize_kernel<Frames><<<dim3((224 * 224 + 255) / 256, mb), 256, 0, c->stream>>>(
+            src, c->d_rects + m0, frame_of ? c->d_frame_of + m0 : nullptr, crops_out + (size_t)m0 * 224 * 224 * 3, swap_rb);
         CK(cudaGetLastError());
     }
     return 0;
+}
+
+// n frames of one size (uploaded into the context's staging buffer when on the host) -> launch_crop_kernel
+int launch_crops(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const int32_t* rects,
+                 const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
+    CK(cudaSetDevice(c->device));
+    const uint8_t* d_frames = frames;
+    if (!frames_are_device) {
+        const size_t bytes = (size_t)n * H * W * 3;
+        if (int rc = frame_staging(c, bytes)) return rc;
+        CK(cudaMemcpyAsync(c->d_frame, frames, bytes, cudaMemcpyHostToDevice, c->stream));
+        d_frames = c->d_frame;
+    }
+    return launch_crop_kernel(c, whenet::OneSizeFrames{d_frames, H, W}, rects, frame_of, m, swap_rb, crops_out);
+}
+
+// n frames of their own sizes: host frames are uploaded into the staging buffer at 256-byte aligned offsets, device frames are
+// read where they are
+int launch_crops_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const int32_t* rects,
+                        const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
+    CK(cudaSetDevice(c->device));
+    whenet::PerFrameSources src{};
+    std::vector<size_t> off(n);
+    size_t total = 0;
+    for (int i = 0; i < n; ++i) {
+        off[i] = total;
+        total += ((size_t)hw[2 * i] * hw[2 * i + 1] * 3 + 255) & ~(size_t)255;
+    }
+    if (!frames_are_device) {
+        if (int rc = frame_staging(c, total)) return rc;
+        for (int i = 0; i < n; ++i)
+            CK(cudaMemcpyAsync(c->d_frame + off[i], frames[i], (size_t)hw[2 * i] * hw[2 * i + 1] * 3, cudaMemcpyHostToDevice, c->stream));
+    }
+    for (int i = 0; i < n; ++i) src.f[i] = {frames_are_device ? frames[i] : c->d_frame + off[i], hw[2 * i + 1]};
+    return launch_crop_kernel(c, src, rects, frame_of, m, swap_rb, crops_out);
 }
 
 }  // namespace
@@ -1533,6 +1565,29 @@ int whenet_crop_boxes_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int
     }
     if (rects_out) memcpy(rects_out, rects.data(), rects.size() * sizeof(int32_t));
     return launch_crops(c, frames, n, H, W, frames_are_device, rects.data(), frame_of, m, swap_rb, crops_out);
+}
+
+int whenet_crop_boxes_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const float* boxes,
+                                const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+    // the context is checked last so that every other argument can be validated without a GPU
+    if (!frames || !hw || !boxes || !frame_of || !crops_out) return fail(WHENET_EINVAL, "null frames, hw, boxes, frame_of or crops_out");
+    if (n < 1 || n > whenet::kMaxCropFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxCropFrames);
+    for (int i = 0; i < n; ++i) {
+        if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
+        if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
+            return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+    }
+    if (m < 1) return fail(WHENET_EINVAL, "m=%d boxes", m);
+    for (int i = 0; i < m; ++i)
+        if (frame_of[i] < 0 || frame_of[i] >= n) return fail(WHENET_EINVAL, "box %d: frame_of=%d outside [0, %d)", i, frame_of[i], n);
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    std::vector<int32_t> rects((size_t)m * 4);
+    for (int i = 0; i < m; ++i) {
+        const bool ok = enlarge_box(boxes + 4 * i, hw[2 * frame_of[i]], hw[2 * frame_of[i] + 1], &rects[(size_t)4 * i]);
+        if (valid_out) valid_out[i] = ok;
+    }
+    if (rects_out) memcpy(rects_out, rects.data(), rects.size() * sizeof(int32_t));
+    return launch_crops_ragged(c, frames, hw, n, frames_are_device, rects.data(), frame_of, m, swap_rb, crops_out);
 }
 
 int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out) {

@@ -9,6 +9,7 @@
 #include <map>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include "../../include/whenet_b200.h"
@@ -59,9 +60,15 @@ struct LayerDev { int Hi, Wi, Ho, Wo, N; Y::IgemmPlan plan; Y::Igemm32Plan plan3
 
 struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
-    void* coef = nullptr;           // letterbox tables (xb, kx, yb, ky) in one allocation
+    void* coef = nullptr;           // letterbox tables (xb, kx, yb, ky; several frames: every frame's, then their LetterboxFrames) in one allocation
     uint8_t* tmp = nullptr;         // horizontal-pass output
 };
+
+// a graph of frames of several sizes: (H0, W0, H1, W1, ...) and swap_rb
+using RaggedKey = std::pair<std::vector<int>, int>;
+constexpr size_t kMaxGraphs = 16;   // captured graphs kept per cache
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // Pillow ImagingResample (libImaging/Resample.c) coefficient tables for BICUBIC: support 2 scaled by the downscale factor,
 // weights normalised in double and quantised to 22 bits (normalize_coeffs_8bpc).
@@ -127,6 +134,7 @@ struct whenet_det {
     float4* d_cand = nullptr; float* d_cand_score = nullptr;
     float* d_boxes = nullptr; float* d_scores = nullptr; int* d_classes = nullptr; int* d_count = nullptr;
     std::map<std::tuple<int, int, int>, GraphEntry> graphs;
+    std::map<RaggedKey, GraphEntry> ragged_graphs;      // whenet_det_detect_ragged_u8's
     int last_n = 0;
 };
 
@@ -141,13 +149,22 @@ void free_layers(whenet_det* d) {
     for (auto& l : d->L) { cudaFree(l.out); cudaFree(l.pooled); l.out = l.pooled = nullptr; }
 }
 
+void free_entry(GraphEntry& e) {
+    if (e.exec) cudaGraphExecDestroy(e.exec);
+    cudaFree(e.coef);
+    cudaFree(e.tmp);
+}
+
+template <class Map>
+void free_graph_map(Map& m) {
+    for (auto& kv : m) free_entry(kv.second);
+    m.clear();
+}
+
+// both caches (weights reloaded, frame buffer reallocated, detector destroyed)
 void free_graphs(whenet_det* d) {
-    for (auto& kv : d->graphs) {
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-        cudaFree(kv.second.coef);
-        cudaFree(kv.second.tmp);
-    }
-    d->graphs.clear();
+    free_graph_map(d->graphs);
+    free_graph_map(d->ragged_graphs);
 }
 
 const __nv_bfloat16* bf(const whenet_det* d, size_t off) { return reinterpret_cast<const __nv_bfloat16*>((const char*)d->warena + off); }
@@ -206,7 +223,9 @@ int enqueue_conv(whenet_det* d, cudaStream_t s, int i, int n) {
     return 0;
 }
 
-int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
+// The letterbox of one H x W frame: geometry, and Pillow's tables appended to `blob`, each 256-byte aligned (int2 loads), at the
+// offsets f records (src and tmp are left to the caller)
+int frame_plan(const whenet_det* d, int H, int W, std::vector<char>& blob, Y::LetterboxFrame* f) {
     // letterbox geometry (reference utils.py:25-33): scale in float64, int() truncation, paste at the floor-halved offsets
     const double scale = std::min((double)d->in_w / W, (double)d->in_h / H);
     const int nw = (int)(W * scale), nh = (int)(H * scale);
@@ -215,21 +234,24 @@ int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
     const int ksx = precompute_coeffs(W, nw, xb, kx), ksy = precompute_coeffs(H, nh, yb, ky);
     const int y0 = yb[0], rows = yb[2 * (nh - 1)] + yb[2 * nh - 1] - y0;      // Pillow's ybox_first / ybox_last
     for (int y = 0; y < nh; ++y) yb[2 * y] -= y0;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };      // each table 256-byte aligned (int2 loads)
-    const size_t b_xb = al(xb.size() * 4), b_kx = al(kx.size() * 4), b_yb = al(yb.size() * 4), b_ky = al(ky.size() * 4);
-    CKD(cudaMalloc(&e->coef, b_xb + b_kx + b_yb + b_ky));
-    char* base = (char*)e->coef;
-    CKD(cudaMemcpy(base, xb.data(), xb.size() * 4, cudaMemcpyHostToDevice));
-    CKD(cudaMemcpy(base + b_xb, kx.data(), kx.size() * 4, cudaMemcpyHostToDevice));
-    CKD(cudaMemcpy(base + b_xb + b_kx, yb.data(), yb.size() * 4, cudaMemcpyHostToDevice));
-    CKD(cudaMemcpy(base + b_xb + b_kx + b_yb, ky.data(), ky.size() * 4, cudaMemcpyHostToDevice));
-    CKD(cudaMalloc(&e->tmp, (size_t)n * rows * nw * 3));
-    Y::LetterboxPlan lp{H, W, nw, nh, (d->in_w - nw) / 2, (d->in_h - nh) / 2, y0, rows, ksx, ksy,
-                        (const int2*)base, (const int*)(base + b_xb), (const int2*)(base + b_xb + b_kx), (const int*)(base + b_xb + b_kx + b_yb)};
-    // the whole body as one graph, captured on the context's private stream
+    int off[4];
+    const std::vector<int>* tabs[4] = {&xb, &kx, &yb, &ky};
+    for (int t = 0; t < 4; ++t) {
+        off[t] = (int)blob.size();
+        blob.resize(align256(blob.size() + tabs[t]->size() * 4), 0);
+        std::memcpy(blob.data() + off[t], tabs[t]->data(), tabs[t]->size() * 4);
+    }
+    *f = Y::LetterboxFrame{0, 0, H, W, nw, nh, (d->in_w - nw) / 2, (d->in_h - nh) / 2, y0, rows, ksx, ksy, off[0], off[1], off[2], off[3]};
+    return 0;
+}
+
+// The letterbox (enqueued by `letterbox` on the stream it is given), the first conv and the body for n frames, as one graph
+// captured on the context's private stream
+template <class Letterbox>
+int capture_forward(whenet_det* d, int n, Letterbox&& letterbox, GraphEntry* e) {
     cudaStream_t s = d->cap_stream;
     CKD(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-    int rc = Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb);
+    int rc = letterbox(s);
     if (!rc && is_fp32(d))
         rc = Y::launch_conv0_32(s, d->d_canvas, bf(d, d->w_off[0]), bf_lo(d, d->w_off[0]), d->barena + d->b_off[0], (float*)d->L[0].out, n,
                                 d->in_h, d->in_w, d->table[0].cout);
@@ -248,24 +270,70 @@ int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
     return 0;
 }
 
+int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
+    std::vector<char> blob;
+    Y::LetterboxFrame f;
+    if (int rc = frame_plan(d, H, W, blob, &f)) return rc;
+    CKD(cudaMalloc(&e->coef, blob.size()));
+    char* base = (char*)e->coef;
+    CKD(cudaMemcpy(base, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+    CKD(cudaMalloc(&e->tmp, (size_t)n * f.rows * f.nw * 3));
+    Y::LetterboxPlan lp{H, W, f.nw, f.nh, f.ox, f.oy, f.y0, f.rows, f.ksx, f.ksy,
+                        (const int2*)(base + f.xb), (const int*)(base + f.kx), (const int2*)(base + f.yb), (const int*)(base + f.ky)};
+    return capture_forward(d, n, [&](cudaStream_t s) { return Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb); },
+                           e);
+}
+
+// frame i at byte offset off[i] of d_frames, hw[2i] x hw[2i+1]
+int make_ragged_entry(whenet_det* d, int n, const int32_t* hw, const std::vector<size_t>& off, int swap_rb, GraphEntry* e) {
+    std::vector<char> blob;
+    std::vector<Y::LetterboxFrame> plans(n);
+    size_t tmp_bytes = 0;
+    long long max_hx = 0;
+    for (int i = 0; i < n; ++i) {
+        Y::LetterboxFrame& f = plans[i];
+        if (int rc = frame_plan(d, hw[2 * i], hw[2 * i + 1], blob, &f)) return rc;
+        f.src = (long long)off[i];
+        f.tmp = (long long)tmp_bytes;
+        tmp_bytes = align256(tmp_bytes + (size_t)f.rows * f.nw * 3);
+        max_hx = std::max(max_hx, (long long)f.rows * f.nw);
+    }
+    const size_t plans_at = blob.size();
+    blob.resize(plans_at + plans.size() * sizeof(Y::LetterboxFrame));
+    std::memcpy(blob.data() + plans_at, plans.data(), plans.size() * sizeof(Y::LetterboxFrame));
+    CKD(cudaMalloc(&e->coef, blob.size()));
+    CKD(cudaMemcpy(e->coef, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+    CKD(cudaMalloc(&e->tmp, tmp_bytes));
+    const char* coef = (const char*)e->coef;
+    const auto* d_plans = (const Y::LetterboxFrame*)(coef + plans_at);
+    return capture_forward(d, n, [&](cudaStream_t s) {
+        return Y::launch_letterbox_ragged(s, d_plans, coef, d->d_frames, e->tmp, d->d_canvas, n, max_hx, d->in_h, d->in_w, swap_rb);
+    }, e);
+}
+
 int check_frames(const whenet_det* d, int n, int H, int W) {
     if (n < 1 || n > d->max_frames) return fail(WHENET_EINVAL, "n=%d outside [1, max_frames=%d]", n, d->max_frames);
     if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
     return 0;
 }
 
-// DecodeParams of one call: yolo_correct_boxes' float32 arithmetic (model.py:157-161) on the host
-Y::DecodeParams decode_params(const whenet_det* d, int img_h, int img_w, float score, float iou, int max_boxes) {
+// DecodeParams of one call of n frames, frame i img_hw[2i] x img_hw[2i+1] (img_hw NULL: every frame img_h x img_w):
+// yolo_correct_boxes' float32 arithmetic (model.py:157-161) on the host, one geo row per frame
+Y::DecodeParams decode_params(const whenet_det* d, int n, const int32_t* img_hw, int img_h, int img_w, float score, float iou, int max_boxes) {
     Y::DecodeParams p{};
     p.cand = d->d_cand; p.cand_score = d->d_cand_score;
     p.out_boxes = d->d_boxes; p.out_scores = d->d_scores; p.out_classes = d->d_classes; p.out_count = d->d_count;
     std::memcpy(p.anchors, d->anchors, sizeof(p.anchors));
     p.gh0 = d->in_h / 32; p.gw0 = d->in_w / 32; p.C = d->num_classes; p.NC = ncand(d); p.max_boxes = max_boxes;
-    p.in_h = (float)d->in_h; p.in_w = (float)d->in_w; p.img_h = (float)img_h; p.img_w = (float)img_w;
-    const float m = std::min(p.in_h / p.img_h, p.in_w / p.img_w);
-    const float nh = std::nearbyint(p.img_h * m), nw = std::nearbyint(p.img_w * m);       // K.round: half to even
-    p.off_y = (p.in_h - nh) / 2.0f / p.in_h; p.off_x = (p.in_w - nw) / 2.0f / p.in_w;
-    p.scale_y = p.in_h / nh; p.scale_x = p.in_w / nw;
+    p.in_h = (float)d->in_h; p.in_w = (float)d->in_w;
+    for (int i = 0; i < n; ++i) {
+        Y::FrameGeo& g = p.geo[i];
+        g.img_h = (float)(img_hw ? img_hw[2 * i] : img_h); g.img_w = (float)(img_hw ? img_hw[2 * i + 1] : img_w);
+        const float m = std::min(p.in_h / g.img_h, p.in_w / g.img_w);
+        const float nh = std::nearbyint(g.img_h * m), nw = std::nearbyint(g.img_w * m);       // K.round: half to even
+        g.off_y = (p.in_h - nh) / 2.0f / p.in_h; g.off_x = (p.in_w - nw) / 2.0f / p.in_w;
+        g.scale_y = p.in_h / nh; g.scale_x = p.in_w / nw;
+    }
     p.score = score; p.iou = iou;
     const int heads = num_heads(d);
     for (int l = 0; l < heads; ++l) p.head[l] = (const float*)d->L[d->table.size() - heads + l].out;
@@ -538,15 +606,62 @@ int whenet_det_detect_u8(whenet_det* d, const uint8_t* frames, int n, int H, int
     const auto key = std::make_tuple(n, H, swap_rb ? W : -W);      // graphs keyed on (n, H, W) and the channel order
     auto it = d->graphs.find(key);
     if (it == d->graphs.end()) {
-        if (d->graphs.size() >= 16) { CKD(cudaStreamSynchronize(d->stream)); free_graphs(d); }
+        if (d->graphs.size() >= kMaxGraphs) { CKD(cudaStreamSynchronize(d->stream)); free_graph_map(d->graphs); }
         GraphEntry e{};
         int rc = make_entry(d, n, H, W, swap_rb ? 1 : 0, &e);
-        if (rc) { if (e.exec) cudaGraphExecDestroy(e.exec); cudaFree(e.coef); cudaFree(e.tmp); return rc; }
+        if (rc) { free_entry(e); return rc; }
         it = d->graphs.emplace(key, e).first;
     }
     CKD(cudaGraphLaunch(it->second.exec, d->stream));
     d->last_n = n;
-    return run_decode(d, decode_params(d, H, W, score, iou, max_boxes), n, boxes, scores, classes, counts);
+    return run_decode(d, decode_params(d, n, nullptr, H, W, score, iou, max_boxes), n, boxes, scores, classes, counts);
+}
+
+int whenet_det_detect_ragged_u8(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int swap_rb,
+                                float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    // the detector is checked after every argument that can be validated without a GPU
+    if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
+    if (n < 1 || n > Y::kMaxFrames) return fail(WHENET_EINVAL, "n=%d outside [1, %d]", n, Y::kMaxFrames);
+    for (int i = 0; i < n; ++i) {
+        if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
+        if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
+            return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+    }
+    if (!boxes || !scores || !classes || !counts) return fail(WHENET_EINVAL, "null output pointer");
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    if (n > d->max_frames) return fail(WHENET_EINVAL, "n=%d outside [1, max_frames=%d]", n, d->max_frames);
+    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+    CKD(cudaSetDevice(d->device));
+    // frames -> the context's input buffer at 256-byte aligned offsets that depend on the sizes only (the captured graph reads
+    // fixed addresses)
+    std::vector<size_t> off(n);
+    size_t bytes = 0;
+    for (int i = 0; i < n; ++i) {
+        off[i] = bytes;
+        bytes += align256((size_t)hw[2 * i] * hw[2 * i + 1] * 3);
+    }
+    if (d->frames_cap < bytes) {
+        CKD(cudaStreamSynchronize(d->stream));
+        cudaFree(d->d_frames);
+        d->d_frames = nullptr; d->frames_cap = 0;
+        free_graphs(d);                         // they captured the old buffer
+        CKD(cudaMalloc(&d->d_frames, bytes));
+        d->frames_cap = bytes;
+    }
+    const cudaMemcpyKind kind = frames_are_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    for (int i = 0; i < n; ++i) CKD(cudaMemcpyAsync(d->d_frames + off[i], frames[i], (size_t)hw[2 * i] * hw[2 * i + 1] * 3, kind, d->stream));
+    RaggedKey key(std::vector<int>(hw, hw + 2 * n), swap_rb ? 1 : 0);
+    auto it = d->ragged_graphs.find(key);
+    if (it == d->ragged_graphs.end()) {
+        if (d->ragged_graphs.size() >= kMaxGraphs) { CKD(cudaStreamSynchronize(d->stream)); free_graph_map(d->ragged_graphs); }
+        GraphEntry e{};
+        int rc = make_ragged_entry(d, n, hw, off, swap_rb ? 1 : 0, &e);
+        if (rc) { free_entry(e); return rc; }
+        it = d->ragged_graphs.emplace(std::move(key), e).first;
+    }
+    CKD(cudaGraphLaunch(it->second.exec, d->stream));
+    d->last_n = n;
+    return run_decode(d, decode_params(d, n, hw, 0, 0, score, iou, max_boxes), n, boxes, scores, classes, counts);
 }
 
 int whenet_det_synchronize(whenet_det* d) {
@@ -692,7 +807,7 @@ int whenet_det_debug_decode(whenet_det* d, const float* head0, const float* head
     if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
     CKD(cudaSetDevice(d->device));
     const float* hs[3] = {head0, head1, head2};
-    Y::DecodeParams p = decode_params(d, img_h, img_w, score, iou, max_boxes);
+    Y::DecodeParams p = decode_params(d, n, nullptr, img_h, img_w, score, iou, max_boxes);
     const int nh = num_heads(d);
     for (int l = 0; l < nh; ++l) {
         const LayerDev& L = d->L[d->table.size() - nh + l];

@@ -2,11 +2,14 @@
 head, demo_video.py:13-23 and 54-58) for the heads of many frames at once."""
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 
 from . import crops as _crops
 from ._lib import WhenetError, check
 from .whenet import _is_device, _ptr
+from .yolo import _frame_list, _frame_table
 
 
 def detect_and_estimate(yolo, whenet, frame_bgr):
@@ -31,13 +34,29 @@ def detect_and_estimate_frames(yolo, whenet, frames_bgr):
     next chunk on its own.  One synchronisation at the end.
 
     A head whose enlarged slice is empty or leaves the frame (where the reference's cv2.resize raises and ends the video
-    loop) gets NaN angles; its box and score are returned as the detector gave them."""
+    loop) gets NaN angles; its box and score are returned as the detector gave them.
+
+    ``frames_bgr`` may also be a list or tuple of (H_i, W_i, 3) uint8 BGR frames of any sizes (several cameras), all numpy
+    arrays or all contiguous CUDA tensors on ``whenet.device``; frames of one size run as the batch above.  Frames of several
+    sizes take the same path through the per-frame entries (``whenet_det_detect_ragged_u8``, ``whenet_crop_boxes_ragged_u8``),
+    each frame's result bit-identical to ``detect_and_estimate`` on that frame alone.  An empty list gives []."""
     return _run(yolo, whenet, frames_bgr, strict=False)
 
 
 def _checked_frames(yolo, whenet, frames):
     if yolo.device != whenet.device:
         raise ValueError("the detector runs on device %d and WHENet on device %d" % (yolo.device, whenet.device))
+    if isinstance(frames, (list, tuple)):
+        frames, dev = _frame_list(frames, whenet.device)
+        if len({tuple(f.shape) for f in frames}) > 1:
+            return frames
+        if not frames:
+            return np.zeros((0, 1, 1, 3), np.uint8)
+        if not dev:
+            return np.stack(frames)
+        import torch
+        with torch.cuda.device(whenet.device):
+            return torch.stack(frames)
     if _is_device(frames):
         if str(frames.dtype) != "torch.uint8" or not frames.is_contiguous():
             raise ValueError("device frames must be a contiguous uint8 CUDA tensor")
@@ -66,12 +85,16 @@ def _raise_first_invalid(L, boxes, H, W):
 
 def _run(yolo, whenet, frames, strict):
     frames = _checked_frames(yolo, whenet, frames)
-    n, H, W = (int(v) for v in frames.shape[:3])
+    ragged = isinstance(frames, list)       # frames of several sizes; otherwise one (n, H, W, 3) array or tensor
+    if ragged:
+        n = len(frames)
+    else:
+        n, H, W = (int(v) for v in frames.shape[:3])
     if n == 0:
         return []
     import torch
     L = whenet._L
-    dev = _is_device(frames)
+    dev = _is_device(frames[0] if ragged else frames)
     step = yolo.max_frames
     n_chunks = -(-n // step)
     results = []            # per chunk: (detections, device angles or None, validity or None)
@@ -79,10 +102,25 @@ def _run(yolo, whenet, frames, strict):
     stage = [None, None]    # host frames: chunk k goes to stage[k % 2]
     crop_buf = None
 
+    def stage_ragged(k, part):
+        """Host frames of several sizes -> views of one device buffer, each frame at a 256-byte aligned offset."""
+        offs = np.cumsum([0] + [-(-f.size // 256) * 256 for f in part])
+        buf = stage[k % 2]
+        if buf is None or buf.numel() < offs[-1]:
+            cap = max(sum(-(-f.size // 256) * 256 for f in frames[j:j + step]) for j in range(0, n, step))
+            buf = stage[k % 2] = torch.empty((cap,), dtype=torch.uint8, device="cuda")
+        views = [buf[int(o):int(o) + f.size].view(f.shape) for f, o in zip(part, offs)]
+        for v, f in zip(views, part):
+            v.copy_(torch.from_numpy(f))
+        torch.cuda.current_stream().synchronize()       # the detector reads them on its own stream
+        return views
+
     def chunk(k):
         lo, hi = k * step, min(n, (k + 1) * step)
         if dev:
             return frames[lo:hi]
+        if ragged:
+            return stage_ragged(k, frames[lo:hi])
         buf = stage[k % 2]
         if buf is None:
             buf = stage[k % 2] = torch.empty((min(step, n), H, W, 3), dtype=torch.uint8, device="cuda")
@@ -96,7 +134,7 @@ def _run(yolo, whenet, frames, strict):
         try:
             cur = chunk(0)
             for k in range(n_chunks):
-                nb = int(cur.shape[0])
+                nb = len(cur)
                 dets = yolo.detect_frames(cur)          # synchronous, on the detector's stream
                 if k + 1 < n_chunks:
                     if not dev:
@@ -114,13 +152,19 @@ def _run(yolo, whenet, frames, strict):
                     valid = np.empty(m, np.int32)
                     d_ang = torch.empty((m, 3), dtype=torch.float32, device="cuda")
                     keep.append(d_ang)
+                    if ragged:
+                        ptrs, hw = _frame_table(cur)
                     for s in range(0, m, whenet.max_batch):
                         mb = min(whenet.max_batch, m - s)
                         if crop_buf is None or crop_buf.shape[0] < mb:
                             crop_buf = torch.empty((mb, 224, 224, 3), dtype=torch.uint8, device="cuda")
                             keep.append(crop_buf)
-                        check(L.whenet_crop_boxes_u8(whenet._h, _ptr(cur), nb, H, W, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, 1,
-                                                     _ptr(crop_buf), None, _ptr(valid[s:])))
+                        if ragged:
+                            check(L.whenet_crop_boxes_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), nb, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]),
+                                                                mb, 1, _ptr(crop_buf), None, _ptr(valid[s:])))
+                        else:
+                            check(L.whenet_crop_boxes_u8(whenet._h, _ptr(cur), nb, H, W, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, 1,
+                                                         _ptr(crop_buf), None, _ptr(valid[s:])))
                         check(L.whenet_forward_u8(whenet._h, _ptr(crop_buf), mb, 1, _ptr(d_ang[s:s + mb]), None, 1))
                     results.append((dets, d_ang, valid))
                 if k + 1 < n_chunks:

@@ -45,6 +45,39 @@ def _tensor_list(layers):
     return t, (arrs, names)
 
 
+def _frame_list(frames, device: int):
+    """A list or tuple of (H_i, W_i, 3) uint8 frames, all numpy arrays or all contiguous CUDA tensors on ``device`` ->
+    (list of C-contiguous frames, whether they are on the device).  Raises ValueError otherwise."""
+    frames = list(frames)
+    dev = [_is_device(f) for f in frames]
+    if any(dev) and not all(dev):
+        raise ValueError("a frame list must be all host (numpy) or all device (CUDA tensor) frames, not a mix")
+    out = []
+    for i, f in enumerate(frames):
+        if dev[i]:
+            if str(f.dtype) != "torch.uint8" or not f.is_contiguous():
+                raise ValueError("frame %d: device frames must be contiguous uint8 CUDA tensors" % i)
+            if f.device.index != device:
+                raise ValueError("frame %d is on cuda:%s, not on cuda:%d" % (i, f.device.index, device))
+        else:
+            f = np.asarray(f)
+            if f.dtype != np.uint8:
+                raise ValueError("frame %d: frames must be uint8, not %s" % (i, f.dtype))
+            f = np.ascontiguousarray(f)
+        if len(f.shape) != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
+            raise ValueError("frame %d: frames must be (H, W, 3) uint8, not %s" % (i, tuple(f.shape)))
+        out.append(f)
+    return out, bool(dev) and dev[0]
+
+
+def _frame_table(frames):
+    """Frames of a list -> the ragged entries' arguments: a ctypes array of their addresses and their (H, W) as int32 pairs
+    (keep both alive over the call)."""
+    ptrs = (C.c_void_p * len(frames))(*(_ptr(f).value for f in frames))
+    hw = np.array([f.shape[:2] for f in frames], np.int32).reshape(-1)
+    return ptrs, hw
+
+
 class YOLO:
     def __init__(self, model_path=None, anchors_path=None, classes_path=None, score=0.3, iou=0.45, model_image_size=(416, 416),
                  gpu_num=1, *, device: Optional[int] = None, max_frames: int = 8, seed: int = 0, precision: str = "bf16", **kwargs):
@@ -103,8 +136,41 @@ class YOLO:
         return self._detect(a[None], swap_rb=False)[0]
 
     def detect_frames(self, frames_bgr) -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
-        """A batch of BGR frames of one size (n, H, W, 3) uint8, numpy or a CUDA tensor -> one detect() tuple per frame."""
-        return self._detect(frames_bgr, swap_rb=True)
+        """A batch of BGR frames of one size (n, H, W, 3) uint8, numpy or a CUDA tensor -> one detect() tuple per frame.
+
+        ``frames_bgr`` may also be a list or tuple of (H_i, W_i, 3) uint8 BGR frames of any sizes, all numpy arrays or all
+        contiguous CUDA tensors on the detector's device.  Frames of one size are stacked and run as the batch above; frames of
+        several sizes run ``max_frames`` at a time through ``whenet_det_detect_ragged_u8``, each letterboxed on its own, and
+        each frame's tuple is what ``detect_frames`` gives that frame alone."""
+        if not isinstance(frames_bgr, (list, tuple)):
+            return self._detect(frames_bgr, swap_rb=True)
+        frames, dev = _frame_list(frames_bgr, self.device)
+        if not frames:
+            return []
+        if len({tuple(f.shape) for f in frames}) == 1:
+            if dev:
+                import torch
+                with torch.cuda.device(self.device):
+                    stacked = torch.stack(frames)
+                    torch.cuda.current_stream().synchronize()   # the detector copies it on its own stream
+                return self._detect(stacked, swap_rb=True)
+            return self._detect(np.stack(frames), swap_rb=True)
+        out = []
+        for off in range(0, len(frames), self.max_frames):
+            out += self._detect_ragged(frames[off:off + self.max_frames], dev)
+        return out
+
+    def _detect_ragged(self, frames, dev: bool, max_boxes: int = 20):
+        nb = len(frames)
+        ptrs, hw = _frame_table(frames)
+        slots = self.num_classes * max_boxes
+        boxes = np.empty((nb, slots, 4), np.float32)
+        scores = np.empty((nb, slots), np.float32)
+        classes = np.empty((nb, slots), np.int32)
+        counts = np.empty((nb,), np.int32)
+        check(self._L.whenet_det_detect_ragged_u8(self._h, C.addressof(ptrs), _ptr(hw), nb, int(dev), 1, self.score, self.iou, max_boxes,
+                                                  _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
+        return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(nb)]
 
     def _detect(self, frames, swap_rb: bool, max_boxes: int = 20):
         dev = _is_device(frames)

@@ -132,6 +132,16 @@ int whenet_crop_boxes_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, i
                          const float* boxes, const int32_t* frame_of, int m, int swap_rb,
                          uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
 
+/* whenet_crop_boxes_u8 for n (1..64) frames that each have their own size: `frames` is a host array of n frame pointers,
+ * frame i is hw[2i] x hw[2i+1] x 3 uint8 (each side 1..16384), all in host memory or all in device memory on the context's
+ * device (frames_are_device).  Each box's margin arithmetic uses its own frame's H and W; the outputs are laid out as
+ * whenet_crop_boxes_u8's, and each crop is the bytes whenet_crop_boxes_u8 gives that box on its frame alone.  Host frames are
+ * uploaded once per call into the context's staging buffer; device frames are read in place.  Every argument but the
+ * context is checked before anything touches a device. */
+int whenet_crop_boxes_ragged_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                const float* boxes, const int32_t* frame_of, int m, int swap_rb,
+                                uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+
 /* Block until everything queued by this context has finished. */
 int whenet_synchronize(whenet_ctx* ctx);
 
@@ -253,6 +263,18 @@ int whenet_det_set_stream(whenet_det* det, void* cuda_stream);
  * captured on the first call for each (n, H, W) and replayed after.  Synchronous. */
 int whenet_det_detect_u8(whenet_det* det, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb,
                          float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
+
+/* whenet_det_detect_u8 for n (1..max_frames) frames that each have their own size, in one forward: `frames` is a host array
+ * of n frame pointers, frame i is hw[2i] x hw[2i+1] x 3 uint8 (each side 1..16384), all in host memory or all in device
+ * memory on the detector's device (frames_are_device).  Each frame is letterboxed with its own tables onto the model-size
+ * canvas; the body, decode and NMS then run on all n canvases at once, and frame i's outputs (laid out as
+ * whenet_det_detect_u8's) are the bits whenet_det_detect_u8 gives it alone.  The frames are copied into the detector's
+ * frame buffer; the forward is a CUDA graph captured on the first call for each ordered list of sizes and swap_rb (at most
+ * 16 such lists are kept, apart from the one-size graphs) and replayed after.  Every argument but the detector is checked
+ * before anything touches a device.  Synchronous. */
+int whenet_det_detect_ragged_u8(whenet_det* det, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                int swap_rb, float score, float iou, int max_boxes,
+                                float* boxes, float* scores, int32_t* classes, int32_t* counts);
 
 /* Block until everything queued by this detector has finished. */
 int whenet_det_synchronize(whenet_det* det);
