@@ -17,7 +17,11 @@ EXPORTS = [
     "whenet_det_create", "whenet_det_load_weights", "whenet_det_num_classes", "whenet_det_set_stream", "whenet_det_detect_u8",
     "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_maxpool",
     "whenet_det_debug_decode", "whenet_det_create_ex", "whenet_det_precision", "whenet_det_detect_ragged_u8", "whenet_crop_boxes_ragged_u8",
+    "whenet_det_detect_yuv_u8", "whenet_det_detect_ragged_yuv_u8", "whenet_crop_boxes_yuv_u8", "whenet_crop_boxes_ragged_yuv_u8",
 ]
+
+# pixel_format -> the ABI's yuv_layout (WHENET_YUV_NV12 / WHENET_YUV_I420); "bgr" is packed 8-bit BGR, the *_u8 entries
+YUV_LAYOUTS = {"nv12": 1, "i420": 2}
 
 
 class WhenetError(RuntimeError):
@@ -72,6 +76,8 @@ def load():
     L.whenet_crop_resize_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, C.c_int, C.c_int, P]
     L.whenet_crop_boxes_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P]
     L.whenet_crop_boxes_ragged_u8.argtypes = [P, P, P, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P]
+    L.whenet_crop_boxes_yuv_u8.argtypes = L.whenet_crop_boxes_u8.argtypes
+    L.whenet_crop_boxes_ragged_yuv_u8.argtypes = L.whenet_crop_boxes_ragged_u8.argtypes
     L.whenet_debug_enlarge_boxes.argtypes = [P, C.c_int, C.c_int, C.c_int, P, P]
     L.whenet_synchronize.argtypes = [P]
     L.whenet_host_alloc.argtypes = [C.c_size_t]
@@ -102,6 +108,8 @@ def load():
     L.whenet_det_set_stream.argtypes = [P, P]
     L.whenet_det_detect_u8.argtypes = [P, P, I, I, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
     L.whenet_det_detect_ragged_u8.argtypes = [P, P, P, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
+    L.whenet_det_detect_yuv_u8.argtypes = L.whenet_det_detect_u8.argtypes
+    L.whenet_det_detect_ragged_yuv_u8.argtypes = L.whenet_det_detect_ragged_u8.argtypes
     L.whenet_det_synchronize.argtypes = [P]
     L.whenet_det_destroy.argtypes = [P]
     L.whenet_det_destroy.restype = None

@@ -4,17 +4,34 @@
 namespace whenet {
 namespace yolo {
 
-int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb) {
+int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb,
+                     int yuv_layout) {
     const long long hx = (long long)lp.rows * lp.nw;
-    letterbox_h_kernel<<<dim3((unsigned)((hx + 255) / 256), n), 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx, swap_rb);
+    const dim3 grid_h((unsigned)((hx + 255) / 256), n);
+    switch (yuv_layout) {
+        case 0: letterbox_h_kernel<<<grid_h, 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx, swap_rb); break;
+        case kYuvNV12:
+            letterbox_h_yuv_kernel<kYuvNV12><<<grid_h, 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx);
+            break;
+        case kYuvI420:
+            letterbox_h_yuv_kernel<kYuvI420><<<grid_h, 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx);
+            break;
+        default: return (int)cudaErrorInvalidValue;
+    }
     letterbox_v_kernel<<<dim3((unsigned)((S_h * S_w + 255) / 256), n), 256, 0, s>>>(tmp, out, lp.nw, lp.nh, lp.rows, S_h, S_w, lp.ox, lp.oy,
                                                                                    lp.yb, lp.ky, lp.ksy);
     return (int)cudaGetLastError();
 }
 
 int launch_letterbox_ragged(cudaStream_t s, const LetterboxFrame* plans, const char* coef, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n,
-                            long long max_hx, int S_h, int S_w, int swap_rb) {
-    letterbox_h_ragged_kernel<<<dim3((unsigned)((max_hx + 255) / 256), n), 256, 0, s>>>(plans, coef, in, tmp, swap_rb);
+                            long long max_hx, int S_h, int S_w, int swap_rb, int yuv_layout) {
+    const dim3 grid_h((unsigned)((max_hx + 255) / 256), n);
+    switch (yuv_layout) {
+        case 0: letterbox_h_ragged_kernel<<<grid_h, 256, 0, s>>>(plans, coef, in, tmp, swap_rb); break;
+        case kYuvNV12: letterbox_h_ragged_yuv_kernel<kYuvNV12><<<grid_h, 256, 0, s>>>(plans, coef, in, tmp); break;
+        case kYuvI420: letterbox_h_ragged_yuv_kernel<kYuvI420><<<grid_h, 256, 0, s>>>(plans, coef, in, tmp); break;
+        default: return (int)cudaErrorInvalidValue;
+    }
     letterbox_v_ragged_kernel<<<dim3((unsigned)((S_h * S_w + 255) / 256), n), 256, 0, s>>>(plans, coef, tmp, out, S_h, S_w);
     return (int)cudaGetLastError();
 }

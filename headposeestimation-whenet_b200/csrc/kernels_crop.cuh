@@ -6,12 +6,14 @@
 // ((b0*(r0>>4))>>16) + ((b1*(r1>>4))>>16) + 2 >> 2 vertical pass, 2x2 box for exact 2x down-scaling.
 // All heads of one frame, of n frames of one size or of n frames of their own sizes come out as ONE uint8 NHWC batch that feeds the
 // stem kernel directly - the reference crops, resizes and runs the network one head at a time
-// (demo_video.py:13-23, 57-58).
+// (demo_video.py:13-23, 57-58).  crop_resize_yuv_kernel does the same on NV12 / I420 frames (yuv.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <type_traits>
+
+#include "yuv.cuh"
 
 namespace whenet {
 
@@ -46,9 +48,10 @@ struct OneSizeFrames {
     const uint8_t* frames;
     int H, W;
 };
-// n <= kMaxCropFrames frames of their own sizes, each H x W x 3 at its own base (the host checked every rect against its H)
+// n <= kMaxCropFrames frames of their own sizes, each H x W x 3 at its own base (the host checked every rect against its H).
+// H locates a YUV frame's chroma plane(s); the BGR kernel does not read it.
 struct PerFrameSources {
-    struct Frame { const uint8_t* base; int W; } f[kMaxCropFrames];
+    struct Frame { const uint8_t* base; int W, H; } f[kMaxCropFrames];
 };
 
 // grid = (ceil(224*224/256), M).  src: the frames; rects[m] = (y0, y1, x0, x1) slice bounds inside frame frame_of[m]
@@ -97,6 +100,61 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
     }
     if (swap_rb) { dst[0] = (uint8_t)v[2]; dst[1] = (uint8_t)v[1]; dst[2] = (uint8_t)v[0]; }
     else { dst[0] = (uint8_t)v[0]; dst[1] = (uint8_t)v[1]; dst[2] = (uint8_t)v[2]; }
+}
+
+// crop_resize_kernel on YUV 4:2:0 frames in layout L (yuv.cuh; OneSizeFrames: H * W * 3/2 bytes apart): each source pixel the
+// resize reads is converted to B, G, R first, and the crop is written in RGB order, so it is the crop crop_resize_kernel
+// gives with swap_rb on cv2.cvtColor's output.
+template <class Frames, int L>
+__global__ void __launch_bounds__(256) crop_resize_yuv_kernel(const __grid_constant__ Frames src_frames,
+                                                              const int4* __restrict__ rects, const int* __restrict__ frame_of,
+                                                              uint8_t* __restrict__ out) {
+    const int m = blockIdx.y;
+    const int pix = blockIdx.x * 256 + threadIdx.x;
+    if (pix >= 224 * 224) return;
+    const int dy = pix / 224, dx = pix - dy * 224;
+    const int4 r = rects[m];
+    const int y0 = r.x, h = r.y - r.x, x0 = r.z, w = r.w - r.z;
+    uint8_t* dst = out + ((long long)m * 224 * 224 + pix) * 3;
+    if (h <= 0 || w <= 0) { dst[0] = 0; dst[1] = 0; dst[2] = 0; return; }
+    const uint8_t* frame;
+    int H, W;
+    if constexpr (std::is_same<Frames, OneSizeFrames>::value) {
+        H = src_frames.H;
+        W = src_frames.W;
+        const long long f = frame_of ? frame_of[m] : 0;
+        frame = src_frames.frames + f * H * W / 2 * 3;
+    } else {
+        const auto& fr = src_frames.f[frame_of[m]];
+        H = fr.H;
+        W = fr.W;
+        frame = fr.base;
+    }
+    int v[3], a[3], b[3], c[3], d[3];
+    if (h == 448 && w == 448) {                     // the 2x2 box of an exact 2x down-scale
+        const int y = y0 + 2 * dy, x = x0 + 2 * dx;
+        yuv_pixel<L>(frame, H, W, y, x, a);
+        yuv_pixel<L>(frame, H, W, y, x + 1, b);
+        yuv_pixel<L>(frame, H, W, y + 1, x, c);
+        yuv_pixel<L>(frame, H, W, y + 1, x + 1, d);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) v[k] = (a[k] + b[k] + c[k] + d[k] + 2) >> 2;
+    } else {
+        const AxisTap tx = axis_tap(dx, w, true), ty = axis_tap(dy, h, false);
+        yuv_pixel<L>(frame, H, W, y0 + ty.s0, x0 + tx.s0, a);
+        yuv_pixel<L>(frame, H, W, y0 + ty.s0, x0 + tx.s1, b);
+        yuv_pixel<L>(frame, H, W, y0 + ty.s1, x0 + tx.s0, c);
+        yuv_pixel<L>(frame, H, W, y0 + ty.s1, x0 + tx.s1, d);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const int h0 = a[k] * tx.w0 + b[k] * tx.w1;
+            const int h1 = c[k] * tx.w0 + d[k] * tx.w1;
+            v[k] = (((ty.w0 * (h0 >> 4)) >> 16) + ((ty.w1 * (h1 >> 4)) >> 16) + 2) >> 2;
+        }
+    }
+    dst[0] = (uint8_t)v[2];
+    dst[1] = (uint8_t)v[1];
+    dst[2] = (uint8_t)v[0];
 }
 
 }  // namespace whenet

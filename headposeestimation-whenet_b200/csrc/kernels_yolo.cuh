@@ -5,6 +5,7 @@
 //                                             the host exactly as ImagingResample does) + the (128,128,128) canvas and the paste
 //                                             (reference utils.py:23-34)
 //   letterbox_{h,v}_ragged_kernel              the same two passes over frames of different sizes, one LetterboxFrame each
+//   letterbox_h{,_ragged}_yuv_kernel<L>        the horizontal passes over NV12 / I420 frames, converting each pixel as it is read
 //   yolo_conv0_kernel<N>                       first conv (3 -> N = 32, tiny: 16, 3x3): im2col row built in shared memory from the
 //                                             uint8 canvas through a v/255 table split into bf16 hi + lo parts, one K = 64 wgmma
 //                                             block per row
@@ -19,6 +20,7 @@
 #include <vector>
 
 #include "kernels_tc.cuh"
+#include "yuv.cuh"
 
 namespace whenet {
 namespace yolo {
@@ -187,10 +189,12 @@ struct LetterboxFrame {
     int H, W, nw, nh, ox, oy, y0, rows, ksx, ksy;
     int xb, kx, yb, ky;
 };
-int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb);
+// yuv_layout 0: packed 8-bit frames (BGR when swap_rb); kYuvNV12 / kYuvI420: 4:2:0 frames (yuv.cuh), swap_rb ignored
+int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb,
+                     int yuv_layout);
 // plans: n device LetterboxFrame; max_hx: the largest rows * nw among them
 int launch_letterbox_ragged(cudaStream_t s, const LetterboxFrame* plans, const char* coef, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n,
-                            long long max_hx, int S_h, int S_w, int swap_rb);
+                            long long max_hx, int S_h, int S_w, int swap_rb, int yuv_layout);
 int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, const float* bias, __nv_bfloat16* out, int n, int S_h, int S_w,
                  int cout);
 int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m);
@@ -284,6 +288,53 @@ __global__ void letterbox_h_ragged_kernel(const LetterboxFrame* __restrict__ pla
     dst[0] = clip8(swap_rb ? s2 : s0);
     dst[1] = clip8(s1);
     dst[2] = clip8(swap_rb ? s0 : s2);
+}
+
+// The horizontal pass over a YUV 4:2:0 frame (yuv.cuh): every tap converts its source pixel to B, G, R and accumulates it as
+// letterbox_h_kernel does, and the row goes to tmp in RGB order, so tmp holds the bits the BGR pass with swap_rb gives on
+// cv2.cvtColor's output.  frame: the frame's Y plane; y: the source row; x0, count, k: the output column's taps.
+template <int L>
+__device__ __forceinline__ void letterbox_h_yuv_taps(const uint8_t* __restrict__ frame, int H, int W, int y, int x0, int count,
+                                                     const int* __restrict__ k, uint8_t* __restrict__ dst) {
+    int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
+    for (int j = 0; j < count; ++j) {
+        const int w = k[j];
+        int p[3];
+        yuv_pixel<L>(frame, H, W, y, x0 + j, p);
+        s0 += p[0] * w;
+        s1 += p[1] * w;
+        s2 += p[2] * w;
+    }
+    dst[0] = clip8(s2);
+    dst[1] = clip8(s1);
+    dst[2] = clip8(s0);
+}
+
+// letterbox_h_kernel on n YUV frames of one size, H * W * 3/2 bytes each
+template <int L>
+__global__ void letterbox_h_yuv_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ tmp, int H, int W, int nw, int y0, int rows,
+                                       const int2* __restrict__ xb, const int* __restrict__ kx, int ksize) {
+    const int f = blockIdx.y;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)rows * nw) return;
+    const int r = (int)(i / nw), x = (int)(i - (long long)r * nw);
+    const int2 b = xb[x];
+    letterbox_h_yuv_taps<L>(in + (long long)f * H * W / 2 * 3, H, W, y0 + r, b.x, b.y, kx + (long long)x * ksize,
+                            tmp + (((long long)f * rows + r) * nw + x) * 3);
+}
+
+// letterbox_h_ragged_kernel on YUV frames of their own sizes
+template <int L>
+__global__ void letterbox_h_ragged_yuv_kernel(const LetterboxFrame* __restrict__ plans, const char* __restrict__ coef,
+                                              const uint8_t* __restrict__ in, uint8_t* __restrict__ tmp) {
+    const LetterboxFrame& P = plans[blockIdx.y];
+    const int nw = P.nw;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)P.rows * nw) return;
+    const int r = (int)(i / nw), x = (int)(i - (long long)r * nw);
+    const int2 b = reinterpret_cast<const int2*>(coef + P.xb)[x];
+    letterbox_h_yuv_taps<L>(in + P.src, P.H, P.W, P.y0 + r, b.x, b.y, reinterpret_cast<const int*>(coef + P.kx) + (long long)x * P.ksx,
+                            tmp + P.tmp + ((long long)r * nw + x) * 3);
 }
 
 __global__ void letterbox_v_ragged_kernel(const LetterboxFrame* __restrict__ plans, const char* __restrict__ coef, const uint8_t* __restrict__ tmp,

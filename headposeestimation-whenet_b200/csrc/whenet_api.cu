@@ -1183,10 +1183,17 @@ int frame_staging(whenet_ctx* c, size_t bytes) {
     return 0;
 }
 
-// The crop table -> crop_resize_kernel<Frames>, one launch per 65535 crops (the grid's y limit).  rects: m x (y0, y1, x0, x1)
-// host int32, an empty one marks a zero crop; frame_of: m host frame indices or NULL (all frame 0, OneSizeFrames only).
+static_assert(whenet::kYuvNV12 == WHENET_YUV_NV12 && whenet::kYuvI420 == WHENET_YUV_I420, "layout codes of yuv.cuh and the ABI");
+
+// bytes of an H x W frame: packed 8-bit BGR / RGB (yuv_layout 0) or YUV 4:2:0 (H and W even)
+size_t frame_bytes(int H, int W, int yuv_layout) { return yuv_layout ? (size_t)H * W / 2 * 3 : (size_t)H * W * 3; }
+
+// The crop table -> crop_resize_kernel<Frames> (yuv_layout 0) or crop_resize_yuv_kernel<Frames, yuv_layout>, one launch per 65535
+// crops (the grid's y limit).  rects: m x (y0, y1, x0, x1) host int32, an empty one marks a zero crop; frame_of: m host frame
+// indices or NULL (all frame 0, OneSizeFrames only).
 template <class Frames>
-int launch_crop_kernel(whenet_ctx* c, const Frames& src, const int32_t* rects, const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
+int launch_crop_kernel(whenet_ctx* c, const Frames& src, const int32_t* rects, const int32_t* frame_of, int m, int swap_rb, int yuv_layout,
+                       uint8_t* crops_out) {
     if (c->rects_cap < m) {
         if (c->d_rects) cudaFree(c->d_rects);
         if (c->d_frame_of) cudaFree(c->d_frame_of);
@@ -1200,8 +1207,15 @@ int launch_crop_kernel(whenet_ctx* c, const Frames& src, const int32_t* rects, c
     Scope sc(c, "crop_resize", (double)m * 224 * 224 * 3 * 2, 0.0);
     for (int m0 = 0; m0 < m; m0 += 65535) {
         const int mb = std::min(65535, m - m0);
-        whenet::crop_resize_kernel<Frames><<<dim3((224 * 224 + 255) / 256, mb), 256, 0, c->stream>>>(
-            src, c->d_rects + m0, frame_of ? c->d_frame_of + m0 : nullptr, crops_out + (size_t)m0 * 224 * 224 * 3, swap_rb);
+        const dim3 grid((224 * 224 + 255) / 256, mb);
+        const int* fo = frame_of ? c->d_frame_of + m0 : nullptr;
+        uint8_t* out = crops_out + (size_t)m0 * 224 * 224 * 3;
+        if (yuv_layout == whenet::kYuvNV12)
+            whenet::crop_resize_yuv_kernel<Frames, whenet::kYuvNV12><<<grid, 256, 0, c->stream>>>(src, c->d_rects + m0, fo, out);
+        else if (yuv_layout == whenet::kYuvI420)
+            whenet::crop_resize_yuv_kernel<Frames, whenet::kYuvI420><<<grid, 256, 0, c->stream>>>(src, c->d_rects + m0, fo, out);
+        else
+            whenet::crop_resize_kernel<Frames><<<grid, 256, 0, c->stream>>>(src, c->d_rects + m0, fo, out, swap_rb);
         CK(cudaGetLastError());
     }
     return 0;
@@ -1209,37 +1223,37 @@ int launch_crop_kernel(whenet_ctx* c, const Frames& src, const int32_t* rects, c
 
 // n frames of one size (uploaded into the context's staging buffer when on the host) -> launch_crop_kernel
 int launch_crops(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const int32_t* rects,
-                 const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
+                 const int32_t* frame_of, int m, int swap_rb, int yuv_layout, uint8_t* crops_out) {
     CK(cudaSetDevice(c->device));
     const uint8_t* d_frames = frames;
     if (!frames_are_device) {
-        const size_t bytes = (size_t)n * H * W * 3;
+        const size_t bytes = n * frame_bytes(H, W, yuv_layout);
         if (int rc = frame_staging(c, bytes)) return rc;
         CK(cudaMemcpyAsync(c->d_frame, frames, bytes, cudaMemcpyHostToDevice, c->stream));
         d_frames = c->d_frame;
     }
-    return launch_crop_kernel(c, whenet::OneSizeFrames{d_frames, H, W}, rects, frame_of, m, swap_rb, crops_out);
+    return launch_crop_kernel(c, whenet::OneSizeFrames{d_frames, H, W}, rects, frame_of, m, swap_rb, yuv_layout, crops_out);
 }
 
 // n frames of their own sizes: host frames are uploaded into the staging buffer at 256-byte aligned offsets, device frames are
 // read where they are
 int launch_crops_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const int32_t* rects,
-                        const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out) {
+                        const int32_t* frame_of, int m, int swap_rb, int yuv_layout, uint8_t* crops_out) {
     CK(cudaSetDevice(c->device));
     whenet::PerFrameSources src{};
     std::vector<size_t> off(n);
     size_t total = 0;
     for (int i = 0; i < n; ++i) {
         off[i] = total;
-        total += ((size_t)hw[2 * i] * hw[2 * i + 1] * 3 + 255) & ~(size_t)255;
+        total += (frame_bytes(hw[2 * i], hw[2 * i + 1], yuv_layout) + 255) & ~(size_t)255;
     }
     if (!frames_are_device) {
         if (int rc = frame_staging(c, total)) return rc;
         for (int i = 0; i < n; ++i)
-            CK(cudaMemcpyAsync(c->d_frame + off[i], frames[i], (size_t)hw[2 * i] * hw[2 * i + 1] * 3, cudaMemcpyHostToDevice, c->stream));
+            CK(cudaMemcpyAsync(c->d_frame + off[i], frames[i], frame_bytes(hw[2 * i], hw[2 * i + 1], yuv_layout), cudaMemcpyHostToDevice, c->stream));
     }
-    for (int i = 0; i < n; ++i) src.f[i] = {frames_are_device ? frames[i] : c->d_frame + off[i], hw[2 * i + 1]};
-    return launch_crop_kernel(c, src, rects, frame_of, m, swap_rb, crops_out);
+    for (int i = 0; i < n; ++i) src.f[i] = {frames_are_device ? frames[i] : c->d_frame + off[i], hw[2 * i + 1], hw[2 * i]};
+    return launch_crop_kernel(c, src, rects, frame_of, m, swap_rb, yuv_layout, crops_out);
 }
 
 }  // namespace
@@ -1545,15 +1559,28 @@ int whenet_crop_resize_u8(whenet_ctx* c, const uint8_t* frame, int H, int W, int
             return fail(WHENET_EINVAL, "box %d: slice [%d:%d, %d:%d] is empty or outside the %dx%d frame (cv2.resize would raise)",
                         i, r[0], r[1], r[2], r[3], H, W);
     }
-    return launch_crops(c, frame, 1, H, W, frame_is_device, rects, nullptr, m, swap_rb, crops_out);
+    return launch_crops(c, frame, 1, H, W, frame_is_device, rects, nullptr, m, swap_rb, 0, crops_out);
 }
 
-int whenet_crop_boxes_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes,
-                         const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+}  // extern "C"
+
+namespace {
+
+int check_yuv_layout(int yuv_layout) {
+    if (yuv_layout != WHENET_YUV_NV12 && yuv_layout != WHENET_YUV_I420)
+        return fail(WHENET_EINVAL, "yuv_layout=%d: WHENET_YUV_NV12 (%d) or WHENET_YUV_I420 (%d)", yuv_layout, WHENET_YUV_NV12, WHENET_YUV_I420);
+    return 0;
+}
+
+// whenet_crop_boxes_u8 (yuv_layout 0) and whenet_crop_boxes_yuv_u8
+int crop_boxes(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes, const int32_t* frame_of,
+               int m, int swap_rb, int yuv_layout, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
     // the context is checked last so that every other argument can be validated without a GPU
     if (!frames || !boxes || !frame_of || !crops_out) return fail(WHENET_EINVAL, "null frames, boxes, frame_of or crops_out");
     if (n < 1 || n > 64) return fail(WHENET_EINVAL, "n=%d frames outside [1, 64]", n);
     if (H < 1 || W < 1) return fail(WHENET_EINVAL, "bad frame size %dx%d", H, W);
+    if (yuv_layout && (H > 16384 || W > 16384 || H % 2 || W % 2))
+        return fail(WHENET_EINVAL, "frame size %dx%d: a 4:2:0 frame has even sides of at most 16384", H, W);
     if (m < 1) return fail(WHENET_EINVAL, "m=%d boxes", m);
     for (int i = 0; i < m; ++i)
         if (frame_of[i] < 0 || frame_of[i] >= n) return fail(WHENET_EINVAL, "box %d: frame_of=%d outside [0, %d)", i, frame_of[i], n);
@@ -1564,11 +1591,12 @@ int whenet_crop_boxes_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int
         if (valid_out) valid_out[i] = ok;
     }
     if (rects_out) memcpy(rects_out, rects.data(), rects.size() * sizeof(int32_t));
-    return launch_crops(c, frames, n, H, W, frames_are_device, rects.data(), frame_of, m, swap_rb, crops_out);
+    return launch_crops(c, frames, n, H, W, frames_are_device, rects.data(), frame_of, m, swap_rb, yuv_layout, crops_out);
 }
 
-int whenet_crop_boxes_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const float* boxes,
-                                const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+// whenet_crop_boxes_ragged_u8 (yuv_layout 0) and whenet_crop_boxes_ragged_yuv_u8
+int crop_boxes_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const float* boxes,
+                      const int32_t* frame_of, int m, int swap_rb, int yuv_layout, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
     // the context is checked last so that every other argument can be validated without a GPU
     if (!frames || !hw || !boxes || !frame_of || !crops_out) return fail(WHENET_EINVAL, "null frames, hw, boxes, frame_of or crops_out");
     if (n < 1 || n > whenet::kMaxCropFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxCropFrames);
@@ -1576,6 +1604,8 @@ int whenet_crop_boxes_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, con
         if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
         if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
             return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+        if (yuv_layout && (hw[2 * i] % 2 || hw[2 * i + 1] % 2))
+            return fail(WHENET_EINVAL, "frame %d: frame size %dx%d: a 4:2:0 frame has even sides", i, hw[2 * i + 1], hw[2 * i]);
     }
     if (m < 1) return fail(WHENET_EINVAL, "m=%d boxes", m);
     for (int i = 0; i < m; ++i)
@@ -1587,7 +1617,34 @@ int whenet_crop_boxes_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, con
         if (valid_out) valid_out[i] = ok;
     }
     if (rects_out) memcpy(rects_out, rects.data(), rects.size() * sizeof(int32_t));
-    return launch_crops_ragged(c, frames, hw, n, frames_are_device, rects.data(), frame_of, m, swap_rb, crops_out);
+    return launch_crops_ragged(c, frames, hw, n, frames_are_device, rects.data(), frame_of, m, swap_rb, yuv_layout, crops_out);
+}
+
+}  // namespace
+
+extern "C" {
+
+int whenet_crop_boxes_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes,
+                         const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+    return crop_boxes(c, frames, n, H, W, frames_are_device, boxes, frame_of, m, swap_rb, 0, crops_out, rects_out, valid_out);
+}
+
+int whenet_crop_boxes_yuv_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes,
+                             const int32_t* frame_of, int m, int yuv_layout, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+    if (int rc = check_yuv_layout(yuv_layout)) return rc;
+    return crop_boxes(c, frames, n, H, W, frames_are_device, boxes, frame_of, m, 1, yuv_layout, crops_out, rects_out, valid_out);
+}
+
+int whenet_crop_boxes_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const float* boxes,
+                                const int32_t* frame_of, int m, int swap_rb, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+    return crop_boxes_ragged(c, frames, hw, n, frames_are_device, boxes, frame_of, m, swap_rb, 0, crops_out, rects_out, valid_out);
+}
+
+int whenet_crop_boxes_ragged_yuv_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                    const float* boxes, const int32_t* frame_of, int m, int yuv_layout, uint8_t* crops_out, int32_t* rects_out,
+                                    int32_t* valid_out) {
+    if (int rc = check_yuv_layout(yuv_layout)) return rc;
+    return crop_boxes_ragged(c, frames, hw, n, frames_are_device, boxes, frame_of, m, 1, yuv_layout, crops_out, rects_out, valid_out);
 }
 
 int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out) {

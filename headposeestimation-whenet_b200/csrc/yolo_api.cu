@@ -64,11 +64,18 @@ struct GraphEntry {
     uint8_t* tmp = nullptr;         // horizontal-pass output
 };
 
-// a graph of frames of several sizes: (H0, W0, H1, W1, ...) and swap_rb
-using RaggedKey = std::pair<std::vector<int>, int>;
+// a graph of n frames of one size: (n, H, swap_rb ? W : -W, yuv_layout)
+using OneSizeKey = std::tuple<int, int, int, int>;
+// a graph of frames of several sizes: (H0, W0, H1, W1, ...), swap_rb and yuv_layout
+using RaggedKey = std::tuple<std::vector<int>, int, int>;
 constexpr size_t kMaxGraphs = 16;   // captured graphs kept per cache
 
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+static_assert(whenet::kYuvNV12 == WHENET_YUV_NV12 && whenet::kYuvI420 == WHENET_YUV_I420, "layout codes of yuv.cuh and the ABI");
+
+// bytes of an H x W frame: packed 8-bit BGR / RGB (yuv_layout 0) or YUV 4:2:0 (H and W even)
+size_t frame_bytes(int H, int W, int yuv_layout) { return yuv_layout ? (size_t)H * W / 2 * 3 : (size_t)H * W * 3; }
 
 // Pillow ImagingResample (libImaging/Resample.c) coefficient tables for BICUBIC: support 2 scaled by the downscale factor,
 // weights normalised in double and quantised to 22 bits (normalize_coeffs_8bpc).
@@ -133,7 +140,7 @@ struct whenet_det {
     uint8_t* d_canvas = nullptr;
     float4* d_cand = nullptr; float* d_cand_score = nullptr;
     float* d_boxes = nullptr; float* d_scores = nullptr; int* d_classes = nullptr; int* d_count = nullptr;
-    std::map<std::tuple<int, int, int>, GraphEntry> graphs;
+    std::map<OneSizeKey, GraphEntry> graphs;
     std::map<RaggedKey, GraphEntry> ragged_graphs;      // whenet_det_detect_ragged_u8's
     int last_n = 0;
 };
@@ -270,7 +277,7 @@ int capture_forward(whenet_det* d, int n, Letterbox&& letterbox, GraphEntry* e) 
     return 0;
 }
 
-int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
+int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, int yuv_layout, GraphEntry* e) {
     std::vector<char> blob;
     Y::LetterboxFrame f;
     if (int rc = frame_plan(d, H, W, blob, &f)) return rc;
@@ -280,12 +287,13 @@ int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, GraphEntry* e) {
     CKD(cudaMalloc(&e->tmp, (size_t)n * f.rows * f.nw * 3));
     Y::LetterboxPlan lp{H, W, f.nw, f.nh, f.ox, f.oy, f.y0, f.rows, f.ksx, f.ksy,
                         (const int2*)(base + f.xb), (const int*)(base + f.kx), (const int2*)(base + f.yb), (const int*)(base + f.ky)};
-    return capture_forward(d, n, [&](cudaStream_t s) { return Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb); },
+    return capture_forward(d, n, [&](cudaStream_t s) { return Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb,
+                                                                             yuv_layout); },
                            e);
 }
 
 // frame i at byte offset off[i] of d_frames, hw[2i] x hw[2i+1]
-int make_ragged_entry(whenet_det* d, int n, const int32_t* hw, const std::vector<size_t>& off, int swap_rb, GraphEntry* e) {
+int make_ragged_entry(whenet_det* d, int n, const int32_t* hw, const std::vector<size_t>& off, int swap_rb, int yuv_layout, GraphEntry* e) {
     std::vector<char> blob;
     std::vector<Y::LetterboxFrame> plans(n);
     size_t tmp_bytes = 0;
@@ -307,7 +315,7 @@ int make_ragged_entry(whenet_det* d, int n, const int32_t* hw, const std::vector
     const char* coef = (const char*)e->coef;
     const auto* d_plans = (const Y::LetterboxFrame*)(coef + plans_at);
     return capture_forward(d, n, [&](cudaStream_t s) {
-        return Y::launch_letterbox_ragged(s, d_plans, coef, d->d_frames, e->tmp, d->d_canvas, n, max_hx, d->in_h, d->in_w, swap_rb);
+        return Y::launch_letterbox_ragged(s, d_plans, coef, d->d_frames, e->tmp, d->d_canvas, n, max_hx, d->in_h, d->in_w, swap_rb, yuv_layout);
     }, e);
 }
 
@@ -586,14 +594,22 @@ int whenet_det_set_stream(whenet_det* d, void* s) {
     return 0;
 }
 
-int whenet_det_detect_u8(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb, float score, float iou,
-                         int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
-    if (!d || !frames) return fail(WHENET_EINVAL, "null detector or frames");
-    if (int rc = check_frames(d, n, H, W)) return rc;
-    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+}  // extern "C"
+
+namespace {
+
+int check_yuv_layout(int yuv_layout) {
+    if (yuv_layout != WHENET_YUV_NV12 && yuv_layout != WHENET_YUV_I420)
+        return fail(WHENET_EINVAL, "yuv_layout=%d: WHENET_YUV_NV12 (%d) or WHENET_YUV_I420 (%d)", yuv_layout, WHENET_YUV_NV12, WHENET_YUV_I420);
+    return 0;
+}
+
+// whenet_det_detect_u8 (yuv_layout 0) and whenet_det_detect_yuv_u8 after their argument checks
+int detect_one_size(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb, int yuv_layout, float score,
+                    float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
     CKD(cudaSetDevice(d->device));
     // frames -> the context's input buffer (the captured graph reads a fixed address); RGB order there
-    const size_t bytes = (size_t)n * H * W * 3;
+    const size_t bytes = n * frame_bytes(H, W, yuv_layout);
     if (d->frames_cap < bytes) {
         CKD(cudaStreamSynchronize(d->stream));
         cudaFree(d->d_frames);
@@ -603,12 +619,12 @@ int whenet_det_detect_u8(whenet_det* d, const uint8_t* frames, int n, int H, int
         d->frames_cap = bytes;
     }
     CKD(cudaMemcpyAsync(d->d_frames, frames, bytes, frames_are_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, d->stream));
-    const auto key = std::make_tuple(n, H, swap_rb ? W : -W);      // graphs keyed on (n, H, W) and the channel order
+    const OneSizeKey key(n, H, swap_rb ? W : -W, yuv_layout);      // graphs keyed on (n, H, W), the channel order and the layout
     auto it = d->graphs.find(key);
     if (it == d->graphs.end()) {
         if (d->graphs.size() >= kMaxGraphs) { CKD(cudaStreamSynchronize(d->stream)); free_graph_map(d->graphs); }
         GraphEntry e{};
-        int rc = make_entry(d, n, H, W, swap_rb ? 1 : 0, &e);
+        int rc = make_entry(d, n, H, W, swap_rb ? 1 : 0, yuv_layout, &e);
         if (rc) { free_entry(e); return rc; }
         it = d->graphs.emplace(key, e).first;
     }
@@ -617,8 +633,9 @@ int whenet_det_detect_u8(whenet_det* d, const uint8_t* frames, int n, int H, int
     return run_decode(d, decode_params(d, n, nullptr, H, W, score, iou, max_boxes), n, boxes, scores, classes, counts);
 }
 
-int whenet_det_detect_ragged_u8(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int swap_rb,
-                                float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+// whenet_det_detect_ragged_u8 (yuv_layout 0) and whenet_det_detect_ragged_yuv_u8
+int detect_ragged(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int swap_rb, int yuv_layout,
+                  float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
     // the detector is checked after every argument that can be validated without a GPU
     if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
     if (n < 1 || n > Y::kMaxFrames) return fail(WHENET_EINVAL, "n=%d outside [1, %d]", n, Y::kMaxFrames);
@@ -626,6 +643,8 @@ int whenet_det_detect_ragged_u8(whenet_det* d, const uint8_t* const* frames, con
         if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
         if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
             return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+        if (yuv_layout && (hw[2 * i] % 2 || hw[2 * i + 1] % 2))
+            return fail(WHENET_EINVAL, "frame %d: frame size %dx%d: a 4:2:0 frame has even sides", i, hw[2 * i + 1], hw[2 * i]);
     }
     if (!boxes || !scores || !classes || !counts) return fail(WHENET_EINVAL, "null output pointer");
     if (!d) return fail(WHENET_EINVAL, "null detector");
@@ -638,7 +657,7 @@ int whenet_det_detect_ragged_u8(whenet_det* d, const uint8_t* const* frames, con
     size_t bytes = 0;
     for (int i = 0; i < n; ++i) {
         off[i] = bytes;
-        bytes += align256((size_t)hw[2 * i] * hw[2 * i + 1] * 3);
+        bytes += align256(frame_bytes(hw[2 * i], hw[2 * i + 1], yuv_layout));
     }
     if (d->frames_cap < bytes) {
         CKD(cudaStreamSynchronize(d->stream));
@@ -649,19 +668,57 @@ int whenet_det_detect_ragged_u8(whenet_det* d, const uint8_t* const* frames, con
         d->frames_cap = bytes;
     }
     const cudaMemcpyKind kind = frames_are_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    for (int i = 0; i < n; ++i) CKD(cudaMemcpyAsync(d->d_frames + off[i], frames[i], (size_t)hw[2 * i] * hw[2 * i + 1] * 3, kind, d->stream));
-    RaggedKey key(std::vector<int>(hw, hw + 2 * n), swap_rb ? 1 : 0);
+    for (int i = 0; i < n; ++i) CKD(cudaMemcpyAsync(d->d_frames + off[i], frames[i], frame_bytes(hw[2 * i], hw[2 * i + 1], yuv_layout), kind, d->stream));
+    RaggedKey key(std::vector<int>(hw, hw + 2 * n), swap_rb ? 1 : 0, yuv_layout);
     auto it = d->ragged_graphs.find(key);
     if (it == d->ragged_graphs.end()) {
         if (d->ragged_graphs.size() >= kMaxGraphs) { CKD(cudaStreamSynchronize(d->stream)); free_graph_map(d->ragged_graphs); }
         GraphEntry e{};
-        int rc = make_ragged_entry(d, n, hw, off, swap_rb ? 1 : 0, &e);
+        int rc = make_ragged_entry(d, n, hw, off, swap_rb ? 1 : 0, yuv_layout, &e);
         if (rc) { free_entry(e); return rc; }
         it = d->ragged_graphs.emplace(std::move(key), e).first;
     }
     CKD(cudaGraphLaunch(it->second.exec, d->stream));
     d->last_n = n;
     return run_decode(d, decode_params(d, n, hw, 0, 0, score, iou, max_boxes), n, boxes, scores, classes, counts);
+}
+
+}  // namespace
+
+extern "C" {
+
+int whenet_det_detect_u8(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb, float score, float iou,
+                         int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    if (!d || !frames) return fail(WHENET_EINVAL, "null detector or frames");
+    if (int rc = check_frames(d, n, H, W)) return rc;
+    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+    return detect_one_size(d, frames, n, H, W, frames_are_device, swap_rb, 0, score, iou, max_boxes, boxes, scores, classes, counts);
+}
+
+int whenet_det_detect_yuv_u8(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int yuv_layout, float score,
+                             float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    // the detector is checked after every argument that can be validated without a GPU
+    if (int rc = check_yuv_layout(yuv_layout)) return rc;
+    if (!frames) return fail(WHENET_EINVAL, "null frames");
+    if (n < 1 || n > Y::kMaxFrames) return fail(WHENET_EINVAL, "n=%d outside [1, %d]", n, Y::kMaxFrames);
+    if (H < 2 || W < 2 || H > 16384 || W > 16384 || H % 2 || W % 2)
+        return fail(WHENET_EINVAL, "frame size %dx%d: a 4:2:0 frame has even sides in [2, 16384]", W, H);
+    if (!boxes || !scores || !classes || !counts) return fail(WHENET_EINVAL, "null output pointer");
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    if (n > d->max_frames) return fail(WHENET_EINVAL, "n=%d outside [1, max_frames=%d]", n, d->max_frames);
+    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+    return detect_one_size(d, frames, n, H, W, frames_are_device, 1, yuv_layout, score, iou, max_boxes, boxes, scores, classes, counts);
+}
+
+int whenet_det_detect_ragged_u8(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int swap_rb,
+                                float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    return detect_ragged(d, frames, hw, n, frames_are_device, swap_rb, 0, score, iou, max_boxes, boxes, scores, classes, counts);
+}
+
+int whenet_det_detect_ragged_yuv_u8(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int yuv_layout,
+                                    float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    if (int rc = check_yuv_layout(yuv_layout)) return rc;
+    return detect_ragged(d, frames, hw, n, frames_are_device, 1, yuv_layout, score, iou, max_boxes, boxes, scores, classes, counts);
 }
 
 int whenet_det_synchronize(whenet_det* d) {

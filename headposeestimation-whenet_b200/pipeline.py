@@ -9,21 +9,25 @@ import numpy as np
 from . import crops as _crops
 from ._lib import WhenetError, check
 from .whenet import _is_device, _ptr
-from .yolo import _frame_list, _frame_table
+from .yolo import _frame_list, _frame_table, _image_size, _pixel_layout, _yuv_image_size
 
 
-def detect_and_estimate(yolo, whenet, frame_bgr):
+def detect_and_estimate(yolo, whenet, frame_bgr, *, pixel_format="bgr"):
     """``frame_bgr``: H x W x 3 uint8 as cv2 delivers it -> (boxes (k,4) float32, scores (k,) float32, angles (k,3) float32
     yaw/pitch/roll in degrees).  The one-frame case of ``detect_and_estimate_frames``, except that a head whose slice is
     empty or outside the frame raises ``WhenetError`` (code -1, naming the box and its slice) as cv2.resize raises in the
-    reference, instead of getting NaN angles."""
+    reference, instead of getting NaN angles.  ``pixel_format="nv12"`` / ``"i420"``: an (H * 3/2, W) YUV 4:2:0 frame in
+    cv2's layout (see ``detect_and_estimate_frames``)."""
+    layout = _pixel_layout(pixel_format)
     frame = np.ascontiguousarray(frame_bgr, dtype=np.uint8)
-    if frame.ndim != 3 or frame.shape[2] != 3:
+    if layout:
+        _yuv_image_size(frame.shape, "frame")
+    elif frame.ndim != 3 or frame.shape[2] != 3:
         raise ValueError("frame must be H x W x 3 uint8")
-    return _run(yolo, whenet, frame[None], strict=True)[0]
+    return _run(yolo, whenet, frame[None], strict=True, pixel_format=pixel_format)[0]
 
 
-def detect_and_estimate_frames(yolo, whenet, frames_bgr):
+def detect_and_estimate_frames(yolo, whenet, frames_bgr, *, pixel_format="bgr"):
     """``frames_bgr``: (n, H, W, 3) uint8 BGR frames of one size, a numpy array or a contiguous CUDA uint8 tensor on
     ``whenet.device`` -> n tuples (boxes (k,4) float32, scores (k,) float32, angles (k,3) float32), per frame bit-identical
     to ``detect_and_estimate`` on that frame alone.
@@ -39,15 +43,20 @@ def detect_and_estimate_frames(yolo, whenet, frames_bgr):
     ``frames_bgr`` may also be a list or tuple of (H_i, W_i, 3) uint8 BGR frames of any sizes (several cameras), all numpy
     arrays or all contiguous CUDA tensors on ``whenet.device``; frames of one size run as the batch above.  Frames of several
     sizes take the same path through the per-frame entries (``whenet_det_detect_ragged_u8``, ``whenet_crop_boxes_ragged_u8``),
-    each frame's result bit-identical to ``detect_and_estimate`` on that frame alone.  An empty list gives []."""
-    return _run(yolo, whenet, frames_bgr, strict=False)
+    each frame's result bit-identical to ``detect_and_estimate`` on that frame alone.  An empty list gives [].
+
+    ``pixel_format="nv12"`` or ``"i420"`` takes YUV 4:2:0 video frames in cv2's layout (what hardware and software video
+    decoders hand out) instead of BGR: (n, H * 3/2, W) uint8, or a list or tuple of (H_i * 3/2, W_i) frames, H and W even.
+    The letterbox and the crops convert each pixel as they read it, so host frames upload half the bytes of BGR frames, and
+    the results are the bits ``detect_and_estimate_frames`` gives on ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12 / _I420)``."""
+    return _run(yolo, whenet, frames_bgr, strict=False, pixel_format=pixel_format)
 
 
-def _checked_frames(yolo, whenet, frames):
+def _checked_frames(yolo, whenet, frames, layout):
     if yolo.device != whenet.device:
         raise ValueError("the detector runs on device %d and WHENet on device %d" % (yolo.device, whenet.device))
     if isinstance(frames, (list, tuple)):
-        frames, dev = _frame_list(frames, whenet.device)
+        frames, dev = _frame_list(frames, whenet.device, layout)
         if len({tuple(f.shape) for f in frames}) > 1:
             return frames
         if not frames:
@@ -66,7 +75,11 @@ def _checked_frames(yolo, whenet, frames):
         frames = np.asarray(frames)
         if frames.dtype != np.uint8:
             raise ValueError("frames must be uint8, not %s" % frames.dtype)
-    if len(frames.shape) != 4 or frames.shape[3] != 3:
+    if layout:
+        if len(frames.shape) != 3:
+            raise ValueError("frames must be (n, H * 3/2, W) uint8 for a 4:2:0 pixel format, not %s" % (tuple(frames.shape),))
+        _yuv_image_size(frames.shape[1:], "a frame")
+    elif len(frames.shape) != 4 or frames.shape[3] != 3:
         raise ValueError("frames must be (n, H, W, 3) uint8, not %s" % (tuple(frames.shape),))
     return frames
 
@@ -83,15 +96,15 @@ def _raise_first_invalid(L, boxes, H, W):
                       % (i, y0, y1, x0, x1, H, W))
 
 
-def _run(yolo, whenet, frames, strict):
-    frames = _checked_frames(yolo, whenet, frames)
-    ragged = isinstance(frames, list)       # frames of several sizes; otherwise one (n, H, W, 3) array or tensor
-    if ragged:
-        n = len(frames)
-    else:
-        n, H, W = (int(v) for v in frames.shape[:3])
+def _run(yolo, whenet, frames, strict, pixel_format="bgr"):
+    layout = _pixel_layout(pixel_format)
+    frames = _checked_frames(yolo, whenet, frames, layout)
+    ragged = isinstance(frames, list)       # frames of several sizes; otherwise one (n, H, W, 3) or (n, H * 3/2, W) array or tensor
+    n = len(frames) if ragged else int(frames.shape[0])
     if n == 0:
         return []
+    if not ragged:
+        H, W = _image_size(frames.shape[1:], layout)
     import torch
     L = whenet._L
     dev = _is_device(frames[0] if ragged else frames)
@@ -123,7 +136,7 @@ def _run(yolo, whenet, frames, strict):
             return stage_ragged(k, frames[lo:hi])
         buf = stage[k % 2]
         if buf is None:
-            buf = stage[k % 2] = torch.empty((min(step, n), H, W, 3), dtype=torch.uint8, device="cuda")
+            buf = stage[k % 2] = torch.empty((min(step, n),) + tuple(frames.shape[1:]), dtype=torch.uint8, device="cuda")
         buf[:hi - lo].copy_(torch.from_numpy(np.ascontiguousarray(frames[lo:hi])))
         torch.cuda.current_stream().synchronize()       # the detector reads it on its own stream
         return buf[:hi - lo]
@@ -135,7 +148,7 @@ def _run(yolo, whenet, frames, strict):
             cur = chunk(0)
             for k in range(n_chunks):
                 nb = len(cur)
-                dets = yolo.detect_frames(cur)          # synchronous, on the detector's stream
+                dets = yolo.detect_frames(cur, pixel_format=pixel_format)      # synchronous, on the detector's stream
                 if k + 1 < n_chunks:
                     if not dev:
                         whenet.synchronize()            # chunk k-1's crops have read the buffer chunk k+1 goes to
@@ -153,18 +166,21 @@ def _run(yolo, whenet, frames, strict):
                     d_ang = torch.empty((m, 3), dtype=torch.float32, device="cuda")
                     keep.append(d_ang)
                     if ragged:
-                        ptrs, hw = _frame_table(cur)
+                        ptrs, hw = _frame_table(cur, layout)
                     for s in range(0, m, whenet.max_batch):
                         mb = min(whenet.max_batch, m - s)
                         if crop_buf is None or crop_buf.shape[0] < mb:
                             crop_buf = torch.empty((mb, 224, 224, 3), dtype=torch.uint8, device="cuda")
                             keep.append(crop_buf)
+                        # layout in place of swap_rb = 1: the YUV entries write RGB crops as the BGR ones do with it
                         if ragged:
-                            check(L.whenet_crop_boxes_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), nb, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]),
-                                                                mb, 1, _ptr(crop_buf), None, _ptr(valid[s:])))
+                            crop = L.whenet_crop_boxes_ragged_yuv_u8 if layout else L.whenet_crop_boxes_ragged_u8
+                            check(crop(whenet._h, C.addressof(ptrs), _ptr(hw), nb, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, layout or 1,
+                                       _ptr(crop_buf), None, _ptr(valid[s:])))
                         else:
-                            check(L.whenet_crop_boxes_u8(whenet._h, _ptr(cur), nb, H, W, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, 1,
-                                                         _ptr(crop_buf), None, _ptr(valid[s:])))
+                            crop = L.whenet_crop_boxes_yuv_u8 if layout else L.whenet_crop_boxes_u8
+                            check(crop(whenet._h, _ptr(cur), nb, H, W, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, layout or 1,
+                                       _ptr(crop_buf), None, _ptr(valid[s:])))
                         check(L.whenet_forward_u8(whenet._h, _ptr(crop_buf), mb, 1, _ptr(d_ang[s:s + mb]), None, 1))
                     results.append((dets, d_ang, valid))
                 if k + 1 < n_chunks:

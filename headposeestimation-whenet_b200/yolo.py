@@ -45,9 +45,35 @@ def _tensor_list(layers):
     return t, (arrs, names)
 
 
-def _frame_list(frames, device: int):
-    """A list or tuple of (H_i, W_i, 3) uint8 frames, all numpy arrays or all contiguous CUDA tensors on ``device`` ->
-    (list of C-contiguous frames, whether they are on the device).  Raises ValueError otherwise."""
+def _pixel_layout(pixel_format) -> int:
+    """``pixel_format`` -> the C entries' yuv_layout: 0 for "bgr" (packed 8-bit BGR, the *_u8 entries), WHENET_YUV_NV12 for
+    "nv12", WHENET_YUV_I420 for "i420" (the *_yuv_u8 entries).  Raises ValueError otherwise."""
+    if isinstance(pixel_format, str) and (pixel_format == "bgr" or pixel_format in _lib.YUV_LAYOUTS):
+        return _lib.YUV_LAYOUTS.get(pixel_format, 0)
+    raise ValueError("pixel_format must be 'bgr', 'nv12' or 'i420', not %r" % (pixel_format,))
+
+
+def _yuv_image_size(shape, what: str) -> Tuple[int, int]:
+    """The shape of a YUV 4:2:0 frame in cv2's layout, (H * 3/2, W) -> its image size (H, W); ValueError naming ``what``
+    unless the shape is 2-D with a row count divisible by 3 and an even width (so H and W are even and at least 2)."""
+    if len(shape) != 2:
+        raise ValueError("%s must be (H * 3/2, W) uint8 for a 4:2:0 pixel format, not %s" % (what, tuple(shape)))
+    rows, w = (int(v) for v in shape)
+    if rows < 3 or rows % 3:
+        raise ValueError("%s has %d rows: a 4:2:0 frame has H * 3/2 rows, a positive multiple of 3" % (what, rows))
+    if w < 2 or w % 2:
+        raise ValueError("%s is %d pixels wide: a 4:2:0 frame has an even width" % (what, w))
+    return rows // 3 * 2, w
+
+
+def _image_size(shape, layout: int) -> Tuple[int, int]:
+    """(H, W) of a checked frame of the given layout: (H, W, 3) BGR or (H * 3/2, W) YUV 4:2:0."""
+    return (int(shape[0]), int(shape[1])) if not layout else (int(shape[0]) // 3 * 2, int(shape[1]))
+
+
+def _frame_list(frames, device: int, layout: int = 0):
+    """A list or tuple of (H_i, W_i, 3) uint8 frames (YUV layouts: (H_i * 3/2, W_i)), all numpy arrays or all contiguous CUDA
+    tensors on ``device`` -> (list of C-contiguous frames, whether they are on the device).  Raises ValueError otherwise."""
     frames = list(frames)
     dev = [_is_device(f) for f in frames]
     if any(dev) and not all(dev):
@@ -64,17 +90,19 @@ def _frame_list(frames, device: int):
             if f.dtype != np.uint8:
                 raise ValueError("frame %d: frames must be uint8, not %s" % (i, f.dtype))
             f = np.ascontiguousarray(f)
-        if len(f.shape) != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
+        if layout:
+            _yuv_image_size(f.shape, "frame %d" % i)
+        elif len(f.shape) != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
             raise ValueError("frame %d: frames must be (H, W, 3) uint8, not %s" % (i, tuple(f.shape)))
         out.append(f)
     return out, bool(dev) and dev[0]
 
 
-def _frame_table(frames):
-    """Frames of a list -> the ragged entries' arguments: a ctypes array of their addresses and their (H, W) as int32 pairs
-    (keep both alive over the call)."""
+def _frame_table(frames, layout: int = 0):
+    """Frames of a list -> the ragged entries' arguments: a ctypes array of their addresses and their image sizes (H, W) as
+    int32 pairs (keep both alive over the call)."""
     ptrs = (C.c_void_p * len(frames))(*(_ptr(f).value for f in frames))
-    hw = np.array([f.shape[:2] for f in frames], np.int32).reshape(-1)
+    hw = np.array([_image_size(f.shape, layout) for f in frames], np.int32).reshape(-1)
     return ptrs, hw
 
 
@@ -135,16 +163,21 @@ class YOLO:
         a = np.asarray(image.convert("RGB") if hasattr(image, "convert") else image)
         return self._detect(a[None], swap_rb=False)[0]
 
-    def detect_frames(self, frames_bgr) -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
+    def detect_frames(self, frames_bgr, *, pixel_format: str = "bgr") -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
         """A batch of BGR frames of one size (n, H, W, 3) uint8, numpy or a CUDA tensor -> one detect() tuple per frame.
 
         ``frames_bgr`` may also be a list or tuple of (H_i, W_i, 3) uint8 BGR frames of any sizes, all numpy arrays or all
         contiguous CUDA tensors on the detector's device.  Frames of one size are stacked and run as the batch above; frames of
         several sizes run ``max_frames`` at a time through ``whenet_det_detect_ragged_u8``, each letterboxed on its own, and
-        each frame's tuple is what ``detect_frames`` gives that frame alone."""
+        each frame's tuple is what ``detect_frames`` gives that frame alone.
+
+        ``pixel_format="nv12"`` or ``"i420"`` takes YUV 4:2:0 video frames in cv2's layout instead: (n, H * 3/2, W) uint8, or a
+        list or tuple of (H_i * 3/2, W_i) frames, H and W even.  The letterbox converts each pixel as it reads it, and the
+        result is the bits ``detect_frames`` gives on ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12 / _I420)``."""
+        layout = _pixel_layout(pixel_format)
         if not isinstance(frames_bgr, (list, tuple)):
-            return self._detect(frames_bgr, swap_rb=True)
-        frames, dev = _frame_list(frames_bgr, self.device)
+            return self._detect(frames_bgr, swap_rb=True, layout=layout)
+        frames, dev = _frame_list(frames_bgr, self.device, layout)
         if not frames:
             return []
         if len({tuple(f.shape) for f in frames}) == 1:
@@ -153,34 +186,43 @@ class YOLO:
                 with torch.cuda.device(self.device):
                     stacked = torch.stack(frames)
                     torch.cuda.current_stream().synchronize()   # the detector copies it on its own stream
-                return self._detect(stacked, swap_rb=True)
-            return self._detect(np.stack(frames), swap_rb=True)
+                return self._detect(stacked, swap_rb=True, layout=layout)
+            return self._detect(np.stack(frames), swap_rb=True, layout=layout)
         out = []
         for off in range(0, len(frames), self.max_frames):
-            out += self._detect_ragged(frames[off:off + self.max_frames], dev)
+            out += self._detect_ragged(frames[off:off + self.max_frames], dev, layout=layout)
         return out
 
-    def _detect_ragged(self, frames, dev: bool, max_boxes: int = 20):
+    def _detect_ragged(self, frames, dev: bool, max_boxes: int = 20, layout: int = 0):
         nb = len(frames)
-        ptrs, hw = _frame_table(frames)
+        ptrs, hw = _frame_table(frames, layout)
         slots = self.num_classes * max_boxes
         boxes = np.empty((nb, slots, 4), np.float32)
         scores = np.empty((nb, slots), np.float32)
         classes = np.empty((nb, slots), np.int32)
         counts = np.empty((nb,), np.int32)
-        check(self._L.whenet_det_detect_ragged_u8(self._h, C.addressof(ptrs), _ptr(hw), nb, int(dev), 1, self.score, self.iou, max_boxes,
-                                                  _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
+        fn = self._L.whenet_det_detect_ragged_yuv_u8 if layout else self._L.whenet_det_detect_ragged_u8
+        check(fn(self._h, C.addressof(ptrs), _ptr(hw), nb, int(dev), layout or 1, self.score, self.iou, max_boxes,
+                 _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
         return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(nb)]
 
-    def _detect(self, frames, swap_rb: bool, max_boxes: int = 20):
+    def _detect(self, frames, swap_rb: bool, max_boxes: int = 20, layout: int = 0):
         dev = _is_device(frames)
         if not dev:
             frames = np.ascontiguousarray(frames, dtype=np.uint8)
         elif not frames.is_contiguous() or str(frames.dtype) != "torch.uint8":
             raise ValueError("device frames must be a contiguous uint8 CUDA tensor")
-        if len(frames.shape) != 4 or frames.shape[3] != 3:
+        if layout:
+            if len(frames.shape) != 3:
+                raise ValueError("frames must be (n, H * 3/2, W) uint8 for a 4:2:0 pixel format, not %s" % (tuple(frames.shape),))
+            H, W = _yuv_image_size(frames.shape[1:], "a frame")
+            n = int(frames.shape[0])
+            entry, code = "whenet_det_detect_yuv_u8", layout
+        elif len(frames.shape) != 4 or frames.shape[3] != 3:
             raise ValueError("frames must be (n, H, W, 3) uint8")
-        n, H, W = (int(v) for v in frames.shape[:3])
+        else:
+            n, H, W = (int(v) for v in frames.shape[:3])
+            entry, code = "whenet_det_detect_u8", int(swap_rb)
         out = []
         for off in range(0, n, self.max_frames):
             nb = min(self.max_frames, n - off)
@@ -189,8 +231,8 @@ class YOLO:
             scores = np.empty((nb, slots), np.float32)
             classes = np.empty((nb, slots), np.int32)
             counts = np.empty((nb,), np.int32)
-            check(self._L.whenet_det_detect_u8(self._h, _ptr(frames[off:off + nb]), nb, H, W, int(dev), int(swap_rb), self.score, self.iou,
-                                               max_boxes, _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
+            check(getattr(self._L, entry)(self._h, _ptr(frames[off:off + nb]), nb, H, W, int(dev), code, self.score, self.iou, max_boxes,
+                                          _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
             for i in range(nb):
                 k = int(counts[i])
                 out.append((boxes[i, :k].copy(), scores[i, :k].copy(), classes[i, :k].copy()))

@@ -35,6 +35,14 @@ extern "C" {
 #define WHENET_PRECISION_BF16  1   /* bf16 activations, fp32 accumulate: the throughput mode  */
 #define WHENET_PRECISION_FP16  2   /* fp16 activations, fp32 accumulate                       */
 
+/* Planar YUV 4:2:0 video frames (the *_yuv_u8 entries): cv2's contiguous (H * 3/2) x W uint8 layout, H and W even - the
+ * H x W Y plane, then for NV12 one (H/2) x W plane of interleaved U, V pairs (U first), for I420 the (H/2) x (W/2) U plane
+ * followed by the (H/2) x (W/2) V plane.  Each pixel is converted as it is read with cv2.cvtColor's COLOR_YUV2BGR_NV12 /
+ * COLOR_YUV2BGR_I420 arithmetic (BT.601 limited range, 20-bit fixed point), so every result is the bits the BGR entry gives
+ * on cvtColor's output. */
+#define WHENET_YUV_NV12        1
+#define WHENET_YUV_I420        2
+
 #define WHENET_IMG        224
 #define WHENET_N_YAW      120      /* reference whenet.py:11 */
 #define WHENET_N_PITCH     66      /* reference whenet.py:12 */
@@ -141,6 +149,18 @@ int whenet_crop_boxes_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, i
 int whenet_crop_boxes_ragged_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
                                 const float* boxes, const int32_t* frame_of, int m, int swap_rb,
                                 uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+
+/* whenet_crop_boxes_u8 and whenet_crop_boxes_ragged_u8 on YUV 4:2:0 frames (WHENET_YUV_NV12 / WHENET_YUV_I420 in
+ * `yuv_layout`, in place of swap_rb): H, W and hw are the image sizes (each side even, at most 16384), each frame is
+ * H * W * 3/2 bytes.  The margin arithmetic and validity are those of the BGR entries; each crop is RGB, the bytes the BGR
+ * entry with swap_rb gives on cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420).  Every argument but the context is checked
+ * before anything touches a device. */
+int whenet_crop_boxes_yuv_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, int W, int frames_are_device,
+                             const float* boxes, const int32_t* frame_of, int m, int yuv_layout,
+                             uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+int whenet_crop_boxes_ragged_yuv_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                    const float* boxes, const int32_t* frame_of, int m, int yuv_layout,
+                                    uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
 
 /* Block until everything queued by this context has finished. */
 int whenet_synchronize(whenet_ctx* ctx);
@@ -275,6 +295,17 @@ int whenet_det_detect_u8(whenet_det* det, const uint8_t* frames, int n, int H, i
 int whenet_det_detect_ragged_u8(whenet_det* det, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
                                 int swap_rb, float score, float iou, int max_boxes,
                                 float* boxes, float* scores, int32_t* classes, int32_t* counts);
+
+/* whenet_det_detect_u8 and whenet_det_detect_ragged_u8 on YUV 4:2:0 frames (WHENET_YUV_NV12 / WHENET_YUV_I420 in
+ * `yuv_layout`, in place of swap_rb): H, W and hw are the image sizes (each side even, 2..16384), each frame is H * W * 3/2
+ * bytes.  The letterbox converts each source pixel as it reads it; everything after it is the BGR path's, and the outputs are
+ * the bits the BGR entry with swap_rb gives on cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420).  The graph caches key on the
+ * layout too.  Every argument but the detector (and n against its max_frames) is checked before anything touches a device. */
+int whenet_det_detect_yuv_u8(whenet_det* det, const uint8_t* frames, int n, int H, int W, int frames_are_device, int yuv_layout,
+                             float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
+int whenet_det_detect_ragged_yuv_u8(whenet_det* det, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                    int yuv_layout, float score, float iou, int max_boxes,
+                                    float* boxes, float* scores, int32_t* classes, int32_t* counts);
 
 /* Block until everything queued by this detector has finished. */
 int whenet_det_synchronize(whenet_det* det);
