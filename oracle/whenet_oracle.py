@@ -243,6 +243,147 @@ class Oracle:
                 block_in = x   # stem output feeds block 1 (never added: Cin != Cout)
         return [outs["yaw_new"], outs["pitch_new"], outs["roll_new"]]
 
+    # -- one stage at a time -------------------------------------------------
+    def stage_layers(self) -> Dict[str, object]:
+        """The layer names of every stage, from the same ``layer_names`` walk as the forward.
+
+        Returns ``{"stem": (conv, bn), "blocks": [ {expand: (conv, bn) | None, dw, dw_bn, stride, se: [conv, conv],
+        proj, proj_bn, skip}, ... ], "head": (conv, bn)}``."""
+        stem = head = pend = None
+        blocks: List[dict] = []
+        cur: Optional[dict] = None
+        pend_conv = None
+        in_se = 0
+        for name in self.layer_names:
+            m = re.match(r"([a-z_0-9]+?)_(\d+)$", name)
+            kind, num = (m.group(1), int(m.group(2))) if m else (name, 0)
+            if kind == "conv2d":
+                if in_se:
+                    cur["se"].append(name)
+                    in_se -= 1
+                elif cur is not None and cur["proj"] is None:
+                    cur["proj"] = name
+                else:
+                    pend_conv = name
+            elif kind == "batch_normalization":
+                if stem is None:
+                    stem, pend_conv = (pend_conv, name), None
+                elif cur is not None and cur["proj"] is not None and cur["proj_bn"] is None:
+                    cur["proj_bn"] = name
+                elif cur is not None and cur["dw_bn"] is None:
+                    cur["dw_bn"] = name
+                else:
+                    pend, pend_conv = (pend_conv, name), None
+            elif kind == "depthwise_conv2d":
+                cur = {"expand": pend, "dw": name, "dw_bn": None, "stride": 2 if num in DW_STRIDE2 else 1,
+                       "se": [], "proj": None, "proj_bn": None, "skip": False}
+                blocks.append(cur)
+                pend = None
+            elif kind == "lambda":
+                in_se = 2
+            elif kind == "add":
+                cur["skip"] = True
+        head = pend
+        return {"stem": stem, "blocks": blocks, "head": head}
+
+    def _fold(self, conv: str, bn: str, kernel: str = "/kernel:0"):
+        """BN folded into the preceding conv in float64: (kernel * scale, shift)."""
+        w = self.w
+        scale = w[bn + "/gamma:0"] / np.sqrt(w[bn + "/moving_variance:0"] + self.bn_eps)
+        shift = w[bn + "/beta:0"] - w[bn + "/moving_mean:0"] * scale
+        k = w[conv + kernel]
+        return k * (scale if kernel == "/kernel:0" else scale[:, None]), shift
+
+    def run_stage(self, stage: str, x: np.ndarray, block: int = 0, gate: Optional[np.ndarray] = None,
+                  resid: Optional[np.ndarray] = None, symmetric_pad: Optional[bool] = None) -> Dict[str, np.ndarray]:
+        """One stage of the network on a given input, every weight folded and applied in ``self.dtype``.
+
+        Returns the stage's intermediate values and the matching sums of absolute terms (``S_*``), which an
+        error bound of the same arithmetic in another precision needs.  NHWC throughout.
+
+        * ``"stem"``:    x = normalised image (N,224,224,3) -> ``pre``, ``S``, ``out`` = swish(pre)
+        * ``"dw"``:      x = block input (the stem output for block 1); ``block`` = 1..16 ->
+                         [``pre_e``, ``S_e``, ``X_e`` (sum |x|), ``shift_e``, ``e``] for blocks with an expand conv, then
+                         ``pre``, ``S`` (sum |e w|), ``X`` (sum |e| over the window), ``w`` (folded depthwise kernel,
+                         (k,k,C)), ``shift``, ``out``
+        * ``"gate"``:    x = depthwise output -> ``mean``, ``z1``, ``S_z1``, ``a``, ``z2``, ``S_z2``, ``w1``, ``w2``, ``out``
+        * ``"project"``: x = depthwise output, ``gate`` (N,C), ``resid`` = block input or None -> ``pre``, ``S``,
+                         ``X`` (sum |x g|), ``shift``, ``out``
+        * ``"head"``:    x = block 16 output -> ``pre``, ``S``, ``X``, ``shift``, ``out``
+        * ``"dense"``:   x = pooled features (N,1280) -> ``logits`` (three arrays), ``S`` (three arrays)
+        """
+        sym = self.symmetric_pad if symmetric_pad is None else bool(symmetric_pad)
+        L = self.stage_layers()
+        x = np.asarray(x, dtype=self.dtype)
+        w = self.w
+        r: Dict[str, np.ndarray] = {}
+        if stage == "stem":
+            conv, bn = L["stem"]
+            k, sh = self._fold(conv, bn)
+            r["pre"] = conv2d_same(x, k, 2, sym) + sh
+            r["S"] = conv2d_same(np.abs(x), np.abs(k), 2, sym) + np.abs(sh)
+            r["out"] = swish(r["pre"])
+            return r
+        if stage in ("dw", "gate", "project"):
+            b = L["blocks"][block - 1]
+        if stage == "dw":
+            if b["expand"] is not None:
+                k, sh = self._fold(*b["expand"])
+                c = k.shape[-1]
+                r["pre_e"] = x.reshape(-1, x.shape[-1]) @ k.reshape(-1, c) + sh
+                r["S_e"] = np.abs(x).reshape(-1, x.shape[-1]) @ np.abs(k).reshape(-1, c)
+                r["X_e"] = np.abs(x).sum(axis=-1).reshape(x.shape[:3] + (1,))
+                r["pre_e"] = r["pre_e"].reshape(x.shape[:3] + (c,))
+                r["S_e"] = r["S_e"].reshape(x.shape[:3] + (c,))
+                r["shift_e"] = sh
+                x = r["e"] = swish(r["pre_e"])
+            k, sh = self._fold(b["dw"], b["dw_bn"], "/depthwise_kernel:0")
+            r["w"] = k[:, :, :, 0]
+            r["shift"] = sh
+            r["pre"] = depthwise_same(x, k, b["stride"], sym) + sh
+            r["S"] = depthwise_same(np.abs(x), np.abs(k), b["stride"], sym)
+            r["X"] = depthwise_same(np.abs(x), np.ones_like(k), b["stride"], sym)
+            r["out"] = swish(r["pre"])
+            return r
+        if stage == "gate":
+            c1, c2 = b["se"]
+            w1, b1 = w[c1 + "/kernel:0"][0, 0], w[c1 + "/bias:0"]
+            w2, b2 = w[c2 + "/kernel:0"][0, 0], w[c2 + "/bias:0"]
+            r["mean"] = x.mean(axis=(1, 2))
+            r["z1"] = r["mean"] @ w1 + b1
+            r["S_z1"] = np.abs(r["mean"]) @ np.abs(w1) + np.abs(b1)
+            r["a"] = swish(r["z1"])
+            r["z2"] = r["a"] @ w2 + b2
+            r["S_z2"] = np.abs(r["a"]) @ np.abs(w2) + np.abs(b2)
+            r["out"] = _sigmoid(r["z2"])
+            r["w1"], r["w2"] = w1, w2
+            return r
+        if stage == "project":
+            k, sh = self._fold(b["proj"], b["proj_bn"])
+            k = k[0, 0]
+            xg = x * gate[:, None, None, :]
+            r["pre"] = (xg.reshape(-1, k.shape[0]) @ k).reshape(x.shape[:3] + (k.shape[1],)) + sh
+            r["S"] = (np.abs(xg).reshape(-1, k.shape[0]) @ np.abs(k)).reshape(r["pre"].shape) + np.abs(sh)
+            r["X"] = np.abs(xg).sum(axis=-1)[..., None]
+            r["shift"] = sh
+            r["out"] = r["pre"] + (resid if resid is not None else 0.0)
+            return r
+        if stage == "head":
+            k, sh = self._fold(*L["head"])
+            k = k[0, 0]
+            r["pre"] = (x.reshape(-1, k.shape[0]) @ k).reshape(x.shape[:3] + (k.shape[1],)) + sh
+            r["S"] = (np.abs(x).reshape(-1, k.shape[0]) @ np.abs(k)).reshape(r["pre"].shape)
+            r["X"] = np.abs(x).sum(axis=-1)[..., None]
+            r["shift"] = sh
+            r["out"] = swish(r["pre"])
+            return r
+        if stage == "dense":
+            names = ("yaw_new", "pitch_new", "roll_new")
+            r["logits"] = [x @ w[n + "/kernel:0"] + w[n + "/bias:0"] for n in names]
+            r["S"] = [np.abs(x) @ np.abs(w[n + "/kernel:0"]) + np.abs(w[n + "/bias:0"]) for n in names]
+            return r
+        raise ValueError("unknown stage %r" % stage)
+
     # -- the reference surface -----------------------------------------------
     def predict(self, img_normalised, taps=None):
         return self.forward_normalised(img_normalised, taps)
