@@ -18,6 +18,7 @@ EXPORTS = [
     "whenet_det_synchronize", "whenet_det_destroy", "whenet_det_debug_tap", "whenet_det_debug_conv", "whenet_det_debug_maxpool",
     "whenet_det_debug_decode", "whenet_det_create_ex", "whenet_det_precision", "whenet_det_detect_ragged_u8", "whenet_crop_boxes_ragged_u8",
     "whenet_det_detect_yuv_u8", "whenet_det_detect_ragged_yuv_u8", "whenet_crop_boxes_yuv_u8", "whenet_crop_boxes_ragged_yuv_u8",
+    "whenet_det_create_large", "whenet_det_debug_force_large_decode",
 ]
 
 # pixel_format -> the ABI's yuv_layout (WHENET_YUV_NV12 / WHENET_YUV_I420); "bgr" is packed 8-bit BGR, the *_u8 entries
@@ -102,6 +103,8 @@ def load():
     I = C.c_int
     L.whenet_det_create.argtypes = [C.POINTER(P), I, I, I, I]
     L.whenet_det_create_ex.argtypes = [C.POINTER(P), I, I, I, I, I]
+    L.whenet_det_create_large.argtypes = [C.POINTER(P), I, I, I, I, I]
+    L.whenet_det_debug_force_large_decode.argtypes = [P, I]
     L.whenet_det_precision.argtypes = [P]
     L.whenet_det_load_weights.argtypes = [P, C.POINTER(Tensor), I, P, I]
     L.whenet_det_num_classes.argtypes = [P]

@@ -80,7 +80,7 @@ int launch_igemm_m(cudaStream_t s, const IgemmParams& p, int un, size_t smem, in
     return (int)cudaErrorInvalidValue;
 }
 
-int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
+int launch_igemm_mode(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
     switch (mode) {
         case kLeaky: return launch_igemm_m<kLeaky>(s, p, un, smem, grid_n, grid_m);
         case kLeakyRes: return launch_igemm_m<kLeakyRes>(s, p, un, smem, grid_n, grid_m);
@@ -90,8 +90,36 @@ int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t 
     return (int)cudaErrorInvalidValue;
 }
 
-int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n) {
-    yolo_decode_nms_kernel<<<n, kNmsThreads, 0, s>>>(p);
+// More M tiles than gridDim.y holds: one launch per group of whole frames (igemm_group_frames), each with its frames' in, up,
+// resid and out.  A frame's tiles and their results do not depend on the frames around it.
+// grid_m: the tiles of all p.M rows.  One group (every call that fits) launches p itself.
+int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
+    const long long hw = (long long)p.Ho * p.Wo;
+    const size_t out_elem = mode == kLinearF32 ? 4 : 2;
+    return for_each_frame_group((int)(p.M / hw), hw, [&](int f0, int nf) {
+        if (nf * hw == p.M) return launch_igemm_mode(s, p, mode, un, smem, grid_n, grid_m);
+        IgemmParams q = p;
+        q.in = p.in + (size_t)f0 * p.Hi * p.Wi * (p.Cin - p.c_up);
+        if (p.up) q.up = p.up + (size_t)f0 * (p.Hi / 2) * (p.Wi / 2) * p.c_up;
+        if (p.resid) q.resid = p.resid + (size_t)f0 * hw * p.N;
+        q.out = (char*)p.out + (size_t)f0 * hw * p.N * out_elem;
+        q.M = (int)(nf * hw);
+        return launch_igemm_mode(s, q, mode, un, smem, grid_n, (q.M + BM - 1) / BM);
+    });
+}
+
+int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n, bool force_large, unsigned long long* keep, int* keep_count) {
+    if (!force_large && !large_decode_route(p.NC)) {
+        yolo_decode_nms_kernel<<<n, kNmsThreads, 0, s>>>(p);
+        return (int)cudaGetLastError();
+    }
+    if (!keep || !keep_count || p.NC > kMaxCandidates) return (int)cudaErrorInvalidValue;
+    const int alive_bytes = (p.NC + 31) / 32 * 4;
+    cudaError_t e = cudaFuncSetAttribute(yolo_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLargeAliveBytes);
+    if (e != cudaSuccess) return (int)e;
+    yolo_decode_kernel<<<dim3((p.NC + 255) / 256, n), 256, 0, s>>>(p);
+    yolo_nms_kernel<<<dim3(p.C, n), kNmsThreads, alive_bytes, s>>>(p, keep, keep_count);
+    yolo_pack_kernel<<<n, 256, 0, s>>>(p, keep, keep_count);
     return (int)cudaGetLastError();
 }
 

@@ -50,7 +50,7 @@ int launch_igemm32_m(cudaStream_t s, const Igemm32Params& p, int un, size_t smem
     return (int)cudaErrorInvalidValue;
 }
 
-int launch_igemm32(cudaStream_t s, const Igemm32Params& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
+int launch_igemm32_mode(cudaStream_t s, const Igemm32Params& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
     switch (mode) {
         case kLeaky: return launch_igemm32_m<kLeaky>(s, p, un, smem, grid_n, grid_m);
         case kLeakyRes: return launch_igemm32_m<kLeakyRes>(s, p, un, smem, grid_n, grid_m);
@@ -58,6 +58,21 @@ int launch_igemm32(cudaStream_t s, const Igemm32Params& p, int mode, int un, siz
         case kLinearF32: return launch_igemm32_m<kLinearF32>(s, p, un, smem, grid_n, grid_m);
     }
     return (int)cudaErrorInvalidValue;
+}
+
+// launch_igemm's split into groups of whole frames past gridDim.y's limit; every tensor is fp32 here
+int launch_igemm32(cudaStream_t s, const Igemm32Params& p, int mode, int un, size_t smem, int grid_n, int grid_m) {
+    const long long hw = (long long)p.Ho * p.Wo;
+    return for_each_frame_group((int)(p.M / hw), hw, [&](int f0, int nf) {
+        if (nf * hw == p.M) return launch_igemm32_mode(s, p, mode, un, smem, grid_n, grid_m);
+        Igemm32Params q = p;
+        q.in = p.in + (size_t)f0 * p.Hi * p.Wi * (p.Cin - p.c_up);
+        if (p.up) q.up = p.up + (size_t)f0 * (p.Hi / 2) * (p.Wi / 2) * p.c_up;
+        if (p.resid) q.resid = p.resid + (size_t)f0 * hw * p.N;
+        q.out = p.out + (size_t)f0 * hw * p.N;
+        q.M = (int)(nf * hw);
+        return launch_igemm32_mode(s, q, mode, un, smem, grid_n, (q.M + BM - 1) / BM);
+    });
 }
 
 }  // namespace yolo

@@ -14,6 +14,8 @@
 //                                             zero-filled (= the padding); concat convs read [upsample(up), skip] virtually
 //   yolo_maxpool_kernel                        tiny YOLOv3's 2x2 max-pools (stride 2, or stride 1 with TF SAME padding)
 //   yolo_decode_nms_kernel                     one CTA per frame: decode every candidate, per-class score mask, greedy NMS
+//   yolo_decode_kernel / yolo_nms_kernel /     the same past kNmsPer x kNmsThreads candidates (model inputs above 608): decode over
+//   yolo_pack_kernel                           (candidate blocks x frames), NMS per (class, frame), pack per frame
 //
 // Storage bf16 NHWC, fp32 accumulation; the output convs write fp32.
 #pragma once
@@ -148,6 +150,31 @@ constexpr int kNmsThreads = 1024;
 constexpr int kNmsPer = 24;             // candidates per thread: 24 x 1024 >= 22,743 (608 x 608)
 constexpr int kMaxBoxes = 256;
 
+// The decode + NMS route for more candidates than yolo_decode_nms_kernel holds (kNmsPer * kNmsThreads): one alive bit per
+// candidate in shared memory, up to the 1,032,192 candidates of YOLOv3 at 4096 x 4096 (126 KB).
+constexpr int kMaxSide = 4096;          // whenet_det_create_large's largest input side
+constexpr int kMaxCandidates = 3 * (kMaxSide / 32) * (kMaxSide / 32) * 21;
+constexpr int kLargeAliveBytes = kMaxCandidates / 32 * 4;
+inline bool large_decode_route(int NC) { return NC > kNmsPer * kNmsThreads; }
+
+// Conv launches put the M tiles on gridDim.y, which holds at most 65,535.  A call with more tiles runs as groups of whole frames,
+// this many frames (of hw output pixels each) per group; one frame needs at most 32,768 tiles (conv 1 at 4096 x 4096).
+constexpr int kMaxGridY = 65535;
+inline int igemm_group_frames(long long hw) {
+    const long long g = (long long)kMaxGridY * BM / hw;
+    return g < 1 ? 1 : g > (1 << 30) ? (1 << 30) : (int)g;
+}
+// The launches of a conv over n frames of hw output pixels: fn(f0, nf) for each group of nf frames from frame f0 (one group of
+// all n while their tiles fit gridDim.y); stops at and returns the first nonzero fn result.  launch_igemm, launch_igemm32 and
+// tools/yolo_plan_dump.cu all go through it.
+template <class Fn>
+int for_each_frame_group(int n, long long hw, Fn&& fn) {
+    const int g = ((long long)n * hw + BM - 1) / BM <= kMaxGridY ? n : igemm_group_frames(hw);
+    for (int f0 = 0; f0 < n; f0 += g)
+        if (int rc = fn(f0, n - f0 < g ? n - f0 : g)) return rc;
+    return 0;
+}
+
 constexpr int kMaxFrames = 64;          // frames per detector call (whenet_det_create's max_frames)
 
 // yolo_correct_boxes (model.py:159-161) of one frame, float32 on the host
@@ -199,7 +226,9 @@ int launch_conv0(cudaStream_t s, const uint8_t* img, const __nv_bfloat16* w0, co
                  int cout);
 int launch_igemm(cudaStream_t s, const IgemmParams& p, int mode, int un, size_t smem, int grid_n, int grid_m);
 int launch_maxpool(cudaStream_t s, const __nv_bfloat16* in, __nv_bfloat16* out, int n, int H, int W, int C, int stride);
-int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n);
+// The one-CTA kernel when NC <= kNmsPer * kNmsThreads, else (or with force_large) decode / NMS / pack.  The second route keeps
+// each (frame, class)'s kept keys in keep ([n][C][kMaxBoxes]) and their count in keep_count ([n][C]); it needs both.
+int launch_decode_nms(cudaStream_t s, const DecodeParams& p, int n, bool force_large, unsigned long long* keep, int* keep_count);
 
 #ifndef WHENET_YOLO_HOST_ONLY
 // ----------------------------------------------------------------------------- letterbox
@@ -641,6 +670,32 @@ __device__ __forceinline__ float iou_tf(float4 a, float4 b) {
     return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
 }
 
+// Decode candidate i of frame f (model.py:125-187; candidates ordered layer 0, 1 (, 2), then (y, x, anchor)) with the frame's
+// yolo_correct_boxes row g: its box to cand[i], its class scores to cscore[c * NC + i].  yolo_decode_kernel's body; the loop of
+// yolo_decode_nms_kernel does the same operations in the same order.
+__device__ __forceinline__ void decode_candidate(const DecodeParams& p, const FrameGeo& g, int f, int i, float4* cand, float* cscore) {
+    const int CH = 5 + p.C;
+    int l = 0, rem = i;
+    int gh = p.gh0, gw = p.gw0;
+    while (rem >= 3 * gh * gw) { rem -= 3 * gh * gw; ++l; gh *= 2; gw *= 2; }
+    const int cell = rem / 3, a = rem - cell * 3;
+    const int y = cell / gw, x = cell - y * gw;
+    const float* t = p.head[l] + (((long long)f * gh + y) * gw + x) * 3 * CH + a * CH;
+    const int an = 3 * l + a;                                           // the host put anchor_mask[l][a] in this slot
+    const float bx = __fdiv_rn(__fadd_rn(sigmoidf_(t[0]), (float)x), (float)gw);
+    const float by = __fdiv_rn(__fadd_rn(sigmoidf_(t[1]), (float)y), (float)gh);
+    const float bw = __fdiv_rn(__fmul_rn(expf(t[2]), p.anchors[2 * an]), p.in_w);
+    const float bh = __fdiv_rn(__fmul_rn(expf(t[3]), p.anchors[2 * an + 1]), p.in_h);
+    // yolo_correct_boxes (model.py:153-176)
+    const float yc = __fmul_rn(__fsub_rn(by, g.off_y), g.scale_y), xc = __fmul_rn(__fsub_rn(bx, g.off_x), g.scale_x);
+    const float hh = __fmul_rn(bh, g.scale_y), ww = __fmul_rn(bw, g.scale_x);
+    const float hh2 = __fdiv_rn(hh, 2.0f), ww2 = __fdiv_rn(ww, 2.0f);
+    cand[i] = make_float4(__fmul_rn(__fsub_rn(yc, hh2), g.img_h), __fmul_rn(__fsub_rn(xc, ww2), g.img_w),
+                          __fmul_rn(__fadd_rn(yc, hh2), g.img_h), __fmul_rn(__fadd_rn(xc, ww2), g.img_w));
+    const float conf = sigmoidf_(t[4]);
+    for (int c = 0; c < p.C; ++c) cscore[(long long)c * p.NC + i] = __fmul_rn(conf, sigmoidf_(t[5 + c]));
+}
+
 __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __grid_constant__ DecodeParams p) {
     const int f = blockIdx.x, tid = threadIdx.x;
     const int CH = 5 + p.C;
@@ -651,7 +706,8 @@ __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __gr
     __syncthreads();
     float4* cand = p.cand + (long long)f * p.NC;
     float* cscore = p.cand_score + (long long)f * p.C * p.NC;
-    // ---- decode (model.py:125-187): candidates ordered layer 0, 1 (, 2), then (y, x, anchor)
+    // ---- decode (model.py:125-187): decode_candidate's operations, kept inline here because calling it changes this kernel's
+    // register allocation
     for (int i = tid; i < p.NC; i += kNmsThreads) {
         int l = 0, rem = i;
         int gh = p.gh0, gw = p.gw0;
@@ -738,6 +794,116 @@ __global__ void __launch_bounds__(kNmsThreads) yolo_decode_nms_kernel(const __gr
         kept_total += kept;
     }
     if (tid == 0) p.out_count[f] = kept_total;
+}
+
+// ----------------------------------------------------------------------------- decode + NMS past kNmsPer * kNmsThreads candidates
+// Three kernels with yolo_decode_nms_kernel's arithmetic, keys and order: the decode over (candidate blocks x frames), greedy NMS
+// per (class, frame) with one alive bit per candidate in shared memory, and the pack into the outputs' class-by-class layout.
+__global__ void __launch_bounds__(256) yolo_decode_kernel(const __grid_constant__ DecodeParams p) {
+    const int f = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= p.NC) return;
+    const FrameGeo g = p.geo[f];
+    decode_candidate(p, g, f, i, p.cand + (long long)f * p.NC, p.cand_score + (long long)f * p.C * p.NC);
+}
+
+// The largest key of the CTA (kNmsThreads threads) to every thread
+__device__ __forceinline__ unsigned long long block_max_key(unsigned long long v, unsigned long long* s_red, unsigned long long* s_best) {
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
+        v = u > v ? u : v;
+    }
+    if ((tid & 31) == 0) s_red[tid >> 5] = v;
+    __syncthreads();
+    if (tid < 32) {
+        v = s_red[tid];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
+            v = u > v ? u : v;
+        }
+        if (tid == 0) *s_best = v;
+    }
+    __syncthreads();
+    v = *s_best;
+    __syncthreads();                                                // s_red / s_best are rewritten by the next call
+    return v;
+}
+
+// Greedy NMS of class blockIdx.x of frame blockIdx.y.  Alive word w (dynamic shared memory) holds candidates 32w .. 32w + 31;
+// thread t owns words t, t + kNmsThreads, ... and alone clears their bits.  Each round suppresses against the box just kept and
+// finds the next largest key among the survivors in the same pass.  Kept keys go to keep[(f * C + c) * kMaxBoxes + k].
+__global__ void __launch_bounds__(kNmsThreads) yolo_nms_kernel(const __grid_constant__ DecodeParams p, unsigned long long* __restrict__ keep,
+                                                               int* __restrict__ keep_count) {
+    extern __shared__ uint32_t s_alive[];
+    __shared__ unsigned long long s_red[kNmsThreads / 32];
+    __shared__ unsigned long long s_best;
+    const int c = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
+    const float4* cand = p.cand + (long long)f * p.NC;
+    const float* sc = p.cand_score + ((long long)f * p.C + c) * p.NC;
+    const int nw = (p.NC + 31) >> 5;
+    // the class mask (model.py:211: score >= threshold), one coalesced ballot per word
+    for (int w = tid >> 5; w < nw; w += kNmsThreads / 32) {
+        const int i = w * 32 + lane;
+        const uint32_t b = __ballot_sync(0xffffffffu, i < p.NC && sc[i] >= p.score);
+        if (lane == 0) s_alive[w] = b;
+    }
+    __syncthreads();
+    // scores are >= 0: their float bits order like the floats; ~i makes the lower index win a tie
+    auto key = [&](int i) { return ((unsigned long long)__float_as_uint(sc[i]) << 32) | (unsigned)(~i); };
+    unsigned long long best = 0ull;
+    for (int w = tid; w < nw; w += kNmsThreads)
+        for (uint32_t b = s_alive[w]; b; b &= b - 1u) {
+            const unsigned long long k = key(w * 32 + __ffs(b) - 1);
+            best = k > best ? k : best;
+        }
+    unsigned long long* out = keep + ((long long)f * p.C + c) * kMaxBoxes;
+    int kept = 0;
+    while (kept < p.max_boxes) {
+        best = block_max_key(best, s_red, &s_best);
+        if (best == 0ull) break;
+        if (tid == 0) out[kept] = best;
+        if (++kept == p.max_boxes) break;
+        const int bi = (int)(~(unsigned)(best & 0xffffffffu));
+        const float4 bb = cand[bi];
+        best = 0ull;
+        for (int w = tid; w < nw; w += kNmsThreads) {
+            uint32_t a = s_alive[w];
+            for (uint32_t b = a; b; b &= b - 1u) {
+                const int j = __ffs(b) - 1, i = w * 32 + j;
+                if (i == bi || iou_tf(cand[i], bb) > p.iou) {
+                    a &= ~(1u << j);
+                } else {
+                    const unsigned long long k = key(i);
+                    best = k > best ? k : best;
+                }
+            }
+            s_alive[w] = a;
+        }
+    }
+    if (tid == 0) keep_count[f * p.C + c] = kept;
+}
+
+// frame blockIdx.x: its classes' kept boxes in order, class by class, and its count
+__global__ void __launch_bounds__(256) yolo_pack_kernel(const __grid_constant__ DecodeParams p, const unsigned long long* __restrict__ keep,
+                                                        const int* __restrict__ keep_count) {
+    const int f = blockIdx.x;
+    const float4* cand = p.cand + (long long)f * p.NC;
+    int base = 0;
+    for (int c = 0; c < p.C; ++c) {
+        const int k = keep_count[f * p.C + c];
+        const unsigned long long* kk = keep + ((long long)f * p.C + c) * kMaxBoxes;
+        for (int j = threadIdx.x; j < k; j += 256) {
+            const unsigned long long key = kk[j];
+            const long long o = (long long)f * p.C * p.max_boxes + base + j;
+            reinterpret_cast<float4*>(p.out_boxes)[o] = cand[(int)(~(unsigned)(key & 0xffffffffu))];
+            p.out_scores[o] = __uint_as_float((unsigned)(key >> 32));
+            p.out_classes[o] = c;
+        }
+        base += k;
+    }
+    if (threadIdx.x == 0) p.out_count[f] = base;
 }
 
 #endif  // WHENET_YOLO_HOST_ONLY

@@ -140,6 +140,9 @@ struct whenet_det {
     uint8_t* d_canvas = nullptr;
     float4* d_cand = nullptr; float* d_cand_score = nullptr;
     float* d_boxes = nullptr; float* d_scores = nullptr; int* d_classes = nullptr; int* d_count = nullptr;
+    // the second decode route's kept keys and counts ([max_frames][C][kMaxBoxes], [max_frames][C]), allocated on its first use
+    unsigned long long* d_keep = nullptr; int* d_keep_count = nullptr;
+    bool force_large_decode = false;    // whenet_det_debug_force_large_decode
     std::map<OneSizeKey, GraphEntry> graphs;
     std::map<RaggedKey, GraphEntry> ragged_graphs;      // whenet_det_detect_ragged_u8's
     int last_n = 0;
@@ -154,6 +157,54 @@ bool is_fp32(const whenet_det* d) { return d->precision == WHENET_PRECISION_FP32
 
 void free_layers(whenet_det* d) {
     for (auto& l : d->L) { cudaFree(l.out); cudaFree(l.pooled); l.out = l.pooled = nullptr; }
+}
+
+// the activations and every decode workspace (they are sized by the network, the class count and max_frames)
+void free_activations(whenet_det* d) {
+    free_layers(d);
+    cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
+    cudaFree(d->d_keep); cudaFree(d->d_keep_count);
+    d->d_cand = nullptr; d->d_cand_score = nullptr; d->d_boxes = nullptr; d->d_scores = nullptr; d->d_classes = nullptr; d->d_count = nullptr;
+    d->d_keep = nullptr; d->d_keep_count = nullptr;
+}
+
+// cudaMalloc that names the request when it fails.  The failed call's error is cleared, so that a later launch check does not
+// report it and the process goes on using the device.
+int dev_alloc(void** p, size_t bytes, const char* what) {
+    const cudaError_t e = cudaMalloc(p, bytes);
+    if (e == cudaSuccess) return 0;
+    *p = nullptr;
+    cudaGetLastError();
+    return fail(WHENET_ECUDA, "cudaMalloc of %zu bytes (%.1f GB) for %s failed: %s", bytes, bytes / 1e9, what, cudaGetErrorString(e));
+}
+template <class T>
+int dev_alloc(T** p, size_t bytes, const char* what) { return dev_alloc(reinterpret_cast<void**>(p), bytes, what); }
+
+// Bytes whenet_det_load_weights allocates per frame for network T (tiny: 13 convs) with C classes at an h x w model input:
+// every conv output, every pooled conv input, the decoded boxes and the class scores
+size_t activation_bytes_per_frame(const std::vector<ConvCfg>& T, bool tiny, int h, int w, int C, bool f32) {
+    std::vector<int> Ho(T.size()), Wo(T.size());
+    size_t b = 0;
+    for (size_t i = 0; i < T.size(); ++i) {
+        const ConvCfg& c = T[i];
+        const int Hi = Y::pooled(c.src < 0 ? h : Ho[c.src], c.pool), Wi = Y::pooled(c.src < 0 ? w : Wo[c.src], c.pool);
+        Ho[i] = Hi / c.stride; Wo[i] = Wi / c.stride;
+        const int N = c.head >= 0 ? 3 * (5 + C) : c.cout;
+        b += (size_t)Ho[i] * Wo[i] * N * (c.head >= 0 || f32 ? 4 : 2);
+        if (c.pool) b += (size_t)Hi * Wi * c.cin * (f32 ? 4 : 2);
+    }
+    const size_t nc = (size_t)3 * (h / 32) * (w / 32) * (tiny ? 5 : 21);
+    return b + nc * 16 + (size_t)C * nc * 4;
+}
+
+// A request larger than the whole device is refused before anything is allocated for it
+int check_fits(int device, size_t bytes, const char* what) {
+    size_t free_b = 0, total_b = 0;
+    CKD(cudaMemGetInfo(&free_b, &total_b));
+    if (bytes > total_b)
+        return fail(WHENET_ECUDA, "%s needs %zu bytes (%.1f GB) of device memory; device %d has %zu bytes (%.1f GB) in all", what, bytes, bytes / 1e9,
+                    device, total_b, total_b / 1e9);
+    return 0;
 }
 
 void free_entry(GraphEntry& e) {
@@ -284,7 +335,7 @@ int make_entry(whenet_det* d, int n, int H, int W, int swap_rb, int yuv_layout, 
     CKD(cudaMalloc(&e->coef, blob.size()));
     char* base = (char*)e->coef;
     CKD(cudaMemcpy(base, blob.data(), blob.size(), cudaMemcpyHostToDevice));
-    CKD(cudaMalloc(&e->tmp, (size_t)n * f.rows * f.nw * 3));
+    if (int rc = dev_alloc(&e->tmp, (size_t)n * f.rows * f.nw * 3, "the letterbox's horizontal pass")) return rc;
     Y::LetterboxPlan lp{H, W, f.nw, f.nh, f.ox, f.oy, f.y0, f.rows, f.ksx, f.ksy,
                         (const int2*)(base + f.xb), (const int*)(base + f.kx), (const int2*)(base + f.yb), (const int*)(base + f.ky)};
     return capture_forward(d, n, [&](cudaStream_t s) { return Y::launch_letterbox(s, lp, d->d_frames, e->tmp, d->d_canvas, n, d->in_h, d->in_w, swap_rb,
@@ -311,7 +362,7 @@ int make_ragged_entry(whenet_det* d, int n, const int32_t* hw, const std::vector
     std::memcpy(blob.data() + plans_at, plans.data(), plans.size() * sizeof(Y::LetterboxFrame));
     CKD(cudaMalloc(&e->coef, blob.size()));
     CKD(cudaMemcpy(e->coef, blob.data(), blob.size(), cudaMemcpyHostToDevice));
-    CKD(cudaMalloc(&e->tmp, tmp_bytes));
+    if (int rc = dev_alloc(&e->tmp, tmp_bytes, "the letterbox's horizontal pass")) return rc;
     const char* coef = (const char*)e->coef;
     const auto* d_plans = (const Y::LetterboxFrame*)(coef + plans_at);
     return capture_forward(d, n, [&](cudaStream_t s) {
@@ -349,7 +400,17 @@ Y::DecodeParams decode_params(const whenet_det* d, int n, const int32_t* img_hw,
 }
 
 int run_decode(whenet_det* d, const Y::DecodeParams& p, int n, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
-    const int rc = Y::launch_decode_nms(d->stream, p, n);
+    if ((d->force_large_decode || Y::large_decode_route(p.NC)) && !d->d_keep) {
+        const size_t slots = (size_t)d->max_frames * d->num_classes;
+        int rc = dev_alloc(&d->d_keep, slots * Y::kMaxBoxes * 8, "the kept NMS keys");
+        if (!rc) rc = dev_alloc(&d->d_keep_count, slots * 4, "the kept NMS counts");
+        if (rc) {                       // both or neither: the next call allocates them again
+            cudaFree(d->d_keep);
+            d->d_keep = nullptr;
+            return rc;
+        }
+    }
+    const int rc = Y::launch_decode_nms(d->stream, p, n, d->force_large_decode, d->d_keep, d->d_keep_count);
     if (rc) return fail(WHENET_ECUDA, "decode/NMS launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     const size_t slots = (size_t)n * p.C * p.max_boxes;
     CKD(cudaMemcpyAsync(boxes, d->d_boxes, slots * 16, cudaMemcpyDeviceToHost, d->stream));
@@ -426,11 +487,17 @@ int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, in
     return whenet_det_create_ex(out, device, input_h, input_w, max_frames, WHENET_PRECISION_BF16);
 }
 
-int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision) {
+}  // extern "C"
+
+namespace {
+
+// whenet_det_create_ex (sides up to 608) and whenet_det_create_large (up to 4096)
+int create_detector(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision, int max_side) {
     if (!out) return fail(WHENET_EINVAL, "out is NULL");
     *out = nullptr;
     for (int v : {input_h, input_w})
-        if (v < 32 || v > 608 || v % 32) return fail(WHENET_EINVAL, "input size %dx%d: both must be multiples of 32 in [32, 608]", input_w, input_h);
+        if (v < 32 || v > max_side || v % 32)
+            return fail(WHENET_EINVAL, "input size %dx%d: both must be multiples of 32 in [32, %d]", input_w, input_h, max_side);
     if (max_frames < 1 || max_frames > 64) return fail(WHENET_EINVAL, "max_frames=%d outside [1, 64]", max_frames);
     if (precision != WHENET_PRECISION_BF16 && precision != WHENET_PRECISION_FP32)
         return fail(WHENET_EINVAL, "precision %d: the detector runs in WHENET_PRECISION_BF16 (%d) or WHENET_PRECISION_FP32 (%d)", precision,
@@ -443,6 +510,12 @@ int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w,
     CKD(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0)
         return fail(WHENET_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
+    // the canvases and the smallest network's activations (tiny YOLOv3, one class): a detector that cannot hold even these is
+    // refused before its first buffer
+    const bool f32 = precision == WHENET_PRECISION_FP32;
+    const size_t least = (size_t)max_frames * ((size_t)input_h * input_w * 3 +
+                                               activation_bytes_per_frame(Y::make_tiny_table(), true, input_h, input_w, 1, f32));
+    if (int rc = check_fits(device, least, "a detector of this size, precision and max_frames")) return rc;
     whenet_det* d = new whenet_det();
     d->device = device; d->in_h = input_h; d->in_w = input_w; d->max_frames = max_frames; d->sm_count = prop.multiProcessorCount;
     d->precision = precision;
@@ -453,10 +526,21 @@ int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w,
         cudaStreamCreateWithFlags(&d->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
         return bail(fail(WHENET_ECUDA, "stream creation failed"));
     d->stream = d->own_stream;
-    if (cudaMalloc(&d->d_canvas, (size_t)max_frames * input_h * input_w * 3) != cudaSuccess)
-        return bail(fail(WHENET_ECUDA, "out of device memory (canvas)"));
+    if (int rc = dev_alloc(&d->d_canvas, (size_t)max_frames * input_h * input_w * 3, "the letterboxed canvases")) return bail(rc);
     *out = d;
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision) {
+    return create_detector(out, device, input_h, input_w, max_frames, precision, 608);
+}
+
+int whenet_det_create_large(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision) {
+    return create_detector(out, device, input_h, input_w, max_frames, precision, Y::kMaxSide);
 }
 
 int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors, const float* anchors, int n_anchors) {
@@ -527,15 +611,19 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
         for (int o = 0; o < N; ++o) hb[b_off.back() + o] = (float)shift[o];
     }
     CKD(cudaSetDevice(d->device));
+    // everything the detector will hold; more than the device has is refused here, the detector left as it was
+    const size_t total = (hw.size() + hw_lo.size()) * 2 + hb.size() * 4 +
+                         (size_t)d->max_frames * ((size_t)d->in_h * d->in_w * 3 + activation_bytes_per_frame(T, tiny, d->in_h, d->in_w, C, f32));
+    if (int rc = check_fits(d->device, total, "this network at this size, precision and max_frames")) return rc;
     CKD(cudaStreamSynchronize(d->stream));
     free_graphs(d);
     cudaFree(d->warena); cudaFree(d->warena_lo); cudaFree(d->barena);
     d->warena = nullptr; d->warena_lo = nullptr; d->barena = nullptr; d->loaded = false;
-    CKD(cudaMalloc(&d->warena, hw.size() * 2));
-    CKD(cudaMalloc(&d->barena, hb.size() * 4));
+    if (int rc = dev_alloc(&d->warena, hw.size() * 2, "the conv weights")) return rc;
+    if (int rc = dev_alloc(&d->barena, hb.size() * 4, "the conv biases")) return rc;
     CKD(cudaMemcpy(d->warena, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice));
     if (f32) {
-        CKD(cudaMalloc(&d->warena_lo, hw_lo.size() * 2));
+        if (int rc = dev_alloc(&d->warena_lo, hw_lo.size() * 2, "the conv weights' lo parts")) return rc;
         CKD(cudaMemcpy(d->warena_lo, hw_lo.data(), hw_lo.size() * 2, cudaMemcpyHostToDevice));
     }
     CKD(cudaMemcpy(d->barena, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
@@ -548,11 +636,10 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
             d->anchors[2 * (3 * l + a) + 1] = anchors[2 * an + 1];
         }
     // activations: one buffer per conv output and per pooled conv input (the concat and residual sources and the taps stay
-    // addressable), workspaces; rebuilt when the network or the class count changes
+    // addressable), workspaces; rebuilt when the network or the class count changes.  A failed allocation frees them all and
+    // leaves the detector without weights.
     if (C != d->num_classes || tiny != d->tiny || !d->L[0].out) {
-        free_layers(d);
-        cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
-        d->d_cand = nullptr; d->d_cand_score = nullptr; d->d_boxes = nullptr; d->d_scores = nullptr; d->d_classes = nullptr; d->d_count = nullptr;
+        free_activations(d);
         d->num_classes = C;
         d->tiny = tiny;
         d->table = T;
@@ -566,16 +653,26 @@ int whenet_det_load_weights(whenet_det* d, const whenet_tensor* t, int n_tensors
             l.N = c.head >= 0 ? 3 * (5 + C) : c.cout;
             if (f32) l.plan32 = Y::plan_igemm32(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
             else l.plan = Y::plan_igemm(l.Ho, l.Wo, l.N, c.cin, c.k, d->sm_count);
-            CKD(cudaMalloc(&l.out, (size_t)d->max_frames * l.Ho * l.Wo * l.N * (c.head >= 0 || f32 ? 4 : 2)));
-            if (c.pool) CKD(cudaMalloc(&l.pooled, (size_t)d->max_frames * l.Hi * l.Wi * c.cin * (f32 ? 4 : 2)));
+        }
+        int rc = 0;
+        for (size_t i = 0; i < T.size() && !rc; ++i) {
+            const ConvCfg& c = T[i];
+            LayerDev& l = d->L[i];
+            rc = dev_alloc(&l.out, (size_t)d->max_frames * l.Ho * l.Wo * l.N * (c.head >= 0 || f32 ? 4 : 2), "a conv output");
+            if (!rc && c.pool) rc = dev_alloc(&l.pooled, (size_t)d->max_frames * l.Hi * l.Wi * c.cin * (f32 ? 4 : 2), "a max-pool output");
         }
         const size_t nc = (size_t)ncand(d), slots = (size_t)d->max_frames * C * Y::kMaxBoxes;
-        CKD(cudaMalloc(&d->d_cand, (size_t)d->max_frames * nc * 16));
-        CKD(cudaMalloc(&d->d_cand_score, (size_t)d->max_frames * C * nc * 4));
-        CKD(cudaMalloc(&d->d_boxes, slots * 16));
-        CKD(cudaMalloc(&d->d_scores, slots * 4));
-        CKD(cudaMalloc(&d->d_classes, slots * 4));
-        CKD(cudaMalloc(&d->d_count, (size_t)d->max_frames * 4));
+        if (!rc) rc = dev_alloc(&d->d_cand, (size_t)d->max_frames * nc * 16, "the decoded boxes");
+        if (!rc) rc = dev_alloc(&d->d_cand_score, (size_t)d->max_frames * C * nc * 4, "the class scores");
+        if (!rc) rc = dev_alloc(&d->d_boxes, slots * 16, "the output boxes");
+        if (!rc) rc = dev_alloc(&d->d_scores, slots * 4, "the output scores");
+        if (!rc) rc = dev_alloc(&d->d_classes, slots * 4, "the output classes");
+        if (!rc) rc = dev_alloc(&d->d_count, (size_t)d->max_frames * 4, "the output counts");
+        if (rc) {
+            free_activations(d);
+            d->num_classes = 0;
+            return rc;
+        }
     }
     d->loaded = true;
     return 0;
@@ -615,7 +712,7 @@ int detect_one_size(whenet_det* d, const uint8_t* frames, int n, int H, int W, i
         cudaFree(d->d_frames);
         d->d_frames = nullptr; d->frames_cap = 0;
         free_graphs(d);                         // they captured the old buffer
-        CKD(cudaMalloc(&d->d_frames, bytes));
+        if (int rc = dev_alloc(&d->d_frames, bytes, "the input frames")) return rc;
         d->frames_cap = bytes;
     }
     CKD(cudaMemcpyAsync(d->d_frames, frames, bytes, frames_are_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, d->stream));
@@ -664,7 +761,7 @@ int detect_ragged(whenet_det* d, const uint8_t* const* frames, const int32_t* hw
         cudaFree(d->d_frames);
         d->d_frames = nullptr; d->frames_cap = 0;
         free_graphs(d);                         // they captured the old buffer
-        CKD(cudaMalloc(&d->d_frames, bytes));
+        if (int rc = dev_alloc(&d->d_frames, bytes, "the input frames")) return rc;
         d->frames_cap = bytes;
     }
     const cudaMemcpyKind kind = frames_are_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
@@ -733,9 +830,8 @@ void whenet_det_destroy(whenet_det* d) {
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_graphs(d);
-    free_layers(d);
+    free_activations(d);
     cudaFree(d->warena); cudaFree(d->warena_lo); cudaFree(d->barena); cudaFree(d->d_frames); cudaFree(d->d_canvas);
-    cudaFree(d->d_cand); cudaFree(d->d_cand_score); cudaFree(d->d_boxes); cudaFree(d->d_scores); cudaFree(d->d_classes); cudaFree(d->d_count);
     if (d->own_stream) cudaStreamDestroy(d->own_stream);
     if (d->cap_stream) cudaStreamDestroy(d->cap_stream);
     delete d;
@@ -872,6 +968,12 @@ int whenet_det_debug_decode(whenet_det* d, const float* head0, const float* head
         CKD(cudaMemcpyAsync(L.out, hs[l], bytes, cudaMemcpyHostToDevice, d->stream));
     }
     return run_decode(d, p, n, boxes, scores, classes, counts);
+}
+
+int whenet_det_debug_force_large_decode(whenet_det* d, int on) {
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    d->force_large_decode = on != 0;
+    return 0;
 }
 
 }  // extern "C"

@@ -8,6 +8,16 @@ flagged by ``self.random_weights``; the reference's trained ``head_detect.h5`` i
 As in the reference (yolo_postprocess.py:71-79), the anchors pick the network: 9 anchors mean YOLOv3 (``yolo_body``), 6 mean
 tiny YOLOv3 (``tiny_yolo_body``, ``self.tiny``).
 
+``model_image_size`` is (h, w), multiples of 32 up to 608 per side (``whenet_det_create_ex``) or, above that, up to 4096
+(``whenet_det_create_large``, DESIGN.md 8.6): a 1080p camera letterboxes to 1088 x 1920 with no downscale, so small heads
+keep their pixels.  The reference's image-sized mode, ``model_image_size=(None, None)``, letterboxes each W x H image to
+(H - H % 32, W - W % 32); it is refused here, and for a camera of known size the explicit size gives the same result:
+(1056, 1920) for 1920 x 1080 frames, (704, 1280) for 1280 x 720, (2144, 3840) for 3840 x 2160.
+
+``max_boxes`` (keyword only, 1..256, default 20 as in the reference's ``yolo_eval``) caps the boxes kept per class in every
+``detect`` / ``detect_frames`` call and so in ``pipeline.detect_and_estimate(_frames)``: crowds at high resolution hold more
+than 20 heads.
+
 ``precision`` (keyword only) is ``"bf16"`` (the default: bf16 activations, fp32 accumulation) or ``"fp32"``, the parity mode:
 fp32 activations and every conv as three bf16 MMAs on the hi / lo split of activations and weights (DESIGN.md 8.3).  The
 reference runs its detector in float32.
@@ -107,18 +117,23 @@ def _frame_table(frames, layout: int = 0):
 
 
 class YOLO:
+    max_boxes = 20          # per class and frame (the reference's yolo_eval default); the constructor's keyword sets it
     def __init__(self, model_path=None, anchors_path=None, classes_path=None, score=0.3, iou=0.45, model_image_size=(416, 416),
-                 gpu_num=1, *, device: Optional[int] = None, max_frames: int = 8, seed: int = 0, precision: str = "bf16", **kwargs):
+                 gpu_num=1, *, device: Optional[int] = None, max_frames: int = 8, seed: int = 0, precision: str = "bf16", max_boxes: int = 20,
+                 **kwargs):
         if precision not in _PRECISIONS:
             raise ValueError("precision must be one of %s, not %r" % (sorted(_PRECISIONS), precision))
+        if isinstance(max_boxes, bool) or not isinstance(max_boxes, (int, np.integer)) or not 1 <= max_boxes <= 256:
+            raise ValueError("max_boxes must be an int in [1, 256], not %r" % (max_boxes,))
         self.__dict__.update(kwargs)
         self.precision = precision
+        self.max_boxes = int(max_boxes)
         self.model_path, self.anchors_path, self.classes_path = model_path, anchors_path, classes_path
         self.score, self.iou, self.gpu_num = float(score), float(iou), gpu_num
         size = tuple(model_image_size)
         if len(size) != 2 or None in size:
             raise ValueError("model_image_size (None, None) (image-sized input) is not supported; use multiples of 32")
-        yolo_arch.check_size(*size)
+        yolo_arch.check_size(*size, max_size=yolo_arch.LARGE_MAX_SIZE)
         self.model_image_size = size
         self.anchors = yolo_arch.read_anchors(os.path.expanduser(anchors_path)) if anchors_path else yolo_arch.DEFAULT_ANCHORS.copy()
         if self.anchors.shape not in ((9, 2), (6, 2)):
@@ -142,8 +157,13 @@ class YOLO:
         self.max_frames = int(max_frames)
         self._L = _lib.load()
         self._h = C.c_void_p()
-        check(self._L.whenet_det_create_ex(C.byref(self._h), self.device, size[0], size[1], self.max_frames, _PRECISIONS[precision]))
-        self.load_layers(layers)
+        create = self._L.whenet_det_create_ex if max(size) <= yolo_arch.MAX_SIZE else self._L.whenet_det_create_large
+        check(create(C.byref(self._h), self.device, size[0], size[1], self.max_frames, _PRECISIONS[precision]))
+        try:
+            self.load_layers(layers)
+        except Exception:
+            self.close()            # a detector that could not take its weights frees its device memory at once
+            raise
 
     def load_layers(self, layers, anchors=None):
         """Mapped layers (``yolo_arch.map_weights``) -> device.  ``anchors`` ((w, h) pairs, 9 or 6) replace the detector's
@@ -193,7 +213,8 @@ class YOLO:
             out += self._detect_ragged(frames[off:off + self.max_frames], dev, layout=layout)
         return out
 
-    def _detect_ragged(self, frames, dev: bool, max_boxes: int = 20, layout: int = 0):
+    def _detect_ragged(self, frames, dev: bool, max_boxes: Optional[int] = None, layout: int = 0):
+        max_boxes = self.max_boxes if max_boxes is None else max_boxes
         nb = len(frames)
         ptrs, hw = _frame_table(frames, layout)
         slots = self.num_classes * max_boxes
@@ -206,7 +227,8 @@ class YOLO:
                  _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
         return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(nb)]
 
-    def _detect(self, frames, swap_rb: bool, max_boxes: int = 20, layout: int = 0):
+    def _detect(self, frames, swap_rb: bool, max_boxes: Optional[int] = None, layout: int = 0):
+        max_boxes = self.max_boxes if max_boxes is None else max_boxes
         dev = _is_device(frames)
         if not dev:
             frames = np.ascontiguousarray(frames, dtype=np.uint8)
@@ -287,6 +309,11 @@ class YOLO:
         check(self._L.whenet_det_debug_decode(self._h, _ptr(hs[0]), _ptr(hs[1]), _ptr(hs[2]) if len(hs) > 2 else None, n, img_h, img_w, self.score, self.iou, max_boxes,
                                               _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
         return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(n)]
+
+    def debug_force_large_decode(self, on: bool = True):
+        """Run decode + NMS through the route for more than 24,576 candidates whatever the size (see
+        whenet_det_debug_force_large_decode); False restores the choice by candidate count."""
+        check(self._L.whenet_det_debug_force_large_decode(self._h, int(bool(on))))
 
     def synchronize(self):
         check(self._L.whenet_det_synchronize(self._h))

@@ -45,6 +45,7 @@ DEFAULT_ANCHORS = np.array([[10, 13], [16, 30], [33, 23], [30, 61], [62, 45], [5
                            dtype=np.float64)
 DEFAULT_CLASSES = ["head"]
 MIN_SIZE, MAX_SIZE = 32, 608
+LARGE_MAX_SIZE = 4096      # whenet_det_create_large: sides above MAX_SIZE up to this (DESIGN.md 8.6)
 
 
 @dataclass(frozen=True)
@@ -180,12 +181,14 @@ def out_hw(h: int, w: int, tiny: bool = False) -> List[Tuple[int, int]]:
     return [(ih // L.stride, iw // L.stride) for L, (ih, iw) in zip(table(tiny), in_hw(h, w, tiny))]
 
 
-def check_size(h: int, w: int) -> None:
+def check_size(h: int, w: int, max_size: int = MAX_SIZE) -> None:
+    """ValueError unless h and w are multiples of 32 in [MIN_SIZE, max_size] (MAX_SIZE, or LARGE_MAX_SIZE for a detector made
+    by whenet_det_create_large)."""
     for v in (h, w):
         if v is None:
             raise ValueError("model_image_size (None, None) (image-sized input) is not supported")
-        if v % 32 or not MIN_SIZE <= v <= MAX_SIZE:
-            raise ValueError("model_image_size must be multiples of 32 in [%d, %d], got (%r, %r)" % (MIN_SIZE, MAX_SIZE, h, w))
+        if v % 32 or not MIN_SIZE <= v <= max_size:
+            raise ValueError("model_image_size must be multiples of 32 in [%d, %d], got (%r, %r)" % (MIN_SIZE, max_size, h, w))
 
 
 def macs_per_frame(h: int, w: int, num_classes: int = 1, tiny: bool = False) -> int:

@@ -240,8 +240,8 @@ const char* whenet_version(void);
 void whenet_destroy(whenet_ctx* ctx);
 
 /* ==== YOLOv3 head detector (reference yolo_v3/yolo_postprocess.py:26-205, yolo_v3/model.py) ====
- * A detector handle is bound to one device, one stream and one model input size (multiples of 32 in [32, 608]; the
- * reference's model_image_size, default 416 x 416) and is NOT thread-safe.  Errors use the WHENET_E* codes and
+ * A detector handle is bound to one device, one stream and one model input size (multiples of 32 in [32, 608], or up to 4096
+ * through whenet_det_create_large; the reference's model_image_size, default 416 x 416) and is NOT thread-safe.  Errors use the WHENET_E* codes and
  * whenet_last_error().  Storage is bf16, accumulation fp32; the head logits stay fp32 (whenet_det_create).  The fp32
  * parity mode (whenet_det_create_ex with WHENET_PRECISION_FP32) keeps every activation in fp32 and runs each conv as three
  * bf16 MMAs on the hi / lo split of activations and weights, with fp32 accumulation (DESIGN.md 8.3). */
@@ -255,6 +255,23 @@ int whenet_det_create(whenet_det** out, int device, int input_h, int input_w, in
  * and 164 MB at 608 x 608 in bf16 (tiny YOLOv3: 15 and 32 MB), and twice that in fp32: 153 and 328 MB (tiny: 30 and 63 MB);
  * they are allocated for `max_frames` frames. */
 int whenet_det_create_ex(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision);
+
+/* whenet_det_create_ex for model inputs up to 4096 x 4096: both sides multiples of 32 in [32, 4096], either precision, either
+ * network; anything else is WHENET_EINVAL before a device is touched.  A 1080p frame letterboxes to 1088 x 1920 without a
+ * downscale (1056 x 1920 is the reference's image-sized mode, model_image_size=(None, None), on 1080p).  Every other entry
+ * works on such a detector unchanged.  Above 24,576 candidates per frame (3 * (H/32) * (W/32) * 21, tiny: * 5) decode and
+ * NMS run as three kernels with the one-CTA kernel's results; conv launches with more than 65,535 M tiles run as groups of
+ * whole frames.  Device memory per frame (activations, canvas, decode workspaces; one class), from the layer table:
+ *                       YOLOv3 bf16   YOLOv3 fp32   tiny bf16   tiny fp32
+ *   1088 x 1920            936 MB       1.86 GB      186 MB      364 MB
+ *   2176 x 3840           3.75 GB       7.44 GB      743 MB     1.46 GB
+ *   4096 x 4096           7.52 GB       14.9 GB     1.49 GB     2.92 GB
+ * all of it allocated for `max_frames` frames (most of it by whenet_det_load_weights).  A request larger than the whole device
+ * is refused before its first buffer with WHENET_ECUDA naming the bytes it needs: at create when even tiny YOLOv3 with one
+ * class would not fit, at whenet_det_load_weights (the detector left as it was) for the network loaded.  An allocation that
+ * fails otherwise returns WHENET_ECUDA naming its bytes; the detector is then left without weights (or, at create, not
+ * made), and the device keeps working. */
+int whenet_det_create_large(whenet_det** out, int device, int input_h, int input_w, int max_frames, int precision);
 
 /* The detector's precision (WHENET_PRECISION_BF16 or WHENET_PRECISION_FP32). */
 int whenet_det_precision(whenet_det* det);
@@ -333,6 +350,11 @@ int whenet_det_debug_maxpool(whenet_det* det, const float* x, int n, int H, int 
  * may be NULL. */
 int whenet_det_debug_decode(whenet_det* det, const float* head0, const float* head1, const float* head2, int n, int img_h, int img_w,
                             float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
+
+/* Test hook: on != 0 runs every later decode + NMS of this detector through the route for more than 24,576 candidates
+ * (decode, per-class NMS and pack kernels) whatever its candidate count, so that both routes can be compared where both run;
+ * 0 restores the choice by candidate count. */
+int whenet_det_debug_force_large_decode(whenet_det* det, int on);
 
 #ifdef __cplusplus
 }

@@ -7,6 +7,8 @@
 //   build_tmp/yolo_plan_dump conv SM Ho Wo N Cin k [Ho Wo N Cin k ...]
 // and the fp32 parity mode's plans (plan_igemm32, with the CTAs per SM each plan assumes):
 //   build_tmp/yolo_plan_dump net32 C SM [H W] | tiny32 C SM [H W] | conv32 SM Ho Wo N Cin k [...]
+// and the frame groups launch_igemm / launch_igemm32 split a conv of n frames of Ho x Wo output pixels into:
+//   build_tmp/yolo_plan_dump split Ho Wo n [Ho Wo n ...]
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -49,6 +51,8 @@ static void net(int h, int w, int C, int sm, bool tiny, bool fp32 = false) {
 
 int main(int argc, char** argv) {
     printf("nms per %d threads %d max_boxes %d\n", kNmsPer, kNmsThreads, kMaxBoxes);
+    printf("large nms above %d candidates max_candidates %d alive_bytes %d max_side %d grid_y %d\n", kNmsPer * kNmsThreads, kMaxCandidates,
+           kLargeAliveBytes, kMaxSide, kMaxGridY);
     const std::string cmd = argc >= 2 ? argv[1] : "";
     if (argc >= 4 && (cmd == "net" || cmd == "tiny" || cmd == "net32" || cmd == "tiny32")) {
         const bool tiny = cmd.rfind("tiny", 0) == 0, fp32 = cmd.size() > 2 && cmd.substr(cmd.size() - 2) == "32";
@@ -67,6 +71,19 @@ int main(int argc, char** argv) {
         }
         return 0;
     }
-    fprintf(stderr, "usage: %s net|net32 C SM [H W] | tiny|tiny32 C SM [H W] | conv|conv32 SM Ho Wo N Cin k [...]\n", argv[0]);
+    if (argc >= 5 && cmd == "split" && (argc - 2) % 3 == 0) {
+        for (int a = 2; a < argc; a += 3) {
+            const int Ho = atoi(argv[a]), Wo = atoi(argv[a + 1]), n = atoi(argv[a + 2]);
+            const long long hw = (long long)Ho * Wo;
+            printf("split Ho %d Wo %d n %d", Ho, Wo, n);
+            for_each_frame_group(n, hw, [&](int f0, int nf) {          // the launchers' own grouping
+                printf(" | f0 %d nf %d tiles %lld", f0, nf, (nf * hw + BM - 1) / BM);
+                return 0;
+            });
+            printf("\n");
+        }
+        return 0;
+    }
+    fprintf(stderr, "usage: %s net|net32 C SM [H W] | tiny|tiny32 C SM [H W] | conv|conv32 SM Ho Wo N Cin k [...] | split Ho Wo n [...]\n", argv[0]);
     return 2;
 }
