@@ -19,6 +19,7 @@ EXPORTS = [
     "whenet_det_debug_decode", "whenet_det_create_ex", "whenet_det_precision", "whenet_det_detect_ragged_u8", "whenet_crop_boxes_ragged_u8",
     "whenet_det_detect_yuv_u8", "whenet_det_detect_ragged_yuv_u8", "whenet_crop_boxes_yuv_u8", "whenet_crop_boxes_ragged_yuv_u8",
     "whenet_det_create_large", "whenet_det_debug_force_large_decode",
+    "whenet_draw_heads_u8", "whenet_draw_heads_ragged_u8", "whenet_debug_overlay_segments",
 ]
 
 # pixel_format -> the ABI's yuv_layout (WHENET_YUV_NV12 / WHENET_YUV_I420); "bgr" is packed 8-bit BGR, the *_u8 entries
@@ -80,6 +81,9 @@ def load():
     L.whenet_crop_boxes_yuv_u8.argtypes = L.whenet_crop_boxes_u8.argtypes
     L.whenet_crop_boxes_ragged_yuv_u8.argtypes = L.whenet_crop_boxes_ragged_u8.argtypes
     L.whenet_debug_enlarge_boxes.argtypes = [P, C.c_int, C.c_int, C.c_int, P, P]
+    L.whenet_draw_heads_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P, P, C.c_int, P]
+    L.whenet_draw_heads_ragged_u8.argtypes = [P, P, P, C.c_int, P, P, P, C.c_int, P]
+    L.whenet_debug_overlay_segments.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P]
     L.whenet_synchronize.argtypes = [P]
     L.whenet_host_alloc.argtypes = [C.c_size_t]
     L.whenet_host_alloc.restype = P

@@ -23,6 +23,7 @@
 #include "kernels_tc.cuh"
 #include "kernels_fused.cuh"
 #include "kernels_crop.cuh"
+#include "kernels_overlay.cuh"
 #include "kernels_k2.cuh"
 #include "kernels_tc32.cuh"
 #include "kernels_dwse.cuh"
@@ -205,6 +206,8 @@ struct whenet_ctx {
     // crop front-end staging
     uint8_t* d_frame = nullptr; size_t frame_cap = 0;
     int4* d_rects = nullptr; int* d_frame_of = nullptr; int rects_cap = 0;
+    // head overlay segment table
+    whenet::OverlaySeg* d_segs = nullptr; int segs_cap = 0;
     // taps
     bool taps_on = false;
     std::map<std::string, std::pair<float*, size_t>> taps;
@@ -1620,6 +1623,157 @@ int crop_boxes_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t
     return launch_crops_ragged(c, frames, hw, n, frames_are_device, rects.data(), frame_of, m, swap_rb, yuv_layout, crops_out);
 }
 
+// ----------------------------------------------------------------------------- head overlay (DESIGN.md section 8.7)
+// One head -> the 7 segments reference demo_video.py:26,29 draws (utils.py:40-42): the rectangle as its 4 edges (cv2.rectangle
+// with thickness 2 gives the pixels of these 4 cv2.line calls), then the red, green and blue axes.  Every scalar keeps the type
+// numpy 2 gives it in the reference: a bound clamped by max(0, v) / min(W, v) is a Python int, so tdx and size are a Python
+// float and int (double arithmetic) when BOTH x bounds clamped, float32 otherwise; likewise tdy for y.  An np.float32 meeting
+// a Python float rounds that float to float32 first.  Returns false where the reference raises (empty or out-of-frame slice,
+// a non-finite float32 radian): such a head is not drawn.  Compiled without FMA contraction (build.py), as CPython evaluates.
+constexpr int kSegsPerHead = 7;
+
+struct PyNum {            // a float32 or a double, as the reference's value has it
+    double v; bool dbl;
+};
+inline PyNum py_add(PyNum a, PyNum b) {
+    return (a.dbl && b.dbl) ? PyNum{a.v + b.v, true} : PyNum{(double)((float)a.v + (float)b.v), false};
+}
+inline PyNum py_mul(PyNum size, double e) {      // size * (double expression)
+    return size.dbl ? PyNum{size.v * e, true} : PyNum{(double)((float)size.v * (float)e), false};
+}
+
+bool head_segments(const float* box, const float* ang, int H, int W, int32_t seg[kSegsPerHead][4]) {
+    int32_t r[4];
+    if (!enlarge_box(box, H, W, r)) return false;
+    float y_min = box[0], x_min = box[1], y_max = box[2], x_max = box[3];
+    const float vy0 = y_min - std::fabs(y_min - y_max) / 10.f;
+    const bool cy0 = !(vy0 > 0.f);
+    y_min = cy0 ? 0.f : vy0;
+    const float vy1 = y_max + std::fabs(y_min - y_max) / 10.f;
+    const bool cy1 = !(vy1 < (float)H);
+    y_max = cy1 ? (float)H : vy1;
+    const float vx0 = x_min - std::fabs(x_min - x_max) / 5.f;
+    const bool cx0 = !(vx0 > 0.f);
+    x_min = cx0 ? 0.f : vx0;
+    const float vx1 = x_max + std::fabs(x_min - x_max) / 5.f;
+    const bool cx1 = !(vx1 < (float)W);
+    x_max = cx1 ? (float)W : vx1;
+    const float pi = (float)M_PI;
+    const float pitch = ang[1] * pi / 180.f, yaw = -(ang[0] * pi / 180.f), roll = ang[2] * pi / 180.f;
+    if (!std::isfinite(pitch) || !std::isfinite(yaw) || !std::isfinite(roll)) return false;
+    const bool xd = cx0 && cx1, yd = cy0 && cy1;
+    const PyNum tdx = xd ? PyNum{W / 2.0, true} : PyNum{(double)((x_min + x_max) / 2.f), false};
+    const PyNum tdy = yd ? PyNum{H / 2.0, true} : PyNum{(double)((y_min + y_max) / 2.f), false};
+    const PyNum size = xd ? PyNum{(double)(W / 2), true} : PyNum{(double)std::floor(std::fabs(x_max - x_min) / 2.f), false};
+    const double cp = std::cos((double)pitch), sp = std::sin((double)pitch), cyw = std::cos((double)yaw), syw = std::sin((double)yaw);
+    const double cr = std::cos((double)roll), sr = std::sin((double)roll);
+    const PyNum x1 = py_add(py_mul(size, cyw * cr), tdx);
+    const PyNum y1 = py_add(py_mul(size, cp * sr + cr * sp * syw), tdy);
+    const PyNum x2 = py_add(py_mul(size, -cyw * sr), tdx);
+    const PyNum y2 = py_add(py_mul(size, cp * cr - sp * syw * sr), tdy);
+    const PyNum x3 = py_add(py_mul(size, syw), tdx);
+    const PyNum y3 = py_add(py_mul(size, -cyw * sp), tdy);
+    const int X0 = r[2], Y0 = r[0], X1 = r[3], Y1 = r[1];
+    const int cx = (int)tdx.v, cyc = (int)tdy.v;
+    const int32_t s[kSegsPerHead][4] = {{X0, Y0, X1, Y0}, {X1, Y0, X1, Y1}, {X1, Y1, X0, Y1}, {X0, Y1, X0, Y0},
+                                        {cx, cyc, (int)x1.v, (int)y1.v}, {cx, cyc, (int)x2.v, (int)y2.v}, {cx, cyc, (int)x3.v, (int)y3.v}};
+    memcpy(seg, s, sizeof(s));
+    return true;
+}
+
+constexpr uint32_t kSegColor[kSegsPerHead] = {0, 0, 0, 0, 0xff0000u, 0x00ff00u, 0x0000ffu};   // b | g << 8 | r << 16
+
+// A thickness-2 segment on an H x W frame -> its device record; false when it draws nothing (oracle/draw_oracle.py)
+bool overlay_seg(const int32_t p[4], uint32_t bgr, int H, int W, whenet::OverlaySeg* s) {
+    long long x0 = p[0] + 2LL, y0 = p[1] + 2LL, x1 = p[2] + 2LL, y1 = p[3] + 2LL;
+    if (!whenet::ov_clip(W + 4LL, H + 4LL, x0, y0, x1, y1)) return false;
+    x0 -= 2; y0 -= 2; x1 -= 2; y1 -= 2;
+    *s = whenet::OverlaySeg{};
+    s->q0x = (int)x0; s->q0y = (int)y0; s->q1x = (int)x1; s->q1y = (int)y1;
+    s->bgr = bgr;
+    long long lo = std::min(y0, y1) - 1, hi = std::max(y0, y1) + 1;
+    const double dx = (double)(x0 - x1), dy = (double)(y1 - y0);
+    double rr = dx * dx + dy * dy;
+    if (std::fabs(rr) > 2.220446049250313e-16) {
+        rr = 65536.0 / std::sqrt(rr);
+        const long long dpx = std::llrint(dy * rr), dpy = std::llrint(dx * rr);     // round half to even, as cvRound
+        const long long X0 = x0 * 65536, Y0 = y0 * 65536, X1 = x1 * 65536, Y1 = y1 * 65536;
+        const long long vx[4] = {X0 + dpx, X0 - dpx, X1 - dpx, X1 + dpx}, vy[4] = {Y0 + dpy, Y0 - dpy, Y1 - dpy, Y1 + dpy};
+        s->quad = 1;
+        for (int k = 0; k < 4; ++k) {
+            s->vx[k] = vx[k]; s->vy[k] = vy[k];
+            lo = std::min(lo, (vy[k] + 32768) >> 16);
+            hi = std::max(hi, (vy[k] + 32768) >> 16);
+        }
+    }
+    lo = std::max(lo, 0LL);
+    hi = std::min(hi, (long long)H - 1);
+    if (lo > hi) return false;
+    s->y_lo = (int)lo; s->y_hi = (int)hi;
+    return true;
+}
+
+// heads -> the segment table grouped by frame, in result order within a frame, and the launch
+int draw_heads(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes, const float* angles,
+               const int32_t* frame_of, int m, int32_t* drawn_out) {
+    whenet::OverlayFrames fr{};
+    std::vector<std::vector<whenet::OverlaySeg>> per(n);
+    int32_t seg[kSegsPerHead][4];
+    for (int i = 0; i < m; ++i) {
+        const int f = frame_of[i], H = hw[2 * f], W = hw[2 * f + 1];
+        const bool ok = head_segments(boxes + 4 * i, angles + 3 * i, H, W, seg);
+        if (drawn_out) drawn_out[i] = ok;
+        if (!ok) continue;
+        for (int k = 0; k < kSegsPerHead; ++k) {
+            whenet::OverlaySeg s;
+            if (overlay_seg(seg[k], kSegColor[k], H, W, &s)) per[f].push_back(s);
+        }
+    }
+    std::vector<whenet::OverlaySeg> segs;
+    int maxH = 0;
+    for (int f = 0; f < n; ++f) {
+        fr.seg_begin[f] = (int)segs.size();
+        segs.insert(segs.end(), per[f].begin(), per[f].end());
+        fr.ptr[f] = frames[f]; fr.H[f] = hw[2 * f]; fr.W[f] = hw[2 * f + 1];
+        maxH = std::max(maxH, fr.H[f]);
+    }
+    fr.seg_begin[n] = (int)segs.size();
+    const int total = (int)segs.size();
+    if (total == 0) return 0;
+    CK(cudaSetDevice(c->device));
+    if (c->segs_cap < total) {
+        if (c->d_segs) cudaFree(c->d_segs);
+        c->d_segs = nullptr; c->segs_cap = 0;
+        CK(cudaMalloc(&c->d_segs, (size_t)total * sizeof(whenet::OverlaySeg)));
+        c->segs_cap = total;
+    }
+    CK(cudaMemcpyAsync(c->d_segs, segs.data(), (size_t)total * sizeof(whenet::OverlaySeg), cudaMemcpyHostToDevice, c->stream));
+    Scope sc(c, "draw_heads", 0.0, 0.0);
+    whenet::overlay_draw_kernel<<<dim3((maxH + 127) / 128, n), 128, 0, c->stream>>>(fr, c->d_segs);
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int draw_heads_checked(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes, const float* angles,
+                       const int32_t* frame_of, int m, int32_t* drawn_out) {
+    // the context is checked last so that every other argument can be validated without a GPU
+    if (n < 1 || n > whenet::kMaxCropFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxCropFrames);
+    for (int i = 0; i < n; ++i) {
+        if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
+        if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
+            return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+    }
+    if (m < 0) return fail(WHENET_EINVAL, "m=%d heads", m);
+    if (m == 0) return 0;
+    if (!boxes || !angles || !frame_of) return fail(WHENET_EINVAL, "null boxes, angles or frame_of");
+    for (int i = 0; i < m; ++i)
+        if (frame_of[i] < 0 || frame_of[i] >= n) return fail(WHENET_EINVAL, "head %d: frame_of=%d outside [0, %d)", i, frame_of[i], n);
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    return draw_heads(c, frames, hw, n, boxes, angles, frame_of, m, drawn_out);
+}
+
+static_assert(whenet::kOverlayMaxFrames == whenet::kMaxCropFrames, "overlay frame table holds every crop frame");
+
 }  // namespace
 
 extern "C" {
@@ -1645,6 +1799,39 @@ int whenet_crop_boxes_ragged_yuv_u8(whenet_ctx* c, const uint8_t* const* frames,
                                     int32_t* valid_out) {
     if (int rc = check_yuv_layout(yuv_layout)) return rc;
     return crop_boxes_ragged(c, frames, hw, n, frames_are_device, boxes, frame_of, m, 1, yuv_layout, crops_out, rects_out, valid_out);
+}
+
+int whenet_draw_heads_u8(whenet_ctx* c, uint8_t* frames, int n, int H, int W, const float* boxes, const float* angles,
+                         const int32_t* frame_of, int m, int32_t* drawn_out) {
+    if (!frames) return fail(WHENET_EINVAL, "null frames");
+    if (n < 1 || n > whenet::kMaxCropFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxCropFrames);
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    uint8_t* ptrs[whenet::kMaxCropFrames];
+    int32_t hw[2 * whenet::kMaxCropFrames];
+    for (int i = 0; i < n; ++i) {
+        ptrs[i] = frames + (size_t)i * H * W * 3;
+        hw[2 * i] = H; hw[2 * i + 1] = W;
+    }
+    return draw_heads_checked(c, ptrs, hw, n, boxes, angles, frame_of, m, drawn_out);
+}
+
+int whenet_draw_heads_ragged_u8(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes,
+                                const float* angles, const int32_t* frame_of, int m, int32_t* drawn_out) {
+    if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
+    return draw_heads_checked(c, frames, hw, n, boxes, angles, frame_of, m, drawn_out);
+}
+
+int whenet_debug_overlay_segments(const float* boxes, const float* angles, int m, int H, int W, int32_t* seg_out, int32_t* drawn_out) {
+    if (!boxes || !angles || m < 1) return fail(WHENET_EINVAL, "null boxes or angles, or m=%d heads", m);
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    for (int i = 0; i < m; ++i) {
+        int32_t seg[kSegsPerHead][4] = {};
+        const bool ok = head_segments(boxes + 4 * i, angles + 3 * i, H, W, seg);
+        if (!ok) memset(seg, 0, sizeof(seg));
+        if (seg_out) memcpy(seg_out + (size_t)i * kSegsPerHead * 4, seg, sizeof(seg));
+        if (drawn_out) drawn_out[i] = ok;
+    }
+    return 0;
 }
 
 int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out) {
@@ -1913,6 +2100,7 @@ void whenet_destroy(whenet_ctx* c) {
     if (c->d_frame) cudaFree(c->d_frame);
     if (c->d_rects) cudaFree(c->d_rects);
     if (c->d_frame_of) cudaFree(c->d_frame_of);
+    if (c->d_segs) cudaFree(c->d_segs);
     for (auto& kv : c->taps) cudaFree(kv.second.first);
     for (auto& p : c->ev_used) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }
     for (auto e : c->ev_pool) cudaEventDestroy(e);

@@ -5,6 +5,8 @@ so annotated frames are pixel-identical to the reference's for the same angles.
   ``axis_endpoints`` / ``draw_axis``   reference utils.py:13-43
   ``annotate_head``                    reference demo_video.py:25-34  (rectangle, axes, optional yaw/pitch/roll text)
   ``process_frame``                    reference demo_video.py:11-35,57-58 for all heads of one frame
+  ``draw_heads``                       demo_video.py:26,29 (display="simple") for every head of a batch of DEVICE frames, on
+                                       the GPU in place (``whenet_draw_heads_u8``, DESIGN.md section 8.7)
 
 ``process_frame(reference_order=True)`` reproduces the reference's order of operations bit for bit: it annotates the frame
 after EACH head and cuts the next head's crop from the already annotated frame (demo_video.py:57-58 calls
@@ -12,6 +14,10 @@ process_detection head by head on the same array), one forward per head.  ``refe
 every crop from the CLEAN frame on the GPU in one batch (``WHENet.get_angle_from_frame``) and annotates afterwards; crops that
 overlap an earlier head's rectangle / axes / text then differ from the reference's by those drawn pixels - a deliberate
 deviation (the drawn overlay is not image content), documented in DESIGN.md.
+
+``draw_heads`` draws on the clean frames what ``oracle/overlay_oracle.process_detection_ref`` draws for each head, pixel for
+pixel, with the reference's float32 scalar types (``draw_axis`` below turns the angles into Python floats first, which moves an
+axis end point for about 1 head in 100,000; DESIGN.md section 8.7).  Text (``display="full"``) stays on the host.
 """
 from __future__ import annotations
 
@@ -86,3 +92,67 @@ def process_frame(model, frame, boxes, display: str = "simple", reference_order:
         for i in range(n):
             annotate_head(frame, bounds[i], yaw[i], pitch[i], roll[i], display)
     return frame, yaw, pitch, roll
+
+
+def draw_heads(whenet, frames, results):
+    """Draw every head of ``results`` into ``frames`` on the GPU, in place: a black thickness-2 rectangle around the
+    margin-enlarged box, then the red, green and blue pose axes, bit-identical to the reference's cv2 calls
+    (demo_video.py:26,29 with display="simple").  Heads are drawn in result order.
+
+    ``frames``: a contiguous (n, H, W, 3) uint8 BGR CUDA tensor on ``whenet.device``, or a list or tuple of contiguous
+    (H_i, W_i, 3) ones; ``results``: what ``pipeline.detect_and_estimate_frames`` returned for those frames.  A head is
+    skipped where the reference would raise: its enlarged slice is empty or leaves the frame, or an angle's float32 radian
+    is not finite (the NaN angles of invalid slices).  Returns the per-frame (k,) bool arrays of drawn heads after one
+    synchronisation.  Host frames are refused (``process_frame`` is the host path)."""
+    import ctypes as C
+    import torch
+    from ._lib import check
+    from .whenet import _is_device, _ptr
+    frame_list = isinstance(frames, (list, tuple))
+    items = list(frames) if frame_list else [frames]
+    for f in items:
+        if not _is_device(f):
+            raise ValueError("draw_heads draws on CUDA tensors; use process_frame for host frames")
+        if str(f.dtype) != "torch.uint8" or not f.is_contiguous():
+            raise ValueError("frames must be contiguous uint8 CUDA tensors")
+        if f.device.index != whenet.device:
+            raise ValueError("frames are on cuda:%s, WHENet on cuda:%d" % (f.device.index, whenet.device))
+        if len(f.shape) != (3 if frame_list else 4) or f.shape[-1] != 3:
+            raise ValueError("frames must be BGR (n, H, W, 3) or a list of (H, W, 3), not %s" % (tuple(f.shape),))
+    n = len(items) if frame_list else int(frames.shape[0])
+    if len(results) != n:
+        raise ValueError("%d results for %d frames" % (len(results), n))
+    if n == 0:
+        return []
+    counts = [len(r[0]) for r in results]
+    m = sum(counts)
+    if m == 0:
+        return [np.zeros((0,), bool) for _ in range(n)]
+    boxes = np.ascontiguousarray(np.concatenate([np.asarray(r[0], np.float32).reshape(-1, 4) for r in results]), np.float32)
+    angles = np.ascontiguousarray(np.concatenate([np.asarray(r[2], np.float32).reshape(-1, 3) for r in results]), np.float32)
+    frame_of = np.repeat(np.arange(n, dtype=np.int32), counts)
+    drawn = np.zeros(m, np.int32)
+    L = whenet._L
+    with torch.cuda.device(whenet.device):
+        torch.cuda.current_stream().synchronize()       # frames the caller wrote on torch's stream are complete
+        for lo in range(0, n, 64):
+            hi = min(n, lo + 64)
+            a, b = int(np.searchsorted(frame_of, lo)), int(np.searchsorted(frame_of, hi))
+            if a == b:
+                continue
+            fo = np.ascontiguousarray(frame_of[a:b] - lo)
+            if frame_list:
+                ptrs = (C.c_void_p * (hi - lo))(*[f.data_ptr() for f in items[lo:hi]])
+                hw = np.array([f.shape[:2] for f in items[lo:hi]], np.int32)
+                check(L.whenet_draw_heads_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, _ptr(boxes[a:]), _ptr(angles[a:]),
+                                                    _ptr(fo), b - a, _ptr(drawn[a:])))
+            else:
+                _, H, W, _c = frames.shape
+                check(L.whenet_draw_heads_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, _ptr(boxes[a:]), _ptr(angles[a:]),
+                                             _ptr(fo), b - a, _ptr(drawn[a:])))
+        whenet.synchronize()
+    out, off = [], 0
+    for k in counts:
+        out.append(drawn[off:off + k].astype(bool))
+        off += k
+    return out

@@ -202,6 +202,23 @@ int whenet_debug_raise_timeout(whenet_ctx* ctx);
 /* The margin arithmetic of whenet_crop_boxes_u8 alone, on the host (no context, no GPU): m boxes of an H x W frame ->
  * rects_out / valid_out as that call fills them (each may be NULL). */
 int whenet_debug_enlarge_boxes(const float* boxes, int m, int H, int W, int32_t* rects_out, int32_t* valid_out);
+/* Head overlay (DESIGN.md section 8.7): draws, for each of m heads, what reference demo_video.py:26,29 draws with
+   display="simple" - a black thickness-2 rectangle around the margin-enlarged box, then the red, green and blue pose axes
+   (utils.py:40-42) - into device BGR frames IN PLACE on the context's stream, pixel-identical to OpenCV's cv2.rectangle /
+   cv2.line.  Heads are drawn in order, a later one over an earlier one.  boxes: m x (y_min, x_min, y_max, x_max) float32,
+   angles: m x (yaw, pitch, roll) float32 degrees, frame_of: m frame indices, all on the host.  A head is drawn exactly when
+   the reference would draw it without raising: its enlarged slice is valid (as the crop entries' valid_out) and its three
+   float32 radians are finite; drawn_out (optional, m int32) says which were.  m = 0 is a no-op.  n in [1, 64], sides in
+   [1, 16384].  frames: n frames of H x W x 3 bytes back to back. */
+int whenet_draw_heads_u8(whenet_ctx* ctx, uint8_t* frames, int n, int H, int W, const float* boxes, const float* angles,
+                         const int32_t* frame_of, int m, int32_t* drawn_out);
+/* the same on n device frames of their own sizes: frames[i] is H_i x W_i x 3, hw = n x (H_i, W_i) int32 on the host */
+int whenet_draw_heads_ragged_u8(whenet_ctx* ctx, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes,
+                                const float* angles, const int32_t* frame_of, int m, int32_t* drawn_out);
+/* The overlay's host geometry without a GPU: per head 7 segments (x0, y0, x1, y1) int32 in draw order - the rectangle's
+   top, right, bottom and left edges, then the red, green and blue axes - zeros for a head not drawn (drawn_out[i] = 0). */
+int whenet_debug_overlay_segments(const float* boxes, const float* angles, int m, int H, int W, int32_t* seg_out, int32_t* drawn_out);
+
 
 /* Time every kernel of the NEXT forwards with CUDA events. */
 int whenet_profile_enable(whenet_ctx* ctx, int enable);
