@@ -126,6 +126,10 @@ template <> __device__ __forceinline__ uint32_t ones2<__half>() { return 0x3c003
 __device__ __forceinline__ uint32_t sw128(int r, int c) {
     return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
 }
+// the same for 64-byte rows (SWIZZLE_64B): chunk c (0..3) of row r lands at chunk c ^ ((r >> 1) & 3); 8-row atoms of 512 B
+__device__ __forceinline__ uint32_t sw64(int r, int c) {
+    return (uint32_t)(r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
+}
 
 // exact floor(x / d) for the small non-negative ints of the tile arithmetic (x < 2^17, d < 2^8), with inv = 1.0f / d:
 // (x + 0.5) / d is at least 0.5 / d away from every integer, far more than the float rounding error

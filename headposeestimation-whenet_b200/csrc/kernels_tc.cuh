@@ -123,6 +123,23 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     d |= (uint64_t)1 << 62;
     return d;
 }
+// K-major SWIZZLE_64B descriptor: as make_desc with SBO >> 4 = 32 (8 rows x 64 B) and layout = 2 (SWIZZLE_64B).  The
+// operand sits on 512-byte atoms; a K step of 16 elements still advances the start address field by 2.
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)32 << 32;
+    d |= (uint64_t)2 << 62;
+    return d;
+}
+// the descriptor of a K-major operand with ROWB-byte rows (128: SWIZZLE_128B, 64: SWIZZLE_64B)
+template <int ROWB>
+__device__ __forceinline__ uint64_t make_desc_rows(uint32_t saddr) {
+    static_assert(ROWB == 64 || ROWB == 128, "rows of 64 or 128 bytes");
+    if constexpr (ROWB == 64) return make_desc_sw64(saddr);
+    else return make_desc(saddr);
+}
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

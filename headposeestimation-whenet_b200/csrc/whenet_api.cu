@@ -363,16 +363,18 @@ PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
     }
     return fn;
 }
-// K-major weight matrix [rows][K] (16-bit): box = {64, box_rows}
-int make_tmap_w(CUtensorMap* tm, const void* base, int rows, int K, int box_rows, bool is_bf16) {
+// K-major weight matrix [rows][K] (16-bit): box = {64, box_rows} in SWIZZLE_128B rows, or {32, box_rows} in SWIZZLE_64B rows
+// when row_bytes is 64
+int make_tmap_w(CUtensorMap* tm, const void* base, int rows, int K, int box_rows, bool is_bf16, int row_bytes = 128) {
     auto fn = tmap_encode_fn();
     if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-    const cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+    const cuuint32_t box[2] = {(cuuint32_t)row_bytes / 2, (cuuint32_t)box_rows};
     const cuuint32_t estr[2] = {1, 1};
     const CUresult r = fn(tm, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides,
-                          box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(weights %dx%d, box %d) failed: %d", rows, K, box_rows, (int)r);
     return 0;
@@ -392,17 +394,19 @@ int make_tmap_kd_e(CUtensorMap* tm, const void* base, int n, int H, int C, int c
     if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(KD tile %dx%dx%dx%d, box %dx%dx%d) failed: %d", n, H, H, C, pw, pw, cc, (int)r);
     return 0;
 }
-// K1X's block input (bf16) [n][H][H][C]: box {64, iw, iw, 1}, SWIZZLE_128B - a halo tile lands as the K-major A operand, one
-// 128-byte row per pixel; channels >= C and pixels outside the image are zero-filled
-int make_tmap_k1x_in(CUtensorMap* tm, const void* base, int n, int H, int C, int iw) {
+// K1X's block input (bf16) [n][H][H][C]: box {row_bytes / 2, iw, iw, 1}, SWIZZLE_128B (128-byte rows) or SWIZZLE_64B (64-byte
+// rows) - a halo tile lands as the K-major A operand, one row per pixel; channels >= C and pixels outside the image are
+// zero-filled
+int make_tmap_k1x_in(CUtensorMap* tm, const void* base, int n, int H, int C, int iw, int row_bytes) {
     auto fn = tmap_encode_fn();
     if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)H, (cuuint64_t)H, (cuuint64_t)n};
     const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * C * 2, (cuuint64_t)H * H * C * 2};
-    const cuuint32_t box[4] = {64, (cuuint32_t)iw, (cuuint32_t)iw, 1};
+    const cuuint32_t box[4] = {(cuuint32_t)row_bytes / 2, (cuuint32_t)iw, (cuuint32_t)iw, 1};
     const cuuint32_t estr[4] = {1, 1, 1, 1};
     const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                          row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(K1X input %dx%dx%dx%d, box %dx%d) failed: %d", n, H, H, C, iw, iw, (int)r);
     return 0;
 }
@@ -732,17 +736,18 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                         whenet::fused::DwSeParams q{};
                         int rc = 0;
                         if (c->tmaps.size() > 512) c->tmaps.clear();
+                        const int rowb = whenet::fused::k1x_row_bytes(b.cin);          // A and W rows: 64 or 128 bytes
                         const TmapKey kx{600 + b.idx, nb, (const void*)cur}, kwx{700 + b.idx, 0, (const void*)w.wt_exp_aug}, kw{500 + b.idx, 0, (const void*)w.w_dw16};
                         auto ix = c->tmaps.find(kx);
                         if (ix == c->tmaps.end()) {
                             CUtensorMap tm;
-                            if ((rc = make_tmap_k1x_in(&tm, cur, nb, b.hin, b.cin, p.IW))) return rc;
+                            if ((rc = make_tmap_k1x_in(&tm, cur, nb, b.hin, b.cin, p.IW, rowb))) return rc;
                             ix = c->tmaps.emplace(kx, tm).first;
                         }
                         auto iwx = c->tmaps.find(kwx);
                         if (iwx == c->tmaps.end()) {
                             CUtensorMap tm;
-                            if ((rc = make_tmap_w(&tm, w.wt_exp_aug, b.cexp, b.cin + 8, p.CC, true))) return rc;
+                            if ((rc = make_tmap_w(&tm, w.wt_exp_aug, b.cexp, b.cin + 8, p.CC, true, rowb))) return rc;
                             iwx = c->tmaps.emplace(kwx, tm).first;
                         }
                         auto iw = c->tmaps.find(kw);

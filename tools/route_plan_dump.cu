@@ -29,8 +29,8 @@ template <int KS, int S, int HIN, int CC, int CIN> static void kdx_line(const Bl
 template <int KS, int S, int HIN, int TH, int R, int CC, int CIN> static void k1x_line(const Blk& b) {
     using X = fused::K1X<KS, S, HIN, TH, R, CC, CIN>;
     if (b.k == KS && b.s == S && b.hin == HIN && b.cin == CIN)
-        printf("  k1x b%02d th %d r %d cc %d cin %d tiles %d pix %d halves %d ksteps %d lanes %d smem %zu chunks %d\n", b.idx, TH, R, CC, CIN, X::TILES,
-               X::NPIX, X::HALVES, X::KSTEPS, X::PY, X::SMEM, b.cexp / CC);
+        printf("  k1x b%02d th %d r %d cc %d cin %d tiles %d pix %d halves %d ksteps %d lanes %d smem %zu chunks %d ctas_per_sm %d row_bytes %d\n", b.idx,
+               TH, R, CC, CIN, X::TILES, X::NPIX, X::HALVES, X::KSTEPS, X::PY, X::SMEM, b.cexp / CC, X::CTAS_PER_SM, X::ROWB);
 }
 static void k2_line(const char* what, int idx, long long M, int K, int N, int hw, bool gate) {
     tc::K2Params p{};
