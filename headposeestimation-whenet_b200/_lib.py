@@ -11,7 +11,7 @@ PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2}
 
 EXPORTS = [
     "whenet_create", "whenet_load_weights", "whenet_export_packed", "whenet_import_packed", "whenet_set_stream", "whenet_forward_u8", "whenet_forward_u8_async", "whenet_forward_f32",
-    "whenet_crop_resize_u8", "whenet_crop_boxes_u8", "whenet_debug_enlarge_boxes", "whenet_synchronize", "whenet_host_alloc", "whenet_host_free", "whenet_debug_enable_taps", "whenet_debug_tap",
+    "whenet_crop_resize_u8", "whenet_crop_boxes_u8", "whenet_debug_enlarge_boxes", "whenet_synchronize", "whenet_host_alloc", "whenet_host_free", "whenet_debug_enable_taps", "whenet_debug_tap_crops", "whenet_debug_tap",
     "whenet_debug_conv1x1", "whenet_debug_decode", "whenet_debug_raise_timeout", "whenet_debug_set_k1_plan", "whenet_profile_enable", "whenet_profile_read", "whenet_launch_count", "whenet_set_option",
     "whenet_last_error", "whenet_version", "whenet_destroy",
     "whenet_det_create", "whenet_det_load_weights", "whenet_det_num_classes", "whenet_det_set_stream", "whenet_det_detect_u8",
@@ -91,6 +91,7 @@ def load():
     L.whenet_host_free.restype = None
     L.whenet_debug_enable_taps.argtypes = [P, C.c_int]
     L.whenet_debug_tap.argtypes = [P, C.c_char_p, P, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.whenet_debug_tap_crops.argtypes = [P, P, C.c_int]
     L.whenet_debug_conv1x1.argtypes = [P, C.c_int, P, P, P, P, P, P, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     L.whenet_debug_decode.argtypes = [P, P, C.c_int, P]
     L.whenet_debug_raise_timeout.argtypes = [P]

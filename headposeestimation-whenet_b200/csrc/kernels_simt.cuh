@@ -858,11 +858,13 @@ static __global__ void __launch_bounds__(96) decode_only_kernel(const float* __r
 // raises the context's timeout flag from the device (test hook: proves every synchronising path reports it)
 static __global__ void raise_flag_kernel(int* flag) { *reinterpret_cast<volatile int*>(flag) = 1; }
 
-// T -> float copy for debug taps
+// T -> float gather for debug taps: CTA row y copies crop map[y].x (relative to src) into tap row map[y].y
 template <typename T>
-__global__ void tap_copy_kernel(const T* __restrict__ src, float* __restrict__ dst, long long n) {
-    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = Store<T>::ld(src + i);
+__global__ void tap_gather_kernel(const T* __restrict__ src, float* __restrict__ dst, const int2* __restrict__ map, int base,
+                                  long long per) {
+    const int2 m = map[blockIdx.y];
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < per) dst[(long long)m.y * per + i] = Store<T>::ld(src + (long long)(m.x - base) * per + i);
 }
 
 }  // namespace whenet

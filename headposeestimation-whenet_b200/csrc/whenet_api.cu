@@ -208,9 +208,14 @@ struct whenet_ctx {
     int4* d_rects = nullptr; int* d_frame_of = nullptr; int rects_cap = 0;
     // head overlay segment table
     whenet::OverlaySeg* d_segs = nullptr; int segs_cap = 0;
-    // taps
-    bool taps_on = false;
-    std::map<std::string, std::pair<float*, size_t>> taps;
+    // taps (whenet_debug_enable_taps): 0 off, 1 first chunk of <= 8 crops on the one-stream route, 2 every chunk on the
+    // untapped route.  Keyed by the canonical name ("dw%d" also holds a gated "dwg%d"); `valid`: written by the last forward.
+    struct Tap { float* p = nullptr; size_t cap = 0, n = 0; bool valid = false; int forms = 0; };   // forms: 1 ungated, 2 gated rows
+    int taps_mode = 0;
+    std::map<std::string, Tap> taps;
+    std::vector<int> tap_sel;                 // mode 2: the crops to tap, in tap-row order (empty: all)
+    std::vector<int2> tap_map;                // this forward: (crop, tap row), sorted by crop
+    int2* d_tap_map = nullptr; int tap_map_cap = 0;
     // profile
     bool prof_on = false;
     std::vector<EvPair> ev_used;
@@ -267,37 +272,59 @@ struct Scope {
     }
 };
 
-template <typename T>
-int add_tap(whenet_ctx* c, const std::string& name, const T* src, size_t n) {
-    auto it = c->taps.find(name);
-    if (it != c->taps.end() && it->second.second != n) {
-        cudaFree(it->second.first);
-        c->taps.erase(it);
-        it = c->taps.end();
+// Before the first kernel of a tapped forward: invalidate every tap, map the tapped crops (`crops`: crop indices of the call in
+// tap-row order) to their rows, and size every tap buffer for them, so that no allocation runs between launches.
+int prepare_taps(whenet_ctx* c, const std::vector<int>& crops) {
+    for (auto& kv : c->taps) { kv.second.valid = false; kv.second.forms = 0; }
+    c->tap_map.clear();
+    const int k = (int)crops.size();
+    if (k == 0) return 0;
+    if (k > 65535) return fail(WHENET_EINVAL, "%d tapped crops: select at most 65535 (whenet_debug_tap_crops)", k);
+    for (int r = 0; r < k; ++r) c->tap_map.push_back(make_int2(crops[r], r));
+    std::stable_sort(c->tap_map.begin(), c->tap_map.end(), [](const int2& a, const int2& b) { return a.x < b.x; });
+    std::vector<std::pair<std::string, size_t>> per{{"stem", (size_t)112 * 112 * 32}, {"head", (size_t)49 * 1280}, {"pooled", 1280}};
+    for (const BlockCfg& b : c->blocks) {
+        per.push_back({"dw" + std::to_string(b.idx), (size_t)b.hout * b.hout * b.cexp});
+        per.push_back({"gate" + std::to_string(b.idx), (size_t)b.cexp});
+        per.push_back({"block" + std::to_string(b.idx), (size_t)b.hout * b.hout * b.cout});
     }
-    float* dst;
-    if (it == c->taps.end()) {
-        CK(cudaMalloc(&dst, n * sizeof(float)));
-        c->taps[name] = {dst, n};
-    } else dst = it->second.first;
-    whenet::tap_copy_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(src, dst, (long long)n);
-    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));                 // the previous forward's tap copies are done with the map and buffers
+    for (auto& pr : per) {
+        whenet_ctx::Tap& t = c->taps[pr.first];
+        t.n = (size_t)k * pr.second;
+        if (t.cap < t.n) {
+            if (t.p) cudaFree(t.p);
+            t.p = nullptr; t.cap = 0;
+            CK(cudaMalloc(&t.p, t.n * sizeof(float)));
+            t.cap = t.n;
+        }
+    }
+    if (c->tap_map_cap < k) {
+        if (c->d_tap_map) cudaFree(c->d_tap_map);
+        c->d_tap_map = nullptr; c->tap_map_cap = 0;
+        CK(cudaMalloc(&c->d_tap_map, (size_t)k * sizeof(int2)));
+        c->tap_map_cap = k;
+    }
+    CK(cudaMemcpy(c->d_tap_map, c->tap_map.data(), (size_t)k * sizeof(int2), cudaMemcpyHostToDevice));
     return 0;
 }
-template <>
-int add_tap<float>(whenet_ctx* c, const std::string& name, const float* src, size_t n) {
+
+// Copy the tapped crops among [off, off + nb) of the call out of `src` (this chunk's tensor, per_crop elements per crop) into
+// their rows of tap `name`, on the chunk's stream.  `gated`: a depthwise output gated in place (read back as "dwg%d").
+template <typename T>
+int add_tap(whenet_ctx* c, const std::string& name, const T* src, size_t per_crop, int off, int nb, bool gated = false) {
     auto it = c->taps.find(name);
-    if (it != c->taps.end() && it->second.second != n) {
-        cudaFree(it->second.first);
-        c->taps.erase(it);
-        it = c->taps.end();
+    if (it == c->taps.end() || it->second.n != c->tap_map.size() * per_crop)
+        return fail(WHENET_EINVAL, "tap %s was not prepared for this forward", name.c_str());
+    const auto lo = std::lower_bound(c->tap_map.begin(), c->tap_map.end(), off, [](const int2& a, int v) { return a.x < v; });
+    const auto hi = std::lower_bound(c->tap_map.begin(), c->tap_map.end(), off + nb, [](const int2& a, int v) { return a.x < v; });
+    if (hi > lo) {
+        whenet::tap_gather_kernel<T><<<dim3((unsigned)((per_crop + 255) / 256), (unsigned)(hi - lo)), 256, 0, c->stream>>>(
+            src, it->second.p, c->d_tap_map + (lo - c->tap_map.begin()), off, (long long)per_crop);
+        CK(cudaGetLastError());
+        it->second.forms |= gated ? 2 : 1;
     }
-    float* dst;
-    if (it == c->taps.end()) {
-        CK(cudaMalloc(&dst, n * sizeof(float)));
-        c->taps[name] = {dst, n};
-    } else dst = it->second.first;
-    CK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+    it->second.valid = true;
     return 0;
 }
 
@@ -534,8 +561,11 @@ int launch_dw(whenet_ctx* c, const char* name, const BlockCfg& b, const BlockW& 
 }
 
 template <typename T, bool IN_U8>
-int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, float* d_logits, bool taps) {
+int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, float* d_logits, bool taps, int off) {
     char nm[48];
+    // taps: record this chunk (crops off .. off + nb - 1 of the call).  Mode 1 also leaves the depthwise outputs ungated;
+    // mode 2 changes no launch and no kernel parameter.
+    const bool plain_dw = taps && c->taps_mode == 1;
     T* cur = (T*)c->bufA;
     T* oth = (T*)c->bufB;
     T* E = (T*)c->bufE;
@@ -557,8 +587,8 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
         CK(cudaGetLastError());
     }
     if (taps) {
-        int rc = stem_half ? add_tap<__half>(c, "stem", reinterpret_cast<const __half*>(cur), (size_t)nb * 112 * 112 * 32)
-                           : add_tap<T>(c, "stem", cur, (size_t)nb * 112 * 112 * 32);
+        int rc = stem_half ? add_tap<__half>(c, "stem", reinterpret_cast<const __half*>(cur), (size_t)112 * 112 * 32, off, nb)
+                           : add_tap<T>(c, "stem", cur, (size_t)112 * 112 * 32, off, nb);
         if (rc) return rc;
     }
     for (size_t i = 0; i < c->blocks.size(); ++i) {
@@ -684,7 +714,7 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                 if (split == 1 && c->se_tail && c->kd_tail) {
                     p.se_tail = 1;
                     se_in_k1 = true;
-                    if (c->se_scale_out && !taps) { p.scale_out = 1; d_gated = true; }
+                    if (c->se_scale_out && !plain_dw) { p.scale_out = 1; d_gated = true; }
                 }
                 snprintf(nm, sizeof nm, "b%02d.kd", b.idx);
                 if (split == 1) {
@@ -721,8 +751,8 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                         p.se_tail = 1;
                         p.inv_hw = 1.0f / (float)(b.hout * b.hout);
                         se_in_k1 = true;
-                        // ... and applies it to its depthwise output (not under taps: the dw tap is the ungated tensor)
-                        if (c->se_scale_out && !taps) { p.scale_out = 1; d_gated = true; }
+                        // ... and applies it to its depthwise output (not under mode-1 taps, whose dw tap is the ungated tensor)
+                        if (c->se_scale_out && !plain_dw) { p.scale_out = 1; d_gated = true; }
                     }
                 }
                 snprintf(nm, sizeof nm, "b%02d.k1", b.idx);
@@ -810,18 +840,18 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
         if (rc) return rc;
         if (taps) {
             snprintf(nm, sizeof nm, "dw%d", b.idx);
-            if ((rc = add_tap<T>(c, nm, D, (size_t)nb * b.hout * b.hout * b.cexp))) return rc;
+            if ((rc = add_tap<T>(c, nm, D, (size_t)b.hout * b.hout * b.cexp, off, nb, d_gated))) return rc;
             snprintf(nm, sizeof nm, "gate%d", b.idx);
-            if ((rc = add_tap<float>(c, nm, c->d_gate, (size_t)nb * b.cexp))) return rc;
+            if ((rc = add_tap<float>(c, nm, c->d_gate, (size_t)b.cexp, off, nb))) return rc;
             snprintf(nm, sizeof nm, "block%d", b.idx);
-            if ((rc = add_tap<T>(c, nm, oth, (size_t)nb * b.hout * b.hout * b.cout))) return rc;
+            if ((rc = add_tap<T>(c, nm, oth, (size_t)b.hout * b.hout * b.cout, off, nb))) return rc;
         }
         std::swap(cur, oth);
     }
     int rc = launch_pw<T>(c, "head.conv", cur, c->w_head, c->wt_head, c->b_head, nullptr, nullptr, E,
                           (long long)nb * 49, 320, 1280, 49, true);
     if (rc) return rc;
-    if (taps && (rc = add_tap<T>(c, "head", E, (size_t)nb * 49 * 1280))) return rc;
+    if (taps && (rc = add_tap<T>(c, "head", E, (size_t)49 * 1280, off, nb))) return rc;
     {
         Scope sc(c, "head.fc_decode", (double)nb * (49.0 * 1280 * sizeof(T) + 12), 2.0 * nb * (1280.0 * 252 + 49 * 1280));
         if (nb >= 64 && c->head_batch) {
@@ -838,7 +868,7 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                                                                          taps ? c->d_pooled : nullptr);
         CK(cudaGetLastError());
     }
-    if (taps && (rc = add_tap<float>(c, "pooled", c->d_pooled, (size_t)nb * 1280))) return rc;
+    if (taps && (rc = add_tap<float>(c, "pooled", c->d_pooled, (size_t)1280, off, nb))) return rc;
     return 0;
 }
 
@@ -913,6 +943,7 @@ int upload_input(whenet_ctx* c, void* dst, const void* src, size_t bytes, cudaSt
 
 template <typename T, bool IN_U8>
 int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* angles_out, float* logits_out, int out_is_device) {
+    for (auto& kv : c->taps) kv.second.valid = false;     // a tap is only ever read from the forward that wrote it
     int rc = ensure_ws(c);
     if (rc) return rc;
     const size_t in_es = IN_U8 ? 1 : 4;
@@ -920,7 +951,7 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
     float* d_ang = out_is_device ? angles_out : c->d_angles_slot[oslot];
     float* d_log = logits_out ? (out_is_device ? logits_out : c->d_logits_slot[oslot]) : nullptr;
     // ---- device-resident forwards can be replayed from a captured graph (66 -> 1 launch; small-batch latency)
-    const bool graphable = c->use_graph && in_is_device && out_is_device && !c->prof_on && !c->taps_on;
+    const bool graphable = c->use_graph && in_is_device && out_is_device && !c->prof_on && !c->taps_mode;
     GraphKey key{n, IN_U8 ? 1 : 0, c->cfg_epoch, in, d_ang, d_log};
     if (graphable) {
         for (auto& g : c->graphs)
@@ -934,7 +965,21 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
     const int64_t launches0 = c->launches;
     // ---- two-stream mode (device-resident input, one pass): the two half batches run on two streams so that the
     //      low-occupancy kernels of one half (late K1 blocks: one CTA per SM) share the SMs with kernels of the other
-    if (c->n_streams >= 2 && !graphable && !c->taps_on && n <= c->chunk && n >= 64) {
+    const bool two_streams = c->n_streams >= 2 && !graphable && c->taps_mode != 1 && n <= c->chunk && n >= 64;
+    const int step = in_is_device ? c->chunk : std::max(1, std::min(c->chunk, c->host_chunk));
+    if (c->taps_mode) {
+        // mode 1: the first chunk if it has at most 8 crops (one stream); mode 2: the selected crops, or all of them
+        std::vector<int> crops;
+        if (c->taps_mode == 2 && !c->tap_sel.empty()) {
+            for (int i : c->tap_sel)
+                if (i >= n) return fail(WHENET_EINVAL, "tapped crop %d outside the call's %d crops", i, n);
+            crops = c->tap_sel;
+        }
+        else if (c->taps_mode == 2 || std::min(step, n) <= 8)
+            for (int i = 0; i < (c->taps_mode == 2 ? n : std::min(step, n)); ++i) crops.push_back(i);
+        if ((rc = prepare_taps(c, crops))) return rc;
+    }
+    if (two_streams) {
         const size_t es = esize(c->precision);
         const int parts = c->n_streams;
         const int per = (n + parts - 1) / parts;
@@ -964,7 +1009,7 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
             c->d_partial = sv.part + (size_t)off * c->ws_part;    c->d_gate = sv.gate + (size_t)off * 1152;
             c->d_pooled = sv.pooled + (size_t)off * 1280;         c->d_se_counter = sv.ctr + off;
             rc2 = forward_chunk<T, IN_U8>(c, d_src, nb, d_ang + (size_t)off * 3,
-                                          d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr, false);
+                                          d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr, c->taps_mode == 2, off);
             if (rc2 == 0 && cudaEventRecord(c->ev_join[h], c->aux_stream[h]) != cudaSuccess) rc2 = fail(WHENET_ECUDA, "event record failed");
         }
         c->bufA = sv.A; c->bufB = sv.B; c->bufE = sv.E; c->bufD = sv.D;
@@ -984,7 +1029,6 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
         }
         return 0;
     }
-    const int step = in_is_device ? c->chunk : std::max(1, std::min(c->chunk, c->host_chunk));
     int ci = 0;
     for (int off = 0; off < n; off += step, ++ci) {
         const int nb = std::min(step, n - off);
@@ -1001,7 +1045,7 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
             d_in = c->d_in[slot];
         }
         rc = forward_chunk<T, IN_U8>(c, d_in, nb, d_ang + (size_t)off * 3, d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr,
-                                     c->taps_on && off == 0 && nb <= 8);
+                                     c->taps_mode == 2 || (c->taps_mode == 1 && off == 0 && nb <= 8), off);
         if (rc) {
             if (graphable) { cudaGraph_t g = nullptr; cudaStreamEndCapture(c->stream, &g); if (g) cudaGraphDestroy(g); }
             return rc;
@@ -1869,20 +1913,38 @@ void whenet_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 int whenet_debug_enable_taps(whenet_ctx* c, int enable) {
     if (!c) return fail(WHENET_EINVAL, "null context");
-    c->taps_on = enable != 0;
+    if (enable < 0 || enable > 2) return fail(WHENET_EINVAL, "tap mode %d is not 0, 1 or 2", enable);
+    c->taps_mode = enable;
+    return 0;
+}
+
+int whenet_debug_tap_crops(whenet_ctx* c, const int* idx, int k) {
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    if (k < 0 || k > 64 || (k > 0 && !idx)) return fail(WHENET_EINVAL, "select 0..64 crops (got %d)", k);
+    for (int i = 0; i < k; ++i)
+        if (idx[i] < 0) return fail(WHENET_EINVAL, "negative crop index %d", idx[i]);
+    c->tap_sel.assign(idx, idx + k);
     return 0;
 }
 
 int whenet_debug_tap(whenet_ctx* c, const char* name, float* out, size_t cap, size_t* n_elems) {
     if (!c || !name) return fail(WHENET_EINVAL, "bad arguments");
-    auto it = c->taps.find(name);
-    if (it == c->taps.end()) return fail(WHENET_ENOTFOUND, "no tap named %s (enable taps and run a forward with n<=8)", name);
-    if (n_elems) *n_elems = it->second.second;
+    // "dwg%d" reads the "dw%d" buffer when the last forward gated that block's depthwise output in place
+    const bool want_gated = !strncmp(name, "dwg", 3);
+    const std::string key = want_gated ? "dw" + std::string(name + 3) : std::string(name);
+    auto it = c->taps.find(key);
+    if (it == c->taps.end() || !it->second.valid)
+        return fail(WHENET_ENOTFOUND, "the last forward wrote no tap named %s (taps off, or mode 1 with more than 8 crops)", name);
+    const whenet_ctx::Tap& t = it->second;
+    if (!strncmp(name, "dw", 2) && t.forms == 3) return fail(WHENET_EINVAL, "tap %s holds gated and ungated crops", name);
+    if (!strncmp(name, "dw", 2) && t.forms != 0 && (t.forms == 2) != want_gated)
+        return fail(WHENET_ENOTFOUND, "no tap named %s: the last forward wrote %s%s", name, want_gated ? "dw" : "dwg", key.c_str() + 2);
+    if (n_elems) *n_elems = t.n;
     if (!out) return 0;
-    if (cap < it->second.second) return fail(WHENET_EINVAL, "tap %s needs %zu elements, buffer holds %zu", name, it->second.second, cap);
+    if (cap < t.n) return fail(WHENET_EINVAL, "tap %s needs %zu elements, buffer holds %zu", name, t.n, cap);
     CK(cudaSetDevice(c->device));
-    CK(cudaStreamSynchronize(c->stream));
-    CK(cudaMemcpy(out, it->second.first, it->second.second * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaStreamSynchronize(c->stream));                 // the halves' streams (and their tap copies) joined it
+    CK(cudaMemcpy(out, t.p, t.n * sizeof(float), cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -2106,7 +2168,8 @@ void whenet_destroy(whenet_ctx* c) {
     if (c->d_rects) cudaFree(c->d_rects);
     if (c->d_frame_of) cudaFree(c->d_frame_of);
     if (c->d_segs) cudaFree(c->d_segs);
-    for (auto& kv : c->taps) cudaFree(kv.second.first);
+    for (auto& kv : c->taps) cudaFree(kv.second.p);
+    if (c->d_tap_map) cudaFree(c->d_tap_map);
     for (auto& p : c->ev_used) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }
     for (auto e : c->ev_pool) cudaEventDestroy(e);
     if (c->d_arena) cudaFree(c->d_arena);

@@ -252,8 +252,14 @@ class WHENet:
     def set_option(self, key: str, value: int):
         check(self._L.whenet_set_option(self._h, key.encode(), int(value)))
 
-    def enable_taps(self, on: bool = True):
-        check(self._L.whenet_debug_enable_taps(self._h, int(on)))
+    def enable_taps(self, on: bool = True, faithful: bool = False, crops=None):
+        """Record intermediate tensors of the next forwards (``tap``).  ``faithful=False``: the first chunk of at most 8
+        crops, on a one-stream route with ungated depthwise outputs.  ``faithful=True``: every chunk at any batch, on the
+        route of the untapped call (in-place gated depthwise outputs are named ``dwg%d``); ``crops`` limits the taps to
+        those crop indices of each call, in that order (at most 64; None: every crop)."""
+        sel = np.ascontiguousarray(np.asarray([] if crops is None else list(crops), dtype=np.int32))
+        check(self._L.whenet_debug_tap_crops(self._h, _ptr(sel) if sel.size else None, int(sel.size)))
+        check(self._L.whenet_debug_enable_taps(self._h, (2 if faithful else 1) if on else 0))
 
     def tap(self, name: str) -> np.ndarray:
         n = C.c_size_t(0)

@@ -171,11 +171,23 @@ void  whenet_host_free(void* p);
 
 /* ---- test / measurement hooks (no reference counterpart) ---- */
 
-/* Keep float32 copies of intermediate tensors of the NEXT forwards
- * ("stem", "dw1".."dw16", "gate1".."gate16", "block1".."block16", "head",
- * "pooled"); only for n <= 8. */
+/* Keep float32 copies of intermediate tensors of the NEXT forwards ("stem", "dw1".."dw16" or "dwg1".."dwg16",
+ * "gate1".."gate16", "block1".."block16", "head", "pooled"), crop-major, one row per tapped crop.
+ * enable = 0: off.
+ * enable = 1: the first chunk of the call, if it has at most 8 crops.  The forward then runs on one stream and leaves every
+ *   depthwise output ungated ("dw%d"), so its route can differ from the untapped one.
+ * enable = 2: every chunk and both halves of a two-stream pass, at any batch, on the untapped route: the launches and every
+ *   kernel parameter are those of the same call without taps.  The one difference: where the one-CTA head kernel alone has
+ *   the pooled vector (batches below 64), it also writes it out for the "pooled" tap.  A block whose depthwise output was
+ *   gated in place (the SE tails' scale_out) records the 16-bit d * g as "dwg%d" instead of "dw%d".  The tap buffers are
+ *   allocated before the first kernel.  Without a selection (whenet_debug_tap_crops) every crop is tapped: 12.8 MB per crop.
+ * Every forward invalidates the previous taps; a tapped forward under enable != 0 never replays a captured graph. */
 int whenet_debug_enable_taps(whenet_ctx* ctx, int enable);
-/* Copy a tap to host; *n_elems receives its element count (call with out=NULL to query). */
+/* Mode 2: tap only crops idx[0..k) of each call, in that order (k <= 64; k = 0 taps every crop).  A forward with an index
+ * >= its batch fails with WHENET_EINVAL before its first launch. */
+int whenet_debug_tap_crops(whenet_ctx* ctx, const int* idx, int k);
+/* Copy a tap to host; *n_elems receives its element count (call with out=NULL to query).  WHENET_ENOTFOUND for a tap the
+ * last forward did not write. */
 int whenet_debug_tap(whenet_ctx* ctx, const char* name, float* out, size_t cap_elems, size_t* n_elems);
 
 /* Run ONE 1x1 convolution through the kernel family chosen by use_tc (0 CUDA-core, 1 tensor core):

@@ -1,8 +1,8 @@
 """Every WHENet stage on the GPU, element by element, against float64 on its own GPU input (DESIGN §2.1).
 
 A stage's input is the previous tap (an exact float32 copy of the storage type), so |got - ref| <= 2 B must hold for every
-element, B being the first-order bound of tests/whenet_bounds.py (validated on the CPU by test_whenet_bounds_cpu.py).
-The routes below reach every 16-bit block kernel of the product; the profile's layer names pin which one ran.
+element, B being the first-order bound of tests/whenet_bounds.py (validated on the CPU by test_whenet_bounds_cpu.py); the
+checker is tests/elementwise_check.py.  The routes below reach every 16-bit block kernel of the product; the profile's layer names pin which one ran.
 
 Negative controls run on the reference side only, on the default bf16 route's data: a transposed depthwise kernel, an E
 tile read one pixel off, symmetric padding on the stride-2 stages, a squeeze that loses the map's last row and a project
@@ -13,9 +13,10 @@ import os
 import numpy as np
 import pytest
 
+import elementwise_check as ec
 import whenet_bounds as wb
 from conftest import GOLD, SNAP
-from whenet_oracle import depthwise_same, load_oracle, preprocess, softmax, swish
+from whenet_oracle import depthwise_same, load_oracle, preprocess, swish
 
 pytestmark = pytest.mark.gpu
 
@@ -71,53 +72,7 @@ def oracle():
 @pytest.fixture(scope="module", autouse=True)
 def ratio_table():
     yield RATIOS
-    kinds = ["stem", "dw", "gate", "block", "head", "pooled", "angles"]
-    print("\nworst |got - ref| / B per route and tap kind (assertion: <= 2); share within one ulp of the storage type")
-    print("%-14s" % "route" + "".join("%9s" % k for k in kinds) + "   1-ulp")
-    for route, d in RATIOS.items():
-        print("%-14s" % route + "".join("%9.3f" % d[k][0] if k in d else "%9s" % "-" for k in kinds) +
-              "   %.4f" % d["_ulp"])
-
-
-def _check(route, kind, name, got, ref, b, shape, store, stats):
-    got = got.reshape(shape).astype(np.float64)
-    assert np.isfinite(got).all(), (route, name, "non-finite values")
-    err = np.abs(got - ref)
-    r = err / b
-    i = np.unravel_index(int(np.argmax(r)), r.shape)
-    assert r[i] <= 2.0, ("%s %s: element %s got %.9g ref %.9g B %.3g (ratio %.2f)" %
-                         (route, name, tuple(int(v) for v in i), got[i], ref[i], b[i], r[i]))
-    prev = stats.setdefault(kind, (0.0, ""))
-    if r[i] > prev[0]:
-        stats[kind] = (float(r[i]), name)
-    if store is not None:
-        stats["_n"] = stats.get("_n", 0) + err.size
-        stats["_in"] = stats.get("_in", 0) + int((err <= wb.ulp(ref, store)).sum())
-    return got
-
-
-def _project_forms(oracle, b, d, g, res):
-    """Share of the GPU's bf16 project outputs reproduced bit for bit by each gate rounding (fp32 accumulation and
-    epilogue emulated; the few elements whose accumulation order flips a rounding do not match either way)."""
-    k, sh = oracle._fold(b["proj"], b["proj_bn"])
-    wq = _bf16(k[0, 0])
-    n, c = d.shape[0], d.shape[3]
-    acc = {"w*g": np.einsum("npk,nkj->npj", d.reshape(n, -1, c), _bf16(wq[None] * g[:, :, None])),
-           "a*g": _bf16(d * g[:, None, None, :]).reshape(n, -1, c) @ wq}
-    out = {}
-    for form, v in acc.items():
-        y = _f32(_f32(v.reshape(d.shape[:3] + (wq.shape[1],))) + _f32(sh))
-        out[form] = _bf16(_f32(y + res) if res is not None else y)
-    return out
-
-
-def _bf16(x):
-    import torch
-    return torch.from_numpy(np.asarray(x, dtype=np.float64)).to(torch.bfloat16).to(torch.float64).numpy()
-
-
-def _f32(x):
-    return np.asarray(x, dtype=np.float64).astype(np.float32).astype(np.float64)
+    ec.print_table(RATIOS, "worst |got - ref| / B per route and tap kind (assertion: <= 2); share within one ulp of the storage type")
 
 
 def _run_route(m, x, nb, a, route, oracle, blocks, expect, keep_refs=False):
@@ -137,59 +92,10 @@ def _run_route(m, x, nb, a, route, oracle, blocks, expect, keep_refs=False):
     m.enable_taps(True)
     ang = np.stack(m.get_angle(x), axis=1).astype(np.float64)
     m.enable_taps(False)
-    stats = {}
-    keep = {}
-    xn = preprocess(x)
-    r = oracle.run_stage("stem", xn)
-    stem = m.tap("stem").reshape(r["out"].shape).astype(np.float64)
-    if a.stem_store == "fp16" and a.store == "bf16":
-        assert np.array_equal(stem.astype(np.float16).astype(np.float64), stem), "stem tap is not fp16"
-    _check(route, "stem", "stem", stem, r["out"], wb.stem(r, a), r["out"].shape, a.stem_store, stats)
-    if keep_refs:
-        keep["stem"] = (stem, r)
-    prev = stem
-    for i in range(1, 17):
-        b = blocks[i - 1]
-        rd = oracle.run_stage("dw", prev, i)
-        b_e = wb.expand(rd, a, prev.shape[-1]) if b["expand"] is not None else None
-        bd = wb.depthwise(rd, a, i, b["stride"], b_e)
-        d = _check(route, "dw", "dw%d" % i, m.tap("dw%d" % i), rd["out"], bd, rd["out"].shape, a.store, stats)
-        hw = d.shape[1] * d.shape[2]
-        rg = oracle.run_stage("gate", d, i)
-        g = _check(route, "gate", "gate%d" % i, m.tap("gate%d" % i), rg["out"], wb.gate(rg, a, np.abs(d).mean(axis=(1, 2)), hw),
-                   rg["out"].shape, None, stats)
-        res = prev if b["skip"] else None
-        rp = oracle.run_stage("project", d, i, gate=g, resid=res)
-        y = _check(route, "block", "block%d" % i, m.tap("block%d" % i), rp["out"], wb.project(rp, a, d.shape[-1]),
-                   rp["out"].shape, a.store, stats)
-        if route in PROJECT_FORM and i <= 5:
-            forms = _project_forms(oracle, b, d, g, res)
-            share = {f: float((v == y).mean()) for f, v in forms.items()}
-            other = "a*g" if PROJECT_FORM[route] == "w*g" else "w*g"
-            print("%s block %d project: bitwise share %s" % (route, i, share))
-            assert share[PROJECT_FORM[route]] >= 0.9 and share[PROJECT_FORM[route]] > share[other] + 0.05, (route, i, share)
-        if keep_refs:
-            keep[i] = (prev, rd, bd, d, rg, g, rp, y)
-        prev = y
-    rh = oracle.run_stage("head", prev)
-    h = _check(route, "head", "head", m.tap("head"), rh["out"], wb.head(rh, a), rh["out"].shape, a.store, stats)
-    p = _check(route, "pooled", "pooled", m.tap("pooled"), h.mean(axis=(1, 2)), wb.pooled(h), (nb, 1280), None, stats)
-    rdn = oracle.run_stage("dense", p)
-    ref_ang = np.stack([v.astype(np.float64) for v in _decode64(rdn["logits"])], axis=1)
-    _check(route, "angles", "angles", ang, ref_ang, np.stack(wb.angles(rdn, rdn["logits"]), axis=1), (nb, 3), None, stats)
-    stats["_ulp"] = stats["_in"] / stats["_n"]
-    RATIOS[route] = stats
-    print("%s: worst ratio %s; %.4f of stored elements within one ulp" %
-          (route, {k: "%.3f (%s)" % v for k, v in stats.items() if not k.startswith("_")}, stats["_ulp"]))
+    keep = {} if keep_refs else None
+    RATIOS[route] = ec.check_stages(route, ec.tap_reader(m), x, ang, a, oracle, blocks, {}, keep=keep,
+                                    project_form=PROJECT_FORM.get(route))
     return keep
-
-
-def _decode64(logits):
-    out = []
-    for lg, off in zip(logits, (180.0, 99.0, 99.0)):
-        v = np.arange(lg.shape[1], dtype=np.float64)
-        out.append((softmax(lg) * v).sum(axis=1) * 3 - off)
-    return out
 
 
 def _exceeds(got, ref, b):

@@ -42,18 +42,32 @@ def _model(n, streams=1, graph=0):
     return m
 
 
-def test_taps_bit_identical_around_the_grid():
-    """One stream with taps: the dw / gate / block taps of blocks 2-6 and the angles, at every batch of _batches()."""
+def _per_crop():
+    """Elements per crop of the dw / gate / block taps of blocks 2-6."""
+    from whenet_b200 import arch
+    out = {}
+    for b in arch.blocks():
+        if b.idx in EARLY:
+            out.update({"dw%d" % b.idx: b.hout * b.hout * b.cexp, "gate%d" % b.idx: b.cexp, "block%d" % b.idx: b.hout * b.hout * b.cout})
+    return out
+
+
+def test_faithful_taps_bit_identical_around_the_grid():
+    """One stream with faithful taps (the untapped route, every crop): the dw / gate / block taps of blocks 2-6 and the
+    angles, at every batch of _batches().  Each tap must hold exactly n crops, so no tap of an earlier call can pass."""
     batches = _batches()
+    per = _per_crop()
     m = _model(max(batches))
-    m.enable_taps(True)
+    m.enable_taps(True, faithful=True)
     for n in batches:
         crops = _crops(n, 100 + n)
         got = {}
         for route in (0, 1):
             m.set_option("k1x", route)
             ang = np.stack(m.get_angle(crops), axis=1)
-            got[route] = (ang, {"%s%d" % (k, i): m.tap("%s%d" % (k, i)) for i in EARLY for k in ("dw", "gate", "block")})
+            got[route] = (ang, {k: m.tap(k) for k in per})
+            for k, v in got[route][1].items():
+                assert v.size == n * per[k], (n, route, k, v.size)
         assert np.isfinite(got[0][0]).all() and np.array_equal(got[0][0], got[1][0]), n
         for k, v in got[0][1].items():
             assert np.array_equal(v, got[1][1][k]), (n, k)

@@ -21,14 +21,35 @@ def _crops(sample_crops, jitter_crops, n):
     return np.clip(crops, 0, 255).astype(np.uint8)
 
 
-def _taps(m):
-    return {"%s%d" % (k, i): m.tap("%s%d" % (k, i)) for i in LATE for k in ("dw", "gate", "block")}
+def _taps(m, n):
+    """dw (dwg where the depthwise output was gated in place) / gate / block taps of blocks 7-16, (n, elements) each."""
+    from whenet_b200 import WhenetError
+    out = {}
+    for i in LATE:
+        for k in ("dw", "gate", "block"):
+            try:
+                v = m.tap("%s%d" % (k, i))
+            except WhenetError:
+                if k != "dw":
+                    raise
+                k, v = "dwg", m.tap("dwg%d" % i)
+            out["%s%d" % (k, i)] = v.reshape(n, -1)
+    return out
+
+
+def _gate16(d, g):
+    """round16(float32(d) * float32(g)) in bf16: what the in-place gate of the SE tail stores."""
+    import torch
+    dg = d.reshape(d.shape[0], -1, g.shape[1]).astype(np.float32) * g.astype(np.float32)[:, None, :]
+    return torch.from_numpy(dg).to(torch.bfloat16).float().numpy().reshape(d.shape)
 
 
 @pytest.mark.parametrize("kd_tail", [0, 1])
 def test_on_chip_expand_matches_split_route(sample_crops, jitter_crops, kd_tail):
-    """256 crops in one pass (one CTA per crop, E on chip) against 8-crop passes (chunks split over CTAs, E through memory);
-    the dw / gate / block taps (recorded for passes of at most 8 crops) with the on-chip route forced at 8 crops."""
+    """256 crops in one pass (one CTA per crop, E on chip) against 8-crop passes (chunks split over CTAs, E through memory).
+    The 256-crop pass's own dw / gate / block taps (faithful taps: the launches of the untapped pass) against those of the
+    8-crop split passes.  With kd_tail=1 the 256-crop pass gates its depthwise output in place (dwg%d); the split route's
+    ungated d then has to give it exactly as round16(float32(d) * float32(g))."""
     import whenet_b200
     n, part = 256, 8
     crops = _crops(sample_crops, jitter_crops, n)
@@ -39,18 +60,22 @@ def test_on_chip_expand_matches_split_route(sample_crops, jitter_crops, kd_tail)
     whole = np.stack(m.get_angle(crops), axis=1)
     parts = np.concatenate([np.stack(m.get_angle(crops[i:i + part]), axis=1) for i in range(0, n, part)])
     assert np.array_equal(whole, parts)
-    m.enable_taps(True)
+    m.enable_taps(True, faithful=True)
+    assert np.array_equal(np.stack(m.get_angle(crops), axis=1), whole)
+    whole_taps = _taps(m, n)
+    assert sum(k.startswith("dwg") for k in whole_taps) == (len(LATE) if kd_tail else 0), sorted(whole_taps)
+    m.set_option("k1_split_ctas", 120)                       # 8 crops: chunks split over CTAs -> expand GEMM + KD
     for i in (0, 120, 248):
-        sub = crops[i:i + part]
-        m.set_option("k1_split_ctas", 120)                   # 8 crops: chunks split over CTAs -> expand GEMM + KD
-        split = np.stack(m.get_angle(sub), axis=1)
-        split_taps = _taps(m)
-        m.set_option("k1_split_ctas", 0)                     # one CTA per crop -> expand on chip
-        fused = np.stack(m.get_angle(sub), axis=1)
-        fused_taps = _taps(m)
-        assert np.array_equal(fused, split) and np.array_equal(fused, whole[i:i + part])
-        for k, v in fused_taps.items():
-            assert np.array_equal(v, split_taps[k]), (i, k)
+        split = np.stack(m.get_angle(crops[i:i + part]), axis=1)
+        split_taps = _taps(m, part)
+        assert np.array_equal(split, whole[i:i + part])
+        for k, v in whole_taps.items():
+            if k.startswith("dwg") and k not in split_taps:
+                blk = int(k[3:])
+                ref = _gate16(split_taps["dw%d" % blk], split_taps["gate%d" % blk])
+            else:
+                ref = split_taps[k]
+            assert np.array_equal(v[i:i + part], ref), (i, k)
     m.close()
 
 

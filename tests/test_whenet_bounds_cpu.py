@@ -3,7 +3,8 @@
 Each kernel family's rounding steps are emulated in numpy / torch at every block's real shapes and weights (bf16
 rounding through torch, fp16 through numpy, fused fp16 / fp32 FMAs as one rounding of the exact float64 result, tanh
 perturbed by +-2^-11 relative, the fp32 tensor-core mode's operands split into bf16 hi + lo with the lo * lo product
-dropped), on the oracle's activations of a committed crop and of a uniform-random crop.  The
+dropped, the in-place gate of the SE tails as a 16-bit rounding of the fp32 product), on the oracle's activations of a
+committed crop and of a uniform-random crop.  The
 emulated error must stay inside B (the GPU test allows 2 B); the worst emulated / B per family is printed.
 """
 import os
@@ -149,7 +150,12 @@ def emulate_block(o, blk, b, x, a, sgn, route_k2=False):
     a1 = f32(z1 / (1 + np.exp(-z1.astype(np.float32))))
     z2 = f32(a1.astype(np.float32) @ rg["w2"].astype(np.float32) + o.w[b["se"][1] + "/bias:0"])
     g = f32(1 / (1 + np.exp(-z2.astype(np.float32))))
-    out["gate"] = (g, rg["out"], wb.gate(rg, a, np.abs(d).mean(axis=(1, 2)), ho * ho))
+    b_g = wb.gate(rg, a, np.abs(d).mean(axis=(1, 2)), ho * ho)
+    out["gate"] = (g, rg["out"], b_g)
+    if a.sixteen:
+        # the SE tails' in-place gate (scale_out): round16(float32(d) * float32(g)), against the float64 d * g
+        dg = rnd(f32(d * g[:, None, None, :]), a.store)
+        out["gated"] = (dg, ri["out"] * rg["out"][:, None, None, :], wb.gated(out["dw"][2], ri["out"], rg["out"], b_g, a))
     # project: pw_tc2 / pw_tc3 round bf16(w) * g, K2 rounds d * g; the fp32 kernels gate A in fp32
     k, sh = o._fold(b["proj"], b["proj_bn"])
     k = k[0, 0]
@@ -203,4 +209,4 @@ def test_emulated_error_within_bound(a, acts):
         print("%s %-10s worst emulated/B = %.3f (block %d, element %s)" % (a.weights, fam, r, blk, i))
     for fam, (r, blk, i) in worst.items():
         assert r <= 1.0, (a.weights, fam, r, blk, i)
-    assert set(worst) >= {"stem", "expand", "dw_" + a.dw, "dw_" + a.dw1, "gate", "project", "head"}
+    assert set(worst) >= {"stem", "expand", "dw_" + a.dw, "dw_" + a.dw1, "gate", "project", "head"} | ({"gated"} if a.sixteen else set())

@@ -106,11 +106,12 @@ def depthwise(r, a: Arith, block: int, stride: int, b_e=None):
     return swish_bound(r["pre"], b_pre, a, fast=a.sixteen) + U[a.store] * np.abs(r["out"])
 
 
-def gate(r, a: Arith, d_abs_mean, hw: int):
+def gate(r, a: Arith, d_abs_mean, hw: int, b_in_mean=None):
     """SE gate from the squeeze sums.  The sums are formed from the fp32 depthwise values BEFORE the 16-bit store
     (dw_strip_finish), while the reference starts from the stored tap: u_store mean|d|, plus hw fp32 additions.  Then two
-    fp32 FCs (K+1 roundings each), swish and sigmoid through expf."""
-    b_mean = (U[a.store] + (hw + 1) * U32) * d_abs_mean
+    fp32 FCs (K+1 roundings each), swish and sigmoid through expf.  b_in_mean: the mean distance of the reference's input
+    from the values the kernel summed, where it is not the stored tap (default u_store mean|d|)."""
+    b_mean = (U[a.store] * d_abs_mean if b_in_mean is None else b_in_mean) + (hw + 1) * U32 * d_abs_mean
     cexp = r["w1"].shape[0]
     cse = r["w1"].shape[1]
     b_z1 = b_mean @ np.abs(r["w1"]) + (cexp + 1) * U32 * r["S_z1"]
@@ -118,6 +119,15 @@ def gate(r, a: Arith, d_abs_mean, hw: int):
     b_z2 = b_a @ np.abs(r["w2"]) + (cse + 1) * U32 * r["S_z2"]
     g = r["out"]
     return g * (1 - g) * b_z2 + 4 * U32 * g
+
+
+def gated(b_dw, d, g, b_gate, a: Arith):
+    """A depthwise output gated in place by the SE tail (scale_out, recorded as "dwg"): the stored d (within b_dw of the
+    reference d) times the fp32 gate g (within b_gate), one fp32 product and one 16-bit store: |g| B_dw + |d| B_gate +
+    u_store |d g|.  d: (n, h, w, c), g: (n, c)."""
+    g4 = np.asarray(g)[:, None, None, :]
+    b_g4 = np.asarray(b_gate)[:, None, None, :]
+    return np.abs(g4) * b_dw + np.abs(d) * b_g4 + (U[a.store] + U32) * np.abs(d * g4)
 
 
 def project(r, a: Arith, k: int):
