@@ -17,6 +17,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 namespace whenet {
 
 // ----------------------------------------------------------------------------- storage helpers
@@ -179,88 +181,186 @@ __global__ void __launch_bounds__(256) stem_kernel(const void* __restrict__ in_,
     st8(out + (gid >> 2) * 32 + cg * 8, acc);
 }
 
-// ----------------------------------------------------------------------------- stem, tiled
-// One CTA = two output rows of one crop (224 threads, one output pixel x 32 channels each).
-// The 5 input rows are loaded with 16-byte vectors, normalised through the LUT once and staged as fp32 in
-// shared memory (one extra zero pixel/row: TF-SAME puts its single pad row/column AFTER index 223).
-// The 27x32 BN-folded weights + 32 shifts arrive as a __grid_constant__ kernel parameter, so every FFMA
-// takes its weight straight from the constant bank (864 FFMA per thread, no weight loads at all).
+// ----------------------------------------------------------------------------- stem, register-blocked
+// A tile = 8 output rows of one crop; a persistent CTA of 224 threads walks tiles blockIdx.x, + gridDim.x, ...  A thread
+// computes 4 consecutive output pixels along x x 16 channels (64 fp32 accumulators), first for channels 0-15, then for
+// 16-31: the channel half is a template argument, so every weight address is warp-uniform and an immediate.  The 27x32
+// BN-folded weights sit in shared memory and are read as broadcast 16-byte loads; each weight feeds 4 FFMAs (one per
+// pixel).  Each output is bias + fmaf over (ky, kx, ci) in that order, then swish: the padding taps are FMA'd with
+// staged zeros (fmaf(0, w, acc) decides the sign of a zero).
+//
+// The tile's 17 input rows arrive raw by cp.async, issued while the previous tile computes, and are then converted once
+// to fp32 (u8 through the LUT) in 9 planes per row, plane kx*3+ci holding x[2*ox + kx][ci] for ox = 0..111 (TF SAME
+// puts its single pad row/column after index 223: row 224 and the last element of the kx = 2 planes are zeros).  A tap
+// is then one conflict-free 16-byte load of the thread's 4 pixels.  Each half's outputs go through shared memory
+// (XOR-swizzled 16-byte chunks) and leave as whole 32-byte sectors.
 struct StemParams { float w[27 * 32]; float b[32]; };
 
-template <typename T, bool IN_U8, bool FAST>
-__global__ void __launch_bounds__(224) stem_tile_kernel(const void* __restrict__ in_, T* __restrict__ out,
-                                                        const __grid_constant__ StemParams sp,
-                                                        const float* __restrict__ lut) {
-    constexpr int ROWF = 225 * 3 + 1;              // floats per staged row (225 pixels incl. the zero pad pixel)
-    __shared__ float s_in[5 * ROWF];
-    __shared__ float s_lut[768];
-    const int tid = threadIdx.x;
-    const int n = blockIdx.y, oy0 = blockIdx.x * 2;
-    if (IN_U8) {
-        for (int i = tid; i < 768; i += 224) s_lut[i] = lut[i];
-        __syncthreads();
-    }
-    // stage rows 2*oy0 .. 2*oy0+4 (row 224 does not exist -> zeros)
-    if (IN_U8) {
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(in_) + (long long)n * 224 * 224 * 3;
-        for (int v = tid; v < 5 * 42; v += 224) {           // 42 x 16 bytes per input row
-            const int r = v / 42, q = v - r * 42;
-            const int iy = 2 * oy0 + r;
-            float* dst = &s_in[r * ROWF + q * 16];
-            if (iy < 224) {
-                const uint4 raw = *reinterpret_cast<const uint4*>(src + (long long)iy * 672 + q * 16);
-                const uint8_t* b = reinterpret_cast<const uint8_t*>(&raw);
+constexpr int kStemRows = 8;                      // output rows per tile
+constexpr int kStemTilesPerCrop = 112 / kStemRows;
+constexpr int kStemThreads = kStemRows * 28;      // one thread per quad of output pixels
+constexpr int kStemPlane = 112;                   // floats per plane (one per output column)
+constexpr int kStemRowF = 9 * kStemPlane + 8;     // floats per staged input row; 8 mod 16 keeps a quarter-warp that spans
+                                                  // two output rows (input rows 2 apart) on disjoint banks
+constexpr int kStemInRows = 2 * kStemRows + 1;
+
+// shared memory: planes | the stage of channels 0-15, which also holds the next tile's raw rows | LUT (u8) | weights.
+// Channels 16-31 are staged over the planes.  16-bit storage, u8 input: 102 KB, two CTAs per SM.
+template <typename T, bool IN_U8>
+struct StemSmem {
+    static constexpr size_t PLANES = (size_t)kStemInRows * kStemRowF * 4;
+    static constexpr size_t RAW_ROW = 672 * (IN_U8 ? 1 : 4);                     // bytes of one input row
+    static constexpr size_t STAGE = (size_t)kStemRows * 112 * 16 * sizeof(T);
+    static constexpr size_t RAW = (size_t)kStemInRows * RAW_ROW;
+    static constexpr size_t UNION = STAGE > RAW ? STAGE : RAW;
+    static constexpr size_t LUT = PLANES + UNION, W = LUT + (IN_U8 ? 768 * 4 : 0);
+    static constexpr size_t BYTES = W + 27 * 32 * 4;
+};
+
+// One channel half for pixel quad q (output row q / 28, columns 4 (q % 28) + 0..3): FMA, swish into `stage`, store.
+// HALF 1 stages over the planes, hence its barrier before the stage writes.
+template <int HALF, typename T, bool FAST>
+__device__ __forceinline__ void stem_half(const float* s_in, const float* s_w, uint4* stage, T* out_run, int q, int tid,
+                                          const StemParams& sp) {
+    float acc[4][16];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) dst[j] = s_lut[((q * 16 + j) % 3) * 256 + b[j]];
-            } else {
+    for (int c = 0; c < 16; ++c)
 #pragma unroll
-                for (int j = 0; j < 16; ++j) dst[j] = 0.f;
+        for (int p = 0; p < 4; ++p) acc[p][c] = sp.b[HALF * 16 + c];
+    const int oyl = q / 28;
+    const float* x0 = s_in + 2 * oyl * kStemRowF + 4 * (q - oyl * 28);
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int t = 0; t < 9; ++t) {                   // kx*3 + ci
+            const float4 x = *reinterpret_cast<const float4*>(x0 + ky * kStemRowF + t * kStemPlane);
+            const float xs[4] = {x.x, x.y, x.z, x.w};
+            float ws[16];
+#pragma unroll
+            for (int c4 = 0; c4 < 4; ++c4) {
+                const float4 w4 = *reinterpret_cast<const float4*>(s_w + (ky * 9 + t) * 32 + HALF * 16 + 4 * c4);
+                ws[4 * c4] = w4.x; ws[4 * c4 + 1] = w4.y; ws[4 * c4 + 2] = w4.z; ws[4 * c4 + 3] = w4.w;
             }
+#pragma unroll
+            for (int c = 0; c < 16; ++c)
+#pragma unroll
+                for (int p = 0; p < 4; ++p) acc[p][c] = fmaf(xs[p], ws[c], acc[p][c]);
         }
-    } else {
-        const float* src = reinterpret_cast<const float*>(in_) + (long long)n * 224 * 224 * 3;
-        for (int v = tid; v < 5 * 168; v += 224) {          // 168 x float4 per input row
-            const int r = v / 168, q = v - r * 168;
-            const int iy = 2 * oy0 + r;
-            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (iy < 224) x = *reinterpret_cast<const float4*>(src + (long long)iy * 672 + q * 4);
-            float* dst = &s_in[r * ROWF + q * 4];
-            dst[0] = x.x; dst[1] = x.y; dst[2] = x.z; dst[3] = x.w;
+    if (HALF == 1) __syncthreads();
+    // 16-byte chunk k of the half's stage (pixel k / CPH, chunk k % CPH of its 16 channels) is stored at
+    // k ^ ((k >> SH) & 7): a quarter-warp's chunks (same pixel slot, consecutive quads) then fall on distinct banks, and
+    // so do 8 consecutive chunks read back
+    constexpr int CPH = (int)sizeof(T);                     // 16-byte chunks per pixel and half (16 channels)
+    constexpr int SH = CPH == 2 ? 3 : 4;                    // log2(4 * CPH): k >> SH is the quad index
+    constexpr int VPC = 16 / (int)sizeof(T);                // values per chunk
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+#pragma unroll
+        for (int j = 0; j < CPH; ++j) {
+            const int k = (q * 4 + p) * CPH + j;
+            float o[VPC];
+#pragma unroll
+            for (int e = 0; e < VPC; ++e) o[e] = FAST ? swish_fast(acc[p][j * VPC + e]) : swish_f(acc[p][j * VPC + e]);
+            T* dst = reinterpret_cast<T*>(stage + (k ^ ((k >> SH) & 7)));
+            if constexpr (sizeof(T) == 2) st8<T>(dst, o);
+            else st4(dst, o);
         }
-    }
-    if (tid < 15) s_in[(tid / 3) * ROWF + 672 + tid % 3] = 0.f;   // pad pixel (column 224) of the 5 rows
     __syncthreads();
-    const int oyl = tid / 112, ox = tid - oyl * 112;
-    // 32 output channels as 16 pairs, weights from the constant bank, the scalar input broadcast
-    float2 acc2[16];
+    uint4* g = reinterpret_cast<uint4*>(out_run + HALF * 16);
 #pragma unroll
-    for (int c = 0; c < 16; ++c) acc2[c] = make_float2(sp.b[2 * c], sp.b[2 * c + 1]);
+    for (int k = tid; k < kStemRows * 112 * CPH; k += kStemThreads)
+        g[(k / CPH) * 2 * CPH + k % CPH] = stage[k ^ ((k >> SH) & 7)];
+}
+
+// cp.async the existing input rows 2*oy0 .. 2*oy0+16 of tile `tile` into `raw` (row 224 does not exist: never read)
+template <bool IN_U8>
+__device__ __forceinline__ void stem_fetch(const void* in_, char* raw, int tile, int tid) {
+    constexpr int ROW = 672 * (IN_U8 ? 1 : 4), CPR = ROW / 16;
+    const int n = tile / kStemTilesPerCrop, oy0 = (tile - n * kStemTilesPerCrop) * kStemRows;
+    const int rows = min(kStemInRows, 224 - 2 * oy0);
+    const char* src = reinterpret_cast<const char*>(in_) + ((long long)n * 224 + 2 * oy0) * ROW;
+    for (int i = tid; i < rows * CPR; i += kStemThreads) {
+        const uint32_t dst = (uint32_t)__cvta_generic_to_shared(raw + i * 16);
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src + (long long)i * 16) : "memory");
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+template <typename T, bool IN_U8, bool FAST>
+__global__ void __launch_bounds__(kStemThreads, 2) stem_tile_kernel(const void* __restrict__ in_, T* __restrict__ out,
+                                                                    const __grid_constant__ StemParams sp,
+                                                                    const float* __restrict__ lut, int n_img) {
+    using S = StemSmem<T, IN_U8>;
+    extern __shared__ float4 stem_smem_v[];
+    char* base = reinterpret_cast<char*>(stem_smem_v);
+    float* s_in = reinterpret_cast<float*>(base);
+    char* s_raw = base + S::PLANES;
+    uint4* stage0 = reinterpret_cast<uint4*>(base + S::PLANES);
+    float* s_lut = reinterpret_cast<float*>(base + S::LUT);
+    float* s_w = reinterpret_cast<float*>(base + S::W);
+    const int tid = threadIdx.x;
+    const int tiles = n_img * kStemTilesPerCrop;
+    int tile = blockIdx.x;
+    if (tile < tiles) stem_fetch<IN_U8>(in_, s_raw, tile, tid);
+    for (int i = tid; i < 27 * 32; i += kStemThreads) s_w[i] = sp.w[i];
+    if (IN_U8)
+        for (int i = tid; i < 768; i += kStemThreads) s_lut[i] = lut[i];
+    for (; tile < tiles; tile += gridDim.x) {
+        const int n = tile / kStemTilesPerCrop, oy0 = (tile - n * kStemTilesPerCrop) * kStemRows;
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        __syncthreads();                                    // raw rows in; the previous tile's output stage is drained
+        // item (r, m) = input columns 2m, 2m+1 of input row 2*oy0 + r
+        for (int i = tid; i < kStemInRows * 112; i += kStemThreads) {
+            const int r = i / 112, m = i - r * 112;
+            float v[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};    // row 224 (TF SAME's pad row) is staged as zeros
+            if (2 * oy0 + r < 224) {
+                const char* src = s_raw + r * S::RAW_ROW;
 #pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-        const float* row = &s_in[(2 * oyl + ky) * ROWF + 6 * ox];
+                for (int k = 0; k < 3; ++k) {
+                    if (IN_U8) {
+                        const uint16_t u = reinterpret_cast<const uint16_t*>(src + 6 * m)[k];
+                        v[2 * k] = s_lut[((2 * k) % 3) * 256 + (u & 0xff)];
+                        v[2 * k + 1] = s_lut[((2 * k + 1) % 3) * 256 + (u >> 8)];
+                    } else {
+                        const float2 f = reinterpret_cast<const float2*>(src + 24 * m)[k];
+                        v[2 * k] = f.x; v[2 * k + 1] = f.y;
+                    }
+                }
+            }
+            float* row = s_in + r * kStemRowF;
 #pragma unroll
-        for (int t = 0; t < 9; ++t) {                       // kx*3 + ci
-            const float x = row[t];
-            const float2 xx = make_float2(x, x);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) {
-                const float2 w2 = make_float2(sp.w[(ky * 9 + t) * 32 + 2 * c], sp.w[(ky * 9 + t) * 32 + 2 * c + 1]);
-                acc2[c].x = fmaf(xx.x, w2.x, acc2[c].x);
-                acc2[c].y = fmaf(xx.y, w2.y, acc2[c].y);
+            for (int ci = 0; ci < 3; ++ci) {
+                row[ci * kStemPlane + m] = v[ci];                                  // kx = 0: column 2m
+                row[(3 + ci) * kStemPlane + m] = v[3 + ci];                        // kx = 1: column 2m + 1
+                if (m > 0) row[(6 + ci) * kStemPlane + m - 1] = v[ci];             // kx = 2: column 2(m - 1) + 2
+                else row[(6 + ci) * kStemPlane + 111] = 0.f;                       // ... and the pad column 224
             }
         }
+        __syncthreads();
+        T* out_run = out + ((long long)n * 112 + oy0) * 112 * 32;   // the tile's 8 rows: one contiguous run of NHWC
+        stem_half<0, T, FAST>(s_in, s_w, stage0, out_run, tid, tid, sp);
+        __syncthreads();                                    // stage 0 drained: the next tile's rows may land there
+        if (tile + (int)gridDim.x < tiles) stem_fetch<IN_U8>(in_, s_raw, tile + gridDim.x, tid);
+        stem_half<1, T, FAST>(s_in, s_w, reinterpret_cast<uint4*>(base), out_run, tid, tid, sp);
     }
-    float acc[32];
-#pragma unroll
-    for (int c = 0; c < 16; ++c) { acc[2 * c] = acc2[c].x; acc[2 * c + 1] = acc2[c].y; }
-    T* dst = out + (((long long)n * 112 + oy0 + oyl) * 112 + ox) * 32;
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-        float o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = FAST ? swish_fast(acc[g * 8 + j]) : swish_f(acc[g * 8 + j]);
-        st8<T>(dst + g * 8, o);
-    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+}
+
+// `in` must be 16-byte aligned (cp.async of whole rows).  Grid: as many CTAs as fit on the device, at most one per tile.
+template <typename T, bool IN_U8, bool FAST>
+cudaError_t launch_stem_tile(cudaStream_t stream, const void* in, T* out, const StemParams& sp, const float* lut, int n) {
+    auto kfn = stem_tile_kernel<T, IN_U8, FAST>;
+    constexpr size_t smem = StemSmem<T, IN_U8>::BYTES;
+    cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int dev = 0, sms = 0, per_sm = 0;
+    if (e == cudaSuccess) e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kfn, kStemThreads, smem);
+    if (e != cudaSuccess) return e;
+    if (per_sm < 1) return cudaErrorInvalidConfiguration;
+    const long long tiles = (long long)n * kStemTilesPerCrop;
+    kfn<<<(unsigned)std::min(tiles, (long long)per_sm * sms), kStemThreads, smem, stream>>>(in, out, sp, lut, n);
+    return cudaGetLastError();
 }
 
 // ----------------------------------------------------------------------------- 1x1 conv (CUDA-core GEMM)

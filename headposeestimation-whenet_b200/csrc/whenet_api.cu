@@ -577,14 +577,14 @@ int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, floa
                  2.0 * nb * 112.0 * 112 * 27 * 32);
         if (stem_half) {
             // block 1's depthwise is KD (HFMA2 over an fp16 tile): the stem output, read by nothing else, is written as fp16
-            whenet::stem_tile_kernel<__half, IN_U8, true><<<dim3(56, nb), 224, 0, c->stream>>>(d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut);
+            CK((whenet::launch_stem_tile<__half, IN_U8, true>(c->stream, d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut, nb)));
         } else if (c->stem_variant == 0) {
             const long long total = (long long)nb * 112 * 112 * 4;
             whenet::stem_kernel<T, IN_U8><<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(d_in, cur, c->w_stem, c->b_stem, c->lut, nb);
+            CK(cudaGetLastError());
         } else {
-            whenet::stem_tile_kernel<T, IN_U8, (sizeof(T) == 2)><<<dim3(56, nb), 224, 0, c->stream>>>(d_in, cur, c->stem_params, c->lut);
+            CK((whenet::launch_stem_tile<T, IN_U8, (sizeof(T) == 2)>(c->stream, d_in, cur, c->stem_params, c->lut, nb)));
         }
-        CK(cudaGetLastError());
     }
     if (taps) {
         int rc = stem_half ? add_tap<__half>(c, "stem", reinterpret_cast<const __half*>(cur), (size_t)112 * 112 * 32, off, nb)
