@@ -20,6 +20,8 @@ EXPORTS = [
     "whenet_det_detect_yuv_u8", "whenet_det_detect_ragged_yuv_u8", "whenet_crop_boxes_yuv_u8", "whenet_crop_boxes_ragged_yuv_u8",
     "whenet_det_create_large", "whenet_det_debug_force_large_decode",
     "whenet_draw_heads_u8", "whenet_draw_heads_ragged_u8", "whenet_debug_overlay_segments",
+    "whenet_draw_heads_ex_u8", "whenet_draw_heads_ex_ragged_u8", "whenet_put_text_u8", "whenet_put_text_ragged_u8",
+    "whenet_debug_text_segments", "whenet_debug_label_text",
 ]
 
 # pixel_format -> the ABI's yuv_layout (WHENET_YUV_NV12 / WHENET_YUV_I420); "bgr" is packed 8-bit BGR, the *_u8 entries
@@ -84,6 +86,12 @@ def load():
     L.whenet_draw_heads_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P, P, C.c_int, P]
     L.whenet_draw_heads_ragged_u8.argtypes = [P, P, P, C.c_int, P, P, P, C.c_int, P]
     L.whenet_debug_overlay_segments.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P]
+    L.whenet_draw_heads_ex_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P, P, C.c_int, C.c_int, P]
+    L.whenet_draw_heads_ex_ragged_u8.argtypes = [P, P, P, C.c_int, P, P, P, C.c_int, C.c_int, P]
+    L.whenet_put_text_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, C.c_int]
+    L.whenet_put_text_ragged_u8.argtypes = [P, P, P, C.c_int, P, P, P, P, P, P, C.c_int]
+    L.whenet_debug_text_segments.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_double, C.c_int, P, C.c_int, P]
+    L.whenet_debug_label_text.argtypes = [P, C.c_int, P, C.c_int]
     L.whenet_synchronize.argtypes = [P]
     L.whenet_host_alloc.argtypes = [C.c_size_t]
     L.whenet_host_alloc.restype = P

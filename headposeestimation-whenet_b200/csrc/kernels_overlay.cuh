@@ -197,4 +197,63 @@ __global__ void __launch_bounds__(128) overlay_draw_kernel(const __grid_constant
     }
 }
 
+// ----------------------------------------------------------------------------- text (DESIGN.md section 8.8)
+// A thickness-1 LINE_8 segment of cv2.putText (oracle/text_oracle.py draw_line1): the host rounds its 16.16 end points to
+// pixels, clips them against the frame and orders them left end first; OpenCV's 8-connected LineIterator then puts pixel k
+// of the major axis ceil((2Bk - A) / 2A) pixels along the minor one (A = major length, B = minor length).
+struct OverlayThin {
+    int x1, y1, x2, y2;       // clipped pixel end points, x1 <= x2
+    int y_lo, y_hi;           // min / max of y1, y2
+    uint32_t bgr;
+    int pad;
+};
+
+constexpr int kOverlayBandRows = 32;      // one warp of rows shares one band's primitive list
+
+__host__ __device__ inline void ov_thin_row(const OverlayThin& t, uint8_t* row, int W, int y) {
+    const long long dx = t.x2 - t.x1, dy = t.y2 >= t.y1 ? t.y2 - t.y1 : t.y1 - t.y2;
+    const long long k = t.y2 >= t.y1 ? y - t.y1 : t.y1 - y;         // steps from the left end point along y
+    if (dy > dx) {                      // y-major: one pixel per row
+        if (k < 0 || k > dy) return;
+        const long long m = ov_ceil_div(2 * dx * k - dy, 2 * dy);
+        ov_put(row, W, t.x1 + (m > 0 ? m : 0), t.bgr);
+    } else {                            // x-major: the run of steps whose minor offset is k
+        if (k < 0 || k > dy) return;
+        long long lo = 0, hi = dx;
+        if (dy > 0) {
+            lo = ov_floor_div(2 * dx * k - dx, 2 * dy) + 1;
+            hi = ov_floor_div(2 * dx * k + dx, 2 * dy);
+            lo = lo < 0 ? 0 : lo;
+            hi = hi > dx ? dx : hi;
+        }
+        ov_span(row, W, t.x1 + lo, t.x1 + hi, t.bgr);
+    }
+}
+
+// grid (ceil(max H / blockDim.x), n frames); thread = one row of one frame.  fr.seg_begin[f] is frame f's first band;
+// band b's primitives, in draw order, are items[band_begin[b] .. band_begin[b + 1]): i >= 0 is segs[i] (thickness 2),
+// i < 0 is thin[~i] (thickness 1).
+__global__ void __launch_bounds__(128) overlay_draw_banded_kernel(const __grid_constant__ OverlayFrames fr, const OverlaySeg* __restrict__ segs,
+                                                                  const OverlayThin* __restrict__ thin, const int* __restrict__ band_begin,
+                                                                  const int* __restrict__ items) {
+    const int f = blockIdx.y;
+    const int y = blockIdx.x * blockDim.x + threadIdx.x;
+    const int H = fr.H[f], W = fr.W[f];
+    if (y >= H) return;
+    uint8_t* row = fr.ptr[f] + (size_t)y * W * 3;
+    const int b = fr.seg_begin[f] + y / kOverlayBandRows;
+    for (int j = __ldg(&band_begin[b]), e = __ldg(&band_begin[b + 1]); j < e; ++j) {
+        const int i = __ldg(&items[j]);
+        if (i >= 0) {
+            if (y < __ldg(&segs[i].y_lo) || y > __ldg(&segs[i].y_hi)) continue;
+            const OverlaySeg s = segs[i];
+            overlay_seg_row(s, row, H, W, y);
+        } else {
+            const OverlayThin t = thin[~i];
+            if (y < t.y_lo || y > t.y_hi) continue;
+            ov_thin_row(t, row, W, y);
+        }
+    }
+}
+
 }  // namespace whenet

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
+#include <charconv>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -208,6 +210,10 @@ struct whenet_ctx {
     int4* d_rects = nullptr; int* d_frame_of = nullptr; int rects_cap = 0;
     // head overlay segment table
     whenet::OverlaySeg* d_segs = nullptr; int segs_cap = 0;
+    // text and display="full" overlay: thickness-1 segments, band table and banded item list
+    whenet::OverlayThin* d_thin = nullptr; int thin_cap = 0;
+    int* d_bands = nullptr; int bands_cap = 0;
+    int* d_items = nullptr; int items_cap = 0;
     // taps (whenet_debug_enable_taps): 0 off, 1 first chunk of <= 8 crops on the one-stream route, 2 every chunk on the
     // untapped route.  Keyed by the canonical name ("dw%d" also holds a gated "dwg%d"); `valid`: written by the last forward.
     struct Tap { float* p = nullptr; size_t cap = 0, n = 0; bool valid = false; int forms = 0; };   // forms: 1 ungated, 2 gated rows
@@ -1821,6 +1827,253 @@ int draw_heads_checked(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw,
     return draw_heads(c, frames, hw, n, boxes, angles, frame_of, m, drawn_out);
 }
 
+// ----------------------------------------------------------------------------- text (DESIGN.md section 8.8)
+// cv2.putText(img, text, org, FONT_HERSHEY_SIMPLEX, scale, color, 1) as thickness-1 segments (oracle/text_oracle.py), and the
+// labels of reference demo_video.py:31-34 (display="full").
+#include "hershey_simplex.inc"
+
+constexpr int kTextMaxLen = 4096;
+constexpr int kTextMaxItems = 1 << 20;
+constexpr long long kTextMaxChars = 1 << 22;             // characters per put_text call (at most 40 segments each)
+constexpr int kLabelMaxHeads = 1 << 16;                  // heads per display="full" call
+constexpr size_t kOverlayMaxItems = 0x7fffffff;          // primitives and banded entries are indexed with int
+constexpr int kTextMaxOrg = 1 << 24;
+constexpr double kTextMaxScale = 256.0;
+constexpr float kLabelScale = 0.4f;
+constexpr uint32_t kLabelColor = 100u | 255u << 8;          // (100, 255, 0) BGR
+
+// "{}".format(np.round(np.float32(a))) under numpy 2: round half to even in float32; an empty format spec then formats the
+// value as a Python float, i.e. the shortest round-trip digits of the double, positional with a trailing ".0" below 1e16
+// and scientific ("1e+16", "3.4028234663852886e+38") from there.
+std::string label_number(float a) {
+    const float v = std::nearbyint(a);
+    if (std::isnan(v)) return "nan";
+    if (std::isinf(v)) return v < 0 ? "-inf" : "inf";
+    char buf[64];
+    const auto r = std::to_chars(buf, buf + sizeof(buf), (double)v, std::chars_format::scientific);
+    const std::string s(buf, r.ptr);                        // [-]d[.ddd]e(+|-)xx, shortest digits
+    const size_t e = s.find('e');
+    const bool neg = s[0] == '-';
+    std::string digits;
+    for (size_t i = neg; i < e; ++i)
+        if (s[i] != '.') digits += s[i];
+    const int exp10 = std::atoi(s.c_str() + e + 1);
+    std::string out = neg ? "-" : "";
+    if (v == 0.f || std::fabs((double)v) < 1e16) {          // v is an integer, so exp10 >= digits.size() - 1
+        out += digits + std::string(exp10 + 1 - (int)digits.size(), '0') + ".0";
+    } else {
+        out += digits.substr(0, 1);
+        if (digits.size() > 1) out += "." + digits.substr(1);
+        char ex[16];
+        snprintf(ex, sizeof(ex), "e+%02d", exp10);
+        out += ex;
+    }
+    return out;
+}
+
+// The 16.16 segments putText draws for `text` at `org`, in draw order (x1, y1, x2, y2)
+void text_segments16(const char* text, int ox, int oy, double scale, std::vector<long long>& out) {
+    const long long hscale = std::llrint(scale * 65536.0), vscale = hscale;     // cvRound
+    long long pen_x = (long long)ox * 65536, pen_y = (long long)oy * 65536 + kHersheyBaseLine * vscale;
+    for (const char* p = text; *p; ++p) {
+        const char* g = kHersheySimplex[*p - 32];
+        const long long advance = (g[1] - 'R') * hscale;
+        pen_x -= (g[0] - 'R') * hscale;
+        long long px = 0, py = 0;
+        int npts = 0;
+        for (const char* q = g + 2;; ) {
+            if (*q == ' ' || !*q) {
+                if (!*q) break;
+                ++q;
+                npts = 0;
+            } else {
+                const long long x = (q[0] - 'R') * hscale + pen_x, y = (q[1] - 'R') * vscale + pen_y;
+                if (npts++ > 0) out.insert(out.end(), {px, py, x, y});
+                px = x; py = y;
+                q += 2;
+            }
+        }
+        pen_x += advance;
+    }
+}
+
+// One 16.16 segment -> its thickness-1 record on an H x W frame; false when it misses the frame
+bool thin_seg(const long long* s, uint32_t bgr, int H, int W, whenet::OverlayThin* t) {
+    long long x1 = (s[0] + 32768) >> 16, y1 = (s[1] + 32768) >> 16, x2 = (s[2] + 32768) >> 16, y2 = (s[3] + 32768) >> 16;
+    if (!whenet::ov_clip(W, H, x1, y1, x2, y2)) return false;
+    if (x2 < x1) { std::swap(x1, x2); std::swap(y1, y2); }
+    *t = whenet::OverlayThin{(int)x1, (int)y1, (int)x2, (int)y2, (int)std::min(y1, y2), (int)std::max(y1, y2), bgr, 0};
+    return true;
+}
+
+// The primitives of every frame in draw order, banded by kOverlayBandRows rows, and the launch
+struct OverlayList {
+    std::vector<whenet::OverlaySeg> segs;
+    std::vector<whenet::OverlayThin> thin;
+    std::vector<std::vector<std::array<int, 3>>> per;      // frame -> (item, y_lo, y_hi)
+    std::vector<long long> s16;                             // one text's 16.16 segments, reused
+    bool overflow = false;                                  // more primitives than an int indexes
+    explicit OverlayList(int n) : per(n) {}
+    void add_text(int f, const char* text, int ox, int oy, double scale, uint32_t bgr, int H, int W) {
+        s16.clear();
+        text_segments16(text, ox, oy, scale, s16);
+        for (size_t k = 0; k < s16.size(); k += 4) {
+            whenet::OverlayThin t;
+            if (!thin_seg(&s16[k], bgr, H, W, &t)) continue;
+            if (thin.size() >= kOverlayMaxItems) { overflow = true; return; }
+            per[f].push_back({~(int)thin.size(), t.y_lo, t.y_hi});
+            thin.push_back(t);
+        }
+    }
+};
+
+template <typename T>
+int upload(whenet_ctx* c, T** buf, int* cap, const std::vector<T>& v) {
+    if (v.empty()) return 0;
+    if (*cap < (int)v.size()) {
+        if (*buf) cudaFree(*buf);
+        *buf = nullptr; *cap = 0;
+        CK(cudaMalloc(buf, v.size() * sizeof(T)));
+        *cap = (int)v.size();
+    }
+    CK(cudaMemcpyAsync(*buf, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, c->stream));
+    return 0;
+}
+
+int draw_overlay_list(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const OverlayList& L) {
+    whenet::OverlayFrames fr{};
+    std::vector<int> band_begin(1, 0), items;
+    int maxH = 0;
+    size_t total = 0;                                       // banded entries, counted before anything is indexed with int
+    for (int f = 0; f < n; ++f)
+        for (const auto& p : L.per[f]) total += (size_t)(p[2] / whenet::kOverlayBandRows - p[1] / whenet::kOverlayBandRows + 1);
+    if (L.overflow || L.segs.size() >= kOverlayMaxItems || total >= kOverlayMaxItems)
+        return fail(WHENET_EINVAL, "too many segments in one call (%zu banded entries, limit %zu)", total, kOverlayMaxItems);
+    for (int f = 0; f < n; ++f) {
+        const int H = hw[2 * f], nb = (H + whenet::kOverlayBandRows - 1) / whenet::kOverlayBandRows;
+        fr.ptr[f] = frames[f]; fr.H[f] = H; fr.W[f] = hw[2 * f + 1];
+        fr.seg_begin[f] = (int)band_begin.size() - 1;
+        maxH = std::max(maxH, H);
+        std::vector<int> cnt(nb + 1, 0);                      // counting sort by band, stable in draw order
+        for (const auto& p : L.per[f])
+            for (int b = p[1] / whenet::kOverlayBandRows; b <= p[2] / whenet::kOverlayBandRows; ++b) ++cnt[b + 1];
+        for (int b = 0; b < nb; ++b) cnt[b + 1] += cnt[b];
+        const int base = (int)items.size();
+        items.resize(base + cnt[nb]);
+        std::vector<int> pos(cnt.begin(), cnt.end() - 1);
+        for (const auto& p : L.per[f])
+            for (int b = p[1] / whenet::kOverlayBandRows; b <= p[2] / whenet::kOverlayBandRows; ++b) items[base + pos[b]++] = p[0];
+        for (int b = 0; b < nb; ++b) band_begin.push_back(base + cnt[b + 1]);
+    }
+    fr.seg_begin[n] = (int)band_begin.size() - 1;
+    if (items.empty()) return 0;
+    CK(cudaSetDevice(c->device));
+    if (int rc = upload(c, &c->d_segs, &c->segs_cap, L.segs)) return rc;
+    if (int rc = upload(c, &c->d_thin, &c->thin_cap, L.thin)) return rc;
+    if (int rc = upload(c, &c->d_bands, &c->bands_cap, band_begin)) return rc;
+    if (int rc = upload(c, &c->d_items, &c->items_cap, items)) return rc;
+    Scope sc(c, "draw_overlay", 0.0, 0.0);
+    whenet::overlay_draw_banded_kernel<<<dim3((maxH + 127) / 128, n), 128, 0, c->stream>>>(fr, c->d_segs, c->d_thin, c->d_bands, c->d_items);
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// display="full": each drawn head's 7 segments, then its yaw, pitch and roll labels at (int(x_min), int(y_min) - 0 / 15 / 30)
+int draw_heads_full(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes, const float* angles,
+                    const int32_t* frame_of, int m, int32_t* drawn_out) {
+    OverlayList L(n);
+    int32_t seg[kSegsPerHead][4];
+    static const char* const kLabel[3] = {"yaw: ", "pitch: ", "roll: "};
+    for (int i = 0; i < m; ++i) {
+        const int f = frame_of[i], H = hw[2 * f], W = hw[2 * f + 1];
+        const bool ok = head_segments(boxes + 4 * i, angles + 3 * i, H, W, seg);
+        if (drawn_out) drawn_out[i] = ok;
+        if (!ok) continue;
+        for (int k = 0; k < kSegsPerHead; ++k) {
+            whenet::OverlaySeg s;
+            if (!overlay_seg(seg[k], kSegColor[k], H, W, &s)) continue;
+            L.per[f].push_back({(int)L.segs.size(), s.y_lo, s.y_hi});
+            L.segs.push_back(s);
+        }
+        const int ox = seg[0][0], oy = seg[0][1];             // the rectangle's (int(x_min), int(y_min))
+        for (int k = 0; k < 3; ++k)
+            L.add_text(f, (kLabel[k] + label_number(angles[3 * i + k])).c_str(), ox, oy - 15 * k, kLabelScale, kLabelColor, H, W);
+    }
+    return draw_overlay_list(c, frames, hw, n, L);
+}
+
+int check_frames(uint8_t* const* frames, const int32_t* hw, int n) {
+    if (n < 1 || n > whenet::kMaxCropFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxCropFrames);
+    for (int i = 0; i < n; ++i) {
+        if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
+        if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
+            return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+    }
+    return 0;
+}
+
+int check_text(const char* text, int ox, int oy, double scale, int thickness) {
+    if (!text) return fail(WHENET_EINVAL, "null text");
+    if (thickness != 1) return fail(WHENET_EINVAL, "thickness %d: only 1 is supported", thickness);
+    if (!(scale > 0.0 && scale <= kTextMaxScale)) return fail(WHENET_EINVAL, "scale %g outside (0, %g]", scale, kTextMaxScale);
+    if (ox < -kTextMaxOrg || ox > kTextMaxOrg || oy < -kTextMaxOrg || oy > kTextMaxOrg)
+        return fail(WHENET_EINVAL, "origin (%d, %d) outside +-%d", ox, oy, kTextMaxOrg);
+    int len = 0;
+    for (const char* p = text; *p; ++p, ++len) {
+        if (*p < 32 || *p > 126) return fail(WHENET_EINVAL, "character %d at %d is not printable ASCII", (int)(unsigned char)*p, len);
+        if (len >= kTextMaxLen) return fail(WHENET_EINVAL, "text longer than %d characters", kTextMaxLen);
+    }
+    return 0;
+}
+
+int put_text_checked(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const int32_t* frame_of, const char* const* texts,
+                     const int32_t* org, const double* scale, const uint8_t* bgr, const int32_t* thickness, int m) {
+    if (int rc = check_frames(frames, hw, n)) return rc;
+    if (m < 0 || m > kTextMaxItems) return fail(WHENET_EINVAL, "m=%d text items outside [0, %d]", m, kTextMaxItems);
+    if (m == 0) return 0;
+    if (!frame_of || !texts || !org || !scale || !bgr || !thickness) return fail(WHENET_EINVAL, "null item array");
+    long long chars = 0;
+    for (int i = 0; i < m; ++i) {
+        if (frame_of[i] < 0 || frame_of[i] >= n) return fail(WHENET_EINVAL, "item %d: frame_of=%d outside [0, %d)", i, frame_of[i], n);
+        if (int rc = check_text(texts[i], org[2 * i], org[2 * i + 1], scale[i], thickness[i])) return rc;
+        chars += (long long)strlen(texts[i]);
+    }
+    if (chars > kTextMaxChars) return fail(WHENET_EINVAL, "%lld characters in one call, limit %lld", chars, kTextMaxChars);
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    OverlayList L(n);
+    for (int i = 0; i < m; ++i) {
+        const int f = frame_of[i];
+        const uint32_t col = bgr[3 * i] | (uint32_t)bgr[3 * i + 1] << 8 | (uint32_t)bgr[3 * i + 2] << 16;
+        L.add_text(f, texts[i], org[2 * i], org[2 * i + 1], scale[i], col, hw[2 * f], hw[2 * f + 1]);
+    }
+    return draw_overlay_list(c, frames, hw, n, L);
+}
+
+int draw_heads_ex_checked(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes, const float* angles,
+                          const int32_t* frame_of, int m, int display, int32_t* drawn_out) {
+    if (display != 0 && display != 1) return fail(WHENET_EINVAL, "display=%d: 0 (simple) or 1 (full)", display);
+    if (display == 0) return draw_heads_checked(c, frames, hw, n, boxes, angles, frame_of, m, drawn_out);
+    if (int rc = check_frames(frames, hw, n)) return rc;
+    if (m < 0 || m > kLabelMaxHeads) return fail(WHENET_EINVAL, "m=%d heads outside [0, %d] with display=1", m, kLabelMaxHeads);
+    if (m == 0) return 0;
+    if (!boxes || !angles || !frame_of) return fail(WHENET_EINVAL, "null boxes, angles or frame_of");
+    for (int i = 0; i < m; ++i)
+        if (frame_of[i] < 0 || frame_of[i] >= n) return fail(WHENET_EINVAL, "head %d: frame_of=%d outside [0, %d)", i, frame_of[i], n);
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    return draw_heads_full(c, frames, hw, n, boxes, angles, frame_of, m, drawn_out);
+}
+
+int dense_frames(uint8_t* frames, int n, int H, int W, uint8_t** ptrs, int32_t* hw) {
+    if (!frames) return fail(WHENET_EINVAL, "null frames");
+    if (n < 1 || n > whenet::kMaxCropFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxCropFrames);
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    for (int i = 0; i < n; ++i) {
+        ptrs[i] = frames + (size_t)i * H * W * 3;
+        hw[2 * i] = H; hw[2 * i + 1] = W;
+    }
+    return 0;
+}
+
 static_assert(whenet::kOverlayMaxFrames == whenet::kMaxCropFrames, "overlay frame table holds every crop frame");
 
 }  // namespace
@@ -1879,6 +2132,55 @@ int whenet_debug_overlay_segments(const float* boxes, const float* angles, int m
         if (!ok) memset(seg, 0, sizeof(seg));
         if (seg_out) memcpy(seg_out + (size_t)i * kSegsPerHead * 4, seg, sizeof(seg));
         if (drawn_out) drawn_out[i] = ok;
+    }
+    return 0;
+}
+
+int whenet_draw_heads_ex_u8(whenet_ctx* c, uint8_t* frames, int n, int H, int W, const float* boxes, const float* angles,
+                            const int32_t* frame_of, int m, int display, int32_t* drawn_out) {
+    uint8_t* ptrs[whenet::kMaxCropFrames];
+    int32_t hw[2 * whenet::kMaxCropFrames];
+    if (int rc = dense_frames(frames, n, H, W, ptrs, hw)) return rc;
+    return draw_heads_ex_checked(c, ptrs, hw, n, boxes, angles, frame_of, m, display, drawn_out);
+}
+
+int whenet_draw_heads_ex_ragged_u8(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes,
+                                   const float* angles, const int32_t* frame_of, int m, int display, int32_t* drawn_out) {
+    if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
+    return draw_heads_ex_checked(c, frames, hw, n, boxes, angles, frame_of, m, display, drawn_out);
+}
+
+int whenet_put_text_u8(whenet_ctx* c, uint8_t* frames, int n, int H, int W, const int32_t* frame_of, const char* const* texts,
+                       const int32_t* org, const double* scale, const uint8_t* bgr, const int32_t* thickness, int m) {
+    uint8_t* ptrs[whenet::kMaxCropFrames];
+    int32_t hw[2 * whenet::kMaxCropFrames];
+    if (int rc = dense_frames(frames, n, H, W, ptrs, hw)) return rc;
+    return put_text_checked(c, ptrs, hw, n, frame_of, texts, org, scale, bgr, thickness, m);
+}
+
+int whenet_put_text_ragged_u8(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, const int32_t* frame_of,
+                              const char* const* texts, const int32_t* org, const double* scale, const uint8_t* bgr,
+                              const int32_t* thickness, int m) {
+    if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
+    return put_text_checked(c, frames, hw, n, frame_of, texts, org, scale, bgr, thickness, m);
+}
+
+int whenet_debug_text_segments(const char* text, int org_x, int org_y, double scale, int thickness, int64_t* seg_out, int cap,
+                               int32_t* count_out) {
+    if (int rc = check_text(text, org_x, org_y, scale, thickness)) return rc;
+    std::vector<long long> s;
+    text_segments16(text, org_x, org_y, scale, s);
+    const int count = (int)(s.size() / 4);
+    if (count_out) *count_out = count;
+    if (seg_out) memcpy(seg_out, s.data(), (size_t)std::min(count, std::max(cap, 0)) * 4 * sizeof(int64_t));
+    return 0;
+}
+
+int whenet_debug_label_text(const float* angles, int m, char* out, int stride) {
+    if (!angles || !out || m < 1 || stride < 32) return fail(WHENET_EINVAL, "null angles or out, m=%d, stride=%d < 32", m, stride);
+    for (int i = 0; i < m; ++i) {
+        const std::string t = label_number(angles[i]);
+        snprintf(out + (size_t)i * stride, stride, "%s", t.c_str());
     }
     return 0;
 }
@@ -2168,6 +2470,9 @@ void whenet_destroy(whenet_ctx* c) {
     if (c->d_rects) cudaFree(c->d_rects);
     if (c->d_frame_of) cudaFree(c->d_frame_of);
     if (c->d_segs) cudaFree(c->d_segs);
+    if (c->d_thin) cudaFree(c->d_thin);
+    if (c->d_bands) cudaFree(c->d_bands);
+    if (c->d_items) cudaFree(c->d_items);
     for (auto& kv : c->taps) cudaFree(kv.second.p);
     if (c->d_tap_map) cudaFree(c->d_tap_map);
     for (auto& p : c->ev_used) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }

@@ -17,7 +17,9 @@ deviation (the drawn overlay is not image content), documented in DESIGN.md.
 
 ``draw_heads`` draws on the clean frames what ``oracle/overlay_oracle.process_detection_ref`` draws for each head, pixel for
 pixel, with the reference's float32 scalar types (``draw_axis`` below turns the angles into Python floats first, which moves an
-axis end point for about 1 head in 100,000; DESIGN.md section 8.7).  Text (``display="full"``) stays on the host.
+axis end point for about 1 head in 100,000; DESIGN.md section 8.7).  ``display="full"`` adds the yaw, pitch and roll labels
+of demo_video.py:31-34, and ``put_text`` draws any cv2.putText(FONT_HERSHEY_SIMPLEX, thickness 1) text, both on the GPU
+(DESIGN.md section 8.8).
 """
 from __future__ import annotations
 
@@ -94,10 +96,35 @@ def process_frame(model, frame, boxes, display: str = "simple", reference_order:
     return frame, yaw, pitch, roll
 
 
-def draw_heads(whenet, frames, results):
+DISPLAYS = {"simple": 0, "full": 1}
+# put_text's limits, as the library checks them (include/whenet_b200.h)
+TEXT_MAX_LEN, TEXT_MAX_CHARS, TEXT_MAX_ITEMS, TEXT_MAX_ORG, TEXT_MAX_SCALE = 4096, 1 << 22, 1 << 20, 1 << 24, 256.0
+
+
+def _device_frames(whenet, frames, who):
+    """(frame list?, items, n) of device BGR frames, or ValueError."""
+    from .whenet import _is_device
+    frame_list = isinstance(frames, (list, tuple))
+    items = list(frames) if frame_list else [frames]
+    for f in items:
+        if not _is_device(f):
+            raise ValueError("%s draws on CUDA tensors; use process_frame for host frames" % who)
+        if str(f.dtype) != "torch.uint8" or not f.is_contiguous():
+            raise ValueError("frames must be contiguous uint8 CUDA tensors")
+        if f.device.index != whenet.device:
+            raise ValueError("frames are on cuda:%s, WHENet on cuda:%d" % (f.device.index, whenet.device))
+        if len(f.shape) != (3 if frame_list else 4) or f.shape[-1] != 3:
+            raise ValueError("frames must be BGR (n, H, W, 3) or a list of (H, W, 3), not %s" % (tuple(f.shape),))
+    return frame_list, items, (len(items) if frame_list else int(frames.shape[0]))
+
+
+def draw_heads(whenet, frames, results, display: str = "simple"):
     """Draw every head of ``results`` into ``frames`` on the GPU, in place: a black thickness-2 rectangle around the
     margin-enlarged box, then the red, green and blue pose axes, bit-identical to the reference's cv2 calls
-    (demo_video.py:26,29 with display="simple").  Heads are drawn in result order.
+    (demo_video.py:26,29 with display="simple").  Heads are drawn in result order.  ``display="full"`` also draws, after each
+    head's axes, its three labels (demo_video.py:31-34): "yaw: ", "pitch: " and "roll: " with the float32 angle rounded as
+    ``np.round`` prints it, FONT_HERSHEY_SIMPLEX at scale 0.4 in (100, 255, 0), at (int(x_min), int(y_min)) and 15 and 30
+    rows higher, bit-identical to cv2.putText.  Any other ``display`` raises ``ValueError``.
 
     ``frames``: a contiguous (n, H, W, 3) uint8 BGR CUDA tensor on ``whenet.device``, or a list or tuple of contiguous
     (H_i, W_i, 3) ones; ``results``: what ``pipeline.detect_and_estimate_frames`` returned for those frames.  A head is
@@ -107,19 +134,11 @@ def draw_heads(whenet, frames, results):
     import ctypes as C
     import torch
     from ._lib import check
-    from .whenet import _is_device, _ptr
-    frame_list = isinstance(frames, (list, tuple))
-    items = list(frames) if frame_list else [frames]
-    for f in items:
-        if not _is_device(f):
-            raise ValueError("draw_heads draws on CUDA tensors; use process_frame for host frames")
-        if str(f.dtype) != "torch.uint8" or not f.is_contiguous():
-            raise ValueError("frames must be contiguous uint8 CUDA tensors")
-        if f.device.index != whenet.device:
-            raise ValueError("frames are on cuda:%s, WHENet on cuda:%d" % (f.device.index, whenet.device))
-        if len(f.shape) != (3 if frame_list else 4) or f.shape[-1] != 3:
-            raise ValueError("frames must be BGR (n, H, W, 3) or a list of (H, W, 3), not %s" % (tuple(f.shape),))
-    n = len(items) if frame_list else int(frames.shape[0])
+    from .whenet import _ptr
+    if display not in DISPLAYS:
+        raise ValueError("display must be one of %s, not %r" % (sorted(DISPLAYS), display))
+    full = DISPLAYS[display]
+    frame_list, items, n = _device_frames(whenet, frames, "draw_heads")
     if len(results) != n:
         raise ValueError("%d results for %d frames" % (len(results), n))
     if n == 0:
@@ -144,15 +163,105 @@ def draw_heads(whenet, frames, results):
             if frame_list:
                 ptrs = (C.c_void_p * (hi - lo))(*[f.data_ptr() for f in items[lo:hi]])
                 hw = np.array([f.shape[:2] for f in items[lo:hi]], np.int32)
-                check(L.whenet_draw_heads_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, _ptr(boxes[a:]), _ptr(angles[a:]),
-                                                    _ptr(fo), b - a, _ptr(drawn[a:])))
+                if full:
+                    check(L.whenet_draw_heads_ex_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, _ptr(boxes[a:]),
+                                                           _ptr(angles[a:]), _ptr(fo), b - a, full, _ptr(drawn[a:])))
+                else:
+                    check(L.whenet_draw_heads_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, _ptr(boxes[a:]), _ptr(angles[a:]),
+                                                        _ptr(fo), b - a, _ptr(drawn[a:])))
             else:
                 _, H, W, _c = frames.shape
-                check(L.whenet_draw_heads_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, _ptr(boxes[a:]), _ptr(angles[a:]),
-                                             _ptr(fo), b - a, _ptr(drawn[a:])))
+                if full:
+                    check(L.whenet_draw_heads_ex_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, _ptr(boxes[a:]), _ptr(angles[a:]),
+                                                    _ptr(fo), b - a, full, _ptr(drawn[a:])))
+                else:
+                    check(L.whenet_draw_heads_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, _ptr(boxes[a:]), _ptr(angles[a:]),
+                                                 _ptr(fo), b - a, _ptr(drawn[a:])))
         whenet.synchronize()
     out, off = [], 0
     for k in counts:
         out.append(drawn[off:off + k].astype(bool))
         off += k
     return out
+
+
+def put_text(whenet, frames, items):
+    """Draw text into device BGR ``frames`` on the GPU, in place, bit-identical to
+    ``cv2.putText(frame, text, org, cv2.FONT_HERSHEY_SIMPLEX, scale, color, thickness)`` (LINE_8).
+
+    ``frames``: as ``draw_heads``.  ``items``: a sequence of ``(frame_index, text, (x, y), scale, (b, g, r))`` or
+    ``(frame_index, text, (x, y), scale, (b, g, r), thickness)`` tuples, drawn in order.  ``text`` is printable ASCII of at
+    most 4096 characters (2^22 in all per 64 frames); |x|, |y| <= 2^24; 0 < scale <= 256; colour channels are integers in
+    [0, 255]; only thickness 1 is supported.  Every item and frame is checked here, before anything is drawn, and a bad one
+    raises ``ValueError``.  The library can still refuse a group of 64 frames after earlier groups were drawn in one case
+    only: text so large that its row-banded segment list would exceed 2^31 entries.  Synchronises once."""
+    import ctypes as C
+    import torch
+    from ._lib import WhenetError, check
+    from .whenet import _ptr
+    import math
+    frame_list, fitems, n = _device_frames(whenet, frames, "put_text")
+    if n == 0 or len(items) == 0:
+        return
+    for k, f in enumerate(fitems if frame_list else [frames[0]]):
+        H, W = int(f.shape[-3]), int(f.shape[-2])
+        if not (1 <= H <= 16384 and 1 <= W <= 16384):
+            raise ValueError("frame %d: size %dx%d outside [1, 16384]" % (k, W, H))
+    rows = []
+    for it in items:
+        it = tuple(it)
+        if len(it) not in (5, 6):
+            raise ValueError("an item is (frame_index, text, (x, y), scale, (b, g, r)[, thickness]), not %r" % (it,))
+        f, text, (x, y), scale, col = it[:5]
+        thick = it[5] if len(it) == 6 else 1
+        if int(f) != f or not 0 <= f < n:
+            raise ValueError("frame index %r outside [0, %d)" % (f, n))
+        if not isinstance(text, str) or len(text) > TEXT_MAX_LEN or not all(32 <= ord(ch) <= 126 for ch in text):
+            raise ValueError("text must be printable ASCII of at most %d characters: %r" % (TEXT_MAX_LEN, text))
+        if int(x) != x or int(y) != y or abs(x) > TEXT_MAX_ORG or abs(y) > TEXT_MAX_ORG:
+            raise ValueError("origin %r must be integers within +-2^24" % ((x, y),))
+        if not (math.isfinite(float(scale)) and 0 < float(scale) <= TEXT_MAX_SCALE):
+            raise ValueError("scale %r outside (0, %g]" % (scale, TEXT_MAX_SCALE))
+        col = tuple(col)
+        if len(col) != 3 or any(int(v) != v or not 0 <= v <= 255 for v in col):
+            raise ValueError("colour %r must be three integers in [0, 255]" % (col,))
+        if thick != 1:
+            raise ValueError("thickness %r: only 1 is supported" % (thick,))
+        rows.append((int(f), text.encode("ascii"), int(x), int(y), float(scale), [int(v) for v in col]))
+    fo = np.array([r[0] for r in rows], np.int32)
+    for lo in range(0, n, 64):          # the library's per-call limits, one call per 64 frames
+        chunk = [len(r[1]) for r in rows if lo <= r[0] < lo + 64]
+        if len(chunk) > TEXT_MAX_ITEMS or sum(chunk) > TEXT_MAX_CHARS:
+            raise ValueError("more than 2^20 items or 2^22 characters for frames %d..%d" % (lo, min(n, lo + 64) - 1))
+    texts = [r[1] for r in rows]
+    org = np.array([[r[2], r[3]] for r in rows], np.int32).reshape(-1, 2)
+    scale = np.array([r[4] for r in rows], np.float64)
+    bgr = np.array([r[5] for r in rows], np.uint8).reshape(-1, 3)
+    thick = np.ones(len(rows), np.int32)
+    L = whenet._L
+    with torch.cuda.device(whenet.device):
+        torch.cuda.current_stream().synchronize()
+        for lo in range(0, n, 64):
+            hi = min(n, lo + 64)
+            sel = np.nonzero((fo >= lo) & (fo < hi))[0]
+            if len(sel) == 0:
+                continue
+            tp = (C.c_char_p * len(sel))(*[texts[i] for i in sel])
+            f_sel = np.ascontiguousarray(fo[sel] - lo)
+            o_sel, s_sel = np.ascontiguousarray(org[sel]), np.ascontiguousarray(scale[sel])
+            c_sel, t_sel = np.ascontiguousarray(bgr[sel]), np.ascontiguousarray(thick[sel])
+            try:
+                if frame_list:
+                    ptrs = (C.c_void_p * (hi - lo))(*[f.data_ptr() for f in fitems[lo:hi]])
+                    hw = np.array([f.shape[:2] for f in fitems[lo:hi]], np.int32)
+                    check(L.whenet_put_text_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, _ptr(f_sel), C.addressof(tp),
+                                                      _ptr(o_sel), _ptr(s_sel), _ptr(c_sel), _ptr(t_sel), len(sel)))
+                else:
+                    _, H, W, _c = frames.shape
+                    check(L.whenet_put_text_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, _ptr(f_sel), C.addressof(tp),
+                                               _ptr(o_sel), _ptr(s_sel), _ptr(c_sel), _ptr(t_sel), len(sel)))
+            except WhenetError as e:
+                if e.code == -1:
+                    raise ValueError(str(e)) from e
+                raise
+        whenet.synchronize()

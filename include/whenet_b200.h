@@ -230,6 +230,34 @@ int whenet_draw_heads_ragged_u8(whenet_ctx* ctx, uint8_t* const* frames, const i
 /* The overlay's host geometry without a GPU: per head 7 segments (x0, y0, x1, y1) int32 in draw order - the rectangle's
    top, right, bottom and left edges, then the red, green and blue axes - zeros for a head not drawn (drawn_out[i] = 0). */
 int whenet_debug_overlay_segments(const float* boxes, const float* angles, int m, int H, int W, int32_t* seg_out, int32_t* drawn_out);
+/* Head overlay with a display mode (DESIGN.md section 8.8): display 0 draws exactly what whenet_draw_heads_u8 draws
+   (display="simple"); display 1 ("full") adds, after each drawn head's rectangle and axes, the three labels of reference
+   demo_video.py:31-34: cv2.putText(img, "yaw: {}".format(np.round(yaw)), (int(x_min), int(y_min)), FONT_HERSHEY_SIMPLEX,
+   0.4, (100, 255, 0), 1), then "pitch: " 15 rows and "roll: " 30 rows higher, the numbers formatted from the float32 angles
+   as the reference formats them ("-12.0", "-0.0").  Any other display is WHENET_EINVAL; with display 1, m is at most 65536;
+   every other argument as whenet_draw_heads_u8. */
+int whenet_draw_heads_ex_u8(whenet_ctx* ctx, uint8_t* frames, int n, int H, int W, const float* boxes, const float* angles,
+                            const int32_t* frame_of, int m, int display, int32_t* drawn_out);
+int whenet_draw_heads_ex_ragged_u8(whenet_ctx* ctx, uint8_t* const* frames, const int32_t* hw, int n, const float* boxes,
+                                   const float* angles, const int32_t* frame_of, int m, int display, int32_t* drawn_out);
+/* Text on device BGR frames in place, pixel-identical to cv2.putText(img, texts[i], (org[2i], org[2i+1]),
+   FONT_HERSHEY_SIMPLEX, scale[i], (bgr[3i], bgr[3i+1], bgr[3i+2]), thickness[i]) with LINE_8 and bottomLeftOrigin=false, for
+   m items drawn in order into frame frame_of[i].  texts: NUL-terminated printable ASCII (32..126), at most 4096
+   characters each and 2^22 in all; m at most 2^20; thickness must be 1; scale in (0, 256]; origin coordinates within
+   +-2^24.  Anything else, or more segments than an int indexes, is WHENET_EINVAL.
+   m = 0 is a no-op; n and frame sizes as whenet_draw_heads_u8.  All arrays are on the host. */
+int whenet_put_text_u8(whenet_ctx* ctx, uint8_t* frames, int n, int H, int W, const int32_t* frame_of, const char* const* texts,
+                       const int32_t* org, const double* scale, const uint8_t* bgr, const int32_t* thickness, int m);
+int whenet_put_text_ragged_u8(whenet_ctx* ctx, uint8_t* const* frames, const int32_t* hw, int n, const int32_t* frame_of,
+                              const char* const* texts, const int32_t* org, const double* scale, const uint8_t* bgr,
+                              const int32_t* thickness, int m);
+/* The text geometry without a GPU: the 16.16 segments (x1, y1, x2, y2) int64 putText strokes for one item, in draw order.
+   *count_out = their number; at most cap are written to seg_out (either may be NULL).  Arguments checked as above. */
+int whenet_debug_text_segments(const char* text, int org_x, int org_y, double scale, int thickness, int64_t* seg_out, int cap,
+                               int32_t* count_out);
+/* The number of each display="full" label: str(np.round(np.float32(a))) for m float32 angles, NUL-terminated, one per
+   `stride` (>= 32) bytes of out. */
+int whenet_debug_label_text(const float* angles, int m, char* out, int stride);
 
 
 /* Time every kernel of the NEXT forwards with CUDA events. */

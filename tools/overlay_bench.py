@@ -1,6 +1,8 @@
 """Head overlay on device frames: overlay.draw_heads against download + reference-typed cv2 drawing + upload, on 8
-synthetic 1080p frames with about 20 heads each, the two arms alternating and checked bit-equal; then the chain
-detect_and_estimate_frames + draw_heads against detect_and_estimate_frames alone.  Prints the card it ran on."""
+synthetic 1080p frames with about 20 heads each, the two arms alternating and checked bit-equal; the same with
+display="full" (labels, DESIGN.md section 8.8): draw_heads(display="full"), display="simple" and the host round trip with
+the labels, alternating, full checked bit-equal to the host; then the chain detect_and_estimate_frames + draw_heads against
+detect_and_estimate_frames alone.  Prints the card it ran on."""
 import os
 import subprocess
 import sys
@@ -28,6 +30,12 @@ def main(reps=20):
         x_max = min(W, x_max + abs(x_min - x_max) / 5)
         cv2.rectangle(img, (int(x_min), int(y_min)), (int(x_max), int(y_max)), (0, 0, 0), 2)
         O.draw_axis_ref(img, ang[0], ang[1], ang[2], tdx=(x_min + x_max) / 2, tdy=(y_min + y_max) / 2, size=abs(x_max - x_min) // 2)
+        return int(x_min), int(y_min)
+
+    def ref_draw_full(img, box, ang):
+        x, y = ref_draw(img, box, ang)
+        for k, name in enumerate(("yaw", "pitch", "roll")):
+            cv2.putText(img, "%s: {}".format(np.round(ang[k])) % name, (x, y - 15 * k), cv2.FONT_HERSHEY_SIMPLEX, 0.4, (100, 255, 0), 1)
     print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip())
     n, H, W = 8, 1080, 1920
@@ -60,6 +68,28 @@ def main(reps=20):
             t_gpu.append(t1 - t0); t_host.append(t3 - t2)
     print("draw_heads        %.3f ms per frame (median of %d calls of %d frames)" % (np.median(t_gpu) * 1e3 / n, reps, n))
     print("download+cv2+up   %.3f ms per frame" % (np.median(t_host) * 1e3 / n))
+
+    t_full, t_simple, t_hfull = [], [], []
+    for r in range(reps + 2):
+        dev.copy_(torch.from_numpy(frames)); torch.cuda.synchronize()
+        t0 = time.perf_counter(); overlay.draw_heads(wn, dev, res, display="full"); t1 = time.perf_counter()
+        got = dev.cpu().numpy()
+        dev.copy_(torch.from_numpy(frames)); torch.cuda.synchronize()
+        t2 = time.perf_counter(); overlay.draw_heads(wn, dev, res, display="simple"); t3 = time.perf_counter()
+        dev.copy_(torch.from_numpy(frames)); torch.cuda.synchronize()
+        t4 = time.perf_counter()
+        host = dev.cpu().numpy()
+        for f in range(n):
+            for i in range(20):
+                ref_draw_full(host[f], res[f][0][i], res[f][2][i])
+        dev.copy_(torch.from_numpy(host)); torch.cuda.synchronize()
+        t5 = time.perf_counter()
+        assert np.array_equal(got, host)
+        if r >= 2:
+            t_full.append(t1 - t0); t_simple.append(t3 - t2); t_hfull.append(t5 - t4)
+    print("draw_heads full   %.3f ms per frame" % (np.median(t_full) * 1e3 / n))
+    print("draw_heads simple %.3f ms per frame" % (np.median(t_simple) * 1e3 / n))
+    print("download+cv2 full+up %.3f ms per frame" % (np.median(t_hfull) * 1e3 / n))
     yolo = whenet_b200.YOLO(None, max_frames=8)
     for _ in range(3):
         pipeline.detect_and_estimate_frames(yolo, wn, dev)
