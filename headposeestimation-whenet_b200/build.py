@@ -13,7 +13,7 @@ _SIMT_TC = ["kernels_simt.cuh", "kernels_tc.cuh"]
 _ABI = os.path.join("..", "..", "include", "whenet_b200.h")
 # translation unit -> the headers it depends on (a unit is recompiled when it or one of them is newer than its object)
 UNITS = {
-    "whenet_api.cu": _SIMT_TC + ["api_error.h", "kernels_fused.cuh", "kernels_crop.cuh", "kernels_overlay.cuh", "hershey_simplex.inc", "yuv.cuh", "kernels_k2.cuh", "kernels_tc32.cuh", "kernels_dwse.cuh", "kernels_k1x.cuh", _ABI],
+    "whenet_api.cu": _SIMT_TC + ["api_error.h", "kernels_fused.cuh", "kernels_crop.cuh", "kernels_overlay.cuh", "hershey_simplex.inc", "yuv.cuh", "kernels_k2.cuh", "kernels_tc32.cuh", "kernels_dwse.cuh", "kernels_k1x.cuh", "jpeg_api.h", _ABI],
     "inst_k1_bf16.cu": _SIMT_TC + ["kernels_fused.cuh", "kernels_dwse.cuh", "kernels_k1x.cuh"],
     "inst_k1_f16.cu": _SIMT_TC + ["kernels_fused.cuh"],
     "inst_dwse.cu": _SIMT_TC + ["kernels_fused.cuh", "kernels_dwse.cuh"],
@@ -21,6 +21,7 @@ UNITS = {
     "inst_yolo.cu": _SIMT_TC + ["kernels_yolo.cuh", "yuv.cuh"],
     "inst_yolo32.cu": _SIMT_TC + ["kernels_yolo.cuh", "kernels_yolo32.cuh", "yuv.cuh"],
     "yolo_api.cu": _SIMT_TC + ["kernels_yolo.cuh", "kernels_yolo32.cuh", "yuv.cuh", "api_error.h", _ABI],
+    "jpeg_api.cu": ["kernels_jpeg.cuh", "jpeg_api.h", "api_error.h", _ABI],
 }
 SOURCES = list(UNITS)
 HEADERS = sorted({h for hs in UNITS.values() for h in hs})

@@ -1,0 +1,338 @@
+// jpeg_api.cu - whenet_encode_jpeg_u8 / _ragged_u8 and whenet_debug_jpeg_header (DESIGN.md section 8.9): baseline JPEG files of
+// device or host BGR frames, byte-identical to cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, quality]).
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdint>
+#include <cstring>
+#include <vector>
+
+#include "../../include/whenet_b200.h"
+#include "api_error.h"
+#include "jpeg_api.h"
+#include "kernels_jpeg.cuh"
+
+using whenet::api::fail;
+namespace J = whenet::jpeg;
+
+#define JCK(call)                                                                                  \
+    do {                                                                                           \
+        cudaError_t e__ = (call);                                                                  \
+        if (e__ != cudaSuccess)                                                                    \
+            return fail(WHENET_ECUDA, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,         \
+                        cudaGetErrorString(e__));                                                  \
+    } while (0)
+
+namespace whenet {
+namespace jpeg {
+
+// Every buffer grows to what a call needs and is kept for the next call; all are freed by destroy().
+struct State {
+    uint32_t* d_huff = nullptr;                 // 4 x 256 entries: length << 16 | code
+    Frame* d_frames = nullptr;
+    long long* d_small = nullptr;               // per-frame bit totals, then the n + 1 output offsets
+    long long* h_small = nullptr;               // pinned
+    uint8_t* d_in = nullptr; size_t in_cap = 0;                 // host frames, uploaded
+    int16_t* d_coef = nullptr; size_t coef_cap = 0;             // elements
+    int* d_bits = nullptr; size_t bits_cap = 0;                 // per block
+    long long* d_excl = nullptr; size_t excl_cap = 0;           // per block + 1, then per chunk + 1
+    long long* d_tiles = nullptr; size_t tiles_cap = 0;
+    uint32_t* d_raw = nullptr; size_t raw_cap = 0;              // bytes
+    int* d_ffc = nullptr; size_t ffc_cap = 0;                   // 0xFF bytes per chunk
+    long long* d_ffx = nullptr; size_t ffx_cap = 0;
+    uint8_t* d_out = nullptr; size_t out_cap = 0;
+    uint8_t* h_out = nullptr; size_t h_cap = 0;                 // pinned: the files handed to the caller
+};
+
+}  // namespace jpeg
+}  // namespace whenet
+
+namespace {
+
+// T.81 Annex K.1 (natural order) and K.3
+const uint8_t kLumaQ[64] = {16, 11, 10, 16, 24,  40,  51,  61,  12, 12, 14, 19, 26,  58,  60,  55,  14, 13, 16, 24, 40,  57,
+                            69, 56, 14, 17, 22,  29,  51,  87,  80, 62, 18, 22, 37,  56,  68,  109, 103, 77, 24, 35, 55,  64,
+                            81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100, 103, 99};
+const uint8_t kChromaQ[64] = {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99,
+                              99, 99, 47, 66, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99,
+                              99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99};
+const uint8_t kZigzagHost[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                                 41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                                 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+const uint8_t kDcCounts[2][16] = {{0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0}, {0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0}};
+const uint8_t kDcSyms[12] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11};
+const uint8_t kAcCounts[2][16] = {{0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7d}, {0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77}};
+const uint8_t kAcSyms[2][162] = {
+    {0x01, 0x02, 0x03, 0x00, 0x04, 0x11, 0x05, 0x12, 0x21, 0x31, 0x41, 0x06, 0x13, 0x51, 0x61, 0x07, 0x22, 0x71, 0x14, 0x32, 0x81,
+     0x91, 0xa1, 0x08, 0x23, 0x42, 0xb1, 0xc1, 0x15, 0x52, 0xd1, 0xf0, 0x24, 0x33, 0x62, 0x72, 0x82, 0x09, 0x0a, 0x16, 0x17, 0x18,
+     0x19, 0x1a, 0x25, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x34, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47, 0x48,
+     0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75,
+     0x76, 0x77, 0x78, 0x79, 0x7a, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99,
+     0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3,
+     0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe1, 0xe2, 0xe3, 0xe4, 0xe5,
+     0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf1, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+    {0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 0x21, 0x31, 0x06, 0x12, 0x41, 0x51, 0x07, 0x61, 0x71, 0x13, 0x22, 0x32, 0x81, 0x08,
+     0x14, 0x42, 0x91, 0xa1, 0xb1, 0xc1, 0x09, 0x23, 0x33, 0x52, 0xf0, 0x15, 0x62, 0x72, 0xd1, 0x0a, 0x16, 0x24, 0x34, 0xe1, 0x25,
+     0xf1, 0x17, 0x18, 0x19, 0x1a, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47,
+     0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74,
+     0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x82, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97,
+     0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba,
+     0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4,
+     0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa}};
+
+// IJG quality scaling, clamped to baseline's [1, 255]; natural order
+void quant_table(int quality, int chroma, int out[64]) {
+    const int s = quality < 50 ? 5000 / quality : 200 - 2 * quality;
+    for (int i = 0; i < 64; ++i) out[i] = std::min(255, std::max(1, ((chroma ? kChromaQ : kLumaQ)[i] * s + 50) / 100));
+}
+
+// canonical codes (T.81 Annex C): table[symbol] = length << 16 | code
+void huff_table(const uint8_t counts[16], const uint8_t* syms, uint32_t table[256]) {
+    uint32_t code = 0;
+    int k = 0;
+    for (int len = 1; len <= 16; ++len) {
+        for (int i = 0; i < counts[len - 1]; ++i) table[syms[k++]] = (uint32_t)len << 16 | code++;
+        code <<= 1;
+    }
+}
+
+// SOI, APP0 (JFIF 1.01, density 1:1, no thumbnail), DQT luma and chroma (zigzag), SOF0, DHT DC0 AC0 DC1 AC1, SOS
+int header_bytes(int H, int W, int quality, uint8_t* out) {
+    uint8_t* p = out;
+    auto seg = [&](uint8_t marker, int len) { *p++ = 0xFF; *p++ = marker; *p++ = (uint8_t)((len + 2) >> 8); *p++ = (uint8_t)(len + 2); };
+    *p++ = 0xFF; *p++ = 0xD8;
+    seg(0xE0, 14);
+    const uint8_t app0[14] = {'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
+    memcpy(p, app0, 14); p += 14;
+    for (int t = 0; t < 2; ++t) {
+        int q[64];
+        quant_table(quality, t, q);
+        seg(0xDB, 65);
+        *p++ = (uint8_t)t;
+        for (int k = 0; k < 64; ++k) *p++ = (uint8_t)q[kZigzagHost[k]];
+    }
+    seg(0xC0, 15);
+    const uint8_t sof[15] = {8, (uint8_t)(H >> 8), (uint8_t)H, (uint8_t)(W >> 8), (uint8_t)W, 3, 1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1};
+    memcpy(p, sof, 15); p += 15;
+    for (int t = 0; t < 4; ++t) {
+        const int chroma = t >> 1, ac = t & 1;
+        const uint8_t* counts = ac ? kAcCounts[chroma] : kDcCounts[chroma];
+        int nsym = 0;
+        for (int i = 0; i < 16; ++i) nsym += counts[i];
+        seg(0xC4, 17 + nsym);
+        *p++ = (uint8_t)(ac << 4 | chroma);
+        memcpy(p, counts, 16); p += 16;
+        memcpy(p, ac ? kAcSyms[chroma] : kDcSyms, nsym); p += nsym;
+    }
+    seg(0xDA, 10);
+    const uint8_t sos[10] = {3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0};
+    memcpy(p, sos, 10); p += 10;
+    return (int)(p - out);
+}
+
+template <class T>
+int grow(T*& p, size_t& cap, size_t need) {
+    if (need <= cap) return 0;
+    if (p) cudaFree(p);
+    p = nullptr; cap = 0;
+    JCK(cudaMalloc(&p, need * sizeof(T)));
+    cap = need;
+    return 0;
+}
+
+int grow_host(uint8_t*& p, size_t& cap, size_t need) {
+    if (need <= cap) return 0;
+    if (p) cudaFreeHost(p);
+    p = nullptr; cap = 0;
+    JCK(cudaHostAlloc((void**)&p, need, cudaHostAllocDefault));
+    cap = need;
+    return 0;
+}
+
+int create(J::State*& st) {
+    st = new J::State();
+    JCK(cudaMalloc(&st->d_huff, 4 * 256 * sizeof(uint32_t)));
+    JCK(cudaMalloc(&st->d_frames, J::kMaxFrames * sizeof(J::Frame)));
+    JCK(cudaMalloc(&st->d_small, (J::kMaxFrames + 1) * sizeof(long long)));
+    JCK(cudaHostAlloc((void**)&st->h_small, (J::kMaxFrames + 1) * sizeof(long long), cudaHostAllocDefault));
+    std::vector<uint32_t> huff(4 * 256, 0);
+    for (int t = 0; t < 4; ++t) {
+        const int chroma = t >> 1, ac = t & 1;
+        huff_table(ac ? kAcCounts[chroma] : kDcCounts[chroma], ac ? kAcSyms[chroma] : kDcSyms, huff.data() + 256 * t);
+    }
+    JCK(cudaMemcpy(st->d_huff, huff.data(), huff.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+// exclusive scan of count values into out[0 .. count]; out[count] = the total
+template <typename T>
+int scan(J::State* st, cudaStream_t s, const T* in, long long count, long long* out) {
+    const long long tiles = (count + J::kScanTile - 1) / J::kScanTile;
+    if (int rc = grow(st->d_tiles, st->tiles_cap, (size_t)tiles)) return rc;
+    J::jpeg_scan_tiles_kernel<T><<<(unsigned)tiles, J::kScanThreads, 0, s>>>(in, count, st->d_tiles);
+    J::jpeg_scan_sums_kernel<<<1, J::kScanThreads, 0, s>>>(st->d_tiles, tiles, out + count);
+    J::jpeg_scan_apply_kernel<T><<<(unsigned)tiles, J::kScanThreads, 0, s>>>(in, count, st->d_tiles, out);
+    JCK(cudaGetLastError());
+    return 0;
+}
+
+int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int quality,
+           const uint8_t** data_out, int64_t* offsets_out) {
+    JCK(cudaSetDevice(t.device));
+    if (!*t.state)
+        if (int rc = create(*t.state)) return rc;
+    J::State* st = *t.state;
+    const cudaStream_t s = t.stream;
+
+    std::vector<J::Frame> fr(n);
+    long long ctas = 0, blocks = 0;
+    size_t in_bytes = 0;
+    for (int i = 0; i < n; ++i) {
+        J::Frame& f = fr[i];
+        f.H = hw[2 * i]; f.W = hw[2 * i + 1];
+        f.mcux = (f.W + 15) / 16; f.mcuy = (f.H + 15) / 16;
+        f.strips = (f.mcux + J::kStripMcus - 1) / J::kStripMcus;
+        f.cta0 = ctas; f.blk0 = blocks;
+        ctas += (long long)f.strips * f.mcuy;
+        blocks += 6LL * f.mcux * f.mcuy;
+        in_bytes += (size_t)f.H * f.W * 3;
+        f.src = frames[i];
+    }
+    if (!frames_are_device) {
+        if (int rc = grow(st->d_in, st->in_cap, in_bytes)) return rc;
+        size_t o = 0;
+        for (int i = 0; i < n; ++i) {
+            const size_t b = (size_t)fr[i].H * fr[i].W * 3;
+            JCK(cudaMemcpyAsync(st->d_in + o, frames[i], b, cudaMemcpyHostToDevice, s));
+            fr[i].src = st->d_in + o;
+            o += b;
+        }
+    }
+    J::Quant qt;
+    for (int c = 0; c < 2; ++c) {
+        int q[64];
+        quant_table(quality, c, q);
+        for (int k = 0; k < 64; ++k) qt.q8[c][k] = (uint16_t)(8 * q[k]);
+    }
+    if (int rc = grow(st->d_coef, st->coef_cap, (size_t)blocks * 64)) return rc;
+    if (int rc = grow(st->d_bits, st->bits_cap, (size_t)blocks)) return rc;
+    if (int rc = grow(st->d_excl, st->excl_cap, (size_t)blocks + 1)) return rc;
+    JCK(cudaMemcpyAsync(st->d_frames, fr.data(), n * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
+
+    // coefficients, bit lengths, bit offsets; the per-frame totals size the bitstream exactly
+    J::jpeg_transform_kernel<<<(unsigned)ctas, J::kTransformThreads, 0, s>>>(st->d_frames, n, qt, st->d_coef);
+    const unsigned code_grid = (unsigned)((blocks + J::kCodeThreads - 1) / J::kCodeThreads);
+    J::jpeg_code_kernel<0><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, st->d_huff, st->d_bits, nullptr, nullptr);
+    JCK(cudaGetLastError());
+    if (int rc = scan(st, s, st->d_bits, blocks, st->d_excl)) return rc;
+    J::jpeg_frame_bits_kernel<<<1, J::kMaxFrames, 0, s>>>(st->d_frames, n, st->d_excl, st->d_small);
+    JCK(cudaGetLastError());
+    JCK(cudaMemcpyAsync(st->h_small, st->d_small, n * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    JCK(cudaStreamSynchronize(s));
+    long long raw = 0;
+    for (int i = 0; i < n; ++i) {
+        fr[i].raw0 = raw;
+        fr[i].nbytes = (st->h_small[i] + 7) / 8;
+        raw += (fr[i].nbytes + J::kChunk - 1) / J::kChunk * J::kChunk;
+    }
+    const long long chunks = raw / J::kChunk;
+
+    // the codes, then 0x00 after every 0xFF
+    if (int rc = grow(st->d_raw, st->raw_cap, (size_t)raw / 4)) return rc;
+    JCK(cudaMemsetAsync(st->d_raw, 0, (size_t)raw, s));
+    JCK(cudaMemcpyAsync(st->d_frames, fr.data(), n * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
+    J::jpeg_code_kernel<1><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, st->d_huff, nullptr, st->d_excl, st->d_raw);
+    if (int rc = grow(st->d_ffc, st->ffc_cap, (size_t)chunks)) return rc;
+    if (int rc = grow(st->d_ffx, st->ffx_cap, (size_t)chunks + 1)) return rc;
+    const unsigned chunk_grid = (unsigned)((chunks + 255) / 256);
+    J::jpeg_ff_count_kernel<<<chunk_grid, 256, 0, s>>>(reinterpret_cast<const uint4*>(st->d_raw), chunks, st->d_ffc);
+    JCK(cudaGetLastError());
+    if (int rc = scan(st, s, st->d_ffc, chunks, st->d_ffx)) return rc;
+    J::jpeg_place_kernel<<<1, 32, 0, s>>>(st->d_frames, n, st->d_ffx, st->d_small);
+    JCK(cudaGetLastError());
+    JCK(cudaMemcpyAsync(st->h_small, st->d_small, (n + 1) * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    JCK(cudaStreamSynchronize(s));
+    const long long total = st->h_small[n];
+    if (int rc = grow(st->d_out, st->out_cap, (size_t)total)) return rc;
+    J::jpeg_stuff_kernel<<<chunk_grid, 256, 0, s>>>(st->d_frames, n, reinterpret_cast<const uint4*>(st->d_raw), chunks, st->d_ffx, st->d_small,
+                                                    st->d_out);
+    JCK(cudaGetLastError());
+    if (int rc = grow_host(st->h_out, st->h_cap, (size_t)total)) return rc;
+    JCK(cudaMemcpyAsync(st->h_out, st->d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+    JCK(cudaStreamSynchronize(s));
+
+    // the host frames each stream: header before, EOI after
+    for (int i = 0; i <= n; ++i) offsets_out[i] = st->h_small[i];
+    for (int i = 0; i < n; ++i) {
+        header_bytes(fr[i].H, fr[i].W, quality, st->h_out + offsets_out[i]);
+        st->h_out[offsets_out[i + 1] - 2] = 0xFF;
+        st->h_out[offsets_out[i + 1] - 1] = 0xD9;
+    }
+    *data_out = st->h_out;
+    return 0;
+}
+
+int encode_checked(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int quality,
+                   const uint8_t** data_out, int64_t* offsets_out) {
+    // the context is checked last so that every other argument can be validated without a GPU
+    if (n < 1 || n > J::kMaxFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, J::kMaxFrames);
+    for (int i = 0; i < n; ++i) {
+        if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
+        if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
+            return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
+    }
+    if (quality < 1 || quality > 100) return fail(WHENET_EINVAL, "quality %d outside [1, 100]", quality);
+    if (!data_out || !offsets_out) return fail(WHENET_EINVAL, "null data_out or offsets_out");
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    return encode(J::target(c), frames, hw, n, frames_are_device, quality, data_out, offsets_out);
+}
+
+}  // namespace
+
+namespace whenet {
+namespace jpeg {
+
+void destroy(State* st) {
+    if (!st) return;
+    for (void* p : {(void*)st->d_huff, (void*)st->d_frames, (void*)st->d_small, (void*)st->d_in, (void*)st->d_coef, (void*)st->d_bits,
+                    (void*)st->d_excl, (void*)st->d_tiles, (void*)st->d_raw, (void*)st->d_ffc, (void*)st->d_ffx, (void*)st->d_out})
+        if (p) cudaFree(p);
+    if (st->h_small) cudaFreeHost(st->h_small);
+    if (st->h_out) cudaFreeHost(st->h_out);
+    delete st;
+}
+
+}  // namespace jpeg
+}  // namespace whenet
+
+extern "C" {
+
+int whenet_encode_jpeg_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, int quality,
+                          const uint8_t** data_out, int64_t* offsets_out) {
+    if (!frames) return fail(WHENET_EINVAL, "null frames");
+    if (n < 1 || n > J::kMaxFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, J::kMaxFrames);
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    const uint8_t* ptrs[J::kMaxFrames];
+    int32_t hw[2 * J::kMaxFrames];
+    for (int i = 0; i < n; ++i) {
+        ptrs[i] = frames + (size_t)i * H * W * 3;
+        hw[2 * i] = H; hw[2 * i + 1] = W;
+    }
+    return encode_checked(c, ptrs, hw, n, frames_are_device, quality, data_out, offsets_out);
+}
+
+int whenet_encode_jpeg_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int quality,
+                                 const uint8_t** data_out, int64_t* offsets_out) {
+    if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
+    return encode_checked(c, frames, hw, n, frames_are_device, quality, data_out, offsets_out);
+}
+
+int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, int* len) {
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    if (quality < 1 || quality > 100) return fail(WHENET_EINVAL, "quality %d outside [1, 100]", quality);
+    if (!out || !len || cap < J::kHeaderBytes) return fail(WHENET_EINVAL, "null out or len, or cap %d < %d", cap, J::kHeaderBytes);
+    *len = header_bytes(H, W, quality, out);
+    return 0;
+}
+
+}  // extern "C"

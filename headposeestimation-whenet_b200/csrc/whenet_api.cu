@@ -30,6 +30,7 @@
 #include "kernels_tc32.cuh"
 #include "kernels_dwse.cuh"
 #include "kernels_k1x.cuh"
+#include "jpeg_api.h"
 #include <cudaTypedefs.h>
 
 // The fused-kernel launchers are instantiated in their own translation units (inst_k1_bf16.cu, inst_k1_f16.cu, inst_dwse.cu)
@@ -214,6 +215,8 @@ struct whenet_ctx {
     whenet::OverlayThin* d_thin = nullptr; int thin_cap = 0;
     int* d_bands = nullptr; int bands_cap = 0;
     int* d_items = nullptr; int items_cap = 0;
+    // JPEG encoder scratch (jpeg_api.cu), created by the first encode
+    whenet::jpeg::State* jpeg = nullptr;
     // taps (whenet_debug_enable_taps): 0 off, 1 first chunk of <= 8 crops on the one-stream route, 2 every chunk on the
     // untapped route.  Keyed by the canonical name ("dw%d" also holds a gated "dwg%d"); `valid`: written by the last forward.
     struct Tap { float* p = nullptr; size_t cap = 0, n = 0; bool valid = false; int forms = 0; };   // forms: 1 ungated, 2 gated rows
@@ -2078,6 +2081,8 @@ static_assert(whenet::kOverlayMaxFrames == whenet::kMaxCropFrames, "overlay fram
 
 }  // namespace
 
+whenet::jpeg::Target whenet::jpeg::target(whenet_ctx* c) { return {&c->jpeg, c->device, c->stream}; }
+
 extern "C" {
 
 int whenet_crop_boxes_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes,
@@ -2473,6 +2478,7 @@ void whenet_destroy(whenet_ctx* c) {
     if (c->d_thin) cudaFree(c->d_thin);
     if (c->d_bands) cudaFree(c->d_bands);
     if (c->d_items) cudaFree(c->d_items);
+    whenet::jpeg::destroy(c->jpeg);
     for (auto& kv : c->taps) cudaFree(kv.second.p);
     if (c->d_tap_map) cudaFree(c->d_tap_map);
     for (auto& p : c->ev_used) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }

@@ -258,6 +258,20 @@ int whenet_debug_text_segments(const char* text, int org_x, int org_y, double sc
 /* The number of each display="full" label: str(np.round(np.float32(a))) for m float32 angles, NUL-terminated, one per
    `stride` (>= 32) bytes of out. */
 int whenet_debug_label_text(const float* angles, int m, char* out, int stride);
+/* Baseline JPEG files of n BGR frames (DESIGN.md section 8.9), byte-identical to
+   cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, quality]): 4:2:0, the Annex K tables scaled by the IJG quality
+   rule, no restart markers.  frames: n frames of H x W x 3 bytes back to back, in device memory (frames_are_device = 1) or
+   host memory (0).  n in [1, 64], sides in [1, 16384], quality in [1, 100]; anything else is WHENET_EINVAL before any device
+   call.  Runs on the context's stream and returns when the files are on the host: *data_out points into a pinned buffer
+   the context owns, valid until its next encode call; offsets_out (n + 1 int64 on the host): file i is
+   data[offsets[i] : offsets[i + 1]].  Scratch grows with the call and is freed with the context. */
+int whenet_encode_jpeg_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, int W, int frames_are_device, int quality,
+                          const uint8_t** data_out, int64_t* offsets_out);
+/* the same on n frames of their own sizes: frames[i] is H_i x W_i x 3, hw = n x (H_i, W_i) int32 on the host */
+int whenet_encode_jpeg_ragged_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                 int quality, const uint8_t** data_out, int64_t* offsets_out);
+/* The bytes of a file before its entropy-coded data (SOI .. SOS, 623 bytes) without a GPU; cap >= 623. */
+int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, int* len);
 
 
 /* Time every kernel of the NEXT forwards with CUDA events. */
