@@ -21,7 +21,7 @@ UNITS = {
     "inst_yolo.cu": _SIMT_TC + ["kernels_yolo.cuh", "yuv.cuh"],
     "inst_yolo32.cu": _SIMT_TC + ["kernels_yolo.cuh", "kernels_yolo32.cuh", "yuv.cuh"],
     "yolo_api.cu": _SIMT_TC + ["kernels_yolo.cuh", "kernels_yolo32.cuh", "yuv.cuh", "api_error.h", _ABI],
-    "jpeg_api.cu": ["kernels_jpeg.cuh", "jpeg_api.h", "api_error.h", _ABI],
+    "jpeg_api.cu": ["kernels_jpeg.cuh", "jpeg_api.h", "api_error.h", "jpeg_decode.inc", "kernels_jpeg_dec.cuh", _ABI],
 }
 SOURCES = list(UNITS)
 HEADERS = sorted({h for hs in UNITS.values() for h in hs})

@@ -1,10 +1,12 @@
 // jpeg_api.cu - whenet_encode_jpeg_u8 / _ragged_u8 and whenet_debug_jpeg_header (DESIGN.md section 8.9): baseline JPEG files of
-// device or host BGR frames, byte-identical to cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, quality]).
+// device or host BGR frames, byte-identical to cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, quality]).  The decoder
+// (section 8.10) is jpeg_decode.inc, included at the end.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <string>
 #include <vector>
 
 #include "../../include/whenet_b200.h"
@@ -42,6 +44,7 @@ struct State {
     long long* d_ffx = nullptr; size_t ffx_cap = 0;
     uint8_t* d_out = nullptr; size_t out_cap = 0;
     uint8_t* h_out = nullptr; size_t h_cap = 0;                 // pinned: the files handed to the caller
+    DecState* dec = nullptr;                                    // the decoder's scratch (jpeg_decode.inc)
 };
 
 }  // namespace jpeg
@@ -292,8 +295,17 @@ int encode_checked(whenet_ctx* c, const uint8_t* const* frames, const int32_t* h
 namespace whenet {
 namespace jpeg {
 
+int dec_state(Target t, DecState**& slot) {
+    JCK(cudaSetDevice(t.device));
+    if (!*t.state)
+        if (int rc = create(*t.state)) return rc;
+    slot = &(*t.state)->dec;
+    return 0;
+}
+
 void destroy(State* st) {
     if (!st) return;
+    destroy_dec(st->dec);
     for (void* p : {(void*)st->d_huff, (void*)st->d_frames, (void*)st->d_small, (void*)st->d_in, (void*)st->d_coef, (void*)st->d_bits,
                     (void*)st->d_excl, (void*)st->d_tiles, (void*)st->d_raw, (void*)st->d_ffc, (void*)st->d_ffx, (void*)st->d_out})
         if (p) cudaFree(p);
@@ -336,3 +348,5 @@ int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, i
 }
 
 }  // extern "C"
+
+#include "jpeg_decode.inc"

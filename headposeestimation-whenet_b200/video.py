@@ -1,15 +1,21 @@
-"""Video output on the GPU path: JPEG encoding of device BGR frames and a Motion-JPEG AVI writer (DESIGN.md section 8.9).
+"""Video on the GPU path: JPEG encoding and decoding of device BGR frames, and Motion-JPEG AVI files (DESIGN.md sections 8.9
+and 8.10).
 
   ``encode_jpeg``   device (or host) BGR frames -> JPEG files, byte-identical to cv2.imencode(".jpg", frame,
                     [cv2.IMWRITE_JPEG_QUALITY, quality]), encoded by the library's CUDA kernels (``whenet_encode_jpeg_u8``)
+  ``decode_jpeg``   JPEG files -> device BGR frames, pixel-identical to cv2.imdecode(buf, cv2.IMREAD_COLOR), decoded by the
+                    library's CUDA kernels (``whenet_decode_jpeg_u8``)
   ``MJPGWriter``    writes those files as an MJPG AVI: what reference demo_video.py:46-47,60 writes through
                     cv2.VideoWriter(..., fourcc 'MJPG'), without the frames leaving the GPU uncompressed
+  ``MJPGReader``    reads the JPEG files of an MJPG AVI (the reference's cap.read(), demo_video.py:44,51)
 
-The reference's loop becomes::
+The reference's loop becomes a transcode on the device::
 
-    results = pipeline.detect_and_estimate_frames(yolo, whenet, frames)
-    overlay.draw_heads(whenet, frames, results)
-    writer.write(video.encode_jpeg(whenet, frames))
+    with video.MJPGReader(src) as r, video.MJPGWriter(dst, r.fps, r.frame_size) as w:
+        while (frames := r.read_frames(whenet, 8)) is not None:
+            results = pipeline.detect_and_estimate_frames(yolo, whenet, frames)
+            overlay.draw_heads(whenet, frames, results, display="full")
+            w.write(video.encode_jpeg(whenet, frames))
 """
 from __future__ import annotations
 
@@ -98,6 +104,82 @@ def encode_jpeg(whenet, frames, quality: int = 95) -> list:
             for i in range(hi - lo):
                 out.append(C.string_at(data.value + int(offsets[i]), int(offsets[i + 1] - offsets[i])))
     return out
+
+
+def _jpeg_files(files):
+    """``files`` as a list of bytes, or ValueError naming the first item that is not bytes-like."""
+    if isinstance(files, (bytes, bytearray, memoryview)) or not isinstance(files, (list, tuple)):
+        raise ValueError("files must be a list or tuple of bytes-like JPEG files, not %s" % type(files).__name__)
+    out = []
+    for i, f in enumerate(files):
+        if isinstance(f, bytes):
+            out.append(f)
+        elif isinstance(f, (bytearray, memoryview)) or (isinstance(f, np.ndarray) and f.dtype == np.uint8 and f.ndim == 1):
+            out.append(bytes(f))
+        else:
+            raise ValueError("file %d is %s, not bytes" % (i, type(f).__name__))
+    return out
+
+
+def jpeg_info(data: bytes):
+    """(H, W) of the frame ``decode_jpeg`` makes of ``data`` (after its EXIF orientation), parsed on the host without a GPU;
+    ValueError with the reason for a file outside the supported subset (DESIGN.md section 8.10)."""
+    import ctypes as C
+    from ._lib import load
+    hw = (C.c_int32 * 2)()
+    msg = C.create_string_buffer(256)
+    if load().whenet_jpeg_info(data, len(data), hw, msg, len(msg)) != 0:
+        raise ValueError(msg.value.decode("utf-8", "replace"))
+    return int(hw[0]), int(hw[1])
+
+
+def _decode_into(whenet, files, outs, first_index=0):
+    """Decode ``files`` (bytes) into the contiguous (H, W, 3) uint8 CUDA tensors ``outs`` in groups of 64."""
+    import ctypes as C
+    import torch
+    from ._lib import WhenetError, check
+    L = whenet._L
+    with torch.cuda.device(whenet.device):
+        torch.cuda.current_stream().synchronize()       # the outputs' memory is no longer in use on torch's stream
+        for lo in range(0, len(files), MAX_FRAMES_PER_CALL):
+            hi = min(len(files), lo + MAX_FRAMES_PER_CALL)
+            k = hi - lo
+            bufs = [C.create_string_buffer(f, len(f)) for f in files[lo:hi]]
+            ptrs = (C.c_void_p * k)(*[C.addressof(b) for b in bufs])
+            sizes = (C.c_int64 * k)(*[len(f) for f in files[lo:hi]])
+            dst = (C.c_void_p * k)(*[o.data_ptr() for o in outs[lo:hi]])
+            status = (C.c_int32 * k)()
+            try:
+                check(L.whenet_decode_jpeg_u8(whenet._h, ptrs, sizes, k, dst, status))
+            except WhenetError as e:
+                bad = next((i for i in range(k) if status[i]), None)
+                msg = str(e).split(": ", 1)[-1]
+                if bad is not None:
+                    msg = "file %d: %s" % (first_index + lo + bad, msg.split(": ", 1)[-1])
+                raise ValueError(msg) from None
+
+
+def decode_jpeg(whenet, files) -> list:
+    """Decode JPEG ``files`` (a list of bytes-like objects) on ``whenet``'s GPU and stream into BGR frames, each equal to
+    ``cv2.imdecode(np.frombuffer(f, np.uint8), cv2.IMREAD_COLOR)``: baseline or extended-sequential Huffman, 1 or 3 components,
+    4:4:4, 4:2:2 or 4:2:0, restart intervals, files without DHT, EXIF orientation applied, sides 1..16384.
+
+    Returns a list of contiguous (H_i, W_i, 3) uint8 CUDA tensors on ``whenet.device``, decoded in groups of 64 files with one
+    synchronisation each; n = 0 gives [].  Bad arguments, a file outside that subset (checked before any device work) or
+    corrupt entropy-coded data raise ``ValueError`` naming the file index and the reason."""
+    import torch
+    files = _jpeg_files(files)
+    if not files:
+        return []
+    shapes = []
+    for i, f in enumerate(files):
+        try:
+            shapes.append(jpeg_info(f))
+        except ValueError as e:
+            raise ValueError("file %d: %s" % (i, e)) from None
+    outs = [torch.empty((h, w, 3), dtype=torch.uint8, device="cuda:%d" % whenet.device) for h, w in shapes]
+    _decode_into(whenet, files, outs)
+    return outs
 
 
 # ----------------------------------------------------------------------------------------------------------------- AVI
@@ -285,6 +367,203 @@ class MJPGWriter:
         f.seek(end)
         f.close()
         self._f = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+        return False
+
+
+class MJPGReader:
+    """The JPEG files of a Motion-JPEG AVI, read on the host: the counterpart of ``MJPGWriter`` and what the reference reads
+    through cv2.VideoCapture.  The first video stream whose handler or compression is MJPG (any case) is read; ``fps`` comes
+    from its ``strh`` rate / scale and ``frame_size`` = (width, height) from its ``strf``.
+
+    Frames are found through the OpenDML super index (``indx`` -> ``ix##`` standard indexes, across ``AVIX`` segments), else
+    ``idx1`` (offsets relative to ``movi`` or absolute, told apart by the first entry), else by walking the ``movi`` lists.
+    Chunks of other streams and JUNK are skipped, and a last chunk cut short by the end of the file is not returned.
+
+    ``read(n)`` returns up to n JPEG files as bytes ([] at the end); ``read_frames(whenet, n)`` decodes up to n of them into one
+    (k, H, W, 3) uint8 CUDA tensor (``None`` at the end).  ``len()`` is the number of frames.  Use as a context manager or call
+    ``close()``."""
+
+    def __init__(self, path):
+        self._f = open(path, "rb")
+        try:
+            self._f.seek(0, 2)
+            self._size = self._f.tell()
+            self._parse()
+        except Exception:
+            self._f.close()
+            raise
+        self._next = 0
+
+    # -- RIFF
+    def _read_at(self, off, n):
+        self._f.seek(off)
+        return self._f.read(n)
+
+    def _chunks(self, start, end):
+        """(fourcc, data offset, data size, list type or None) of the chunks in [start, end)."""
+        pos = start
+        while pos + 8 <= min(end, self._size):
+            hdr = self._read_at(pos, 12)
+            fcc, size = hdr[:4], struct.unpack("<I", hdr[4:8])[0]
+            if fcc in (b"LIST", b"RIFF"):
+                yield fcc, pos + 12, size - 4, hdr[8:12]
+            else:
+                yield fcc, pos + 8, size, None
+            pos += 8 + size + (size & 1)
+
+    def _parse(self):
+        head = self._read_at(0, 12)
+        if len(head) < 12 or head[:4] != b"RIFF" or head[8:12] != b"AVI ":
+            raise ValueError("not a RIFF AVI file")
+        self._stream = None
+        indx = None
+        movis, idx1 = [], None
+        riffs = [(12, 8 + struct.unpack("<I", head[4:8])[0])]
+        pos = riffs[0][1] + (riffs[0][1] & 1)
+        while pos + 12 <= self._size:               # AVIX segments
+            h = self._read_at(pos, 12)
+            size = struct.unpack("<I", h[4:8])[0]
+            if h[:4] == b"RIFF" and h[8:12] == b"AVIX":
+                riffs.append((pos + 12, pos + 8 + size))
+            pos += 8 + size + (size & 1)
+        for r, (start, end) in enumerate(riffs):
+            for fcc, off, size, kind in self._chunks(start, end):
+                if kind == b"hdrl" and r == 0:
+                    indx = self._parse_hdrl(off, off + size)
+                elif kind == b"movi":
+                    movis.append((off - 4, off + size))     # the 'movi' fourcc, the list's end
+                elif fcc == b"idx1" and r == 0:
+                    idx1 = (off, size)
+        if self._stream is None:
+            raise ValueError("no MJPG video stream")
+        ids = (b"%02ddc" % self._stream, b"%02ddb" % self._stream)
+        frames = None
+        if indx:
+            frames = self._from_indx(indx, ids)
+        if not frames and idx1 and movis:
+            frames = self._from_idx1(idx1, movis[0][0], ids)
+        if not frames:
+            frames = []
+            for start, end in movis:
+                self._walk_movi(start + 4, end, ids, frames)
+        self._frames = [(o, n) for o, n in frames if o + n <= self._size]
+
+    def _parse_hdrl(self, start, end):
+        n = 0
+        for fcc, off, size, kind in self._chunks(start, end):
+            if kind != b"strl":
+                continue
+            strh = strf = indx = None
+            for f2, o2, s2, _ in self._chunks(off, off + size):
+                if f2 == b"strh":
+                    strh = self._read_at(o2, s2)
+                elif f2 == b"strf":
+                    strf = self._read_at(o2, s2)
+                elif f2 == b"indx":
+                    indx = (o2, s2)
+            if self._stream is None and strh and len(strh) >= 28 and strh[:4] == b"vids":
+                handler = strh[4:8].upper()
+                comp = strf[16:20].upper() if strf and len(strf) >= 20 else b""
+                if handler == b"MJPG" or comp == b"MJPG":
+                    scale, rate = struct.unpack("<II", strh[20:28])
+                    self.fps = rate / scale if scale else 0.0
+                    if strf and len(strf) >= 12:
+                        w, h = struct.unpack("<ii", strf[4:12])
+                    else:
+                        w, h = struct.unpack("<HH", strh[52:56]) if len(strh) >= 56 else (0, 0)
+                    self.frame_size = (int(w), abs(int(h)))
+                    self._stream = n
+                    return indx
+            n += 1
+        return None
+
+    def _from_indx(self, indx, ids):
+        off, size = indx
+        d = self._read_at(off, size)
+        if len(d) < 24:
+            return None
+        longs, sub, itype, entries = struct.unpack("<HBBI", d[:8])
+        if itype != 0 or longs != 4:                # AVI_INDEX_OF_INDEXES
+            return None
+        frames = []
+        for e in range(entries):
+            if 24 + 16 * e + 16 > len(d):
+                break
+            qoff, qsize, _ = struct.unpack("<QII", d[24 + 16 * e:40 + 16 * e])
+            ix = self._read_at(qoff, qsize)
+            if len(ix) < 32:
+                break
+            longs, sub, itype, n, cid, base = struct.unpack("<HBBI4sQ", ix[8:28])
+            if itype != 1 or longs != 2 or cid not in ids:
+                return None
+            for k in range(n):
+                if 32 + 8 * k + 8 > len(ix):
+                    break
+                o, s = struct.unpack("<II", ix[32 + 8 * k:40 + 8 * k])
+                frames.append((base + o, s & 0x7FFFFFFF))
+        return frames
+
+    def _from_idx1(self, idx1, movi, ids):
+        off, size = idx1
+        d = self._read_at(off, size)
+        entries = [struct.unpack("<4sIII", d[i:i + 16]) for i in range(0, len(d) - 15, 16)]
+        if not entries:
+            return None
+        first = entries[0]
+        base = movi if self._read_at(movi + first[2], 4) == first[0] else 0
+        return [(base + o + 8, s) for cid, _, o, s in entries if cid in ids]
+
+    def _walk_movi(self, start, end, ids, frames):
+        for fcc, off, size, kind in self._chunks(start, end):
+            if kind is not None:
+                self._walk_movi(off, off + size, ids, frames)       # LIST rec
+            elif fcc in ids:
+                frames.append((off, size))
+
+    # -- API
+    def __len__(self):
+        return len(self._frames)
+
+    def read(self, n=1):
+        """Up to ``n`` more JPEG files as bytes; [] at the end."""
+        if self._f is None:
+            raise ValueError("read on a closed MJPGReader")
+        out = []
+        for off, size in self._frames[self._next:self._next + max(0, int(n))]:
+            out.append(self._read_at(off, size))
+        self._next += len(out)
+        return out
+
+    def read_frames(self, whenet, n=1):
+        """Up to ``n`` more frames decoded on ``whenet``'s GPU into one (k, H, W, 3) uint8 CUDA tensor, or None at the end.  A
+        frame whose size differs from ``frame_size`` raises ValueError."""
+        import torch
+        first = self._next
+        files = self.read(n)
+        if not files:
+            return None
+        w, h = self.frame_size
+        for i, f in enumerate(files):
+            try:
+                hw = jpeg_info(f)
+            except ValueError as e:
+                raise ValueError("frame %d: %s" % (first + i, e)) from None
+            if hw != (h, w):
+                raise ValueError("frame %d is %dx%d, the stream's frame_size %dx%d" % (first + i, hw[1], hw[0], w, h))
+        out = torch.empty((len(files), h, w, 3), dtype=torch.uint8, device="cuda:%d" % whenet.device)
+        _decode_into(whenet, files, list(out), first_index=first)
+        return out
+
+    def close(self):
+        if self._f is not None:
+            self._f.close()
+            self._f = None
 
     def __enter__(self):
         return self

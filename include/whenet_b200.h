@@ -272,6 +272,23 @@ int whenet_encode_jpeg_ragged_u8(whenet_ctx* ctx, const uint8_t* const* frames, 
                                  int quality, const uint8_t** data_out, int64_t* offsets_out);
 /* The bytes of a file before its entropy-coded data (SOI .. SOS, 623 bytes) without a GPU; cap >= 623. */
 int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, int* len);
+/* JPEG decoding (DESIGN.md section 8.10), pixel-identical to cv2.imdecode(buf, cv2.IMREAD_COLOR): SOF0 / SOF1 8-bit Huffman,
+   one interleaved scan, 1 component (replicated to B = G = R) or 3 (YCbCr) at 4:4:4, 4:2:2 or 4:2:0, restart intervals,
+   Annex K tables where no DHT defines one, EXIF orientation 1..8 applied, sides 1..16384.
+   whenet_jpeg_info parses a file's header on the host without a GPU: hw_out = (H, W) of the decoded frame (after the
+   orientation), or WHENET_EINVAL with the reason in msg (cap bytes, may be NULL) and whenet_last_error(). */
+int whenet_jpeg_info(const uint8_t* data, int64_t len, int32_t* hw_out, char* msg, int cap);
+/* Decode n (1..64) host files (files[i], sizes[i] bytes) into caller-owned device frames out_frames[i], each H_i x W_i x 3
+   BGR as whenet_jpeg_info gives.  A header error is WHENET_EINVAL naming the file before any device call.  Runs on the
+   context's device and stream and returns when the frames are complete.  status_out (n int32 on the host, may be NULL):
+   per file 0, or bits 1 truncated data, 2 restart markers out of sequence or miscounted, 4 a marker inside the entropy-coded
+   data, 8 an invalid Huffman code, 16 an AC run past coefficient 63, 32 more or fewer blocks than the MCUs; any nonzero
+   status makes the call return WHENET_EINVAL (that file's frame is then undefined) and leaves the context usable.  Scratch
+   grows with the call and is freed with the context. */
+int whenet_decode_jpeg_u8(whenet_ctx* ctx, const uint8_t* const* files, const int64_t* sizes, int n, uint8_t* const* out_frames,
+                          int32_t* status_out);
+/* Bits per subsequence of the self-synchronising Huffman decode, 32..65536, or 0 for the default (2048). */
+int whenet_debug_jpeg_piece_bits(whenet_ctx* ctx, int bits);
 
 
 /* Time every kernel of the NEXT forwards with CUDA events. */
