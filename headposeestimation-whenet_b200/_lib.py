@@ -23,6 +23,7 @@ EXPORTS = [
     "whenet_draw_heads_ex_u8", "whenet_draw_heads_ex_ragged_u8", "whenet_put_text_u8", "whenet_put_text_ragged_u8",
     "whenet_debug_text_segments", "whenet_debug_label_text",
     "whenet_encode_jpeg_u8", "whenet_encode_jpeg_ragged_u8", "whenet_debug_jpeg_header",
+    "whenet_encode_jpeg_ex_u8", "whenet_debug_jpeg_header_ex", "whenet_debug_jpeg_optimal_table", "whenet_debug_jpeg_optimal_table_gpu",
     "whenet_jpeg_info", "whenet_decode_jpeg_u8", "whenet_debug_jpeg_piece_bits",
 ]
 
@@ -34,6 +35,12 @@ class WhenetError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("whenet_b200 error %d: %s" % (code, msg))
         self.code = code
+
+
+class JpegOptions(C.Structure):
+    """``whenet_jpeg_options``"""
+    _fields_ = [("quality", C.c_int), ("chroma_quality", C.c_int), ("sampling", C.c_int), ("restart_interval", C.c_int),
+                ("optimize", C.c_int)]
 
 
 class Tensor(C.Structure):
@@ -97,6 +104,10 @@ def load():
     L.whenet_encode_jpeg_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(P), P]
     L.whenet_encode_jpeg_ragged_u8.argtypes = [P, P, P, C.c_int, C.c_int, C.c_int, C.POINTER(P), P]
     L.whenet_debug_jpeg_header.argtypes = [C.c_int, C.c_int, C.c_int, P, C.c_int, P]
+    L.whenet_encode_jpeg_ex_u8.argtypes = [P, P, P, C.c_int, C.c_int, C.c_int, P, C.POINTER(P), P]
+    L.whenet_debug_jpeg_header_ex.argtypes = [C.c_int, C.c_int, C.c_int, P, P, C.c_int, P]
+    L.whenet_debug_jpeg_optimal_table.argtypes = [P, P, P, P]
+    L.whenet_debug_jpeg_optimal_table_gpu.argtypes = [P, P, P, P, P]
     L.whenet_jpeg_info.argtypes = [P, C.c_int64, P, C.c_char_p, C.c_int]
     L.whenet_decode_jpeg_u8.argtypes = [P, P, P, C.c_int, P, P]
     L.whenet_debug_jpeg_piece_bits.argtypes = [P, C.c_int]

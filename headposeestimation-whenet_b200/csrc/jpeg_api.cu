@@ -1,6 +1,7 @@
-// jpeg_api.cu - whenet_encode_jpeg_u8 / _ragged_u8 and whenet_debug_jpeg_header (DESIGN.md section 8.9): baseline JPEG files of
-// device or host BGR frames, byte-identical to cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, quality]).  The decoder
-// (section 8.10) is jpeg_decode.inc, included at the end.
+// jpeg_api.cu - whenet_encode_jpeg_u8 / _ragged_u8 / _ex_u8 and their debug entries (DESIGN.md sections 8.9 and 8.11): baseline
+// JPEG files of device or host BGR or gray frames, byte-identical to cv2.imencode(".jpg", frame, params) with the quality,
+// sampling, restart-interval, optimised-Huffman and luma/chroma-quality parameters.  The decoder (section 8.10) is
+// jpeg_decode.inc, included at the end.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -30,17 +31,23 @@ namespace jpeg {
 
 // Every buffer grows to what a call needs and is kept for the next call; all are freed by destroy().
 struct State {
-    uint32_t* d_huff = nullptr;                 // 4 x 256 entries: length << 16 | code
+    uint32_t* d_huff = nullptr;                 // 4 x 256 entries: length << 16 | code (Annex K)
+    uint32_t* d_ohuff = nullptr;                // optimised: 4 x 256 entries per frame
+    int* d_hist = nullptr;                      // optimised: 4 x 256 symbol counts per frame
+    uint8_t* d_dht = nullptr;                   // optimised: 4 x kDhtBytes per frame, read back with the segment chunk total
+    uint8_t* h_dht = nullptr;                   // pinned
     Frame* d_frames = nullptr;
-    long long* d_small = nullptr;               // per-frame bit totals, then the n + 1 output offsets
+    long long* d_small = nullptr;               // the n + 1 output offsets
     long long* h_small = nullptr;               // pinned
     uint8_t* d_in = nullptr; size_t in_cap = 0;                 // host frames, uploaded
     int16_t* d_coef = nullptr; size_t coef_cap = 0;             // elements
     int* d_bits = nullptr; size_t bits_cap = 0;                 // per block
-    long long* d_excl = nullptr; size_t excl_cap = 0;           // per block + 1, then per chunk + 1
+    long long* d_excl = nullptr; size_t excl_cap = 0;           // per block + 1
+    int* d_segc = nullptr; size_t segc_cap = 0;                 // chunks per segment
+    long long* d_segx = nullptr; size_t segx_cap = 0;           // per segment + 1: first chunk
     long long* d_tiles = nullptr; size_t tiles_cap = 0;
     uint32_t* d_raw = nullptr; size_t raw_cap = 0;              // bytes
-    int* d_ffc = nullptr; size_t ffc_cap = 0;                   // 0xFF bytes per chunk
+    int* d_ffc = nullptr; size_t ffc_cap = 0;                   // output bytes per chunk
     long long* d_ffx = nullptr; size_t ffx_cap = 0;
     uint8_t* d_out = nullptr; size_t out_cap = 0;
     uint8_t* h_out = nullptr; size_t h_cap = 0;                 // pinned: the files handed to the caller
@@ -99,38 +106,101 @@ void huff_table(const uint8_t counts[16], const uint8_t* syms, uint32_t table[25
     }
 }
 
-// SOI, APP0 (JFIF 1.01, density 1:1, no thumbnail), DQT luma and chroma (zigzag), SOF0, DHT DC0 AC0 DC1 AC1, SOS
-int header_bytes(int H, int W, int quality, uint8_t* out) {
+// What a call encodes: luma and chroma qualities, MCU shape (J::Shape, kGray for one channel), restart interval in MCUs
+// (0 = none), optimised tables.
+struct Opts {
+    int quality, chroma_quality, shape, restart, optimize;
+};
+constexpr int kMaxHeaderBytes = 2 + 18 + 2 * 69 + 19 + 4 * (5 + J::kDhtBytes) + 6 + 14;
+
+// SOI, APP0 (JFIF 1.01, density 1:1, no thumbnail), DQT luma and chroma (zigzag), SOF0, DHT DC0 AC0 DC1 AC1, DRI when restarts,
+// SOS; gray has one DQT, one component and DHT DC0 AC0.  dht: the optimised tables (4 x kDhtBytes), or nullptr for Annex K.
+int header_bytes(int H, int W, const Opts& o, const uint8_t* dht, uint8_t* out) {
+    const bool gray = o.shape == J::kGray;
+    const int nc = gray ? 1 : 3;
     uint8_t* p = out;
     auto seg = [&](uint8_t marker, int len) { *p++ = 0xFF; *p++ = marker; *p++ = (uint8_t)((len + 2) >> 8); *p++ = (uint8_t)(len + 2); };
     *p++ = 0xFF; *p++ = 0xD8;
     seg(0xE0, 14);
     const uint8_t app0[14] = {'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
     memcpy(p, app0, 14); p += 14;
-    for (int t = 0; t < 2; ++t) {
+    for (int t = 0; t < (gray ? 1 : 2); ++t) {
         int q[64];
-        quant_table(quality, t, q);
+        quant_table(t ? o.chroma_quality : o.quality, t, q);
         seg(0xDB, 65);
         *p++ = (uint8_t)t;
         for (int k = 0; k < 64; ++k) *p++ = (uint8_t)q[kZigzagHost[k]];
     }
-    seg(0xC0, 15);
-    const uint8_t sof[15] = {8, (uint8_t)(H >> 8), (uint8_t)H, (uint8_t)(W >> 8), (uint8_t)W, 3, 1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1};
-    memcpy(p, sof, 15); p += 15;
-    for (int t = 0; t < 4; ++t) {
+    seg(0xC0, 6 + 3 * nc);
+    const uint8_t ysf = o.shape == J::k420 ? 0x22 : o.shape == J::k422 ? 0x21 : 0x11;
+    const uint8_t sof[15] = {8, (uint8_t)(H >> 8), (uint8_t)H, (uint8_t)(W >> 8), (uint8_t)W, (uint8_t)nc, 1, ysf, 0, 2, 0x11, 1, 3, 0x11, 1};
+    memcpy(p, sof, 6 + 3 * nc); p += 6 + 3 * nc;
+    for (int t = 0; t < (gray ? 2 : 4); ++t) {
         const int chroma = t >> 1, ac = t & 1;
-        const uint8_t* counts = ac ? kAcCounts[chroma] : kDcCounts[chroma];
+        const uint8_t* counts = dht ? dht + t * J::kDhtBytes : ac ? kAcCounts[chroma] : kDcCounts[chroma];
+        const uint8_t* syms = dht ? counts + 16 : ac ? kAcSyms[chroma] : kDcSyms;
         int nsym = 0;
         for (int i = 0; i < 16; ++i) nsym += counts[i];
         seg(0xC4, 17 + nsym);
         *p++ = (uint8_t)(ac << 4 | chroma);
         memcpy(p, counts, 16); p += 16;
-        memcpy(p, ac ? kAcSyms[chroma] : kDcSyms, nsym); p += nsym;
+        memcpy(p, syms, nsym); p += nsym;
     }
-    seg(0xDA, 10);
-    const uint8_t sos[10] = {3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0};
-    memcpy(p, sos, 10); p += 10;
+    if (o.restart) {
+        seg(0xDD, 2);
+        *p++ = (uint8_t)(o.restart >> 8); *p++ = (uint8_t)o.restart;
+    }
+    seg(0xDA, 4 + 2 * nc);
+    const uint8_t sos[10] = {(uint8_t)nc, 1, 0x00, 2, 0x11, 3, 0x11};
+    memcpy(p, sos, 1 + 2 * nc); p += 1 + 2 * nc;
+    *p++ = 0; *p++ = 63; *p++ = 0;
     return (int)(p - out);
+}
+
+// libjpeg's jpeg_gen_optimal_table on the host, as jpeg_huff_build_kernel runs it on the device: bits = codes per length
+// 1..16, vals = the symbols by length then value.  Returns the number of symbols, or -1 for a code longer than 32 bits
+// (libjpeg refuses those).
+int gen_optimal_table(const int32_t* counts, uint8_t bits[16], uint8_t vals[256]) {
+    long long freq[257];
+    int codesize[257], others[257], nb[33] = {0};
+    for (int i = 0; i < 257; ++i) { freq[i] = i < 256 ? counts[i] : 1; codesize[i] = 0; others[i] = -1; }
+    for (;;) {
+        int c1 = -1, c2 = -1;
+        long long v = 1000000000LL;
+        for (int i = 0; i <= 256; ++i)
+            if (freq[i] && freq[i] <= v) { v = freq[i]; c1 = i; }
+        v = 1000000000LL;
+        for (int i = 0; i <= 256; ++i)
+            if (freq[i] && freq[i] <= v && i != c1) { v = freq[i]; c2 = i; }
+        if (c2 < 0) break;
+        freq[c1] += freq[c2];
+        freq[c2] = 0;
+        ++codesize[c1];
+        while (others[c1] >= 0) { c1 = others[c1]; ++codesize[c1]; }
+        others[c1] = c2;
+        ++codesize[c2];
+        while (others[c2] >= 0) { c2 = others[c2]; ++codesize[c2]; }
+    }
+    for (int i = 0; i <= 256; ++i)
+        if (codesize[i]) {
+            if (codesize[i] > 32) return -1;
+            ++nb[codesize[i]];
+        }
+    for (int i = 32; i > 16; --i)
+        while (nb[i] > 0) {
+            int j = i - 2;
+            while (nb[j] == 0) --j;
+            nb[i] -= 2; nb[i - 1] += 1; nb[j + 1] += 2; nb[j] -= 1;
+        }
+    int i = 16;
+    while (nb[i] == 0) --i;
+    nb[i] -= 1;
+    for (int l = 1; l <= 16; ++l) bits[l - 1] = (uint8_t)nb[l];
+    int p = 0;
+    for (int l = 1; l <= 32; ++l)
+        for (int j = 0; j < 256; ++j)
+            if (codesize[j] == l) vals[p++] = (uint8_t)j;
+    return p;
 }
 
 template <class T>
@@ -179,85 +249,139 @@ int scan(J::State* st, cudaStream_t s, const T* in, long long count, long long* 
     return 0;
 }
 
-int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int quality,
+// Runs f(J::Mcu<shape>{}) for the call's MCU shape.
+template <class F>
+void by_shape(int shape, F&& f) {
+    switch (shape) {
+    case J::k420: f(J::Mcu<J::k420>{}); break;
+    case J::k422: f(J::Mcu<J::k422>{}); break;
+    case J::k444: f(J::Mcu<J::k444>{}); break;
+    default: f(J::Mcu<J::kGray>{}); break;
+    }
+}
+
+int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const Opts& o,
            const uint8_t** data_out, int64_t* offsets_out) {
     JCK(cudaSetDevice(t.device));
     if (!*t.state)
         if (int rc = create(*t.state)) return rc;
     J::State* st = *t.state;
     const cudaStream_t s = t.stream;
+    int bpm = 0, mw = 0, mh = 0, strip = 0, tables = 0;
+    by_shape(o.shape, [&](auto m) {
+        using M = decltype(m);
+        bpm = M::blocks; mw = 8 * M::h; mh = 8 * M::v; strip = M::strip; tables = M::tables;
+    });
+    const int channels = o.shape == J::kGray ? 1 : 3;
 
     std::vector<J::Frame> fr(n);
-    long long ctas = 0, blocks = 0;
+    long long ctas = 0, blocks = 0, segs = 0;
     size_t in_bytes = 0;
     for (int i = 0; i < n; ++i) {
         J::Frame& f = fr[i];
         f.H = hw[2 * i]; f.W = hw[2 * i + 1];
-        f.mcux = (f.W + 15) / 16; f.mcuy = (f.H + 15) / 16;
-        f.strips = (f.mcux + J::kStripMcus - 1) / J::kStripMcus;
-        f.cta0 = ctas; f.blk0 = blocks;
+        f.mcux = (f.W + mw - 1) / mw; f.mcuy = (f.H + mh - 1) / mh;
+        f.strips = (f.mcux + strip - 1) / strip;
+        const int mcus = f.mcux * f.mcuy;
+        f.rst = o.restart ? std::min(o.restart, mcus) : mcus;
+        f.nseg = (mcus + f.rst - 1) / f.rst;
+        f.hdr = 0;
+        f.cta0 = ctas; f.blk0 = blocks; f.seg0 = segs;
         ctas += (long long)f.strips * f.mcuy;
-        blocks += 6LL * f.mcux * f.mcuy;
-        in_bytes += (size_t)f.H * f.W * 3;
+        blocks += (long long)bpm * mcus;
+        segs += f.nseg;
+        in_bytes += (size_t)f.H * f.W * channels;
         f.src = frames[i];
     }
     if (!frames_are_device) {
         if (int rc = grow(st->d_in, st->in_cap, in_bytes)) return rc;
-        size_t o = 0;
+        size_t off = 0;
         for (int i = 0; i < n; ++i) {
-            const size_t b = (size_t)fr[i].H * fr[i].W * 3;
-            JCK(cudaMemcpyAsync(st->d_in + o, frames[i], b, cudaMemcpyHostToDevice, s));
-            fr[i].src = st->d_in + o;
-            o += b;
+            const size_t b = (size_t)fr[i].H * fr[i].W * channels;
+            JCK(cudaMemcpyAsync(st->d_in + off, frames[i], b, cudaMemcpyHostToDevice, s));
+            fr[i].src = st->d_in + off;
+            off += b;
         }
     }
     J::Quant qt;
     for (int c = 0; c < 2; ++c) {
         int q[64];
-        quant_table(quality, c, q);
+        quant_table(c ? o.chroma_quality : o.quality, c, q);
         for (int k = 0; k < 64; ++k) qt.q8[c][k] = (uint16_t)(8 * q[k]);
     }
     if (int rc = grow(st->d_coef, st->coef_cap, (size_t)blocks * 64)) return rc;
     if (int rc = grow(st->d_bits, st->bits_cap, (size_t)blocks)) return rc;
     if (int rc = grow(st->d_excl, st->excl_cap, (size_t)blocks + 1)) return rc;
+    if (int rc = grow(st->d_segc, st->segc_cap, (size_t)segs)) return rc;
+    if (int rc = grow(st->d_segx, st->segx_cap, (size_t)segs + 1)) return rc;
     JCK(cudaMemcpyAsync(st->d_frames, fr.data(), n * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
 
-    // coefficients, bit lengths, bit offsets; the per-frame totals size the bitstream exactly
-    J::jpeg_transform_kernel<<<(unsigned)ctas, J::kTransformThreads, 0, s>>>(st->d_frames, n, qt, st->d_coef);
+    // coefficients; optimised tables from the frames' own symbols; bit lengths, bit offsets, chunks per segment
     const unsigned code_grid = (unsigned)((blocks + J::kCodeThreads - 1) / J::kCodeThreads);
-    J::jpeg_code_kernel<0><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, st->d_huff, st->d_bits, nullptr, nullptr);
+    const uint32_t* huff = st->d_huff;
+    int huff_stride = 0;
+    by_shape(o.shape, [&](auto m) {
+        J::jpeg_transform_kernel<decltype(m)::kShape><<<(unsigned)ctas, J::kTransformThreads, 0, s>>>(st->d_frames, n, qt, st->d_coef);
+    });
+    if (o.optimize) {
+        if (!st->d_hist) {
+            JCK(cudaMalloc(&st->d_hist, J::kMaxFrames * 1024 * sizeof(int)));
+            JCK(cudaMalloc(&st->d_ohuff, J::kMaxFrames * 1024 * sizeof(uint32_t)));
+            JCK(cudaMalloc(&st->d_dht, J::kMaxFrames * 4 * J::kDhtBytes));
+            JCK(cudaHostAlloc((void**)&st->h_dht, J::kMaxFrames * 4 * J::kDhtBytes, cudaHostAllocDefault));
+        }
+        JCK(cudaMemsetAsync(st->d_hist, 0, (size_t)n * 1024 * sizeof(int), s));
+        JCK(cudaMemsetAsync(st->d_dht, 0, (size_t)n * 4 * J::kDhtBytes, s));
+        by_shape(o.shape, [&](auto m) {
+            J::jpeg_code_kernel<2, decltype(m)::kShape><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, nullptr, 0, nullptr,
+                                                                                             nullptr, nullptr, nullptr, st->d_hist);
+        });
+        J::jpeg_huff_build_kernel<<<n * tables, 32, 0, s>>>(st->d_hist, tables, st->d_ohuff, st->d_dht);
+        huff = st->d_ohuff;
+        huff_stride = 1024;
+    }
+    by_shape(o.shape, [&](auto m) {
+        J::jpeg_code_kernel<0, decltype(m)::kShape><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, huff, huff_stride,
+                                                                                         st->d_bits, nullptr, nullptr, nullptr, nullptr);
+    });
     JCK(cudaGetLastError());
     if (int rc = scan(st, s, st->d_bits, blocks, st->d_excl)) return rc;
-    J::jpeg_frame_bits_kernel<<<1, J::kMaxFrames, 0, s>>>(st->d_frames, n, st->d_excl, st->d_small);
+    J::jpeg_seg_chunks_kernel<<<(unsigned)((segs + 255) / 256), 256, 0, s>>>(st->d_frames, n, segs, bpm, st->d_excl, st->d_segc);
     JCK(cudaGetLastError());
-    JCK(cudaMemcpyAsync(st->h_small, st->d_small, n * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    if (int rc = scan(st, s, st->d_segc, segs, st->d_segx)) return rc;
+    JCK(cudaMemcpyAsync(st->h_small, st->d_segx + segs, sizeof(long long), cudaMemcpyDeviceToHost, s));
+    if (o.optimize) JCK(cudaMemcpyAsync(st->h_dht, st->d_dht, (size_t)n * 4 * J::kDhtBytes, cudaMemcpyDeviceToHost, s));
     JCK(cudaStreamSynchronize(s));
-    long long raw = 0;
+    const long long chunks = st->h_small[0];
+    uint8_t hdr[kMaxHeaderBytes];
     for (int i = 0; i < n; ++i) {
-        fr[i].raw0 = raw;
-        fr[i].nbytes = (st->h_small[i] + 7) / 8;
-        raw += (fr[i].nbytes + J::kChunk - 1) / J::kChunk * J::kChunk;
+        const uint8_t* dht = o.optimize ? st->h_dht + (size_t)i * 4 * J::kDhtBytes : nullptr;
+        if (dht && dht[0] == 0xFF) return fail(WHENET_EINVAL, "frame %d: an optimised Huffman code is longer than 32 bits", i);
+        fr[i].hdr = header_bytes(fr[i].H, fr[i].W, o, dht, hdr);
     }
-    const long long chunks = raw / J::kChunk;
 
-    // the codes, then 0x00 after every 0xFF
-    if (int rc = grow(st->d_raw, st->raw_cap, (size_t)raw / 4)) return rc;
-    JCK(cudaMemsetAsync(st->d_raw, 0, (size_t)raw, s));
+    // the codes, then 0x00 after every 0xFF and RSTm between segments
+    if (int rc = grow(st->d_raw, st->raw_cap, (size_t)chunks * J::kChunk / 4)) return rc;
+    JCK(cudaMemsetAsync(st->d_raw, 0, (size_t)chunks * J::kChunk, s));
     JCK(cudaMemcpyAsync(st->d_frames, fr.data(), n * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
-    J::jpeg_code_kernel<1><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, st->d_huff, nullptr, st->d_excl, st->d_raw);
+    by_shape(o.shape, [&](auto m) {
+        J::jpeg_code_kernel<1, decltype(m)::kShape><<<code_grid, J::kCodeThreads, 0, s>>>(st->d_frames, n, blocks, st->d_coef, huff, huff_stride,
+                                                                                         nullptr, st->d_excl, st->d_segx, st->d_raw, nullptr);
+    });
     if (int rc = grow(st->d_ffc, st->ffc_cap, (size_t)chunks)) return rc;
     if (int rc = grow(st->d_ffx, st->ffx_cap, (size_t)chunks + 1)) return rc;
     const unsigned chunk_grid = (unsigned)((chunks + 255) / 256);
-    J::jpeg_ff_count_kernel<<<chunk_grid, 256, 0, s>>>(reinterpret_cast<const uint4*>(st->d_raw), chunks, st->d_ffc);
+    const uint4* raw4 = reinterpret_cast<const uint4*>(st->d_raw);
+    J::jpeg_out_count_kernel<<<chunk_grid, 256, 0, s>>>(st->d_frames, n, st->d_segx, segs, bpm, st->d_excl, raw4, chunks, st->d_ffc);
     JCK(cudaGetLastError());
     if (int rc = scan(st, s, st->d_ffc, chunks, st->d_ffx)) return rc;
-    J::jpeg_place_kernel<<<1, 32, 0, s>>>(st->d_frames, n, st->d_ffx, st->d_small);
+    J::jpeg_place_kernel<<<1, 32, 0, s>>>(st->d_frames, n, st->d_segx, st->d_ffx, st->d_small);
     JCK(cudaGetLastError());
     JCK(cudaMemcpyAsync(st->h_small, st->d_small, (n + 1) * sizeof(long long), cudaMemcpyDeviceToHost, s));
     JCK(cudaStreamSynchronize(s));
     const long long total = st->h_small[n];
     if (int rc = grow(st->d_out, st->out_cap, (size_t)total)) return rc;
-    J::jpeg_stuff_kernel<<<chunk_grid, 256, 0, s>>>(st->d_frames, n, reinterpret_cast<const uint4*>(st->d_raw), chunks, st->d_ffx, st->d_small,
+    J::jpeg_stuff_kernel<<<chunk_grid, 256, 0, s>>>(st->d_frames, n, st->d_segx, segs, bpm, st->d_excl, raw4, chunks, st->d_ffx, st->d_small,
                                                     st->d_out);
     JCK(cudaGetLastError());
     if (int rc = grow_host(st->h_out, st->h_cap, (size_t)total)) return rc;
@@ -267,7 +391,7 @@ int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, 
     // the host frames each stream: header before, EOI after
     for (int i = 0; i <= n; ++i) offsets_out[i] = st->h_small[i];
     for (int i = 0; i < n; ++i) {
-        header_bytes(fr[i].H, fr[i].W, quality, st->h_out + offsets_out[i]);
+        header_bytes(fr[i].H, fr[i].W, o, o.optimize ? st->h_dht + (size_t)i * 4 * J::kDhtBytes : nullptr, st->h_out + offsets_out[i]);
         st->h_out[offsets_out[i + 1] - 2] = 0xFF;
         st->h_out[offsets_out[i + 1] - 1] = 0xD9;
     }
@@ -275,8 +399,30 @@ int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, 
     return 0;
 }
 
-int encode_checked(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int quality,
-                   const uint8_t** data_out, int64_t* offsets_out) {
+// Checks the options of one call (channels 1 or 3) and fills o; WHENET_EINVAL otherwise.
+int check_options(int channels, const whenet_jpeg_options* opts, Opts& o) {
+    if (channels != 1 && channels != 3) return fail(WHENET_EINVAL, "channels %d is neither 1 nor 3", channels);
+    if (!opts) return fail(WHENET_EINVAL, "null options");
+    const whenet_jpeg_options& p = *opts;
+    if (p.quality < 1 || p.quality > 100) return fail(WHENET_EINVAL, "quality %d outside [1, 100]", p.quality);
+    if (p.chroma_quality < 1 || p.chroma_quality > 100) return fail(WHENET_EINVAL, "chroma_quality %d outside [1, 100]", p.chroma_quality);
+    if (p.sampling != 420 && p.sampling != 422 && p.sampling != 444) return fail(WHENET_EINVAL, "sampling %d is not 420, 422 or 444", p.sampling);
+    if (p.restart_interval < 0 || p.restart_interval > 65535) return fail(WHENET_EINVAL, "restart_interval %d outside [0, 65535]", p.restart_interval);
+    if (p.optimize != 0 && p.optimize != 1) return fail(WHENET_EINVAL, "optimize %d is neither 0 nor 1", p.optimize);
+    if (channels == 1 && (p.sampling != 420 || p.chroma_quality != p.quality))
+        return fail(WHENET_EINVAL, "one-channel frames take sampling 420 and chroma_quality = quality (a gray file has no chroma)");
+    if (p.chroma_quality != p.quality && p.sampling != 444)
+        return fail(WHENET_EINVAL, "chroma_quality %d != quality %d needs sampling 444 (libjpeg codes it as 4:4:4)", p.chroma_quality, p.quality);
+    o.quality = p.quality;
+    o.chroma_quality = p.chroma_quality;
+    o.shape = channels == 1 ? J::kGray : p.sampling == 420 ? J::k420 : p.sampling == 422 ? J::k422 : J::k444;
+    o.restart = p.restart_interval;
+    o.optimize = p.optimize;
+    return 0;
+}
+
+int encode_checked(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int channels, int frames_are_device,
+                   const whenet_jpeg_options* opts, const uint8_t** data_out, int64_t* offsets_out) {
     // the context is checked last so that every other argument can be validated without a GPU
     if (n < 1 || n > J::kMaxFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, J::kMaxFrames);
     for (int i = 0; i < n; ++i) {
@@ -284,11 +430,14 @@ int encode_checked(whenet_ctx* c, const uint8_t* const* frames, const int32_t* h
         if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
             return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
     }
-    if (quality < 1 || quality > 100) return fail(WHENET_EINVAL, "quality %d outside [1, 100]", quality);
+    Opts o;
+    if (int rc = check_options(channels, opts, o)) return rc;
     if (!data_out || !offsets_out) return fail(WHENET_EINVAL, "null data_out or offsets_out");
     if (!c) return fail(WHENET_EINVAL, "null context");
-    return encode(J::target(c), frames, hw, n, frames_are_device, quality, data_out, offsets_out);
+    return encode(J::target(c), frames, hw, n, frames_are_device, o, data_out, offsets_out);
 }
+
+whenet_jpeg_options default_options(int quality) { return whenet_jpeg_options{quality, quality, 420, 0, 0}; }
 
 }  // namespace
 
@@ -306,10 +455,12 @@ int dec_state(Target t, DecState**& slot) {
 void destroy(State* st) {
     if (!st) return;
     destroy_dec(st->dec);
-    for (void* p : {(void*)st->d_huff, (void*)st->d_frames, (void*)st->d_small, (void*)st->d_in, (void*)st->d_coef, (void*)st->d_bits,
-                    (void*)st->d_excl, (void*)st->d_tiles, (void*)st->d_raw, (void*)st->d_ffc, (void*)st->d_ffx, (void*)st->d_out})
+    for (void* p : {(void*)st->d_huff, (void*)st->d_ohuff, (void*)st->d_hist, (void*)st->d_dht, (void*)st->d_frames, (void*)st->d_small,
+                    (void*)st->d_in, (void*)st->d_coef, (void*)st->d_bits, (void*)st->d_excl, (void*)st->d_segc, (void*)st->d_segx,
+                    (void*)st->d_tiles, (void*)st->d_raw, (void*)st->d_ffc, (void*)st->d_ffx, (void*)st->d_out})
         if (p) cudaFree(p);
     if (st->h_small) cudaFreeHost(st->h_small);
+    if (st->h_dht) cudaFreeHost(st->h_dht);
     if (st->h_out) cudaFreeHost(st->h_out);
     delete st;
 }
@@ -330,20 +481,85 @@ int whenet_encode_jpeg_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, in
         ptrs[i] = frames + (size_t)i * H * W * 3;
         hw[2 * i] = H; hw[2 * i + 1] = W;
     }
-    return encode_checked(c, ptrs, hw, n, frames_are_device, quality, data_out, offsets_out);
+    const whenet_jpeg_options o = default_options(quality);
+    return encode_checked(c, ptrs, hw, n, 3, frames_are_device, &o, data_out, offsets_out);
 }
 
 int whenet_encode_jpeg_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int quality,
                                  const uint8_t** data_out, int64_t* offsets_out) {
     if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
-    return encode_checked(c, frames, hw, n, frames_are_device, quality, data_out, offsets_out);
+    const whenet_jpeg_options o = default_options(quality);
+    return encode_checked(c, frames, hw, n, 3, frames_are_device, &o, data_out, offsets_out);
+}
+
+int whenet_encode_jpeg_ex_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int channels, int frames_are_device,
+                             const whenet_jpeg_options* opts, const uint8_t** data_out, int64_t* offsets_out) {
+    if (!frames || !hw) return fail(WHENET_EINVAL, "null frames or hw");
+    return encode_checked(c, frames, hw, n, channels, frames_are_device, opts, data_out, offsets_out);
 }
 
 int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, int* len) {
     if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
     if (quality < 1 || quality > 100) return fail(WHENET_EINVAL, "quality %d outside [1, 100]", quality);
-    if (!out || !len || cap < J::kHeaderBytes) return fail(WHENET_EINVAL, "null out or len, or cap %d < %d", cap, J::kHeaderBytes);
-    *len = header_bytes(H, W, quality, out);
+    constexpr int kDefaultHeaderBytes = 623;
+    if (!out || !len || cap < kDefaultHeaderBytes) return fail(WHENET_EINVAL, "null out or len, or cap %d < %d", cap, kDefaultHeaderBytes);
+    *len = header_bytes(H, W, Opts{quality, quality, J::k420, 0, 0}, nullptr, out);
+    return 0;
+}
+
+int whenet_debug_jpeg_header_ex(int H, int W, int channels, const whenet_jpeg_options* opts, uint8_t* out, int cap, int* len) {
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "bad frame size %dx%d", W, H);
+    Opts o;
+    if (int rc = check_options(channels, opts, o)) return rc;
+    if (o.optimize) return fail(WHENET_EINVAL, "an optimised header depends on the frame's symbols");
+    uint8_t buf[kMaxHeaderBytes];
+    const int n = header_bytes(H, W, o, nullptr, buf);
+    if (!out || !len || cap < n) return fail(WHENET_EINVAL, "null out or len, or cap %d < %d", cap, n);
+    memcpy(out, buf, n);
+    *len = n;
+    return 0;
+}
+
+int whenet_debug_jpeg_optimal_table(const int32_t* counts, uint8_t* bits_out, uint8_t* vals_out, int* nvals_out) {
+    if (!counts || !bits_out || !vals_out || !nvals_out) return fail(WHENET_EINVAL, "null counts, bits_out, vals_out or nvals_out");
+    for (int i = 0; i < 256; ++i)
+        if (counts[i] < 0) return fail(WHENET_EINVAL, "counts[%d] = %d is negative", i, counts[i]);
+    const int nv = gen_optimal_table(counts, bits_out, vals_out);
+    if (nv < 0) return fail(WHENET_EINVAL, "a code would be longer than 32 bits");
+    *nvals_out = nv;
+    return 0;
+}
+
+int whenet_debug_jpeg_optimal_table_gpu(whenet_ctx* c, const int32_t* counts, uint8_t* bits_out, uint8_t* vals_out, int* nvals_out) {
+    if (!counts || !bits_out || !vals_out || !nvals_out) return fail(WHENET_EINVAL, "null counts, bits_out, vals_out or nvals_out");
+    for (int i = 0; i < 256; ++i)
+        if (counts[i] < 0) return fail(WHENET_EINVAL, "counts[%d] = %d is negative", i, counts[i]);
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    const J::Target t = J::target(c);
+    JCK(cudaSetDevice(t.device));
+    int* d_hist = nullptr;
+    uint32_t* d_huff = nullptr;
+    uint8_t* d_dht = nullptr;
+    uint8_t dht[J::kDhtBytes];
+    cudaError_t e = cudaMalloc(&d_hist, 1024 * sizeof(int));
+    if (e == cudaSuccess) e = cudaMalloc(&d_huff, 1024 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_dht, 4 * J::kDhtBytes);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_hist, counts, 256 * sizeof(int), cudaMemcpyHostToDevice, t.stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_dht, 0, J::kDhtBytes, t.stream);
+    if (e == cudaSuccess) {
+        J::jpeg_huff_build_kernel<<<1, 32, 0, t.stream>>>(d_hist, 1, d_huff, d_dht);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dht, d_dht, J::kDhtBytes, cudaMemcpyDeviceToHost, t.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(t.stream);
+    cudaFree(d_hist); cudaFree(d_huff); cudaFree(d_dht);
+    if (e != cudaSuccess) return fail(WHENET_ECUDA, "optimal table on the device: %s", cudaGetErrorString(e));
+    if (dht[0] == 0xFF) return fail(WHENET_EINVAL, "a code would be longer than 32 bits");
+    int nv = 0;
+    for (int i = 0; i < 16; ++i) nv += dht[i];
+    memcpy(bits_out, dht, 16);
+    memcpy(vals_out, dht + 16, nv);
+    *nvals_out = nv;
     return 0;
 }
 

@@ -1,13 +1,17 @@
-// kernels_jpeg.cuh - baseline JPEG encoding of packed BGR frames, byte-identical to cv2.imencode (libjpeg-turbo defaults: 4:2:0,
-// Annex K Huffman tables, islow FDCT, no restart markers).  DESIGN.md section 8.9; oracle/jpeg_oracle.py restates every step.
+// kernels_jpeg.cuh - baseline JPEG encoding of packed BGR or gray frames, byte-identical to cv2.imencode (libjpeg-turbo: islow
+// FDCT; 4:2:0, 4:2:2, 4:4:4 or gray; Annex K or optimised Huffman tables; restart intervals).  DESIGN.md sections 8.9 and 8.11;
+// oracle/jpeg_oracle.py restates every step.
 //
-// One call encodes up to 64 frames of their own sizes.  Every kernel reads the call's frame table and works on global indices
-// (transform CTAs, blocks, 16-byte chunks) that it maps back to a frame, so a frame's bytes never depend on the other frames.
-//   jpeg_transform_kernel   colour conversion, 4:2:0 downsampling, FDCT, quantisation, zigzag: int16 coefficients per block
-//   jpeg_code_kernel<0>     each block's Huffman bit length
-//   jpeg_scan_*             exclusive int64 scan (bit offsets of blocks; 0xFF counts of chunks)
-//   jpeg_code_kernel<1>     each block writes its codes at its bit offset (atomicOr into a zeroed buffer where words are shared)
-//   jpeg_ff_count_kernel / jpeg_stuff_kernel   0x00 after every 0xFF, each frame's stream at its place in the output
+// One call encodes up to 64 frames of their own sizes with one option set.  Every kernel reads the call's frame table and works
+// on global indices (transform CTAs, blocks, segments, 16-byte chunks) that it maps back to a frame, so a frame's bytes never
+// depend on the other frames.  A segment is one restart interval, or the whole frame without restarts.
+//   jpeg_transform_kernel<S>   colour conversion, downsampling of MCU shape S, FDCT, quantisation, zigzag: int16 per block
+//   jpeg_code_kernel<2, S>     optimised tables only: per-frame symbol histograms, then jpeg_huff_build_kernel builds the tables
+//   jpeg_code_kernel<0, S>     each block's Huffman bit length
+//   jpeg_scan_*                exclusive int64 scan (bit offsets of blocks; chunks of segments; output bytes of chunks)
+//   jpeg_seg_chunks_kernel     16-byte chunks of each segment's unstuffed stream (every segment starts on a chunk)
+//   jpeg_code_kernel<1, S>     each block writes its codes at its bit offset (atomicOr into a zeroed buffer where words are shared)
+//   jpeg_out_count_kernel / jpeg_stuff_kernel   0x00 after every 0xFF and RSTm between segments, each frame at its place
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -16,21 +20,33 @@ namespace whenet {
 namespace jpeg {
 
 constexpr int kMaxFrames = 64;
-constexpr int kStripMcus = 8;          // a transform CTA codes 8 MCUs (128 x 16 pixels) of one MCU row
-constexpr int kStripBlocks = 6 * kStripMcus;
+constexpr int kStripBlocks = 48;       // a transform CTA codes 48 blocks of one MCU row (8 MCUs at 4:2:0)
 constexpr int kTransformThreads = 256;
 constexpr int kCodeThreads = 128;
 constexpr int kScanThreads = 256, kScanItems = 8, kScanTile = kScanThreads * kScanItems;
-constexpr int kChunk = 16;             // bytes per stuffing thread; every frame's unstuffed stream starts on a chunk
-constexpr int kHeaderBytes = 623;      // SOI .. SOS of this encoder's files (the same for every size and quality)
+constexpr int kChunk = 16;             // bytes per stuffing thread; every segment's unstuffed stream starts on a chunk
+constexpr int kDhtBytes = 16 + 256;    // one optimised table as DHT carries it: counts per length 1..16, then the symbols
+
+// MCU shapes: luma sampling h x v, luma blocks row by row, then Cb and Cr; gray has one block of samples per MCU
+enum Shape { k420 = 0, k422 = 1, k444 = 2, kGray = 3 };
+template <int S>
+struct Mcu {
+    static constexpr int kShape = S;
+    static constexpr int h = S <= k422 ? 2 : 1, v = S == k420 ? 2 : 1;
+    static constexpr int luma = h * v, blocks = luma + (S == kGray ? 0 : 2);
+    static constexpr int strip = kStripBlocks / blocks;     // MCUs per transform CTA
+    static constexpr int tables = S == kGray ? 2 : 4;       // DC0 AC0 (DC1 AC1)
+};
 
 struct Frame {
-    const uint8_t* src;     // H x W x 3 BGR
+    const uint8_t* src;     // H x W x 3 BGR, or H x W gray
     int H, W, mcux, mcuy, strips;   // strips: transform CTAs per MCU row
+    int rst;                // MCUs per segment: the restart interval, or mcux * mcuy
+    int nseg;               // segments of the frame
+    int hdr;                // header bytes (SOI .. SOS) before the frame's entropy-coded data
     long long cta0;         // first transform CTA of the frame
     long long blk0;         // first block (scan order) of the frame in the call
-    long long raw0;         // first byte of its unstuffed stream (a multiple of kChunk)
-    long long nbytes;       // unstuffed bytes, last byte padded with 1s
+    long long seg0;         // first segment of the frame in the call
 };
 
 struct Quant {
@@ -97,61 +113,69 @@ __constant__ uint8_t kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 
 
 constexpr int kBlkStride = 72;   // 8 rows of 9 ints: row and column passes are both free of bank conflicts
 
-// One CTA per strip of kStripMcus MCUs of one MCU row.  Writes the strip's blocks (6 per MCU: Y00 Y01 Y10 Y11 Cb Cr) as zigzag
-// int16 at coef[(blk0 + 6 * mcu + b) * 64].  Luma replicates the last row and column to the block boundary; chroma replicates
-// the last column to the chroma block boundary and (odd H) the last row once, downsamples with bias 1, 2, 1, 2, ..., and then
-// replicates the last downsampled row.  Luma blocks past the image (dummy blocks) get AC 0 and the DC of the block before them.
+// One CTA per strip of Mcu<S>::strip MCUs of one MCU row.  Writes the strip's blocks as zigzag int16 at
+// coef[(blk0 + blocks * mcu + b) * 64].  Luma (and gray) replicates the last row and column to the block boundary.  Chroma
+// replicates the last column to h x its block boundary and the last row to a multiple of v, sums the h x v pixels with a bias
+// that alternates along a row (4:2:0: 1, 2; 4:2:2: 0, 1), shifts, and then replicates the last downsampled row.  A luma block
+// past the image (a dummy block, only where an MCU has two luma blocks along an axis) gets AC 0 and the DC of the block before
+// it in the MCU.  Quantisation takes qt.q8[0] for luma and qt.q8[1] for chroma.
+template <int S>
 __global__ void __launch_bounds__(kTransformThreads) jpeg_transform_kernel(const Frame* __restrict__ frames, int n, Quant qt,
                                                                            int16_t* __restrict__ coef) {
+    using M = Mcu<S>;
     __shared__ int ws[kStripBlocks * kBlkStride];
     const int f = find_frame<&Frame::cta0>(frames, n, blockIdx.x);
     const Frame fr = frames[f];
     const long long cta = blockIdx.x - fr.cta0;
-    const int my = (int)(cta / fr.strips), mx0 = (int)(cta % fr.strips) * kStripMcus;
-    const int nm = min(kStripMcus, fr.mcux - mx0);
-    const int H = fr.H, W = fr.W, ch = (H + 1) >> 1;
+    const int my = (int)(cta / fr.strips), mx0 = (int)(cta % fr.strips) * M::strip;
+    const int nm = min(M::strip, fr.mcux - mx0);
+    const int H = fr.H, W = fr.W, ch = (H + M::v - 1) / M::v;
     const uint8_t* __restrict__ src = fr.src;
 
-    // samples minus 128: 64 chroma cells per MCU, each with its 2 x 2 luma pixels
+    // samples minus 128: 64 chroma cells per MCU, each with its h x v luma pixels
     for (int i = threadIdx.x; i < nm * 64; i += kTransformThreads) {
         const int m = i >> 6, ly = (i >> 3) & 7, lx = i & 7;
         const int cy = my * 8 + ly, cx = (mx0 + m) * 8 + lx;
-        int* blk = ws + m * 6 * kBlkStride;
+        int* blk = ws + m * M::blocks * kBlkStride;
+        if (S == kGray) {
+            blk[ly * 9 + lx] = __ldg(src + (size_t)min(cy, H - 1) * W + min(cx, W - 1)) - 128;
+            continue;
+        }
         int sb = 0, sr = 0;
         const int yc = min(cy, ch - 1);
-        for (int dy = 0; dy < 2; ++dy)
-            for (int dx = 0; dx < 2; ++dx) {
-                const int x = min(2 * cx + dx, W - 1);
+        for (int dy = 0; dy < M::v; ++dy)
+            for (int dx = 0; dx < M::h; ++dx) {
+                const int x = min(M::h * cx + dx, W - 1);
                 int b, g, r;
-                load_bgr(src + ((size_t)min(2 * cy + dy, H - 1) * W + x) * 3, b, g, r);
-                const int yy = 2 * ly + dy, xx = 2 * lx + dx;
-                blk[((yy >> 3) * 2 + (xx >> 3)) * kBlkStride + (yy & 7) * 9 + (xx & 7)] = rgb_y(r, g, b) - 128;
-                load_bgr(src + ((size_t)min(2 * yc + dy, H - 1) * W + x) * 3, b, g, r);
+                load_bgr(src + ((size_t)min(M::v * cy + dy, H - 1) * W + x) * 3, b, g, r);
+                const int yy = M::v * ly + dy, xx = M::h * lx + dx;
+                blk[((yy >> 3) * M::h + (xx >> 3)) * kBlkStride + (yy & 7) * 9 + (xx & 7)] = rgb_y(r, g, b) - 128;
+                if (M::v == 2) load_bgr(src + ((size_t)min(2 * yc + dy, H - 1) * W + x) * 3, b, g, r);
                 sb += rgb_cb(r, g, b);
                 sr += rgb_cr(r, g, b);
             }
-        const int bias = 1 + (lx & 1);
-        blk[4 * kBlkStride + ly * 9 + lx] = ((sb + bias) >> 2) - 128;
-        blk[5 * kBlkStride + ly * 9 + lx] = ((sr + bias) >> 2) - 128;
+        const int bias = S == k420 ? 1 + (lx & 1) : S == k422 ? lx & 1 : 0, shift = S == k420 ? 2 : S == k422 ? 1 : 0;
+        blk[M::luma * kBlkStride + ly * 9 + lx] = ((sb + bias) >> shift) - 128;
+        blk[(M::luma + 1) * kBlkStride + ly * 9 + lx] = ((sr + bias) >> shift) - 128;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < nm * 48; i += kTransformThreads) fdct_pass<true>(ws + (i >> 3) * kBlkStride + (i & 7) * 9, 1);
+    for (int i = threadIdx.x; i < nm * M::blocks * 8; i += kTransformThreads) fdct_pass<true>(ws + (i >> 3) * kBlkStride + (i & 7) * 9, 1);
     __syncthreads();
-    for (int i = threadIdx.x; i < nm * 48; i += kTransformThreads) fdct_pass<false>(ws + (i >> 3) * kBlkStride + (i & 7), 9);
+    for (int i = threadIdx.x; i < nm * M::blocks * 8; i += kTransformThreads) fdct_pass<false>(ws + (i >> 3) * kBlkStride + (i & 7), 9);
     __syncthreads();
 
     const int bx = (W + 7) >> 3, by = (H + 7) >> 3;
-    int16_t* __restrict__ out = coef + (fr.blk0 + 6LL * ((long long)my * fr.mcux + mx0)) * 64;
-    for (int i = threadIdx.x; i < nm * 6 * 64; i += kTransformThreads) {
-        const int k = i & 63, blkn = i >> 6, m = blkn / 6, b = blkn - 6 * m;
-        const int comp = b < 4 ? 0 : 1;
+    int16_t* __restrict__ out = coef + (fr.blk0 + (long long)M::blocks * ((long long)my * fr.mcux + mx0)) * 64;
+    for (int i = threadIdx.x; i < nm * M::blocks * 64; i += kTransformThreads) {
+        const int k = i & 63, blkn = i >> 6, m = blkn / M::blocks, b = blkn - M::blocks * m;
+        const int comp = b < M::luma ? 0 : 1;
         int src_b = b;      // a dummy luma block takes the DC of the last real block before it in the MCU
-        if (b < 4) {
-            auto dummy = [&](int bb) { return 2 * (mx0 + m) + (bb & 1) >= bx || 2 * my + (bb >> 1) >= by; };
+        if (M::luma > 1 && b < M::luma) {
+            auto dummy = [&](int bb) { return M::h * (mx0 + m) + bb % M::h >= bx || M::v * my + bb / M::h >= by; };
             while (src_b > 0 && dummy(src_b)) --src_b;
         }
         int v;
-        if (src_b != b) v = k == 0 ? quantise(ws[(m * 6 + src_b) * kBlkStride], qt.q8[0][0]) : 0;
+        if (src_b != b) v = k == 0 ? quantise(ws[(m * M::blocks + src_b) * kBlkStride], qt.q8[0][0]) : 0;
         else {
             const int nat = kZigzag[k];
             v = quantise(ws[blkn * kBlkStride + (nat >> 3) * 9 + (nat & 7)], qt.q8[comp][nat]);
@@ -162,7 +186,7 @@ __global__ void __launch_bounds__(kTransformThreads) jpeg_transform_kernel(const
 
 // Huffman table: huff[t * 256 + symbol] = length << 16 | code, t = 0 DC luma, 1 AC luma, 2 DC chroma, 3 AC chroma
 struct BitSink {
-    uint32_t* words;     // the frame's stream as little-endian words of big-endian bit order (bswap on store)
+    uint32_t* words;     // the segment's stream as little-endian words of big-endian bit order (bswap on store)
     long long w;         // word being filled
     unsigned long long acc;
     int nacc;            // bits in acc; the first word starts with (bit offset & 31) bits owned by the blocks before
@@ -185,22 +209,48 @@ struct BitSink {
 
 __device__ __forceinline__ int bit_length(int a) { return a ? 32 - __clz(a) : 0; }
 
-// One thread per block of the call.  kEmit = 0: bits[g] = the block's coded length.  kEmit = 1: the block's codes at bit
-// offset excl[g] - excl[blk0] of its frame's stream, and the frame's last block pads the final byte with 1s.
-template <int kEmit>
+// The bit total of segment k of a frame: its blocks' lengths from the exclusive scan excl.
+__device__ __forceinline__ long long seg_bits(const Frame& fr, int k, int bpm, const long long* __restrict__ excl) {
+    const long long b0 = fr.blk0 + (long long)k * fr.rst * bpm;
+    const long long b1 = fr.blk0 + (long long)min((k + 1) * fr.rst, fr.mcux * fr.mcuy) * bpm;
+    return excl[b1] - excl[b0];
+}
+
+// One thread per block of the call.  The DC prediction is the previous block of the same component in the block's segment.
+//   kMode 0: bits[g] = the block's coded length.
+//   kMode 1: the block's codes at bit offset excl[g] - excl[first block of its segment] of the segment's stream, which starts
+//            at chunk seg_cx[segment]; the segment's last block pads the final byte with 1s.
+//   kMode 2: the block's symbols counted into hist[frame * 1024 + table * 256 + symbol], through a CTA histogram for the
+//            frame of the CTA's first block (EOB alone would contend on one global counter per frame).
+// huff_stride: 0 = one table set for the call (Annex K), 1024 = one per frame (optimised).
+template <int kMode, int S>
 __global__ void __launch_bounds__(kCodeThreads) jpeg_code_kernel(const Frame* __restrict__ frames, int n, long long nblocks,
                                                                  const int16_t* __restrict__ coef, const uint32_t* __restrict__ huff,
-                                                                 int* __restrict__ bits, const long long* __restrict__ excl,
-                                                                 uint32_t* __restrict__ raw) {
-    const long long g = (long long)blockIdx.x * kCodeThreads + threadIdx.x;
-    if (g >= nblocks) return;
+                                                                 int huff_stride, int* __restrict__ bits, const long long* __restrict__ excl,
+                                                                 const long long* __restrict__ seg_cx, uint32_t* __restrict__ raw,
+                                                                 int* __restrict__ hist) {
+    using M = Mcu<S>;
+    __shared__ int sh[kMode == 2 ? 4 * 256 : 1];
+    const long long g0 = (long long)blockIdx.x * kCodeThreads;
+    long long g = g0 + threadIdx.x;
+    const bool live = g < nblocks;
+    int f0 = 0;
+    if (kMode == 2) {
+        for (int i = threadIdx.x; i < 4 * 256; i += kCodeThreads) sh[i] = 0;
+        f0 = find_frame<&Frame::blk0>(frames, n, g0);
+        __syncthreads();
+        if (!live) g = nblocks - 1;         // walks a real block but counts nothing
+    } else if (!live) {
+        return;
+    }
     const int f = find_frame<&Frame::blk0>(frames, n, g);
     const Frame& fr = frames[f];
-    const long long l = g - fr.blk0, mcu = l / 6;
-    const int b = (int)(l - 6 * mcu), comp = b < 4 ? 0 : 1;
-    long long prev = -1;                       // previous block of the same component in scan order
-    if (b >= 1 && b <= 3) prev = g - 1;
-    else if (mcu > 0) prev = b == 0 ? g - 3 : g - 6;
+    const int l = (int)(g - fr.blk0), mcu = l / M::blocks;
+    const int b = l - M::blocks * mcu, comp = b < M::luma ? 0 : 1;
+    const int seg = mcu / fr.rst;
+    long long prev = -1;                       // previous block of the same component in the segment
+    if (b >= 1 && b < M::luma) prev = g - 1;
+    else if (mcu != seg * fr.rst) prev = b == 0 ? g - M::blocks + M::luma - 1 : g - M::blocks;
     // a mask of the nonzero coefficients; the values themselves are read again (from L1) only where the mask has a bit
     const int16_t* __restrict__ c = coef + g * 64;
     unsigned long long nz = 0;
@@ -213,27 +263,36 @@ __global__ void __launch_bounds__(kCodeThreads) jpeg_code_kernel(const Frame* __
             nz |= (unsigned long long)((w[j] & 0xffffu) != 0) << (8 * i + 2 * j) | (unsigned long long)((w[j] >> 16) != 0) << (8 * i + 2 * j + 1);
     }
     const int pred = prev >= 0 ? coef[prev * 64] : 0;
-    const uint32_t* __restrict__ dc_t = huff + comp * 512;
+    const int t_dc = comp * 2;
+    const uint32_t* __restrict__ dc_t = huff + (long long)f * huff_stride + t_dc * 256;
     const uint32_t* __restrict__ ac_t = dc_t + 256;
+    int* __restrict__ h_dc = (f == f0 ? sh : hist + (long long)f * 1024) + t_dc * 256;
+    int* __restrict__ h_ac = h_dc + 256;
 
     BitSink s{};
     long long total = 0;
-    if (kEmit) {
-        const long long off = excl[g] - excl[fr.blk0];
-        s.words = raw + (fr.raw0 >> 2);
+    const long long gs = fr.blk0 + (long long)seg * fr.rst * M::blocks;    // the segment's first block
+    if (kMode == 1) {
+        const long long off = excl[g] - excl[gs];
+        s.words = raw + seg_cx[fr.seg0 + seg] * (kChunk / 4);
         s.w = off >> 5;
         s.nacc = (int)(off & 31);
         s.first = true;
     }
-    auto put = [&](uint32_t hc, int extra, int nb) {      // a Huffman code then nb extra bits
+    auto put = [&](const uint32_t* __restrict__ t, int* __restrict__ h, int sym, int extra, int nb) {    // a code then nb extra bits
+        if (kMode == 2) {
+            if (live) atomicAdd(h + sym, 1);
+            return;
+        }
+        const uint32_t hc = __ldg(t + sym);
         const int len = (int)(hc >> 16);
-        if (kEmit) s.put(((hc & 0xffff) << nb) | (uint32_t)(extra & ((1 << nb) - 1)), len + nb);
+        if (kMode == 1) s.put(((hc & 0xffff) << nb) | (uint32_t)(extra & ((1 << nb) - 1)), len + nb);
         else total += len + nb;
     };
     {
         const int diff = __ldg(c) - pred;
         const int nb = bit_length(diff < 0 ? -diff : diff);
-        put(__ldg(dc_t + nb), diff < 0 ? diff - 1 : diff, nb);
+        put(dc_t, h_dc, nb, diff < 0 ? diff - 1 : diff, nb);
     }
     nz &= ~1ull;
     int last = 0;
@@ -241,19 +300,142 @@ __global__ void __launch_bounds__(kCodeThreads) jpeg_code_kernel(const Frame* __
         const int k = __ffsll((long long)nz) - 1;
         nz &= nz - 1;
         int run = k - last - 1;
-        for (; run > 15; run -= 16) put(__ldg(ac_t + 0xF0), 0, 0);
+        for (; run > 15; run -= 16) put(ac_t, h_ac, 0xF0, 0, 0);
         const int v = __ldg(c + k);
         const int nb = bit_length(v < 0 ? -v : v);
-        put(__ldg(ac_t + (run << 4 | nb)), v < 0 ? v - 1 : v, nb);
+        put(ac_t, h_ac, run << 4 | nb, v < 0 ? v - 1 : v, nb);
         last = k;
     }
-    if (last < 63) put(__ldg(ac_t), 0, 0);
-    if (!kEmit) { bits[g] = (int)total; return; }
-    if (l == 6LL * fr.mcux * fr.mcuy - 1) {
-        const int pad = (int)((8 - ((excl[g + 1] - excl[fr.blk0]) & 7)) & 7);
+    if (last < 63) put(ac_t, h_ac, 0, 0, 0);
+    if (kMode == 0) { bits[g] = (int)total; return; }
+    if (kMode == 2) {
+        __syncthreads();
+        int* __restrict__ hf = hist + (long long)f0 * 1024;
+        for (int i = threadIdx.x; i < M::tables * 256; i += kCodeThreads)
+            if (sh[i]) atomicAdd(hf + i, sh[i]);
+        return;
+    }
+    if (g == fr.blk0 + (long long)min((seg + 1) * fr.rst, fr.mcux * fr.mcuy) * M::blocks - 1) {
+        const int pad = (int)((8 - ((excl[g + 1] - excl[gs]) & 7)) & 7);
         if (pad) s.put((1u << pad) - 1, pad);
     }
     s.flush();
+}
+
+// ---- optimised Huffman tables: libjpeg's jpeg_gen_optimal_table, one warp per (frame, table)
+constexpr int kSymsPerLane = 9;        // 32 x 9 >= 257 symbols: 0..255 and the reserved 256
+
+// The warp's smallest (count << 9 | 511 - symbol) over live symbols other than `skip`: the smallest count, ties to the
+// largest symbol, as libjpeg's "<=" scan picks.  ~0 when there is none.
+__device__ __forceinline__ unsigned long long warp_min_sym(const long long (&freq)[kSymsPerLane], int lane, int skip) {
+    unsigned long long key = ~0ull;
+#pragma unroll
+    for (int k = 0; k < kSymsPerLane; ++k) {
+        const int j = lane * kSymsPerLane + k;
+        if (freq[k] && j != skip) key = min(key, (unsigned long long)freq[k] << 9 | (unsigned)(511 - j));
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) key = min(key, __shfl_xor_sync(0xffffffffu, key, o));
+    return key;
+}
+
+// hist: nfreq[f * 1024 + t * 256 + symbol] counts; one 32-thread CTA per (frame f, table t < tables).  Writes the code table
+// huff[f * 1024 + t * 256 + symbol] (0 for unused symbols) and dht[(f * 4 + t) * kDhtBytes]: counts per length 1..16, then the
+// symbols by length, then value.
+__global__ void __launch_bounds__(32) jpeg_huff_build_kernel(const int* __restrict__ hist, int tables, uint32_t* __restrict__ huff,
+                                                             uint8_t* __restrict__ dht) {
+    __shared__ int nbits[33];
+    __shared__ uint8_t vals[256];
+    const int f = blockIdx.x / tables, t = blockIdx.x - f * tables, lane = threadIdx.x;
+    const int* __restrict__ h = hist + f * 1024 + t * 256;
+    long long freq[kSymsPerLane];
+    int size[kSymsPerLane], group[kSymsPerLane];
+#pragma unroll
+    for (int k = 0; k < kSymsPerLane; ++k) {
+        const int j = lane * kSymsPerLane + k;
+        freq[k] = j < 256 ? h[j] : j == 256;
+        size[k] = 0;
+        group[k] = j;         // the live symbol whose count holds this one's
+    }
+    for (;;) {
+        const unsigned long long k1 = warp_min_sym(freq, lane, -1);
+        const int c1 = 511 - (int)(k1 & 511);
+        const unsigned long long k2 = warp_min_sym(freq, lane, c1);
+        if (k2 == ~0ull) break;
+        const int c2 = 511 - (int)(k2 & 511);
+#pragma unroll
+        for (int k = 0; k < kSymsPerLane; ++k) {
+            const int j = lane * kSymsPerLane + k;
+            if (j == c1) freq[k] += (long long)(k2 >> 9);
+            if (j == c2) freq[k] = 0;
+            if (group[k] == c1 || group[k] == c2) { ++size[k]; group[k] = c1; }
+        }
+    }
+    // codes per length, then libjpeg's adjustment of lengths past 16 and the removal of the reserved code.  libjpeg refuses
+    // a length past 32 (counts that grow like Fibonacci numbers past ~2^22 per table); dht's first byte 0xFF reports it.
+    int over = 0;
+#pragma unroll
+    for (int k = 0; k < kSymsPerLane; ++k) over += size[k] > 32;
+    if (__reduce_add_sync(0xffffffffu, over)) {
+        if (lane == 0) dht[(f * 4 + t) * kDhtBytes] = 0xFF;
+        return;
+    }
+    if (lane == 0) nbits[0] = 0;
+    for (int len = 1; len <= 32; ++len) {
+        int cnt = 0;
+#pragma unroll
+        for (int k = 0; k < kSymsPerLane; ++k) cnt += size[k] == len;
+        cnt = __reduce_add_sync(0xffffffffu, cnt);
+        if (lane == 0) nbits[len] = cnt;
+    }
+    // symbols 0..255 by length, then value: the symbols of a lane are consecutive, so lanes take places in order
+    int base = 0;
+    for (int len = 1; len <= 32; ++len) {
+        int cnt = 0;
+#pragma unroll
+        for (int k = 0; k < kSymsPerLane; ++k) cnt += size[k] == len && lane * kSymsPerLane + k < 256;
+        int incl = cnt;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        int p = base + incl - cnt;
+#pragma unroll
+        for (int k = 0; k < kSymsPerLane; ++k) {
+            const int j = lane * kSymsPerLane + k;
+            if (size[k] == len && j < 256) vals[p++] = (uint8_t)j;
+        }
+        base += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    uint32_t* __restrict__ table = huff + f * 1024 + t * 256;
+    for (int j = lane; j < 256; j += 32) table[j] = 0;
+    __syncwarp();
+    if (lane == 0) {
+        for (int i = 32; i > 16; --i)
+            while (nbits[i] > 0) {
+                int j = i - 2;
+                while (nbits[j] == 0) --j;
+                nbits[i] -= 2;
+                nbits[i - 1] += 1;
+                nbits[j + 1] += 2;
+                nbits[j] -= 1;
+            }
+        int i = 16;
+        while (nbits[i] == 0) --i;
+        nbits[i] -= 1;
+        uint8_t* __restrict__ d = dht + (f * 4 + t) * kDhtBytes;
+        uint32_t code = 0;
+        int p = 0;
+        for (int len = 1; len <= 16; ++len) {
+            d[len - 1] = (uint8_t)nbits[len];
+            for (int q = 0; q < nbits[len]; ++q, ++p) {
+                table[vals[p]] = (uint32_t)len << 16 | code++;
+                d[16 + p] = vals[p];
+            }
+            code <<= 1;
+        }
+    }
 }
 
 // ---- exclusive scan of int32 or int64 values into int64 (out[count] = total): tile sums, one CTA over the sums, tile re-scan
@@ -327,59 +509,93 @@ __global__ void __launch_bounds__(kScanThreads) jpeg_scan_apply_kernel(const T* 
     }
 }
 
-// ---- per-frame totals and output placement (one thread per frame)
-__global__ void jpeg_frame_bits_kernel(const Frame* __restrict__ frames, int n, const long long* __restrict__ excl, long long* __restrict__ fbits) {
-    const int f = threadIdx.x;
-    if (f >= n) return;
-    const Frame& fr = frames[f];
-    fbits[f] = excl[fr.blk0 + 6LL * fr.mcux * fr.mcuy] - excl[fr.blk0];
+// ---- segments, output placement and stuffing
+// chunks[s] = 16-byte chunks of segment s's unstuffed stream (at least one: a segment has a block, a block a DC code)
+__global__ void __launch_bounds__(256) jpeg_seg_chunks_kernel(const Frame* __restrict__ frames, int n, long long nseg, int bpm,
+                                                              const long long* __restrict__ excl, int* __restrict__ chunks) {
+    const long long s = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (s >= nseg) return;
+    const int f = find_frame<&Frame::seg0>(frames, n, s);
+    const long long bytes = (seg_bits(frames[f], (int)(s - frames[f].seg0), bpm, excl) + 7) >> 3;
+    chunks[s] = (int)((bytes + kChunk - 1) / kChunk);
 }
 
-// offsets[f] = where frame f's file starts in the output: header, stuffed stream, EOI; offsets[n] = the total
-__global__ void jpeg_place_kernel(const Frame* __restrict__ frames, int n, const long long* __restrict__ ffx, long long* __restrict__ offsets) {
-    if (threadIdx.x != 0) return;
-    long long o = 0;
-    for (int f = 0; f < n; ++f) {
-        const Frame& fr = frames[f];
-        offsets[f] = o;
-        const long long c0 = fr.raw0 / kChunk, c1 = (fr.raw0 + fr.nbytes + kChunk - 1) / kChunk;
-        o += kHeaderBytes + fr.nbytes + (ffx[c1] - ffx[c0]) + 2;
+// The segment whose chunks [seg_cx[s], seg_cx[s + 1]) hold chunk i.
+__device__ __forceinline__ long long find_seg(const long long* __restrict__ seg_cx, long long nseg, long long i) {
+    long long lo = 0, hi = nseg - 1;
+    while (lo < hi) {
+        const long long mid = (lo + hi + 1) >> 1;
+        if (seg_cx[mid] <= i) lo = mid; else hi = mid - 1;
     }
-    offsets[n] = o;
+    return lo;
 }
 
-__global__ void __launch_bounds__(256) jpeg_ff_count_kernel(const uint4* __restrict__ raw, long long nchunks, int* __restrict__ count) {
+// Where chunk i is in its segment: frame f, segment k of the frame, byte pos in the segment, m stream bytes in the chunk, and
+// whether an RSTm follows it (the last chunk of a segment other than the frame's last).
+struct ChunkPlace {
+    int f, k, m;
+    bool rst;
+};
+__device__ __forceinline__ ChunkPlace place_chunk(const Frame* __restrict__ frames, int n, const long long* __restrict__ seg_cx, long long nseg,
+                                                  int bpm, const long long* __restrict__ excl, long long i) {
+    const long long s = find_seg(seg_cx, nseg, i);
+    ChunkPlace p;
+    p.f = find_frame<&Frame::seg0>(frames, n, s);
+    const Frame& fr = frames[p.f];
+    p.k = (int)(s - fr.seg0);
+    const long long pos = (i - seg_cx[s]) * kChunk, nbytes = (seg_bits(fr, p.k, bpm, excl) + 7) >> 3;
+    p.m = (int)min((long long)kChunk, nbytes - pos);
+    p.rst = pos + kChunk >= nbytes && p.k + 1 < fr.nseg;
+    return p;
+}
+
+// count[i] = output bytes of chunk i: its stream bytes, a 0x00 after each 0xFF, and 2 for an RSTm after it
+__global__ void __launch_bounds__(256) jpeg_out_count_kernel(const Frame* __restrict__ frames, int n, const long long* __restrict__ seg_cx,
+                                                             long long nseg, int bpm, const long long* __restrict__ excl,
+                                                             const uint4* __restrict__ raw, long long nchunks, int* __restrict__ count) {
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
     if (i >= nchunks) return;
+    const ChunkPlace p = place_chunk(frames, n, seg_cx, nseg, bpm, excl, i);
     const uint4 v = __ldg(raw + i);
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    int c = 0;
+    int c = p.m + (p.rst ? 2 : 0);      // bytes past the stream inside the chunk are zero, so they never count as 0xFF
 #pragma unroll
     for (int j = 0; j < 16; ++j) c += ((w[j >> 2] >> (8 * (j & 3))) & 0xff) == 0xff;
     count[i] = c;
 }
 
-// bytes past a frame's stream inside its last chunk are zero, so they never count as 0xFF
-__global__ void __launch_bounds__(256) jpeg_stuff_kernel(const Frame* __restrict__ frames, int n, const uint4* __restrict__ raw, long long nchunks,
-                                                        const long long* __restrict__ ffx, const long long* __restrict__ offsets,
-                                                        uint8_t* __restrict__ out) {
+// offsets[f] = where frame f's file starts in the output: header, stuffed stream with its RSTm, EOI; offsets[n] = the total
+__global__ void jpeg_place_kernel(const Frame* __restrict__ frames, int n, const long long* __restrict__ seg_cx,
+                                  const long long* __restrict__ outx, long long* __restrict__ offsets) {
+    if (threadIdx.x != 0) return;
+    long long o = 0;
+    for (int f = 0; f < n; ++f) {
+        const Frame& fr = frames[f];
+        offsets[f] = o;
+        o += fr.hdr + (outx[seg_cx[fr.seg0 + fr.nseg]] - outx[seg_cx[fr.seg0]]) + 2;
+    }
+    offsets[n] = o;
+}
+
+__global__ void __launch_bounds__(256) jpeg_stuff_kernel(const Frame* __restrict__ frames, int n, const long long* __restrict__ seg_cx,
+                                                        long long nseg, int bpm, const long long* __restrict__ excl,
+                                                        const uint4* __restrict__ raw, long long nchunks, const long long* __restrict__ outx,
+                                                        const long long* __restrict__ offsets, uint8_t* __restrict__ out) {
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
     if (i >= nchunks) return;
-    const int f = find_frame<&Frame::raw0>(frames, n, i * kChunk);
-    const Frame& fr = frames[f];
-    const long long pos = i * kChunk - fr.raw0;
-    if (pos >= fr.nbytes) return;
-    uint8_t* dst = out + offsets[f] + kHeaderBytes + pos + (ffx[i] - ffx[fr.raw0 / kChunk]);
+    const ChunkPlace p = place_chunk(frames, n, seg_cx, nseg, bpm, excl, i);
+    const Frame& fr = frames[p.f];
+    uint8_t* dst = out + offsets[p.f] + fr.hdr + (outx[i] - outx[seg_cx[fr.seg0]]);
     const uint4 v = __ldg(raw + i);
-    const int m = (int)min((long long)kChunk, fr.nbytes - pos);
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int j = 0; j < kChunk; ++j) {
-        if (j >= m) return;
+        if (j >= p.m) break;
         const uint8_t byte = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
         *dst++ = byte;
         if (byte == 0xff) *dst++ = 0;
     }
+    if (p.rst) { dst[0] = 0xFF; dst[1] = (uint8_t)(0xD0 + (p.k & 7)); }
 }
 
 }  // namespace jpeg

@@ -1,8 +1,9 @@
-"""Video on the GPU path: JPEG encoding and decoding of device BGR frames, and Motion-JPEG AVI files (DESIGN.md sections 8.9
-and 8.10).
+"""Video on the GPU path: JPEG encoding and decoding of device BGR frames, and Motion-JPEG AVI files (DESIGN.md sections 8.9,
+8.10 and 8.11).
 
-  ``encode_jpeg``   device (or host) BGR frames -> JPEG files, byte-identical to cv2.imencode(".jpg", frame,
-                    [cv2.IMWRITE_JPEG_QUALITY, quality]), encoded by the library's CUDA kernels (``whenet_encode_jpeg_u8``)
+  ``encode_jpeg``   device (or host) BGR or gray frames -> JPEG files, byte-identical to cv2.imencode(".jpg", frame,
+                    params) with the quality, sampling, restart, optimise and chroma-quality parameters, encoded by the
+                    library's CUDA kernels (``whenet_encode_jpeg_u8``, ``whenet_encode_jpeg_ex_u8``)
   ``decode_jpeg``   JPEG files -> device BGR frames, pixel-identical to cv2.imdecode(buf, cv2.IMREAD_COLOR), decoded by the
                     library's CUDA kernels (``whenet_decode_jpeg_u8``)
   ``MJPGWriter``    writes those files as an MJPG AVI: what reference demo_video.py:46-47,60 writes through
@@ -29,8 +30,12 @@ MAX_FRAMES_PER_CALL = 64
 MAX_SIDE = 16384
 
 
+SAMPLINGS = {"420": 420, "422": 422, "444": 444}
+
+
 def _frame_list(whenet, frames):
-    """(on device?, items, (H, W) per frame) of BGR frames, or ValueError before anything runs."""
+    """(on device?, items, (H, W) per frame, channels) of BGR frames or one-channel (gray) frames, or ValueError before anything
+    runs."""
     from .whenet import _is_device
     if isinstance(frames, (list, tuple)):
         items, ndim = list(frames), 3
@@ -51,39 +56,76 @@ def _frame_list(whenet, frames):
                 raise ValueError("frames must be CUDA tensors or numpy arrays, not %s" % type(f).__name__)
             if f.dtype != np.uint8 or not f.flags.c_contiguous:
                 raise ValueError("frames must be C-contiguous uint8 arrays")
-        if len(f.shape) != ndim or f.shape[-1] != 3:
-            raise ValueError("frames must be BGR (n, H, W, 3) or a list of (H, W, 3), not %s" % (tuple(f.shape),))
+        if len(f.shape) != ndim or f.shape[-1] not in (1, 3):
+            raise ValueError("frames must be BGR (n, H, W, 3) or gray (n, H, W, 1), or a list of (H, W, 3) or (H, W, 1), not %s"
+                             % (tuple(f.shape),))
         H, W = int(f.shape[-3]), int(f.shape[-2])
         if not (1 <= H <= MAX_SIDE and 1 <= W <= MAX_SIDE):
             raise ValueError("frame size %dx%d: each side must be in [1, %d]" % (W, H, MAX_SIDE))
+    channels = {int(f.shape[-1]) for f in items}
+    if len(channels) > 1:
+        raise ValueError("frames mix 1 and 3 channels")
     if ndim == 4:
         n = int(frames.shape[0])
         frames_hw = [(int(frames.shape[1]), int(frames.shape[2]))] * n
     else:
         frames_hw = [(int(f.shape[0]), int(f.shape[1])) for f in items]
-    return dev, items, frames_hw
+    return dev, items, frames_hw, channels.pop() if channels else 3
 
 
-def encode_jpeg(whenet, frames, quality: int = 95) -> list:
-    """JPEG files of BGR ``frames``, each byte-identical to ``cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY,
-    quality])[1].tobytes()`` (baseline, 4:2:0, the standard Huffman tables), encoded on ``whenet``'s GPU and stream.
+def _is_int(x, lo, hi):
+    return not isinstance(x, (bool, np.bool_)) and isinstance(x, (int, np.integer)) and lo <= x <= hi
+
+
+def encode_jpeg(whenet, frames, quality: int = 95, *, sampling: str = "420", restart_interval: int = 0, optimize: bool = False,
+                chroma_quality=None) -> list:
+    """JPEG files of BGR or gray ``frames``, each byte-identical to ``cv2.imencode(".jpg", frame, params)[1].tobytes()``
+    (baseline), encoded on ``whenet``'s GPU and stream.  ``params`` are:
+
+      - ``[IMWRITE_JPEG_QUALITY, quality]``, or, when ``chroma_quality`` is given and differs from ``quality``,
+        ``[IMWRITE_JPEG_LUMA_QUALITY, quality, IMWRITE_JPEG_CHROMA_QUALITY, chroma_quality]``;
+      - then ``[IMWRITE_JPEG_SAMPLING_FACTOR, IMWRITE_JPEG_SAMPLING_FACTOR_<sampling>]``;
+      - then ``[IMWRITE_JPEG_RST_INTERVAL, restart_interval]`` if it is nonzero;
+      - then ``[IMWRITE_JPEG_OPTIMIZE, 1]`` if ``optimize``.
+
+    The defaults give the plain ``[IMWRITE_JPEG_QUALITY, quality]`` file (4:2:0, the standard Huffman tables, no restart
+    markers).  ``sampling`` is "420", "422" or "444"; ``restart_interval`` an int in 0..65535 MCUs; ``optimize`` a bool
+    (optimal Huffman tables per frame); ``chroma_quality`` None or an int in 1..100.  cv2 silently codes two different
+    qualities as 4:4:4, so ``chroma_quality != quality`` requires ``sampling="444"``.
 
     ``frames``: what ``overlay.draw_heads`` takes - a contiguous (n, H, W, 3) uint8 CUDA tensor on ``whenet.device`` or a list
-    of contiguous (H_i, W_i, 3) ones - or numpy arrays of the same shapes, which are uploaded.  Sides are 1..16384 and
-    ``quality`` an int in 1..100; anything else raises ``ValueError`` before anything runs.  Waits for torch's current
-    stream, then encodes in groups of 64 frames with one synchronisation each.  Only the compressed bytes leave the GPU.
-    Returns one ``bytes`` per frame; n = 0 gives []."""
+    of contiguous (H_i, W_i, 3) ones - or numpy arrays of the same shapes, which are uploaded.  Gray frames are (n, H, W, 1)
+    or (H_i, W_i, 1) and equal ``cv2.imencode(".jpg", frame[..., 0], params)``; they take the default ``sampling`` and
+    ``chroma_quality``, and a call takes one channel count.  Sides are 1..16384.  Anything else raises ``ValueError`` before
+    anything runs.  Waits for torch's current stream, then encodes in groups of 64 frames with one synchronisation each.
+    Only the compressed bytes leave the GPU.  Returns one ``bytes`` per frame; n = 0 gives []."""
     import ctypes as C
-    from ._lib import check
+    from ._lib import JpegOptions, check
     from .whenet import _ptr
-    if isinstance(quality, (bool, np.bool_)) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
+    if not _is_int(quality, 1, 100):
         raise ValueError("quality must be an int in [1, 100], not %r" % (quality,))
-    dev, items, frames_hw = _frame_list(whenet, frames)
+    if sampling not in SAMPLINGS:
+        raise ValueError("sampling must be \"420\", \"422\" or \"444\", not %r" % (sampling,))
+    if not _is_int(restart_interval, 0, 65535):
+        raise ValueError("restart_interval must be an int in [0, 65535] MCUs, not %r" % (restart_interval,))
+    if not isinstance(optimize, (bool, np.bool_)):
+        raise ValueError("optimize must be a bool, not %r" % (optimize,))
+    if chroma_quality is not None and not _is_int(chroma_quality, 1, 100):
+        raise ValueError("chroma_quality must be None or an int in [1, 100], not %r" % (chroma_quality,))
+    cq = quality if chroma_quality is None else int(chroma_quality)
+    if cq != quality and sampling != "444":
+        raise ValueError("chroma_quality %d != quality %d needs sampling=\"444\" (cv2 codes differing qualities as 4:4:4)"
+                         % (cq, quality))
+    dev, items, frames_hw, channels = _frame_list(whenet, frames)
+    if channels == 1 and (sampling != "420" or cq != quality):
+        raise ValueError("gray frames take the default sampling and chroma_quality")
     n = len(frames_hw)
     if n == 0:
         return []
     import torch
     L = whenet._L
+    opts = JpegOptions(int(quality), cq, SAMPLINGS[sampling], int(restart_interval), int(bool(optimize)))
+    default = (cq, sampling, restart_interval, bool(optimize), channels) == (quality, "420", 0, False, 3)
     out = []
     data = C.c_void_p()
     offsets = np.zeros(MAX_FRAMES_PER_CALL + 1, np.int64)
@@ -92,15 +134,20 @@ def encode_jpeg(whenet, frames, quality: int = 95) -> list:
             torch.cuda.current_stream().synchronize()       # frames the caller wrote on torch's stream are complete
         for lo in range(0, n, MAX_FRAMES_PER_CALL):
             hi = min(n, lo + MAX_FRAMES_PER_CALL)
-            if not isinstance(frames, (list, tuple)):
+            if not isinstance(frames, (list, tuple)) and default:
                 H, W = frames_hw[0]
                 check(L.whenet_encode_jpeg_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, int(dev), int(quality), C.byref(data),
                                               _ptr(offsets)))
             else:
-                ptrs = (C.c_void_p * (hi - lo))(*[_ptr(f) for f in items[lo:hi]])
+                src = items[lo:hi] if isinstance(frames, (list, tuple)) else [frames[i] for i in range(lo, hi)]
+                ptrs = (C.c_void_p * (hi - lo))(*[_ptr(f) for f in src])
                 hw = np.array(frames_hw[lo:hi], np.int32)
-                check(L.whenet_encode_jpeg_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, int(dev), int(quality), C.byref(data),
-                                                     _ptr(offsets)))
+                if default:
+                    check(L.whenet_encode_jpeg_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, int(dev), int(quality),
+                                                         C.byref(data), _ptr(offsets)))
+                else:
+                    check(L.whenet_encode_jpeg_ex_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, channels, int(dev), C.byref(opts),
+                                                     C.byref(data), _ptr(offsets)))
             for i in range(hi - lo):
                 out.append(C.string_at(data.value + int(offsets[i]), int(offsets[i + 1] - offsets[i])))
     return out

@@ -258,7 +258,7 @@ int whenet_debug_text_segments(const char* text, int org_x, int org_y, double sc
 /* The number of each display="full" label: str(np.round(np.float32(a))) for m float32 angles, NUL-terminated, one per
    `stride` (>= 32) bytes of out. */
 int whenet_debug_label_text(const float* angles, int m, char* out, int stride);
-/* Baseline JPEG files of n BGR frames (DESIGN.md section 8.9), byte-identical to
+/* Baseline JPEG files of n BGR frames (DESIGN.md section 8.9; options in section 8.11), byte-identical to
    cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, quality]): 4:2:0, the Annex K tables scaled by the IJG quality
    rule, no restart markers.  frames: n frames of H x W x 3 bytes back to back, in device memory (frames_are_device = 1) or
    host memory (0).  n in [1, 64], sides in [1, 16384], quality in [1, 100]; anything else is WHENET_EINVAL before any device
@@ -272,6 +272,29 @@ int whenet_encode_jpeg_ragged_u8(whenet_ctx* ctx, const uint8_t* const* frames, 
                                  int quality, const uint8_t** data_out, int64_t* offsets_out);
 /* The bytes of a file before its entropy-coded data (SOI .. SOS, 623 bytes) without a GPU; cap >= 623. */
 int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, int* len);
+/* JPEG options (DESIGN.md section 8.11).  A call with them equals cv2.imencode(".jpg", frame, params) where params are
+   IMWRITE_JPEG_QUALITY quality (or, when chroma_quality != quality, IMWRITE_JPEG_LUMA_QUALITY quality and
+   IMWRITE_JPEG_CHROMA_QUALITY chroma_quality), IMWRITE_JPEG_SAMPLING_FACTOR sampling, IMWRITE_JPEG_RST_INTERVAL
+   restart_interval and IMWRITE_JPEG_OPTIMIZE optimize; a one-channel frame is the (H, W) image cv2 codes as gray. */
+typedef struct whenet_jpeg_options {
+    int quality;            /* 1..100: the luma table, and the chroma table unless chroma_quality differs */
+    int chroma_quality;     /* 1..100; != quality needs sampling 444 (libjpeg codes it as 4:4:4 whatever the sampling) */
+    int sampling;           /* 420, 422 or 444: luma sampling 2x2, 2x1 or 1x1; Cb and Cr 1x1 */
+    int restart_interval;   /* 0..65535 MCUs per restart interval; 0 = no restart markers */
+    int optimize;           /* 0: Annex K Huffman tables; 1: optimal tables per frame (libjpeg's jpeg_gen_optimal_table) */
+} whenet_jpeg_options;
+/* whenet_encode_jpeg_ragged_u8 with options: frames[i] is H_i x W_i x channels (1 = gray, 3 = BGR); a gray call takes
+   sampling 420 and chroma_quality == quality.  Every argument is checked as above, WHENET_EINVAL before any device call.
+   whenet_encode_jpeg_u8 and _ragged_u8 are this call with channels 3 and {quality, quality, 420, 0, 0}. */
+int whenet_encode_jpeg_ex_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int channels,
+                             int frames_are_device, const whenet_jpeg_options* opts, const uint8_t** data_out, int64_t* offsets_out);
+/* The header (SOI .. SOS, at most 629 bytes) of a file with options (optimize 0 only) without a GPU; *len = its bytes. */
+int whenet_debug_jpeg_header_ex(int H, int W, int channels, const whenet_jpeg_options* opts, uint8_t* out, int cap, int* len);
+/* libjpeg's jpeg_gen_optimal_table on 256 symbol counts (>= 0) on the host: bits_out[16] = codes per length 1..16,
+   vals_out[*nvals_out] = the symbols by length, then value.  WHENET_EINVAL for a code past 32 bits, as libjpeg refuses it.
+   The _gpu variant runs the encoder's device kernel on the context's stream and returns when done. */
+int whenet_debug_jpeg_optimal_table(const int32_t* counts, uint8_t* bits_out, uint8_t* vals_out, int* nvals_out);
+int whenet_debug_jpeg_optimal_table_gpu(whenet_ctx* ctx, const int32_t* counts, uint8_t* bits_out, uint8_t* vals_out, int* nvals_out);
 /* JPEG decoding (DESIGN.md section 8.10), pixel-identical to cv2.imdecode(buf, cv2.IMREAD_COLOR): SOF0 / SOF1 8-bit Huffman,
    one interleaved scan, 1 component (replicated to B = G = R) or 3 (YCbCr) at 4:4:4, 4:2:2 or 4:2:0, restart intervals,
    Annex K tables where no DHT defines one, EXIF orientation 1..8 applied, sides 1..16384.
