@@ -40,7 +40,7 @@ class WhenetError(RuntimeError):
 class JpegOptions(C.Structure):
     """``whenet_jpeg_options``"""
     _fields_ = [("quality", C.c_int), ("chroma_quality", C.c_int), ("sampling", C.c_int), ("restart_interval", C.c_int),
-                ("optimize", C.c_int)]
+                ("optimize", C.c_int), ("progressive", C.c_int)]
 
 
 class Tensor(C.Structure):

@@ -1,13 +1,14 @@
-// jpeg_api.cu - whenet_encode_jpeg_u8 / _ragged_u8 / _ex_u8 and their debug entries (DESIGN.md sections 8.9 and 8.11): baseline
-// JPEG files of device or host BGR or gray frames, byte-identical to cv2.imencode(".jpg", frame, params) with the quality,
-// sampling, restart-interval, optimised-Huffman and luma/chroma-quality parameters.  The decoder (section 8.10) is
-// jpeg_decode.inc, included at the end.
+// jpeg_api.cu - whenet_encode_jpeg_u8 / _ragged_u8 / _ex_u8 and their debug entries (DESIGN.md sections 8.9, 8.11 and 8.12):
+// baseline or progressive JPEG files of device or host BGR or gray frames, byte-identical to cv2.imencode(".jpg", frame, params)
+// with the quality, sampling, restart-interval, optimised-Huffman, luma/chroma-quality and progressive parameters.  The
+// decoder (section 8.10) is jpeg_decode.inc, included at the end.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/whenet_b200.h"
@@ -51,6 +52,19 @@ struct State {
     long long* d_ffx = nullptr; size_t ffx_cap = 0;
     uint8_t* d_out = nullptr; size_t out_cap = 0;
     uint8_t* h_out = nullptr; size_t h_cap = 0;                 // pinned: the files handed to the caller
+    // progressive (section 8.12): the scan table, each scan as a Frame, its n * scans + 1 offsets, optimal tables per slot
+    ProgScan* d_pscans = nullptr;
+    Frame* d_pframes = nullptr;
+    long long* d_psmall = nullptr;
+    long long* h_psmall = nullptr;              // pinned
+    int* d_phist = nullptr;
+    uint32_t* d_phuff = nullptr;
+    uint8_t* d_pdht = nullptr;
+    uint8_t* h_pdht = nullptr;                  // pinned
+    uint8_t* d_pemit = nullptr; size_t pemit_cap = 0;           // per unit: codes a symbol
+    uint8_t* d_pjoin = nullptr; size_t pjoin_cap = 0;           // per unit: ends in an EOB run
+    int* d_peob = nullptr; size_t peob_cap = 0;                 // per unit: the length of the EOB run piece starting there
+    long long* d_pemitx = nullptr; size_t pemitx_cap = 0;       // per unit + 1: exclusive scan of d_pemit
     DecState* dec = nullptr;                                    // the decoder's scratch (jpeg_decode.inc)
 };
 
@@ -109,13 +123,13 @@ void huff_table(const uint8_t counts[16], const uint8_t* syms, uint32_t table[25
 // What a call encodes: luma and chroma qualities, MCU shape (J::Shape, kGray for one channel), restart interval in MCUs
 // (0 = none), optimised tables.
 struct Opts {
-    int quality, chroma_quality, shape, restart, optimize;
+    int quality, chroma_quality, shape, restart, optimize, progressive;
 };
 constexpr int kMaxHeaderBytes = 2 + 18 + 2 * 69 + 19 + 4 * (5 + J::kDhtBytes) + 6 + 14;
 
-// SOI, APP0 (JFIF 1.01, density 1:1, no thumbnail), DQT luma and chroma (zigzag), SOF0, DHT DC0 AC0 DC1 AC1, DRI when restarts,
-// SOS; gray has one DQT, one component and DHT DC0 AC0.  dht: the optimised tables (4 x kDhtBytes), or nullptr for Annex K.
-int header_bytes(int H, int W, const Opts& o, const uint8_t* dht, uint8_t* out) {
+// SOI, APP0 (JFIF 1.01, density 1:1, no thumbnail), DQT luma and chroma (zigzag), and SOF0 (baseline) or SOF2 (progressive);
+// gray has one DQT and one component.  Returns the bytes written.
+int frame_header(int H, int W, const Opts& o, uint8_t sof, uint8_t* out) {
     const bool gray = o.shape == J::kGray;
     const int nc = gray ? 1 : 3;
     uint8_t* p = out;
@@ -131,10 +145,20 @@ int header_bytes(int H, int W, const Opts& o, const uint8_t* dht, uint8_t* out) 
         *p++ = (uint8_t)t;
         for (int k = 0; k < 64; ++k) *p++ = (uint8_t)q[kZigzagHost[k]];
     }
-    seg(0xC0, 6 + 3 * nc);
+    seg(sof, 6 + 3 * nc);
     const uint8_t ysf = o.shape == J::k420 ? 0x22 : o.shape == J::k422 ? 0x21 : 0x11;
-    const uint8_t sof[15] = {8, (uint8_t)(H >> 8), (uint8_t)H, (uint8_t)(W >> 8), (uint8_t)W, (uint8_t)nc, 1, ysf, 0, 2, 0x11, 1, 3, 0x11, 1};
-    memcpy(p, sof, 6 + 3 * nc); p += 6 + 3 * nc;
+    const uint8_t sofb[15] = {8, (uint8_t)(H >> 8), (uint8_t)H, (uint8_t)(W >> 8), (uint8_t)W, (uint8_t)nc, 1, ysf, 0, 2, 0x11, 1, 3, 0x11, 1};
+    memcpy(p, sofb, 6 + 3 * nc); p += 6 + 3 * nc;
+    return (int)(p - out);
+}
+
+// frame_header with SOF0, then DHT DC0 AC0 DC1 AC1, DRI when restarts, SOS; gray has DHT DC0 AC0.  dht: the optimised tables
+// (4 x kDhtBytes), or nullptr for Annex K.
+int header_bytes(int H, int W, const Opts& o, const uint8_t* dht, uint8_t* out) {
+    const bool gray = o.shape == J::kGray;
+    const int nc = gray ? 1 : 3;
+    uint8_t* p = out + frame_header(H, W, o, 0xC0, out);
+    auto seg = [&](uint8_t marker, int len) { *p++ = 0xFF; *p++ = marker; *p++ = (uint8_t)((len + 2) >> 8); *p++ = (uint8_t)(len + 2); };
     for (int t = 0; t < (gray ? 2 : 4); ++t) {
         const int chroma = t >> 1, ac = t & 1;
         const uint8_t* counts = dht ? dht + t * J::kDhtBytes : ac ? kAcCounts[chroma] : kDcCounts[chroma];
@@ -260,21 +284,17 @@ void by_shape(int shape, F&& f) {
     }
 }
 
-int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const Opts& o,
-           const uint8_t** data_out, int64_t* offsets_out) {
-    JCK(cudaSetDevice(t.device));
-    if (!*t.state)
-        if (int rc = create(*t.state)) return rc;
-    J::State* st = *t.state;
-    const cudaStream_t s = t.stream;
-    int bpm = 0, mw = 0, mh = 0, strip = 0, tables = 0;
+// The call's frame table (fr, uploaded to st->d_frames) and the quantised coefficients of every block in st->d_coef, on
+// stream s; *blocks_out = the blocks of the call.  Host frames are uploaded first.
+int transform(J::State* st, cudaStream_t s, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const Opts& o,
+              std::vector<J::Frame>& fr, long long* blocks_out) {
+    int bpm = 0, mw = 0, mh = 0, strip = 0;
     by_shape(o.shape, [&](auto m) {
         using M = decltype(m);
-        bpm = M::blocks; mw = 8 * M::h; mh = 8 * M::v; strip = M::strip; tables = M::tables;
+        bpm = M::blocks; mw = 8 * M::h; mh = 8 * M::v; strip = M::strip;
     });
     const int channels = o.shape == J::kGray ? 1 : 3;
-
-    std::vector<J::Frame> fr(n);
+    fr.assign(n, J::Frame{});
     long long ctas = 0, blocks = 0, segs = 0;
     size_t in_bytes = 0;
     for (int i = 0; i < n; ++i) {
@@ -310,19 +330,40 @@ int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, 
         for (int k = 0; k < 64; ++k) qt.q8[c][k] = (uint16_t)(8 * q[k]);
     }
     if (int rc = grow(st->d_coef, st->coef_cap, (size_t)blocks * 64)) return rc;
+    JCK(cudaMemcpyAsync(st->d_frames, fr.data(), n * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
+    by_shape(o.shape, [&](auto m) {
+        J::jpeg_transform_kernel<decltype(m)::kShape><<<(unsigned)ctas, J::kTransformThreads, 0, s>>>(st->d_frames, n, qt, st->d_coef);
+    });
+    JCK(cudaGetLastError());
+    *blocks_out = blocks;
+    return 0;
+}
+
+int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const Opts& o,
+           const uint8_t** data_out, int64_t* offsets_out) {
+    JCK(cudaSetDevice(t.device));
+    if (!*t.state)
+        if (int rc = create(*t.state)) return rc;
+    J::State* st = *t.state;
+    const cudaStream_t s = t.stream;
+    int bpm = 0, tables = 0;
+    by_shape(o.shape, [&](auto m) {
+        using M = decltype(m);
+        bpm = M::blocks; tables = M::tables;
+    });
+    std::vector<J::Frame> fr;
+    long long blocks = 0;
+    if (int rc = transform(st, s, frames, hw, n, frames_are_device, o, fr, &blocks)) return rc;
+    const long long segs = fr[n - 1].seg0 + fr[n - 1].nseg;
     if (int rc = grow(st->d_bits, st->bits_cap, (size_t)blocks)) return rc;
     if (int rc = grow(st->d_excl, st->excl_cap, (size_t)blocks + 1)) return rc;
     if (int rc = grow(st->d_segc, st->segc_cap, (size_t)segs)) return rc;
     if (int rc = grow(st->d_segx, st->segx_cap, (size_t)segs + 1)) return rc;
-    JCK(cudaMemcpyAsync(st->d_frames, fr.data(), n * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
 
-    // coefficients; optimised tables from the frames' own symbols; bit lengths, bit offsets, chunks per segment
+    // optimised tables from the frames' own symbols; bit lengths, bit offsets, chunks per segment
     const unsigned code_grid = (unsigned)((blocks + J::kCodeThreads - 1) / J::kCodeThreads);
     const uint32_t* huff = st->d_huff;
     int huff_stride = 0;
-    by_shape(o.shape, [&](auto m) {
-        J::jpeg_transform_kernel<decltype(m)::kShape><<<(unsigned)ctas, J::kTransformThreads, 0, s>>>(st->d_frames, n, qt, st->d_coef);
-    });
     if (o.optimize) {
         if (!st->d_hist) {
             JCK(cudaMalloc(&st->d_hist, J::kMaxFrames * 1024 * sizeof(int)));
@@ -399,6 +440,200 @@ int encode(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, 
     return 0;
 }
 
+// ---- progressive files (DESIGN.md section 8.12)
+// libjpeg's jpeg_simple_progression: (component, -1 for all; Ss, Se, Ah, Al)
+struct ScanDef {
+    int comp, Ss, Se, Ah, Al;
+};
+const ScanDef kScriptColor[10] = {{-1, 0, 0, 0, 1}, {0, 1, 5, 0, 2},  {2, 1, 63, 0, 1}, {1, 1, 63, 0, 1}, {0, 6, 63, 0, 2},
+                                  {0, 1, 63, 2, 1}, {-1, 0, 0, 1, 0}, {2, 1, 63, 1, 0}, {1, 1, 63, 1, 0}, {0, 1, 63, 1, 0}};
+const ScanDef kScriptGray[6] = {{-1, 0, 0, 0, 1}, {0, 1, 5, 0, 2}, {0, 6, 63, 0, 2}, {0, 1, 63, 2, 1}, {-1, 0, 0, 1, 0}, {0, 1, 63, 1, 0}};
+constexpr int kMaxScans = 10, kMaxSlots = 10;      // per frame: scans, optimal tables
+constexpr int kMaxScanHeaderBytes = 2 * (4 + J::kDhtBytes + 1) + 6 + 14;
+
+// One scan's DHTs (its optimal tables, dht = slot p.slot's kDhtBytes; none for DC refinement), DRI before the first scan when
+// restarts, and SOS.  Returns the bytes written.
+int scan_header(const ScanDef& d, int nc, int restart, bool first, const uint8_t* dht, uint8_t* out) {
+    uint8_t* p = out;
+    auto seg = [&](uint8_t marker, int len) { *p++ = 0xFF; *p++ = marker; *p++ = (uint8_t)((len + 2) >> 8); *p++ = (uint8_t)(len + 2); };
+    if (!(d.Ss == 0 && d.Ah)) {
+        const int ntab = d.Ss == 0 ? (nc == 3 ? 2 : 1) : 1;
+        for (int t = 0; t < ntab; ++t) {
+            const uint8_t* counts = dht + t * J::kDhtBytes;
+            int nsym = 0;
+            for (int i = 0; i < 16; ++i) nsym += counts[i];
+            seg(0xC4, 17 + nsym);
+            *p++ = (uint8_t)(d.Ss == 0 ? t : 0x10 | (d.comp == 0 ? 0 : 1));
+            memcpy(p, counts, 16 + nsym); p += 16 + nsym;
+        }
+    }
+    if (first && restart) {
+        seg(0xDD, 2);
+        *p++ = (uint8_t)(restart >> 8); *p++ = (uint8_t)restart;
+    }
+    const int ns = d.comp < 0 ? nc : 1;
+    seg(0xDA, 4 + 2 * ns);
+    *p++ = (uint8_t)ns;
+    for (int i = 0; i < ns; ++i) {
+        const int c = d.comp < 0 ? i : d.comp, t = c == 0 ? 0 : 1;
+        *p++ = (uint8_t)(c + 1);
+        *p++ = (uint8_t)(d.Ss ? t : d.Ah ? 0 : t << 4);
+    }
+    *p++ = (uint8_t)d.Ss; *p++ = (uint8_t)d.Se; *p++ = (uint8_t)(d.Ah << 4 | d.Al);
+    return (int)(p - out);
+}
+
+// The progressive files: the baseline transform, then every scan of every frame coded by the jpeg_prog_* kernels with its own
+// optimal tables.  For placement and stuffing each scan is a Frame (pf) of the baseline kernels whose header is its DHT, DRI
+// and SOS bytes and whose two closing bytes are the next scan's first two, or EOI: a frame's first scan also carries SOI ..
+// SOF2, and a later scan's header is two bytes shorter.  The same three synchronisations as the baseline call.
+int encode_progressive(J::Target t, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const Opts& o,
+                       const uint8_t** data_out, int64_t* offsets_out) {
+    JCK(cudaSetDevice(t.device));
+    if (!*t.state)
+        if (int rc = create(*t.state)) return rc;
+    J::State* st = *t.state;
+    const cudaStream_t s = t.stream;
+    const bool gray = o.shape == J::kGray;
+    const int nc = gray ? 1 : 3, ns = gray ? 6 : 10;
+    const ScanDef* script = gray ? kScriptGray : kScriptColor;
+    int slots = 0;          // tables per frame
+    for (int k = 0; k < ns; ++k) slots += script[k].Ss == 0 ? (script[k].Ah ? 0 : nc == 3 ? 2 : 1) : 1;
+
+    std::vector<J::Frame> fr;
+    long long blocks = 0;
+    if (int rc = transform(st, s, frames, hw, n, frames_are_device, o, fr, &blocks)) return rc;
+    const int nv = n * ns;
+    std::vector<J::ProgScan> ps(nv);
+    std::vector<J::Frame> pf(nv);
+    long long units = 0, segs = 0;
+    for (int i = 0; i < n; ++i) {
+        const int mcus = fr[i].mcux * fr[i].mcuy, bw = (fr[i].W + 7) / 8, bh = (fr[i].H + 7) / 8;
+        int slot = i * slots;
+        for (int k = 0; k < ns; ++k) {
+            const ScanDef& d = script[k];
+            J::ProgScan& p = ps[i * ns + k];
+            p.units = d.comp == 0 ? bw * bh : mcus;       // a one-component luma scan skips the dummy blocks
+            p.rst = o.restart ? std::min(o.restart, p.units) : p.units;
+            p.u0 = units; p.blk0 = fr[i].blk0; p.seg0 = segs;
+            p.mcux = fr[i].mcux; p.bw = bw;
+            p.slot = d.Ss == 0 && d.Ah ? -1 : slot;
+            slot += d.Ss == 0 ? (d.Ah ? 0 : nc == 3 ? 2 : 1) : 1;
+            p.comp = d.comp; p.Ss = d.Ss; p.Se = d.Se; p.Ah = d.Ah; p.Al = d.Al;
+            J::Frame& f = pf[i * ns + k];
+            f = J::Frame{};
+            f.mcux = p.units; f.mcuy = 1; f.rst = p.rst;
+            f.nseg = (p.units + p.rst - 1) / p.rst;
+            f.blk0 = p.u0; f.seg0 = p.seg0;
+            units += p.units;
+            segs += f.nseg;
+        }
+    }
+    if (!st->d_pscans) {
+        JCK(cudaMalloc(&st->d_pscans, J::kMaxFrames * kMaxScans * sizeof(J::ProgScan)));
+        JCK(cudaMalloc(&st->d_pframes, J::kMaxFrames * kMaxScans * sizeof(J::Frame)));
+        JCK(cudaMalloc(&st->d_psmall, (J::kMaxFrames * kMaxScans + 1) * sizeof(long long)));
+        JCK(cudaHostAlloc((void**)&st->h_psmall, (J::kMaxFrames * kMaxScans + 1) * sizeof(long long), cudaHostAllocDefault));
+        JCK(cudaMalloc(&st->d_phist, J::kMaxFrames * kMaxSlots * 256 * sizeof(int)));
+        JCK(cudaMalloc(&st->d_phuff, J::kMaxFrames * kMaxSlots * 256 * sizeof(uint32_t)));
+        JCK(cudaMalloc(&st->d_pdht, J::kMaxFrames * kMaxSlots * J::kDhtBytes));
+        JCK(cudaHostAlloc((void**)&st->h_pdht, J::kMaxFrames * kMaxSlots * J::kDhtBytes, cudaHostAllocDefault));
+    }
+    if (int rc = grow(st->d_bits, st->bits_cap, (size_t)units)) return rc;
+    if (int rc = grow(st->d_excl, st->excl_cap, (size_t)units + 1)) return rc;
+    if (int rc = grow(st->d_pemit, st->pemit_cap, (size_t)units)) return rc;
+    if (int rc = grow(st->d_pjoin, st->pjoin_cap, (size_t)units)) return rc;
+    if (int rc = grow(st->d_peob, st->peob_cap, (size_t)units)) return rc;
+    if (int rc = grow(st->d_pemitx, st->pemitx_cap, (size_t)units + 1)) return rc;
+    if (int rc = grow(st->d_segc, st->segc_cap, (size_t)segs)) return rc;
+    if (int rc = grow(st->d_segx, st->segx_cap, (size_t)segs + 1)) return rc;
+    JCK(cudaMemcpyAsync(st->d_pscans, ps.data(), nv * sizeof(J::ProgScan), cudaMemcpyHostToDevice, s));
+    JCK(cudaMemcpyAsync(st->d_pframes, pf.data(), nv * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
+
+    // flags; EOB run pieces; per-scan tables; bit lengths, bit offsets, chunks per segment
+    const unsigned grid = (unsigned)((units + J::kCodeThreads - 1) / J::kCodeThreads);
+    auto code = [&](auto mode) {
+        by_shape(o.shape, [&](auto m) {
+            J::jpeg_prog_code_kernel<decltype(mode)::value, decltype(m)::kShape><<<grid, J::kCodeThreads, 0, s>>>(
+                st->d_pscans, nv, units, st->d_coef, st->d_phuff, st->d_bits, st->d_pemit, st->d_pjoin, st->d_peob, st->d_excl, st->d_segx,
+                st->d_raw, st->d_phist);
+        });
+    };
+    code(std::integral_constant<int, J::kProgShape>{});
+    JCK(cudaGetLastError());
+    if (int rc = scan(st, s, st->d_bits, units, st->d_excl)) return rc;
+    if (int rc = scan(st, s, st->d_pemit, units, st->d_pemitx)) return rc;
+    J::jpeg_prog_partition_kernel<<<(unsigned)((units + 255) / 256), 256, 0, s>>>(st->d_pscans, nv, units, st->d_pemit, st->d_pjoin, st->d_excl,
+                                                                                  st->d_pemitx, st->d_peob);
+    JCK(cudaMemsetAsync(st->d_phist, 0, (size_t)n * slots * 256 * sizeof(int), s));
+    JCK(cudaMemsetAsync(st->d_pdht, 0, (size_t)n * slots * J::kDhtBytes, s));
+    code(std::integral_constant<int, J::kProgHist>{});
+    // slot q's histogram, table and DHT bytes are at q * 256 and q * kDhtBytes: the layout of (frame q / 4, table q % 4)
+    J::jpeg_huff_build_kernel<<<n * slots, 32, 0, s>>>(st->d_phist, 4, st->d_phuff, st->d_pdht);
+    code(std::integral_constant<int, J::kProgBits>{});
+    JCK(cudaGetLastError());
+    if (int rc = scan(st, s, st->d_bits, units, st->d_excl)) return rc;
+    J::jpeg_seg_chunks_kernel<<<(unsigned)((segs + 255) / 256), 256, 0, s>>>(st->d_pframes, nv, segs, 1, st->d_excl, st->d_segc);
+    JCK(cudaGetLastError());
+    if (int rc = scan(st, s, st->d_segc, segs, st->d_segx)) return rc;
+    JCK(cudaMemcpyAsync(st->h_psmall, st->d_segx + segs, sizeof(long long), cudaMemcpyDeviceToHost, s));
+    JCK(cudaMemcpyAsync(st->h_pdht, st->d_pdht, (size_t)n * slots * J::kDhtBytes, cudaMemcpyDeviceToHost, s));
+    JCK(cudaStreamSynchronize(s));
+    const long long chunks = st->h_psmall[0];
+    uint8_t hdr[kMaxHeaderBytes + kMaxScanHeaderBytes];
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < ns; ++k) {
+            const J::ProgScan& p = ps[i * ns + k];
+            const uint8_t* dht = p.slot >= 0 ? st->h_pdht + (size_t)p.slot * J::kDhtBytes : nullptr;
+            if (dht && (dht[0] == 0xFF || (script[k].Ss == 0 && nc == 3 && dht[J::kDhtBytes] == 0xFF)))
+                return fail(WHENET_EINVAL, "frame %d scan %d: an optimal Huffman code is longer than 32 bits", i, k);
+            pf[i * ns + k].hdr = scan_header(script[k], nc, o.restart, k == 0, dht, hdr) +
+                                 (k == 0 ? frame_header(fr[i].H, fr[i].W, o, 0xC2, hdr) : -2);
+        }
+
+    // the codes, then 0x00 after every 0xFF and RSTm between segments
+    if (int rc = grow(st->d_raw, st->raw_cap, (size_t)chunks * J::kChunk / 4)) return rc;
+    JCK(cudaMemsetAsync(st->d_raw, 0, (size_t)chunks * J::kChunk, s));
+    JCK(cudaMemcpyAsync(st->d_pframes, pf.data(), nv * sizeof(J::Frame), cudaMemcpyHostToDevice, s));
+    code(std::integral_constant<int, J::kProgEmit>{});
+    if (int rc = grow(st->d_ffc, st->ffc_cap, (size_t)chunks)) return rc;
+    if (int rc = grow(st->d_ffx, st->ffx_cap, (size_t)chunks + 1)) return rc;
+    const unsigned chunk_grid = (unsigned)((chunks + 255) / 256);
+    const uint4* raw4 = reinterpret_cast<const uint4*>(st->d_raw);
+    J::jpeg_out_count_kernel<<<chunk_grid, 256, 0, s>>>(st->d_pframes, nv, st->d_segx, segs, 1, st->d_excl, raw4, chunks, st->d_ffc);
+    JCK(cudaGetLastError());
+    if (int rc = scan(st, s, st->d_ffc, chunks, st->d_ffx)) return rc;
+    J::jpeg_place_kernel<<<1, 32, 0, s>>>(st->d_pframes, nv, st->d_segx, st->d_ffx, st->d_psmall);
+    JCK(cudaGetLastError());
+    JCK(cudaMemcpyAsync(st->h_psmall, st->d_psmall, (nv + 1) * sizeof(long long), cudaMemcpyDeviceToHost, s));
+    JCK(cudaStreamSynchronize(s));
+    const long long total = st->h_psmall[nv];
+    if (int rc = grow(st->d_out, st->out_cap, (size_t)total)) return rc;
+    J::jpeg_stuff_kernel<<<chunk_grid, 256, 0, s>>>(st->d_pframes, nv, st->d_segx, segs, 1, st->d_excl, raw4, chunks, st->d_ffx, st->d_psmall,
+                                                    st->d_out);
+    JCK(cudaGetLastError());
+    if (int rc = grow_host(st->h_out, st->h_cap, (size_t)total)) return rc;
+    JCK(cudaMemcpyAsync(st->h_out, st->d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+    JCK(cudaStreamSynchronize(s));
+
+    // the host writes the headers between the scans' streams, and EOI
+    for (int i = 0; i < n; ++i) {
+        offsets_out[i] = st->h_psmall[i * ns];
+        for (int k = 0; k < ns; ++k) {
+            const J::ProgScan& p = ps[i * ns + k];
+            uint8_t* d = st->h_out + st->h_psmall[i * ns + k] - (k ? 2 : 0);
+            if (k == 0) d += frame_header(fr[i].H, fr[i].W, o, 0xC2, d);
+            scan_header(script[k], nc, o.restart, k == 0, p.slot >= 0 ? st->h_pdht + (size_t)p.slot * J::kDhtBytes : nullptr, d);
+        }
+        const long long end = st->h_psmall[(i + 1) * ns];
+        st->h_out[end - 2] = 0xFF;
+        st->h_out[end - 1] = 0xD9;
+    }
+    offsets_out[n] = st->h_psmall[nv];
+    *data_out = st->h_out;
+    return 0;
+}
+
 // Checks the options of one call (channels 1 or 3) and fills o; WHENET_EINVAL otherwise.
 int check_options(int channels, const whenet_jpeg_options* opts, Opts& o) {
     if (channels != 1 && channels != 3) return fail(WHENET_EINVAL, "channels %d is neither 1 nor 3", channels);
@@ -409,6 +644,7 @@ int check_options(int channels, const whenet_jpeg_options* opts, Opts& o) {
     if (p.sampling != 420 && p.sampling != 422 && p.sampling != 444) return fail(WHENET_EINVAL, "sampling %d is not 420, 422 or 444", p.sampling);
     if (p.restart_interval < 0 || p.restart_interval > 65535) return fail(WHENET_EINVAL, "restart_interval %d outside [0, 65535]", p.restart_interval);
     if (p.optimize != 0 && p.optimize != 1) return fail(WHENET_EINVAL, "optimize %d is neither 0 nor 1", p.optimize);
+    if (p.progressive != 0 && p.progressive != 1) return fail(WHENET_EINVAL, "progressive %d is neither 0 nor 1", p.progressive);
     if (channels == 1 && (p.sampling != 420 || p.chroma_quality != p.quality))
         return fail(WHENET_EINVAL, "one-channel frames take sampling 420 and chroma_quality = quality (a gray file has no chroma)");
     if (p.chroma_quality != p.quality && p.sampling != 444)
@@ -418,6 +654,7 @@ int check_options(int channels, const whenet_jpeg_options* opts, Opts& o) {
     o.shape = channels == 1 ? J::kGray : p.sampling == 420 ? J::k420 : p.sampling == 422 ? J::k422 : J::k444;
     o.restart = p.restart_interval;
     o.optimize = p.optimize;
+    o.progressive = p.progressive;
     return 0;
 }
 
@@ -434,10 +671,11 @@ int encode_checked(whenet_ctx* c, const uint8_t* const* frames, const int32_t* h
     if (int rc = check_options(channels, opts, o)) return rc;
     if (!data_out || !offsets_out) return fail(WHENET_EINVAL, "null data_out or offsets_out");
     if (!c) return fail(WHENET_EINVAL, "null context");
+    if (o.progressive) return encode_progressive(J::target(c), frames, hw, n, frames_are_device, o, data_out, offsets_out);
     return encode(J::target(c), frames, hw, n, frames_are_device, o, data_out, offsets_out);
 }
 
-whenet_jpeg_options default_options(int quality) { return whenet_jpeg_options{quality, quality, 420, 0, 0}; }
+whenet_jpeg_options default_options(int quality) { return whenet_jpeg_options{quality, quality, 420, 0, 0, 0}; }
 
 }  // namespace
 
@@ -457,9 +695,13 @@ void destroy(State* st) {
     destroy_dec(st->dec);
     for (void* p : {(void*)st->d_huff, (void*)st->d_ohuff, (void*)st->d_hist, (void*)st->d_dht, (void*)st->d_frames, (void*)st->d_small,
                     (void*)st->d_in, (void*)st->d_coef, (void*)st->d_bits, (void*)st->d_excl, (void*)st->d_segc, (void*)st->d_segx,
-                    (void*)st->d_tiles, (void*)st->d_raw, (void*)st->d_ffc, (void*)st->d_ffx, (void*)st->d_out})
+                    (void*)st->d_tiles, (void*)st->d_raw, (void*)st->d_ffc, (void*)st->d_ffx, (void*)st->d_out, (void*)st->d_pscans,
+                    (void*)st->d_pframes, (void*)st->d_psmall, (void*)st->d_phist, (void*)st->d_phuff, (void*)st->d_pdht, (void*)st->d_pemit,
+                    (void*)st->d_pjoin, (void*)st->d_peob, (void*)st->d_pemitx})
         if (p) cudaFree(p);
     if (st->h_small) cudaFreeHost(st->h_small);
+    if (st->h_psmall) cudaFreeHost(st->h_psmall);
+    if (st->h_pdht) cudaFreeHost(st->h_pdht);
     if (st->h_dht) cudaFreeHost(st->h_dht);
     if (st->h_out) cudaFreeHost(st->h_out);
     delete st;
@@ -503,7 +745,7 @@ int whenet_debug_jpeg_header(int H, int W, int quality, uint8_t* out, int cap, i
     if (quality < 1 || quality > 100) return fail(WHENET_EINVAL, "quality %d outside [1, 100]", quality);
     constexpr int kDefaultHeaderBytes = 623;
     if (!out || !len || cap < kDefaultHeaderBytes) return fail(WHENET_EINVAL, "null out or len, or cap %d < %d", cap, kDefaultHeaderBytes);
-    *len = header_bytes(H, W, Opts{quality, quality, J::k420, 0, 0}, nullptr, out);
+    *len = header_bytes(H, W, Opts{quality, quality, J::k420, 0, 0, 0}, nullptr, out);
     return 0;
 }
 
@@ -512,6 +754,7 @@ int whenet_debug_jpeg_header_ex(int H, int W, int channels, const whenet_jpeg_op
     Opts o;
     if (int rc = check_options(channels, opts, o)) return rc;
     if (o.optimize) return fail(WHENET_EINVAL, "an optimised header depends on the frame's symbols");
+    if (o.progressive) return fail(WHENET_EINVAL, "a progressive file's scan headers depend on the frame's symbols");
     uint8_t buf[kMaxHeaderBytes];
     const int n = header_bytes(H, W, o, nullptr, buf);
     if (!out || !len || cap < n) return fail(WHENET_EINVAL, "null out or len, or cap %d < %d", cap, n);

@@ -598,5 +598,261 @@ __global__ void __launch_bounds__(256) jpeg_stuff_kernel(const Frame* __restrict
     if (p.rst) { dst[0] = 0xFF; dst[1] = (uint8_t)(0xD0 + (p.k & 7)); }
 }
 
+// ---- progressive files (DESIGN.md section 8.12): the same coefficients, coded as libjpeg's scan script
+// A unit is one MCU of an interleaved (DC) scan, or one block of a one-component scan in the component's own raster order.
+// Every scan of every frame of the call is one entry of the scan table, and its units follow the previous scan's units, so
+// each kernel below runs all scans of the call in one grid.  For placement, output counting and stuffing each scan is a
+// Frame of the existing kernels: units are its blocks (bpm 1), a restart interval of units its segment.
+//   jpeg_prog_code_kernel<kProgShape, S>   flags: emits a symbol, ends in an EOB run (joins), correction bits it adds to a run
+//   jpeg_prog_partition_kernel             splits each EOB run at 0x7FFF blocks and 937 buffered correction bits
+//   jpeg_prog_code_kernel<kProgHist, S>    per-scan symbol histograms (jpeg_huff_build_kernel then builds each table)
+//   jpeg_prog_code_kernel<kProgBits, S>    each unit's bit length;  <kProgEmit, S> its bits at its offset
+constexpr int kEobRunMax = 0x7FFF;
+constexpr int kMaxCorrBits = 1000 - 64 + 1;    // a run is flushed once its buffered correction bits pass this (libjpeg)
+enum ProgMode { kProgShape = 0, kProgHist = 1, kProgBits = 2, kProgEmit = 3 };
+
+struct ProgScan {
+    long long u0;           // first unit of the scan in the call
+    long long blk0;         // the frame's first block in coef
+    long long seg0;         // first segment of the scan in the call
+    int units, rst;         // units of the scan; units per segment
+    int mcux, bw;           // MCUs per row of the frame; blocks per row of the component (one-component scans)
+    int slot;               // table slot of component 0 (DC) or of the scan's AC table; DC chroma is slot + 1; -1: no table
+    int comp;               // the component of a one-component scan; -1 for all (interleaved)
+    int Ss, Se, Ah, Al;
+};
+
+__device__ __forceinline__ int find_scan(const ProgScan* __restrict__ sc, int n, long long u) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (sc[mid].u0 <= u) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// One thread per unit of the call.  kMode:
+//   kProgShape: emit[u] = the unit codes a symbol, join[u] = it ends in zeros (so it joins an EOB run), corr[u] = the
+//               correction bits it adds to that run; eob[u] = 0.  DC units emit and never join.
+//   kProgHist:  the unit's symbols, and the EOBn symbol of a run piece starting at it (eob[u] > 0), counted into
+//               hist[slot * 256 + symbol] through a CTA histogram for the two slots of the CTA's first unit.
+//   kProgBits:  bits[u] = its coded length;  kProgEmit: its bits at excl[u] - excl[first unit of its segment] in the
+//               segment's stream at chunk seg_cx[segment], the segment's last unit padding the final byte with 1s.
+// A unit's bits are its symbols (with the correction bits refinement buffers between them), then the EOBn symbol and its run
+// length of a piece starting at it, then its own correction bits that the run carries: the stream order, as the blocks of a
+// piece after its first send nothing but their correction bits.
+template <int kMode, int S>
+__global__ void __launch_bounds__(kCodeThreads) jpeg_prog_code_kernel(const ProgScan* __restrict__ scans, int nscans, long long nunits,
+                                                                      const int16_t* __restrict__ coef, const uint32_t* __restrict__ huff,
+                                                                      int* __restrict__ bits, uint8_t* __restrict__ emit,
+                                                                      uint8_t* __restrict__ join, int* __restrict__ eob,
+                                                                      const long long* __restrict__ excl, const long long* __restrict__ seg_cx,
+                                                                      uint32_t* __restrict__ raw, int* __restrict__ hist) {
+    using M = Mcu<S>;
+    __shared__ int sh[kMode == kProgHist ? 2 * 256 : 1];
+    const long long g0 = (long long)blockIdx.x * kCodeThreads;
+    long long u = g0 + threadIdx.x;
+    const bool live = u < nunits;
+    int slot0 = -1;
+    if (kMode == kProgHist) {
+        for (int i = threadIdx.x; i < 2 * 256; i += kCodeThreads) sh[i] = 0;
+        slot0 = scans[find_scan(scans, nscans, g0)].slot;
+        __syncthreads();
+        if (!live) u = nunits - 1;          // walks a real unit but counts nothing
+    } else if (!live) {
+        return;
+    }
+    const ProgScan p = scans[find_scan(scans, nscans, u)];
+    const int l = (int)(u - p.u0), seg = l / p.rst;
+    const bool seg_first = l == seg * p.rst;
+    const long long us = p.u0 + (long long)seg * p.rst;        // the segment's first unit
+    const bool seg_last = l + 1 == min((seg + 1) * p.rst, p.units);
+    const int run = kMode == kProgShape ? 0 : eob[u];
+
+    BitSink s{};
+    long long total = 0;
+    if (kMode == kProgEmit) {
+        if (excl[u + 1] == excl[u] && !seg_last) return;
+        const long long off = excl[u] - excl[us];
+        s.words = raw + seg_cx[p.seg0 + seg] * (kChunk / 4);
+        s.w = off >> 5;
+        s.nacc = (int)(off & 31);
+        s.first = true;
+    }
+    auto sym = [&](int t, int symbol, uint32_t extra, int nb) {     // table slot p.slot + t, then nb extra bits
+        if (kMode == kProgHist) {
+            if (!live) return;
+            const int sl = p.slot + t;
+            if (slot0 >= 0 && (unsigned)(sl - slot0) < 2u) atomicAdd(sh + (sl - slot0) * 256 + symbol, 1);
+            else atomicAdd(hist + sl * 256 + symbol, 1);
+            return;
+        }
+        if (kMode == kProgShape) return;
+        const uint32_t hc = __ldg(huff + (p.slot + t) * 256 + symbol);
+        const int len = (int)(hc >> 16);
+        if (kMode == kProgEmit) s.put(((hc & 0xffff) << nb) | (extra & ((1u << nb) - 1)), len + nb);
+        else total += len + nb;
+    };
+    auto put_bits = [&](unsigned long long v, int nb) {             // nb <= 63 raw bits
+        if (kMode == kProgEmit) {
+            for (; nb > 32; nb -= 32) s.put((uint32_t)(v >> (nb - 32)), 32);
+            s.put((uint32_t)(v & ((1ull << nb) - 1)), nb);
+        } else if (kMode == kProgBits) {
+            total += nb;
+        }
+    };
+
+    bool emits = true, joins = false;
+    int ncorr = 0;
+    unsigned long long corr = 0;        // the correction bits this unit hands to its run
+    if (p.Ss == 0) {
+        // DC: every block of the MCU (one block for gray), the prediction being the previous block of the same component in
+        // the segment, shifted by Al
+        const long long g = p.blk0 + (long long)l * M::blocks;
+#pragma unroll
+        for (int b = 0; b < M::blocks; ++b) {
+            const int v = coef[(g + b) * 64] >> p.Al;
+            if (p.Ah) { put_bits(v & 1, 1); continue; }
+            long long prev = -1;
+            if (b >= 1 && b < M::luma) prev = g + b - 1;
+            else if (!seg_first) prev = b == 0 ? g - M::blocks + M::luma - 1 : g + b - M::blocks;
+            const int diff = v - (prev >= 0 ? coef[prev * 64] >> p.Al : 0);
+            const int nb = bit_length(diff < 0 ? -diff : diff);
+            sym(b < M::luma ? 0 : 1, nb, (uint32_t)(diff < 0 ? diff - 1 : diff), nb);
+        }
+    } else {
+        long long g;
+        if (p.comp == 0) {
+            const int by = l / p.bw, bx = l - by * p.bw;
+            g = p.blk0 + (long long)((by / M::v) * p.mcux + bx / M::h) * M::blocks + (by % M::v) * M::h + bx % M::h;
+        } else {
+            g = p.blk0 + (long long)l * M::blocks + M::luma + p.comp - 1;
+        }
+        // masks of the band's coefficients with |c| >> Al == 1 and > 1
+        const int16_t* __restrict__ c = coef + g * 64;
+        unsigned long long one = 0, big = 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int4 q = __ldg(reinterpret_cast<const int4*>(c) + i);
+            const uint32_t w[4] = {(uint32_t)q.x, (uint32_t)q.y, (uint32_t)q.z, (uint32_t)q.w};
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int v = (int16_t)(w[j >> 1] >> (16 * (j & 1)));
+                const int a = (v < 0 ? -v : v) >> p.Al;
+                one |= (unsigned long long)(a == 1) << (8 * i + j);
+                big |= (unsigned long long)(a > 1) << (8 * i + j);
+            }
+        }
+        const unsigned long long band = (~0ull >> (63 - p.Se)) & (~0ull << p.Ss);
+        one &= band;
+        big &= band;
+        int last = p.Ss - 1;
+        if (p.Ah == 0) {
+            unsigned long long nz = one | big;
+            emits = nz != 0;
+            while (nz) {
+                const int k = __ffsll((long long)nz) - 1;
+                nz &= nz - 1;
+                int r = k - last - 1;
+                for (; r > 15; r -= 16) sym(0, 0xF0, 0, 0);
+                const int v = __ldg(c + k), a = (v < 0 ? -v : v) >> p.Al;
+                const int nb = bit_length(a);
+                sym(0, r << 4 | nb, (uint32_t)(v < 0 ? ~a : a), nb);
+                last = k;
+            }
+            joins = last < p.Se;
+        } else {
+            // refinement: a coefficient that was nonzero before sends one correction bit, buffered until the next symbol;
+            // zero runs past 15 send ZRL only up to the last newly nonzero coefficient
+            const int eob_k = one ? 63 - __clzll((long long)one) : -1;
+            unsigned long long nz = one | big;
+            emits = one != 0;
+            int r = 0;
+            while (nz) {
+                const int k = __ffsll((long long)nz) - 1;
+                nz &= nz - 1;
+                r += k - last - 1;
+                last = k;
+                for (; r > 15 && k <= eob_k; r -= 16) {
+                    sym(0, 0xF0, 0, 0);
+                    put_bits(corr, ncorr);
+                    corr = 0; ncorr = 0;
+                }
+                const int v = __ldg(c + k);
+                if ((big >> k) & 1) {
+                    corr = corr << 1 | (((v < 0 ? -v : v) >> p.Al) & 1);
+                    ++ncorr;
+                    continue;
+                }
+                sym(0, r << 4 | 1, v < 0 ? 0 : 1, 1);
+                put_bits(corr, ncorr);
+                corr = 0; ncorr = 0; r = 0;
+            }
+            r += p.Se - last;
+            joins = r > 0 || ncorr > 0;
+        }
+    }
+    if (kMode == kProgShape) {
+        emit[u] = emits;
+        join[u] = joins;
+        bits[u] = joins ? ncorr : 0;
+        eob[u] = 0;
+        return;
+    }
+    if (run > 0) {
+        const int nb = 31 - __clz(run);
+        sym(0, nb << 4, (uint32_t)run, nb);
+    }
+    if (joins) put_bits(corr, ncorr);
+    if (kMode == kProgBits) { bits[u] = (int)total; return; }
+    if (kMode == kProgHist) {
+        __syncthreads();
+        if (slot0 >= 0)
+            for (int i = threadIdx.x; i < 2 * 256; i += kCodeThreads)
+                if (sh[i]) atomicAdd(hist + slot0 * 256 + i, sh[i]);
+        return;
+    }
+    if (seg_last) {
+        const int pad = (int)((8 - ((excl[u + 1] - excl[us]) & 7)) & 7);
+        if (pad) s.put((1u << pad) - 1, pad);
+    }
+    s.flush();
+}
+
+// One thread per unit.  A run starts at a joining unit that is its segment's first, emits a symbol, or follows a unit that
+// did not join; it ends before the next emitting unit or at the segment's end.  Its starting thread splits it greedily where
+// libjpeg flushes: after 0x7FFF units, or after the unit that takes the buffered correction bits past kMaxCorrBits.  corr_x
+// and emit_x are exclusive scans of the units' correction bits and emit flags; eob[first unit of each piece] = its length.
+__global__ void __launch_bounds__(256) jpeg_prog_partition_kernel(const ProgScan* __restrict__ scans, int nscans, long long nunits,
+                                                                  const uint8_t* __restrict__ emit, const uint8_t* __restrict__ join,
+                                                                  const long long* __restrict__ corr_x, const long long* __restrict__ emit_x,
+                                                                  int* __restrict__ eob) {
+    const long long u = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (u >= nunits || !join[u]) return;
+    const ProgScan& p = scans[find_scan(scans, nscans, u)];
+    const int l = (int)(u - p.u0), seg = l / p.rst;
+    if (l != seg * p.rst && !emit[u] && join[u - 1]) return;
+    long long lo = u, hi = p.u0 + min((seg + 1) * p.rst, p.units) - 1;    // the run's end: no emitting unit in (u, end]
+    const long long e0 = emit_x[u + 1];
+    while (lo < hi) {
+        const long long mid = (lo + hi + 1) >> 1;
+        if (emit_x[mid + 1] == e0) lo = mid; else hi = mid - 1;
+    }
+    const long long end = lo;
+    for (long long q = u; q <= end;) {
+        long long e = min(q + kEobRunMax - 1, end);
+        if (p.Ah && corr_x[e + 1] - corr_x[q] > kMaxCorrBits) {     // the first unit that passes the cap
+            long long a = q, b = e;
+            while (a < b) {
+                const long long mid = (a + b) >> 1;
+                if (corr_x[mid + 1] - corr_x[q] > kMaxCorrBits) b = mid; else a = mid + 1;
+            }
+            e = a;
+        }
+        eob[q] = (int)(e - q + 1);
+        q = e + 1;
+    }
+}
+
 }  // namespace jpeg
 }  // namespace whenet

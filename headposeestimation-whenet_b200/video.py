@@ -78,20 +78,23 @@ def _is_int(x, lo, hi):
 
 
 def encode_jpeg(whenet, frames, quality: int = 95, *, sampling: str = "420", restart_interval: int = 0, optimize: bool = False,
-                chroma_quality=None) -> list:
+                chroma_quality=None, progressive: bool = False) -> list:
     """JPEG files of BGR or gray ``frames``, each byte-identical to ``cv2.imencode(".jpg", frame, params)[1].tobytes()``
-    (baseline), encoded on ``whenet``'s GPU and stream.  ``params`` are:
+    (baseline, or progressive), encoded on ``whenet``'s GPU and stream.  ``params`` are:
 
       - ``[IMWRITE_JPEG_QUALITY, quality]``, or, when ``chroma_quality`` is given and differs from ``quality``,
         ``[IMWRITE_JPEG_LUMA_QUALITY, quality, IMWRITE_JPEG_CHROMA_QUALITY, chroma_quality]``;
       - then ``[IMWRITE_JPEG_SAMPLING_FACTOR, IMWRITE_JPEG_SAMPLING_FACTOR_<sampling>]``;
       - then ``[IMWRITE_JPEG_RST_INTERVAL, restart_interval]`` if it is nonzero;
-      - then ``[IMWRITE_JPEG_OPTIMIZE, 1]`` if ``optimize``.
+      - then ``[IMWRITE_JPEG_OPTIMIZE, 1]`` if ``optimize``;
+      - then ``[IMWRITE_JPEG_PROGRESSIVE, 1]`` if ``progressive``.
 
     The defaults give the plain ``[IMWRITE_JPEG_QUALITY, quality]`` file (4:2:0, the standard Huffman tables, no restart
     markers).  ``sampling`` is "420", "422" or "444"; ``restart_interval`` an int in 0..65535 MCUs; ``optimize`` a bool
     (optimal Huffman tables per frame); ``chroma_quality`` None or an int in 1..100.  cv2 silently codes two different
-    qualities as 4:4:4, so ``chroma_quality != quality`` requires ``sampling="444"``.
+    qualities as 4:4:4, so ``chroma_quality != quality`` requires ``sampling="444"``.  ``progressive`` a bool: libjpeg's
+    progressive scan script with optimal tables per scan (DESIGN.md section 8.12), usually smaller than the optimised file;
+    ``optimize`` then changes nothing, as in cv2.  MJPG players expect baseline frames, so keep it off for ``MJPGWriter``.
 
     ``frames``: what ``overlay.draw_heads`` takes - a contiguous (n, H, W, 3) uint8 CUDA tensor on ``whenet.device`` or a list
     of contiguous (H_i, W_i, 3) ones - or numpy arrays of the same shapes, which are uploaded.  Gray frames are (n, H, W, 1)
@@ -110,6 +113,8 @@ def encode_jpeg(whenet, frames, quality: int = 95, *, sampling: str = "420", res
         raise ValueError("restart_interval must be an int in [0, 65535] MCUs, not %r" % (restart_interval,))
     if not isinstance(optimize, (bool, np.bool_)):
         raise ValueError("optimize must be a bool, not %r" % (optimize,))
+    if not isinstance(progressive, (bool, np.bool_)):
+        raise ValueError("progressive must be a bool, not %r" % (progressive,))
     if chroma_quality is not None and not _is_int(chroma_quality, 1, 100):
         raise ValueError("chroma_quality must be None or an int in [1, 100], not %r" % (chroma_quality,))
     cq = quality if chroma_quality is None else int(chroma_quality)
@@ -124,8 +129,8 @@ def encode_jpeg(whenet, frames, quality: int = 95, *, sampling: str = "420", res
         return []
     import torch
     L = whenet._L
-    opts = JpegOptions(int(quality), cq, SAMPLINGS[sampling], int(restart_interval), int(bool(optimize)))
-    default = (cq, sampling, restart_interval, bool(optimize), channels) == (quality, "420", 0, False, 3)
+    opts = JpegOptions(int(quality), cq, SAMPLINGS[sampling], int(restart_interval), int(bool(optimize)), int(bool(progressive)))
+    default = (cq, sampling, restart_interval, bool(optimize), bool(progressive), channels) == (quality, "420", 0, False, False, 3)
     out = []
     data = C.c_void_p()
     offsets = np.zeros(MAX_FRAMES_PER_CALL + 1, np.int64)
@@ -264,6 +269,8 @@ class MJPGWriter:
     a ``movi`` list of ``00dc`` chunks padded to even length, an ``ix00`` standard index per ``movi`` list, and ``idx1`` with a
     keyframe entry per frame of the first segment.  Past ``SEGMENT_LIMIT`` bytes the file continues in ``RIFF AVIX`` segments;
     frame counts, sizes and the super index are fixed up on ``close()``.
+
+    MJPG players expect baseline frames, which is what cv2.VideoWriter writes: encode them with ``progressive=False``.
 
     ``frame_size`` is ``(width, height)`` as for cv2.VideoWriter; ``fps`` > 0.  ``write`` takes one JPEG or a sequence of them
     and refuses (``ValueError``, nothing written) any item that does not start with SOI or whose SOF0 size differs from

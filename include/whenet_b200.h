@@ -282,13 +282,17 @@ typedef struct whenet_jpeg_options {
     int sampling;           /* 420, 422 or 444: luma sampling 2x2, 2x1 or 1x1; Cb and Cr 1x1 */
     int restart_interval;   /* 0..65535 MCUs per restart interval; 0 = no restart markers */
     int optimize;           /* 0: Annex K Huffman tables; 1: optimal tables per frame (libjpeg's jpeg_gen_optimal_table) */
+    int progressive;        /* 0: baseline (SOF0); 1: progressive (SOF2, DESIGN.md section 8.12), equal to cv2 with
+                               IMWRITE_JPEG_PROGRESSIVE 1: libjpeg's scan script with optimal tables per scan, so optimize is
+                               ignored, as cv2 ignores it.  Left out of an initialiser it is 0, the baseline file. */
 } whenet_jpeg_options;
 /* whenet_encode_jpeg_ragged_u8 with options: frames[i] is H_i x W_i x channels (1 = gray, 3 = BGR); a gray call takes
    sampling 420 and chroma_quality == quality.  Every argument is checked as above, WHENET_EINVAL before any device call.
-   whenet_encode_jpeg_u8 and _ragged_u8 are this call with channels 3 and {quality, quality, 420, 0, 0}. */
+   whenet_encode_jpeg_u8 and _ragged_u8 are this call with channels 3 and {quality, quality, 420, 0, 0, 0}. */
 int whenet_encode_jpeg_ex_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int channels,
                              int frames_are_device, const whenet_jpeg_options* opts, const uint8_t** data_out, int64_t* offsets_out);
-/* The header (SOI .. SOS, at most 629 bytes) of a file with options (optimize 0 only) without a GPU; *len = its bytes. */
+/* The header (SOI .. SOS, at most 629 bytes) of a file with options (optimize 0 and progressive 0 only: those headers
+   depend on the frame's symbols) without a GPU; *len = its bytes. */
 int whenet_debug_jpeg_header_ex(int H, int W, int channels, const whenet_jpeg_options* opts, uint8_t* out, int cap, int* len);
 /* libjpeg's jpeg_gen_optimal_table on 256 symbol counts (>= 0) on the host: bits_out[16] = codes per length 1..16,
    vals_out[*nvals_out] = the symbols by length, then value.  WHENET_EINVAL for a code past 32 bits, as libjpeg refuses it.

@@ -4,9 +4,9 @@ byte-equal on every repetition; then the chain detect_and_estimate_frames + draw
 detect_and_estimate_frames + draw_heads.  Prints the card it ran on.  Usage: python tools/jpeg_bench.py [quality]
 
 ``python tools/jpeg_bench.py --options [quality]`` times the option sets of DESIGN.md section 8.11 instead (default, 4:4:4,
-optimised tables, a restart interval of one MCU row, 4:4:4 + optimised), each against download + cv2.imencode with the same
+optimised tables, a restart interval of one MCU row, 4:4:4 + optimised; progressive alone and at 4:4:4, section 8.12), each against download + cv2.imencode with the same
 parameters on the same frames, arms alternating and checked byte-equal every repetition; then, with torch.profiler, the
-kernel time of the optimised path's histogram and table build.  ``--default-only`` prints one JSON line with the default
+kernel time of the optimised path's histogram and table build and of each progressive kernel.  ``--default-only`` prints one JSON line with the default
 path's per-frame time (for comparing two builds)."""
 import os
 import subprocess
@@ -44,13 +44,15 @@ def card():
                           capture_output=True, text=True).stdout.strip()
 
 
-def cv2_params(quality, sampling="420", restart_interval=0, optimize=False):
+def cv2_params(quality, sampling="420", restart_interval=0, optimize=False, progressive=False):
     import cv2
     p = [cv2.IMWRITE_JPEG_QUALITY, quality, cv2.IMWRITE_JPEG_SAMPLING_FACTOR, getattr(cv2, "IMWRITE_JPEG_SAMPLING_FACTOR_" + sampling)]
     if restart_interval:
         p += [cv2.IMWRITE_JPEG_RST_INTERVAL, restart_interval]
     if optimize:
         p += [cv2.IMWRITE_JPEG_OPTIMIZE, 1]
+    if progressive:
+        p += [cv2.IMWRITE_JPEG_PROGRESSIVE, 1]
     return p
 
 
@@ -64,7 +66,8 @@ def options(quality=95, reps=20):
     dev = annotated_frames(wn)
     n = dev.shape[0]
     sets = [("default", {}), ("444", dict(sampling="444")), ("optimize", dict(optimize=True)),
-            ("restart 1 MCU row", dict(restart_interval=(1920 + 15) // 16)), ("444 + optimize", dict(sampling="444", optimize=True))]
+            ("restart 1 MCU row", dict(restart_interval=(1920 + 15) // 16)), ("444 + optimize", dict(sampling="444", optimize=True)),
+            ("progressive", dict(progressive=True)), ("444 + progressive", dict(sampling="444", progressive=True))]
     times = {name: ([], []) for name, _ in sets}
     sizes = {}
     for r in range(reps + 2):
@@ -101,6 +104,15 @@ def options(quality=95, reps=20):
         print("  %8.4f  %s" % (v, k[:100]))
     opt = sum(v for k, v in per.items() if "code_kernel<2" in k or "huff_build" in k)
     print("  histogram + table build: %.4f ms per frame of %.4f ms of kernels" % (opt, total))
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(10):
+            video.encode_jpeg(wn, dev, quality, progressive=True)
+        torch.cuda.synchronize()
+    per = {e.key: e.device_time_total / 10 / n / 1e3 for e in prof.key_averages() if "jpeg" in e.key}
+    print("progressive=True kernels, ms per frame (torch.profiler, 10 calls of %d frames):" % n)
+    for k, v in sorted(per.items(), key=lambda kv: -kv[1]):
+        print("  %8.4f  %s" % (v, k[:100]))
+    print("  total %.4f ms per frame of kernels" % sum(per.values()))
 
 
 def default_only(quality=95, reps=20):
