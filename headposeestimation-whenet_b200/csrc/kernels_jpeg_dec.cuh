@@ -182,40 +182,65 @@ JD_HD PieceResult decode_piece(const DecFrame& fr, const Tables& t, const uint8_
 }
 
 // ---------------------------------------------------------------------------------------------------- pixels
-// libjpeg's islow IDCT (jidctint.c, CONST_BITS 13, PASS1_BITS 2), columns first.  The coefficient x quantiser product is taken
-// modulo 2^16 and the output is clamped to [0, 255], as libjpeg-turbo's SIMD IDCT does; for coefficients an encoder makes from
-// 8-bit samples neither wraps nor clamps beyond what the C code's range-limit table does.
+// libjpeg's islow IDCT (jidctint.c, CONST_BITS 13, PASS1_BITS 2), columns first, with the 16-bit steps of libjpeg-turbo's SIMD
+// version, which cv2.imdecode runs (the numpy model in oracle/jpeg_decode_oracle.py pins each one against cv2):
+//   - the coefficient x quantiser product is taken modulo 2^16;
+//   - a block whose coefficient rows 1..7 are all zero skips the column pass: every workspace row is the dequantised row 0
+//     shifted left by PASS1_BITS modulo 2^16;
+//   - the pairwise sums d0 + d4, d0 - d4, d7 + d3 and d5 + d1 of both passes are taken modulo 2^16 (the other sums of the C
+//     code are folded into 32-bit multiply-adds there, so they stay exact here);
+//   - each pass saturates its descaled output to int16; the row pass then clamps to [-128, 127] and adds 128.
+// No 32-bit sum can overflow: the largest, |tmp12 +- o1|, stays below 2^31 - 2^17 for any int16 inputs.  For coefficients an
+// encoder makes from 8-bit samples nothing wraps or saturates, and the result is the C code's.
 __host__ __device__ constexpr int c13(double x) { return (int)(x * 8192.0 + 0.5); }
+JD_HD int s16(int x) { return (int)(int16_t)x; }
 
-template <int kShift, typename In, typename Out, typename F>
-JD_HD void idct_pass(const In* d, int s, Out* o, int os, F load) {
+template <int kShift, typename In, typename F>
+JD_HD void idct_pass(const In* d, int s, int16_t* o, int os, F load) {
     const int z2e = load(d[2 * s], 2), z3e = load(d[6 * s], 6);
     const int z1 = (z2e + z3e) * c13(0.541196100);
     const int tmp2 = z1 - z3e * c13(1.847759065), tmp3 = z1 + z2e * c13(0.765366865);
     const int a = load(d[0], 0), b = load(d[4 * s], 4);
-    const int tmp0 = (a + b) * 8192, tmp1 = (a - b) * 8192;
+    const int tmp0 = s16(a + b) * 8192, tmp1 = s16(a - b) * 8192;
     const int tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
     int o0 = load(d[7 * s], 7), o1 = load(d[5 * s], 5), o2 = load(d[3 * s], 3), o3 = load(d[s], 1);
-    int z1o = o0 + o3, z2o = o1 + o2, z3o = o0 + o2, z4o = o1 + o3;
+    int z1o = o0 + o3, z2o = o1 + o2, z3o = s16(o0 + o2), z4o = s16(o1 + o3);
     const int z5 = (z3o + z4o) * c13(1.175875602);
     o0 *= c13(0.298631336); o1 *= c13(2.053119869); o2 *= c13(3.072711026); o3 *= c13(1.501321110);
     z1o *= -c13(0.899976223); z2o *= -c13(2.562915447); z3o *= -c13(1.961570560); z4o *= -c13(0.390180644);
     z3o += z5; z4o += z5;
     o0 += z1o + z3o; o1 += z2o + z4o; o2 += z2o + z3o; o3 += z1o + z4o;
-    auto put = [&](int i, int x) { o[i * os] = Out((x + (1 << (kShift - 1))) >> kShift); };
+    auto put = [&](int i, int x) {
+        const int v = (x + (1 << (kShift - 1))) >> kShift;
+        o[i * os] = (int16_t)(v < -32768 ? -32768 : v > 32767 ? 32767 : v);
+    };
     put(0, tmp10 + o3); put(7, tmp10 - o3); put(1, tmp11 + o2); put(6, tmp11 - o2);
     put(2, tmp12 + o1); put(5, tmp12 - o1); put(3, tmp13 + o0); put(4, tmp13 - o0);
 }
 
-// column `col` of a block (natural-order coefficients) -> ws[col], ws[8 + col], ...
-JD_HD void idct_column(const int16_t* coef, const uint16_t* q, int col, int* ws) {
-    auto deq = [&](int16_t c, int row) { return (int)(int16_t)(c * q[row * 8 + col]); };
-    idct_pass<13 - 2>(coef + col, 8, ws + col, 8, deq);
+// column `col` of a block has a non-zero coefficient in rows 1..7 (no block with one takes the DC-only column pass)
+JD_HD bool idct_column_ac(const int16_t* coef, int col) {
+    int nz = 0;
+#pragma unroll
+    for (int r = 1; r < 8; ++r) nz |= coef[r * 8 + col];
+    return nz != 0;
+}
+// column `col` of a block (natural-order coefficients) -> ws[col], ws[8 + col], ...; dc_only: no column of the block has a
+// non-zero coefficient in rows 1..7
+JD_HD void idct_column(const int16_t* coef, const uint16_t* q, int col, bool dc_only, int16_t* ws) {
+    auto deq = [&](int16_t c, int row) { return s16(c * q[row * 8 + col]); };
+    if (dc_only) {
+        const int16_t v = (int16_t)(deq(coef[col], 0) * 4);
+#pragma unroll
+        for (int r = 0; r < 8; ++r) ws[r * 8 + col] = v;
+    } else {
+        idct_pass<13 - 2>(coef + col, 8, ws + col, 8, deq);
+    }
 }
 // row `row` of the workspace -> 8 samples
-JD_HD void idct_row(const int* ws, int row, uint8_t* out) {
-    int v[8];
-    idct_pass<13 + 2 + 3>(ws + row * 8, 1, v, 1, [](int x, int) { return x; });
+JD_HD void idct_row(const int16_t* ws, int row, uint8_t* out) {
+    int16_t v[8];
+    idct_pass<13 + 2 + 3>(ws + row * 8, 1, v, 1, [](int16_t x, int) { return (int)x; });
     for (int i = 0; i < 8; ++i) out[i] = (uint8_t)(v[i] < -128 ? 0 : v[i] > 127 ? 255 : v[i] + 128);
 }
 
@@ -759,15 +784,16 @@ constexpr int kIdctBlocks = 32;      // blocks per CTA, 8 threads each
 
 __global__ void __launch_bounds__(256) jd_idct_kernel(const DecFrame* __restrict__ fr, int n, const Tables* __restrict__ tabs, long long nblocks,
                                                       const int16_t* __restrict__ coef, uint8_t* __restrict__ planes) {
-    __shared__ int ws[kIdctBlocks][64];
+    __shared__ int16_t ws[kIdctBlocks][64];
     const int lb = threadIdx.x >> 3, t = threadIdx.x & 7;
     const long long g = (long long)blockIdx.x * kIdctBlocks + lb;
-    const bool live = g < nblocks;
+    const bool live = g < nblocks;      // the same for the 8 threads of a block
     int f = 0, c = 0, bx = 0, by = 0;
     if (live) {
         f = find_by(n, [&](int k) { return fr[k].blk0; }, g);
         c = block_place(fr[f], g - fr[f].blk0, bx, by);
-        idct_column(coef + g * 64, tabs[f].q[c], t, ws[lb]);
+        const bool ac = __any_sync(0xffu << (threadIdx.x & 24), idct_column_ac(coef + g * 64, t));
+        idct_column(coef + g * 64, tabs[f].q[c], t, !ac, ws[lb]);
     }
     __syncthreads();
     if (!live) return;

@@ -10,7 +10,9 @@ Annex K tables for slots 0 / 1 without DHT, EXIF orientation.  The steps:
   entropy data   T.81 F.2.2: 0xFF 0x00 is a data 0xFF, a run of 0xFF fill bytes before a marker is dropped, RSTn ends a
                  restart interval (DC predictions reset, the next interval starts byte-aligned)
   dequantise     the coefficient x quantiser product taken modulo 2^16 (libjpeg-turbo's SIMD IDCT multiplies in 16-bit lanes)
-  IDCT           libjpeg's islow (jidctint.c): CONST_BITS 13, PASS1_BITS 2, columns first, + 128, clamped to [0, 255]
+  IDCT           libjpeg's islow (jidctint.c): CONST_BITS 13, PASS1_BITS 2, columns first, with the 16-bit steps of
+                 libjpeg-turbo's SIMD code (idct_islow): the DC-only column shortcut, pairwise sums modulo 2^16, an int16
+                 saturation between the passes, then clamped to [-128, 127] and + 128
   upsampling     libjpeg's fancy upsampling (jdsample.c) with the real downsampled width and height replicated at the edges;
                  a chroma plane at most 2 samples wide is replicated instead (jdsample.c uses the fancy path above that)
   colour         jdcolor.c's YCbCr -> RGB tables with 16 fraction bits, written as BGR; 1 component is replicated to B = G = R
@@ -252,30 +254,66 @@ def _c(x):
     return int(x * 8192 + 0.5)
 
 
-def _idct_1d(d, shift):
-    """One islow pass along axis 1 of d (n, 8, ...) in int64, descaled by shift."""
+def _s16(x):
+    return ((x + 32768) & 0xFFFF) - 32768
+
+
+def _idct_1d(d, shift, sums, saturate):
+    """One islow pass along axis 1 of d (n, 8, ...) in int64, descaled by shift.  ``sums`` names the pairwise sums taken
+    modulo 2^16: "even" (d0 + d4, d0 - d4), "odd" (d7 + d3, d5 + d1) and "rotation" (d2 + d6, d7 + d1, d5 + d3, which
+    libjpeg-turbo's SIMD code folds into 32-bit multiply-adds).  ``saturate``: the output is saturated to int16."""
+    w = {k: (_s16 if k in sums else (lambda x: x)) for k in ("even", "odd", "rotation")}
     z2, z3 = d[:, 2], d[:, 6]
-    z1 = (z2 + z3) * _c(0.541196100)
+    z1 = w["rotation"](z2 + z3) * _c(0.541196100)
     t2, t3 = z1 - z3 * _c(1.847759065), z1 + z2 * _c(0.765366865)
-    t0, t1 = (d[:, 0] + d[:, 4]) * 8192, (d[:, 0] - d[:, 4]) * 8192
+    t0, t1 = w["even"](d[:, 0] + d[:, 4]) * 8192, w["even"](d[:, 0] - d[:, 4]) * 8192
     t10, t13, t11, t12 = t0 + t3, t0 - t3, t1 + t2, t1 - t2
     o0, o1, o2, o3 = d[:, 7], d[:, 5], d[:, 3], d[:, 1]
-    z1, z2, z3, z4 = o0 + o3, o1 + o2, o0 + o2, o1 + o3
+    z1, z2, z3, z4 = w["rotation"](o0 + o3), w["rotation"](o1 + o2), w["odd"](o0 + o2), w["odd"](o1 + o3)
     z5 = (z3 + z4) * _c(1.175875602)
     o0, o1, o2, o3 = o0 * _c(0.298631336), o1 * _c(2.053119869), o2 * _c(3.072711026), o3 * _c(1.501321110)
     z1, z2 = z1 * -_c(0.899976223), z2 * -_c(2.562915447)
     z3, z4 = z3 * -_c(1.961570560) + z5, z4 * -_c(0.390180644) + z5
     o0, o1, o2, o3 = o0 + z1 + z3, o1 + z2 + z4, o2 + z2 + z3, o3 + z1 + z4
     out = np.stack([t10 + o3, t11 + o2, t12 + o1, t13 + o0, t13 - o0, t12 - o1, t11 - o2, t10 - o3], 1)
-    return (out + (1 << (shift - 1))) >> shift
+    if np.abs(d).max(initial=0) <= 32768:                   # int16 inputs: the SIMD code's 32-bit sums never overflow
+        assert np.abs(out).max(initial=0) < 2**31 - 2**17
+    out = (out + (1 << (shift - 1))) >> shift
+    return np.clip(out, -32768, 32767) if saturate else out
 
 
-def idct_islow(coef: np.ndarray, q: np.ndarray) -> np.ndarray:
-    """(n, 64) natural-order coefficients -> (n, 8, 8) samples."""
-    deq = ((coef * q + 32768) & 0xFFFF) - 32768        # 16-bit product
-    cols = _idct_1d(deq.reshape(-1, 8, 8), 11)          # along rows index: columns first
-    rows = _idct_1d(cols.transpose(0, 2, 1), 18).transpose(0, 2, 1)
-    return np.clip(rows + 128, 0, 255)
+# The model of cv2's IDCT, step by step; each keyword of idct_islow names one step, and the values other than these are the
+# alternatives tests/test_jpeg_decode_range_cpu.py shows cv2 does not take.
+IDCT_MODEL = dict(dequant="wrap", shortcut="coef", pass1_sums=("even", "odd"), pass2_sums=("even", "odd"), between="saturate",
+                  final="saturate")
+
+
+def idct_islow(coef: np.ndarray, q: np.ndarray, **steps) -> np.ndarray:
+    """(n, 64) natural-order coefficients -> (n, 8, 8) samples, as libjpeg-turbo's SIMD islow IDCT computes them (x86-64):
+      dequant   "wrap": the coefficient x quantiser product modulo 2^16 (16-bit lane multiplies); "exact"
+      shortcut  "coef": a block whose coefficient rows 1..7 are all zero skips the column pass, and every workspace row is
+                row 0's dequantised value shifted left by PASS1_BITS modulo 2^16; "product": the same, decided on the
+                dequantised values; None: no shortcut
+      pass1_sums, pass2_sums   the pairwise sums each pass takes modulo 2^16 (see _idct_1d)
+      between   "saturate": the column pass output saturated to int16 (a saturating pack); "wrap": modulo 2^16; None: exact
+      final     "saturate": clamped to [-128, 127], + 128; "wrap": the low 8 bits, + 128
+    """
+    s = dict(IDCT_MODEL, **steps)
+    coef = np.asarray(coef, np.int64).reshape(-1, 64)
+    deq = coef * np.asarray(q, np.int64).reshape(64)
+    if s["dequant"] == "wrap":
+        deq = _s16(deq)
+    d = deq.reshape(-1, 8, 8)
+    ws = _idct_1d(d, 11, s["pass1_sums"], s["between"] == "saturate")          # along the rows index: columns first
+    if s["between"] == "wrap":
+        ws = _s16(ws)
+    if s["shortcut"]:
+        dc_only = ~(coef if s["shortcut"] == "coef" else deq).reshape(-1, 8, 8)[:, 1:].any(axis=(1, 2))
+        ws[dc_only] = np.repeat(_s16(d[dc_only, :1] * 4), 8, axis=1)
+    rows = _idct_1d(ws.transpose(0, 2, 1), 18, s["pass2_sums"], True).transpose(0, 2, 1)
+    if s["final"] == "wrap":
+        return ((rows + 128) & 0xFF)
+    return np.clip(rows, -128, 127) + 128
 
 
 def _upsample(p: np.ndarray, hs: int, vs: int, H: int, W: int) -> np.ndarray:
@@ -308,7 +346,10 @@ def _orient(img: np.ndarray, o: int) -> np.ndarray:
             5: t, 6: lambda a: t(a)[:, ::-1], 7: lambda a: t(a)[::-1, ::-1], 8: lambda a: t(a)[::-1]}[o](img)
 
 
-def decode(data: bytes) -> np.ndarray:
+def coefficients(data: bytes):
+    """(header, blocks): the entropy stage alone.  blocks[c] is component c's (rows, cols, 64) int64 grid of quantised
+    coefficients in natural order over whole MCUs, DC as the running prediction taken modulo 2^16 (libjpeg keeps it in an
+    int and stores it as a 16-bit JCOEF)."""
     h = parse(data)
     H, W, comps, hs, vs = h["H"], h["W"], h["comps"], h["hs"], h["vs"]
     nc = len(comps)
@@ -329,13 +370,24 @@ def decode(data: bytes) -> np.ndarray:
     zz[:, 0] = ((zz[:, 0] + 32768) & 0xFFFF) - 32768
     nat = np.zeros_like(zz)
     nat[:, ZIGZAG] = zz
-    planes = []
+    blocks = []
     for c in range(nc):
         h_c, v_c = (hs, vs) if c == 0 else (1, 1)
-        idx = np.nonzero(comp_of == c)[0]
-        px = idct_islow(nat[idx], h["q"][c])             # scan order: MCU rows, MCUs, then the component's v x h blocks
-        px = px.reshape(mcuy, mcux, v_c, h_c, 8, 8).transpose(0, 2, 4, 1, 3, 5).reshape(mcuy * v_c * 8, mcux * h_c * 8)
-        planes.append(px)
+        b = nat[comp_of == c]                            # scan order: MCU rows, MCUs, then the component's v x h blocks
+        blocks.append(b.reshape(mcuy, mcux, v_c, h_c, 64).transpose(0, 2, 1, 3, 4).reshape(mcuy * v_c, mcux * h_c, 64))
+    return h, blocks
+
+
+def decode(data: bytes, **idct_steps) -> np.ndarray:
+    """The BGR frame; ``idct_steps`` replace steps of the IDCT model (see idct_islow)."""
+    h, blocks = coefficients(data)
+    H, W, hs, vs = h["H"], h["W"], h["hs"], h["vs"]
+    nc = len(blocks)
+    planes = []
+    for c, b in enumerate(blocks):
+        rows, cols = b.shape[:2]
+        px = idct_islow(b.reshape(-1, 64), h["q"][c], **idct_steps)
+        planes.append(px.reshape(rows, cols, 8, 8).transpose(0, 2, 1, 3).reshape(rows * 8, cols * 8))
     Y = planes[0][:H, :W]
     if nc == 1:
         bgr = np.stack([Y, Y, Y], -1)

@@ -163,9 +163,10 @@ def test_dump_short_subsequences(dump_tool, tmp_path, bits):
     assert_equal_cv2(dump_tool, tmp_path, files, bits)
 
 
-def test_dump_corrupt_files(dump_tool, tmp_path):
+def test_dump_corrupt_files_equal_cv2(dump_tool, tmp_path):
     """Seeded byte flips and truncations: each ends in a frame, a status or a refused header, never a sanitizer report, and
-    every decoded frame but one known case equals cv2's (the set is pinned, so a new divergence fails)."""
+    every decoded frame equals cv2's.  Variant 91's flipped byte leaves luma DC values up to 1555 (12440 dequantised) in
+    blocks without AC rows, which only the 16-bit IDCT steps of DESIGN.md section 8.10 decode as cv2 does."""
     rng = np.random.default_rng(7)
     bases = [encode(frame("noise", 37, 53), 75), encode(frame("gradient", 64, 80), 50, "422", rst=2),
              encode(frame("noise", 24, 24), 95, "gray"), open(os.path.join(GOLDEN, SAMPLES[0]), "rb").read()]
@@ -187,7 +188,7 @@ def test_dump_corrupt_files(dump_tool, tmp_path):
             if ref is None or not np.array_equal(res[1], ref):
                 differ.append(k)
     assert {"status", "ok", "einval"} <= kinds
-    assert ok == 66 and differ == [91], (ok, differ)      # the one known divergence: DESIGN.md section 8.10
+    assert ok == 66 and differ == [], (ok, differ)
 
 
 def fill_and_trailing_segments(jpeg):

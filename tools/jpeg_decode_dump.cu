@@ -119,8 +119,10 @@ static int decode(const std::vector<uint8_t>& file, const Header& h, int S, std:
     for (long long g = 0; g < fr.nblk; ++g) {
         int bx, by;
         const int c = block_place(fr, g, bx, by);
-        int ws[64];
-        for (int col = 0; col < 8; ++col) idct_column(coef.data() + g * 64, h.t.q[c], col, ws);
+        int16_t ws[64];
+        bool ac = false;
+        for (int col = 0; col < 8; ++col) ac |= idct_column_ac(coef.data() + g * 64, col);
+        for (int col = 0; col < 8; ++col) idct_column(coef.data() + g * 64, h.t.q[c], col, !ac, ws);
         for (int row = 0; row < 8; ++row) idct_row(ws, row, pl.data() + fr.plane0[c] + ((size_t)by * 8 + row) * fr.pw[c] + (size_t)bx * 8);
     }
     out.assign((size_t)fr.oH * fr.oW * 3, 0);
