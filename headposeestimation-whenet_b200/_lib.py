@@ -24,7 +24,7 @@ EXPORTS = [
     "whenet_debug_text_segments", "whenet_debug_label_text",
     "whenet_encode_jpeg_u8", "whenet_encode_jpeg_ragged_u8", "whenet_debug_jpeg_header",
     "whenet_encode_jpeg_ex_u8", "whenet_debug_jpeg_header_ex", "whenet_debug_jpeg_optimal_table", "whenet_debug_jpeg_optimal_table_gpu",
-    "whenet_jpeg_info", "whenet_decode_jpeg_u8", "whenet_debug_jpeg_piece_bits",
+    "whenet_jpeg_info", "whenet_decode_jpeg_u8", "whenet_debug_jpeg_piece_bits", "whenet_jpeg_info_ex", "whenet_decode_jpeg_ex_u8",
 ]
 
 # pixel_format -> the ABI's yuv_layout (WHENET_YUV_NV12 / WHENET_YUV_I420); "bgr" is packed 8-bit BGR, the *_u8 entries
@@ -111,6 +111,8 @@ def load():
     L.whenet_jpeg_info.argtypes = [P, C.c_int64, P, C.c_char_p, C.c_int]
     L.whenet_decode_jpeg_u8.argtypes = [P, P, P, C.c_int, P, P]
     L.whenet_debug_jpeg_piece_bits.argtypes = [P, C.c_int]
+    L.whenet_jpeg_info_ex.argtypes = [P, C.c_int64, C.c_int, C.c_int, P, C.c_char_p, C.c_int]
+    L.whenet_decode_jpeg_ex_u8.argtypes = [P, P, P, C.c_int, C.c_int, C.c_int, P, P]
     L.whenet_synchronize.argtypes = [P]
     L.whenet_host_alloc.argtypes = [C.c_size_t]
     L.whenet_host_alloc.restype = P

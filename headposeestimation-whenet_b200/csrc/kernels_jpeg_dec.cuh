@@ -14,6 +14,9 @@
 //                                                          predecessor's end state until no state changes
 //   jd_check_kernel / jd_write_kernel                      per-interval block counts; coefficients written in natural order
 //   jd_idct_kernel / jd_color_kernel                       dequantise + islow IDCT; fancy upsampling, YCbCr->BGR, orientation
+// The reduced and gray modes (cv2's IMREAD_REDUCED_* and IMREAD_GRAYSCALE, DESIGN.md section 8.13) share every stage up to the
+// coefficients; jd_idct_kernel<true> stores each component at its own IDCT size (8, 4, 2 or 1 samples square) and
+// jd_color_kernel<kColorScaled / kColorGray> converts those planes.
 #pragma once
 #include <cstdint>
 #include <cstring>
@@ -79,7 +82,15 @@ struct DecFrame {
     long long blk0, nblk;   // first block in the call; blocks
     long long plane0[3];    // component planes in the call's plane buffer
     long long pix0;         // first coded pixel in the call
-    uint8_t* out;           // oH x oW x 3 BGR
+    uint8_t* out;           // oH x oW x 3 BGR (x 1 in gray mode)
+};
+
+struct DecScaled {          // what the reduced and gray modes add to a DecFrame (frame_scaled)
+    int sc[3];              // IDCT size of each component: 8, 4, 2 or 1
+    int dH, dW;             // decoded size before the orientation: ceil(H / d) x ceil(W / d)
+    int gray;               // the luma plane alone, oH x oW x 1
+    int uh, uv;             // chroma upsampling factors (1 or 2) from its plane to dH x dW
+    int cw, ch;             // chroma plane extent; cw = 1 where libjpeg replicates instead of fancy upsampling
 };
 
 struct Piece {              // one subsequence: frame-local bit range [start, end) of interval iv (call-wide), which ends at iend
@@ -244,6 +255,93 @@ JD_HD void idct_row(const int16_t* ws, int row, uint8_t* out) {
     for (int i = 0; i < 8; ++i) out[i] = (uint8_t)(v[i] < -128 ? 0 : v[i] > 127 ? 255 : v[i] + 128);
 }
 
+// libjpeg's reduced IDCTs (jidctred.c: jpeg_idct_4x4, jpeg_idct_2x2, jpeg_idct_1x1), columns first, with the 16- and 32-bit
+// steps of libjpeg-turbo's SSE2 versions, which cv2.imdecode runs (oracle/jpeg_scaled_decode_oracle.py pins each one):
+//   - the coefficient x quantiser product is taken modulo 2^16;
+//   - every multiply-add sum and its rounding constant are taken modulo 2^32 (each product of an int16 and a constant fits
+//     an int32, so unsigned sums give the SIMD lanes' result), then shifted arithmetically;
+//   - 4x4: a block whose coefficient rows 1, 2, 3, 5, 6, 7 are all zero skips the column pass (every workspace row is the
+//     dequantised row 0 shifted left by PASS1_BITS modulo 2^16); otherwise the column pass saturates to int16;
+//   - 2x2: columns 1, 3, 5, 7 of the column pass saturate to int16, column 0 stays 32-bit, and its row-pass even term
+//     (<< 15) is taken modulo 2^32;
+//   - the row pass saturates to int16, then clamps to [-128, 127] and adds 128.
+// 4x4 reads no coefficient of row or column 4; 2x2 reads only rows and columns 0, 1, 3, 5 and 7.
+JD_HD int desc32(uint32_t sum, int shift) { return (int)(sum + (1u << (shift - 1))) >> shift; }
+JD_HD int16_t sat16(int v) { return (int16_t)(v < -32768 ? -32768 : v > 32767 ? 32767 : v); }
+JD_HD uint8_t clamp_sample(int v) { return (uint8_t)(v < -128 ? 0 : v > 127 ? 255 : v + 128); }
+
+// 1-D 4-point transform of d[0], d[s], ... d[7 s] (index 4 unused) -> 4 descaled int32 outputs
+template <typename In, typename F>
+JD_HD void idct4_pass(const In* d, int s, int shift, F load, int* o) {
+    const uint32_t t0 = (uint32_t)(load(d[0], 0) * 16384);
+    const uint32_t t2 = (uint32_t)(load(d[2 * s], 2) * 15137) - (uint32_t)(load(d[6 * s], 6) * 6270);
+    const int z1 = load(d[7 * s], 7), z2 = load(d[5 * s], 5), z3 = load(d[3 * s], 3), z4 = load(d[s], 1);
+    const uint32_t o0 = (uint32_t)(z2 * 11893) + (uint32_t)(z4 * 8697) - (uint32_t)(z1 * 1730) - (uint32_t)(z3 * 17799);
+    const uint32_t o2 = (uint32_t)(z3 * 7373) + (uint32_t)(z4 * 20995) - (uint32_t)(z1 * 4176) - (uint32_t)(z2 * 4926);
+    o[0] = desc32(t0 + t2 + o2, shift);
+    o[1] = desc32(t0 - t2 + o0, shift);
+    o[2] = desc32(t0 - t2 - o0, shift);
+    o[3] = desc32(t0 + t2 - o2, shift);
+}
+// the 2-point odd part of d[s], d[3 s], d[5 s], d[7 s]
+template <typename In, typename F>
+JD_HD uint32_t idct2_odd(const In* d, int s, F load) {
+    return (uint32_t)(load(d[5 * s], 5) * 6967) + (uint32_t)(load(d[s], 1) * 29692) - (uint32_t)(load(d[7 * s], 7) * 5906) -
+           (uint32_t)(load(d[3 * s], 3) * 10426);
+}
+
+// rows 1, 2, 3, 5, 6, 7 of column `col` hold a non-zero coefficient (no block with one takes the 4x4 shortcut)
+JD_HD bool idct4_column_ac(const int16_t* coef, int col) {
+    return (coef[8 + col] | coef[16 + col] | coef[24 + col] | coef[40 + col] | coef[48 + col] | coef[56 + col]) != 0;
+}
+// column `col` (not 4) of a block -> ws[col], ws[8 + col], ws[16 + col], ws[24 + col]
+JD_HD void idct4_column(const int16_t* coef, const uint16_t* q, int col, bool dc_only, int16_t* ws) {
+    auto deq = [&](int16_t c, int row) { return s16(c * q[row * 8 + col]); };
+    if (dc_only) {
+        const int16_t v = (int16_t)(deq(coef[col], 0) * 4);
+        for (int r = 0; r < 4; ++r) ws[r * 8 + col] = v;
+        return;
+    }
+    int o[4];
+    idct4_pass(coef + col, 8, 13 - 2 + 1, deq, o);
+    for (int r = 0; r < 4; ++r) ws[r * 8 + col] = sat16(o[r]);
+}
+// row `row` (0..3) of the workspace -> 4 samples
+JD_HD void idct4_row(const int16_t* ws, int row, uint8_t* out) {
+    int o[4];
+    idct4_pass(ws + row * 8, 1, 13 + 2 + 3 + 1, [](int16_t x, int) { return (int)x; }, o);
+    for (int i = 0; i < 4; ++i) out[i] = clamp_sample(sat16(o[i]));
+}
+// column `col` (0, 1, 3, 5 or 7) -> rows 0 and 1 of the workspace.  Column 0 keeps its 32-bit value, stored as two halves in
+// columns 2 (low) and 4 (high), which the 2x2 IDCT never reads.
+JD_HD void idct2_column(const int16_t* coef, const uint16_t* q, int col, int16_t* ws) {
+    auto deq = [&](int16_t c, int row) { return s16(c * q[row * 8 + col]); };
+    const uint32_t t10 = (uint32_t)(deq(coef[col], 0) * 32768), od = idct2_odd(coef + col, 8, deq);
+    const int v[2] = {desc32(t10 + od, 13 - 2 + 2), desc32(t10 - od, 13 - 2 + 2)};
+    for (int r = 0; r < 2; ++r) {
+        if (col) {
+            ws[r * 8 + col] = sat16(v[r]);
+        } else {
+            ws[r * 8 + 2] = (int16_t)(uint16_t)(uint32_t)v[r];
+            ws[r * 8 + 4] = (int16_t)(uint16_t)((uint32_t)v[r] >> 16);
+        }
+    }
+}
+JD_HD void idct2_row(const int16_t* ws, int row, uint8_t* out) {
+    const int16_t* w = ws + row * 8;
+    const uint32_t c0 = (uint32_t)(uint16_t)w[2] | (uint32_t)(uint16_t)w[4] << 16;
+    const uint32_t e = c0 << 15, od = idct2_odd(w, 1, [](int16_t x, int) { return (int)x; });
+    out[0] = clamp_sample(sat16(desc32(e + od, 13 + 2 + 3 + 2)));
+    out[1] = clamp_sample(sat16(desc32(e - od, 13 + 2 + 3 + 2)));
+}
+// DC only: (DC x q + 4) >> 3 through libjpeg's 1024-entry range-limit table (jdmaster.c, index masked by RANGE_MASK); the
+// quantiser is a signed 16-bit multiplier there
+JD_HD uint8_t idct1(const int16_t* coef, const uint16_t* q) {
+    const int v = ((int)coef[0] * (int)(int16_t)q[0] + 4) >> 3;
+    const int i = v & 1023;
+    return (uint8_t)(i < 128 ? i + 128 : i < 512 ? 255 : i < 896 ? 0 : i - 896);
+}
+
 // one chroma sample at coded pixel (y, x) with libjpeg's fancy upsampling; the plane's real extent is cw x ch, replicated.
 // libjpeg upsamples a chroma plane of width <= 2 by plain replication instead (jdsample.c).
 JD_HD int chroma_at(const uint8_t* p, int pw, int cw, int ch, int hs, int vs, int y, int x) {
@@ -293,6 +391,16 @@ JD_HD void pixel_bgr(const DecFrame& fr, const uint8_t* planes, int y, int x, ui
     const int cw = (fr.W + fr.hs - 1) / fr.hs, ch = (fr.H + fr.vs - 1) / fr.vs;
     const int cb = chroma_at(planes + fr.plane0[1], fr.pw[1], cw, ch, fr.hs, fr.vs, y, x);
     const int cr = chroma_at(planes + fr.plane0[2], fr.pw[2], cw, ch, fr.hs, fr.vs, y, x);
+    ycc_bgr(yv, cb, cr, o);
+}
+
+// the BGR pixel of decoded position (y, x) of a reduced frame: chroma without upsampling, or h2v1 / h2v2 (fancy, or replicated
+// where cw says so)
+JD_HD void pixel_bgr_scaled(const DecFrame& fr, const DecScaled& z, const uint8_t* planes, int y, int x, uint8_t* o) {
+    const int yv = planes[fr.plane0[0] + (size_t)y * fr.pw[0] + x];
+    if (fr.ncomp == 1) { o[0] = o[1] = o[2] = (uint8_t)yv; return; }
+    const int cb = chroma_at(planes + fr.plane0[1], fr.pw[1], z.cw, z.ch, z.uh, z.uv, y, x);
+    const int cr = chroma_at(planes + fr.plane0[2], fr.pw[2], z.cw, z.ch, z.uh, z.uv, y, x);
     ycc_bgr(yv, cb, cr, o);
 }
 
@@ -569,6 +677,36 @@ inline void frame_of(const Header& h, DecFrame& f) {
     }
 }
 
+// the reduced / gray frame of a parsed header: 1 / d scale (d = 1, 2, 4, 8), colour or gray.  libjpeg's
+// jpeg_core_output_dimensions rule (jdmaster.c): the luma IDCT is m = 8 / d square; a chroma component's doubles from m while
+// it stays <= 8 and both the luma's sampling factors times m divide by twice it.  libjpeg turns fancy upsampling off at m = 1.
+inline void frame_scaled(const Header& h, int d, bool gray, DecFrame& f, DecScaled& z) {
+    frame_of(h, f);
+    memset(&z, 0, sizeof(z));
+    const int m = 8 / d;
+    z.dH = (h.H + d - 1) / d;
+    z.dW = (h.W + d - 1) / d;
+    if (h.orient >= 5) { f.oH = z.dW; f.oW = z.dH; } else { f.oH = z.dH; f.oW = z.dW; }
+    z.gray = gray;
+    z.sc[0] = m;
+    for (int c = 1; c < h.ncomp; ++c) {
+        int s = m;
+        while (s < 8 && (h.hs * m) % (2 * s) == 0 && (h.vs * m) % (2 * s) == 0) s *= 2;
+        z.sc[c] = s;
+    }
+    for (int c = 0; c < h.ncomp; ++c) {
+        f.pw[c] = h.mcux * (c ? 1 : h.hs) * z.sc[c];
+        f.ph[c] = h.mcuy * (c ? 1 : h.vs) * z.sc[c];
+    }
+    if (h.ncomp == 3) {
+        z.uh = h.hs * m / z.sc[1];
+        z.uv = h.vs * m / z.sc[1];
+        z.cw = (z.dW + z.uh - 1) / z.uh;
+        z.ch = (z.dH + z.uv - 1) / z.uv;
+        if (m == 1) z.cw = 1;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------- unstuffing (GPU)
 JD_HD bool is_rst(int b) { return b >= 0xD0 && b <= 0xD7; }
 
@@ -782,21 +920,52 @@ __global__ void __launch_bounds__(128) jd_write_kernel(Bufs B, long long npieces
 // ---------------------------------------------------------------------------------------------------- pixels (GPU)
 constexpr int kIdctBlocks = 32;      // blocks per CTA, 8 threads each
 
+// kScaled: each component at its IDCT size zs[f].sc[c] (8 threads per block still: columns, then rows), chroma skipped in gray
+// mode; otherwise every block 8x8 and zs is unused
+template <bool kScaled>
 __global__ void __launch_bounds__(256) jd_idct_kernel(const DecFrame* __restrict__ fr, int n, const Tables* __restrict__ tabs, long long nblocks,
-                                                      const int16_t* __restrict__ coef, uint8_t* __restrict__ planes) {
+                                                      const int16_t* __restrict__ coef, uint8_t* __restrict__ planes,
+                                                      const DecScaled* __restrict__ zs) {
     __shared__ int16_t ws[kIdctBlocks][64];
     const int lb = threadIdx.x >> 3, t = threadIdx.x & 7;
     const long long g = (long long)blockIdx.x * kIdctBlocks + lb;
-    const bool live = g < nblocks;      // the same for the 8 threads of a block
-    int f = 0, c = 0, bx = 0, by = 0;
+    bool live = g < nblocks;            // the same for the 8 threads of a block
+    int f = 0, c = 0, bx = 0, by = 0, sz = 8;
     if (live) {
         f = find_by(n, [&](int k) { return fr[k].blk0; }, g);
         c = block_place(fr[f], g - fr[f].blk0, bx, by);
-        const bool ac = __any_sync(0xffu << (threadIdx.x & 24), idct_column_ac(coef + g * 64, t));
-        idct_column(coef + g * 64, tabs[f].q[c], t, !ac, ws[lb]);
+        if (kScaled) {
+            sz = zs[f].sc[c];
+            if (c && zs[f].gray) live = false;
+        }
+        if (!kScaled || (live && sz == 8)) {
+            const bool ac = __any_sync(0xffu << (threadIdx.x & 24), idct_column_ac(coef + g * 64, t));
+            idct_column(coef + g * 64, tabs[f].q[c], t, !ac, ws[lb]);
+        } else if (live && sz == 4) {
+            const bool ac = __any_sync(0xffu << (threadIdx.x & 24), idct4_column_ac(coef + g * 64, t));
+            if (t != 4) idct4_column(coef + g * 64, tabs[f].q[c], t, !ac, ws[lb]);
+        } else if (live && sz == 2) {
+            if (t < 2 || (t & 1)) idct2_column(coef + g * 64, tabs[f].q[c], t, ws[lb]);
+        }
     }
     __syncthreads();
     if (!live) return;
+    if (kScaled && sz < 8) {
+        const DecFrame& F = fr[f];
+        uint8_t* dst = planes + F.plane0[c] + ((size_t)by * sz + t) * F.pw[c] + (size_t)bx * sz;
+        if (sz == 4 && t < 4) {
+            uint8_t v[4];
+            idct4_row(ws[lb], t, v);
+            *reinterpret_cast<uint32_t*>(dst) = v[0] | v[1] << 8 | v[2] << 16 | (uint32_t)v[3] << 24;
+        } else if (sz == 2 && t < 2) {
+            uint8_t v[2];
+            idct2_row(ws[lb], t, v);
+            *reinterpret_cast<uint16_t*>(dst) = (uint16_t)(v[0] | v[1] << 8);
+        } else if (sz == 1 && t == 0) {
+            *dst = idct1(coef + g * 64, tabs[f].q[c]);
+        }
+        return;
+    }
     uint8_t v[8];
     idct_row(ws[lb], t, v);
     const DecFrame& F = fr[f];
@@ -807,17 +976,31 @@ __global__ void __launch_bounds__(256) jd_idct_kernel(const DecFrame* __restrict
     *reinterpret_cast<uint2*>(dst) = w;
 }
 
-__global__ void __launch_bounds__(256) jd_color_kernel(const DecFrame* __restrict__ fr, int n, long long npix, const uint8_t* __restrict__ planes) {
+enum { kColorFull, kColorScaled, kColorGray };
+
+// one thread per decoded pixel: kColorFull the full-size BGR frame (zs unused), kColorScaled a reduced one (H x W is then
+// zs[f].dH x dW), kColorGray the luma plane alone into oH x oW x 1
+template <int kMode>
+__global__ void __launch_bounds__(256) jd_color_kernel(const DecFrame* __restrict__ fr, int n, long long npix, const uint8_t* __restrict__ planes,
+                                                       const DecScaled* __restrict__ zs) {
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
     if (i >= npix) return;
     const int f = find_by(n, [&](int k) { return fr[k].pix0; }, i);
     const DecFrame& F = fr[f];
     const long long l = i - F.pix0;
-    const int y = (int)(l / F.W), x = (int)(l - (long long)y * F.W);
+    const int W = kMode == kColorFull ? F.W : zs[f].dW;
+    const int y = (int)(l / W), x = (int)(l - (long long)y * W);
     uint8_t o[3];
-    pixel_bgr(F, planes, y, x, o);
+    if (kMode == kColorFull) pixel_bgr(F, planes, y, x, o);
+    else if (kMode == kColorScaled) pixel_bgr_scaled(F, zs[f], planes, y, x, o);
+    else o[0] = planes[F.plane0[0] + (size_t)y * F.pw[0] + x];
     int oy, ox;
-    orient_dst(F.orient, F.H, F.W, y, x, oy, ox);
+    if (kMode == kColorFull) orient_dst(F.orient, F.H, F.W, y, x, oy, ox);
+    else orient_dst(F.orient, zs[f].dH, zs[f].dW, y, x, oy, ox);
+    if (kMode == kColorGray) {
+        F.out[(size_t)oy * F.oW + ox] = o[0];
+        return;
+    }
     uint8_t* d = F.out + ((size_t)oy * F.oW + ox) * 3;
     d[0] = o[0]; d[1] = o[1]; d[2] = o[2];
 }

@@ -5,7 +5,8 @@
                     params) with the quality, sampling, restart, optimise and chroma-quality parameters, encoded by the
                     library's CUDA kernels (``whenet_encode_jpeg_u8``, ``whenet_encode_jpeg_ex_u8``)
   ``decode_jpeg``   JPEG files -> device BGR frames, pixel-identical to cv2.imdecode(buf, cv2.IMREAD_COLOR), decoded by the
-                    library's CUDA kernels (``whenet_decode_jpeg_u8``)
+                    library's CUDA kernels (``whenet_decode_jpeg_u8``); at 1/2, 1/4 or 1/8 scale or gray as with
+                    IMREAD_REDUCED_* and IMREAD_GRAYSCALE (``whenet_decode_jpeg_ex_u8``, section 8.13)
   ``MJPGWriter``    writes those files as an MJPG AVI: what reference demo_video.py:46-47,60 writes through
                     cv2.VideoWriter(..., fourcc 'MJPG'), without the frames leaving the GPU uncompressed
   ``MJPGReader``    reads the JPEG files of an MJPG AVI (the reference's cap.read(), demo_video.py:44,51)
@@ -173,20 +174,31 @@ def _jpeg_files(files):
     return out
 
 
-def jpeg_info(data: bytes):
-    """(H, W) of the frame ``decode_jpeg`` makes of ``data`` (after its EXIF orientation), parsed on the host without a GPU;
-    ValueError with the reason for a file outside the supported subset (DESIGN.md section 8.10)."""
+def _decode_mode(reduce, gray):
+    """(scale_denom, channels) of decode_jpeg's ``reduce`` and ``gray``, or ValueError."""
+    if isinstance(reduce, bool) or not isinstance(reduce, int) or reduce not in (1, 2, 4, 8):
+        raise ValueError("reduce must be the int 1, 2, 4 or 8, not %r" % (reduce,))
+    if not isinstance(gray, bool):
+        raise ValueError("gray must be a bool, not %r" % (gray,))
+    return reduce, 1 if gray else 3
+
+
+def jpeg_info(data: bytes, *, reduce=1):
+    """(H, W) of the frame ``decode_jpeg`` makes of ``data`` (after its EXIF orientation) at 1 / ``reduce`` scale:
+    (ceil(H / reduce), ceil(W / reduce)) as cv2.imdecode gives with IMREAD_REDUCED_*_``reduce``.  Parsed on the host without
+    a GPU; ValueError with the reason for a file outside the supported subset (DESIGN.md sections 8.10 and 8.13)."""
     import ctypes as C
     from ._lib import load
+    d, _ = _decode_mode(reduce, False)
     hw = (C.c_int32 * 2)()
     msg = C.create_string_buffer(256)
-    if load().whenet_jpeg_info(data, len(data), hw, msg, len(msg)) != 0:
+    if load().whenet_jpeg_info_ex(data, len(data), d, 3, hw, msg, len(msg)) != 0:
         raise ValueError(msg.value.decode("utf-8", "replace"))
     return int(hw[0]), int(hw[1])
 
 
-def _decode_into(whenet, files, outs, first_index=0):
-    """Decode ``files`` (bytes) into the contiguous (H, W, 3) uint8 CUDA tensors ``outs`` in groups of 64."""
+def _decode_into(whenet, files, outs, first_index=0, reduce=1, channels=3):
+    """Decode ``files`` (bytes) into the contiguous (H, W, channels) uint8 CUDA tensors ``outs`` in groups of 64."""
     import ctypes as C
     import torch
     from ._lib import WhenetError, check
@@ -202,7 +214,10 @@ def _decode_into(whenet, files, outs, first_index=0):
             dst = (C.c_void_p * k)(*[o.data_ptr() for o in outs[lo:hi]])
             status = (C.c_int32 * k)()
             try:
-                check(L.whenet_decode_jpeg_u8(whenet._h, ptrs, sizes, k, dst, status))
+                if reduce == 1 and channels == 3:
+                    check(L.whenet_decode_jpeg_u8(whenet._h, ptrs, sizes, k, dst, status))
+                else:
+                    check(L.whenet_decode_jpeg_ex_u8(whenet._h, ptrs, sizes, k, reduce, channels, dst, status))
             except WhenetError as e:
                 bad = next((i for i in range(k) if status[i]), None)
                 msg = str(e).split(": ", 1)[-1]
@@ -211,26 +226,32 @@ def _decode_into(whenet, files, outs, first_index=0):
                 raise ValueError(msg) from None
 
 
-def decode_jpeg(whenet, files) -> list:
+def decode_jpeg(whenet, files, *, reduce=1, gray=False) -> list:
     """Decode JPEG ``files`` (a list of bytes-like objects) on ``whenet``'s GPU and stream into BGR frames, each equal to
     ``cv2.imdecode(np.frombuffer(f, np.uint8), cv2.IMREAD_COLOR)``: baseline or extended-sequential Huffman, 1 or 3 components,
     4:4:4, 4:2:2 or 4:2:0, restart intervals, files without DHT, EXIF orientation applied, sides 1..16384.
 
-    Returns a list of contiguous (H_i, W_i, 3) uint8 CUDA tensors on ``whenet.device``, decoded in groups of 64 files with one
+    ``reduce`` (1, 2, 4 or 8) decodes at that fraction of the size inside the IDCT, as ``cv2.IMREAD_REDUCED_COLOR_<reduce>``
+    does: (ceil(H / reduce), ceil(W / reduce), 3) frames.  ``gray=True`` gives the luma plane alone as (H', W', 1) frames, as
+    ``cv2.IMREAD_GRAYSCALE`` (``cv2.IMREAD_REDUCED_GRAYSCALE_<reduce>`` with ``reduce``) does; ``encode_jpeg`` takes them as
+    gray frames.  DESIGN.md section 8.13.
+
+    Returns a list of contiguous (H_i, W_i, C) uint8 CUDA tensors on ``whenet.device``, decoded in groups of 64 files with one
     synchronisation each; n = 0 gives [].  Bad arguments, a file outside that subset (checked before any device work) or
     corrupt entropy-coded data raise ``ValueError`` naming the file index and the reason."""
     import torch
+    d, channels = _decode_mode(reduce, gray)
     files = _jpeg_files(files)
     if not files:
         return []
     shapes = []
     for i, f in enumerate(files):
         try:
-            shapes.append(jpeg_info(f))
+            shapes.append(jpeg_info(f, reduce=d))
         except ValueError as e:
             raise ValueError("file %d: %s" % (i, e)) from None
-    outs = [torch.empty((h, w, 3), dtype=torch.uint8, device="cuda:%d" % whenet.device) for h, w in shapes]
-    _decode_into(whenet, files, outs)
+    outs = [torch.empty((h, w, channels), dtype=torch.uint8, device="cuda:%d" % whenet.device) for h, w in shapes]
+    _decode_into(whenet, files, outs, reduce=d, channels=channels)
     return outs
 
 
@@ -594,24 +615,28 @@ class MJPGReader:
         self._next += len(out)
         return out
 
-    def read_frames(self, whenet, n=1):
+    def read_frames(self, whenet, n=1, *, reduce=1, gray=False):
         """Up to ``n`` more frames decoded on ``whenet``'s GPU into one (k, H, W, 3) uint8 CUDA tensor, or None at the end.  A
-        frame whose size differs from ``frame_size`` raises ValueError."""
+        frame whose size differs from ``frame_size`` raises ValueError.  ``reduce`` and ``gray`` are decode_jpeg's
+        (cv2.IMREAD_REDUCED_COLOR_<reduce>, cv2.IMREAD_GRAYSCALE, cv2.IMREAD_REDUCED_GRAYSCALE_<reduce>): the tensor is then
+        (k, ceil(H / reduce), ceil(W / reduce), 3 or 1), and each frame is checked against the reduced ``frame_size``."""
         import torch
+        d, channels = _decode_mode(reduce, gray)
         first = self._next
         files = self.read(n)
         if not files:
             return None
         w, h = self.frame_size
+        w, h = -(-w // d), -(-h // d)
         for i, f in enumerate(files):
             try:
-                hw = jpeg_info(f)
+                hw = jpeg_info(f, reduce=d)
             except ValueError as e:
                 raise ValueError("frame %d: %s" % (first + i, e)) from None
             if hw != (h, w):
                 raise ValueError("frame %d is %dx%d, the stream's frame_size %dx%d" % (first + i, hw[1], hw[0], w, h))
-        out = torch.empty((len(files), h, w, 3), dtype=torch.uint8, device="cuda:%d" % whenet.device)
-        _decode_into(whenet, files, list(out), first_index=first)
+        out = torch.empty((len(files), h, w, channels), dtype=torch.uint8, device="cuda:%d" % whenet.device)
+        _decode_into(whenet, files, list(out), first_index=first, reduce=d, channels=channels)
         return out
 
     def close(self):

@@ -314,6 +314,14 @@ int whenet_jpeg_info(const uint8_t* data, int64_t len, int32_t* hw_out, char* ms
    grows with the call and is freed with the context. */
 int whenet_decode_jpeg_u8(whenet_ctx* ctx, const uint8_t* const* files, const int64_t* sizes, int n, uint8_t* const* out_frames,
                           int32_t* status_out);
+/* Reduced and gray decoding (DESIGN.md section 8.13): scale_denom 1, 2, 4 or 8 and channels 3 (BGR) or 1 (the luma plane),
+   pixel-identical to cv2.imdecode with IMREAD_REDUCED_COLOR_d / IMREAD_REDUCED_GRAYSCALE_d (IMREAD_COLOR / IMREAD_GRAYSCALE at
+   d = 1).  whenet_jpeg_info_ex gives hw_out = (ceil(H / d), ceil(W / d)) after the orientation; whenet_decode_jpeg_ex_u8 writes
+   H_i x W_i x channels frames of that size.  Otherwise as whenet_jpeg_info / whenet_decode_jpeg_u8, which are the (1, 3)
+   case; a scale_denom or channels outside those sets is WHENET_EINVAL before any device call. */
+int whenet_jpeg_info_ex(const uint8_t* data, int64_t len, int scale_denom, int channels, int32_t* hw_out, char* msg, int cap);
+int whenet_decode_jpeg_ex_u8(whenet_ctx* ctx, const uint8_t* const* files, const int64_t* sizes, int n, int scale_denom,
+                             int channels, uint8_t* const* out_frames, int32_t* status_out);
 /* Bits per subsequence of the self-synchronising Huffman decode, 32..65536, or 0 for the default (2048). */
 int whenet_debug_jpeg_piece_bits(whenet_ctx* ctx, int bits);
 
