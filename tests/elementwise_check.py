@@ -40,6 +40,20 @@ def tap_reader(m):
     return get
 
 
+TAP_NAMES = ["stem", "head", "pooled"] + ["%s%d" % (k, i) for i in range(1, 17) for k in ("dw", "dwg", "gate", "block")]
+
+
+def read_taps(m, k):
+    """Every tap the last forward of m wrote, as (k crops, elements per crop)."""
+    get = tap_reader(m)
+    out = {}
+    for name in TAP_NAMES:
+        v = get(name)
+        if v is not None:
+            out[name] = v.reshape(k, -1)
+    return out
+
+
 def check(route, kind, name, got, ref, b, shape, store, stats):
     got = got.reshape(shape).astype(np.float64)
     assert np.isfinite(got).all(), (route, name, "non-finite values")
@@ -151,6 +165,79 @@ def check_stages(route, get, x, ang, a, oracle, blocks, stats, keep=None, projec
     print("%s: worst ratio %s; %.4f of stored elements within one ulp" %
           (route, {k: "%.3f (%s)" % v for k, v in stats.items() if not k.startswith("_")}, stats["_ulp"]))
     return stats
+
+
+# K1X instances (bf16): output tiles per crop and resident CTAs per SM, as in test_gpu_k1x_persistent.py
+K1X_TILES = {2: 49, 3: 16, 4: 16, 6: 4}
+K1X_CTAS_PER_SM = {2: 3, 3: 3, 4: 3, 6: 2}
+MAX_SEL = 16
+
+
+def halves(n):
+    """(offset, crops) of the two half batches of a two-stream pass."""
+    per = (n + 1) // 2
+    return [(0, per), (per, n - per)]
+
+
+def edge_crops(passes, sms, k1x):
+    """(kind, crop) at the schedule's edges of the given passes ((offset, crops) each), in priority order: "first" / "last"
+    crop of each pass, the last (ragged) group of four of se_gate_batch / head_fc_decode_batch ("ragged"), a crop sharing a
+    128-row K2 tile with its neighbour at 196 and 49 pixels per crop ("k2_shared"), and (bf16, k1x) the crop holding the
+    first item of each K1X block's second persistent round ("k1x_round")."""
+    out = []
+    for off, h in passes:
+        out += [("first", off), ("last", off + h - 1)]
+    for off, h in passes:
+        out.append(("ragged", off + (h - 1) // 4 * 4))
+    off0, h0 = passes[0]
+    for hw in (196, 49):
+        c = next((c for c in range(h0) if (c * hw) // 128 != ((c + 1) * hw - 1) // 128), None)
+        if c is not None:
+            out.append(("k2_shared", off0 + c))
+    if k1x:
+        for b, t in K1X_TILES.items():                        # items run crop-major: the crop holding a round's first item
+            grid = K1X_CTAS_PER_SM[b] * sms
+            for off, h in passes:
+                if h * t > grid:
+                    out.append(("k1x_round", off + grid // t))
+    return out
+
+
+def select_crops(n, sms, k1x, passes=None, kinds=None, limit=MAX_SEL):
+    """Distinct edge crops of an n-crop call (default: its two halves), in priority order, at most ``limit``; ``kinds``
+    keeps only those kinds of edge_crops."""
+    out = []
+    for kind, c in edge_crops(passes or halves(n), sms, k1x):
+        if (kinds is None or kind in kinds) and c not in out:
+            out.append(c)
+    return out[:limit]
+
+
+def taps_mismatch(big, small, store):
+    """Names of the taps (dict name -> (crops, elements)) that differ bit for bit between two runs of the same crops.  A block
+    whose depthwise output is gated in place on one side only is compared through round16(float32(d) * float32(g)), which
+    is what the in-place gate computes."""
+    bad = []
+    for i in range(1, 17):
+        for k in ("gate", "block"):
+            if not np.array_equal(big["%s%d" % (k, i)], small["%s%d" % (k, i)]):
+                bad.append("%s%d" % (k, i))
+        kb = "dwg%d" % i if "dwg%d" % i in big else "dw%d" % i
+        ks = "dwg%d" % i if "dwg%d" % i in small else "dw%d" % i
+        if kb == ks:
+            ok = np.array_equal(big[kb], small[ks])
+        else:
+            d, dg = (small[ks], big[kb]) if kb.startswith("dwg") else (big[kb], small[ks])
+            g = small["gate%d" % i]
+            k_ = d.shape[0]
+            emu = round16(d.reshape(k_, -1, g.shape[1]).astype(np.float32) * g.astype(np.float32)[:, None, :], store)
+            ok = np.array_equal(dg, emu.reshape(k_, -1))
+        if not ok:
+            bad.append("%s/%s" % (kb, ks))
+    for k in ("stem", "head", "pooled"):
+        if not np.array_equal(big[k], small[k]):
+            bad.append(k)
+    return bad
 
 
 def print_table(ratios, title):

@@ -31,10 +31,6 @@ CONFIGS = {
     "fp32_split_512": ("fp32", {"tensor_cores": 1}, 512, wb.FP32_SPLIT),
     "bf16_kd_tail_512": ("bf16", {"kd_tail": 1}, 512, wb.BF16),
 }
-# K1X instances (bf16): output tiles per crop and resident CTAs per SM, as in test_gpu_k1x_persistent.py
-K1X_TILES = {2: 49, 3: 16, 4: 16, 6: 4}
-K1X_CTAS_PER_SM = {2: 3, 3: 3, 4: 3, 6: 2}
-MAX_SEL = 16
 RATIOS = {}
 _RUNS = {}
 
@@ -42,30 +38,6 @@ _RUNS = {}
 def _sms():
     import torch
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def select_crops(n, sms, k1x):
-    """Crops at the schedule's edges, in priority order, at most MAX_SEL."""
-    per = (n + 1) // 2
-    halves = [(0, per), (per, n - per)]
-    sel = []
-    for off, h in halves:                                     # first and last crop of each half
-        sel += [off, off + h - 1]
-    for off, h in halves:                                     # the last (ragged) group of four: se_gate_batch, head_fc_decode_batch
-        sel.append(off + (h - 1) // 4 * 4)
-    for hw in (196, 49):                                      # a crop sharing a 128-row K2 tile with its neighbour
-        sel.append(next(c for c in range(per) if (c * hw) // 128 != ((c + 1) * hw - 1) // 128))
-    if k1x:
-        for b, t in K1X_TILES.items():                        # items run crop-major: the crop holding a round's first item
-            grid = K1X_CTAS_PER_SM[b] * sms
-            for off, h in halves:
-                if h * t > grid:
-                    sel.append(off + grid // t)
-    out = []
-    for c in sel:
-        if c not in out:
-            out.append(c)
-    return out[:MAX_SEL]
 
 
 def _specials():
@@ -116,26 +88,13 @@ def _forward(m, xd, n):
     return out + (names,)
 
 
-TAP_NAMES = ["stem", "head", "pooled"] + ["%s%d" % (k, i) for i in range(1, 17) for k in ("dw", "dwg", "gate", "block")]
-
-
-def _read_taps(m, k):
-    get = ec.tap_reader(m)
-    out = {}
-    for name in TAP_NAMES:
-        v = get(name)
-        if v is not None:
-            out[name] = v.reshape(k, -1)
-    return out
-
-
 def _run(config):
     """One GPU pass per configuration, shared by (a), (b) and (c)."""
     if config in _RUNS:
         return _RUNS[config]
     import torch
     prec, opts, n, _a = CONFIGS[config]
-    sel = select_crops(n, _sms(), prec == "bf16")
+    sel = ec.select_crops(n, _sms(), prec == "bf16")
     x = _batch(n, sel, 1000 + n)
     xd = torch.from_numpy(x).cuda()
     m = _model(prec, opts, n)
@@ -143,7 +102,7 @@ def _run(config):
         plain = _forward(m, xd, n)
         m.enable_taps(True, faithful=True, crops=sel)
         tapped = _forward(m, xd, n)
-        taps = _read_taps(m, len(sel))
+        taps = ec.read_taps(m, len(sel))
     finally:
         m.close()
     _RUNS[config] = dict(sel=sel, x=x[sel], plain=plain, tapped=tapped, taps=taps)
@@ -199,7 +158,7 @@ def _small_batch_taps(config, x):
     try:
         for i in range(0, len(x), 8):
             m.get_angle(x[i:i + 8])
-            for k, v in _read_taps(m, len(x[i:i + 8])).items():
+            for k, v in ec.read_taps(m, len(x[i:i + 8])).items():
                 out.setdefault(k, []).append(v)
     finally:
         m.close()
@@ -214,26 +173,7 @@ def test_taps_batch_invariant(config):
     a = CONFIGS[config][3]
     big = r["taps"]
     small = _small_batch_taps(config, r["x"])
-    bad = []
-    for i in range(1, 17):
-        for k in ("gate", "block"):
-            if not np.array_equal(big["%s%d" % (k, i)], small["%s%d" % (k, i)]):
-                bad.append("%s%d" % (k, i))
-        kb = "dwg%d" % i if "dwg%d" % i in big else "dw%d" % i
-        ks = "dwg%d" % i if "dwg%d" % i in small else "dw%d" % i
-        if kb == ks:
-            ok = np.array_equal(big[kb], small[ks])
-        else:
-            d, dg = (small[ks], big[kb]) if kb.startswith("dwg") else (big[kb], small[ks])
-            g = small["gate%d" % i]
-            k_ = d.shape[0]
-            emu = ec.round16(d.reshape(k_, -1, g.shape[1]).astype(np.float32) * g.astype(np.float32)[:, None, :], a.store)
-            ok = np.array_equal(dg, emu.reshape(k_, -1))
-        if not ok:
-            bad.append("%s/%s" % (kb, ks))
-    for k in ("stem", "head", "pooled"):
-        if not np.array_equal(big[k], small[k]):
-            bad.append(k)
+    bad = ec.taps_mismatch(big, small, a.store)
     assert not bad, (config, bad)
 
 
@@ -249,13 +189,13 @@ def test_tap_selection_and_staleness():
         m.enable_taps(True, faithful=True)
         m.forward_device(xd, ang)
         m.synchronize()
-        full = _read_taps(m, n)
+        full = ec.read_taps(m, n)
         assert all(v.shape[0] == n for v in full.values())
         sel = [69, 3, 35, 34, 0]                              # both halves (35 + 35), out of order
         m.enable_taps(True, faithful=True, crops=sel)
         m.forward_device(xd, ang)
         m.synchronize()
-        part = _read_taps(m, len(sel))
+        part = ec.read_taps(m, len(sel))
         assert sorted(part) == sorted(full)
         for k, v in part.items():
             assert np.array_equal(v, full[k][sel]), k
