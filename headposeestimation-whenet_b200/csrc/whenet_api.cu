@@ -16,6 +16,7 @@
 #include <map>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <type_traits>
 #include <vector>
 
@@ -121,9 +122,23 @@ struct BlockW {   // device pointers into the fp32 arena
 };
 
 struct K1Plan { bool valid = false; whenet::fused::K1Params p{}; int R = 0; int NT = 256; size_t smem = 0; };
+// Which operand a cached tensor map describes.  K2: activations keyed by (K, M), weights by (N, K).  KD and K1X: keyed by
+// (block, crops), or (block, 0) for weights, whose map does not depend on the batch.
+enum class TmapKind {
+    K2A, K2W,                  // K2's A and W
+    KdE, KdDw, KdIn, KdExp,    // KD's E tiles, depthwise weights, block input and expand weights (on-chip expand)
+    K1xIn, K1xExp, K1xDw,      // K1X's block input, augmented expand weights and depthwise weights
+};
 struct TmapKey {
-    int block, n; const void* ptr;
-    bool operator<(const TmapKey& o) const { return block != o.block ? block < o.block : (n != o.n ? n < o.n : ptr < o.ptr); }
+    TmapKind kind; int i, j; const void* ptr;
+    bool operator<(const TmapKey& o) const { return std::tie(kind, i, j, ptr) < std::tie(o.kind, o.i, o.j, o.ptr); }
+};
+// One pass through the net: its stream and its views of the context's workspace buffers (see pass_view)
+struct Pass {
+    cudaStream_t stream;
+    void *A, *B, *E, *D;       // block input / output (ping-pong), expanded tensor, depthwise output
+    float *partial, *gate, *pooled;
+    int* se_counter;
 };
 struct GraphKey {
     int n, in_u8, sig;
@@ -146,7 +161,7 @@ struct whenet_ctx {
     int dw_variant = 1;     // 0 = one output per thread, 1 = register-blocked strips
     int pw_variant = 4;     // tensor-core 1x1 kernel: 2 = pw_tc2 (one tile per CTA, cp.async ring), 3 = K2 (persistent, TMA, warp-specialised),
                             // 4 = per layer (launch_pw)
-    std::map<TmapKey, CUtensorMap> tmaps2;  // K2 tensor maps: activations by (K, M, pointer), weights by (-N, K, pointer)
+    std::map<TmapKey, CUtensorMap> tmaps2;  // K2 tensor maps
     int pw_stage_cap = 0, pw_smem_kb = 54, pw_min_ctas = 132;    // pw_tc2 ring: max stages (0 = up to 4) and per-CTA smem budget that trades depth for co-residency
     int stem_variant = 1;   // 0 = 4 threads / pixel straight from global, 1 = smem-tiled, weights in the constant bank
     whenet::StemParams stem_params{};
@@ -169,7 +184,7 @@ struct whenet_ctx {
     int k1x = 0;               // bf16: the blocks with a K1X instance (K1 fed by TMA, same bits) run it where a CTA holds all chunks of its tile; 0 = K1
     int kd_from = 7;           // bf16: blocks >= kd_from whose map fits one CTA run expand GEMM (fp16 E through L2) + KD; 0 = off
     std::vector<K1Plan> k1;
-    std::map<TmapKey, CUtensorMap> tmaps;   // KD tensor maps: E tiles by (100 + block, crops, buffer), depthwise weights by (200 + block, 0, pointer)
+    std::map<TmapKey, CUtensorMap> tmaps;   // KD and K1X tensor maps
     int sm_count = 132;
     K1Plan dw1;                // block 1 (no expand): depthwise-only instance of K1
     int dw1_fused = 1;
@@ -251,8 +266,9 @@ int check_timeout(whenet_ctx* c) {
 // ----------------------------------------------------------------------------- profiling helpers
 struct Scope {
     whenet_ctx* c;
+    cudaStream_t s;
     int ev = -1;
-    Scope(whenet_ctx* ctx, const char* name, double bytes, double flops) : c(ctx) {
+    Scope(whenet_ctx* ctx, cudaStream_t stream, const char* name, double bytes, double flops) : c(ctx), s(stream) {
         c->launches++;
         if (!c->prof_on) return;
         auto it = c->stat_idx.find(name);
@@ -272,12 +288,12 @@ struct Scope {
             else cudaEventCreate(e);
         }
         p.stat = si;
-        cudaEventRecord(p.a, c->stream);
+        cudaEventRecord(p.a, s);
         c->ev_used.push_back(p);
         ev = (int)c->ev_used.size() - 1;
     }
     ~Scope() {
-        if (ev >= 0) cudaEventRecord(c->ev_used[ev].b, c->stream);
+        if (ev >= 0) cudaEventRecord(c->ev_used[ev].b, s);
     }
 };
 
@@ -319,16 +335,16 @@ int prepare_taps(whenet_ctx* c, const std::vector<int>& crops) {
 }
 
 // Copy the tapped crops among [off, off + nb) of the call out of `src` (this chunk's tensor, per_crop elements per crop) into
-// their rows of tap `name`, on the chunk's stream.  `gated`: a depthwise output gated in place (read back as "dwg%d").
+// their rows of tap `name`, on the chunk's stream `s`.  `gated`: a depthwise output gated in place (read back as "dwg%d").
 template <typename T>
-int add_tap(whenet_ctx* c, const std::string& name, const T* src, size_t per_crop, int off, int nb, bool gated = false) {
+int add_tap(whenet_ctx* c, cudaStream_t s, const std::string& name, const T* src, size_t per_crop, int off, int nb, bool gated = false) {
     auto it = c->taps.find(name);
     if (it == c->taps.end() || it->second.n != c->tap_map.size() * per_crop)
         return fail(WHENET_EINVAL, "tap %s was not prepared for this forward", name.c_str());
     const auto lo = std::lower_bound(c->tap_map.begin(), c->tap_map.end(), off, [](const int2& a, int v) { return a.x < v; });
     const auto hi = std::lower_bound(c->tap_map.begin(), c->tap_map.end(), off + nb, [](const int2& a, int v) { return a.x < v; });
     if (hi > lo) {
-        whenet::tap_gather_kernel<T><<<dim3((unsigned)((per_crop + 255) / 256), (unsigned)(hi - lo)), 256, 0, c->stream>>>(
+        whenet::tap_gather_kernel<T><<<dim3((unsigned)((per_crop + 255) / 256), (unsigned)(hi - lo)), 256, 0, s>>>(
             src, it->second.p, c->d_tap_map + (lo - c->tap_map.begin()), off, (long long)per_crop);
         CK(cudaGetLastError());
         it->second.forms |= gated ? 2 : 1;
@@ -388,8 +404,20 @@ int ensure_ws(whenet_ctx* c) {
     return 0;
 }
 
-// ----------------------------------------------------------------------------- TMA tensor maps (K2, KD)
-PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
+// The workspace of crops off, off + 1, ... for a pass on stream s.  A two-stream forward runs each part of the batch on its own
+// stream with its own crop range of every buffer.
+Pass pass_view(const whenet_ctx* c, int off, cudaStream_t s) {
+    const size_t es = esize(c->precision), o = (size_t)off;
+    return {s,
+            (char*)c->bufA + o * c->ws_io * es, (char*)c->bufB + o * c->ws_io * es,
+            (char*)c->bufE + o * c->ws_ex * es, (char*)c->bufD + o * c->ws_dw * es,
+            c->d_partial + o * c->ws_part, c->d_gate + o * 1152, c->d_pooled + o * 1280, c->d_se_counter + o};
+}
+
+// ----------------------------------------------------------------------------- TMA tensor maps (K2, KD, K1X)
+// cuTensorMapEncodeTiled for a dense 16-bit tensor: dims[0] is contiguous and each stride is the product of the dims before it
+int encode_tmap16(CUtensorMap* tm, const char* what, const void* base, bool is_bf16, std::initializer_list<long long> dims,
+                  std::initializer_list<int> box, CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2) {
     static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
     if (!fn) {
         void* f = nullptr;
@@ -397,133 +425,118 @@ PFN_cuTensorMapEncodeTiled_v12000 tmap_encode_fn() {
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
             fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
     }
-    return fn;
-}
-// K-major weight matrix [rows][K] (16-bit): box = {64, box_rows} in SWIZZLE_128B rows, or {32, box_rows} in SWIZZLE_64B rows
-// when row_bytes is 64
-int make_tmap_w(CUtensorMap* tm, const void* base, int rows, int K, int box_rows, bool is_bf16, int row_bytes = 128) {
-    auto fn = tmap_encode_fn();
     if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)row_bytes / 2, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(tm, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides,
-                          box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(weights %dx%d, box %d) failed: %d", rows, K, box_rows, (int)r);
+    const int rank = (int)dims.size();
+    cuuint64_t dim[4], stride[4];
+    cuuint32_t bx[4], estr[4] = {1, 1, 1, 1};
+    for (int d = 0; d < rank; ++d) {
+        dim[d] = (cuuint64_t)dims.begin()[d];
+        bx[d] = (cuuint32_t)box.begin()[d];
+        stride[d] = (d ? stride[d - 1] : 2) * dim[d];     // bytes between steps of dim d + 1
+    }
+    const CUresult r = fn(tm, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), dim,
+                          stride, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        std::string dims_s, box_s;
+        for (int d = 0; d < rank; ++d) { dims_s += " " + std::to_string(dim[d]); box_s += " " + std::to_string(bx[d]); }
+        return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(%s, dims%s, box%s) failed: %d", what, dims_s.c_str(), box_s.c_str(), (int)r);
+    }
     return 0;
 }
 
+// K-major weight matrix [rows][K] (16-bit): box = {64, box_rows} in SWIZZLE_128B rows, or {32, box_rows} in SWIZZLE_64B rows
+// when row_bytes is 64
+int make_tmap_w(CUtensorMap* tm, const void* base, int rows, int K, int box_rows, bool is_bf16, int row_bytes = 128) {
+    return encode_tmap16(tm, "K-major matrix", base, is_bf16, {K, rows}, {row_bytes / 2, box_rows},
+                         row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+}
 // KD operands (fp16, no swizzle): E [n][H][H][C] with box {cc, pw, pw, 1} (started at (-pad, -pad) the out-of-image part of the
 // box is zero-filled = TF-SAME padding), depthwise weights [kk][C] with box {cc, kk}
 int make_tmap_kd_e(CUtensorMap* tm, const void* base, int n, int H, int C, int cc, int pw) {
-    auto fn = tmap_encode_fn();
-    if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)H, (cuuint64_t)H, (cuuint64_t)n};
-    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * C * 2, (cuuint64_t)H * H * C * 2};
-    const cuuint32_t box[4] = {(cuuint32_t)cc, (cuuint32_t)pw, (cuuint32_t)pw, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(KD tile %dx%dx%dx%d, box %dx%dx%d) failed: %d", n, H, H, C, pw, pw, cc, (int)r);
-    return 0;
+    return encode_tmap16(tm, "KD tile", base, false, {C, H, H, n}, {cc, pw, pw, 1}, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+}
+int make_tmap_kd_w(CUtensorMap* tm, const void* base, int kk, int C, int cc) {
+    return encode_tmap16(tm, "KD weights", base, false, {C, kk}, {cc, kk}, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // K1X's block input (bf16) [n][H][H][C]: box {row_bytes / 2, iw, iw, 1}, SWIZZLE_128B (128-byte rows) or SWIZZLE_64B (64-byte
 // rows) - a halo tile lands as the K-major A operand, one row per pixel; channels >= C and pixels outside the image are
 // zero-filled
 int make_tmap_k1x_in(CUtensorMap* tm, const void* base, int n, int H, int C, int iw, int row_bytes) {
-    auto fn = tmap_encode_fn();
-    if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)H, (cuuint64_t)H, (cuuint64_t)n};
-    const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * C * 2, (cuuint64_t)H * H * C * 2};
-    const cuuint32_t box[4] = {(cuuint32_t)row_bytes / 2, (cuuint32_t)iw, (cuuint32_t)iw, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(K1X input %dx%dx%dx%d, box %dx%d) failed: %d", n, H, H, C, iw, iw, (int)r);
-    return 0;
+    return encode_tmap16(tm, "K1X input", base, true, {C, H, H, n}, {row_bytes / 2, iw, iw, 1},
+                         row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
-int make_tmap_kd_w(CUtensorMap* tm, const void* base, int kk, int C, int cc) {
-    auto fn = tmap_encode_fn();
-    if (!fn) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)kk};
-    const cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)cc, (cuuint32_t)kk};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(WHENET_ECUDA, "cuTensorMapEncodeTiled(KD weights %dx%d, box %d) failed: %d", kk, C, cc, (int)r);
+
+// Copy the map cached under `key` to *out, encoding it with make(&map) on a miss.  A cache holding more than `limit` maps is
+// emptied first, so that buffers of past batch sizes do not pile up.
+template <class Make>
+int cached_tmap(std::map<TmapKey, CUtensorMap>& cache, size_t limit, const TmapKey& key, CUtensorMap* out, Make make) {
+    if (cache.size() > limit) cache.clear();
+    auto it = cache.find(key);
+    if (it == cache.end()) {
+        CUtensorMap tm;
+        if (int rc = make(&tm)) return rc;
+        it = cache.emplace(key, tm).first;
+    }
+    *out = it->second;
     return 0;
 }
 
 // ----------------------------------------------------------------------------- launches
+// A 1x1 conv on stream s.  use_tc, variant: the kernel family (a forward passes the context's use_tc and pw_variant)
 template <typename T>
-int launch_pw(whenet_ctx* c, const char* name, const T* A, const float* W, const void* Wt16, const float* bias,
-              const float* gate, const T* resid, T* out, long long M, int K, int N, int hw, bool swish, bool out_half = false) {
+int launch_pw(whenet_ctx* c, cudaStream_t s, int use_tc, int variant, const char* name, const T* A, const float* W, const void* Wt16,
+              const float* bias, const float* gate, const T* resid, T* out, long long M, int K, int N, int hw, bool swish, bool out_half = false) {
     const double bytes = (double)M * (K + N + (resid ? N : 0)) * sizeof(T);
     const double flops = 2.0 * (double)M * K * N;
-    Scope sc(c, name, bytes, flops);
+    Scope sc(c, s, name, bytes, flops);
     if constexpr (sizeof(T) == 2) {
         // pw_variant 4 (default): K2 for the ungated convs (expands, head, projects whose input is already gated) and for the gated
         // projects of the small maps; pw_tc2 (per-crop gate on W) for the gated projects of blocks 1-6 and for the fp16-output
         // expands that feed KD at small batches
-        const bool want_k2 = c->pw_variant == 3 || (c->pw_variant == 4 && (gate == nullptr || hw <= 196));
-        if (c->use_tc && Wt16 && want_k2 && !out_half) {
+        const bool want_k2 = variant == 3 || (variant == 4 && (gate == nullptr || hw <= 196));
+        if (use_tc && Wt16 && want_k2 && !out_half) {
             whenet::tc::K2Params kp{};
             size_t smem = 0;
             // (the persistent kernel needs enough tiles to keep every SM busy for a while; below that pw_tc2's N split wins)
             if (whenet::tc::plan_k2(M, K, N, hw, gate != nullptr, c->precision == WHENET_PRECISION_BF16, &kp, &smem) &&
-                (c->pw_variant == 3 || kp.tiles >= 2 * c->sm_count)) {
-                if (c->tmaps2.size() > 1024) c->tmaps2.clear();
-                const TmapKey ka{K, (int)M, (const void*)A}, kw{-N, K, Wt16};
-                auto ia = c->tmaps2.find(ka);
-                if (ia == c->tmaps2.end()) {
-                    CUtensorMap tm;
-                    int rc = make_tmap_w(&tm, A, (int)M, K, whenet::tc::BM, c->precision == WHENET_PRECISION_BF16);
-                    if (rc) return rc;
-                    ia = c->tmaps2.emplace(ka, tm).first;
-                }
-                auto iw = c->tmaps2.find(kw);
-                if (iw == c->tmaps2.end()) {
-                    CUtensorMap tm;
-                    int rc = make_tmap_w(&tm, Wt16, N, K, kp.n_tile, c->precision == WHENET_PRECISION_BF16);
-                    if (rc) return rc;
-                    iw = c->tmaps2.emplace(kw, tm).first;
-                }
-                kp.tmA = ia->second; kp.tmW = iw->second;
+                (variant == 3 || kp.tiles >= 2 * c->sm_count)) {
+                const bool bf16 = c->precision == WHENET_PRECISION_BF16;
+                int rc = cached_tmap(c->tmaps2, 1024, {TmapKind::K2A, K, (int)M, A}, &kp.tmA,
+                                     [&](CUtensorMap* tm) { return make_tmap_w(tm, A, (int)M, K, whenet::tc::BM, bf16); });
+                if (!rc)
+                    rc = cached_tmap(c->tmaps2, 1024, {TmapKind::K2W, N, K, Wt16}, &kp.tmW,
+                                     [&](CUtensorMap* tm) { return make_tmap_w(tm, Wt16, N, K, kp.n_tile, bf16); });
+                if (rc) return rc;
                 kp.bias = bias; kp.gate = gate; kp.resid = resid; kp.out = out; kp.tflag = c->d_tflag;
-                int rc = whenet::tc::launch_k2<T>(c->stream, kp, smem, swish, gate != nullptr, resid != nullptr, c->sm_count);
+                rc = whenet::tc::launch_k2<T>(s, kp, smem, swish, gate != nullptr, resid != nullptr, c->sm_count);
                 if (rc == 0) { CK(cudaGetLastError()); return 0; }
                 if (rc < 0) return fail(WHENET_ECUDA, "K2 launch failed for %s (rc=%d)", name, rc);
             }
             // shape or epilogue not covered by K2 -> pw_tc2 below
         }
-        if (c->use_tc && Wt16 && gate && hw >= 784 && c->pw3 && !out_half && !swish) {
+        if (use_tc && Wt16 && gate && hw >= 784 && c->pw3 && !out_half && !swish) {
             // gated projects of the large maps: several tiles of one crop per CTA (pw_tc3; same bits as pw_tc2's per-crop route)
-            int rc = whenet::tc::launch_pw_tc3<T>(c->stream, A, Wt16, bias, gate, resid, out, M, K, N, hw);
+            int rc = whenet::tc::launch_pw_tc3<T>(s, A, Wt16, bias, gate, resid, out, M, K, N, hw);
             if (rc == 0) { CK(cudaGetLastError()); return 0; }
             if (rc < 0) return fail(WHENET_ECUDA, "pw_tc3 launch failed for %s (rc=%d)", name, rc);
         }
-        if (c->use_tc && Wt16) {
-            int rc = whenet::tc::launch_pw_tc2<T>(c->stream, A, Wt16, bias, gate, resid, out, M, K, N, hw, swish, c->pw_stage_cap, c->pw_smem_kb, c->pw_min_ctas, out_half);
+        if (use_tc && Wt16) {
+            int rc = whenet::tc::launch_pw_tc2<T>(s, A, Wt16, bias, gate, resid, out, M, K, N, hw, swish, c->pw_stage_cap, c->pw_smem_kb, c->pw_min_ctas, out_half);
             if (rc == 0) { CK(cudaGetLastError()); return 0; }
             if (rc < 0) return fail(WHENET_ECUDA, "tensor-core 1x1 launch failed for %s (rc=%d)", name, rc);
             // rc > 0: shape not supported by the tensor-core kernel -> CUDA-core kernel below
         }
     }
     if constexpr (sizeof(T) == 4) {
-        if (c->use_tc && Wt16 && c->split_lo_bytes) {
-            int rc = whenet::tc::launch_pw_tc32(c->stream, A, Wt16, (const char*)Wt16 + c->split_lo_bytes, bias, gate, resid, out, M, K, N, hw, swish);
+        if (use_tc && Wt16 && c->split_lo_bytes) {
+            int rc = whenet::tc::launch_pw_tc32(s, A, Wt16, (const char*)Wt16 + c->split_lo_bytes, bias, gate, resid, out, M, K, N, hw, swish);
             if (rc == 0) { CK(cudaGetLastError()); return 0; }
             if (rc < 0) return fail(WHENET_ECUDA, "split-bf16 tensor-core 1x1 launch failed for %s (rc=%d)", name, rc);
         }
     }
     if (out_half) return fail(WHENET_EINVAL, "fp16-output 1x1 conv needs the tensor-core kernel (%s)", name);
     dim3 grid((unsigned)((M + 63) / 64), (unsigned)((N + 63) / 64));
-#define PW(SW, GA, RE) whenet::pw_conv_kernel<T, SW, GA, RE><<<grid, 256, 0, c->stream>>>(A, W, bias, gate, resid, out, M, K, N, hw)
+#define PW(SW, GA, RE) whenet::pw_conv_kernel<T, SW, GA, RE><<<grid, 256, 0, s>>>(A, W, bias, gate, resid, out, M, K, N, hw)
     if (swish && !gate && !resid) PW(true, false, false);
     else if (!swish && gate && !resid) PW(false, true, false);
     else if (!swish && gate && resid) PW(false, true, true);
@@ -536,7 +549,7 @@ int launch_pw(whenet_ctx* c, const char* name, const T* A, const float* W, const
 }
 
 template <typename T>
-int launch_dw(whenet_ctx* c, const char* name, const BlockCfg& b, const BlockW& w, const T* in, T* out, int nb, int* tiles_out) {
+int launch_dw(whenet_ctx* c, const Pass& ps, const char* name, const BlockCfg& b, const BlockW& w, const T* in, T* out, int nb, int* tiles_out) {
     const int rows = b.hout >= 28 ? 8 : b.hout;     // output rows per CTA
     const int tiles = (b.hout + rows - 1) / rows;
     *tiles_out = tiles;
@@ -546,9 +559,9 @@ int launch_dw(whenet_ctx* c, const char* name, const BlockCfg& b, const BlockW& 
     const size_t smem = (size_t)py * b.cexp * sizeof(float);
     const double bytes = (double)nb * ((double)b.hin * b.hin + (double)b.hout * b.hout) * b.cexp * sizeof(T);
     const double flops = 2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp;
-    Scope sc(c, name, bytes, flops);
-#define DW(KS, S) whenet::dw_conv_kernel<T, KS, S><<<grid, block, smem, c->stream>>>(in, w.w_dw, w.b_dw, out, c->d_partial, b.hin, b.hout, b.cexp, b.pad, rows)
-#define DWS(KS, S, R) whenet::dw_strip_kernel<T, KS, S, R, (sizeof(T) == 2)><<<grid, block, smem, c->stream>>>(in, w.w_dw, w.b_dw, out, c->d_partial, b.hin, b.hout, b.cexp, b.pad, rows)
+    Scope sc(c, ps.stream, name, bytes, flops);
+#define DW(KS, S) whenet::dw_conv_kernel<T, KS, S><<<grid, block, smem, ps.stream>>>(in, w.w_dw, w.b_dw, out, ps.partial, b.hin, b.hout, b.cexp, b.pad, rows)
+#define DWS(KS, S, R) whenet::dw_strip_kernel<T, KS, S, R, (sizeof(T) == 2)><<<grid, block, smem, ps.stream>>>(in, w.w_dw, w.b_dw, out, ps.partial, b.hin, b.hout, b.cexp, b.pad, rows)
     if (c->dw_variant == 0) {
         if (b.k == 3 && b.s == 1) DW(3, 1);
         else if (b.k == 3 && b.s == 2) DW(3, 2);
@@ -569,315 +582,336 @@ int launch_dw(whenet_ctx* c, const char* name, const BlockCfg& b, const BlockW& 
     return 0;
 }
 
+// ----------------------------------------------------------------------------- forward: stem, block routes, SE gate, head
 template <typename T, bool IN_U8>
-int forward_chunk(whenet_ctx* c, const void* d_in, int nb, float* d_angles, float* d_logits, bool taps, int off) {
+int run_stem(whenet_ctx* c, const Pass& ps, const void* d_in, int nb, bool stem_half) {
+    T* out = (T*)ps.A;
+    Scope sc(c, ps.stream, "stem", (double)nb * (kImgElems * (IN_U8 ? 1.0 : 4.0) + 112.0 * 112 * 32 * sizeof(T)),
+             2.0 * nb * 112.0 * 112 * 27 * 32);
+    if (stem_half) {
+        // block 1's depthwise is KD (HFMA2 over an fp16 tile): the stem output, read by nothing else, is written as fp16
+        CK((whenet::launch_stem_tile<__half, IN_U8, true>(ps.stream, d_in, reinterpret_cast<__half*>(out), c->stem_params, c->lut, nb)));
+    } else if (c->stem_variant == 0) {
+        const long long total = (long long)nb * 112 * 112 * 4;
+        whenet::stem_kernel<T, IN_U8><<<(unsigned)((total + 255) / 256), 256, 0, ps.stream>>>(d_in, out, c->w_stem, c->b_stem, c->lut, nb);
+        CK(cudaGetLastError());
+    } else {
+        CK((whenet::launch_stem_tile<T, IN_U8, (sizeof(T) == 2)>(ps.stream, d_in, out, c->stem_params, c->lut, nb)));
+    }
+    return 0;
+}
+
+// What a block's depthwise route leaves for the SE gate and the project conv
+struct DwResult {
+    int tiles = 0;            // squeeze partials per crop in Pass::partial
+    bool gate_done = false;   // the route computed the SE gate itself (options se_fused / se_tail)
+    bool d_gated = false;     // ... and D already carries it
+};
+
+// Block 1, bf16, stem output in fp16: KD over 14x14 spatial tiles of the stem output (TMA, HFMA2)
+int kd_stem_tiles(whenet_ctx* c, const Pass& ps, const __nv_bfloat16* cur, int nb, DwResult* r) {
+    using T = __nv_bfloat16;
+    const BlockCfg& b = c->blocks[0];
+    const BlockW& w = c->bw[0];
+    whenet::fused::DwSeParams p{};
+    int rc = cached_tmap(c->tmaps, 512, {TmapKind::KdE, b.idx, nb, cur}, &p.tmE,
+                         [&](CUtensorMap* tm) { return make_tmap_kd_e(tm, cur, nb, b.hin, b.cexp, 32, 16); });
+    if (!rc)
+        rc = cached_tmap(c->tmaps, 512, {TmapKind::KdDw, b.idx, 0, w.w_dw16}, &p.tmW,
+                         [&](CUtensorMap* tm) { return make_tmap_kd_w(tm, w.w_dw16, 9, b.cexp, 32); });
+    if (rc) return rc;
+    p.b_dw = w.b_dw_h; p.tflag = c->d_tflag; p.out = ps.D; p.partial = ps.partial;
+    p.C = b.cexp; p.pad = b.pad; p.Cse = b.cse; p.inv_hw = 1.0f / (float)(b.hout * b.hout);
+    int split = 1;
+    {
+        const int n_tiles = (b.hin / 14) * (b.hin / 14);
+        while (split < n_tiles && (long long)nb * split < c->k1_split_ctas) ++split;
+    }
+    char nm[48];
+    snprintf(nm, sizeof nm, "b%02d.dw", b.idx);
+    Scope sc(c, ps.stream, nm, (double)nb * 2.0 * b.hin * b.hin * b.cexp * sizeof(T), 2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
+    rc = whenet::fused::launch_dwse_spatial<T>(ps.stream, p, b.hin, nb, split);
+    if (rc != 0) return fail(WHENET_ECUDA, "KD (block 1) launch failed (rc=%d)", rc);
+    CK(cudaGetLastError());
+    r->tiles = (b.hin / 14) * (b.hin / 14);
+    return 0;
+}
+
+// Late blocks, bf16 (whole map in one CTA): KD (depthwise + SE + gating, one CTA per crop).  Small batches spread one crop's
+// channel chunks over several CTAs (the gate then comes from se_gate_kernel) and read E from an expand GEMM; otherwise each CTA
+// computes its crop's expand conv on chip and E never leaves the SM.
+int kd_block(whenet_ctx* c, const Pass& ps, size_t i, const __nv_bfloat16* cur, int nb, bool plain_dw, DwResult* r) {
+    using T = __nv_bfloat16;
+    const BlockCfg& b = c->blocks[i];
+    const BlockW& w = c->bw[i];
+    T* E = (T*)ps.E;
+    char nm[48];
+    const int cc = whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp);
+    int split = 1;
+    while (split < b.cexp / cc && (long long)nb * split < c->k1_split_ctas) ++split;
+    int rc = 0;
+    if (split > 1) {
+        snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
+        rc = launch_pw<T>(c, ps.stream, c->use_tc, c->pw_variant, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, E,
+                          (long long)nb * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, true, true);
+        if (rc) return rc;
+    }
+    whenet::fused::DwSeParams p{};
+    const int pw = (b.hout - 1) * b.s + b.k;
+    rc = cached_tmap(c->tmaps, 512, {TmapKind::KdDw, b.idx, 0, w.w_dw16}, &p.tmW,
+                     [&](CUtensorMap* tm) { return make_tmap_kd_w(tm, w.w_dw16, b.k * b.k, b.cexp, cc); });
+    if (rc) return rc;
+    if (split > 1) {
+        rc = cached_tmap(c->tmaps, 512, {TmapKind::KdE, b.idx, nb, E}, &p.tmE,
+                         [&](CUtensorMap* tm) { return make_tmap_kd_e(tm, E, nb, b.hin, b.cexp, cc, pw); });
+    } else {
+        // block input [nb*H*W][Cin]: box rows = one crop's pixels rounded up to a swizzle atom; expand weights [Cexp][Cin]
+        rc = cached_tmap(c->tmaps, 512, {TmapKind::KdIn, b.idx, nb, cur}, &p.tmX,
+                         [&](CUtensorMap* tm) { return make_tmap_w(tm, cur, nb * b.hin * b.hin, b.cin, (b.hin * b.hin + 7) / 8 * 8, true); });
+        if (!rc)
+            rc = cached_tmap(c->tmaps, 512, {TmapKind::KdExp, b.idx, 0, w.wt_exp}, &p.tmWx,
+                             [&](CUtensorMap* tm) { return make_tmap_w(tm, w.wt_exp, b.cexp, b.cin, cc, true); });
+        p.b_exp = w.b_exp;
+    }
+    if (rc) return rc;
+    p.b_dw = w.b_dw_h; p.tflag = c->d_tflag;
+    p.out = ps.D; p.partial = ps.partial;
+    p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = ps.gate; p.Cse = b.cse;
+    p.inv_hw = 1.0f / (float)(b.hout * b.hout);
+    p.C = b.cexp; p.pad = b.pad;
+    if (split == 1 && c->se_tail && c->kd_tail) {
+        p.se_tail = 1;
+        r->gate_done = true;
+        if (c->se_scale_out && !plain_dw) { p.scale_out = 1; r->d_gated = true; }
+    }
+    snprintf(nm, sizeof nm, "b%02d.kd", b.idx);
+    if (split == 1) {
+        Scope sc(c, ps.stream, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
+                 2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
+        rc = whenet::fused::launch_dwse_x<T>(ps.stream, p, b.k, b.s, b.hin, b.cin, nb);
+        if (rc != 0) return fail(WHENET_ECUDA, "KD (on-chip expand) launch failed for block %d (rc=%d)", b.idx, rc);
+        CK(cudaGetLastError());
+    } else {
+        Scope sc(c, ps.stream, nm, (double)nb * ((double)b.hin * b.hin + (double)b.hout * b.hout) * b.cexp * sizeof(T),
+                 2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
+        rc = whenet::fused::launch_dwse<T>(ps.stream, p, b.k, b.s, b.hin, nb, split);
+        if (rc != 0) return fail(WHENET_ECUDA, "KD launch failed for block %d (rc=%d)", b.idx, rc);
+        CK(cudaGetLastError());
+    }
+    r->tiles = 1;
+    return 0;
+}
+
+// Block 1, 16-bit: K1's depthwise-only instance
+template <typename T>
+int k1_dw_only(whenet_ctx* c, const Pass& ps, const T* cur, int nb, DwResult* r) {
+    const BlockCfg& b = c->blocks[0];
+    const BlockW& w = c->bw[0];
+    whenet::fused::K1Params p = c->dw1.p;
+    p.in = cur; p.wt_aug = nullptr; p.w_dw = w.w_dw_h; p.b_dw = w.b_dw_h; p.out = ps.D; p.partial = ps.partial; p.tflag = c->d_tflag;
+    p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = ps.gate; p.Cse = b.cse;
+    r->gate_done = c->se_fused != 0;
+    p.se_counter = r->gate_done ? ps.se_counter : nullptr;
+    char nm[48];
+    snprintf(nm, sizeof nm, "b%02d.dw", b.idx);
+    Scope sc(c, ps.stream, nm, (double)nb * 2.0 * b.hin * b.hin * b.cexp * sizeof(T), 2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
+    int rc = whenet::fused::launch_dw_only<T>(ps.stream, p, c->dw1.smem, nb);
+    if (rc != 0) return fail(WHENET_ECUDA, "depthwise-only K1 launch failed (rc=%d)", rc);
+    CK(cudaGetLastError());
+    r->tiles = p.tiles_x * p.tiles_y;
+    return 0;
+}
+
+// K1X, bf16: the tiles and bits of K1's plan `p`, with the block input and the weights fed by TMA
+int launch_k1x_block(whenet_ctx* c, const Pass& ps, size_t i, const __nv_bfloat16* cur, int nb, const whenet::fused::K1Params& p) {
+    const BlockCfg& b = c->blocks[i];
+    const BlockW& w = c->bw[i];
+    const int rowb = whenet::fused::k1x_row_bytes(b.cin);          // A and W rows: 64 or 128 bytes
+    whenet::fused::DwSeParams q{};
+    int rc = cached_tmap(c->tmaps, 512, {TmapKind::K1xIn, b.idx, nb, cur}, &q.tmX,
+                         [&](CUtensorMap* tm) { return make_tmap_k1x_in(tm, cur, nb, b.hin, b.cin, p.IW, rowb); });
+    if (!rc)
+        rc = cached_tmap(c->tmaps, 512, {TmapKind::K1xExp, b.idx, 0, w.wt_exp_aug}, &q.tmWx,
+                         [&](CUtensorMap* tm) { return make_tmap_w(tm, w.wt_exp_aug, b.cexp, b.cin + 8, p.CC, true, rowb); });
+    if (!rc)
+        rc = cached_tmap(c->tmaps, 512, {TmapKind::K1xDw, b.idx, 0, w.w_dw16}, &q.tmW,
+                         [&](CUtensorMap* tm) { return make_tmap_kd_w(tm, w.w_dw16, b.k * b.k, b.cexp, p.CC); });
+    if (rc) return rc;
+    q.b_dw = w.b_dw_h; q.tflag = c->d_tflag; q.out = ps.D; q.partial = ps.partial; q.C = b.cexp; q.pad = b.pad;
+    rc = whenet::fused::launch_k1x<__nv_bfloat16>(ps.stream, q, b.k, b.s, b.hin, b.cin, p.TH, c->k1[i].R, p.CC, nb);
+    if (rc != 0) return fail(WHENET_ECUDA, "K1X launch failed for block %d (rc=%d)", b.idx, rc);
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// 16-bit blocks with a K1 plan: expand + depthwise in one kernel (K1, or K1X where its conditions hold)
+template <typename T>
+int k1_block(whenet_ctx* c, const Pass& ps, size_t i, const T* cur, int nb, bool plain_dw, DwResult* r) {
+    const BlockCfg& b = c->blocks[i];
+    const BlockW& w = c->bw[i];
+    whenet::fused::K1Params p = c->k1[i].p;
+    p.in = cur; p.wt_aug = w.wt_exp_aug; p.w_dw = w.w_dw_h; p.w_dw16 = w.w_dw16; p.b_dw = w.b_dw_h; p.out = ps.D; p.partial = ps.partial; p.tflag = c->d_tflag;
+    p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = ps.gate; p.Cse = b.cse;
+    r->gate_done = c->se_fused && p.NB == 1;
+    p.se_counter = r->gate_done ? ps.se_counter : nullptr;
+    // small batches: spread one crop's chunks over several CTAs until the grid covers the SMs about twice
+    {
+        const long long ctas = (long long)p.tiles_x * p.tiles_y * ((nb + p.NB - 1) / p.NB);
+        int split = 1;
+        while (split < p.n_chunks && ctas * split < c->k1_split_ctas) ++split;
+        p.chunks_per_cta = (p.n_chunks + split - 1) / split;
+        // one tile per image and no chunk split: the CTA sees every pixel and channel of its crops and
+        // computes their SE gate in its tail (same bits as se_gate_kernel, which is then not launched)
+        if (c->se_tail && !r->gate_done && p.tiles_x * p.tiles_y == 1 && split == 1) {
+            p.se_tail = 1;
+            p.inv_hw = 1.0f / (float)(b.hout * b.hout);
+            r->gate_done = true;
+            // ... and applies it to its depthwise output (not under mode-1 taps, whose dw tap is the ungated tensor)
+            if (c->se_scale_out && !plain_dw) { p.scale_out = 1; r->d_gated = true; }
+        }
+    }
+    r->tiles = p.tiles_x * p.tiles_y;
+    char nm[48];
+    snprintf(nm, sizeof nm, "b%02d.k1", b.idx);
+    Scope sc(c, ps.stream, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
+             2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        // throughput batches (a CTA holds every chunk of its tile): K1X, the same tiles and bits fed by TMA
+        if (c->k1x && c->use_tc && p.chunks_per_cta == p.n_chunks && !r->gate_done &&
+            whenet::fused::k1x_has_instance(b.k, b.s, b.hin, b.cin, b.pad, p, c->k1[i].R))
+            return launch_k1x_block(c, ps, i, cur, nb, p);
+    }
+    int rc = whenet::fused::launch_k1<T>(ps.stream, p, b.k, b.s, c->k1[i].R, c->k1[i].NT, c->k1[i].smem, nb);
+    if (rc != 0) return fail(WHENET_ECUDA, "K1 launch failed for block %d (rc=%d)", b.idx, rc);
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// Any block: expand GEMM (if the block has an expand conv) + stand-alone depthwise
+template <typename T>
+int expand_dw(whenet_ctx* c, const Pass& ps, size_t i, const T* cur, int nb, DwResult* r) {
+    const BlockCfg& b = c->blocks[i];
+    const BlockW& w = c->bw[i];
+    char nm[48];
+    const T* dw_in = cur;
+    if (b.has_expand) {
+        snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
+        int rc = launch_pw<T>(c, ps.stream, c->use_tc, c->pw_variant, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, (T*)ps.E,
+                              (long long)nb * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, true);
+        if (rc) return rc;
+        dw_in = (const T*)ps.E;
+    }
+    snprintf(nm, sizeof nm, "b%02d.dw", b.idx);
+    return launch_dw<T>(c, ps, nm, b, w, dw_in, (T*)ps.D, nb, &r->tiles);
+}
+
+// Block i's expand and depthwise (D and the squeeze partials), on the first route whose conditions hold
+template <typename T>
+int run_dw_route(whenet_ctx* c, const Pass& ps, size_t i, const T* cur, int nb, bool stem_half, bool plain_dw, DwResult* r) {
+    const BlockCfg& b = c->blocks[i];
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        if (i == 0 && stem_half) return kd_stem_tiles(c, ps, cur, nb, r);
+        // late blocks (whole map in one CTA): expand GEMM + KD, or KD with the expand on chip, instead of K1
+        const bool use_kd = c->use_fused && c->use_tc && c->kd_from > 0 && b.idx >= c->kd_from &&
+                            b.has_expand && whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp) > 0;
+        if (use_kd) return kd_block(c, ps, i, cur, nb, plain_dw, r);
+    }
+    if constexpr (sizeof(T) == 2) {
+        // (block 1 has no expand conv, so this route and KD's never compete)
+        if (i == 0 && c->use_fused && c->dw1_fused && c->dw1.valid) return k1_dw_only<T>(c, ps, cur, nb, r);
+        if (c->use_fused && c->k1[i].valid && b.idx <= c->fused_max_block) return k1_block<T>(c, ps, i, cur, nb, plain_dw, r);
+    }
+    return expand_dw<T>(c, ps, i, cur, nb, r);
+}
+
+// Block b's SE gate from the squeeze partials its depthwise left (`tiles` per crop)
+int se_gate(whenet_ctx* c, const Pass& ps, const BlockCfg& b, const BlockW& w, int nb, int tiles) {
+    char nm[48];
+    snprintf(nm, sizeof nm, "b%02d.se", b.idx);
+    Scope sc(c, ps.stream, nm, (double)nb * (tiles + 1) * b.cexp * 4.0, 4.0 * nb * b.cexp * b.cse);
+    const float inv_hw = 1.0f / (float)(b.hout * b.hout);
+    const size_t se_smem = (b.cexp + b.cse) * sizeof(float);
+    if (nb >= 64 && c->se_batch) {
+        // throughput batches: four crops per CTA share every FC weight load (bit-identical gates)
+        constexpr int SEB = 4;
+        whenet::se_gate_batch_kernel<SEB, 512><<<(nb + SEB - 1) / SEB, 512, SEB * se_smem, ps.stream>>>(
+            ps.partial, tiles, inv_hw, w.w_se1t, w.b_se1, w.w_se2, w.b_se2, ps.gate, b.cexp, b.cse, nb);
+    } else if (nb < 64 || c->se_wide)     // 32 warps per crop cut the FC latency chain
+        whenet::se_gate_kernel<1024><<<nb, 1024, se_smem, ps.stream>>>(
+            ps.partial, tiles, inv_hw, w.w_se1t, w.b_se1, w.w_se2, w.b_se2, ps.gate, b.cexp, b.cse);
+    else
+        whenet::se_gate_kernel<256><<<nb, 256, se_smem, ps.stream>>>(
+            ps.partial, tiles, inv_hw, w.w_se1t, w.b_se1, w.w_se2, w.b_se2, ps.gate, b.cexp, b.cse);
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// Global average pool of the head features in E, Dense and the angle decode
+template <typename T>
+int head_fc_decode(whenet_ctx* c, const Pass& ps, int nb, float* d_angles, float* d_logits, bool taps) {
+    const T* E = (const T*)ps.E;
+    Scope sc(c, ps.stream, "head.fc_decode", (double)nb * (49.0 * 1280 * sizeof(T) + 12), 2.0 * nb * (1280.0 * 252 + 49 * 1280));
+    if (nb >= 64 && c->head_batch) {
+        // throughput batches: GAP kernel + Dense/decode for four crops per CTA (same bits as the one-CTA-per-crop kernel)
+        constexpr int HB = 4;
+        whenet::head_pool_kernel<T><<<nb, 160, 0, ps.stream>>>(E, ps.pooled);
+        c->launches++;                     // two kernels under one profile scope
+        auto kfn = whenet::head_fc_decode_batch_kernel<HB>;
+        const size_t hsm = (size_t)HB * (1280 + 256) * sizeof(float);
+        CK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
+        kfn<<<(nb + HB - 1) / HB, 512, hsm, ps.stream>>>(ps.pooled, c->w_fct, c->b_fc, d_angles, d_logits, nb);
+    } else
+        whenet::head_pool_fc_decode_kernel<T><<<nb, 256, 0, ps.stream>>>(E, nullptr, c->w_fct, c->b_fc, d_angles, d_logits,
+                                                                          taps ? ps.pooled : nullptr);
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// One pass of nb crops through the net on ps.stream, in ps's workspace
+template <typename T, bool IN_U8>
+int forward_chunk(whenet_ctx* c, const Pass& ps, const void* d_in, int nb, float* d_angles, float* d_logits, bool taps, int off) {
     char nm[48];
     // taps: record this chunk (crops off .. off + nb - 1 of the call).  Mode 1 also leaves the depthwise outputs ungated;
     // mode 2 changes no launch and no kernel parameter.
     const bool plain_dw = taps && c->taps_mode == 1;
-    T* cur = (T*)c->bufA;
-    T* oth = (T*)c->bufB;
-    T* E = (T*)c->bufE;
-    T* D = (T*)c->bufD;
+    T* cur = (T*)ps.A;
+    T* oth = (T*)ps.B;
+    const T* D = (const T*)ps.D;
     const bool stem_half = std::is_same<T, __nv_bfloat16>::value && c->use_fused && c->use_tc && c->dw1_kd && c->stem_variant != 0 && !c->blocks.empty() &&
                            !c->blocks[0].has_expand && c->blocks[0].cexp == 32 && c->blocks[0].k == 3 && c->blocks[0].s == 1 && c->blocks[0].hin % 14 == 0;
-    {
-        Scope sc(c, "stem", (double)nb * (kImgElems * (IN_U8 ? 1.0 : 4.0) + 112.0 * 112 * 32 * sizeof(T)),
-                 2.0 * nb * 112.0 * 112 * 27 * 32);
-        if (stem_half) {
-            // block 1's depthwise is KD (HFMA2 over an fp16 tile): the stem output, read by nothing else, is written as fp16
-            CK((whenet::launch_stem_tile<__half, IN_U8, true>(c->stream, d_in, reinterpret_cast<__half*>(cur), c->stem_params, c->lut, nb)));
-        } else if (c->stem_variant == 0) {
-            const long long total = (long long)nb * 112 * 112 * 4;
-            whenet::stem_kernel<T, IN_U8><<<(unsigned)((total + 255) / 256), 256, 0, c->stream>>>(d_in, cur, c->w_stem, c->b_stem, c->lut, nb);
-            CK(cudaGetLastError());
-        } else {
-            CK((whenet::launch_stem_tile<T, IN_U8, (sizeof(T) == 2)>(c->stream, d_in, cur, c->stem_params, c->lut, nb)));
-        }
-    }
+    int rc = run_stem<T, IN_U8>(c, ps, d_in, nb, stem_half);
+    if (rc) return rc;
     if (taps) {
-        int rc = stem_half ? add_tap<__half>(c, "stem", reinterpret_cast<const __half*>(cur), (size_t)112 * 112 * 32, off, nb)
-                           : add_tap<T>(c, "stem", cur, (size_t)112 * 112 * 32, off, nb);
+        rc = stem_half ? add_tap<__half>(c, ps.stream, "stem", reinterpret_cast<const __half*>(cur), (size_t)112 * 112 * 32, off, nb)
+                       : add_tap<T>(c, ps.stream, "stem", cur, (size_t)112 * 112 * 32, off, nb);
         if (rc) return rc;
     }
     for (size_t i = 0; i < c->blocks.size(); ++i) {
         const BlockCfg& b = c->blocks[i];
         const BlockW& w = c->bw[i];
-        const T* dw_in = cur;
-        int tiles = 0;
-        bool did_k1 = false;
-        bool se_in_k1 = false;      // the SE gate came out of the fused kernel's tail (options se_fused / se_tail)
-        bool d_gated = false;       // ... and D already carries it
-        // bf16 late blocks (whole map in one CTA): expand GEMM + KD instead of K1
-        const bool use_kd = std::is_same<T, __nv_bfloat16>::value && c->use_fused && c->use_tc && c->kd_from > 0 && b.idx >= c->kd_from &&
-                            b.has_expand && whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp) > 0;
-        if constexpr (sizeof(T) == 2) {
-            if (i == 0 && stem_half) {
-              if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-                whenet::fused::DwSeParams p{};
-                if (c->tmaps.size() > 512) c->tmaps.clear();
-                const TmapKey ke{100 + b.idx, nb, (const void*)cur}, kw{200 + b.idx, 0, (const void*)w.w_dw16};
-                auto ie = c->tmaps.find(ke);
-                if (ie == c->tmaps.end()) {
-                    CUtensorMap tm;
-                    int rc = make_tmap_kd_e(&tm, cur, nb, b.hin, b.cexp, 32, 16);
-                    if (rc) return rc;
-                    ie = c->tmaps.emplace(ke, tm).first;
-                }
-                auto iw = c->tmaps.find(kw);
-                if (iw == c->tmaps.end()) {
-                    CUtensorMap tm;
-                    int rc = make_tmap_kd_w(&tm, w.w_dw16, 9, b.cexp, 32);
-                    if (rc) return rc;
-                    iw = c->tmaps.emplace(kw, tm).first;
-                }
-                p.tmE = ie->second; p.tmW = iw->second;
-                p.b_dw = w.b_dw_h; p.tflag = c->d_tflag; p.out = D; p.partial = c->d_partial;
-                p.C = b.cexp; p.pad = b.pad; p.Cse = b.cse; p.inv_hw = 1.0f / (float)(b.hout * b.hout);
-                int split = 1;
-                {
-                    const int n_tiles = (b.hin / 14) * (b.hin / 14);
-                    while (split < n_tiles && (long long)nb * split < c->k1_split_ctas) ++split;
-                }
-                snprintf(nm, sizeof nm, "b%02d.dw", b.idx);
-                Scope sc(c, nm, (double)nb * 2.0 * b.hin * b.hin * b.cexp * sizeof(T), 2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
-                int rc = whenet::fused::launch_dwse_spatial<T>(c->stream, p, b.hin, nb, split);
-                if (rc != 0) return fail(WHENET_ECUDA, "KD (block 1) launch failed (rc=%d)", rc);
-                CK(cudaGetLastError());
-                tiles = (b.hin / 14) * (b.hin / 14);
-                did_k1 = true;
-              }
-            } else if (i == 0 && !did_k1 && c->use_fused && c->dw1_fused && c->dw1.valid) {
-                whenet::fused::K1Params p = c->dw1.p;
-                p.in = cur; p.wt_aug = nullptr; p.w_dw = w.w_dw_h; p.b_dw = w.b_dw_h; p.out = D; p.partial = c->d_partial; p.tflag = c->d_tflag;
-                p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = c->d_gate; p.Cse = b.cse;
-                se_in_k1 = c->se_fused != 0;
-                p.se_counter = se_in_k1 ? c->d_se_counter : nullptr;
-                snprintf(nm, sizeof nm, "b%02d.dw", b.idx);
-                Scope sc(c, nm, (double)nb * 2.0 * b.hin * b.hin * b.cexp * sizeof(T), 2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
-                int rc = whenet::fused::launch_dw_only<T>(c->stream, p, c->dw1.smem, nb);
-                if (rc != 0) return fail(WHENET_ECUDA, "depthwise-only K1 launch failed (rc=%d)", rc);
-                CK(cudaGetLastError());
-                tiles = p.tiles_x * p.tiles_y;
-                did_k1 = true;
-            } else if (use_kd) {
-              if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-                // late blocks: KD (depthwise + SE + gating, one CTA per crop).  Small batches spread one crop's channel chunks
-                // over several CTAs (the gate then comes from se_gate_kernel) and read E from an expand GEMM; otherwise each
-                // CTA computes its crop's expand conv on chip and E never leaves the SM.
-                const int cc = whenet::fused::dwse_chunk(b.k, b.s, b.hin, b.cexp);
-                int split = 1;
-                while (split < b.cexp / cc && (long long)nb * split < c->k1_split_ctas) ++split;
-                int rc = 0;
-                if (split > 1) {
-                    snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
-                    rc = launch_pw<T>(c, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, E,
-                                      (long long)nb * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, true, true);
-                    if (rc) return rc;
-                }
-                whenet::fused::DwSeParams p{};
-                {
-                    const int pw = (b.hout - 1) * b.s + b.k;
-                    if (c->tmaps.size() > 512) c->tmaps.clear();
-                    const TmapKey kw{200 + b.idx, 0, (const void*)w.w_dw16};
-                    auto iw = c->tmaps.find(kw);
-                    if (iw == c->tmaps.end()) {
-                        CUtensorMap tm;
-                        if ((rc = make_tmap_kd_w(&tm, w.w_dw16, b.k * b.k, b.cexp, cc))) return rc;
-                        iw = c->tmaps.emplace(kw, tm).first;
-                    }
-                    p.tmW = iw->second;
-                    if (split > 1) {
-                        const TmapKey ke{100 + b.idx, nb, (const void*)E};
-                        auto ie = c->tmaps.find(ke);
-                        if (ie == c->tmaps.end()) {
-                            CUtensorMap tm;
-                            if ((rc = make_tmap_kd_e(&tm, E, nb, b.hin, b.cexp, cc, pw))) return rc;
-                            ie = c->tmaps.emplace(ke, tm).first;
-                        }
-                        p.tmE = ie->second;
-                    } else {
-                        // block input [nb*H*W][Cin]: box rows = one crop's pixels rounded up to a swizzle atom; expand weights [Cexp][Cin]
-                        const TmapKey kx{300 + b.idx, nb, (const void*)cur}, kwx{400 + b.idx, 0, (const void*)w.wt_exp};
-                        auto ix = c->tmaps.find(kx);
-                        if (ix == c->tmaps.end()) {
-                            CUtensorMap tm;
-                            if ((rc = make_tmap_w(&tm, cur, nb * b.hin * b.hin, b.cin, (b.hin * b.hin + 7) / 8 * 8, true))) return rc;
-                            ix = c->tmaps.emplace(kx, tm).first;
-                        }
-                        auto iwx = c->tmaps.find(kwx);
-                        if (iwx == c->tmaps.end()) {
-                            CUtensorMap tm;
-                            if ((rc = make_tmap_w(&tm, w.wt_exp, b.cexp, b.cin, cc, true))) return rc;
-                            iwx = c->tmaps.emplace(kwx, tm).first;
-                        }
-                        p.tmX = ix->second; p.tmWx = iwx->second;
-                        p.b_exp = w.b_exp;
-                    }
-                }
-                p.b_dw = w.b_dw_h; p.tflag = c->d_tflag;
-                p.out = D; p.partial = c->d_partial;
-                p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = c->d_gate; p.Cse = b.cse;
-                p.inv_hw = 1.0f / (float)(b.hout * b.hout);
-                p.C = b.cexp; p.pad = b.pad;
-                if (split == 1 && c->se_tail && c->kd_tail) {
-                    p.se_tail = 1;
-                    se_in_k1 = true;
-                    if (c->se_scale_out && !plain_dw) { p.scale_out = 1; d_gated = true; }
-                }
-                snprintf(nm, sizeof nm, "b%02d.kd", b.idx);
-                if (split == 1) {
-                    Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
-                             2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
-                    rc = whenet::fused::launch_dwse_x<T>(c->stream, p, b.k, b.s, b.hin, b.cin, nb);
-                    if (rc != 0) return fail(WHENET_ECUDA, "KD (on-chip expand) launch failed for block %d (rc=%d)", b.idx, rc);
-                    CK(cudaGetLastError());
-                } else {
-                    Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin + (double)b.hout * b.hout) * b.cexp * sizeof(T),
-                             2.0 * nb * (double)b.hout * b.hout * b.k * b.k * b.cexp);
-                    rc = whenet::fused::launch_dwse<T>(c->stream, p, b.k, b.s, b.hin, nb, split);
-                    if (rc != 0) return fail(WHENET_ECUDA, "KD launch failed for block %d (rc=%d)", b.idx, rc);
-                    CK(cudaGetLastError());
-                }
-                tiles = 1;
-                did_k1 = true;
-              }
-            } else if (c->use_fused && c->k1[i].valid && b.idx <= c->fused_max_block) {
-                whenet::fused::K1Params p = c->k1[i].p;
-                p.in = cur; p.wt_aug = w.wt_exp_aug; p.w_dw = w.w_dw_h; p.w_dw16 = w.w_dw16; p.b_dw = w.b_dw_h; p.out = D; p.partial = c->d_partial; p.tflag = c->d_tflag;
-                p.w_se1t = w.w_se1t; p.b_se1 = w.b_se1; p.w_se2 = w.w_se2; p.b_se2 = w.b_se2; p.gate = c->d_gate; p.Cse = b.cse;
-                se_in_k1 = c->se_fused && p.NB == 1;
-                p.se_counter = se_in_k1 ? c->d_se_counter : nullptr;
-                // small batches: spread one crop's chunks over several CTAs until the grid covers the SMs about twice
-                {
-                    const long long ctas = (long long)p.tiles_x * p.tiles_y * ((nb + p.NB - 1) / p.NB);
-                    int split = 1;
-                    while (split < p.n_chunks && ctas * split < c->k1_split_ctas) ++split;
-                    p.chunks_per_cta = (p.n_chunks + split - 1) / split;
-                    // one tile per image and no chunk split: the CTA sees every pixel and channel of its crops and
-                    // computes their SE gate in its tail (same bits as se_gate_kernel, which is then not launched)
-                    if (c->se_tail && !se_in_k1 && p.tiles_x * p.tiles_y == 1 && split == 1) {
-                        p.se_tail = 1;
-                        p.inv_hw = 1.0f / (float)(b.hout * b.hout);
-                        se_in_k1 = true;
-                        // ... and applies it to its depthwise output (not under mode-1 taps, whose dw tap is the ungated tensor)
-                        if (c->se_scale_out && !plain_dw) { p.scale_out = 1; d_gated = true; }
-                    }
-                }
-                snprintf(nm, sizeof nm, "b%02d.k1", b.idx);
-                Scope sc(c, nm, (double)nb * ((double)b.hin * b.hin * b.cin + (double)b.hout * b.hout * b.cexp) * sizeof(T),
-                         2.0 * nb * ((double)b.hin * b.hin * b.cin * b.cexp + (double)b.hout * b.hout * b.k * b.k * b.cexp));
-                bool did_k1x = false;
-                if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-                    // throughput batches (a CTA holds every chunk of its tile): K1X, the same tiles and bits fed by TMA
-                    if (c->k1x && c->use_tc && p.chunks_per_cta == p.n_chunks && !se_in_k1 &&
-                        whenet::fused::k1x_has_instance(b.k, b.s, b.hin, b.cin, b.pad, p, c->k1[i].R)) {
-                        whenet::fused::DwSeParams q{};
-                        int rc = 0;
-                        if (c->tmaps.size() > 512) c->tmaps.clear();
-                        const int rowb = whenet::fused::k1x_row_bytes(b.cin);          // A and W rows: 64 or 128 bytes
-                        const TmapKey kx{600 + b.idx, nb, (const void*)cur}, kwx{700 + b.idx, 0, (const void*)w.wt_exp_aug}, kw{500 + b.idx, 0, (const void*)w.w_dw16};
-                        auto ix = c->tmaps.find(kx);
-                        if (ix == c->tmaps.end()) {
-                            CUtensorMap tm;
-                            if ((rc = make_tmap_k1x_in(&tm, cur, nb, b.hin, b.cin, p.IW, rowb))) return rc;
-                            ix = c->tmaps.emplace(kx, tm).first;
-                        }
-                        auto iwx = c->tmaps.find(kwx);
-                        if (iwx == c->tmaps.end()) {
-                            CUtensorMap tm;
-                            if ((rc = make_tmap_w(&tm, w.wt_exp_aug, b.cexp, b.cin + 8, p.CC, true, rowb))) return rc;
-                            iwx = c->tmaps.emplace(kwx, tm).first;
-                        }
-                        auto iw = c->tmaps.find(kw);
-                        if (iw == c->tmaps.end()) {
-                            CUtensorMap tm;
-                            if ((rc = make_tmap_kd_w(&tm, w.w_dw16, b.k * b.k, b.cexp, p.CC))) return rc;
-                            iw = c->tmaps.emplace(kw, tm).first;
-                        }
-                        q.tmX = ix->second; q.tmWx = iwx->second; q.tmW = iw->second;
-                        q.b_dw = w.b_dw_h; q.tflag = c->d_tflag; q.out = D; q.partial = c->d_partial; q.C = b.cexp; q.pad = b.pad;
-                        rc = whenet::fused::launch_k1x<T>(c->stream, q, b.k, b.s, b.hin, b.cin, p.TH, c->k1[i].R, p.CC, nb);
-                        if (rc != 0) return fail(WHENET_ECUDA, "K1X launch failed for block %d (rc=%d)", b.idx, rc);
-                        CK(cudaGetLastError());
-                        did_k1x = true;
-                    }
-                }
-                if (!did_k1x) {
-                    int rc = whenet::fused::launch_k1<T>(c->stream, p, b.k, b.s, c->k1[i].R, c->k1[i].NT, c->k1[i].smem, nb);
-                    if (rc != 0) return fail(WHENET_ECUDA, "K1 launch failed for block %d (rc=%d)", b.idx, rc);
-                    CK(cudaGetLastError());
-                }
-                tiles = p.tiles_x * p.tiles_y;
-                did_k1 = true;
-            }
-        }
-        if (!did_k1) {
-        if (b.has_expand) {
-            snprintf(nm, sizeof nm, "b%02d.expand", b.idx);
-            int rc = launch_pw<T>(c, nm, cur, w.w_exp, w.wt_exp, w.b_exp, nullptr, nullptr, E,
-                                  (long long)nb * b.hin * b.hin, b.cin, b.cexp, b.hin * b.hin, true);
-            if (rc) return rc;
-            dw_in = E;
-        }
-        snprintf(nm, sizeof nm, "b%02d.dw", b.idx);
-        int rc = launch_dw<T>(c, nm, b, w, dw_in, D, nb, &tiles);
-        if (rc) return rc;
-        }
-        int rc = 0;
-        if (!se_in_k1) {
-            snprintf(nm, sizeof nm, "b%02d.se", b.idx);
-            Scope sc(c, nm, (double)nb * (tiles + 1) * b.cexp * 4.0, 4.0 * nb * b.cexp * b.cse);
-            const float inv_hw = 1.0f / (float)(b.hout * b.hout);
-            const size_t se_smem = (b.cexp + b.cse) * sizeof(float);
-            if (nb >= 64 && c->se_batch) {
-                // throughput batches: four crops per CTA share every FC weight load (bit-identical gates)
-                constexpr int SEB = 4;
-                whenet::se_gate_batch_kernel<SEB, 512><<<(nb + SEB - 1) / SEB, 512, SEB * se_smem, c->stream>>>(
-                    c->d_partial, tiles, inv_hw, w.w_se1t, w.b_se1, w.w_se2, w.b_se2, c->d_gate, b.cexp, b.cse, nb);
-            } else if (nb < 64 || c->se_wide)     // 32 warps per crop cut the FC latency chain
-                whenet::se_gate_kernel<1024><<<nb, 1024, se_smem, c->stream>>>(
-                    c->d_partial, tiles, inv_hw, w.w_se1t, w.b_se1, w.w_se2, w.b_se2, c->d_gate, b.cexp, b.cse);
-            else
-                whenet::se_gate_kernel<256><<<nb, 256, se_smem, c->stream>>>(
-                    c->d_partial, tiles, inv_hw, w.w_se1t, w.b_se1, w.w_se2, w.b_se2, c->d_gate, b.cexp, b.cse);
-            CK(cudaGetLastError());
-        }
+        DwResult r;
+        if ((rc = run_dw_route<T>(c, ps, i, cur, nb, stem_half, plain_dw, &r))) return rc;
+        if (!r.gate_done && (rc = se_gate(c, ps, b, w, nb, r.tiles))) return rc;
         snprintf(nm, sizeof nm, "b%02d.project", b.idx);
-        rc = launch_pw<T>(c, nm, D, w.w_proj, w.wt_proj, w.b_proj, d_gated ? nullptr : c->d_gate, b.skip ? cur : nullptr, oth,
-                          (long long)nb * b.hout * b.hout, b.cexp, b.cout, b.hout * b.hout, false);
+        rc = launch_pw<T>(c, ps.stream, c->use_tc, c->pw_variant, nm, D, w.w_proj, w.wt_proj, w.b_proj, r.d_gated ? nullptr : ps.gate,
+                          b.skip ? cur : nullptr, oth, (long long)nb * b.hout * b.hout, b.cexp, b.cout, b.hout * b.hout, false);
         if (rc) return rc;
         if (taps) {
             snprintf(nm, sizeof nm, "dw%d", b.idx);
-            if ((rc = add_tap<T>(c, nm, D, (size_t)b.hout * b.hout * b.cexp, off, nb, d_gated))) return rc;
+            if ((rc = add_tap<T>(c, ps.stream, nm, D, (size_t)b.hout * b.hout * b.cexp, off, nb, r.d_gated))) return rc;
             snprintf(nm, sizeof nm, "gate%d", b.idx);
-            if ((rc = add_tap<float>(c, nm, c->d_gate, (size_t)b.cexp, off, nb))) return rc;
+            if ((rc = add_tap<float>(c, ps.stream, nm, ps.gate, (size_t)b.cexp, off, nb))) return rc;
             snprintf(nm, sizeof nm, "block%d", b.idx);
-            if ((rc = add_tap<T>(c, nm, oth, (size_t)b.hout * b.hout * b.cout, off, nb))) return rc;
+            if ((rc = add_tap<T>(c, ps.stream, nm, oth, (size_t)b.hout * b.hout * b.cout, off, nb))) return rc;
         }
         std::swap(cur, oth);
     }
-    int rc = launch_pw<T>(c, "head.conv", cur, c->w_head, c->wt_head, c->b_head, nullptr, nullptr, E,
-                          (long long)nb * 49, 320, 1280, 49, true);
+    rc = launch_pw<T>(c, ps.stream, c->use_tc, c->pw_variant, "head.conv", cur, c->w_head, c->wt_head, c->b_head, nullptr, nullptr,
+                      (T*)ps.E, (long long)nb * 49, 320, 1280, 49, true);
     if (rc) return rc;
-    if (taps && (rc = add_tap<T>(c, "head", E, (size_t)49 * 1280, off, nb))) return rc;
-    {
-        Scope sc(c, "head.fc_decode", (double)nb * (49.0 * 1280 * sizeof(T) + 12), 2.0 * nb * (1280.0 * 252 + 49 * 1280));
-        if (nb >= 64 && c->head_batch) {
-            // throughput batches: GAP kernel + Dense/decode for four crops per CTA (same bits as the one-CTA-per-crop kernel)
-            constexpr int HB = 4;
-            whenet::head_pool_kernel<T><<<nb, 160, 0, c->stream>>>(E, c->d_pooled);
-            c->launches++;                     // two kernels under one profile scope
-            auto kfn = whenet::head_fc_decode_batch_kernel<HB>;
-            const size_t hsm = (size_t)HB * (1280 + 256) * sizeof(float);
-            CK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm));
-            kfn<<<(nb + HB - 1) / HB, 512, hsm, c->stream>>>(c->d_pooled, c->w_fct, c->b_fc, d_angles, d_logits, nb);
-        } else
-        whenet::head_pool_fc_decode_kernel<T><<<nb, 256, 0, c->stream>>>(E, nullptr, c->w_fct, c->b_fc, d_angles, d_logits,
-                                                                         taps ? c->d_pooled : nullptr);
-        CK(cudaGetLastError());
-    }
-    if (taps && (rc = add_tap<float>(c, "pooled", c->d_pooled, (size_t)1280, off, nb))) return rc;
+    if (taps && (rc = add_tap<T>(c, ps.stream, "head", (const T*)ps.E, (size_t)49 * 1280, off, nb))) return rc;
+    if ((rc = head_fc_decode<T>(c, ps, nb, d_angles, d_logits, taps))) return rc;
+    if (taps && (rc = add_tap<float>(c, ps.stream, "pooled", ps.pooled, (size_t)1280, off, nb))) return rc;
     return 0;
 }
 
@@ -989,19 +1023,16 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
         if ((rc = prepare_taps(c, crops))) return rc;
     }
     if (two_streams) {
-        const size_t es = esize(c->precision);
         const int parts = c->n_streams;
         const int per = (n + parts - 1) / parts;
-        struct Saved { void *A, *B, *E, *D; float *part, *gate, *pooled; int* ctr; cudaStream_t s; } sv{c->bufA, c->bufB, c->bufE, c->bufD,
-                                                                                                     c->d_partial, c->d_gate, c->d_pooled, c->d_se_counter, c->stream};
-        CK(cudaEventRecord(c->ev_fork, sv.s));
+        CK(cudaEventRecord(c->ev_fork, c->stream));
         const int slot = in_is_device ? 0 : (int)(c->host_pass_ctr++ & 1u);
         if (!in_is_device) CK(cudaStreamWaitEvent(c->copy_stream, c->ev_free[slot], 0));   // staging slot reusable
-        int rc2 = 0;
-        for (int h = 0; h < parts && rc2 == 0; ++h) {
+        for (int h = 0; h < parts; ++h) {
             const int off = h * per, nb = std::min(per, n - off);
             if (nb <= 0) { CK(cudaEventRecord(c->ev_join[h], c->aux_stream[h])); continue; }
-            CK(cudaStreamWaitEvent(c->aux_stream[h], c->ev_fork, 0));
+            const Pass ps = pass_view(c, off, c->aux_stream[h]);
+            CK(cudaStreamWaitEvent(ps.stream, c->ev_fork, 0));
             const void* d_src = (const char*)in + (size_t)off * kImgElems * in_es;
             if (!in_is_device) {
                 // half h uploads on the copy stream while half h-1 (and the previous call) compute
@@ -1009,21 +1040,14 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
                 if (int urc = upload_input(c, dst, d_src, (size_t)nb * kImgElems * in_es, c->copy_stream, (size_t)off * kImgElems * in_es,
                                            (size_t)n * kImgElems * in_es, h == 0)) return urc;
                 CK(cudaEventRecord(c->ev_half[h], c->copy_stream));
-                CK(cudaStreamWaitEvent(c->aux_stream[h], c->ev_half[h], 0));
+                CK(cudaStreamWaitEvent(ps.stream, c->ev_half[h], 0));
                 d_src = dst;
             }
-            c->stream = c->aux_stream[h];
-            c->bufA = (char*)sv.A + (size_t)off * c->ws_io * es;  c->bufB = (char*)sv.B + (size_t)off * c->ws_io * es;
-            c->bufE = (char*)sv.E + (size_t)off * c->ws_ex * es;  c->bufD = (char*)sv.D + (size_t)off * c->ws_dw * es;
-            c->d_partial = sv.part + (size_t)off * c->ws_part;    c->d_gate = sv.gate + (size_t)off * 1152;
-            c->d_pooled = sv.pooled + (size_t)off * 1280;         c->d_se_counter = sv.ctr + off;
-            rc2 = forward_chunk<T, IN_U8>(c, d_src, nb, d_ang + (size_t)off * 3,
-                                          d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr, c->taps_mode == 2, off);
-            if (rc2 == 0 && cudaEventRecord(c->ev_join[h], c->aux_stream[h]) != cudaSuccess) rc2 = fail(WHENET_ECUDA, "event record failed");
+            rc = forward_chunk<T, IN_U8>(c, ps, d_src, nb, d_ang + (size_t)off * 3,
+                                         d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr, c->taps_mode == 2, off);
+            if (rc) return rc;
+            CK(cudaEventRecord(c->ev_join[h], ps.stream));
         }
-        c->bufA = sv.A; c->bufB = sv.B; c->bufE = sv.E; c->bufD = sv.D;
-        c->d_partial = sv.part; c->d_gate = sv.gate; c->d_pooled = sv.pooled; c->d_se_counter = sv.ctr; c->stream = sv.s;
-        if (rc2) return rc2;
         for (int h = 0; h < parts; ++h) CK(cudaStreamWaitEvent(c->stream, c->ev_join[h], 0));
         if (!in_is_device) CK(cudaEventRecord(c->ev_free[slot], c->stream));
         if (!out_is_device) {
@@ -1038,6 +1062,7 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
         }
         return 0;
     }
+    const Pass ps = pass_view(c, 0, c->stream);
     int ci = 0;
     for (int off = 0; off < n; off += step, ++ci) {
         const int nb = std::min(step, n - off);
@@ -1053,7 +1078,7 @@ int forward_all(whenet_ctx* c, const void* in, int n, int in_is_device, float* a
             CK(cudaStreamWaitEvent(c->stream, c->ev_ready[slot], 0));
             d_in = c->d_in[slot];
         }
-        rc = forward_chunk<T, IN_U8>(c, d_in, nb, d_ang + (size_t)off * 3, d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr,
+        rc = forward_chunk<T, IN_U8>(c, ps, d_in, nb, d_ang + (size_t)off * 3, d_log ? d_log + (size_t)off * WHENET_N_LOGITS : nullptr,
                                      c->taps_mode == 2 || (c->taps_mode == 1 && off == 0 && nb <= 8), off);
         if (rc) {
             if (graphable) { cudaGraph_t g = nullptr; cudaStreamEndCapture(c->stream, &g); if (g) cudaGraphDestroy(g); }
@@ -1265,7 +1290,7 @@ int launch_crop_kernel(whenet_ctx* c, const Frames& src, const int32_t* rects, c
     }
     CK(cudaMemcpyAsync(c->d_rects, rects, (size_t)m * sizeof(int4), cudaMemcpyHostToDevice, c->stream));
     if (frame_of) CK(cudaMemcpyAsync(c->d_frame_of, frame_of, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-    Scope sc(c, "crop_resize", (double)m * 224 * 224 * 3 * 2, 0.0);
+    Scope sc(c, c->stream, "crop_resize", (double)m * 224 * 224 * 3 * 2, 0.0);
     for (int m0 = 0; m0 < m; m0 += 65535) {
         const int mb = std::min(65535, m - m0);
         const dim3 grid((224 * 224 + 255) / 256, mb);
@@ -1806,7 +1831,7 @@ int draw_heads(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, int n, 
         c->segs_cap = total;
     }
     CK(cudaMemcpyAsync(c->d_segs, segs.data(), (size_t)total * sizeof(whenet::OverlaySeg), cudaMemcpyHostToDevice, c->stream));
-    Scope sc(c, "draw_heads", 0.0, 0.0);
+    Scope sc(c, c->stream, "draw_heads", 0.0, 0.0);
     whenet::overlay_draw_kernel<<<dim3((maxH + 127) / 128, n), 128, 0, c->stream>>>(fr, c->d_segs);
     CK(cudaGetLastError());
     return 0;
@@ -1975,7 +2000,7 @@ int draw_overlay_list(whenet_ctx* c, uint8_t* const* frames, const int32_t* hw, 
     if (int rc = upload(c, &c->d_thin, &c->thin_cap, L.thin)) return rc;
     if (int rc = upload(c, &c->d_bands, &c->bands_cap, band_begin)) return rc;
     if (int rc = upload(c, &c->d_items, &c->items_cap, items)) return rc;
-    Scope sc(c, "draw_overlay", 0.0, 0.0);
+    Scope sc(c, c->stream, "draw_overlay", 0.0, 0.0);
     whenet::overlay_draw_banded_kernel<<<dim3((maxH + 127) / 128, n), 128, 0, c->stream>>>(fr, c->d_segs, c->d_thin, c->d_bands, c->d_items);
     CK(cudaGetLastError());
     return 0;
@@ -2284,19 +2309,12 @@ int debug_conv_impl(whenet_ctx* c, int use_tc, const float* A, const float* W, c
     // on the context's stream: a legacy-stream memset is not ordered against kernels of a non-blocking stream and could land on
     // rows the first tiles had already written (seen once in ~20 runs as NaN rows at the start of the output)
     CK(cudaMemsetAsync(dO, 0xFF, hO.size() * sizeof(T), c->stream));
-    const int saved = c->use_tc;
-    c->use_tc = use_tc;
     int rc;
     if (use_tc) {
         rc = 1;
         if constexpr (sizeof(T) == 2)
             if (use_tc == 3) {
-                const int saved_v = c->pw_variant;
-                c->pw_variant = 3;
-                c->tmaps2.clear();
-                rc = launch_pw<T>(c, "debug.conv1x1", dA, dW, dWt, dB, dG, dR, dO, M, K, N, hw, swish != 0);
-                c->pw_variant = saved_v;
-                c->tmaps2.clear();
+                rc = launch_pw<T>(c, c->stream, use_tc, 3, "debug.conv1x1", dA, dW, dWt, dB, dG, dR, dO, M, K, N, hw, swish != 0);
             } else if (use_tc == 5) {
                 rc = whenet::tc::launch_pw_tc3<T>(c->stream, dA, dWt, dB, dG, dR, dO, M, K, N, hw);
             } else
@@ -2322,9 +2340,8 @@ int debug_conv_impl(whenet_ctx* c, int use_tc, const float* A, const float* W, c
         if (rc == 0 && cudaGetLastError() != cudaSuccess) rc = -1;
         if (rc != 0) rc = fail(WHENET_EINVAL, "tensor-core family cannot run M=%lld K=%d N=%d (rc=%d)", M, K, N, rc);
     } else {
-        rc = launch_pw<T>(c, "debug.conv1x1", dA, dW, nullptr, dB, dG, dR, dO, M, K, N, hw, swish != 0);
+        rc = launch_pw<T>(c, c->stream, 0, c->pw_variant, "debug.conv1x1", dA, dW, nullptr, dB, dG, dR, dO, M, K, N, hw, swish != 0);
     }
-    c->use_tc = saved;
     cudaError_t e = cudaStreamSynchronize(c->stream);
     if (rc == 0 && e != cudaSuccess) rc = fail(WHENET_ECUDA, "debug conv failed: %s", cudaGetErrorString(e));
     if (rc == 0 && use_tc) rc = check_timeout(c);

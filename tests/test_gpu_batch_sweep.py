@@ -53,7 +53,7 @@ ROUTES = {
 }
 
 
-# ----------------------------------------------------------------------------- route model (whenet_api.cu forward_all / forward_chunk / launch_pw)
+# ----------------------------------------------------------------------------- route model (whenet_api.cu forward_all / run_dw_route / launch_pw)
 def _cdiv(a, b):
     return -(-a // b)
 
