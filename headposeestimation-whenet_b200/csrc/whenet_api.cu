@@ -189,6 +189,7 @@ struct whenet_ctx {
     K1Plan dw1;                // block 1 (no expand): depthwise-only instance of K1
     int dw1_fused = 1;
     cudaStream_t own_stream = nullptr, stream = nullptr, copy_stream = nullptr;
+    cudaEvent_t ev_switch = nullptr;    // whenet_set_stream: the new stream waits for the old one's work
     bool weights_loaded = false;
     std::vector<BlockCfg> blocks;
     std::vector<BlockW> bw;
@@ -1400,6 +1401,7 @@ int whenet_create(whenet_ctx** out, int device, int max_batch, int precision) {
     CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     c->stream = c->own_stream;
     CK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&c->ev_switch, cudaEventDisableTiming));
     for (int i = 0; i < 4; ++i) {
         CK(cudaStreamCreateWithFlags(&c->aux_stream[i], cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&c->ev_join[i], cudaEventDisableTiming));
@@ -1615,7 +1617,16 @@ int whenet_import_packed(whenet_ctx* c, const float* arena_f32, int64_t n_f32, c
 
 int whenet_set_stream(whenet_ctx* c, void* s) {
     if (!c) return fail(WHENET_EINVAL, "null context");
-    c->stream = s ? (cudaStream_t)s : c->own_stream;
+    const cudaStream_t next = s ? (cudaStream_t)s : c->own_stream;
+    if (next != c->stream) {
+        // every call shares the workspace, the staging and result slots and the crop tables: work queued on the new stream
+        // waits for everything queued on the old one, so it cannot overwrite buffers still in use and whenet_synchronize on
+        // the new stream covers both
+        CK(cudaSetDevice(c->device));
+        CK(cudaEventRecord(c->ev_switch, c->stream));
+        CK(cudaStreamWaitEvent(next, c->ev_switch, 0));
+        c->stream = next;
+    }
     return 0;   // captured graphs are stream independent: they are launched on whatever stream is current
 }
 
@@ -2515,6 +2526,7 @@ void whenet_destroy(whenet_ctx* c) {
         if (c->ev_half[i]) cudaEventDestroy(c->ev_half[i]);
     }
     if (c->ev_fork) cudaEventDestroy(c->ev_fork);
+    if (c->ev_switch) cudaEventDestroy(c->ev_switch);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->ev_stage) cudaEventDestroy(c->ev_stage);

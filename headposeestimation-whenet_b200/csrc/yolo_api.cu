@@ -685,6 +685,8 @@ int whenet_det_precision(whenet_det* d) {
     return d->precision;
 }
 
+// Unlike whenet_set_stream, no event orders the new stream after the old one: every detector entry point synchronises its
+// stream before it returns, so nothing of the detector is in flight at a switch.
 int whenet_det_set_stream(whenet_det* d, void* s) {
     if (!d) return fail(WHENET_EINVAL, "null detector");
     d->stream = s ? (cudaStream_t)s : d->own_stream;

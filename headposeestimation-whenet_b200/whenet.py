@@ -240,7 +240,10 @@ class WHENet:
     def set_stream(self, stream_ptr: Optional[int]):
         """Run on a caller-owned CUDA stream.  ``0`` (torch's default stream) is passed as
         cudaStreamLegacy (handle 0x1) because a NULL handle means "back to the internal stream";
-        ``None`` restores the internal stream."""
+        ``None`` restores the internal stream.  Work queued after a switch runs after all work queued before it, and
+        ``synchronize()`` covers both; the previous stream must still exist at the switch (torch's streams are pooled, so
+        from Python it always does).  Setting the current stream again costs nothing.  Host inputs are uploaded on the
+        context's copy stream, which does not wait for this stream: they must hold their data when the call is made."""
         if stream_ptr is None:
             check(self._L.whenet_set_stream(self._h, None))
         else:

@@ -91,7 +91,16 @@ int whenet_import_packed(whenet_ctx* ctx, const float* arena_f32, int64_t n_f32,
                          const int64_t* index, int64_t n_index);
 
 /* Run on an existing CUDA stream (cudaStream_t / CUstream) instead of the
- * context's own; NULL restores the internal stream. */
+ * context's own; NULL restores the internal stream.  Every call of the context
+ * orders its device work after what was queued on its stream before the call,
+ * and work queued on the stream after the call sees its results.  Switching to
+ * another stream keeps that order: work queued after the switch runs after all
+ * work queued before it, and whenet_synchronize covers both.  The previous
+ * stream must still exist at the switch; setting the current stream again is a
+ * no-op.  Host inputs of the forward entries are the exception: they are read
+ * on the context's copy stream, which does not wait for the caller's stream (so
+ * that the upload of one batch overlaps the compute of the previous one), so a
+ * host input must hold its data when the call is made. */
 int whenet_set_stream(whenet_ctx* ctx, void* cuda_stream);
 
 /* replaces: WHENet.get_angle(img), reference whenet.py:22-34, for uint8 input.

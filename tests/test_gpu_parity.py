@@ -448,6 +448,7 @@ def test_two_stream_mode_bitwise(sample_crops, jitter_crops):
     y = torch.empty((131, 3), dtype=torch.float32, device="cuda")
     for _ in range(4):
         y.zero_()
+        torch.cuda.synchronize()
         m.forward_device(x, y)
         m.synchronize()
         assert np.array_equal(y.cpu().numpy(), ref)

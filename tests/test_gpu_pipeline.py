@@ -28,6 +28,7 @@ def _crop_boxes(wn, frames, boxes, frame_of):
     n, H, W = frames.shape[:3]
     m = len(boxes)
     out = torch.full((m, 224, 224, 3), 77, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
     rects = np.full((m, 4), -1, np.int32)
     valid = np.full(m, -1, np.int32)
     check(wn._L.whenet_crop_boxes_u8(wn._h, _ptr(frames), n, H, W, int(_is_device(frames)), _ptr(boxes), _ptr(frame_of), m, 1,
