@@ -13,7 +13,8 @@ _SIMT_TC = ["kernels_simt.cuh", "kernels_tc.cuh"]
 _ABI = os.path.join("..", "..", "include", "whenet_b200.h")
 # translation unit -> the headers it depends on (a unit is recompiled when it or one of them is newer than its object)
 UNITS = {
-    "whenet_api.cu": _SIMT_TC + ["api_error.h", "kernels_fused.cuh", "kernels_crop.cuh", "kernels_overlay.cuh", "hershey_simplex.inc", "yuv.cuh", "kernels_k2.cuh", "kernels_tc32.cuh", "kernels_dwse.cuh", "kernels_k1x.cuh", "jpeg_api.h", _ABI],
+    "whenet_api.cu": _SIMT_TC + ["api_error.h", "kernels_fused.cuh", "kernels_k2.cuh", "kernels_tc32.cuh", "kernels_dwse.cuh", "kernels_k1x.cuh", "frames_api.h", "jpeg_api.h", _ABI],
+    "frames_api.cu": ["kernels_crop.cuh", "yuv.cuh", "kernels_overlay.cuh", "hershey_simplex.inc", "frames_api.h", "api_error.h", _ABI],
     "inst_k1_bf16.cu": _SIMT_TC + ["kernels_fused.cuh", "kernels_dwse.cuh", "kernels_k1x.cuh"],
     "inst_k1_f16.cu": _SIMT_TC + ["kernels_fused.cuh"],
     "inst_dwse.cu": _SIMT_TC + ["kernels_fused.cuh", "kernels_dwse.cuh"],

@@ -1,5 +1,5 @@
 // Head overlay: thickness-2 LINE_8 segments (OpenCV's cv2.line(img, p0, p1, color, 2) bit for bit, oracle/draw_oracle.py)
-// rasterised into BGR frames in place.  The host (whenet_api.cu) clips each segment's end points against the frame grown by
+// rasterised into BGR frames in place.  The host (frames_api.cu) clips each segment's end points against the frame grown by
 // the thickness and computes its 16.16 quad; everything here is integer arithmetic except the outline clip, which is the
 // same double multiply-then-divide OpenCV truncates (no add, so nothing to contract).
 //

@@ -19,6 +19,7 @@
 #include "kernels_yolo.cuh"
 #include "kernels_yolo32.cuh"
 
+using whenet::api::check_yuv_layout;
 using whenet::api::fail;
 namespace Y = whenet::yolo;
 
@@ -696,12 +697,6 @@ int whenet_det_set_stream(whenet_det* d, void* s) {
 }  // extern "C"
 
 namespace {
-
-int check_yuv_layout(int yuv_layout) {
-    if (yuv_layout != WHENET_YUV_NV12 && yuv_layout != WHENET_YUV_I420)
-        return fail(WHENET_EINVAL, "yuv_layout=%d: WHENET_YUV_NV12 (%d) or WHENET_YUV_I420 (%d)", yuv_layout, WHENET_YUV_NV12, WHENET_YUV_I420);
-    return 0;
-}
 
 // whenet_det_detect_u8 (yuv_layout 0) and whenet_det_detect_yuv_u8 after their argument checks
 int detect_one_size(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb, int yuv_layout, float score,
