@@ -25,10 +25,14 @@ EXPORTS = [
     "whenet_encode_jpeg_u8", "whenet_encode_jpeg_ragged_u8", "whenet_debug_jpeg_header",
     "whenet_encode_jpeg_ex_u8", "whenet_debug_jpeg_header_ex", "whenet_debug_jpeg_optimal_table", "whenet_debug_jpeg_optimal_table_gpu",
     "whenet_jpeg_info", "whenet_decode_jpeg_u8", "whenet_debug_jpeg_piece_bits", "whenet_jpeg_info_ex", "whenet_decode_jpeg_ex_u8",
+    "whenet_det_detect_yuv422_u8", "whenet_det_detect_ragged_yuv422_u8", "whenet_crop_boxes_yuv422_u8", "whenet_crop_boxes_ragged_yuv422_u8",
+    "whenet_yuv_to_bgr_u8", "whenet_yuv_to_bgr_ragged_u8",
 ]
 
 # pixel_format -> the ABI's yuv_layout (WHENET_YUV_NV12 / WHENET_YUV_I420); "bgr" is packed 8-bit BGR, the *_u8 entries
 YUV_LAYOUTS = {"nv12": 1, "i420": 2}
+# pixel_format -> the ABI's yuv422_layout (WHENET_YUV_YUYV / WHENET_YUV_UYVY), the *_yuv422_u8 entries
+YUV422_LAYOUTS = {"yuyv": 3, "uyvy": 4}
 
 
 class WhenetError(RuntimeError):
@@ -91,6 +95,10 @@ def load():
     L.whenet_crop_boxes_ragged_u8.argtypes = [P, P, P, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P]
     L.whenet_crop_boxes_yuv_u8.argtypes = L.whenet_crop_boxes_u8.argtypes
     L.whenet_crop_boxes_ragged_yuv_u8.argtypes = L.whenet_crop_boxes_ragged_u8.argtypes
+    L.whenet_crop_boxes_yuv422_u8.argtypes = L.whenet_crop_boxes_u8.argtypes
+    L.whenet_crop_boxes_ragged_yuv422_u8.argtypes = L.whenet_crop_boxes_ragged_u8.argtypes
+    L.whenet_yuv_to_bgr_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P]
+    L.whenet_yuv_to_bgr_ragged_u8.argtypes = [P, P, P, C.c_int, C.c_int, C.c_int, P]
     L.whenet_debug_enlarge_boxes.argtypes = [P, C.c_int, C.c_int, C.c_int, P, P]
     L.whenet_draw_heads_u8.argtypes = [P, P, C.c_int, C.c_int, C.c_int, P, P, P, C.c_int, P]
     L.whenet_draw_heads_ragged_u8.argtypes = [P, P, P, C.c_int, P, P, P, C.c_int, P]
@@ -147,6 +155,8 @@ def load():
     L.whenet_det_detect_ragged_u8.argtypes = [P, P, P, I, I, I, C.c_float, C.c_float, I, P, P, P, P]
     L.whenet_det_detect_yuv_u8.argtypes = L.whenet_det_detect_u8.argtypes
     L.whenet_det_detect_ragged_yuv_u8.argtypes = L.whenet_det_detect_ragged_u8.argtypes
+    L.whenet_det_detect_yuv422_u8.argtypes = L.whenet_det_detect_u8.argtypes
+    L.whenet_det_detect_ragged_yuv422_u8.argtypes = L.whenet_det_detect_ragged_u8.argtypes
     L.whenet_det_synchronize.argtypes = [P]
     L.whenet_det_destroy.argtypes = [P]
     L.whenet_det_destroy.restype = None

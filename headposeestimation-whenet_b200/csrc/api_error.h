@@ -27,5 +27,13 @@ inline int check_yuv_layout(int yuv_layout) {
     return 0;
 }
 
+// the yuv422_layout argument of the *_yuv422_u8 entry points
+inline int check_yuv422_layout(int yuv422_layout) {
+    if (yuv422_layout != WHENET_YUV_YUYV && yuv422_layout != WHENET_YUV_UYVY)
+        return fail(WHENET_EINVAL, "yuv422_layout=%d: WHENET_YUV_YUYV (%d) or WHENET_YUV_UYVY (%d)", yuv422_layout, WHENET_YUV_YUYV,
+                    WHENET_YUV_UYVY);
+    return 0;
+}
+
 }  // namespace api
 }  // namespace whenet

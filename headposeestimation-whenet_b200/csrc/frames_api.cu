@@ -1,6 +1,7 @@
-// frames_api.cu - the frame crops (whenet_crop_resize_u8, whenet_crop_boxes_*), head overlay (whenet_draw_heads*) and text
-// (whenet_put_text*) of the C ABI, with their debug entries (DESIGN.md sections 8.2, 8.4, 8.5, 8.7 and 8.8): the host geometry
-// and the launches of kernels_crop.cuh and kernels_overlay.cuh on the context's stream.
+// frames_api.cu - the frame crops (whenet_crop_resize_u8, whenet_crop_boxes_*), head overlay (whenet_draw_heads*), text
+// (whenet_put_text*) and YUV -> BGR frame conversion (whenet_yuv_to_bgr_*) of the C ABI, with their debug entries (DESIGN.md
+// sections 8.2, 8.4, 8.5, 8.7, 8.8 and 8.14): the host geometry and the launches of kernels_crop.cuh, kernels_overlay.cuh and
+// yuv.cuh on the context's stream.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -20,6 +21,7 @@
 #include "kernels_overlay.cuh"
 
 using whenet::Scope;
+using whenet::api::check_yuv422_layout;
 using whenet::api::check_yuv_layout;
 using whenet::api::fail;
 namespace F = whenet::frames;
@@ -121,9 +123,13 @@ bool enlarge_box(const float* b, int H, int W, int32_t r[4]) {
 }
 
 static_assert(whenet::kYuvNV12 == WHENET_YUV_NV12 && whenet::kYuvI420 == WHENET_YUV_I420, "layout codes of yuv.cuh and the ABI");
+static_assert(whenet::kYuvYUYV == WHENET_YUV_YUYV && whenet::kYuvUYVY == WHENET_YUV_UYVY, "layout codes of yuv.cuh and the ABI");
 
-// bytes of an H x W frame: packed 8-bit BGR / RGB (yuv_layout 0) or YUV 4:2:0 (H and W even)
-size_t frame_bytes(int H, int W, int yuv_layout) { return yuv_layout ? (size_t)H * W / 2 * 3 : (size_t)H * W * 3; }
+// bytes of an H x W frame: packed 8-bit BGR / RGB (yuv_layout 0), YUV 4:2:0 (H and W even) or packed YUV 4:2:2 (W even)
+size_t frame_bytes(int H, int W, int yuv_layout) {
+    if (whenet::yuv422(yuv_layout)) return (size_t)H * W * 2;
+    return yuv_layout ? (size_t)H * W / 2 * 3 : (size_t)H * W * 3;
+}
 
 // The crop table -> crop_resize_kernel<Frames> (yuv_layout 0) or crop_resize_yuv_kernel<Frames, yuv_layout>, one launch per 65535
 // crops (the grid's y limit).  rects: m x (y0, y1, x0, x1) host int32, an empty one marks a zero crop; frame_of: m host frame
@@ -144,6 +150,10 @@ int launch_crop_kernel(whenet_ctx* c, const F::Target& t, F::State* st, const Fr
             whenet::crop_resize_yuv_kernel<Frames, whenet::kYuvNV12><<<grid, 256, 0, t.stream>>>(src, st->d_rects + m0, fo, out);
         else if (yuv_layout == whenet::kYuvI420)
             whenet::crop_resize_yuv_kernel<Frames, whenet::kYuvI420><<<grid, 256, 0, t.stream>>>(src, st->d_rects + m0, fo, out);
+        else if (yuv_layout == whenet::kYuvYUYV)
+            whenet::crop_resize_yuv_kernel<Frames, whenet::kYuvYUYV><<<grid, 256, 0, t.stream>>>(src, st->d_rects + m0, fo, out);
+        else if (yuv_layout == whenet::kYuvUYVY)
+            whenet::crop_resize_yuv_kernel<Frames, whenet::kYuvUYVY><<<grid, 256, 0, t.stream>>>(src, st->d_rects + m0, fo, out);
         else
             whenet::crop_resize_kernel<Frames><<<grid, 256, 0, t.stream>>>(src, st->d_rects + m0, fo, out, swap_rb);
         CK(cudaGetLastError());
@@ -188,14 +198,16 @@ int launch_crops_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32
     return launch_crop_kernel(c, t, st, src, rects, frame_of, m, swap_rb, yuv_layout, crops_out);
 }
 
-// whenet_crop_boxes_u8 (yuv_layout 0) and whenet_crop_boxes_yuv_u8
+// whenet_crop_boxes_u8 (yuv_layout 0), whenet_crop_boxes_yuv_u8 and whenet_crop_boxes_yuv422_u8
 int crop_boxes(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes, const int32_t* frame_of,
                int m, int swap_rb, int yuv_layout, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
     // the context is checked last so that every other argument can be validated without a GPU
     if (!frames || !boxes || !frame_of || !crops_out) return fail(WHENET_EINVAL, "null frames, boxes, frame_of or crops_out");
     if (n < 1 || n > 64) return fail(WHENET_EINVAL, "n=%d frames outside [1, 64]", n);
     if (H < 1 || W < 1) return fail(WHENET_EINVAL, "bad frame size %dx%d", H, W);
-    if (yuv_layout && (H > 16384 || W > 16384 || H % 2 || W % 2))
+    if (whenet::yuv422(yuv_layout) && (H > 16384 || W < 2 || W > 16384 || W % 2))
+        return fail(WHENET_EINVAL, "frame size %dx%d: a 4:2:2 frame has an even width in [2, 16384] and a height of at most 16384", H, W);
+    if (yuv_layout && !whenet::yuv422(yuv_layout) && (H > 16384 || W > 16384 || H % 2 || W % 2))
         return fail(WHENET_EINVAL, "frame size %dx%d: a 4:2:0 frame has even sides of at most 16384", H, W);
     if (m < 1) return fail(WHENET_EINVAL, "m=%d boxes", m);
     for (int i = 0; i < m; ++i)
@@ -210,7 +222,7 @@ int crop_boxes(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int fr
     return launch_crops(c, frames, n, H, W, frames_are_device, rects.data(), frame_of, m, swap_rb, yuv_layout, crops_out);
 }
 
-// whenet_crop_boxes_ragged_u8 (yuv_layout 0) and whenet_crop_boxes_ragged_yuv_u8
+// whenet_crop_boxes_ragged_u8 (yuv_layout 0), whenet_crop_boxes_ragged_yuv_u8 and whenet_crop_boxes_ragged_yuv422_u8
 int crop_boxes_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, const float* boxes,
                       const int32_t* frame_of, int m, int swap_rb, int yuv_layout, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
     // the context is checked last so that every other argument can be validated without a GPU
@@ -220,7 +232,9 @@ int crop_boxes_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t
         if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
         if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
             return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
-        if (yuv_layout && (hw[2 * i] % 2 || hw[2 * i + 1] % 2))
+        if (whenet::yuv422(yuv_layout) && hw[2 * i + 1] % 2)
+            return fail(WHENET_EINVAL, "frame %d: frame size %dx%d: a 4:2:2 frame has an even width", i, hw[2 * i + 1], hw[2 * i]);
+        if (yuv_layout && !whenet::yuv422(yuv_layout) && (hw[2 * i] % 2 || hw[2 * i + 1] % 2))
             return fail(WHENET_EINVAL, "frame %d: frame size %dx%d: a 4:2:0 frame has even sides", i, hw[2 * i + 1], hw[2 * i]);
     }
     if (m < 1) return fail(WHENET_EINVAL, "m=%d boxes", m);
@@ -234,6 +248,86 @@ int crop_boxes_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t
     }
     if (rects_out) memcpy(rects_out, rects.data(), rects.size() * sizeof(int32_t));
     return launch_crops_ragged(c, frames, hw, n, frames_are_device, rects.data(), frame_of, m, swap_rb, yuv_layout, crops_out);
+}
+
+// ----------------------------------------------------------------------------- YUV -> BGR frames (DESIGN.md section 8.14)
+// the layout argument of whenet_yuv_to_bgr_*
+int check_convert_layout(int layout) {
+    if (layout < WHENET_YUV_NV12 || layout > WHENET_YUV_UYVY)
+        return fail(WHENET_EINVAL, "layout=%d: WHENET_YUV_NV12 (%d), WHENET_YUV_I420 (%d), WHENET_YUV_YUYV (%d) or WHENET_YUV_UYVY (%d)", layout,
+                    WHENET_YUV_NV12, WHENET_YUV_I420, WHENET_YUV_YUYV, WHENET_YUV_UYVY);
+    return 0;
+}
+
+// an H x W frame of the layout: sides in [1, 16384], W even, H even for 4:2:0.  i: the frame's index in the message, or -1
+int check_convert_size(int i, int H, int W, int layout) {
+    char pre[32] = "";
+    if (i >= 0) snprintf(pre, sizeof(pre), "frame %d: ", i);
+    if (H < 1 || W < 1 || H > 16384 || W > 16384) return fail(WHENET_EINVAL, "%sframe size %dx%d: sides must be in [1, 16384]", pre, W, H);
+    if (whenet::yuv422(layout) && W % 2) return fail(WHENET_EINVAL, "%sframe size %dx%d: a 4:2:2 frame has an even width", pre, W, H);
+    if (!whenet::yuv422(layout) && (H % 2 || W % 2)) return fail(WHENET_EINVAL, "%sframe size %dx%d: a 4:2:0 frame has even sides", pre, W, H);
+    return 0;
+}
+
+// pixel pairs (4:2:2) or 2 x 2 blocks (4:2:0) of an H x W frame: the threads of yuv_to_bgr_kernel
+long long convert_units(int H, int W, int layout) { return (long long)(whenet::yuv422(layout) ? H : H / 2) * (W / 2); }
+
+// The frame table (src: device frames) -> one yuv_to_bgr_kernel launch on the context's stream
+int launch_convert(whenet_ctx* c, const F::Target& t, const whenet::YuvConvertFrames& tab, int n, int layout) {
+    long long units = 0;
+    double bytes = 0.0;
+    for (int i = 0; i < n; ++i) {
+        units = std::max(units, convert_units(tab.f[i].H, tab.f[i].W, layout));
+        bytes += (double)frame_bytes(tab.f[i].H, tab.f[i].W, layout) + 3.0 * tab.f[i].H * tab.f[i].W;
+    }
+    Scope sc(c, t.stream, "yuv_to_bgr", bytes, 0.0);
+    const dim3 grid((unsigned)((units + 255) / 256), n);
+    switch (layout) {
+        case whenet::kYuvNV12: whenet::yuv_to_bgr_kernel<whenet::kYuvNV12><<<grid, 256, 0, t.stream>>>(tab); break;
+        case whenet::kYuvI420: whenet::yuv_to_bgr_kernel<whenet::kYuvI420><<<grid, 256, 0, t.stream>>>(tab); break;
+        case whenet::kYuvYUYV: whenet::yuv_to_bgr_kernel<whenet::kYuvYUYV><<<grid, 256, 0, t.stream>>>(tab); break;
+        case whenet::kYuvUYVY: whenet::yuv_to_bgr_kernel<whenet::kYuvUYVY><<<grid, 256, 0, t.stream>>>(tab); break;
+        default: return fail(WHENET_EINVAL, "layout=%d", layout);
+    }
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// n frames of one size; host frames are uploaded into the staging buffer in one copy
+int yuv_to_bgr(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, int layout, uint8_t* out) {
+    const F::Target t = F::target(c);
+    F::State* st;
+    if (int rc = frame_state(t, st)) return rc;
+    const size_t fb = frame_bytes(H, W, layout);
+    if (!frames_are_device) {
+        if (int rc = upload(t, &st->d_frame, &st->frame_cap, frames, n * fb)) return rc;
+        frames = st->d_frame;
+    }
+    whenet::YuvConvertFrames tab{};
+    for (int i = 0; i < n; ++i) tab.f[i] = {frames + i * fb, out + (size_t)i * H * W * 3, H, W};
+    return launch_convert(c, t, tab, n, layout);
+}
+
+// n frames of their own sizes; host frames are uploaded into the staging buffer at 256-byte aligned offsets
+int yuv_to_bgr_ragged(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int layout,
+                      uint8_t* const* out) {
+    const F::Target t = F::target(c);
+    F::State* st;
+    if (int rc = frame_state(t, st)) return rc;
+    std::vector<size_t> off(n);
+    size_t total = 0;
+    for (int i = 0; i < n; ++i) {
+        off[i] = total;
+        total += (frame_bytes(hw[2 * i], hw[2 * i + 1], layout) + 255) & ~(size_t)255;
+    }
+    if (!frames_are_device) {
+        if (int rc = grow(&st->d_frame, &st->frame_cap, total)) return rc;
+        for (int i = 0; i < n; ++i)
+            CK(cudaMemcpyAsync(st->d_frame + off[i], frames[i], frame_bytes(hw[2 * i], hw[2 * i + 1], layout), cudaMemcpyHostToDevice, t.stream));
+    }
+    whenet::YuvConvertFrames tab{};
+    for (int i = 0; i < n; ++i) tab.f[i] = {frames_are_device ? frames[i] : st->d_frame + off[i], out[i], hw[2 * i], hw[2 * i + 1]};
+    return launch_convert(c, t, tab, n, layout);
 }
 
 // ----------------------------------------------------------------------------- head overlay (DESIGN.md section 8.7)
@@ -656,6 +750,42 @@ int whenet_crop_boxes_ragged_yuv_u8(whenet_ctx* c, const uint8_t* const* frames,
                                     int32_t* valid_out) {
     if (int rc = check_yuv_layout(yuv_layout)) return rc;
     return crop_boxes_ragged(c, frames, hw, n, frames_are_device, boxes, frame_of, m, 1, yuv_layout, crops_out, rects_out, valid_out);
+}
+
+int whenet_crop_boxes_yuv422_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, const float* boxes,
+                                const int32_t* frame_of, int m, int yuv422_layout, uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out) {
+    if (int rc = check_yuv422_layout(yuv422_layout)) return rc;
+    return crop_boxes(c, frames, n, H, W, frames_are_device, boxes, frame_of, m, 1, yuv422_layout, crops_out, rects_out, valid_out);
+}
+
+int whenet_crop_boxes_ragged_yuv422_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                       const float* boxes, const int32_t* frame_of, int m, int yuv422_layout, uint8_t* crops_out,
+                                       int32_t* rects_out, int32_t* valid_out) {
+    if (int rc = check_yuv422_layout(yuv422_layout)) return rc;
+    return crop_boxes_ragged(c, frames, hw, n, frames_are_device, boxes, frame_of, m, 1, yuv422_layout, crops_out, rects_out, valid_out);
+}
+
+int whenet_yuv_to_bgr_u8(whenet_ctx* c, const uint8_t* frames, int n, int H, int W, int frames_are_device, int layout, uint8_t* out_frames) {
+    // the context is checked last so that every other argument can be validated without a GPU
+    if (int rc = check_convert_layout(layout)) return rc;
+    if (!frames || !out_frames) return fail(WHENET_EINVAL, "null frames or out_frames");
+    if (n < 1 || n > whenet::kMaxConvertFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxConvertFrames);
+    if (int rc = check_convert_size(-1, H, W, layout)) return rc;
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    return yuv_to_bgr(c, frames, n, H, W, frames_are_device, layout, out_frames);
+}
+
+int whenet_yuv_to_bgr_ragged_u8(whenet_ctx* c, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int layout,
+                                uint8_t* const* out_frames) {
+    if (int rc = check_convert_layout(layout)) return rc;
+    if (!frames || !hw || !out_frames) return fail(WHENET_EINVAL, "null frames, hw or out_frames");
+    if (n < 1 || n > whenet::kMaxConvertFrames) return fail(WHENET_EINVAL, "n=%d frames outside [1, %d]", n, whenet::kMaxConvertFrames);
+    for (int i = 0; i < n; ++i) {
+        if (!frames[i] || !out_frames[i]) return fail(WHENET_EINVAL, "frame %d: null frame or output", i);
+        if (int rc = check_convert_size(i, hw[2 * i], hw[2 * i + 1], layout)) return rc;
+    }
+    if (!c) return fail(WHENET_EINVAL, "null context");
+    return yuv_to_bgr_ragged(c, frames, hw, n, frames_are_device, layout, out_frames);
 }
 
 int whenet_draw_heads_u8(whenet_ctx* c, uint8_t* frames, int n, int H, int W, const float* boxes, const float* angles,

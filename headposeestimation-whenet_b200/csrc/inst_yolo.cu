@@ -16,6 +16,12 @@ int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in,
         case kYuvI420:
             letterbox_h_yuv_kernel<kYuvI420><<<grid_h, 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx);
             break;
+        case kYuvYUYV:
+            letterbox_h_yuv_kernel<kYuvYUYV><<<grid_h, 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx);
+            break;
+        case kYuvUYVY:
+            letterbox_h_yuv_kernel<kYuvUYVY><<<grid_h, 256, 0, s>>>(in, tmp, lp.H, lp.W, lp.nw, lp.y0, lp.rows, lp.xb, lp.kx, lp.ksx);
+            break;
         default: return (int)cudaErrorInvalidValue;
     }
     letterbox_v_kernel<<<dim3((unsigned)((S_h * S_w + 255) / 256), n), 256, 0, s>>>(tmp, out, lp.nw, lp.nh, lp.rows, S_h, S_w, lp.ox, lp.oy,
@@ -30,6 +36,8 @@ int launch_letterbox_ragged(cudaStream_t s, const LetterboxFrame* plans, const c
         case 0: letterbox_h_ragged_kernel<<<grid_h, 256, 0, s>>>(plans, coef, in, tmp, swap_rb); break;
         case kYuvNV12: letterbox_h_ragged_yuv_kernel<kYuvNV12><<<grid_h, 256, 0, s>>>(plans, coef, in, tmp); break;
         case kYuvI420: letterbox_h_ragged_yuv_kernel<kYuvI420><<<grid_h, 256, 0, s>>>(plans, coef, in, tmp); break;
+        case kYuvYUYV: letterbox_h_ragged_yuv_kernel<kYuvYUYV><<<grid_h, 256, 0, s>>>(plans, coef, in, tmp); break;
+        case kYuvUYVY: letterbox_h_ragged_yuv_kernel<kYuvUYVY><<<grid_h, 256, 0, s>>>(plans, coef, in, tmp); break;
         default: return (int)cudaErrorInvalidValue;
     }
     letterbox_v_ragged_kernel<<<dim3((unsigned)((S_h * S_w + 255) / 256), n), 256, 0, s>>>(plans, coef, tmp, out, S_h, S_w);

@@ -6,7 +6,7 @@
 // ((b0*(r0>>4))>>16) + ((b1*(r1>>4))>>16) + 2 >> 2 vertical pass, 2x2 box for exact 2x down-scaling.
 // All heads of one frame, of n frames of one size or of n frames of their own sizes come out as ONE uint8 NHWC batch that feeds the
 // stem kernel directly - the reference crops, resizes and runs the network one head at a time
-// (demo_video.py:13-23, 57-58).  crop_resize_yuv_kernel does the same on NV12 / I420 frames (yuv.cuh).
+// (demo_video.py:13-23, 57-58).  crop_resize_yuv_kernel does the same on NV12 / I420 / YUYV / UYVY frames (yuv.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -102,7 +102,8 @@ __global__ void __launch_bounds__(256) crop_resize_kernel(const __grid_constant_
     else { dst[0] = (uint8_t)v[0]; dst[1] = (uint8_t)v[1]; dst[2] = (uint8_t)v[2]; }
 }
 
-// crop_resize_kernel on YUV 4:2:0 frames in layout L (yuv.cuh; OneSizeFrames: H * W * 3/2 bytes apart): each source pixel the
+// crop_resize_kernel on YUV frames in layout L (yuv.cuh; OneSizeFrames: H * W * 3/2 bytes apart for 4:2:0, H * W * 2 for
+// 4:2:2): each source pixel the
 // resize reads is converted to B, G, R first, and the crop is written in RGB order, so it is the crop crop_resize_kernel
 // gives with swap_rb on cv2.cvtColor's output.
 template <class Frames, int L>
@@ -123,7 +124,7 @@ __global__ void __launch_bounds__(256) crop_resize_yuv_kernel(const __grid_const
         H = src_frames.H;
         W = src_frames.W;
         const long long f = frame_of ? frame_of[m] : 0;
-        frame = src_frames.frames + f * H * W / 2 * 3;
+        frame = src_frames.frames + yuv_frame_offset<L>(f, H, W);
     } else {
         const auto& fr = src_frames.f[frame_of[m]];
         H = fr.H;

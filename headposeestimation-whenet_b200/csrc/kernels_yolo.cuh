@@ -5,7 +5,8 @@
 //                                             the host exactly as ImagingResample does) + the (128,128,128) canvas and the paste
 //                                             (reference utils.py:23-34)
 //   letterbox_{h,v}_ragged_kernel              the same two passes over frames of different sizes, one LetterboxFrame each
-//   letterbox_h{,_ragged}_yuv_kernel<L>        the horizontal passes over NV12 / I420 frames, converting each pixel as it is read
+//   letterbox_h{,_ragged}_yuv_kernel<L>        the horizontal passes over NV12 / I420 / YUYV / UYVY frames, converting each pixel
+//                                             as it is read
 //   yolo_conv0_kernel<N>                       first conv (3 -> N = 32, tiny: 16, 3x3): im2col row built in shared memory from the
 //                                             uint8 canvas through a v/255 table split into bf16 hi + lo parts, one K = 64 wgmma
 //                                             block per row
@@ -216,7 +217,8 @@ struct LetterboxFrame {
     int H, W, nw, nh, ox, oy, y0, rows, ksx, ksy;
     int xb, kx, yb, ky;
 };
-// yuv_layout 0: packed 8-bit frames (BGR when swap_rb); kYuvNV12 / kYuvI420: 4:2:0 frames (yuv.cuh), swap_rb ignored
+// yuv_layout 0: packed 8-bit frames (BGR when swap_rb); kYuvNV12 / kYuvI420 / kYuvYUYV / kYuvUYVY: YUV frames (yuv.cuh),
+// swap_rb ignored
 int launch_letterbox(cudaStream_t s, const LetterboxPlan& lp, const uint8_t* in, uint8_t* tmp, uint8_t* out, int n, int S_h, int S_w, int swap_rb,
                      int yuv_layout);
 // plans: n device LetterboxFrame; max_hx: the largest rows * nw among them
@@ -319,7 +321,7 @@ __global__ void letterbox_h_ragged_kernel(const LetterboxFrame* __restrict__ pla
     dst[2] = clip8(swap_rb ? s0 : s2);
 }
 
-// The horizontal pass over a YUV 4:2:0 frame (yuv.cuh): every tap converts its source pixel to B, G, R and accumulates it as
+// The horizontal pass over a YUV frame (yuv.cuh): every tap converts its source pixel to B, G, R and accumulates it as
 // letterbox_h_kernel does, and the row goes to tmp in RGB order, so tmp holds the bits the BGR pass with swap_rb gives on
 // cv2.cvtColor's output.  frame: the frame's Y plane; y: the source row; x0, count, k: the output column's taps.
 template <int L>
@@ -339,7 +341,7 @@ __device__ __forceinline__ void letterbox_h_yuv_taps(const uint8_t* __restrict__
     dst[2] = clip8(s0);
 }
 
-// letterbox_h_kernel on n YUV frames of one size, H * W * 3/2 bytes each
+// letterbox_h_kernel on n YUV frames of one size, H * W * 3/2 (4:2:0) or H * W * 2 (4:2:2) bytes each
 template <int L>
 __global__ void letterbox_h_yuv_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ tmp, int H, int W, int nw, int y0, int rows,
                                        const int2* __restrict__ xb, const int* __restrict__ kx, int ksize) {
@@ -348,7 +350,7 @@ __global__ void letterbox_h_yuv_kernel(const uint8_t* __restrict__ in, uint8_t* 
     if (i >= (long long)rows * nw) return;
     const int r = (int)(i / nw), x = (int)(i - (long long)r * nw);
     const int2 b = xb[x];
-    letterbox_h_yuv_taps<L>(in + (long long)f * H * W / 2 * 3, H, W, y0 + r, b.x, b.y, kx + (long long)x * ksize,
+    letterbox_h_yuv_taps<L>(in + yuv_frame_offset<L>(f, H, W), H, W, y0 + r, b.x, b.y, kx + (long long)x * ksize,
                             tmp + (((long long)f * rows + r) * nw + x) * 3);
 }
 

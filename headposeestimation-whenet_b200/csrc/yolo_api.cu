@@ -19,6 +19,7 @@
 #include "kernels_yolo.cuh"
 #include "kernels_yolo32.cuh"
 
+using whenet::api::check_yuv422_layout;
 using whenet::api::check_yuv_layout;
 using whenet::api::fail;
 namespace Y = whenet::yolo;
@@ -74,9 +75,13 @@ constexpr size_t kMaxGraphs = 16;   // captured graphs kept per cache
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 static_assert(whenet::kYuvNV12 == WHENET_YUV_NV12 && whenet::kYuvI420 == WHENET_YUV_I420, "layout codes of yuv.cuh and the ABI");
+static_assert(whenet::kYuvYUYV == WHENET_YUV_YUYV && whenet::kYuvUYVY == WHENET_YUV_UYVY, "layout codes of yuv.cuh and the ABI");
 
-// bytes of an H x W frame: packed 8-bit BGR / RGB (yuv_layout 0) or YUV 4:2:0 (H and W even)
-size_t frame_bytes(int H, int W, int yuv_layout) { return yuv_layout ? (size_t)H * W / 2 * 3 : (size_t)H * W * 3; }
+// bytes of an H x W frame: packed 8-bit BGR / RGB (yuv_layout 0), YUV 4:2:0 (H and W even) or packed YUV 4:2:2 (W even)
+size_t frame_bytes(int H, int W, int yuv_layout) {
+    if (whenet::yuv422(yuv_layout)) return (size_t)H * W * 2;
+    return yuv_layout ? (size_t)H * W / 2 * 3 : (size_t)H * W * 3;
+}
 
 // Pillow ImagingResample (libImaging/Resample.c) coefficient tables for BICUBIC: support 2 scaled by the downscale factor,
 // weights normalised in double and quantised to 22 bits (normalize_coeffs_8bpc).
@@ -698,7 +703,7 @@ int whenet_det_set_stream(whenet_det* d, void* s) {
 
 namespace {
 
-// whenet_det_detect_u8 (yuv_layout 0) and whenet_det_detect_yuv_u8 after their argument checks
+// whenet_det_detect_u8 (yuv_layout 0), whenet_det_detect_yuv_u8 and whenet_det_detect_yuv422_u8 after their argument checks
 int detect_one_size(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int swap_rb, int yuv_layout, float score,
                     float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
     CKD(cudaSetDevice(d->device));
@@ -727,7 +732,7 @@ int detect_one_size(whenet_det* d, const uint8_t* frames, int n, int H, int W, i
     return run_decode(d, decode_params(d, n, nullptr, H, W, score, iou, max_boxes), n, boxes, scores, classes, counts);
 }
 
-// whenet_det_detect_ragged_u8 (yuv_layout 0) and whenet_det_detect_ragged_yuv_u8
+// whenet_det_detect_ragged_u8 (yuv_layout 0), whenet_det_detect_ragged_yuv_u8 and whenet_det_detect_ragged_yuv422_u8
 int detect_ragged(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device, int swap_rb, int yuv_layout,
                   float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
     // the detector is checked after every argument that can be validated without a GPU
@@ -737,7 +742,9 @@ int detect_ragged(whenet_det* d, const uint8_t* const* frames, const int32_t* hw
         if (!frames[i]) return fail(WHENET_EINVAL, "frame %d is NULL", i);
         if (hw[2 * i] < 1 || hw[2 * i + 1] < 1 || hw[2 * i] > 16384 || hw[2 * i + 1] > 16384)
             return fail(WHENET_EINVAL, "frame %d: bad frame size %dx%d", i, hw[2 * i + 1], hw[2 * i]);
-        if (yuv_layout && (hw[2 * i] % 2 || hw[2 * i + 1] % 2))
+        if (whenet::yuv422(yuv_layout) && hw[2 * i + 1] % 2)
+            return fail(WHENET_EINVAL, "frame %d: frame size %dx%d: a 4:2:2 frame has an even width", i, hw[2 * i + 1], hw[2 * i]);
+        if (yuv_layout && !whenet::yuv422(yuv_layout) && (hw[2 * i] % 2 || hw[2 * i + 1] % 2))
             return fail(WHENET_EINVAL, "frame %d: frame size %dx%d: a 4:2:0 frame has even sides", i, hw[2 * i + 1], hw[2 * i]);
     }
     if (!boxes || !scores || !classes || !counts) return fail(WHENET_EINVAL, "null output pointer");
@@ -813,6 +820,28 @@ int whenet_det_detect_ragged_yuv_u8(whenet_det* d, const uint8_t* const* frames,
                                     float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
     if (int rc = check_yuv_layout(yuv_layout)) return rc;
     return detect_ragged(d, frames, hw, n, frames_are_device, 1, yuv_layout, score, iou, max_boxes, boxes, scores, classes, counts);
+}
+
+int whenet_det_detect_yuv422_u8(whenet_det* d, const uint8_t* frames, int n, int H, int W, int frames_are_device, int yuv422_layout, float score,
+                                float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts) {
+    // the detector is checked after every argument that can be validated without a GPU
+    if (int rc = check_yuv422_layout(yuv422_layout)) return rc;
+    if (!frames) return fail(WHENET_EINVAL, "null frames");
+    if (n < 1 || n > Y::kMaxFrames) return fail(WHENET_EINVAL, "n=%d outside [1, %d]", n, Y::kMaxFrames);
+    if (H < 1 || W < 2 || H > 16384 || W > 16384 || W % 2)
+        return fail(WHENET_EINVAL, "frame size %dx%d: a 4:2:2 frame has an even width in [2, 16384] and a height in [1, 16384]", W, H);
+    if (!boxes || !scores || !classes || !counts) return fail(WHENET_EINVAL, "null output pointer");
+    if (!d) return fail(WHENET_EINVAL, "null detector");
+    if (n > d->max_frames) return fail(WHENET_EINVAL, "n=%d outside [1, max_frames=%d]", n, d->max_frames);
+    if (int rc = check_decode_args(d, score, iou, max_boxes, boxes, scores, classes, counts)) return rc;
+    return detect_one_size(d, frames, n, H, W, frames_are_device, 1, yuv422_layout, score, iou, max_boxes, boxes, scores, classes, counts);
+}
+
+int whenet_det_detect_ragged_yuv422_u8(whenet_det* d, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                       int yuv422_layout, float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes,
+                                       int32_t* counts) {
+    if (int rc = check_yuv422_layout(yuv422_layout)) return rc;
+    return detect_ragged(d, frames, hw, n, frames_are_device, 1, yuv422_layout, score, iou, max_boxes, boxes, scores, classes, counts);
 }
 
 int whenet_det_synchronize(whenet_det* d) {

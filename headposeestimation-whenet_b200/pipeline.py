@@ -9,7 +9,7 @@ import numpy as np
 from . import crops as _crops
 from ._lib import WhenetError, check
 from .whenet import _is_device, _ptr
-from .yolo import _frame_list, _frame_table, _image_size, _pixel_layout, _yuv_image_size
+from .yolo import _entry_name, _frame_list, _frame_table, _image_size, _is_422, _pixel_layout, _yuv422_image_size, _yuv_image_size
 
 
 def detect_and_estimate(yolo, whenet, frame_bgr, *, pixel_format="bgr"):
@@ -17,10 +17,12 @@ def detect_and_estimate(yolo, whenet, frame_bgr, *, pixel_format="bgr"):
     yaw/pitch/roll in degrees).  The one-frame case of ``detect_and_estimate_frames``, except that a head whose slice is
     empty or outside the frame raises ``WhenetError`` (code -1, naming the box and its slice) as cv2.resize raises in the
     reference, instead of getting NaN angles.  ``pixel_format="nv12"`` / ``"i420"``: an (H * 3/2, W) YUV 4:2:0 frame in
-    cv2's layout (see ``detect_and_estimate_frames``)."""
+    cv2's layout, ``"yuyv"`` / ``"uyvy"``: an (H, W, 2) packed YUV 4:2:2 frame (see ``detect_and_estimate_frames``)."""
     layout = _pixel_layout(pixel_format)
     frame = np.ascontiguousarray(frame_bgr, dtype=np.uint8)
-    if layout:
+    if _is_422(layout):
+        _yuv422_image_size(frame.shape, "frame")
+    elif layout:
         _yuv_image_size(frame.shape, "frame")
     elif frame.ndim != 3 or frame.shape[2] != 3:
         raise ValueError("frame must be H x W x 3 uint8")
@@ -48,7 +50,13 @@ def detect_and_estimate_frames(yolo, whenet, frames_bgr, *, pixel_format="bgr"):
     ``pixel_format="nv12"`` or ``"i420"`` takes YUV 4:2:0 video frames in cv2's layout (what hardware and software video
     decoders hand out) instead of BGR: (n, H * 3/2, W) uint8, or a list or tuple of (H_i * 3/2, W_i) frames, H and W even.
     The letterbox and the crops convert each pixel as they read it, so host frames upload half the bytes of BGR frames, and
-    the results are the bits ``detect_and_estimate_frames`` gives on ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12 / _I420)``."""
+    the results are the bits ``detect_and_estimate_frames`` gives on ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12 / _I420)``.
+
+    ``pixel_format="yuyv"`` or ``"uyvy"`` takes packed YUV 4:2:2 frames (what raw webcams, V4L2 and GStreamer pipelines and
+    HDMI capture cards hand out): (n, H, W, 2) uint8, or a list or tuple of (H_i, W_i, 2) frames, W even, any H.  Host frames
+    upload 2 bytes per pixel, and the results are the bits ``detect_and_estimate_frames`` gives on
+    ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_YUYV / _UYVY)``.  ``video.to_bgr`` turns the same frames into BGR frames on the
+    device for ``overlay.draw_heads`` and ``video.encode_jpeg``."""
     return _run(yolo, whenet, frames_bgr, strict=False, pixel_format=pixel_format)
 
 
@@ -75,7 +83,11 @@ def _checked_frames(yolo, whenet, frames, layout):
         frames = np.asarray(frames)
         if frames.dtype != np.uint8:
             raise ValueError("frames must be uint8, not %s" % frames.dtype)
-    if layout:
+    if _is_422(layout):
+        if len(frames.shape) != 4:
+            raise ValueError("frames must be (n, H, W, 2) uint8 for a 4:2:2 pixel format, not %s" % (tuple(frames.shape),))
+        _yuv422_image_size(frames.shape[1:], "a frame")
+    elif layout:
         if len(frames.shape) != 3:
             raise ValueError("frames must be (n, H * 3/2, W) uint8 for a 4:2:0 pixel format, not %s" % (tuple(frames.shape),))
         _yuv_image_size(frames.shape[1:], "a frame")
@@ -99,7 +111,7 @@ def _raise_first_invalid(L, boxes, H, W):
 def _run(yolo, whenet, frames, strict, pixel_format="bgr"):
     layout = _pixel_layout(pixel_format)
     frames = _checked_frames(yolo, whenet, frames, layout)
-    ragged = isinstance(frames, list)       # frames of several sizes; otherwise one (n, H, W, 3) or (n, H * 3/2, W) array or tensor
+    ragged = isinstance(frames, list)       # frames of several sizes; otherwise one (n, H, W, 3), (n, H * 3/2, W) or (n, H, W, 2) array or tensor
     n = len(frames) if ragged else int(frames.shape[0])
     if n == 0:
         return []
@@ -174,11 +186,11 @@ def _run(yolo, whenet, frames, strict, pixel_format="bgr"):
                             keep.append(crop_buf)
                         # layout in place of swap_rb = 1: the YUV entries write RGB crops as the BGR ones do with it
                         if ragged:
-                            crop = L.whenet_crop_boxes_ragged_yuv_u8 if layout else L.whenet_crop_boxes_ragged_u8
+                            crop = getattr(L, _entry_name("whenet_crop_boxes_ragged", layout))
                             check(crop(whenet._h, C.addressof(ptrs), _ptr(hw), nb, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, layout or 1,
                                        _ptr(crop_buf), None, _ptr(valid[s:])))
                         else:
-                            crop = L.whenet_crop_boxes_yuv_u8 if layout else L.whenet_crop_boxes_u8
+                            crop = getattr(L, _entry_name("whenet_crop_boxes", layout))
                             check(crop(whenet._h, _ptr(cur), nb, H, W, 1, _ptr(boxes[s:]), _ptr(frame_of[s:]), mb, layout or 1,
                                        _ptr(crop_buf), None, _ptr(valid[s:])))
                         check(L.whenet_forward_u8(whenet._h, _ptr(crop_buf), mb, 1, _ptr(d_ang[s:s + mb]), None, 1))

@@ -1,5 +1,5 @@
-"""Video on the GPU path: JPEG encoding and decoding of device BGR frames, and Motion-JPEG AVI files (DESIGN.md sections 8.9,
-8.10 and 8.11).
+"""Video on the GPU path: JPEG encoding and decoding of device BGR frames, YUV frames to BGR, and Motion-JPEG AVI files
+(DESIGN.md sections 8.9, 8.10, 8.11 and 8.14).
 
   ``encode_jpeg``   device (or host) BGR or gray frames -> JPEG files, byte-identical to cv2.imencode(".jpg", frame,
                     params) with the quality, sampling, restart, optimise and chroma-quality parameters, encoded by the
@@ -10,6 +10,8 @@
   ``MJPGWriter``    writes those files as an MJPG AVI: what reference demo_video.py:46-47,60 writes through
                     cv2.VideoWriter(..., fourcc 'MJPG'), without the frames leaving the GPU uncompressed
   ``MJPGReader``    reads the JPEG files of an MJPG AVI (the reference's cap.read(), demo_video.py:44,51)
+  ``to_bgr``        NV12, I420, YUYV or UYVY frames (video decoders, raw cameras, capture cards) -> device BGR frames,
+                    bit-identical to cv2.cvtColor, converted by the library's CUDA kernel (``whenet_yuv_to_bgr_u8``)
 
 The reference's loop becomes a transcode on the device::
 
@@ -18,6 +20,13 @@ The reference's loop becomes a transcode on the device::
             results = pipeline.detect_and_estimate_frames(yolo, whenet, frames)
             overlay.draw_heads(whenet, frames, results, display="full")
             w.write(video.encode_jpeg(whenet, frames))
+
+and a camera or decoder loop that hands out YUV frames stays on the device too::
+
+    results = pipeline.detect_and_estimate_frames(yolo, whenet, frames, pixel_format="yuyv")
+    bgr = video.to_bgr(whenet, frames, "yuyv")
+    overlay.draw_heads(whenet, bgr, results, display="full")
+    writer.write(video.encode_jpeg(whenet, bgr))
 """
 from __future__ import annotations
 
@@ -156,6 +165,79 @@ def encode_jpeg(whenet, frames, quality: int = 95, *, sampling: str = "420", res
                                                      C.byref(data), _ptr(offsets)))
             for i in range(hi - lo):
                 out.append(C.string_at(data.value + int(offsets[i]), int(offsets[i + 1] - offsets[i])))
+    return out
+
+
+def to_bgr(whenet, frames, pixel_format: str):
+    """YUV ``frames`` -> BGR frames on ``whenet``'s GPU, each bit-identical to ``cv2.cvtColor(frame, COLOR_YUV2BGR_<fmt>)``:
+    the frames ``overlay.draw_heads`` and ``encode_jpeg`` take.  ``pixel_format`` is
+
+      - ``"nv12"`` or ``"i420"``: YUV 4:2:0 in cv2's layout, (n, H * 3/2, W) uint8 or a list of (H_i * 3/2, W_i), sides even;
+      - ``"yuyv"`` or ``"uyvy"``: packed YUV 4:2:2, (n, H, W, 2) uint8 or a list of (H_i, W_i, 2), W even, any H.
+
+    Frames are a numpy array or a contiguous CUDA tensor on ``whenet.device``, or a list or tuple of them (all host or all
+    device); image sides are 1..16384.  Returns a contiguous (n, H, W, 3) uint8 CUDA tensor, or for a list a list of
+    (H_i, W_i, 3) ones; n = 0 gives an empty tensor or [].  Waits for torch's current stream, then converts in groups of 64
+    frames with one synchronisation each, so the frames are ready on any stream when it returns.  Host frames are uploaded
+    at their own size (2 bytes per pixel for 4:2:2, 1.5 for 4:2:0).  Anything else raises ``ValueError`` before anything runs."""
+    import ctypes as C
+    from ._lib import YUV_LAYOUTS, YUV422_LAYOUTS, check
+    from .whenet import _is_device, _ptr
+    from .yolo import _frame_list as _yuv_frame_list
+    from .yolo import _image_size, _is_422, _yuv422_image_size, _yuv_image_size
+    if not isinstance(pixel_format, str) or pixel_format not in {**YUV_LAYOUTS, **YUV422_LAYOUTS}:
+        raise ValueError("pixel_format must be 'nv12', 'i420', 'yuyv' or 'uyvy', not %r" % (pixel_format,))
+    layout = {**YUV_LAYOUTS, **YUV422_LAYOUTS}[pixel_format]
+    ragged = isinstance(frames, (list, tuple))
+    if ragged:
+        items, dev = _yuv_frame_list(frames, whenet.device, layout)
+        sizes = [_image_size(f.shape, layout) for f in items]
+    else:
+        dev = _is_device(frames)
+        if dev:
+            if str(frames.dtype) != "torch.uint8" or not frames.is_contiguous():
+                raise ValueError("device frames must be a contiguous uint8 CUDA tensor")
+            if frames.device.index != whenet.device:
+                raise ValueError("frames are on cuda:%s, WHENet on cuda:%d" % (frames.device.index, whenet.device))
+        else:
+            frames = np.asarray(frames)
+            if frames.dtype != np.uint8:
+                raise ValueError("frames must be uint8, not %s" % frames.dtype)
+            frames = np.ascontiguousarray(frames)
+        if _is_422(layout):
+            if len(frames.shape) != 4:
+                raise ValueError("frames must be (n, H, W, 2) uint8 for a 4:2:2 pixel format, not %s" % (tuple(frames.shape),))
+            H, W = _yuv422_image_size(frames.shape[1:], "a frame")
+        else:
+            if len(frames.shape) != 3:
+                raise ValueError("frames must be (n, H * 3/2, W) uint8 for a 4:2:0 pixel format, not %s" % (tuple(frames.shape),))
+            H, W = _yuv_image_size(frames.shape[1:], "a frame")
+        sizes = [(H, W)] * int(frames.shape[0])
+    for H, W in sizes:
+        if H > MAX_SIDE or W > MAX_SIDE:
+            raise ValueError("frame size %dx%d: each side must be in [1, %d]" % (W, H, MAX_SIDE))
+    import torch
+    n = len(sizes)
+    cuda = "cuda:%d" % whenet.device
+    if ragged:
+        out = [torch.empty((h, w, 3), dtype=torch.uint8, device=cuda) for h, w in sizes]
+    else:
+        out = torch.empty((n, H, W, 3), dtype=torch.uint8, device=cuda)
+    if n == 0:
+        return out
+    L = whenet._L
+    with torch.cuda.device(whenet.device):
+        torch.cuda.current_stream().synchronize()       # the frames and the outputs' memory are done with on torch's stream
+        for lo in range(0, n, MAX_FRAMES_PER_CALL):
+            hi = min(n, lo + MAX_FRAMES_PER_CALL)
+            if ragged:
+                ptrs = (C.c_void_p * (hi - lo))(*[_ptr(f).value for f in items[lo:hi]])
+                dst = (C.c_void_p * (hi - lo))(*[o.data_ptr() for o in out[lo:hi]])
+                hw = np.array(sizes[lo:hi], np.int32).reshape(-1)
+                check(L.whenet_yuv_to_bgr_ragged_u8(whenet._h, C.addressof(ptrs), _ptr(hw), hi - lo, int(dev), layout, C.addressof(dst)))
+            else:
+                check(L.whenet_yuv_to_bgr_u8(whenet._h, _ptr(frames[lo:hi]), hi - lo, H, W, int(dev), layout, _ptr(out[lo:hi])))
+            whenet.synchronize()
     return out
 
 

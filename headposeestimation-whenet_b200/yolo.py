@@ -57,10 +57,39 @@ def _tensor_list(layers):
 
 def _pixel_layout(pixel_format) -> int:
     """``pixel_format`` -> the C entries' yuv_layout: 0 for "bgr" (packed 8-bit BGR, the *_u8 entries), WHENET_YUV_NV12 for
-    "nv12", WHENET_YUV_I420 for "i420" (the *_yuv_u8 entries).  Raises ValueError otherwise."""
-    if isinstance(pixel_format, str) and (pixel_format == "bgr" or pixel_format in _lib.YUV_LAYOUTS):
-        return _lib.YUV_LAYOUTS.get(pixel_format, 0)
-    raise ValueError("pixel_format must be 'bgr', 'nv12' or 'i420', not %r" % (pixel_format,))
+    "nv12", WHENET_YUV_I420 for "i420" (the *_yuv_u8 entries), WHENET_YUV_YUYV for "yuyv", WHENET_YUV_UYVY for "uyvy" (the
+    *_yuv422_u8 entries).  Raises ValueError otherwise."""
+    if isinstance(pixel_format, str):
+        if pixel_format == "bgr":
+            return 0
+        if pixel_format in _lib.YUV_LAYOUTS:
+            return _lib.YUV_LAYOUTS[pixel_format]
+        if pixel_format in _lib.YUV422_LAYOUTS:
+            return _lib.YUV422_LAYOUTS[pixel_format]
+    raise ValueError("pixel_format must be 'bgr', 'nv12', 'i420', 'yuyv' or 'uyvy', not %r" % (pixel_format,))
+
+
+def _is_422(layout: int) -> bool:
+    """Whether a yuv_layout is packed 4:2:2 (YUYV or UYVY)."""
+    return layout in _lib.YUV422_LAYOUTS.values()
+
+
+def _entry_name(stem: str, layout: int) -> str:
+    """The C entry for frames of ``layout``: ``stem``_u8 (BGR), ``stem``_yuv_u8 (4:2:0) or ``stem``_yuv422_u8 (4:2:2)."""
+    return stem + ("_yuv422_u8" if _is_422(layout) else "_yuv_u8" if layout else "_u8")
+
+
+def _yuv422_image_size(shape, what: str) -> Tuple[int, int]:
+    """The shape of a packed YUV 4:2:2 frame, (H, W, 2) -> its image size (H, W); ValueError naming ``what`` unless the shape
+    is 3-D with two channels, at least one row and an even width of at least 2."""
+    if len(shape) != 3 or int(shape[2]) != 2:
+        raise ValueError("%s must be (H, W, 2) uint8 for a 4:2:2 pixel format, not %s" % (what, tuple(shape)))
+    h, w = int(shape[0]), int(shape[1])
+    if h < 1:
+        raise ValueError("%s has no rows" % what)
+    if w < 2 or w % 2:
+        raise ValueError("%s is %d pixels wide: a 4:2:2 frame has an even width" % (what, w))
+    return h, w
 
 
 def _yuv_image_size(shape, what: str) -> Tuple[int, int]:
@@ -77,12 +106,12 @@ def _yuv_image_size(shape, what: str) -> Tuple[int, int]:
 
 
 def _image_size(shape, layout: int) -> Tuple[int, int]:
-    """(H, W) of a checked frame of the given layout: (H, W, 3) BGR or (H * 3/2, W) YUV 4:2:0."""
-    return (int(shape[0]), int(shape[1])) if not layout else (int(shape[0]) // 3 * 2, int(shape[1]))
+    """(H, W) of a checked frame of the given layout: (H, W, 3) BGR, (H * 3/2, W) YUV 4:2:0 or (H, W, 2) YUV 4:2:2."""
+    return (int(shape[0]), int(shape[1])) if not layout or _is_422(layout) else (int(shape[0]) // 3 * 2, int(shape[1]))
 
 
 def _frame_list(frames, device: int, layout: int = 0):
-    """A list or tuple of (H_i, W_i, 3) uint8 frames (YUV layouts: (H_i * 3/2, W_i)), all numpy arrays or all contiguous CUDA
+    """A list or tuple of (H_i, W_i, 3) uint8 frames (4:2:0 layouts: (H_i * 3/2, W_i); 4:2:2: (H_i, W_i, 2)), all numpy arrays or all contiguous CUDA
     tensors on ``device`` -> (list of C-contiguous frames, whether they are on the device).  Raises ValueError otherwise."""
     frames = list(frames)
     dev = [_is_device(f) for f in frames]
@@ -100,7 +129,9 @@ def _frame_list(frames, device: int, layout: int = 0):
             if f.dtype != np.uint8:
                 raise ValueError("frame %d: frames must be uint8, not %s" % (i, f.dtype))
             f = np.ascontiguousarray(f)
-        if layout:
+        if _is_422(layout):
+            _yuv422_image_size(f.shape, "frame %d" % i)
+        elif layout:
             _yuv_image_size(f.shape, "frame %d" % i)
         elif len(f.shape) != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
             raise ValueError("frame %d: frames must be (H, W, 3) uint8, not %s" % (i, tuple(f.shape)))
@@ -193,7 +224,11 @@ class YOLO:
 
         ``pixel_format="nv12"`` or ``"i420"`` takes YUV 4:2:0 video frames in cv2's layout instead: (n, H * 3/2, W) uint8, or a
         list or tuple of (H_i * 3/2, W_i) frames, H and W even.  The letterbox converts each pixel as it reads it, and the
-        result is the bits ``detect_frames`` gives on ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12 / _I420)``."""
+        result is the bits ``detect_frames`` gives on ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12 / _I420)``.
+
+        ``pixel_format="yuyv"`` or ``"uyvy"`` takes packed YUV 4:2:2 camera frames: (n, H, W, 2) uint8, or a list or tuple of
+        (H_i, W_i, 2) frames, W even, any H.  The result is the bits ``detect_frames`` gives on
+        ``cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_YUYV / _UYVY)``."""
         layout = _pixel_layout(pixel_format)
         if not isinstance(frames_bgr, (list, tuple)):
             return self._detect(frames_bgr, swap_rb=True, layout=layout)
@@ -222,7 +257,7 @@ class YOLO:
         scores = np.empty((nb, slots), np.float32)
         classes = np.empty((nb, slots), np.int32)
         counts = np.empty((nb,), np.int32)
-        fn = self._L.whenet_det_detect_ragged_yuv_u8 if layout else self._L.whenet_det_detect_ragged_u8
+        fn = getattr(self._L, _entry_name("whenet_det_detect_ragged", layout))
         check(fn(self._h, C.addressof(ptrs), _ptr(hw), nb, int(dev), layout or 1, self.score, self.iou, max_boxes,
                  _ptr(boxes), _ptr(scores), _ptr(classes), _ptr(counts)))
         return [(boxes[i, :counts[i]].copy(), scores[i, :counts[i]].copy(), classes[i, :counts[i]].copy()) for i in range(nb)]
@@ -234,7 +269,13 @@ class YOLO:
             frames = np.ascontiguousarray(frames, dtype=np.uint8)
         elif not frames.is_contiguous() or str(frames.dtype) != "torch.uint8":
             raise ValueError("device frames must be a contiguous uint8 CUDA tensor")
-        if layout:
+        if _is_422(layout):
+            if len(frames.shape) != 4:
+                raise ValueError("frames must be (n, H, W, 2) uint8 for a 4:2:2 pixel format, not %s" % (tuple(frames.shape),))
+            H, W = _yuv422_image_size(frames.shape[1:], "a frame")
+            n = int(frames.shape[0])
+            entry, code = "whenet_det_detect_yuv422_u8", layout
+        elif layout:
             if len(frames.shape) != 3:
                 raise ValueError("frames must be (n, H * 3/2, W) uint8 for a 4:2:0 pixel format, not %s" % (tuple(frames.shape),))
             H, W = _yuv_image_size(frames.shape[1:], "a frame")

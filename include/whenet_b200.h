@@ -42,6 +42,12 @@ extern "C" {
  * on cvtColor's output. */
 #define WHENET_YUV_NV12        1
 #define WHENET_YUV_I420        2
+/* Packed YUV 4:2:2 frames (the *_yuv422_u8 entries, and whenet_yuv_to_bgr_*): H x W x 2 uint8, W even, any H, as cameras,
+ * V4L2, GStreamer and HDMI capture cards hand them out.  Row y holds W/2 pixel pairs; pair p is the bytes Y0 U Y1 V (YUYV,
+ * also called YUY2) or U Y0 V Y1 (UYVY) at 4p, and both pixels share its U and V.  The arithmetic is that of the 4:2:0
+ * layouts: cv2.cvtColor's COLOR_YUV2BGR_YUYV / COLOR_YUV2BGR_UYVY. */
+#define WHENET_YUV_YUYV        3
+#define WHENET_YUV_UYVY        4
 
 #define WHENET_IMG        224
 #define WHENET_N_YAW      120      /* reference whenet.py:11 */
@@ -170,6 +176,33 @@ int whenet_crop_boxes_yuv_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int 
 int whenet_crop_boxes_ragged_yuv_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
                                     const float* boxes, const int32_t* frame_of, int m, int yuv_layout,
                                     uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+
+/* whenet_crop_boxes_u8 and whenet_crop_boxes_ragged_u8 on packed YUV 4:2:2 frames (WHENET_YUV_YUYV / WHENET_YUV_UYVY in
+ * `yuv422_layout`, in place of swap_rb): H, W and hw are the image sizes (W even in [2, 16384], H in [1, 16384]), each frame
+ * is H * W * 2 bytes.  Otherwise as the 4:2:0 entries above: each crop is RGB, the bytes the BGR entry with swap_rb gives on
+ * cv2.cvtColor(frame, COLOR_YUV2BGR_YUYV / _UYVY), and every argument but the context is checked before anything touches a
+ * device. */
+int whenet_crop_boxes_yuv422_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, int W, int frames_are_device,
+                                const float* boxes, const int32_t* frame_of, int m, int yuv422_layout,
+                                uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+int whenet_crop_boxes_ragged_yuv422_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                       const float* boxes, const int32_t* frame_of, int m, int yuv422_layout,
+                                       uint8_t* crops_out, int32_t* rects_out, int32_t* valid_out);
+
+/* YUV frames -> BGR frames on the device, bit-identical to cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420 / _YUYV / _UYVY)
+ * for `layout` WHENET_YUV_NV12, _I420, _YUYV or _UYVY: the frames whenet_draw_heads_u8 and whenet_encode_jpeg_u8 take.
+ * `frames`: n (1..64) frames of one size back to back, host memory or device memory on the context's device
+ * (frames_are_device); H and W are the image size, sides in [1, 16384] (4:2:0: both even; 4:2:2: W even), so a frame is
+ * H * W * 3/2 or H * W * 2 bytes.  `out_frames`: n x H x W x 3 bytes in caller-owned device memory.  Host frames are uploaded
+ * into the context's staging buffer.  Every argument but the context is checked before any device call.  Asynchronous on the
+ * context's stream: work queued on it later sees the frames; synchronise it (whenet_synchronize) before reading them on
+ * another stream. */
+int whenet_yuv_to_bgr_u8(whenet_ctx* ctx, const uint8_t* frames, int n, int H, int W, int frames_are_device, int layout,
+                         uint8_t* out_frames);
+/* the same on n frames of their own sizes: frames[i] is frame i (all host or all device), hw = n x (H_i, W_i) int32 on the
+ * host, out_frames[i] the caller's H_i x W_i x 3 device frame */
+int whenet_yuv_to_bgr_ragged_u8(whenet_ctx* ctx, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                int layout, uint8_t* const* out_frames);
 
 /* Block until everything queued by this context has finished. */
 int whenet_synchronize(whenet_ctx* ctx);
@@ -455,6 +488,16 @@ int whenet_det_detect_yuv_u8(whenet_det* det, const uint8_t* frames, int n, int 
 int whenet_det_detect_ragged_yuv_u8(whenet_det* det, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
                                     int yuv_layout, float score, float iou, int max_boxes,
                                     float* boxes, float* scores, int32_t* classes, int32_t* counts);
+
+/* whenet_det_detect_u8 and whenet_det_detect_ragged_u8 on packed YUV 4:2:2 frames (WHENET_YUV_YUYV / WHENET_YUV_UYVY in
+ * `yuv422_layout`, in place of swap_rb): H, W and hw are the image sizes (W even in [2, 16384], H in [1, 16384]), each frame
+ * is H * W * 2 bytes.  Otherwise as the 4:2:0 entries above: the outputs are the bits the BGR entry with swap_rb gives on
+ * cv2.cvtColor(frame, COLOR_YUV2BGR_YUYV / _UYVY), and the graph caches key on the layout. */
+int whenet_det_detect_yuv422_u8(whenet_det* det, const uint8_t* frames, int n, int H, int W, int frames_are_device, int yuv422_layout,
+                                float score, float iou, int max_boxes, float* boxes, float* scores, int32_t* classes, int32_t* counts);
+int whenet_det_detect_ragged_yuv422_u8(whenet_det* det, const uint8_t* const* frames, const int32_t* hw, int n, int frames_are_device,
+                                       int yuv422_layout, float score, float iou, int max_boxes,
+                                       float* boxes, float* scores, int32_t* classes, int32_t* counts);
 
 /* Block until everything queued by this detector has finished. */
 int whenet_det_synchronize(whenet_det* det);
